@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- the openrec.tf2 training step on B200: BPR (headline), UCML, DLRM; roofline + CPU baseline.
+"""bench.py -- the openrec.tf2 training step on H100: BPR (headline), UCML, DLRM; roofline + CPU baseline.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload bpr|ucml|dlrm] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload bpr|ucml|dlrm] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workloads (BASELINE.json configs): bpr = configs[1] (N = 1) / configs[4] shape (N > 1), ucml = configs[2],
@@ -19,6 +19,9 @@ dlrm = configs[3].  A "step" = one pass of the hot path over one batch of synthe
  cpu_baseline / --impl reference : the CPU restatement of the reference step on the box's host cores
          (oracle/: C+OpenMP port for the pairwise steps, numpy/BLAS oracle for DLRM; TensorFlow is not installable here).
 At N = 1 the default (bpr) line also carries the ucml and dlrm lines, same schema, under "secondary".
+--dump-outputs DIR (N = 1): what the timed path computed in its last timed step, as DIR/<name>.npy (float32 / float64):
+the loss and a fixed sample of the rows that step updated (with their row ids), so that two builds can be compared
+output for output.  Inputs are seeded: the same arguments give the same inputs on every run.
 Prints exactly ONE JSON line on rank 0.
 """
 from __future__ import annotations
@@ -89,7 +92,7 @@ def measured_peaks():
             d = json.load(f)
         return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, 1500.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, 989.0, "fallback (H100 SXM datasheet peaks)"
 
 
 # ---------------------------------------------------------------------------------------
@@ -324,6 +327,30 @@ def run_reference(args, rank, world):
 # ---------------------------------------------------------------------------------------
 # GPU arm
 # ---------------------------------------------------------------------------------------
+DUMP_ROWS = 4096          # rows per embedding table in --dump-outputs (1024 per DLRM table)
+DUMP_MAX_BYTES = 64 << 20
+
+
+def _sample_rows(ids, n, seed):
+    """A fixed, seeded sample of the distinct rows a batch touched (sorted)."""
+    u = np.unique(np.asarray(ids))
+    return np.sort(np.random.default_rng(seed).choice(u, size=min(n, len(u)), replace=False))
+
+
+def dump_outputs(dirname, arrays):
+    """Write {name: array} as dirname/<name>.npy in float32 / float64 (row ids as float64: exact for int32)."""
+    os.makedirs(dirname, exist_ok=True)
+    out = {}
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        out[name] = a if a.dtype in (np.float32, np.float64) else a.astype(np.float64)
+    total = sum(a.nbytes for a in out.values())
+    if total > DUMP_MAX_BYTES:
+        raise SystemExit(f"--dump-outputs: {total} bytes exceed the {DUMP_MAX_BYTES} byte budget")
+    for name, a in out.items():
+        np.save(os.path.join(dirname, name + ".npy"), a)
+
+
 def _timed(fn_step, K, barrier, torch, clocks):
     """EXACTLY K steps between two events, barrier + synchronize on both sides.  -> seconds"""
     barrier()
@@ -339,7 +366,7 @@ def _timed(fn_step, K, barrier, torch, clocks):
     return e0.elapsed_time(e1) * 1e-3
 
 
-def bench_pairwise(wl, args, eng, dev, barrier, clocks, with_extra=True):
+def bench_pairwise(wl, args, eng, dev, barrier, clocks, with_extra=True, dump=None):
     import torch
     from openrec_b200 import native as N
     kind = N.ORX_PAIR_BPR if wl == "bpr" else N.ORX_PAIR_UCML
@@ -371,6 +398,14 @@ def bench_pairwise(wl, args, eng, dev, barrier, clocks, with_extra=True):
         step(i - W)
     seconds = _timed(step, K, barrier, torch, clocks)
     loss_check = out4.cpu().numpy().tolist()
+    if dump:                                       # the last timed step: batch (K - 1) % N_BATCHES
+        u, p, n = (x.cpu().numpy() for x in dev_ids[(K - 1) % N_BATCHES])
+        ru, ri = _sample_rows(u, DUMP_ROWS, 11), _sample_rows(np.concatenate([p, n]), DUMP_ROWS, 12)
+        gu, gi = torch.from_numpy(ru).to(dev), torch.from_numpy(ri).to(dev)
+        dump_outputs(dump, {"loss_l2": out4[:2].cpu().numpy(), "user_rows": ru, "item_rows": ri,
+                            "user": tu[gu].cpu().numpy(), "user_acc": acc[0][gu].cpu().numpy(),
+                            "item": ti[gi].cpu().numpy(), "item_acc": acc[1][gi].cpu().numpy(),
+                            "bias": tb[gi].cpu().numpy(), "bias_acc": acc[2][gi].cpu().numpy()})
     # ---- roofline: the same loop, instrumented (events around the phases of every 8th step), >= 64 samples
     n_inst = 8 * 64 + 8
     eng.profile_enable(True)
@@ -451,11 +486,6 @@ def bench_pairwise(wl, args, eng, dev, barrier, clocks, with_extra=True):
     step_ms = phase_ms[1] / max(n_prof, 1)
     achieved = ALG_BYTES_PER_TRIPLET * B / (step_ms * 1e-3) / 1e9 if step_ms > 0 else 0.0
     traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "k_pair_step_traffic.json")) as f:
-            traffic = json.load(f)["dram_bytes_per_launch"]
-    except Exception:
-        pass
     kname = "k_pair_step<%s,ADAGRAD,D=128,CH=8,4 CTAs/SM>" % ("BPR" if wl == "bpr" else "UCML")
     roofline = {"bound": "hbm", "kernel": kname, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                 "traffic": traffic if wl == "bpr" else None, "peak_source": peak_src + " hbm_gbs, burst copy",
@@ -474,7 +504,7 @@ def bench_pairwise(wl, args, eng, dev, barrier, clocks, with_extra=True):
             "extra": extra}
 
 
-def bench_dlrm(args, eng, dev, barrier, clocks):
+def bench_dlrm(args, eng, dev, barrier, clocks, dump=None):
     import torch
     K, W = args.steps, max(3, args.warmup)
     sys.path.insert(0, os.path.join(ROOT, "compat"))
@@ -512,6 +542,17 @@ def bench_dlrm(args, eng, dev, barrier, clocks):
         step(i)
     seconds = _timed(step, K, barrier, torch, clocks)
     loss_value = float(state["prev"])
+    if dump:                                       # the last timed step: batch (K - 1) % 4
+        sparse = host[(K - 1) % 4][1]
+        arrays = {"loss": np.array([loss_value], dtype=np.float32)}
+        for k, lf in enumerate(model._latent_factors):
+            rows = _sample_rows(sparse[:, k], DUMP_ROWS // 4, 100 + k)
+            arrays[f"emb{k:02d}_rows"] = rows
+            arrays[f"emb{k:02d}"] = lf.embeddings.t[torch.from_numpy(rows).to(dev)].cpu().numpy()
+        emb = {id(lf.embeddings) for lf in model._latent_factors}
+        for j, v in enumerate(v for v in model.trainable_variables if id(v) not in emb):
+            arrays[f"dense{j:02d}"] = v.numpy()
+        dump_outputs(dump, arrays)
     # ---- roofline: the Dense-layer GEMMs (dominant kernels), timed with events around every GEMM call of a few steps
     prof = mlp_ops.GemmProfile()
     t0 = time.time()
@@ -528,7 +569,7 @@ def bench_dlrm(args, eng, dev, barrier, clocks):
     e2e_seconds = _timed(e2e_step, K, barrier, torch, clocks)
     state["last"] = float(state["prev"])
     _, tf_peak, peak_src = measured_peaks()
-    # 3xTF32 on kind::tf32 tensor cores: TF32 dense peak = half the bf16 peak, three MMAs per fp32-equivalent product
+    # 3xTF32 on wgmma .tf32: TF32 dense peak = half the bf16 peak, three MMAs per fp32-equivalent product
     peak = tf_peak / 2.0 / 3.0
     achieved = tc_flops / (tc_ms * 1e-3) / 1e12 if tc_ms > 0 else 0.0
     step_flops = dlrm_flops_per_sample() * DLRM_B
@@ -563,7 +604,7 @@ def make_line(wl, args, world, result, clocks_report, cpu=None):
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload_name(wl, world), "optimizer": "Adagrad (Keras sparse semantics)",
                        "l2_flush": ("none needed: tables + accumulators >= 2 GB per GPU and >= 0.4 GB of random rows touched per "
-                                    "step >> 126 MB L2; id batches rotate"),
+                                    "step >> 50 MB L2; id batches rotate"),
                        "parallelism": "single GPU" if world == 1 else f"row-sharded tables x{world}"},
             "clocks": clocks_report,
             "e2e": {"value": units / result["e2e_seconds"], "unit": unit,
@@ -608,6 +649,8 @@ def run_b200(args, rank, world, local_rank):
         clocks.wait_ready()
     wl = args.workload
     if world > 1:
+        if args.dump_outputs:
+            raise SystemExit("--dump-outputs is implemented for the single-GPU workloads (--gpus 1)")
         if wl != "bpr":
             raise SystemExit("the multi-GPU bench is the row-sharded BPR step (BASELINE configs[4])")
         from openrec_b200 import sharded
@@ -620,10 +663,10 @@ def run_b200(args, rank, world, local_rank):
             real_stdout.flush()
         dist.destroy_process_group()
         return
-    run = {"bpr": lambda: bench_pairwise("bpr", args, eng, dev, barrier, clocks),
-           "ucml": lambda: bench_pairwise("ucml", args, eng, dev, barrier, clocks, with_extra=False),
-           "dlrm": lambda: bench_dlrm(args, eng, dev, barrier, clocks)}
-    result = run[wl]()
+    run = {"bpr": lambda dump=None: bench_pairwise("bpr", args, eng, dev, barrier, clocks, dump=dump),
+           "ucml": lambda dump=None: bench_pairwise("ucml", args, eng, dev, barrier, clocks, with_extra=False, dump=dump),
+           "dlrm": lambda dump=None: bench_dlrm(args, eng, dev, barrier, clocks, dump=dump)}
+    result = run[wl](args.dump_outputs)
     clocks_main = clocks.report()
     cpu_budget = float(os.environ.get("ORX_CPU_BUDGET_S", "24"))
 
@@ -657,6 +700,8 @@ def main():
     ap.add_argument("--workload", default="bpr", choices=["bpr", "ucml", "dlrm"])
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline legs (profiling runs)")
     ap.add_argument("--no-secondary", action="store_true", help="bpr only: do not append the ucml / dlrm lines")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (loss + a fixed sample of updated rows)")
     ap.add_argument("--check", action="store_true",
                     help="--gpus N > 1: after the timed loops run ONE more step on a fresh batch and verify it on rank 0 against "
                          "the oracle over the rows the global batch touches (tests/shard_check.py); the verdict goes to extra.check")

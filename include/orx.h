@@ -1,4 +1,4 @@
-/* orx.h -- C-ABI of liborx.so: the B200 (sm_100a) implementation of the openrec.tf2
+/* orx.h -- C-ABI of liborx.so: the H100 (sm_90a) implementation of the openrec.tf2
  * embedding-lookup -> pair-score -> loss -> sparse-gradient -> optimizer training step.
  *
  * The reference (ylongqi/openrec) is pure Python on TensorFlow and has NO FFI of its own;

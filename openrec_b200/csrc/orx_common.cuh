@@ -1,4 +1,4 @@
-// orx_common.cuh -- shared host/device helpers for liborx (sm_100a only).
+// orx_common.cuh -- shared host/device helpers for liborx (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -100,6 +100,15 @@ static inline void orx_prof_next(orx_ctx* c) {
   if (!c->prof_on) return;
   if (orx_prof_sampled(c)) c->prof_n++;
   c->prof_step++;
+}
+
+// SM count of the current device (cached per device), for grid sizing where no handle is at hand
+static inline int orx_current_sms() {
+  static int sms[64] = {0};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  if (sms[dev] <= 0 && cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms[dev] = 0;
+  return sms[dev] > 0 ? sms[dev] : 132;
 }
 
 int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim, bool full_staging);

@@ -168,8 +168,8 @@ extern "C" int orx_create(int device, orx_handle_t* out) {
   ORX_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   ORX_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    orx_set_error("orx_create: liborx is built for sm_100a only; device %d is sm_%d%d", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    orx_set_error("orx_create: liborx is built for sm_90a only; device %d is sm_%d%d", device, prop.major,
                   prop.minor);
     return ORX_ERR_UNSUPPORTED;
   }

@@ -1,6 +1,6 @@
 // orx_dlrm.cu -- DLRM building blocks (rows a11-a13): strided per-feature gather (K5), second-order
-// interaction fwd/bwd (K6), Dense layers fwd/bwd (K7, fp32 SIMT tiles -- 1e-5 parity first; the tcgen05
-// 3xTF32 path replaces the inner product later), prediction loss.
+// interaction fwd/bwd (K6), Dense layers fwd/bwd (K7, fp32 SIMT tiles -- 1e-5 parity first; the wgmma
+// 3xTF32 path of orx_mlp_tc.cu takes every shape that fills a tile), prediction loss.
 //
 // Reference path: openrec/tf2/recommenders/dlrm.py:63-100, modules/multi_layer_perceptron.py:5-18,
 // modules/second_order_feature_interaction.py:12-34.
@@ -430,7 +430,7 @@ float* orx_splitk_workspace(size_t floats);                                     
 int orx_launch_splitk_reduce(const float* part, int S, int M, int N, float* C, int64_t ldc, const float* bias, int act,
                              cudaStream_t st);
 
-// ORX_MLP_SIMT=1 forces the fp32 SIMT tiles (the reference the tcgen05 path is checked against in the tests)
+// ORX_MLP_SIMT=1 forces the fp32 SIMT tiles (the reference the tensor-core path is checked against in the tests)
 static bool mlp_use_tc() {
   static int v = -1;
   if (v < 0) {
@@ -443,14 +443,15 @@ static bool mlp_use_tc() {
 template <int TA, int TB>
 static int launch_gemm(const float* A, int64_t lda, const float* Bm, int64_t ldb, float* C, int64_t ldc, int M, int N,
                        int K, const float* bias, int act, cudaStream_t st) {
-  if (mlp_use_tc()) {   // tensor cores (tcgen05, 3xTF32) whenever the shape fills a tile reasonably
+  if (mlp_use_tc()) {   // tensor cores (wgmma, 3xTF32) whenever the shape fills a tile reasonably
     const int rc = orx_launch_gemm_tc(TA, TB, A, lda, Bm, ldb, C, ldc, M, N, K, bias, act, st);
     if (rc != ORX_ERR_UNSUPPORTED) return rc;
   }
   const int tiles = ((N + 63) / 64) * ((M + 63) / 64);
   int S = 1;
-  if (tiles < 148 && K >= 1024) {   // dw of a narrow layer (13 x 512, 256 x 1): K = batch, a handful of tiles
-    S = (2 * 148 + tiles - 1) / tiles;
+  const int sms = orx_current_sms();
+  if (tiles < sms && K >= 1024) {   // dw of a narrow layer (13 x 512, 256 x 1): K = batch, a handful of tiles
+    S = (2 * sms + tiles - 1) / tiles;
     if (S > K / 256) S = K / 256;
     if (S > 65535) S = 65535;
   }
@@ -527,7 +528,7 @@ extern "C" int orx_mlp_layer_bwd(orx_handle_t h, const float* x, int64_t ldx, co
     const int cb = (out + 31) / 32;
     int S = 1;
     if (B >= 4096) {
-      S = (2 * 148 + cb - 1) / cb;
+      S = (2 * h->num_sms + cb - 1) / cb;
       if (S > B / 256) S = B / 256;
     }
     if (S > 1) {

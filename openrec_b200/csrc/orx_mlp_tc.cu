@@ -1,26 +1,25 @@
-// orx_mlp_tc.cu -- Dense-layer GEMMs on the 5th-gen tensor cores: TMA-fed tcgen05.mma kind::tf32, accumulators in TMEM.
+// orx_mlp_tc.cu -- Dense-layer GEMMs on the Hopper tensor cores: TMA-fed wgmma .tf32, accumulators in registers.
 //
 // DLRM's MLPs (openrec/tf2/modules/multi_layer_perceptron.py:5-18, recommenders/dlrm.py:34-37,87,90-95) are the one
 // dense contraction on the path.  The parity bar is 1e-5 against an fp32 reference, which plain TF32 (10-bit mantissa)
 // cannot meet, so every fp32 operand is split into two TF32 terms (hi = TF32(v) rounded to nearest, lo = v - hi)
 // and  C += Ahi*Bhi + Ahi*Blo + Alo*Bhi  is accumulated in fp32 (3xTF32, relative error ~2^-21 per product).
 //
-// One CTA computes a 128 x TN tile (TN = 256, or 128 for narrow outputs) of  C[M,N] = op(A)[M,K] * op(B)[K,N], K in
-// blocks of 16, with three kinds of warps and six rings of mbarriers between them:
-//   warp 0 (one lane)  TMA producer: cp.async.bulk.tensor.2d loads the RAW fp32 A and B blocks of a k-block straight from
-//                      the operands' own layouts (row stride = ld; out-of-range rows / k are zero-filled by the TMA) into
-//                      a 3-stage raw ring.  K-contiguous sources arrive as [rows][16] with the 64-byte swizzle,
-//                      M/N-contiguous ones ([k][rows], e.g. w in the forward pass, x and dz in dw = x^T dz) as [16][rows].
-//   warps 2..          converters: read a raw stage (conflict-free: swizzled 128-bit loads, or four coalesced scalars for
-//                      the transposing case), split into hi / lo and store both tiles in the canonical K-major,
-//                      no-swizzle UMMA layout (8-row x 16-byte core matrices, LBO 128 B, SBO 512 B) of a 3-stage operand
-//                      ring -- conflict-free 128-bit stores in both cases.
-//   warp 1 (one lane)  MMA issuer: per k-block 2 k-steps x 3 tcgen05.mma (M = 128, N = TN, K = 8), tcgen05.commit frees the
-//                      operand stage.
-// The tensor core's fp32 accumulation truncates, and over hundreds of accumulations that bias grows linearly with K
-// (measured 3e-4 abs at K = 1024), so a TMEM accumulator only ever sums 4 k-blocks (64 K-elements, 24 MMAs); the
-// converter warps then drain it with tcgen05.ld into fp32 REGISTERS (round-to-nearest adds; a warp owns 32 rows x 64
-// columns) while the MMAs of the next group fill the other TMEM accumulator.
+// One CTA (three warpgroups) computes a 128 x 128 tile of  C[M,N] = op(A)[M,K] * op(B)[K,N], K in blocks of 16, with
+// four rings of mbarriers between its two kinds of warpgroups:
+//   warpgroup 0    converters: read a raw stage (conflict-free: swizzled 128-bit loads, or four coalesced scalars for
+//                  the transposing case), split into hi / lo and store both tiles in the canonical K-major, no-swizzle
+//                  wgmma layout (8-row x 16-byte core matrices, LBO 128 B, SBO 512 B) of a 3-stage operand ring --
+//                  conflict-free 128-bit stores in both cases.  One lane of warp 0 is also the TMA producer:
+//                  cp.async.bulk.tensor.2d loads the RAW fp32 A and B blocks of a k-block straight from the operands' own
+//                  layouts (row stride = ld; out-of-range rows / k are zero-filled by the TMA) into a 4-stage raw ring,
+//                  three k-blocks ahead of the conversion.  K-contiguous sources arrive as [rows][16] with the 64-byte
+//                  swizzle, M/N-contiguous ones ([k][rows], e.g. w in the forward pass, x and dz in dw = x^T dz) as [16][rows].
+//   warpgroups 1-2 MMA: warpgroup g owns rows 64g .. 64g+63 of the tile; per k-block 2 k-steps x 3 wgmma.m64n128k8 with
+//                  both operands read from the operand ring, one k-block in flight while the next one is issued.
+// The tensor core's fp32 accumulation truncates, and over hundreds of accumulations that bias grows linearly with K, so
+// a wgmma accumulator only ever sums 4 k-blocks (64 K-elements, 24 MMAs) before it is added into a second set of fp32
+// registers (round-to-nearest adds) and restarted.
 // Epilogue through shared memory (coalesced rows, + bias, activation); split-K (blockIdx.z) for dw = x^T dz, whose K is
 // the batch.  Shapes TMA cannot describe (row stride not a multiple of 16 bytes) or that are too small for a tile are
 // left to the fp32 SIMT kernel of orx_dlrm.cu (ORX_ERR_UNSUPPORTED).
@@ -31,32 +30,55 @@
 
 namespace {
 
-constexpr int TM = 128, TK = 16;
-constexpr int RAW_STAGES = 3, OP_STAGES = 3, GROUP_KB = 4;
+constexpr int TM = 128, TN = 128, TK = 16;
+constexpr int RAW_STAGES = 4, OP_STAGES = 3, GROUP_KB = 4;
 constexpr int OP_SBO = (TK / 4) * 128;           // bytes between 8-row groups of an operand tile
+constexpr int NCW = 4;                           // converter warps (warpgroup 0)
+constexpr int THREADS = 3 * 128;
+constexpr int RAW_A = TM * TK * 4, RAW_B = TN * TK * 4, RAW_STAGE = RAW_A + RAW_B;
+constexpr int OP_A = TM * TK * 4, OP_B = TN * TK * 4, OP_STAGE = 2 * OP_A + 2 * OP_B;
+constexpr int SMEM = RAW_STAGES * RAW_STAGE + OP_STAGES * OP_STAGE;   // 64 KB + 96 KB
+static_assert(TM * (TN + 1) * 4 <= SMEM, "the epilogue tile must fit in the rings");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// K-major, SWIZZLE_NONE shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp: SmemDescriptor)
+// K-major, no-swizzle shared-memory matrix descriptor of wgmma (PTX ISA: "Matrix Descriptor Format")
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);                  // start address        bits [0,14)
   d |= (uint64_t)(128 >> 4) << 16;                          // leading byte offset  bits [16,30): K-adjacent core matrices
   d |= (uint64_t)(OP_SBO >> 4) << 32;                       // stride byte offset   bits [32,46): next 8-row group
-  d |= (uint64_t)1 << 46;                                   // descriptor version (sm_100)
-  return d;                                                 // base offset 0, layout type SWIZZLE_NONE (bits 61-63 = 0)
+  return d;                                                 // base offset 0, layout type 0 = no swizzle (bits 62-63)
 }
 
-// kind::tf32, D = F32, A/B = TF32, both K-major, M = 128, N = TN (InstrDescriptor bit layout)
-template <int TN>
-__device__ __forceinline__ void mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
+// D[64 x 128] (+)= A[64 x 8] * B[8 x 128]^T, TF32 in, FP32 accumulate, both operands K-major in shared memory.
+// Fragment of D: register j of a thread sits at row 16 * (warp % 4) + lane / 4 + 8 * ((j >> 1) & 1),
+// column 8 * (j >> 2) + 2 * (lane & 3) + (j & 1).
+#define ORX_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
+                  "+f"(d[i + 6]), "+f"(d[i + 7])
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(IDESC), "r"(accumulate)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t}\n"
+      : ORX_D8(0), ORX_D8(8), ORX_D8(16), ORX_D8(24), ORX_D8(32), ORX_D8(40), ORX_D8(48), ORX_D8(56)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
       : "memory");
 }
+#undef ORX_D8
+// the accumulator registers are written asynchronously: keep the compiler from moving their uses across the fences
+__device__ __forceinline__ void fence_operands(float (&d)[64]) {
+#pragma unroll
+  for (int j = 0; j < 64; ++j) asm volatile("" : "+f"(d[j])::"memory");
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
@@ -75,10 +97,6 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
 // one 2-D TMA load: box at (c0 = inner coordinate, c1 = outer coordinate) -> shared memory, completion on `bar`
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tm, int c0, int c1, uint64_t* bar) {
   asm volatile(
@@ -90,7 +108,7 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
 
 // hi = TF32(v) rounded to nearest (cvt.rna: truncation would bias every product the same way and the error would grow
 // linearly with K instead of with sqrt(K)); lo = v - hi exactly (|lo| <= 2^-11 |v|).  lo is handed to the tensor core as
-// it is: kind::tf32 reads the top 19 bits, i.e. truncates lo by at most 2^-10 |lo| <= 2^-21 |v| -- the size of the
+// it is: .tf32 reads the top 19 bits, i.e. truncates lo by at most 2^-10 |lo| <= 2^-21 |v| -- the size of the
 // lo*lo term 3xTF32 drops anyway, and of random sign because hi was rounded to nearest.
 __device__ __forceinline__ float to_tf32(float v) {
   uint32_t r;
@@ -144,155 +162,83 @@ __device__ __forceinline__ void convert_item(const unsigned char* raw, int src_o
   *reinterpret_cast<float4*>(lo_tile + dst_off) = l;
 }
 
-template <int TN>
-struct Cfg {
-  static constexpr int NCW = 4 * (TN / 64);              // converter / drain / epilogue warps: 32 rows x 64 columns each
-  static constexpr int THREADS = (2 + NCW) * 32;
-  static constexpr int RAW_A = TM * TK * 4, RAW_B = TN * TK * 4, RAW_STAGE = RAW_A + RAW_B;
-  static constexpr int OP_A = TM * TK * 4, OP_B = TN * TK * 4, OP_STAGE = 2 * OP_A + 2 * OP_B;
-  static constexpr int SMEM = RAW_STAGES * RAW_STAGE + OP_STAGES * OP_STAGE;   // 216 KB (TN = 256) / 144 KB (TN = 128)
-  static constexpr int TMEM_COLS = 2 * TN;
-  static_assert(TM * (TN + 1) * 4 <= SMEM, "the epilogue tile must fit in the rings");
-};
-
 // TA / TB as in orx_dlrm.cu: TA = 0: A[m*lda + k]; TA = 1: A[k*lda + m]; TB = 0: B[k*ldb + n]; TB = 1: B[n*ldb + k].
-template <int TA, int TB, int TN>
-__global__ void __launch_bounds__(Cfg<TN>::THREADS, 1)
+template <int TA, int TB>
+__global__ void __launch_bounds__(THREADS, 1)
 k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, float* __restrict__ C,
            int64_t ldc, int M, int N, int K, const float* __restrict__ bias, int act, float* __restrict__ part) {
-  using G = Cfg<TN>;
   constexpr bool A_KC = TA == 0, B_KC = TB == 1;   // K-contiguous sources
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  __shared__ __align__(8) uint64_t raw_full[RAW_STAGES], raw_empty[RAW_STAGES], op_full[OP_STAGES], op_empty[OP_STAGES],
-      acc_full[2], acc_empty[2];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ __align__(8) uint64_t raw_full[RAW_STAGES], raw_empty[RAW_STAGES], op_full[OP_STAGES], op_empty[OP_STAGES];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wgi = __shfl_sync(ORX_FULL, (int)threadIdx.x >> 7, 0);   // warpgroup index, visibly warp-uniform
   const int m0 = blockIdx.y * TM, n0 = blockIdx.x * TN;
   unsigned char* raw_ring = smem;
-  unsigned char* op_ring = smem + RAW_STAGES * G::RAW_STAGE;
+  unsigned char* op_ring = smem + RAW_STAGES * RAW_STAGE;
 
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)),
-                 "n"(G::TMEM_COLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
   if (threadIdx.x == 0) {
-    for (int s = 0; s < RAW_STAGES; ++s) { mbar_init(&raw_full[s], 1); mbar_init(&raw_empty[s], G::NCW); }
-    for (int s = 0; s < OP_STAGES; ++s) { mbar_init(&op_full[s], G::NCW); mbar_init(&op_empty[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], G::NCW); }
+    for (int s = 0; s < RAW_STAGES; ++s) { mbar_init(&raw_full[s], 1); mbar_init(&raw_empty[s], NCW); }
+    for (int s = 0; s < OP_STAGES; ++s) { mbar_init(&op_full[s], NCW); mbar_init(&op_empty[s], 8); }   // 8 MMA warps
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_d = tmem_base_s;
 
   // this CTA's range of k-blocks (split-K over blockIdx.z)
   const int nkb_all = (K + TK - 1) / TK;
   const int per = (nkb_all + (int)gridDim.z - 1) / (int)gridDim.z;
   const int kb_lo = blockIdx.z * per;
   const int nkb = max(0, min(nkb_all, kb_lo + per) - kb_lo);
-  const int ngroups = (nkb + GROUP_KB - 1) / GROUP_KB;
 
-  float acc[64];
+  float sum[64];
 #pragma unroll
-  for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+  for (int j = 0; j < 64; ++j) sum[j] = 0.f;
 
-  if (warp == 0) {
-    // ------------------------------------------------ TMA producer
-    if (lane == 0) {
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int rs = kb % RAW_STAGES;
-        if (kb >= RAW_STAGES) mbar_wait(&raw_empty[rs], ((kb / RAW_STAGES) - 1) & 1);
-        unsigned char* st = raw_ring + (size_t)rs * G::RAW_STAGE;
-        const int k0 = (kb_lo + kb) * TK;
-        mbar_expect_tx(&raw_full[rs], G::RAW_STAGE);          // a box is always delivered whole (out of range = zeros)
-        if (A_KC) tma_load_2d(st, &tmA, k0, m0, &raw_full[rs]); else tma_load_2d(st, &tmA, m0, k0, &raw_full[rs]);
-        if (B_KC) tma_load_2d(st + G::RAW_A, &tmB, k0, n0, &raw_full[rs]); else tma_load_2d(st + G::RAW_A, &tmB, n0, k0, &raw_full[rs]);
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      const uint64_t desc0 = make_desc(smem_u32(op_ring));
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int os = kb % OP_STAGES, g = kb / GROUP_KB;
-        const bool g_first = (kb % GROUP_KB) == 0, g_last = (kb % GROUP_KB) == GROUP_KB - 1 || kb == nkb - 1;
-        if (g_first && g >= 2) mbar_wait(&acc_empty[g & 1], ((g >> 1) - 1) & 1);   // group g-2 has been drained from this buffer
-        mbar_wait(&op_full[os], (kb / OP_STAGES) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        // descriptors: the address field is the low 14 bits (16-byte units), everything else is constant
-        const uint64_t a_hi = desc0 + (uint64_t)(os * (G::OP_STAGE >> 4)), a_lo = a_hi + (G::OP_A >> 4),
-                       b_hi = a_lo + (G::OP_A >> 4), b_lo = b_hi + (G::OP_B >> 4);
-        const uint32_t d = tmem_d + (uint32_t)((g & 1) * TN);
-#pragma unroll
-        for (int ks = 0; ks < TK / 8; ++ks) {
-          const uint64_t o = (uint64_t)(ks * (256 >> 4));     // two k-cores of 128 bytes
-          mma_tf32<TN>(d, a_hi + o, b_hi + o, (g_first && ks == 0) ? 0u : 1u);
-          mma_tf32<TN>(d, a_hi + o, b_lo + o, 1u);
-          mma_tf32<TN>(d, a_lo + o, b_hi + o, 1u);
-        }
-        umma_commit(&op_empty[os]);
-        if (g_last) umma_commit(&acc_full[g & 1]);
-      }
-    }
-  } else {
-    // ------------------------------------------------ converters + accumulator drain
-    const int cw = warp - 2;
-    const uint32_t lane_base = (uint32_t)((warp & 3) * 32);   // the TMEM lanes a warp may touch: 32 * (warp % 4)
-    const int cchunk = (cw >> 2) * 64;                         // its 64 accumulator columns
-    auto drain = [&](int g) {
-      const int buf = g & 1;
-      mbar_wait(&acc_full[buf], (g >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll
-      for (int c0 = 0; c0 < 64; c0 += 32) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem_d + (lane_base << 16) + (uint32_t)(buf * TN + cchunk + c0);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-            : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-              "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-              "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-              "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[c0 + j] += __uint_as_float(v[j]);
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
+  if (wgi == 0) {
+    // ------------------------------------------------ TMA producer (one lane) + converters
+    auto load = [&](int kb) {
+      const int rs = kb % RAW_STAGES;
+      unsigned char* st = raw_ring + (size_t)rs * RAW_STAGE;
+      const int k0 = (kb_lo + kb) * TK;
+      mbar_expect_tx(&raw_full[rs], RAW_STAGE);               // a box is always delivered whole (out of range = zeros)
+      if (A_KC) tma_load_2d(st, &tmA, k0, m0, &raw_full[rs]); else tma_load_2d(st, &tmA, m0, k0, &raw_full[rs]);
+      if (B_KC) tma_load_2d(st + RAW_A, &tmB, k0, n0, &raw_full[rs]); else tma_load_2d(st + RAW_A, &tmB, n0, k0, &raw_full[rs]);
     };
+    const bool producer = warp == 0 && lane == 0;
+    if (producer)
+      for (int kb = 0; kb < min(nkb, RAW_STAGES - 1); ++kb) load(kb);
     constexpr int ITEMS_A = TM / 8, ITEMS_B = TN / 8;          // warp-items per tile (32 (row, k-core) pairs each)
-    constexpr int NIT = (ITEMS_A + ITEMS_B) / G::NCW;          // items per warp and k-block (3 or 4); item i of warp cw is
-    static_assert((ITEMS_A + ITEMS_B) % G::NCW == 0 && ITEMS_A % G::NCW == 0, "items must divide evenly");   // cw + NCW*i
-    constexpr int NIT_A = ITEMS_A / G::NCW;                    // the first NIT_A items of a warp belong to A, the rest to B
+    constexpr int NIT = (ITEMS_A + ITEMS_B) / NCW;             // items per warp and k-block; item i of warp w is w + NCW*i
+    static_assert((ITEMS_A + ITEMS_B) % NCW == 0 && ITEMS_A % NCW == 0, "items must divide evenly");
+    constexpr int NIT_A = ITEMS_A / NCW;                       // the first NIT_A items of a warp belong to A, the rest to B
     int src_off[NIT], dst_off[NIT];
 #pragma unroll
     for (int i = 0; i < NIT; ++i) {
-      const int wi = cw + G::NCW * i;
+      const int wi = warp + NCW * i;
       if (i < NIT_A) item_offsets<A_KC>(TM, wi, lane, &src_off[i], &dst_off[i]);
       else item_offsets<B_KC>(TN, wi - ITEMS_A, lane, &src_off[i], &dst_off[i]);
     }
-    int drained = 0;
     for (int kb = 0; kb < nkb; ++kb) {
-      const int rs = kb % RAW_STAGES, os = kb % OP_STAGES, g = kb / GROUP_KB;
+      const int rs = kb % RAW_STAGES, os = kb % OP_STAGES;
+      // refill the raw stage block kb-1 used (every converter warp has left it, or is about to)
+      const int nk = kb + RAW_STAGES - 1;
+      if (producer && nk < nkb) {
+        if (nk >= RAW_STAGES) mbar_wait(&raw_empty[nk % RAW_STAGES], ((nk / RAW_STAGES) - 1) & 1);
+        load(nk);
+      }
+      __syncwarp();
       mbar_wait(&raw_full[rs], (kb / RAW_STAGES) & 1);
       if (kb >= OP_STAGES) mbar_wait(&op_empty[os], ((kb / OP_STAGES) - 1) & 1);   // the MMAs of block kb-3 left this stage
-      const unsigned char* ra = raw_ring + (size_t)rs * G::RAW_STAGE;
-      const unsigned char* rb = ra + G::RAW_A;
-      unsigned char* oa = op_ring + (size_t)os * G::OP_STAGE;
-      unsigned char* ob = oa + 2 * G::OP_A;
+      const unsigned char* ra = raw_ring + (size_t)rs * RAW_STAGE;
+      const unsigned char* rb = ra + RAW_A;
+      unsigned char* oa = op_ring + (size_t)os * OP_STAGE;
+      unsigned char* ob = oa + 2 * OP_A;
 #pragma unroll
       for (int i = 0; i < NIT; ++i) {
-        if (i < NIT_A) convert_item<A_KC, TM>(ra, src_off[i], dst_off[i], oa, oa + G::OP_A);
-        else convert_item<B_KC, TN>(rb, src_off[i], dst_off[i], ob, ob + G::OP_B);
+        if (i < NIT_A) convert_item<A_KC, TM>(ra, src_off[i], dst_off[i], oa, oa + OP_A);
+        else convert_item<B_KC, TN>(rb, src_off[i], dst_off[i], ob, ob + OP_B);
       }
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to the tensor core
       __syncwarp();
@@ -300,28 +246,59 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
         mbar_arrive(&op_full[os]);
         mbar_arrive(&raw_empty[rs]);
       }
-      // drain group g-1 one k-block AFTER group g has started: by then its last MMAs have retired, so the converters do
-      // not sit in the accumulator wait while the tensor core runs out of converted operands
-      if ((kb % GROUP_KB) == 1 && g >= 1) { drain(g - 1); drained = g; }
     }
-    for (int d = drained; d < ngroups; ++d) drain(d);
+  } else {
+    // ------------------------------------------------ MMA warpgroups
+    const int wg = wgi - 1;                                    // rows 64*wg .. 64*wg+63 of the tile
+    float acc[64];
+#pragma unroll
+    for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+    const uint32_t op0 = smem_u32(op_ring);
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&op_empty[s]);
+    };
+    for (int g0 = 0; g0 < nkb; g0 += GROUP_KB) {             // one accumulation group: up to GROUP_KB k-blocks
+      const int g1 = min(nkb, g0 + GROUP_KB);
+      for (int kb = g0; kb < g1; ++kb) {
+        const int os = kb % OP_STAGES;
+        mbar_wait(&op_full[os], (kb / OP_STAGES) & 1);
+        const uint32_t a_hi = op0 + (uint32_t)(os * OP_STAGE + wg * 8 * OP_SBO), a_lo = a_hi + OP_A;
+        const uint32_t b_hi = op0 + (uint32_t)(os * OP_STAGE + 2 * OP_A), b_lo = b_hi + OP_B;
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < TK / 8; ++ks) {
+          const uint32_t o = (uint32_t)(ks * 256);             // two k-cores of 128 bytes
+          wgmma_tf32(acc, make_desc(a_hi + o), make_desc(b_hi + o), (kb == g0 && ks == 0) ? 0u : 1u);
+          wgmma_tf32(acc, make_desc(a_hi + o), make_desc(b_lo + o), 1u);
+          wgmma_tf32(acc, make_desc(a_lo + o), make_desc(b_hi + o), 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                                       // block kb-1 has retired: its stage is free
+        if (kb > g0) release((kb - 1) % OP_STAGES);
+      }
+      wgmma_wait<0>();
+      fence_operands(acc);
+      release((g1 - 1) % OP_STAGES);
+#pragma unroll
+      for (int j = 0; j < 64; ++j) sum[j] += acc[j];
+    }
   }
 
-  // ---- epilogue through shared memory: every MMA has completed (the last drain waited for the last group, and groups
-  // complete in order) and every TMA load has been consumed, so the rings are free: tile[128][TN + 1] floats
+  // ---- epilogue through shared memory: every MMA has completed (the last k-block waited for all of them) and every
+  // TMA load has been consumed, so the rings are free: tile[128][TN + 1] floats
   __syncthreads();
   float* tile = reinterpret_cast<float*>(smem);
-  if (warp >= 2) {
-    const int cw = warp - 2;
-    const int r = (warp & 3) * 32 + lane, c0 = (cw >> 2) * 64;
+  if (warp >= NCW) {
+    const int r0 = 16 * (warp - NCW) + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-    for (int j = 0; j < 64; ++j) tile[r * (TN + 1) + c0 + j] = acc[j];
+    for (int j = 0; j < 64; ++j) tile[(r0 + 8 * ((j >> 1) & 1)) * (TN + 1) + 8 * (j >> 2) + c0 + (j & 1)] = sum[j];
   }
   __syncthreads();
   const bool split = gridDim.z > 1;
   float* out = split ? part + (size_t)blockIdx.z * (size_t)M * (size_t)N : C;
   const int64_t ldo = split ? (int64_t)N : ldc;
-  for (int r = warp; r < TM; r += G::THREADS / 32) {
+  for (int r = warp; r < TM; r += THREADS / 32) {
     const int m = m0 + r;
     if (m >= M) break;
 #pragma unroll
@@ -338,9 +315,6 @@ k_gemm_tma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUte
       }
     }
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_d), "n"(G::TMEM_COLS) : "memory");
 }
 
 // sum of split-K partials (deterministic: fixed order), + bias, activation
@@ -388,17 +362,16 @@ int make_map(CUtensorMap* tm, const float* base, int rows, int K, int64_t ld, bo
   return ORX_OK;
 }
 
-template <int TA, int TB, int TN>
+template <int TA, int TB>
 int launch_tma(const CUtensorMap& ta, const CUtensorMap& tb, float* C, int64_t ldc, int M, int N, int K, const float* bias,
                int act, float* part, int S, cudaStream_t st) {
-  using G = Cfg<TN>;
   static bool done = false;
   if (!done) {
-    ORX_CUDA(cudaFuncSetAttribute(k_gemm_tma<TA, TB, TN>, cudaFuncAttributeMaxDynamicSharedMemorySize, G::SMEM + 1024));
+    ORX_CUDA(cudaFuncSetAttribute(k_gemm_tma<TA, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM + 1024));
     done = true;
   }
   dim3 grid((N + TN - 1) / TN, (M + TM - 1) / TM, S);
-  k_gemm_tma<TA, TB, TN><<<grid, G::THREADS, G::SMEM + 1024, st>>>(ta, tb, C, ldc, M, N, K, bias, act, part);
+  k_gemm_tma<TA, TB><<<grid, THREADS, SMEM + 1024, st>>>(ta, tb, C, ldc, M, N, K, bias, act, part);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
@@ -429,19 +402,19 @@ int orx_launch_splitk_reduce(const float* part, int S, int M, int N, float* C, i
   return ORX_OK;
 }
 
-// C[M,N] = op(A) * op(B) (+bias, act) on tcgen05; same operand conventions as launch_gemm in orx_dlrm.cu.
+// C[M,N] = op(A) * op(B) (+bias, act) on wgmma; same operand conventions as launch_gemm in orx_dlrm.cu.
 // Returns ORX_ERR_UNSUPPORTED for shapes that are left to the SIMT kernel: tiny N / K / M, or operands the TMA cannot
 // describe (base not 16-byte aligned, row stride not a multiple of 16 bytes).
 int orx_launch_gemm_tc(int TA, int TB, const float* A, int64_t lda, const float* Bm, int64_t ldb, float* C, int64_t ldc,
                        int M, int N, int K, const float* bias, int act, cudaStream_t st) {
   if (N < 16 || K < 8 || M < 64) return ORX_ERR_UNSUPPORTED;
   if ((lda & 3) || (ldb & 3) || (((uintptr_t)A | (uintptr_t)Bm) & 15)) return ORX_ERR_UNSUPPORTED;
-  const int TN = N > 128 ? 256 : 128;
   const int tiles = ((N + TN - 1) / TN) * ((M + TM - 1) / TM);
   const int nkb = (K + TK - 1) / TK;
   int S = 1;
-  if (tiles < 148 && nkb >= 32) {             // too few tiles for the machine and a long K: split it
-    S = (2 * 148 + tiles - 1) / tiles;
+  const int sms = orx_current_sms();
+  if (tiles < sms && nkb >= 32) {             // too few tiles for the machine and a long K: split it
+    S = (2 * sms + tiles - 1) / tiles;
     if (S > nkb / 8) S = nkb / 8;             // at least 8 k-blocks (two accumulation groups) per split
     if (S < 1) S = 1;
   }
@@ -454,9 +427,7 @@ int orx_launch_gemm_tc(int TA, int TB, const float* A, int64_t lda, const float*
   int rc;
   if ((rc = make_map(&ta, A, M, K, lda, TA == 0, TM))) return rc;
   if ((rc = make_map(&tb, Bm, N, K, ldb, TB == 1, TN))) return rc;
-#define ORX_TMA(a, b)                                                                                     \
-  rc = TN == 256 ? launch_tma<a, b, 256>(ta, tb, C, ldc, M, N, K, bias, act, part, S, st)                 \
-                 : launch_tma<a, b, 128>(ta, tb, C, ldc, M, N, K, bias, act, part, S, st)
+#define ORX_TMA(a, b) rc = launch_tma<a, b>(ta, tb, C, ldc, M, N, K, bias, act, part, S, st)
   if (TA == 0 && TB == 0) ORX_TMA(0, 0);
   else if (TA == 0 && TB == 1) ORX_TMA(0, 1);
   else if (TA == 1 && TB == 0) ORX_TMA(1, 0);

@@ -286,7 +286,7 @@ class Engine:
 def engine(device=None) -> Engine:
     """The per-device engine; raises (no CPU fallback) when CUDA is unavailable."""
     if not torch.cuda.is_available():
-        raise RuntimeError("openrec_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+        raise RuntimeError("openrec_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
     idx = torch.cuda.current_device() if device is None else torch.device(device).index or 0
     e = _engines.get(idx)
     if e is None:

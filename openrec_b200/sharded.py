@@ -528,12 +528,12 @@ def bench(args, rank, world, eng, barrier, clocks=None):
     # NVLink-bound exchange (SURVEY 8e): bytes per GPU per direction per step: rows out as owner + gradient rows out as home
     rows_each_way = 2 if mode == "home" else 3
     link_bytes = 2.0 * (world - 1) / world * rows_each_way * (D + 1) * 4 * Bsz
-    nvlink_peak = 770.0
+    nvlink_peak = 450.0
     ms = seconds / K * 1e3
     roofline = {"bound": "nvlink", "kernel": "k_sh_serve + k_sh_compute (peer stores)" if mode == "home" else "NCCL all-to-all",
                 "achieved": link_bytes / (seconds / K) / 1e9, "peak": nvlink_peak, "unit": "GB/s",
                 "frac": link_bytes / (seconds / K) / 1e9 / nvlink_peak, "traffic": None,
-                "peak_source": "B200_PROFILING.md measured peer copy 770 GB/s per direction per GPU",
+                "peak_source": "H100 SXM datasheet: NVLink 4, 450 GB/s per direction per GPU",
                 "algorithmic_bytes_per_launch": link_bytes,
                 "note": f"per-GPU per-direction NVLink bytes of the item-row + gradient-row exchange ({rows_each_way} rows each way "
                         f"per triplet, (N-1)/N of them remote) over the WHOLE step time ({ms:.3f} ms): the step also does the local "

@@ -7,7 +7,7 @@ import torch
 
 from .. import native as N
 
-GEMM_KERNEL_NAME = "k_gemm_tma (TMA-fed tcgen05 kind::tf32, 3xTF32, 128x256 tile, TMEM accumulators)"
+GEMM_KERNEL_NAME = "k_gemm_tma (TMA-fed wgmma .tf32, 3xTF32, 128x128 tile, register accumulators)"
 
 
 def _rows(B, n, device):
@@ -37,7 +37,7 @@ class GemmProfile:
         return e0, e1
 
     def totals(self, pure_only=False):
-        """(ms, flops, calls) over all bracketed Dense-layer calls, or only over the calls that are ONE tcgen05 GEMM
+        """(ms, flops, calls) over all bracketed Dense-layer calls, or only over the calls that are ONE wgmma GEMM
         launch (forward layers on the tensor-core path: bias + activation are fused into the GEMM's epilogue)."""
         torch.cuda.synchronize()
         ev = [e for e in self.ev if e[3]] if pure_only else self.ev

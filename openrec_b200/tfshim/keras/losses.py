@@ -1,4 +1,4 @@
-"""tf.keras.losses used by the reference's model files (dlrm.py:52-55, gmf.py:20).  The B200
+"""tf.keras.losses used by the reference's model files (dlrm.py:52-55, gmf.py:20).  The liborx
 recommenders compute their losses inside liborx; these callables exist for user-side evaluation
 glue on already-materialised tensors."""
 from __future__ import annotations

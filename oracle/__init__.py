@@ -6,7 +6,7 @@ legs may import it, and only as the checker (or as the timed CPU arm).
 
 PARITY UNPINNED (TensorFlow part): the arithmetic of the reference path lives in
 TensorFlow/Keras (only pin: ``docs_requirements.txt:2`` ``tensorflow==2.0.1``), which
-is neither vendored in /root/reference nor installable here, and the reference has
+is neither vendored in the reference nor installable here, and the reference has
 no tests / golden vectors.  What *is* pinned: the reference's own Python composition
 (``openrec/tf2/{modules,recommenders,metrics}``) executed verbatim under a torch-backed
 ``tensorflow`` stand-in (``tests/golden/make_golden.py``) -> fixtures in

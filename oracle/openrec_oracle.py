@@ -1,7 +1,7 @@
 """NumPy restatement of the openrec.tf2 hot path -- TEST INFRASTRUCTURE, NOT PRODUCT.
 
 Every function cites the reference file:line it follows (paths relative to
-/root/reference).  TensorFlow-internal semantics that cannot be read here
+the reference checkout).  TensorFlow-internal semantics that cannot be read here
 (gradient of ``maximum``, IndexedSlices aggregation, optimizer formulas, Keras
 loss epsilons) are marked [TF-mem] -- see oracle/__init__.py "PARITY UNPINNED".
 

@@ -1,11 +1,11 @@
 """Generate tests/golden/*.npz by running the REFERENCE's own Python code.
 
-Run in the build container only (needs /root/reference, which does not exist on the GPU box):
+Needs a checkout of the reference (ylongqi/openrec); the fixtures it writes are committed, so the tests do not:
 
-    python tests/golden/make_golden.py
+    OPENREC_REFERENCE=/path/to/openrec python tests/golden/make_golden.py
 
 The reference's openrec/tf2/{modules,recommenders,metrics,data} files are imported verbatim
-from /root/reference; ``tensorflow`` is replaced by the torch stand-in of tf_standin.py
+from that checkout; ``tensorflow`` is replaced by the torch stand-in of tf_standin.py
 (TensorFlow itself is not installable here -- "parity unpinned" for TF internals, see
 oracle/__init__.py).  Forward values and autograd gradients are recorded in float64; the
 fixtures are the pin for oracle/openrec_oracle.py and, through it, for the CUDA kernels.
@@ -23,12 +23,14 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import tf_standin  # noqa: E402
 
-REF = "/root/reference"
+REF = os.environ.get("OPENREC_REFERENCE", "")
 
 
 def _fresh_reference():
     for k in [k for k in sys.modules if k == "openrec" or k.startswith("openrec.")]:
         del sys.modules[k]
+    if not os.path.isdir(os.path.join(REF, "openrec")):
+        raise SystemExit("set OPENREC_REFERENCE to a checkout of ylongqi/openrec")
     tf = tf_standin.install()
     if REF not in sys.path:
         sys.path.insert(0, REF)

@@ -1,5 +1,5 @@
 """A torch(CPU, float64-capable) stand-in for the handful of ``tensorflow`` symbols that
-/root/reference/openrec/tf2/{modules,recommenders,metrics,data} touch.
+the reference's openrec/tf2/{modules,recommenders,metrics,data} touch.
 
 TEST INFRASTRUCTURE used ONLY by tests/golden/make_golden.py to execute the reference's own
 Python composition verbatim and record golden vectors.  It is not the product's tensorflow

@@ -72,10 +72,10 @@ def test_ctypes_argument_lists_match_header(built):
             assert kind_c(decl) == kind_py(t), f"{name} argument {k}: '{decl}' vs {t}"
 
 
-def test_sm100a_only(built):
+def test_sm90a_only(built):
     out = subprocess.run(["cuobjdump", "--list-elf", built], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_no_cpu_fallback(built):

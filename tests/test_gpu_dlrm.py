@@ -167,7 +167,7 @@ def test_dlrm_training_step(tf, optname, mode):
 
 def test_dlrm_full_shape_training_step(tf):
     """BASELINE.json configs[3]: the Criteo shape (26 tables x 1M x 128, B = 32768, MLPs 13-512-256-128 and
-    479-1024-1024-512-256-1, Adagrad): one training step through the class surface (TMA-fed tcgen05 Dense layers, warp
+    479-1024-1024-512-256-1, Adagrad): one training step through the class surface (TMA-fed wgmma Dense layers, warp
     interaction kernels, strided gathers / sparse applies) against the float64 oracle on the touched rows."""
     from openrec.tf2.recommenders import DLRM
     rng = np.random.default_rng(33)
