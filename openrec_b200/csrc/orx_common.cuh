@@ -194,16 +194,46 @@ __device__ __forceinline__ uint32_t orx_hash_insert(const OrxHash& t, int32_t id
   }
 }
 
+// Loads at L2 evict-last priority, for the small random-access structures a step re-reads long after they were last
+// touched (batch index, item bias + its slots) while it streams row traffic many times the L2 through the cache.  The
+// policy is a per-access hint (createpolicy + .L2::cache_hint, carried in the uniform memory descriptor: no per-thread
+// register); it configures no L2 set-aside, and the lines stay evictable.
+__device__ __forceinline__ unsigned long long orx_ld_keep(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("{.reg .b64 pol; createpolicy.fractional.L2::evict_last.b64 pol, 1.0;\n"
+               " ld.global.nc.L2::cache_hint.u64 %0, [%1], pol;}" : "=l"(v) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ int32_t orx_ld_keep(const int32_t* p) {
+  int32_t v;
+  asm volatile("{.reg .b64 pol; createpolicy.fractional.L2::evict_last.b64 pol, 1.0;\n"
+               " ld.global.nc.L2::cache_hint.b32 %0, [%1], pol;}" : "=r"(v) : "l"(p));
+  return v;
+}
+// not .nc: the step that reads an item bias also writes it
+__device__ __forceinline__ float orx_ld_keep(const float* p) {
+  float v;
+  asm volatile("{.reg .b64 pol; createpolicy.fractional.L2::evict_last.b64 pol, 1.0;\n"
+               " ld.global.cg.L2::cache_hint.f32 %0, [%1], pol;}" : "=f"(v) : "l"(p));
+  return v;
+}
+
 // Lookup.  Returns 0 = absent, 1 = present once, 2 = present more than once; *d = staging index if the row
 // has one (duplicates in mode 0, every row in mode 1).
+// DUP_ONLY (mode-0 indexes): the staging index is read only for a row present more than once, the only rows that have
+// one, and *d = -1 otherwise; this saves a dependent random load per probe of a row seen once.  Callers that read *d of
+// rows present once (mode 1: ADAM_DENSE stages every row) keep the default.
+// KEEP: probe at L2 evict-last priority (orx_ld_keep), for kernels that stream table rows beside the probes.
+template <bool DUP_ONLY = false, bool KEEP = false>
 __device__ __forceinline__ uint32_t orx_hash_find(const OrxHash& t, int32_t id, int32_t* d) {
   const unsigned long long mine = orx_slot_word(t.epoch, id);
   uint32_t h = orx_hash32((uint32_t)id, t.shift);
   while (true) {
-    const unsigned long long w = __ldg(t.slots + h);
+    const unsigned long long w = KEEP ? orx_ld_keep(t.slots + h) : __ldg(t.slots + h);
     if ((w & ~ORX_DUP_BIT) == mine) {
-      *d = __ldg(t.didx + h);
-      return (w & ORX_DUP_BIT) ? 2u : 1u;
+      const bool dup = (w & ORX_DUP_BIT) != 0;
+      *d = (!DUP_ONLY || dup) ? (KEEP ? orx_ld_keep(t.didx + h) : __ldg(t.didx + h)) : -1;
+      return dup ? 2u : 1u;
     }
     if ((uint32_t)(w >> 33) != t.epoch) {
       *d = -1;
@@ -222,6 +252,13 @@ __device__ __forceinline__ float orx_group_sum(float v) {
 
 __device__ __forceinline__ float4 orx_ld4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ void orx_st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+// Table rows of the sparse steps (embedding rows and their optimizer-slot rows) at L2 evict-first priority
+// (ld/st.global.cs -> LDG/STG.E.EF.128: no policy register).  A BPR step at the default bench size streams ~370 MB of
+// random 512-byte rows through the 50 MB L2 of an H100, each read once and written once, so a row line is never hit
+// again before it leaves.  Marking them evict-first leaves the L2 to what IS reused over the step: the batch index sets,
+// item bias + its slots, and the compact staging rows (those stay at normal priority).
+__device__ __forceinline__ float4 orx_ld4_stream(const float* p) { return __ldcs(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ void orx_st4_stream(float* p, float4 v) { __stcs(reinterpret_cast<float4*>(p), v); }
 // one 128-bit fire-and-forget reduction (REDG.E.ADD.F32x4 on sm_90+)
 __device__ __forceinline__ void orx_red4(float* p, float4 v) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)

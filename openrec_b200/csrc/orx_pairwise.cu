@@ -90,6 +90,9 @@ struct TripRegs {
 //   ids (coalesced, lanes < CH) -> variable rows of the first one/two triplet groups (they need only
 //   the ids) -> hash probes + bias loads (lanes < CH, overlap the row loads) -> slot rows of the first
 //   groups -> steady state: process one register buffer while the other's 128-bit loads are in flight.
+// L2 priority: table and slot rows are loaded and stored evict-first (orx_ld4_stream / orx_st4_stream); the probes and
+// the item bias + slot loads are evict-last (orx_ld_keep), the staging red.adds and the bias stores normal, so that the
+// index, the bias and the staging rows are still in L2 when they are reused.
 template <int KIND, int OPT, int D, int CH, int MINB, bool PIPE>
 __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
   constexpr int G = (D / 4 < 32) ? D / 4 : 32;  // lanes per triplet
@@ -127,32 +130,32 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
 #pragma unroll
     for (int k = 0; k < K; ++k) {
       const int off = (k * G + gl) * 4;
-      r.u[k] = r.fl ? __ldcg(reinterpret_cast<const float4*>(a.U + (int64_t)r.uu * D + off)) : z4;
-      r.p[k] = r.fl ? __ldcg(reinterpret_cast<const float4*>(a.I + (int64_t)r.pp * D + off)) : z4;
-      r.n[k] = r.fl ? __ldcg(reinterpret_cast<const float4*>(a.I + (int64_t)r.nn * D + off)) : z4;
+      r.u[k] = r.fl ? orx_ld4_stream(a.U + (int64_t)r.uu * D + off) : z4;
+      r.p[k] = r.fl ? orx_ld4_stream(a.I + (int64_t)r.pp * D + off) : z4;
+      r.n[k] = r.fl ? orx_ld4_stream(a.I + (int64_t)r.nn * D + off) : z4;
     }
   };
   Regs ra, rb;
   load_var(0, ra);
   if (PIPE && TPW < CH) load_var(TPW, rb);
 
-  // ---- hash probes + item_bias (lanes < CH), overlapping the row loads above
+  // ---- hash probes + item_bias (lanes < CH), overlapping the row loads above; L2 evict-last (orx_ld_keep)
   float bp = 0.f, bn = 0.f, bps0 = 0.f, bps1 = 0.f, bns0 = 0.f, bns1 = 0.f;
   if (flags & 1) {
-    const uint32_t cu = orx_hash_find(a.hu, u_id, &du);
-    const uint32_t cp = orx_hash_find(a.hi, p_id, &dp);
-    const uint32_t cn = orx_hash_find(a.hi, n_id, &dn);
-    bp = __ldcg(a.Bv + p_id);
-    bn = __ldcg(a.Bv + n_id);
+    const uint32_t cu = orx_hash_find<!STAGE_ONLY, true>(a.hu, u_id, &du);
+    const uint32_t cp = orx_hash_find<!STAGE_ONLY, true>(a.hi, p_id, &dp);
+    const uint32_t cn = orx_hash_find<!STAGE_ONLY, true>(a.hi, n_id, &dn);
+    bp = orx_ld_keep(a.Bv + p_id);
+    bn = orx_ld_keep(a.Bv + n_id);
     if (!STAGE_ONLY) {
       flags |= (cu == 1u ? 2 : 0) | (cp == 1u ? 4 : 0) | (cn == 1u ? 8 : 0);
       if (S0) {
-        if (flags & 4) bps0 = __ldcg(a.Bs0 + p_id);
-        if (flags & 8) bns0 = __ldcg(a.Bs0 + n_id);
+        if (flags & 4) bps0 = orx_ld_keep(a.Bs0 + p_id);
+        if (flags & 8) bns0 = orx_ld_keep(a.Bs0 + n_id);
       }
       if (S1) {
-        if (flags & 4) bps1 = __ldcg(a.Bs1 + p_id);
-        if (flags & 8) bns1 = __ldcg(a.Bs1 + n_id);
+        if (flags & 4) bps1 = orx_ld_keep(a.Bs1 + p_id);
+        if (flags & 8) bns1 = orx_ld_keep(a.Bs1 + n_id);
       }
     }
   }
@@ -170,14 +173,14 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
     for (int k = 0; k < K; ++k) {
       const int off = (k * G + gl) * 4;
       if (S0) {
-        r.us0[k] = (r.fl & 2) ? __ldcg(reinterpret_cast<const float4*>(a.Us0 + (int64_t)r.uu * D + off)) : z4;
-        r.ps0[k] = (r.fl & 4) ? __ldcg(reinterpret_cast<const float4*>(a.Is0 + (int64_t)r.pp * D + off)) : z4;
-        r.ns0[k] = (r.fl & 8) ? __ldcg(reinterpret_cast<const float4*>(a.Is0 + (int64_t)r.nn * D + off)) : z4;
+        r.us0[k] = (r.fl & 2) ? orx_ld4_stream(a.Us0 + (int64_t)r.uu * D + off) : z4;
+        r.ps0[k] = (r.fl & 4) ? orx_ld4_stream(a.Is0 + (int64_t)r.pp * D + off) : z4;
+        r.ns0[k] = (r.fl & 8) ? orx_ld4_stream(a.Is0 + (int64_t)r.nn * D + off) : z4;
       }
       if (S1) {
-        r.us1[k] = (r.fl & 2) ? __ldcg(reinterpret_cast<const float4*>(a.Us1 + (int64_t)r.uu * D + off)) : z4;
-        r.ps1[k] = (r.fl & 4) ? __ldcg(reinterpret_cast<const float4*>(a.Is1 + (int64_t)r.pp * D + off)) : z4;
-        r.ns1[k] = (r.fl & 8) ? __ldcg(reinterpret_cast<const float4*>(a.Is1 + (int64_t)r.nn * D + off)) : z4;
+        r.us1[k] = (r.fl & 2) ? orx_ld4_stream(a.Us1 + (int64_t)r.uu * D + off) : z4;
+        r.ps1[k] = (r.fl & 4) ? orx_ld4_stream(a.Is1 + (int64_t)r.pp * D + off) : z4;
+        r.ns1[k] = (r.fl & 8) ? orx_ld4_stream(a.Is1 + (int64_t)r.nn * D + off) : z4;
       }
     }
   };
@@ -222,25 +225,25 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
         pair_row_grads<KIND>(g, a.c_l2, r.u[k], r.p[k], r.n[k], &gu, &gp, &gn);
         if (!STAGE_ONLY && (r.fl & 2)) {
           const int64_t o = (int64_t)r.uu * D + off;
-          __stcg(reinterpret_cast<float4*>(a.U + o), orx_apply4<OPT>(r.u[k], gu, r.us0[k], r.us1[k], a.opt));
-          if (S0) __stcg(reinterpret_cast<float4*>(a.Us0 + o), r.us0[k]);
-          if (S1) __stcg(reinterpret_cast<float4*>(a.Us1 + o), r.us1[k]);
+          orx_st4_stream(a.U + o, orx_apply4<OPT>(r.u[k], gu, r.us0[k], r.us1[k], a.opt));
+          if (S0) orx_st4_stream(a.Us0 + o, r.us0[k]);
+          if (S1) orx_st4_stream(a.Us1 + o, r.us1[k]);
         } else {
           orx_red4(a.gu + (int64_t)r.du * D + off, gu);
         }
         if (!STAGE_ONLY && (r.fl & 4)) {
           const int64_t o = (int64_t)r.pp * D + off;
-          __stcg(reinterpret_cast<float4*>(a.I + o), orx_apply4<OPT>(r.p[k], gp, r.ps0[k], r.ps1[k], a.opt));
-          if (S0) __stcg(reinterpret_cast<float4*>(a.Is0 + o), r.ps0[k]);
-          if (S1) __stcg(reinterpret_cast<float4*>(a.Is1 + o), r.ps1[k]);
+          orx_st4_stream(a.I + o, orx_apply4<OPT>(r.p[k], gp, r.ps0[k], r.ps1[k], a.opt));
+          if (S0) orx_st4_stream(a.Is0 + o, r.ps0[k]);
+          if (S1) orx_st4_stream(a.Is1 + o, r.ps1[k]);
         } else {
           orx_red4(a.gi + (int64_t)r.dp * D + off, gp);
         }
         if (!STAGE_ONLY && (r.fl & 8)) {
           const int64_t o = (int64_t)r.nn * D + off;
-          __stcg(reinterpret_cast<float4*>(a.I + o), orx_apply4<OPT>(r.n[k], gn, r.ns0[k], r.ns1[k], a.opt));
-          if (S0) __stcg(reinterpret_cast<float4*>(a.Is0 + o), r.ns0[k]);
-          if (S1) __stcg(reinterpret_cast<float4*>(a.Is1 + o), r.ns1[k]);
+          orx_st4_stream(a.I + o, orx_apply4<OPT>(r.n[k], gn, r.ns0[k], r.ns1[k], a.opt));
+          if (S0) orx_st4_stream(a.Is0 + o, r.ns0[k]);
+          if (S1) orx_st4_stream(a.Is1 + o, r.ns1[k]);
         } else {
           orx_red4(a.gi + (int64_t)r.dn * D + off, gn);
         }
@@ -340,9 +343,9 @@ __global__ void __launch_bounds__(256) k_pair_step_generic(const PairArgs a) {
       continue;
     }
     int du, dp, dn;
-    const uint32_t cu = orx_hash_find(a.hu, uu, &du);
-    const uint32_t cp = orx_hash_find(a.hi, pp, &dp);
-    const uint32_t cn = orx_hash_find(a.hi, nn, &dn);
+    const uint32_t cu = orx_hash_find<!STAGE_ONLY>(a.hu, uu, &du);
+    const uint32_t cp = orx_hash_find<!STAGE_ONLY>(a.hi, pp, &dp);
+    const uint32_t cn = orx_hash_find<!STAGE_ONLY>(a.hi, nn, &dn);
     const bool fu = !STAGE_ONLY && cu == 1u, fp = !STAGE_ONLY && cp == 1u, fn = !STAGE_ONLY && cn == 1u;
     float* ur = a.U + (int64_t)uu * D;
     float* pr = a.I + (int64_t)pp * D;
@@ -499,7 +502,8 @@ __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
   // The tail is a chain of dependent round trips (counters -> row id -> rows) over a few thousand rows, i.e. latency,
   // not bandwidth.  A warp therefore takes FOUR staged rows at once, eight lanes per row (a quarter-warp still covers
   // 128 contiguous bytes per access), and issues all of a row's loads before the first use: 12 independent 128-bit
-  // loads per lane in flight at D = 128.
+  // loads per lane in flight at D = 128.  Table and slot rows evict-first, staging rows (G) at normal priority: the
+  // step's red.adds left them in L2.
   const int sub = lane >> 3, sl = lane & 7;
   for (int r0 = gwarp * 4; r0 < nu + ni; r0 += nwarps * 4) {
     const int r = r0 + sub;
@@ -520,18 +524,18 @@ __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
           const int e = e0 + sl + 8 * k;
           const bool ld = on && e < nq;
           g[k] = ld ? __ldcg(reinterpret_cast<const float4*>(G) + e) : z4;
-          w[k] = (ld && !ZERO_ONLY) ? __ldcg(reinterpret_cast<const float4*>(W) + e) : z4;
-          s0v[k] = (ld && S0 && !ZERO_ONLY) ? __ldcg(reinterpret_cast<const float4*>(P0) + e) : z4;
-          s1v[k] = (ld && S1 && !ZERO_ONLY) ? __ldcg(reinterpret_cast<const float4*>(P1) + e) : z4;
+          w[k] = (ld && !ZERO_ONLY) ? orx_ld4_stream(W + 4 * e) : z4;
+          s0v[k] = (ld && S0 && !ZERO_ONLY) ? orx_ld4_stream(P0 + 4 * e) : z4;
+          s1v[k] = (ld && S1 && !ZERO_ONLY) ? orx_ld4_stream(P1 + 4 * e) : z4;
         }
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
           const int e = e0 + sl + 8 * k;
           if (!on || e >= nq) continue;
           if (!ZERO_ONLY) {
-            __stcg(reinterpret_cast<float4*>(W) + e, orx_apply4<OPT>(w[k], g[k], s0v[k], s1v[k], a.opt));
-            if (S0) __stcg(reinterpret_cast<float4*>(P0) + e, s0v[k]);
-            if (S1) __stcg(reinterpret_cast<float4*>(P1) + e, s1v[k]);
+            orx_st4_stream(W + 4 * e, orx_apply4<OPT>(w[k], g[k], s0v[k], s1v[k], a.opt));
+            if (S0) orx_st4_stream(P0 + 4 * e, s0v[k]);
+            if (S1) orx_st4_stream(P1 + 4 * e, s1v[k]);
           }
           __stcg(reinterpret_cast<float4*>(G) + e, z4);
         }
@@ -645,7 +649,9 @@ int orx_launch_adam_sweep(orx_ctx* c, float* var, float* m, float* v, int64_t ro
 // ---------------------------------------------------------------------------------------
 // D = 128 runs 4 CTAs/SM with a single register buffer (64 registers): the fastest of the variants A/B-tested in
 // profiles r1b/r1c/r2a (2-3 CTAs/SM with a register double-buffer, a cp.async shared-memory ring, and a
-// "last arriver applies" form without the tail launch were all slower and are gone).
+// "last arriver applies" form without the tail launch were all slower and are gone).  Re-checked on H100 SXM (700 W)
+// with the L2 priorities of k_pair_step in place, BPR Adagrad at the bench shape: CH = 16 measured the same as CH = 8,
+// 3 CTAs/SM was 1 % slower, and the register double-buffer (PIPE) 1-2 % slower at 2 or 3 CTAs/SM.
 template <int KIND, int OPT>
 static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, int* n_partials) {
   const int B = pa.B;
