@@ -79,6 +79,20 @@ ORX_API int orx_device_count(int* n_out_host);
 ORX_API int orx_stream_synchronize(orx_handle_t h, orx_stream_t stream);
 /* Test hook: place the handle's batch-index epoch counter (31 bits; the wrap path empties the hash tables). */
 ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
+/* Test hook: the kernel variants launched by this handle's DLRM entry points (orx_mlp_layer_*, orx_interact_*) since the
+ * last call, oldest first, at most cap of them (a ring of the last ORX_DISPATCH_LOG_CAP), then clears them.
+ * Record k is rec_host[8k .. 8k+7] = {op, variant, TA, TB, M, N, K, S}: a GEMM C[M,N] = op(A)[M,K] op(B)[K,N] with the
+ * operand layouts TA / TB of orx_dlrm.cu and S split-K slices (1 = no split); an interaction has M = B, N = F, K = D,
+ * TA = TB = 0, S = 1.  Host-side bookkeeping only: no device work, no synchronisation. */
+enum orx_dispatch_op { ORX_OP_GEMM = 0, ORX_OP_INTERACT_FWD = 1, ORX_OP_INTERACT_BWD = 2 };
+enum orx_dispatch_variant {
+  ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
+  ORX_VARIANT_GEMM_SIMT = 1,     /* k_gemm: fp32 SIMT tiles */
+  ORX_VARIANT_INTERACT_WARP = 2, /* k_interact_{fwd,bwd}_warp: one warp per sample */
+  ORX_VARIANT_INTERACT = 3       /* k_interact_{fwd,bwd}: one CTA per sample */
+};
+#define ORX_DISPATCH_LOG_CAP 64
+ORX_API int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec_host, int32_t cap, int32_t* n_host);
 
 /* Measurement hook (bench.py's roofline): while enabled, every 8th *_step call records CUDA events on its launch stream
  * around its launches -- pairwise / pointwise steps: [0] batch index (or the wait for a prefetched one), [1] the fused

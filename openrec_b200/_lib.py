@@ -16,6 +16,9 @@ ORX_PAIR_BPR, ORX_PAIR_UCML = 0, 1
 ORX_POINT_GMF, ORX_POINT_WRMF = 0, 1
 ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST = 0, 1
 ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE = 0, 1, 2, 3
+ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD = 0, 1, 2
+ORX_VARIANT_GEMM_TMA, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_INTERACT = 0, 1, 2, 3
+ORX_DISPATCH_LOG_CAP = 64
 
 
 class OrxOpt(C.Structure):
@@ -55,6 +58,7 @@ SIGNATURES = {
     "orx_device_count": [C.POINTER(C.c_int)],
     "orx_stream_synchronize": [_vp, _vp],
     "orx_debug_set_epoch": [_vp, C.c_uint32],
+    "orx_debug_dispatch_log": [_vp, C.POINTER(_i32), _i32, C.POINTER(_i32)],
     "orx_profile_enable": [_vp, _i32],
     "orx_profile_read": [_vp, C.POINTER(C.c_float), _i32, C.POINTER(_i32)],
     "orx_fill_uniform": [_vp, _vp, _i64, _f, _f, _u64, _vp],

@@ -77,7 +77,15 @@ struct orx_ctx {
   int64_t pf_rows_u, pf_rows_i;
   uint32_t epoch;          // hash epoch of the last step, in [1, 2^31)
   void* shard_ws;          // orx_shard.cu: local scratch of the row-sharded step (orx_shard_ws*)
+  int32_t dispatch[ORX_DISPATCH_LOG_CAP][8];   // orx_debug_dispatch_log: ring of the last DLRM launch decisions
+  int64_t dispatch_n;      // records written since the last read
 };
+
+// append {op, variant, TA, TB, M, N, K, S} to the handle's dispatch ring (host only)
+static inline void orx_log_dispatch(orx_ctx* c, int op, int variant, int TA, int TB, int M, int N, int K, int S) {
+  int32_t* r = c->dispatch[c->dispatch_n++ % ORX_DISPATCH_LOG_CAP];
+  r[0] = op; r[1] = variant; r[2] = TA; r[3] = TB; r[4] = M; r[5] = N; r[6] = K; r[7] = S;
+}
 
 // Start a new hash epoch (once per step, before the index build; `st` = the stream the step runs on).
 // A slot word holds 31 epoch bits: epochs live in [1, 2^31) and on wrap every table is zeroed on `st`, so a stale

@@ -147,6 +147,18 @@ extern "C" int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch) {
   return ORX_OK;
 }
 
+// test hook: which kernel each DLRM entry point launched (tests/test_gpu_dlrm.py asserts the dispatch of every case)
+extern "C" int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec, int32_t cap, int32_t* n) {
+  ORX_REQUIRE(h != nullptr && n && cap >= 0 && (rec || cap == 0), "bad arguments");
+  const int64_t held = h->dispatch_n < ORX_DISPATCH_LOG_CAP ? h->dispatch_n : ORX_DISPATCH_LOG_CAP;
+  const int64_t first = h->dispatch_n - held;   // oldest record still in the ring
+  const int64_t take = held < cap ? held : cap;
+  for (int64_t i = 0; i < take; ++i) memcpy(rec + 8 * i, h->dispatch[(first + i) % ORX_DISPATCH_LOG_CAP], 8 * sizeof(int32_t));
+  *n = (int32_t)take;
+  h->dispatch_n = 0;
+  return ORX_OK;
+}
+
 int orx_ensure_stage(orx_ctx* c, int64_t n_ints) {
   if (n_ints <= c->stage_cap) return ORX_OK;
   ORX_CUDA(cudaDeviceSynchronize());

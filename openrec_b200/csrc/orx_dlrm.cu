@@ -4,8 +4,6 @@
 //
 // Reference path: openrec/tf2/recommenders/dlrm.py:63-100, modules/multi_layer_perceptron.py:5-18,
 // modules/second_order_feature_interaction.py:12-34.
-#include <stdlib.h>
-
 #include "orx_common.cuh"
 
 // ---------------------------------------------------------------------------------------
@@ -315,6 +313,7 @@ extern "C" int orx_interact_fwd(orx_handle_t h, const float* emb, int64_t emb_ld
     if (grid > h->num_sms * 4) grid = h->num_sms * 4;
     k_interact_fwd_warp<<<grid, INTER_WARPS * 32, sm, (cudaStream_t)s>>>(emb, emb_ld, dense, dense_ld, B, F, D, self_interaction, out, out_ld);
     ORX_LAUNCH_CHECK();
+    orx_log_dispatch(h, ORX_OP_INTERACT_FWD, ORX_VARIANT_INTERACT_WARP, 0, 0, B, F, D, 1);
     return ORX_OK;
   }
   const size_t smem = sizeof(float) * (size_t)F * (D + 1);
@@ -322,6 +321,7 @@ extern "C" int orx_interact_fwd(orx_handle_t h, const float* emb, int64_t emb_ld
   if (smem > 48 * 1024) ORX_CUDA(cudaFuncSetAttribute(k_interact_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k_interact_fwd<<<B, 128, smem, (cudaStream_t)s>>>(emb, emb_ld, dense, dense_ld, B, F, D, self_interaction, mode, out, out_ld);
   ORX_LAUNCH_CHECK();
+  orx_log_dispatch(h, ORX_OP_INTERACT_FWD, ORX_VARIANT_INTERACT, 0, 0, B, F, D, 1);
   return ORX_OK;
 }
 
@@ -342,6 +342,7 @@ extern "C" int orx_interact_bwd(orx_handle_t h, const float* emb, int64_t emb_ld
     if (grid > h->num_sms * 3) grid = h->num_sms * 3;
     k_interact_bwd_warp<<<grid, INTER_WARPS * 32, sm, (cudaStream_t)s>>>(emb, emb_ld, dense, dense_ld, dout, dout_ld, B, F, D, self_interaction, demb, demb_ld, ddense, ddense_ld);
     ORX_LAUNCH_CHECK();
+    orx_log_dispatch(h, ORX_OP_INTERACT_BWD, ORX_VARIANT_INTERACT_WARP, 0, 0, B, F, D, 1);
     return ORX_OK;
   }
   const size_t smem = sizeof(float) * ((size_t)F * (D + 1) + (size_t)F * F);
@@ -349,6 +350,7 @@ extern "C" int orx_interact_bwd(orx_handle_t h, const float* emb, int64_t emb_ld
   if (smem > 48 * 1024) ORX_CUDA(cudaFuncSetAttribute(k_interact_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k_interact_bwd<<<B, 128, smem, (cudaStream_t)s>>>(emb, emb_ld, dense, dense_ld, dout, dout_ld, B, F, D, self_interaction, mode, demb, demb_ld, ddense, ddense_ld);
   ORX_LAUNCH_CHECK();
+  orx_log_dispatch(h, ORX_OP_INTERACT_BWD, ORX_VARIANT_INTERACT, 0, 0, B, F, D, 1);
   return ORX_OK;
 }
 
@@ -424,29 +426,18 @@ __global__ void __launch_bounds__(256) k_gemm(const float* __restrict__ A, int64
   }
 }
 
-int orx_launch_gemm_tc(int TA, int TB, const float* A, int64_t lda, const float* Bm, int64_t ldb, float* C, int64_t ldc,
-                       int M, int N, int K, const float* bias, int act, cudaStream_t st);   // orx_mlp_tc.cu
+int orx_launch_gemm_tc(orx_ctx* h, int TA, int TB, const float* A, int64_t lda, const float* Bm, int64_t ldb, float* C,
+                       int64_t ldc, int M, int N, int K, const float* bias, int act, cudaStream_t st);   // orx_mlp_tc.cu
 float* orx_splitk_workspace(size_t floats);                                                  // orx_mlp_tc.cu
 int orx_launch_splitk_reduce(const float* part, int S, int M, int N, float* C, int64_t ldc, const float* bias, int act,
                              cudaStream_t st);
 
-// ORX_MLP_SIMT=1 forces the fp32 SIMT tiles (the reference the tensor-core path is checked against in the tests)
-static bool mlp_use_tc() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("ORX_MLP_SIMT");
-    v = (e && atoi(e)) ? 0 : 1;
-  }
-  return v != 0;
-}
-
 template <int TA, int TB>
-static int launch_gemm(const float* A, int64_t lda, const float* Bm, int64_t ldb, float* C, int64_t ldc, int M, int N,
-                       int K, const float* bias, int act, cudaStream_t st) {
-  if (mlp_use_tc()) {   // tensor cores (wgmma, 3xTF32) whenever the shape fills a tile reasonably
-    const int rc = orx_launch_gemm_tc(TA, TB, A, lda, Bm, ldb, C, ldc, M, N, K, bias, act, st);
-    if (rc != ORX_ERR_UNSUPPORTED) return rc;
-  }
+static int launch_gemm(orx_ctx* h, const float* A, int64_t lda, const float* Bm, int64_t ldb, float* C, int64_t ldc, int M,
+                       int N, int K, const float* bias, int act, cudaStream_t st) {
+  // tensor cores (wgmma, 3xTF32) whenever the shape fills a tile reasonably and the TMA can describe the operands
+  const int rc = orx_launch_gemm_tc(h, TA, TB, A, lda, Bm, ldb, C, ldc, M, N, K, bias, act, st);
+  if (rc != ORX_ERR_UNSUPPORTED) return rc;
   const int tiles = ((N + 63) / 64) * ((M + 63) / 64);
   int S = 1;
   const int sms = orx_current_sms();
@@ -463,6 +454,7 @@ static int launch_gemm(const float* A, int64_t lda, const float* Bm, int64_t ldb
   dim3 grid((N + 63) / 64, (M + 63) / 64, S);
   k_gemm<TA, TB><<<grid, 256, 0, st>>>(A, lda, Bm, ldb, C, ldc, M, N, K, bias, act, part);
   ORX_LAUNCH_CHECK();
+  orx_log_dispatch(h, ORX_OP_GEMM, ORX_VARIANT_GEMM_SIMT, TA, TB, M, N, K, S);
   if (S > 1) return orx_launch_splitk_reduce(part, S, M, N, C, ldc, bias, act, st);
   return ORX_OK;
 }
@@ -474,7 +466,7 @@ extern "C" int orx_mlp_layer_fwd(orx_handle_t h, const float* x, int64_t ldx, in
   ORX_REQUIRE(B >= 0 && in > 0 && out > 0 && ldx >= in && ldy >= out && act >= 0 && act <= 2, "bad sizes");
   if (B == 0) return ORX_OK;
   ORX_CUDA(cudaSetDevice(h->device));
-  return launch_gemm<0, 0>(x, ldx, w, out, y, ldy, B, out, in, bias, act, (cudaStream_t)s);
+  return launch_gemm<0, 0>(h, x, ldx, w, out, y, ldy, B, out, in, bias, act, (cudaStream_t)s);
 }
 
 // dz = dy * act'(y) in place; db[n] = sum_b dz[b,n]
@@ -543,9 +535,9 @@ extern "C" int orx_mlp_layer_bwd(orx_handle_t h, const float* x, int64_t ldx, co
       ORX_LAUNCH_CHECK();
     }
   }
-  int rc = launch_gemm<1, 0>(x, ldx, dy, lddy, dw, out, in, out, B, nullptr, 0, st);   // dw = x^T dz
+  int rc = launch_gemm<1, 0>(h, x, ldx, dy, lddy, dw, out, in, out, B, nullptr, 0, st);   // dw = x^T dz
   if (rc) return rc;
-  if (dx) rc = launch_gemm<0, 1>(dy, lddy, w, out, dx, lddx, B, in, out, nullptr, 0, st);   // dx = dz w^T
+  if (dx) rc = launch_gemm<0, 1>(h, dy, lddy, w, out, dx, lddx, B, in, out, nullptr, 0, st);   // dx = dz w^T
   return rc;
 }
 

@@ -403,10 +403,12 @@ int orx_launch_splitk_reduce(const float* part, int S, int M, int N, float* C, i
 }
 
 // C[M,N] = op(A) * op(B) (+bias, act) on wgmma; same operand conventions as launch_gemm in orx_dlrm.cu.
-// Returns ORX_ERR_UNSUPPORTED for shapes that are left to the SIMT kernel: tiny N / K / M, or operands the TMA cannot
-// describe (base not 16-byte aligned, row stride not a multiple of 16 bytes).
-int orx_launch_gemm_tc(int TA, int TB, const float* A, int64_t lda, const float* Bm, int64_t ldb, float* C, int64_t ldc,
-                       int M, int N, int K, const float* bias, int act, cudaStream_t st) {
+// Returns ORX_ERR_UNSUPPORTED for shapes that are left to the SIMT kernel: tiny N / K / M, operands the TMA cannot
+// describe (base not 16-byte aligned, row stride not a multiple of 16 bytes), or TA = TB = 1, which no Dense-layer GEMM
+// uses.  A launch is recorded in h's dispatch log.
+int orx_launch_gemm_tc(orx_ctx* h, int TA, int TB, const float* A, int64_t lda, const float* Bm, int64_t ldb, float* C,
+                       int64_t ldc, int M, int N, int K, const float* bias, int act, cudaStream_t st) {
+  if (TA == 1 && TB == 1) return ORX_ERR_UNSUPPORTED;
   if (N < 16 || K < 8 || M < 64) return ORX_ERR_UNSUPPORTED;
   if ((lda & 3) || (ldb & 3) || (((uintptr_t)A | (uintptr_t)Bm) & 15)) return ORX_ERR_UNSUPPORTED;
   const int tiles = ((N + TN - 1) / TN) * ((M + TM - 1) / TM);
@@ -429,11 +431,11 @@ int orx_launch_gemm_tc(int TA, int TB, const float* A, int64_t lda, const float*
   if ((rc = make_map(&tb, Bm, N, K, ldb, TB == 1, TN))) return rc;
 #define ORX_TMA(a, b) rc = launch_tma<a, b>(ta, tb, C, ldc, M, N, K, bias, act, part, S, st)
   if (TA == 0 && TB == 0) ORX_TMA(0, 0);
-  else if (TA == 0 && TB == 1) ORX_TMA(0, 1);
-  else if (TA == 1 && TB == 0) ORX_TMA(1, 0);
-  else ORX_TMA(1, 1);
+  else if (TA == 0) ORX_TMA(0, 1);
+  else ORX_TMA(1, 0);
 #undef ORX_TMA
   if (rc) return rc;
+  orx_log_dispatch(h, ORX_OP_GEMM, ORX_VARIANT_GEMM_TMA, TA, TB, M, N, K, S);
   if (S > 1) return orx_launch_splitk_reduce(part, S, M, N, C, ldc, bias, act, st);
   return ORX_OK;
 }

@@ -3,19 +3,25 @@ liborx does all the arithmetic.  Every function enqueues on torch's current CUDA
 from __future__ import annotations
 
 import ctypes as C
+from collections import namedtuple
 
 import torch
 
 from . import _lib
-from ._lib import (ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
-                   ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, OrxOpt,
-                   OrxTable)
+from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE,
+                   ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR, ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF,
+                   ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_GEMM_TMA,
+                   ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, OrxOpt, OrxTable)
 
 __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", "ORX_POINT_GMF", "ORX_POINT_WRMF",
            "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_SCORE_DOT",
-           "ORX_SCORE_NEG_SQDIST"]
+           "ORX_SCORE_NEG_SQDIST", "ORX_OP_GEMM", "ORX_OP_INTERACT_FWD", "ORX_OP_INTERACT_BWD", "ORX_VARIANT_GEMM_TMA",
+           "ORX_VARIANT_GEMM_SIMT", "ORX_VARIANT_INTERACT_WARP", "ORX_VARIANT_INTERACT", "Dispatch"]
 
 _engines = {}
+
+# one record of orx_debug_dispatch_log: which kernel an orx_mlp_layer_* / orx_interact_* call launched
+Dispatch = namedtuple("Dispatch", "op variant ta tb m n k s")
 
 
 def _ptr(t):
@@ -127,6 +133,14 @@ class Engine:
 
     def debug_set_epoch(self, epoch):
         _lib.check(self.lib.orx_debug_set_epoch(self.h, epoch), "orx_debug_set_epoch")
+
+    def debug_dispatch_log(self):
+        """-> [Dispatch] launched by this engine's DLRM calls since the last read (oldest first), and clears them."""
+        rec = (C.c_int32 * (8 * _lib.ORX_DISPATCH_LOG_CAP))()
+        n = C.c_int32()
+        _lib.check(self.lib.orx_debug_dispatch_log(self.h, rec, _lib.ORX_DISPATCH_LOG_CAP, C.byref(n)),
+                   "orx_debug_dispatch_log")
+        return [Dispatch(*rec[8 * i:8 * i + 8]) for i in range(n.value)]
 
     def pairwise_fwd(self, kind, user, item, bias, uid, pid, nid, out4, margin=0.5):
         _lib.check(self.lib.orx_pairwise_fwd(self.h, kind, C.byref(user), C.byref(item), C.byref(bias), _ptr(uid),

@@ -31,10 +31,17 @@ class GemmProfile:
     def __exit__(self, *a):
         GemmProfile.active = None
 
-    def bracket(self, flops, pure=False):
+    def time(self, eng, flops, call):
+        """Run call() between two events; the call is 'pure' when the engine's dispatch log shows exactly one
+        k_gemm_tma launch without split-K."""
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        eng.debug_dispatch_log()                  # drop the records of earlier calls
+        e0.record()
+        call()
+        e1.record()
+        rec = eng.debug_dispatch_log()
+        pure = len(rec) == 1 and rec[0].variant == N.ORX_VARIANT_GEMM_TMA and rec[0].s == 1
         self.ev.append((e0, e1, flops, pure))
-        return e0, e1
 
     def totals(self, pure_only=False):
         """(ms, flops, calls) over all bracketed Dense-layer calls, or only over the calls that are ONE wgmma GEMM
@@ -48,21 +55,15 @@ def _mlp_fwd(eng, x, w, b, act, y):
     p = GemmProfile.active
     if p is None:
         return eng.mlp_fwd(x, w, b, act, y)
-    tc = x.shape[0] >= 64 and w.shape[0] >= 8 and w.shape[1] >= 16 and x.stride(0) % 4 == 0   # orx_launch_gemm_tc's rule
-    e0, e1 = p.bracket(2.0 * x.shape[0] * w.shape[0] * w.shape[1], pure=tc)
-    e0.record()
-    eng.mlp_fwd(x, w, b, act, y)
-    e1.record()
+    p.time(eng, 2.0 * x.shape[0] * w.shape[0] * w.shape[1], lambda: eng.mlp_fwd(x, w, b, act, y))
 
 
 def _mlp_bwd(eng, x, y, w, act, dy, dx, dw, db):
     p = GemmProfile.active
     if p is None:
         return eng.mlp_bwd(x, y, w, act, dy, dx, dw, db)
-    e0, e1 = p.bracket((4.0 if dx is not None else 2.0) * x.shape[0] * w.shape[0] * w.shape[1])
-    e0.record()
-    eng.mlp_bwd(x, y, w, act, dy, dx, dw, db)
-    e1.record()
+    p.time(eng, (4.0 if dx is not None else 2.0) * x.shape[0] * w.shape[0] * w.shape[1],
+           lambda: eng.mlp_bwd(x, y, w, act, dy, dx, dw, db))
 
 ACT = {None: 0, "linear": 0, "relu": 1, "sigmoid": 2}
 
