@@ -79,17 +79,30 @@ ORX_API int orx_device_count(int* n_out_host);
 ORX_API int orx_stream_synchronize(orx_handle_t h, orx_stream_t stream);
 /* Test hook: place the handle's batch-index epoch counter (31 bits; the wrap path empties the hash tables). */
 ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
-/* Test hook: the kernel variants launched by this handle's DLRM entry points (orx_mlp_layer_*, orx_interact_*) since the
- * last call, oldest first, at most cap of them (a ring of the last ORX_DISPATCH_LOG_CAP), then clears them.
+/* Test hook: the kernel variants launched by this handle's DLRM entry points (orx_mlp_layer_*, orx_interact_*) and
+ * sparse steps (orx_pairwise_step, orx_pairwise_step_host, orx_pointwise_step) since the last call, oldest first, at
+ * most cap of them (a ring of the last ORX_DISPATCH_LOG_CAP), then clears them.
  * Record k is rec_host[8k .. 8k+7] = {op, variant, TA, TB, M, N, K, S}: a GEMM C[M,N] = op(A)[M,K] op(B)[K,N] with the
  * operand layouts TA / TB of orx_dlrm.cu and S split-K slices (1 = no split); an interaction has M = B, N = F, K = D,
- * TA = TB = 0, S = 1.  Host-side bookkeeping only: no device work, no synchronisation. */
-enum orx_dispatch_op { ORX_OP_GEMM = 0, ORX_OP_INTERACT_FWD = 1, ORX_OP_INTERACT_BWD = 2 };
+ * TA = TB = 0, S = 1.  A sparse step (one record per call) has TA = kind (orx_pair_kind / orx_point_kind), TB = optimizer
+ * (orx_opt_kind), M = B, N = D, K = the CTAs/SM bound of the fused kernel's __launch_bounds__ (0: none) and S = the batch
+ * index set it used: 0 = built on the caller's stream, 1 or 2 = a consumed prefetch (orx_pairwise_prefetch, or the side
+ * stream of orx_pairwise_step_host).  Host-side bookkeeping only: no device work, no synchronisation. */
+enum orx_dispatch_op {
+  ORX_OP_GEMM = 0,
+  ORX_OP_INTERACT_FWD = 1,
+  ORX_OP_INTERACT_BWD = 2,
+  ORX_OP_PAIRWISE_STEP = 3,  /* orx_pairwise_step, orx_pairwise_step_host */
+  ORX_OP_POINTWISE_STEP = 4  /* orx_pointwise_step */
+};
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
   ORX_VARIANT_GEMM_SIMT = 1,     /* k_gemm: fp32 SIMT tiles */
   ORX_VARIANT_INTERACT_WARP = 2, /* k_interact_{fwd,bwd}_warp: one warp per sample */
-  ORX_VARIANT_INTERACT = 3       /* k_interact_{fwd,bwd}: one CTA per sample */
+  ORX_VARIANT_INTERACT = 3,      /* k_interact_{fwd,bwd}: one CTA per sample */
+  ORX_VARIANT_STEP = 4,          /* k_pair_step / k_point_step specialised on D (32, 64, 128, 256), one register buffer */
+  ORX_VARIANT_STEP_PIPE = 5,     /* k_pair_step with the register double buffer (PIPE) */
+  ORX_VARIANT_STEP_GENERIC = 6   /* k_pair_step_generic / k_point_generic: any D */
 };
 #define ORX_DISPATCH_LOG_CAP 64
 ORX_API int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec_host, int32_t cap, int32_t* n_host);

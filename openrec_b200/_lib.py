@@ -16,8 +16,9 @@ ORX_PAIR_BPR, ORX_PAIR_UCML = 0, 1
 ORX_POINT_GMF, ORX_POINT_WRMF = 0, 1
 ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST = 0, 1
 ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE = 0, 1, 2, 3
-ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD = 0, 1, 2
+ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP = 0, 1, 2, 3, 4
 ORX_VARIANT_GEMM_TMA, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_INTERACT = 0, 1, 2, 3
+ORX_VARIANT_STEP, ORX_VARIANT_STEP_PIPE, ORX_VARIANT_STEP_GENERIC = 4, 5, 6
 ORX_DISPATCH_LOG_CAP = 64
 
 

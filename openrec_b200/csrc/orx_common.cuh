@@ -77,7 +77,7 @@ struct orx_ctx {
   int64_t pf_rows_u, pf_rows_i;
   uint32_t epoch;          // hash epoch of the last step, in [1, 2^31)
   void* shard_ws;          // orx_shard.cu: local scratch of the row-sharded step (orx_shard_ws*)
-  int32_t dispatch[ORX_DISPATCH_LOG_CAP][8];   // orx_debug_dispatch_log: ring of the last DLRM launch decisions
+  int32_t dispatch[ORX_DISPATCH_LOG_CAP][8];   // orx_debug_dispatch_log: ring of the last DLRM / sparse-step launches
   int64_t dispatch_n;      // records written since the last read
 };
 
@@ -354,6 +354,6 @@ int orx_launch_adam_sweep(orx_ctx* c, float* var, float* m, float* v, int64_t ro
                           const float* gstage, const OrxOptDev& o, cudaStream_t st);
 int orx_ensure_partials(orx_ctx* c, int need, cudaStream_t st);
 int orx_launch_reduce_partials(const float* partials, int n, float loss_scale, float* out4, cudaStream_t st);
-int orx_launch_index_build(orx_ctx* c, const int32_t* a, int64_t rows_a, int32_t na, const int32_t* b0,
-                           const int32_t* b1, int64_t rows_b, int32_t nb, int mode /* orx_hash_insert mode: 0 | 1 */,
-                           cudaStream_t st);
+// index of n samples (a[t], b0[t]) or (a[t], b0[t], b1[t]); only samples whose ids are all in range are inserted
+int orx_launch_index_build(orx_ctx* c, const int32_t* a, int64_t rows_a, const int32_t* b0, const int32_t* b1,
+                           int64_t rows_b, int32_t n, int mode /* orx_hash_insert mode: 0 | 1 */, cudaStream_t st);

@@ -147,7 +147,8 @@ extern "C" int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch) {
   return ORX_OK;
 }
 
-// test hook: which kernel each DLRM entry point launched (tests/test_gpu_dlrm.py asserts the dispatch of every case)
+// test hook: which kernel each DLRM entry point and sparse step launched (tests/test_gpu_dlrm.py and
+// tests/test_gpu_kernels.py assert the dispatch of every case)
 extern "C" int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec, int32_t cap, int32_t* n) {
   ORX_REQUIRE(h != nullptr && n && cap >= 0 && (rec || cap == 0), "bad arguments");
   const int64_t held = h->dispatch_n < ORX_DISPATCH_LOG_CAP ? h->dispatch_n : ORX_DISPATCH_LOG_CAP;

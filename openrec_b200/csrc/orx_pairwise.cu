@@ -5,7 +5,7 @@
 //   + tape.gradient + optimizer.apply_gradients (tf2_examples/bpr_citeulike.py:33-39).
 //
 // Synchronous-batch semantics in three launches on one stream:
-//   1. k_index_build : hash every id of the batch; rows hit more than once get a "staging" slot.
+//   1. k_index_build : hash every id of the batch's valid triplets; rows hit more than once get a "staging" slot.
 //   2. k_pair_step   : per triplet gather u,p,n (128-bit loads), score, loss, per-sample gradient.
 //        * a row referenced exactly once in the batch is owned by its triplet: optimizer applied
 //          in registers, row + slots written back once (read once, written once == algorithmic bytes);
@@ -21,21 +21,27 @@
 // ---------------------------------------------------------------------------------------
 // K9: batch index
 // ---------------------------------------------------------------------------------------
-__global__ void k_index_build(OrxHash hu, OrxHash hi, const int32_t* __restrict__ a, int64_t rows_a, int na,
-                              const int32_t* __restrict__ b0, const int32_t* __restrict__ b1, int64_t rows_b, int nb,
+// Sample t of the batch is (a[t], b0[t]) (pointwise) or (a[t], b0[t], b1[t]) (pairwise); one thread per id.  Every bad
+// id is counted.  A good id is inserted only when the whole sample is good: the step skips a sample with a bad id, so a
+// row that only skipped samples reference must not be staged (the tail would apply the optimizer to it with g = 0, which
+// moves an Adam row).
+__global__ void k_index_build(OrxHash hu, OrxHash hi, const int32_t* __restrict__ a, int64_t rows_a,
+                              const int32_t* __restrict__ b0, const int32_t* __restrict__ b1, int64_t rows_b, int n,
                               int stage_all, int32_t* bad) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int total = na + (b1 ? 2 * nb : nb);
-  if (i >= total) return;
-  if (i < na) {
-    const int32_t id = a[i];
-    if (id >= 0 && (int64_t)id < rows_a) orx_hash_insert(hu, id, stage_all);
-    else atomicAdd(bad, 1);
+  if (i >= (b1 ? 3 : 2) * n) return;
+  const int t = i < n ? i : (i < 2 * n ? i - n : i - 2 * n);
+  const int32_t ia = a[t], ib0 = b0[t], ib1 = b1 ? b1[t] : 0;
+  const bool ga = ia >= 0 && (int64_t)ia < rows_a, gb0 = ib0 >= 0 && (int64_t)ib0 < rows_b,
+             gb1 = ib1 >= 0 && (int64_t)ib1 < rows_b;
+  const bool all = ga && gb0 && gb1;
+  if (i < n) {
+    if (!ga) atomicAdd(bad, 1);
+    else if (all) orx_hash_insert(hu, ia, stage_all);
   } else {
-    const int j = i - na;
-    const int32_t id = j < nb ? b0[j] : b1[j - nb];
-    if (id >= 0 && (int64_t)id < rows_b) orx_hash_insert(hi, id, stage_all);
-    else atomicAdd(bad, 1);
+    const bool g = i < 2 * n ? gb0 : gb1;
+    if (!g) atomicAdd(bad, 1);
+    else if (all) orx_hash_insert(hi, i < 2 * n ? ib0 : ib1, stage_all);
   }
 }
 
@@ -61,13 +67,13 @@ int orx_launch_index_build_strided(orx_ctx* c, const int32_t* a, int64_t stride,
   return ORX_OK;
 }
 
-int orx_launch_index_build(orx_ctx* c, const int32_t* a, int64_t rows_a, int32_t na, const int32_t* b0,
-                           const int32_t* b1, int64_t rows_b, int32_t nb, int mode, cudaStream_t st) {
-  const int total = na + (b1 ? 2 * nb : nb);
+int orx_launch_index_build(orx_ctx* c, const int32_t* a, int64_t rows_a, const int32_t* b0, const int32_t* b1,
+                           int64_t rows_b, int32_t n, int mode, cudaStream_t st) {
+  const int total = (b1 ? 3 : 2) * n;
   if (total <= 0) return ORX_OK;
   int rc = orx_next_epoch(c, st);
   if (rc) return rc;
-  k_index_build<<<(total + 255) / 256, 256, 0, st>>>(c->hu, c->hi, a, rows_a, na, b0, b1, rows_b, nb, mode, c->counters + 3);
+  k_index_build<<<(total + 255) / 256, 256, 0, st>>>(c->hu, c->hi, a, rows_a, b0, b1, rows_b, n, mode, c->counters + 3);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
@@ -652,37 +658,43 @@ int orx_launch_adam_sweep(orx_ctx* c, float* var, float* m, float* v, int64_t ro
 // "last arriver applies" form without the tail launch were all slower and are gone).  Re-checked on H100 SXM (700 W)
 // with the L2 priorities of k_pair_step in place, BPR Adagrad at the bench shape: CH = 16 measured the same as CH = 8,
 // 3 CTAs/SM was 1 % slower, and the register double-buffer (PIPE) 1-2 % slower at 2 or 3 CTAs/SM.
+// *variant / *minb: the orx_dispatch_variant launched and its CTAs/SM bound, for the dispatch record.
 template <int KIND, int OPT>
-static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, int* n_partials) {
+static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, int* n_partials, int* variant, int* minb) {
   const int B = pa.B;
   constexpr bool LAZY = (OPT == ORX_OPT_ADAM_LAZY);  // 9 rows per triplet: no register double-buffer
-  auto go = [&](auto kern, int ch) {
+  auto go = [&](auto kern, int ch, int v, int mb) {
     const int nw = (B + ch - 1) / ch;
     const int blocks = (nw + 7) / 8;
     *n_partials = blocks;
+    *variant = v;
+    *minb = mb;
     orx_launch_pdl(kern, dim3(blocks), dim3(256), 0, st, pa);
   };
+  constexpr int PV = LAZY ? ORX_VARIANT_STEP : ORX_VARIANT_STEP_PIPE;
   switch (pa.D) {
-    case 32: go(k_pair_step<KIND, OPT, 32, 8, 2, !LAZY>, 8); break;
-    case 64: go(k_pair_step<KIND, OPT, 64, 8, 2, !LAZY>, 8); break;
+    case 32: go(k_pair_step<KIND, OPT, 32, 8, 2, !LAZY>, 8, PV, 2); break;
+    case 64: go(k_pair_step<KIND, OPT, 64, 8, 2, !LAZY>, 8, PV, 2); break;
     case 128:
-      if (LAZY) go(k_pair_step<KIND, OPT, 128, 8, 3, false>, 8);
-      else go(k_pair_step<KIND, OPT, 128, 8, 4, false>, 8);
+      if (LAZY) go(k_pair_step<KIND, OPT, 128, 8, 3, false>, 8, ORX_VARIANT_STEP, 3);
+      else go(k_pair_step<KIND, OPT, 128, 8, 4, false>, 8, ORX_VARIANT_STEP, 4);
       break;
-    case 256: go(k_pair_step<KIND, OPT, 256, 8, 2, !LAZY>, 8); break;
-    default: go(k_pair_step_generic<KIND, OPT>, 8); break;
+    case 256: go(k_pair_step<KIND, OPT, 256, 8, 2, !LAZY>, 8, PV, 2); break;
+    default: go(k_pair_step_generic<KIND, OPT>, 8, ORX_VARIANT_STEP_GENERIC, 0); break;
   }
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
 
 template <int KIND>
-static int launch_pair_step_kind(const PairArgs& pa, int opt_kind, cudaStream_t st, int* n_partials) {
+static int launch_pair_step_kind(const PairArgs& pa, int opt_kind, cudaStream_t st, int* n_partials, int* variant,
+                                 int* minb) {
   switch (opt_kind) {
-    case ORX_OPT_SGD: return launch_pair_step_kind_opt<KIND, ORX_OPT_SGD>(pa, st, n_partials);
-    case ORX_OPT_ADAGRAD: return launch_pair_step_kind_opt<KIND, ORX_OPT_ADAGRAD>(pa, st, n_partials);
-    case ORX_OPT_ADAM_LAZY: return launch_pair_step_kind_opt<KIND, ORX_OPT_ADAM_LAZY>(pa, st, n_partials);
-    case ORX_OPT_ADAM_DENSE: return launch_pair_step_kind_opt<KIND, ORX_OPT_ADAM_DENSE>(pa, st, n_partials);
+    case ORX_OPT_SGD: return launch_pair_step_kind_opt<KIND, ORX_OPT_SGD>(pa, st, n_partials, variant, minb);
+    case ORX_OPT_ADAGRAD: return launch_pair_step_kind_opt<KIND, ORX_OPT_ADAGRAD>(pa, st, n_partials, variant, minb);
+    case ORX_OPT_ADAM_LAZY: return launch_pair_step_kind_opt<KIND, ORX_OPT_ADAM_LAZY>(pa, st, n_partials, variant, minb);
+    case ORX_OPT_ADAM_DENSE:
+      return launch_pair_step_kind_opt<KIND, ORX_OPT_ADAM_DENSE>(pa, st, n_partials, variant, minb);
   }
   orx_set_error("unknown optimizer kind %d", opt_kind);
   return ORX_ERR_INVALID;
@@ -743,7 +755,7 @@ static int prefetch_issue(orx_ctx* c, const int32_t* uid, const int32_t* pid, co
   int rc = orx_next_epoch(c, ss);
   if (rc) return rc;
   c->pf_u[k].epoch = c->pf_i[k].epoch = c->epoch;
-  k_index_build<<<(3 * B + 255) / 256, 256, 0, ss>>>(c->pf_u[k], c->pf_i[k], uid, rows_u, B, pid, nid, rows_i, B, mode,
+  k_index_build<<<(3 * B + 255) / 256, 256, 0, ss>>>(c->pf_u[k], c->pf_i[k], uid, rows_u, pid, nid, rows_i, B, mode,
                                                      c->counters + 4 * (1 + k) + 3);
   ORX_LAUNCH_CHECK();
   ORX_CUDA(cudaEventRecord(c->pf_done[k], ss));
@@ -805,17 +817,18 @@ static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, con
     c->pf_valid = 0;
   } else {
     if ((rc = prefetch_drop(c, st))) return rc;
-    if ((rc = orx_launch_index_build(c, uid, user->rows, B, pid, nid, item->rows, B, dense ? 1 : 0, st))) return rc;
+    if ((rc = orx_launch_index_build(c, uid, user->rows, pid, nid, item->rows, B, dense ? 1 : 0, st))) return rc;
   }
   const OrxHash& HU = set ? c->pf_u[set - 1] : c->hu;
   const OrxHash& HI = set ? c->pf_i[set - 1] : c->hi;
   int32_t* ctr = c->counters + 4 * set;
   orx_prof_mark(c, 1, st);
   pa.hu = HU; pa.hi = HI;
-  int n_partials = 0;
-  rc = (kind == ORX_PAIR_BPR) ? launch_pair_step_kind<ORX_PAIR_BPR>(pa, opt->kind, st, &n_partials)
-                              : launch_pair_step_kind<ORX_PAIR_UCML>(pa, opt->kind, st, &n_partials);
+  int n_partials = 0, variant = 0, minb = 0;
+  rc = (kind == ORX_PAIR_BPR) ? launch_pair_step_kind<ORX_PAIR_BPR>(pa, opt->kind, st, &n_partials, &variant, &minb)
+                              : launch_pair_step_kind<ORX_PAIR_UCML>(pa, opt->kind, st, &n_partials, &variant, &minb);
   if (rc) return rc;
+  orx_log_dispatch(c, ORX_OP_PAIRWISE_STEP, variant, kind, opt->kind, B, D, minb, set);
   orx_prof_mark(c, 2, st);
   if (dense) {
     if ((rc = orx_launch_adam_sweep(c, user->var, user->s0, user->s1, user->rows, D, HU, c->gu, pa.opt, st))) return rc;

@@ -321,28 +321,33 @@ __global__ void k_gmf_w_terms(const float* W, int D, float* out4, float* d_w, fl
   if (threadIdx.x == 0 && out4) out4[1] += 0.5f * sh[0];
 }
 
+// *variant: the orx_dispatch_variant launched, for the dispatch record
 template <int KIND, int OPT>
-static int launch_point_kind_opt(const PointArgs& pa, cudaStream_t st, int* n_partials) {
+static int launch_point_kind_opt(const PointArgs& pa, cudaStream_t st, int* n_partials, int* variant) {
   const int nw = (pa.B + 7) / 8, blocks = (nw + 7) / 8;
   *n_partials = blocks * 8;
+  *variant = ORX_VARIANT_STEP;
   switch (pa.D) {
     case 32: k_point_step<KIND, OPT, 32, 8><<<blocks, 256, 0, st>>>(pa); break;
     case 64: k_point_step<KIND, OPT, 64, 8><<<blocks, 256, 0, st>>>(pa); break;
     case 128: k_point_step<KIND, OPT, 128, 8><<<blocks, 256, 0, st>>>(pa); break;
     case 256: k_point_step<KIND, OPT, 256, 8><<<blocks, 256, 0, st>>>(pa); break;
-    default: k_point_generic<KIND, OPT, 0><<<blocks, 256, 0, st>>>(pa); break;
+    default:
+      *variant = ORX_VARIANT_STEP_GENERIC;
+      k_point_generic<KIND, OPT, 0><<<blocks, 256, 0, st>>>(pa);
+      break;
   }
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
 
 template <int KIND>
-static int launch_point_kind(const PointArgs& pa, int opt_kind, cudaStream_t st, int* n_partials) {
+static int launch_point_kind(const PointArgs& pa, int opt_kind, cudaStream_t st, int* n_partials, int* variant) {
   switch (opt_kind) {
-    case ORX_OPT_SGD: return launch_point_kind_opt<KIND, ORX_OPT_SGD>(pa, st, n_partials);
-    case ORX_OPT_ADAGRAD: return launch_point_kind_opt<KIND, ORX_OPT_ADAGRAD>(pa, st, n_partials);
-    case ORX_OPT_ADAM_LAZY: return launch_point_kind_opt<KIND, ORX_OPT_ADAM_LAZY>(pa, st, n_partials);
-    case ORX_OPT_ADAM_DENSE: return launch_point_kind_opt<KIND, ORX_OPT_ADAM_DENSE>(pa, st, n_partials);
+    case ORX_OPT_SGD: return launch_point_kind_opt<KIND, ORX_OPT_SGD>(pa, st, n_partials, variant);
+    case ORX_OPT_ADAGRAD: return launch_point_kind_opt<KIND, ORX_OPT_ADAGRAD>(pa, st, n_partials, variant);
+    case ORX_OPT_ADAM_LAZY: return launch_point_kind_opt<KIND, ORX_OPT_ADAM_LAZY>(pa, st, n_partials, variant);
+    case ORX_OPT_ADAM_DENSE: return launch_point_kind_opt<KIND, ORX_OPT_ADAM_DENSE>(pa, st, n_partials, variant);
   }
   orx_set_error("unknown optimizer kind %d", opt_kind);
   return ORX_ERR_INVALID;
@@ -397,15 +402,16 @@ extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_
   const bool dense = opt->kind == ORX_OPT_ADAM_DENSE;
   if ((rc = orx_ensure_workspace(h, B, D, dense))) return rc;
   if ((rc = orx_ensure_partials(h, (B + 7) / 8 + 8, st))) return rc;
-  if ((rc = orx_launch_index_build(h, uid, user->rows, B, iid, nullptr, item->rows, B, dense, st))) return rc;
+  if ((rc = orx_launch_index_build(h, uid, user->rows, iid, nullptr, item->rows, B, dense, st))) return rc;
   PointArgs pa;
   fill_point_args(pa, h, kind, user, item, item_bias, w, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2);
   pa.opt = orx_opt_to_dev(opt);
   pa.gw = (kind == ORX_POINT_GMF) ? h->gw : nullptr;
-  int n_partials = 0;
-  rc = (kind == ORX_POINT_GMF) ? launch_point_kind<ORX_POINT_GMF>(pa, opt->kind, st, &n_partials)
-                               : launch_point_kind<ORX_POINT_WRMF>(pa, opt->kind, st, &n_partials);
+  int n_partials = 0, variant = 0;
+  rc = (kind == ORX_POINT_GMF) ? launch_point_kind<ORX_POINT_GMF>(pa, opt->kind, st, &n_partials, &variant)
+                               : launch_point_kind<ORX_POINT_WRMF>(pa, opt->kind, st, &n_partials, &variant);
   if (rc) return rc;
+  orx_log_dispatch(h, ORX_OP_POINTWISE_STEP, variant, kind, opt->kind, B, D, 0, 0);   // index set 0 always
   if (dense) {
     if ((rc = orx_launch_adam_sweep(h, user->var, user->s0, user->s1, user->rows, D, h->hu, h->gu, pa.opt, st))) return rc;
     if ((rc = orx_launch_adam_sweep(h, item->var, item->s0, item->s1, item->rows, D, h->hi, h->gi, pa.opt, st))) return rc;

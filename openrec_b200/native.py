@@ -8,19 +8,22 @@ from collections import namedtuple
 import torch
 
 from . import _lib
-from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE,
-                   ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR, ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF,
-                   ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_GEMM_TMA,
-                   ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, OrxOpt, OrxTable)
+from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP,
+                   ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR, ORX_PAIR_UCML,
+                   ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
+                   ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_STEP,
+                   ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE, OrxOpt, OrxTable)
 
 __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", "ORX_POINT_GMF", "ORX_POINT_WRMF",
            "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_SCORE_DOT",
-           "ORX_SCORE_NEG_SQDIST", "ORX_OP_GEMM", "ORX_OP_INTERACT_FWD", "ORX_OP_INTERACT_BWD", "ORX_VARIANT_GEMM_TMA",
-           "ORX_VARIANT_GEMM_SIMT", "ORX_VARIANT_INTERACT_WARP", "ORX_VARIANT_INTERACT", "Dispatch"]
+           "ORX_SCORE_NEG_SQDIST", "ORX_OP_GEMM", "ORX_OP_INTERACT_FWD", "ORX_OP_INTERACT_BWD", "ORX_OP_PAIRWISE_STEP",
+           "ORX_OP_POINTWISE_STEP", "ORX_VARIANT_GEMM_TMA", "ORX_VARIANT_GEMM_SIMT", "ORX_VARIANT_INTERACT_WARP",
+           "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC", "Dispatch"]
 
 _engines = {}
 
-# one record of orx_debug_dispatch_log: which kernel an orx_mlp_layer_* / orx_interact_* call launched
+# one record of orx_debug_dispatch_log: which kernel an orx_mlp_layer_* / orx_interact_* call or a sparse step launched
+# (the field meanings per op are in include/orx.h)
 Dispatch = namedtuple("Dispatch", "op variant ta tb m n k s")
 
 
@@ -135,7 +138,8 @@ class Engine:
         _lib.check(self.lib.orx_debug_set_epoch(self.h, epoch), "orx_debug_set_epoch")
 
     def debug_dispatch_log(self):
-        """-> [Dispatch] launched by this engine's DLRM calls since the last read (oldest first), and clears them."""
+        """-> [Dispatch] launched by this engine's DLRM calls and sparse steps since the last read (oldest first), and
+        clears them."""
         rec = (C.c_int32 * (8 * _lib.ORX_DISPATCH_LOG_CAP))()
         n = C.c_int32()
         _lib.check(self.lib.orx_debug_dispatch_log(self.h, rec, _lib.ORX_DISPATCH_LOG_CAP, C.byref(n)),

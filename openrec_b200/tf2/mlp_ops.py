@@ -40,7 +40,8 @@ class GemmProfile:
         call()
         e1.record()
         rec = eng.debug_dispatch_log()
-        pure = len(rec) == 1 and rec[0].variant == N.ORX_VARIANT_GEMM_TMA and rec[0].s == 1
+        pure = len(rec) == 1 and rec[0].op == N.ORX_OP_GEMM and rec[0].variant == N.ORX_VARIANT_GEMM_TMA \
+            and rec[0].s == 1
         self.ev.append((e0, e1, flops, pure))
 
     def totals(self, pure_only=False):
