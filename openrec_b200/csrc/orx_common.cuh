@@ -4,6 +4,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "../../include/orx.h"
 
 // ---------------------------------------------------------------------------------------
@@ -121,6 +123,23 @@ static inline int orx_current_sms() {
 
 int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim, bool full_staging);
 int orx_ensure_stage(orx_ctx* c, int64_t n_ints);
+
+// Runtime kind -> template argument: calls f(std::integral_constant<int, V>{}) for the V among Vs equal to v, and for the
+// last of Vs when none is (every entry point validates v, with its own error message, before it dispatches).  Only the
+// listed values are instantiated.
+template <int V, int... Vs, typename F>
+static inline auto orx_dispatch(int v, F&& f) {
+  if constexpr (sizeof...(Vs) == 0) {
+    return f(std::integral_constant<int, V>{});
+  } else {
+    if (v == V) return f(std::integral_constant<int, V>{});
+    return orx_dispatch<Vs...>(v, f);
+  }
+}
+template <typename F>
+static inline auto orx_dispatch_opt(int opt_kind, F&& f) {
+  return orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE>(opt_kind, f);
+}
 
 // ---------------------------------------------------------------------------------------
 // device helpers
@@ -299,6 +318,15 @@ __device__ __forceinline__ float orx_rcp_fast(float x) {
   return r;
 }
 
+// Which optimizer-slot rows an update reads and writes: S0 = Adagrad accumulator / Adam m, S1 = Adam v.  STAGE_ONLY:
+// ADAM_DENSE updates no row in a step kernel; every row is staged and the sweep (k_adam_sweep) applies Adam to the table.
+template <int OPT>
+struct OrxOptSlots {
+  static constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
+  static constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
+  static constexpr bool STAGE_ONLY = (OPT == ORX_OPT_ADAM_DENSE);
+};
+
 // One optimizer update of one scalar.  OPT is an orx_opt_kind (ADAM_DENSE never reaches here:
 // its rows are staged and swept).
 template <int OPT>
@@ -325,6 +353,100 @@ __device__ __forceinline__ float4 orx_apply4(float4 w, float4 g, float4& s0, flo
   return r;
 }
 
+// One float4 (elements off..off+3) of a sample's gradient for table row `id`: a row that only this sample references
+// (`own`) gets the optimizer in registers -- value w, the caller's slot registers s0 / s1 updated in place -- and row and
+// slots are written back with a 128-bit store (STREAM: evict-first, orx_st4_stream; else __stcg); any other row's
+// gradient is red.add'ed into its staging row d of G.  The addresses are formed inside each branch from the ids: taking
+// precomputed row pointers changes the register allocation of the step kernels.
+template <int OPT, bool STREAM>
+__device__ __forceinline__ void orx_own_or_stage4(bool own, float* W, float* P0, float* P1, int id, float* G, int d,
+                                                  int D, int off, float4 w, float4 g, float4& s0, float4& s1,
+                                                  const OrxOptDev& o) {
+  typedef OrxOptSlots<OPT> SL;
+  auto st = [](float* p, float4 v) {
+    if (STREAM) orx_st4_stream(p, v);
+    else __stcg(reinterpret_cast<float4*>(p), v);
+  };
+  if (!SL::STAGE_ONLY && own) {
+    const int64_t i = (int64_t)id * D + off;
+    st(W + i, orx_apply4<OPT>(w, g, s0, s1, o));
+    if (SL::S0) st(P0 + i, s0);
+    if (SL::S1) st(P1 + i, s1);
+  } else {
+    orx_red4(G + (int64_t)d * D + off, g);
+  }
+}
+
+// One element of a variable (*W, current value w) and of its optimizer slots (*P0, *P1; read only when OPT has them):
+// load the slots, apply the optimizer with gradient g, store value and slots.  (Sites that load with a cache operator
+// or hold the slots in registers call orx_apply.)
+template <int OPT>
+__device__ __forceinline__ void orx_update1(float* W, float* P0, float* P1, float w, float g, const OrxOptDev& o) {
+  typedef OrxOptSlots<OPT> SL;
+  float s0 = SL::S0 ? *P0 : 0.f, s1 = SL::S1 ? *P1 : 0.f;
+  *W = orx_apply<OPT>(w, g, s0, s1, o);
+  if (SL::S0) *P0 = s0;
+  if (SL::S1) *P1 = s1;
+}
+
+// Keras dense Adam (ADAM_DENSE) of element i, m = M, v = V: IEEE sqrtf and division, as the reference computes it.
+__device__ __forceinline__ void orx_adam_dense1(float* W, float* M, float* V, int64_t i, float g, const OrxOptDev& o) {
+  const float mm = o.beta1 * M[i] + (1.f - o.beta1) * g;
+  const float vv = o.beta2 * V[i] + (1.f - o.beta2) * g * g;
+  M[i] = mm;
+  V[i] = vv;
+  W[i] = W[i] - o.lr * mm / (sqrtf(vv) + o.eps);
+}
+
+// One (loss, l2) float partial per block of 8 warps at partials[2 * blockIdx.x], warps summed in a fixed order.
+__device__ __forceinline__ void orx_block_partial(float loss, float l2, float* partials) {
+  __shared__ float sred[8][2];
+  loss = orx_group_sum<32>(loss);
+  l2 = orx_group_sum<32>(l2);
+  if ((threadIdx.x & 31) == 0) {
+    sred[threadIdx.x >> 5][0] = loss;
+    sred[threadIdx.x >> 5][1] = l2;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float l = 0.f, q = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) {
+      l += sred[w][0];
+      q += sred[w][1];
+    }
+    partials[2 * blockIdx.x] = l;
+    partials[2 * blockIdx.x + 1] = q;
+  }
+}
+
+// Deterministic (loss, l2) totals of n float pairs (loss, l2) for one 256-thread block: each thread sums a fixed stride
+// in float64, adds the squares of sq[0..nsq) to its l2 share (GMF weight), then a fixed-order tree.  Every thread of the
+// block calls it and gets the totals in *l / *q.
+__device__ __forceinline__ void orx_block_sum_partials(const float* partials, int n, const float* sq, int nsq,
+                                                       double* l, double* q) {
+  __shared__ double sh[2][256];
+  double sl = 0.0, sq2 = 0.0;
+  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+    sl += (double)__ldcg(partials + 2 * i);
+    sq2 += (double)__ldcg(partials + 2 * i + 1);
+  }
+  if (sq)
+    for (int e = threadIdx.x; e < nsq; e += blockDim.x) sq2 += (double)sq[e] * (double)sq[e];
+  sh[0][threadIdx.x] = sl;
+  sh[1][threadIdx.x] = sq2;
+  __syncthreads();
+  for (int s = 128; s > 0; s >>= 1) {
+    if ((int)threadIdx.x < s) {
+      sh[0][threadIdx.x] += sh[0][threadIdx.x + s];
+      sh[1][threadIdx.x] += sh[1][threadIdx.x + s];
+    }
+    __syncthreads();
+  }
+  *l = sh[0][0];
+  *q = sh[1][0];
+}
+
 #endif  // __CUDACC__
 
 // Arguments of the shared tail kernel (staged rows -> optimizer, hash clear, loss reduction).
@@ -345,6 +467,75 @@ struct TailArgs {
   float *W, *Ws0, *Ws1, *gw;
   float c_l2;
 };
+
+#ifdef __CUDACC__
+// The staged rows of a step: the nu staged user rows (a.hu) and ni staged item rows (a.hi, with the item bias) get the
+// optimizer once each from their summed gradient, and the staging rows are zeroed (ADAM_DENSE: zeroed only, the sweep
+// has applied them).  Every thread of the grid calls it.
+// The tail is a chain of dependent round trips (counters -> row id -> rows) over a few thousand rows, i.e. latency,
+// not bandwidth.  A warp therefore takes FOUR staged rows at once, eight lanes per row (a quarter-warp still covers
+// 128 contiguous bytes per access), and issues all of a row's loads before the first use: 12 independent 128-bit
+// loads per lane in flight at D = 128.  Table and slot rows evict-first, staging rows (G) at normal priority: the
+// step's red.adds left them in L2.
+template <int OPT>
+__device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni) {
+  typedef OrxOptSlots<OPT> SL;
+  constexpr bool ZERO_ONLY = SL::STAGE_ONLY;
+  const int lane = threadIdx.x & 31;
+  const int gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  const int D = a.D;
+  const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  const int sub = lane >> 3, sl = lane & 7;
+  for (int r0 = gwarp * 4; r0 < nu + ni; r0 += nwarps * 4) {
+    const int r = r0 + sub;
+    const bool on = r < nu + ni;
+    const bool is_u = on && r < nu;
+    const int d = on ? (is_u ? r : r - nu) : 0;
+    const int id = on ? (is_u ? a.hu.did[d] : a.hi.did[d]) : 0;
+    float* G = (is_u ? a.gu : a.gi) + (int64_t)d * D;
+    float* W = (is_u ? a.U : a.I) + (int64_t)id * D;
+    float* P0 = (is_u ? a.Us0 : a.Is0) + (int64_t)id * D;
+    float* P1 = (is_u ? a.Us1 : a.Is1) + (int64_t)id * D;
+    if ((D & 3) == 0) {  // 128-bit path: float4 index sl + 8k
+      const int nq = D >> 2;
+      for (int e0 = 0; e0 < nq; e0 += 32) {
+        float4 g[4], w[4], s0v[4], s1v[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const int e = e0 + sl + 8 * k;
+          const bool ld = on && e < nq;
+          g[k] = ld ? __ldcg(reinterpret_cast<const float4*>(G) + e) : z4;
+          w[k] = (ld && !ZERO_ONLY) ? orx_ld4_stream(W + 4 * e) : z4;
+          s0v[k] = (ld && SL::S0) ? orx_ld4_stream(P0 + 4 * e) : z4;
+          s1v[k] = (ld && SL::S1) ? orx_ld4_stream(P1 + 4 * e) : z4;
+        }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const int e = e0 + sl + 8 * k;
+          if (!on || e >= nq) continue;
+          if (!ZERO_ONLY) {
+            orx_st4_stream(W + 4 * e, orx_apply4<OPT>(w[k], g[k], s0v[k], s1v[k], a.opt));
+            if (SL::S0) orx_st4_stream(P0 + 4 * e, s0v[k]);
+            if (SL::S1) orx_st4_stream(P1 + 4 * e, s1v[k]);
+          }
+          __stcg(reinterpret_cast<float4*>(G) + e, z4);
+        }
+      }
+    } else if (on) {
+      for (int e = sl; e < D; e += 8) {
+        if (!ZERO_ONLY) orx_update1<OPT>(W + e, P0 + e, P1 + e, W[e], G[e], a.opt);
+        G[e] = 0.f;
+      }
+    }
+    if (on && !is_u && sl == 0) {     // the item bias of the staged row
+      if (!ZERO_ONLY) orx_update1<OPT>(a.Bv + id, a.Bs0 + id, a.Bs1 + id, a.Bv[id], a.gb[d], a.opt);
+      a.gb[d] = 0.f;
+    }
+  }
+  // (the hash tables are not cleared: the next step uses a new epoch)
+}
+#endif  // __CUDACC__
 
 OrxOptDev orx_opt_to_dev(const orx_opt_t* o);
 int orx_launch_index_build_strided(orx_ctx* c, const int32_t* a, int64_t stride, int64_t rows, int32_t n,

@@ -151,12 +151,8 @@ template <int OPT>
 __global__ void k_dense_apply(float* var, float* s0, float* s1, const float* __restrict__ grad, int64_t n,
                               OrxOptDev o) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    float a = (OPT != ORX_OPT_SGD) ? s0[i] : 0.f, b = (OPT == ORX_OPT_ADAM_LAZY) ? s1[i] : 0.f;
-    var[i] = orx_apply<OPT>(var[i], grad[i], a, b, o);
-    if (OPT != ORX_OPT_SGD) s0[i] = a;
-    if (OPT == ORX_OPT_ADAM_LAZY) s1[i] = b;
-  }
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+    orx_update1<OPT>(var + i, s0 + i, s1 + i, var[i], grad[i], o);
 }
 
 extern "C" int orx_dense_apply(orx_handle_t h, float* var, float* s0, float* s1, const float* grad, int64_t n,
@@ -169,19 +165,17 @@ extern "C" int orx_dense_apply(orx_handle_t h, float* var, float* s0, float* s1,
   int64_t blocks = (n + 255) / 256;
   if (blocks > (int64_t)h->num_sms * 16) blocks = (int64_t)h->num_sms * 16;
   cudaStream_t st = (cudaStream_t)s;
-  switch (opt->kind) {
-    case ORX_OPT_SGD: k_dense_apply<ORX_OPT_SGD><<<(int)blocks, 256, 0, st>>>(var, s0, s1, grad, n, o); break;
-    case ORX_OPT_ADAGRAD:
-      ORX_REQUIRE(s0, "Adagrad needs s0");
-      k_dense_apply<ORX_OPT_ADAGRAD><<<(int)blocks, 256, 0, st>>>(var, s0, s1, grad, n, o);
-      break;
-    case ORX_OPT_ADAM_LAZY:
-    case ORX_OPT_ADAM_DENSE:  // identical on a dense variable
-      ORX_REQUIRE(s0 && s1, "Adam needs s0 and s1");
-      k_dense_apply<ORX_OPT_ADAM_LAZY><<<(int)blocks, 256, 0, st>>>(var, s0, s1, grad, n, o);
-      break;
-    default: orx_set_error("unknown optimizer kind %d", opt->kind); return ORX_ERR_INVALID;
+  if (opt->kind < ORX_OPT_SGD || opt->kind > ORX_OPT_ADAM_DENSE) {
+    orx_set_error("unknown optimizer kind %d", opt->kind);
+    return ORX_ERR_INVALID;
   }
+  if (opt->kind == ORX_OPT_ADAGRAD) ORX_REQUIRE(s0, "Adagrad needs s0");
+  if (opt->kind >= ORX_OPT_ADAM_LAZY) ORX_REQUIRE(s0 && s1, "Adam needs s0 and s1");
+  // ADAM_DENSE runs as ADAM_LAZY: identical on a dense variable
+  const int kind = opt->kind == ORX_OPT_ADAM_DENSE ? ORX_OPT_ADAM_LAZY : opt->kind;
+  orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY>(kind, [&](auto O) {
+    k_dense_apply<decltype(O)::value><<<(int)blocks, 256, 0, st>>>(var, s0, s1, grad, n, o);
+  });
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }

@@ -69,3 +69,19 @@ __device__ __forceinline__ void pair_row_grads(float g, float c2, float4 u, floa
   }
 }
 
+// The same for one element of the rows.
+template <int KIND>
+__device__ __forceinline__ void pair_grads1(float g, float c2, float u, float p, float n, float* gu, float* gp,
+                                            float* gn) {
+  if (KIND == ORX_PAIR_BPR) {
+    *gu = g * (p - n) + c2 * u;
+    *gp = g * u + c2 * p;
+    *gn = -g * u + c2 * n;
+  } else {
+    const float t = 2.f * g;
+    *gu = t * (n - p) + c2 * u;
+    *gp = t * (p - u) + c2 * p;
+    *gn = t * (u - n) + c2 * n;
+  }
+}
+

@@ -104,11 +104,9 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
   constexpr int G = (D / 4 < 32) ? D / 4 : 32;  // lanes per triplet
   constexpr int K = D / (4 * G);                // float4 per lane per row
   constexpr int TPW = 32 / G;                   // triplets in flight per warp
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool STAGE_ONLY = (OPT == ORX_OPT_ADAM_DENSE);
+  typedef OrxOptSlots<OPT> SL;
   static_assert(CH % TPW == 0, "chunk must be a multiple of the triplets per warp");
-  typedef TripRegs<K, S0, S1> Regs;
+  typedef TripRegs<K, SL::S0, SL::S1> Regs;
 
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -148,18 +146,18 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
   // ---- hash probes + item_bias (lanes < CH), overlapping the row loads above; L2 evict-last (orx_ld_keep)
   float bp = 0.f, bn = 0.f, bps0 = 0.f, bps1 = 0.f, bns0 = 0.f, bns1 = 0.f;
   if (flags & 1) {
-    const uint32_t cu = orx_hash_find<!STAGE_ONLY, true>(a.hu, u_id, &du);
-    const uint32_t cp = orx_hash_find<!STAGE_ONLY, true>(a.hi, p_id, &dp);
-    const uint32_t cn = orx_hash_find<!STAGE_ONLY, true>(a.hi, n_id, &dn);
+    const uint32_t cu = orx_hash_find<!SL::STAGE_ONLY, true>(a.hu, u_id, &du);
+    const uint32_t cp = orx_hash_find<!SL::STAGE_ONLY, true>(a.hi, p_id, &dp);
+    const uint32_t cn = orx_hash_find<!SL::STAGE_ONLY, true>(a.hi, n_id, &dn);
     bp = orx_ld_keep(a.Bv + p_id);
     bn = orx_ld_keep(a.Bv + n_id);
-    if (!STAGE_ONLY) {
+    if (!SL::STAGE_ONLY) {
       flags |= (cu == 1u ? 2 : 0) | (cp == 1u ? 4 : 0) | (cn == 1u ? 8 : 0);
-      if (S0) {
+      if (SL::S0) {
         if (flags & 4) bps0 = orx_ld_keep(a.Bs0 + p_id);
         if (flags & 8) bns0 = orx_ld_keep(a.Bs0 + n_id);
       }
-      if (S1) {
+      if (SL::S1) {
         if (flags & 4) bps1 = orx_ld_keep(a.Bs1 + p_id);
         if (flags & 8) bns1 = orx_ld_keep(a.Bs1 + n_id);
       }
@@ -178,12 +176,12 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
 #pragma unroll
     for (int k = 0; k < K; ++k) {
       const int off = (k * G + gl) * 4;
-      if (S0) {
+      if (SL::S0) {
         r.us0[k] = (r.fl & 2) ? orx_ld4_stream(a.Us0 + (int64_t)r.uu * D + off) : z4;
         r.ps0[k] = (r.fl & 4) ? orx_ld4_stream(a.Is0 + (int64_t)r.pp * D + off) : z4;
         r.ns0[k] = (r.fl & 8) ? orx_ld4_stream(a.Is0 + (int64_t)r.nn * D + off) : z4;
       }
-      if (S1) {
+      if (SL::S1) {
         r.us1[k] = (r.fl & 2) ? orx_ld4_stream(a.Us1 + (int64_t)r.uu * D + off) : z4;
         r.ps1[k] = (r.fl & 4) ? orx_ld4_stream(a.Is1 + (int64_t)r.pp * D + off) : z4;
         r.ns1[k] = (r.fl & 8) ? orx_ld4_stream(a.Is1 + (int64_t)r.nn * D + off) : z4;
@@ -229,30 +227,12 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
         const int off = (k * G + gl) * 4;
         float4 gu, gp, gn;
         pair_row_grads<KIND>(g, a.c_l2, r.u[k], r.p[k], r.n[k], &gu, &gp, &gn);
-        if (!STAGE_ONLY && (r.fl & 2)) {
-          const int64_t o = (int64_t)r.uu * D + off;
-          orx_st4_stream(a.U + o, orx_apply4<OPT>(r.u[k], gu, r.us0[k], r.us1[k], a.opt));
-          if (S0) orx_st4_stream(a.Us0 + o, r.us0[k]);
-          if (S1) orx_st4_stream(a.Us1 + o, r.us1[k]);
-        } else {
-          orx_red4(a.gu + (int64_t)r.du * D + off, gu);
-        }
-        if (!STAGE_ONLY && (r.fl & 4)) {
-          const int64_t o = (int64_t)r.pp * D + off;
-          orx_st4_stream(a.I + o, orx_apply4<OPT>(r.p[k], gp, r.ps0[k], r.ps1[k], a.opt));
-          if (S0) orx_st4_stream(a.Is0 + o, r.ps0[k]);
-          if (S1) orx_st4_stream(a.Is1 + o, r.ps1[k]);
-        } else {
-          orx_red4(a.gi + (int64_t)r.dp * D + off, gp);
-        }
-        if (!STAGE_ONLY && (r.fl & 8)) {
-          const int64_t o = (int64_t)r.nn * D + off;
-          orx_st4_stream(a.I + o, orx_apply4<OPT>(r.n[k], gn, r.ns0[k], r.ns1[k], a.opt));
-          if (S0) orx_st4_stream(a.Is0 + o, r.ns0[k]);
-          if (S1) orx_st4_stream(a.Is1 + o, r.ns1[k]);
-        } else {
-          orx_red4(a.gi + (int64_t)r.dn * D + off, gn);
-        }
+        orx_own_or_stage4<OPT, true>(r.fl & 2, a.U, a.Us0, a.Us1, r.uu, a.gu, r.du, D, off, r.u[k], gu, r.us0[k],
+                                     r.us1[k], a.opt);
+        orx_own_or_stage4<OPT, true>(r.fl & 4, a.I, a.Is0, a.Is1, r.pp, a.gi, r.dp, D, off, r.p[k], gp, r.ps0[k],
+                                     r.ps1[k], a.opt);
+        orx_own_or_stage4<OPT, true>(r.fl & 8, a.I, a.Is0, a.Is1, r.nn, a.gi, r.dn, D, off, r.n[k], gn, r.ns0[k],
+                                     r.ns1[k], a.opt);
       }
     }
   };
@@ -289,15 +269,15 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
   if (flags & 1) {
     if (flags & 4) {
       __stcg(a.Bv + p_id, orx_apply<OPT>(bp, g_own, bps0, bps1, a.opt));
-      if (S0) __stcg(a.Bs0 + p_id, bps0);
-      if (S1) __stcg(a.Bs1 + p_id, bps1);
+      if (SL::S0) __stcg(a.Bs0 + p_id, bps0);
+      if (SL::S1) __stcg(a.Bs1 + p_id, bps1);
     } else {
       atomicAdd(a.gb + dp, g_own);
     }
     if (flags & 8) {
       __stcg(a.Bv + n_id, orx_apply<OPT>(bn, -g_own, bns0, bns1, a.opt));
-      if (S0) __stcg(a.Bs0 + n_id, bns0);
-      if (S1) __stcg(a.Bs1 + n_id, bns1);
+      if (SL::S0) __stcg(a.Bs0 + n_id, bns0);
+      if (SL::S1) __stcg(a.Bs1 + n_id, bns1);
     } else {
       atomicAdd(a.gb + dn, -g_own);
     }
@@ -307,32 +287,13 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
   }
 
   // ---- one (loss, l2) partial per block, fixed order => deterministic
-  __shared__ float sred[8][2];
-  loss_acc = orx_group_sum<32>(loss_acc);
-  l2_acc = orx_group_sum<32>(l2_acc);
-  if (lane == 0) {
-    sred[threadIdx.x >> 5][0] = loss_acc;
-    sred[threadIdx.x >> 5][1] = l2_acc;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float l = 0.f, q = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) {
-      l += sred[w][0];
-      q += sred[w][1];
-    }
-    a.partials[2 * blockIdx.x] = l;
-    a.partials[2 * blockIdx.x + 1] = q;
-  }
+  orx_block_partial(loss_acc, l2_acc, a.partials);
 }
 
 // Any dim (e.g. the example's D=50): one triplet per warp-iteration, lanes stride the row.
 template <int KIND, int OPT>
 __global__ void __launch_bounds__(256) k_pair_step_generic(const PairArgs a) {
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool STAGE_ONLY = (OPT == ORX_OPT_ADAM_DENSE);
+  constexpr bool STAGE_ONLY = OrxOptSlots<OPT>::STAGE_ONLY;
   constexpr int CH = 8;
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -375,92 +336,28 @@ __global__ void __launch_bounds__(256) k_pair_step_generic(const PairArgs a) {
     float lt, g;
     pair_score<KIND>(s1, s2, bp, bn, a, &lt, &g);
     if (lane == 0) loss_acc += lt;
-    const float t2 = 2.f * g, c2 = a.c_l2;
     for (int d = lane; d < D; d += 32) {
       const float u = ur[d], p = pr[d], n = nr[d];
       float gu, gp, gn;
-      if (KIND == ORX_PAIR_BPR) {
-        gu = g * (p - n) + c2 * u;
-        gp = g * u + c2 * p;
-        gn = -g * u + c2 * n;
-      } else {
-        gu = t2 * (n - p) + c2 * u;
-        gp = t2 * (p - u) + c2 * p;
-        gn = t2 * (u - n) + c2 * n;
-      }
-      float s0v = 0.f, s1v = 0.f;
-      if (fu) {
-        const int64_t o = (int64_t)uu * D + d;
-        if (S0) s0v = a.Us0[o];
-        if (S1) s1v = a.Us1[o];
-        ur[d] = orx_apply<OPT>(u, gu, s0v, s1v, a.opt);
-        if (S0) a.Us0[o] = s0v;
-        if (S1) a.Us1[o] = s1v;
-      } else {
-        atomicAdd(a.gu + (int64_t)du * D + d, gu);
-      }
-      if (fp) {
-        const int64_t o = (int64_t)pp * D + d;
-        if (S0) s0v = a.Is0[o];
-        if (S1) s1v = a.Is1[o];
-        pr[d] = orx_apply<OPT>(p, gp, s0v, s1v, a.opt);
-        if (S0) a.Is0[o] = s0v;
-        if (S1) a.Is1[o] = s1v;
-      } else {
-        atomicAdd(a.gi + (int64_t)dp * D + d, gp);
-      }
-      if (fn) {
-        const int64_t o = (int64_t)nn * D + d;
-        if (S0) s0v = a.Is0[o];
-        if (S1) s1v = a.Is1[o];
-        nr[d] = orx_apply<OPT>(n, gn, s0v, s1v, a.opt);
-        if (S0) a.Is0[o] = s0v;
-        if (S1) a.Is1[o] = s1v;
-      } else {
-        atomicAdd(a.gi + (int64_t)dn * D + d, gn);
-      }
+      pair_grads1<KIND>(g, a.c_l2, u, p, n, &gu, &gp, &gn);
+      const int64_t ou = (int64_t)uu * D + d, op = (int64_t)pp * D + d, on = (int64_t)nn * D + d;
+      if (fu) orx_update1<OPT>(ur + d, a.Us0 + ou, a.Us1 + ou, u, gu, a.opt);
+      else atomicAdd(a.gu + (int64_t)du * D + d, gu);
+      if (fp) orx_update1<OPT>(pr + d, a.Is0 + op, a.Is1 + op, p, gp, a.opt);
+      else atomicAdd(a.gi + (int64_t)dp * D + d, gp);
+      if (fn) orx_update1<OPT>(nr + d, a.Is0 + on, a.Is1 + on, n, gn, a.opt);
+      else atomicAdd(a.gi + (int64_t)dn * D + d, gn);
     }
     if (lane == 0) {
       const float gbias = (KIND == ORX_PAIR_BPR) ? g : -g;
-      float s0v = 0.f, s1v = 0.f;
-      if (fp) {
-        if (S0) s0v = a.Bs0[pp];
-        if (S1) s1v = a.Bs1[pp];
-        a.Bv[pp] = orx_apply<OPT>(bp, gbias, s0v, s1v, a.opt);
-        if (S0) a.Bs0[pp] = s0v;
-        if (S1) a.Bs1[pp] = s1v;
-      } else {
-        atomicAdd(a.gb + dp, gbias);
-      }
-      if (fn) {
-        if (S0) s0v = a.Bs0[nn];
-        if (S1) s1v = a.Bs1[nn];
-        a.Bv[nn] = orx_apply<OPT>(bn, -gbias, s0v, s1v, a.opt);
-        if (S0) a.Bs0[nn] = s0v;
-        if (S1) a.Bs1[nn] = s1v;
-      } else {
-        atomicAdd(a.gb + dn, -gbias);
-      }
+      if (fp) orx_update1<OPT>(a.Bv + pp, a.Bs0 + pp, a.Bs1 + pp, bp, gbias, a.opt);
+      else atomicAdd(a.gb + dp, gbias);
+      if (fn) orx_update1<OPT>(a.Bv + nn, a.Bs0 + nn, a.Bs1 + nn, bn, -gbias, a.opt);
+      else atomicAdd(a.gb + dn, -gbias);
       if (a.g_out) a.g_out[t] = g;
     }
   }
-  __shared__ float sred[8][2];
-  loss_acc = orx_group_sum<32>(loss_acc);
-  l2_acc = orx_group_sum<32>(l2_acc);
-  if (lane == 0) {
-    sred[threadIdx.x >> 5][0] = loss_acc;
-    sred[threadIdx.x >> 5][1] = l2_acc;
-  }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float l = 0.f, q = 0.f;
-    for (int w = 0; w < 8; ++w) {
-      l += sred[w][0];
-      q += sred[w][1];
-    }
-    a.partials[2 * blockIdx.x] = l;
-    a.partials[2 * blockIdx.x + 1] = q;
-  }
+  orx_block_partial(loss_acc, l2_acc, a.partials);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -477,15 +374,8 @@ __global__ void __launch_bounds__(256) k_adam_sweep(float* var, float* m, float*
     if (lane == 0) c = orx_hash_find(h, (int32_t)r, &d);
     c = __shfl_sync(ORX_FULL, c, 0);
     d = __shfl_sync(ORX_FULL, d, 0);
-    for (int e = lane; e < D; e += 32) {
-      const int64_t off = r * D + e;
-      const float g = c ? gstage[(int64_t)d * D + e] : 0.f;
-      const float mm = o.beta1 * m[off] + (1.f - o.beta1) * g;
-      const float vv = o.beta2 * v[off] + (1.f - o.beta2) * g * g;
-      m[off] = mm;
-      v[off] = vv;
-      var[off] = var[off] - o.lr * mm / (sqrtf(vv) + o.eps);
-    }
+    for (int e = lane; e < D; e += 32)
+      orx_adam_dense1(var, m, v, r * D + e, c ? gstage[(int64_t)d * D + e] : 0.f, o);
   }
 }
 
@@ -493,125 +383,30 @@ __global__ void __launch_bounds__(256) k_adam_sweep(float* var, float* m, float*
 // tail: staged rows -> optimizer (once per unique row), zero staging, clear hash, reduce loss
 // ---------------------------------------------------------------------------------------
 
+// ta.I == nullptr: no item side (orx_sparse_apply: one table, in the user-side index set); ta.out4 == nullptr: no loss.
 template <int OPT>
 __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool ZERO_ONLY = (OPT == ORX_OPT_ADAM_DENSE);
-  const int lane = threadIdx.x & 31;
-  const int gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  orx_pdl_wait();
-  const int nu = a.counters[0], ni = a.counters[1], nbad = a.counters[3];
-  const int D = a.D;
-  const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-  // The tail is a chain of dependent round trips (counters -> row id -> rows) over a few thousand rows, i.e. latency,
-  // not bandwidth.  A warp therefore takes FOUR staged rows at once, eight lanes per row (a quarter-warp still covers
-  // 128 contiguous bytes per access), and issues all of a row's loads before the first use: 12 independent 128-bit
-  // loads per lane in flight at D = 128.  Table and slot rows evict-first, staging rows (G) at normal priority: the
-  // step's red.adds left them in L2.
-  const int sub = lane >> 3, sl = lane & 7;
-  for (int r0 = gwarp * 4; r0 < nu + ni; r0 += nwarps * 4) {
-    const int r = r0 + sub;
-    const bool on = r < nu + ni;
-    const bool is_u = on && r < nu;
-    const int d = on ? (is_u ? r : r - nu) : 0;
-    const int id = on ? (is_u ? a.hu.did[d] : a.hi.did[d]) : 0;
-    float* G = (is_u ? a.gu : a.gi) + (int64_t)d * D;
-    float* W = (is_u ? a.U : a.I) + (int64_t)id * D;
-    float* P0 = (is_u ? a.Us0 : a.Is0) + (int64_t)id * D;
-    float* P1 = (is_u ? a.Us1 : a.Is1) + (int64_t)id * D;
-    if ((D & 3) == 0) {  // 128-bit path: float4 index sl + 8k
-      const int nq = D >> 2;
-      for (int e0 = 0; e0 < nq; e0 += 32) {
-        float4 g[4], w[4], s0v[4], s1v[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int e = e0 + sl + 8 * k;
-          const bool ld = on && e < nq;
-          g[k] = ld ? __ldcg(reinterpret_cast<const float4*>(G) + e) : z4;
-          w[k] = (ld && !ZERO_ONLY) ? orx_ld4_stream(W + 4 * e) : z4;
-          s0v[k] = (ld && S0 && !ZERO_ONLY) ? orx_ld4_stream(P0 + 4 * e) : z4;
-          s1v[k] = (ld && S1 && !ZERO_ONLY) ? orx_ld4_stream(P1 + 4 * e) : z4;
-        }
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int e = e0 + sl + 8 * k;
-          if (!on || e >= nq) continue;
-          if (!ZERO_ONLY) {
-            orx_st4_stream(W + 4 * e, orx_apply4<OPT>(w[k], g[k], s0v[k], s1v[k], a.opt));
-            if (S0) orx_st4_stream(P0 + 4 * e, s0v[k]);
-            if (S1) orx_st4_stream(P1 + 4 * e, s1v[k]);
-          }
-          __stcg(reinterpret_cast<float4*>(G) + e, z4);
-        }
-      }
-    } else if (on) {
-      for (int e = sl; e < D; e += 8) {
-        if (!ZERO_ONLY) {
-          float s0v = S0 ? P0[e] : 0.f, s1v = S1 ? P1[e] : 0.f;
-          W[e] = orx_apply<OPT>(W[e], G[e], s0v, s1v, a.opt);
-          if (S0) P0[e] = s0v;
-          if (S1) P1[e] = s1v;
-        }
-        G[e] = 0.f;
-      }
-    }
-    if (on && !is_u && sl == 0) {     // the item bias of the staged row
-      if (!ZERO_ONLY) {
-        float s0v = S0 ? a.Bs0[id] : 0.f, s1v = S1 ? a.Bs1[id] : 0.f;
-        a.Bv[id] = orx_apply<OPT>(a.Bv[id], a.gb[d], s0v, s1v, a.opt);
-        if (S0) a.Bs0[id] = s0v;
-        if (S1) a.Bs1[id] = s1v;
-      }
-      a.gb[d] = 0.f;
-    }
-  }
-  // (the hash tables are not cleared: the next step uses a new epoch)
-
-  __shared__ double sh[2][256];
   __shared__ bool last;
-  if (blockIdx.x == 0) {
-    // deterministic loss reduction (fixed order, double accumulation)
-    double l = 0.0, q = 0.0;
-    for (int i = threadIdx.x; i < a.n_partials; i += blockDim.x) {
-      l += (double)a.partials[2 * i];
-      q += (double)a.partials[2 * i + 1];
-    }
-    if (a.W)  // GMF: l2_loss also holds 0.5*sum(w^2) of the PRE-step weight (gmf.py:31-32)
-      for (int e = threadIdx.x; e < D; e += blockDim.x) q += (double)a.W[e] * (double)a.W[e];
-    sh[0][threadIdx.x] = l;
-    sh[1][threadIdx.x] = q;
-    __syncthreads();
-    for (int s = 128; s > 0; s >>= 1) {
-      if (threadIdx.x < s) {
-        sh[0][threadIdx.x] += sh[0][threadIdx.x + s];
-        sh[1][threadIdx.x] += sh[1][threadIdx.x + s];
-      }
-      __syncthreads();
-    }
+  orx_pdl_wait();
+  const int nu = *a.hu.counter, ni = a.I ? *a.hi.counter : 0;
+  orx_tail_rows<OPT>(a, nu, ni);
+
+  if (blockIdx.x == 0 && a.out4) {
+    // deterministic loss reduction; GMF: l2_loss also holds 0.5*sum(w^2) of the PRE-step weight (gmf.py:31-32)
+    double l, q;
+    orx_block_sum_partials(a.partials, a.n_partials, a.W, a.W ? a.D : 0, &l, &q);
     if (threadIdx.x == 0) {
-      a.out4[0] = (float)(sh[0][0] * (double)a.loss_scale);
-      a.out4[1] = (float)(0.5 * sh[1][0]);
-      a.out4[2] = (float)nbad;
+      a.out4[0] = (float)(l * (double)a.loss_scale);
+      a.out4[1] = (float)(0.5 * q);
+      a.out4[2] = (float)a.counters[3];
       a.out4[3] = (float)(nu + ni);
     }
     // GMF dense weight: grad = gw + c_l2*w  (gmf.py:31-32), Keras dense apply
     if (a.W) {
-      for (int e = threadIdx.x; e < D; e += blockDim.x) {
+      for (int e = threadIdx.x; e < a.D; e += blockDim.x) {
         const float g = a.gw[e] + a.c_l2 * a.W[e];
-        if (ZERO_ONLY) {  // ADAM_DENSE: dense Adam
-          const float mm = a.opt.beta1 * a.Ws0[e] + (1.f - a.opt.beta1) * g;
-          const float vv = a.opt.beta2 * a.Ws1[e] + (1.f - a.opt.beta2) * g * g;
-          a.Ws0[e] = mm;
-          a.Ws1[e] = vv;
-          a.W[e] = a.W[e] - a.opt.lr * mm / (sqrtf(vv) + a.opt.eps);
-        } else {
-          float s0v = S0 ? a.Ws0[e] : 0.f, s1v = S1 ? a.Ws1[e] : 0.f;
-          a.W[e] = orx_apply<OPT>(a.W[e], g, s0v, s1v, a.opt);
-          if (S0) a.Ws0[e] = s0v;
-          if (S1) a.Ws1[e] = s1v;
-        }
+        if (OrxOptSlots<OPT>::STAGE_ONLY) orx_adam_dense1(a.W, a.Ws0, a.Ws1, e, g, a.opt);
+        else orx_update1<OPT>(a.W + e, a.Ws0 + e, a.Ws1 + e, a.W[e], g, a.opt);
         a.gw[e] = 0.f;
       }
     }
@@ -629,12 +424,9 @@ __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
 
 int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st) {
   const int grid = c->num_sms * 4;  // ~1-2 staged rows per warp: the tail is a latency chain, not bandwidth
-  switch (opt_kind) {
-    case ORX_OPT_SGD: orx_launch_pdl(k_sparse_tail<ORX_OPT_SGD>, dim3(grid), dim3(256), 0, st, ta); break;
-    case ORX_OPT_ADAGRAD: orx_launch_pdl(k_sparse_tail<ORX_OPT_ADAGRAD>, dim3(grid), dim3(256), 0, st, ta); break;
-    case ORX_OPT_ADAM_LAZY: orx_launch_pdl(k_sparse_tail<ORX_OPT_ADAM_LAZY>, dim3(grid), dim3(256), 0, st, ta); break;
-    default: orx_launch_pdl(k_sparse_tail<ORX_OPT_ADAM_DENSE>, dim3(grid), dim3(256), 0, st, ta); break;
-  }
+  orx_dispatch_opt(opt_kind, [&](auto O) {
+    orx_launch_pdl(k_sparse_tail<decltype(O)::value>, dim3(grid), dim3(256), 0, st, ta);
+  });
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
@@ -684,20 +476,6 @@ static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, int* n
   }
   ORX_LAUNCH_CHECK();
   return ORX_OK;
-}
-
-template <int KIND>
-static int launch_pair_step_kind(const PairArgs& pa, int opt_kind, cudaStream_t st, int* n_partials, int* variant,
-                                 int* minb) {
-  switch (opt_kind) {
-    case ORX_OPT_SGD: return launch_pair_step_kind_opt<KIND, ORX_OPT_SGD>(pa, st, n_partials, variant, minb);
-    case ORX_OPT_ADAGRAD: return launch_pair_step_kind_opt<KIND, ORX_OPT_ADAGRAD>(pa, st, n_partials, variant, minb);
-    case ORX_OPT_ADAM_LAZY: return launch_pair_step_kind_opt<KIND, ORX_OPT_ADAM_LAZY>(pa, st, n_partials, variant, minb);
-    case ORX_OPT_ADAM_DENSE:
-      return launch_pair_step_kind_opt<KIND, ORX_OPT_ADAM_DENSE>(pa, st, n_partials, variant, minb);
-  }
-  orx_set_error("unknown optimizer kind %d", opt_kind);
-  return ORX_ERR_INVALID;
 }
 
 static int check_tables(const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias, int opt_kind) {
@@ -825,8 +603,11 @@ static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, con
   orx_prof_mark(c, 1, st);
   pa.hu = HU; pa.hi = HI;
   int n_partials = 0, variant = 0, minb = 0;
-  rc = (kind == ORX_PAIR_BPR) ? launch_pair_step_kind<ORX_PAIR_BPR>(pa, opt->kind, st, &n_partials, &variant, &minb)
-                              : launch_pair_step_kind<ORX_PAIR_UCML>(pa, opt->kind, st, &n_partials, &variant, &minb);
+  rc = orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {
+    return orx_dispatch_opt(opt->kind, [&](auto O) {
+      return launch_pair_step_kind_opt<decltype(K)::value, decltype(O)::value>(pa, st, &n_partials, &variant, &minb);
+    });
+  });
   if (rc) return rc;
   orx_log_dispatch(c, ORX_OP_PAIRWISE_STEP, variant, kind, opt->kind, B, D, minb, set);
   orx_prof_mark(c, 2, st);
@@ -958,22 +739,10 @@ __global__ void __launch_bounds__(256) k_pair_fwd_grad(const PairGradArgs a) {
     s2 = orx_group_sum<32>(s2);
     if (ok) pair_score<KIND>(s1, s2, bp, bn, sa, &lt, &g);
     if (lane == 0) loss_acc += lt;
-    const float t2 = 2.f * g, c2 = a.c_l2;
     if (a.d_user || a.d_pos || a.d_neg) {
       for (int d = lane; d < D; d += 32) {
         float gu = 0.f, gp = 0.f, gn = 0.f;
-        if (ok) {
-          const float u = ur[d], p = pr[d], n = nr[d];
-          if (KIND == ORX_PAIR_BPR) {
-            gu = g * (p - n) + c2 * u;
-            gp = g * u + c2 * p;
-            gn = -g * u + c2 * n;
-          } else {
-            gu = t2 * (n - p) + c2 * u;
-            gp = t2 * (p - u) + c2 * p;
-            gn = t2 * (u - n) + c2 * n;
-          }
-        }
+        if (ok) pair_grads1<KIND>(g, a.c_l2, ur[d], pr[d], nr[d], &gu, &gp, &gn);
         if (a.slots) {
           if (ok) {
             a.d_user[(int64_t)uu * ld + d] = gu;
@@ -1019,25 +788,11 @@ __global__ void __launch_bounds__(256) k_pair_fwd_grad(const PairGradArgs a) {
 }
 
 __global__ void k_reduce_partials(const float* partials, int n, float loss_scale, float* out4) {
-  __shared__ double sh[2][256];
-  double l = 0.0, q = 0.0;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
-    l += (double)partials[2 * i];
-    q += (double)partials[2 * i + 1];
-  }
-  sh[0][threadIdx.x] = l;
-  sh[1][threadIdx.x] = q;
-  __syncthreads();
-  for (int s = 128; s > 0; s >>= 1) {
-    if (threadIdx.x < s) {
-      sh[0][threadIdx.x] += sh[0][threadIdx.x + s];
-      sh[1][threadIdx.x] += sh[1][threadIdx.x + s];
-    }
-    __syncthreads();
-  }
+  double l, q;
+  orx_block_sum_partials(partials, n, nullptr, 0, &l, &q);
   if (threadIdx.x == 0) {
-    out4[0] = (float)(sh[0][0] * (double)loss_scale);
-    out4[1] = (float)(0.5 * sh[1][0]);
+    out4[0] = (float)(l * (double)loss_scale);
+    out4[1] = (float)(0.5 * q);
     out4[2] = 0.f;
     out4[3] = 0.f;
   }

@@ -54,9 +54,7 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
   constexpr int G = (D / 4 < 32) ? D / 4 : 32;
   constexpr int K = D / (4 * G);
   constexpr int TPW = 32 / G;
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool STAGE_ONLY = (OPT == ORX_OPT_ADAM_DENSE);
+  typedef OrxOptSlots<OPT> SL;
   constexpr bool GMF = (KIND == ORX_POINT_GMF);
   __shared__ float sgw[GMF ? D : 1];
 
@@ -80,10 +78,10 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
       const uint32_t ci = orx_hash_find(a.hi, i_id, &di);
       bi = __ldcg(a.Bv + i_id);
       flags = 1;
-      if (!STAGE_ONLY) {
+      if (!SL::STAGE_ONLY) {
         flags |= (cu == 1u ? 2 : 0) | (ci == 1u ? 4 : 0);
-        if (S0 && (flags & 4)) bs0 = __ldcg(a.Bs0 + i_id);
-        if (S1 && (flags & 4)) bs1 = __ldcg(a.Bs1 + i_id);
+        if (SL::S0 && (flags & 4)) bs0 = __ldcg(a.Bs0 + i_id);
+        if (SL::S1 && (flags & 4)) bs1 = __ldcg(a.Bs1 + i_id);
       }
     }
   }
@@ -111,11 +109,11 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
       const int off = (k * G + gl) * 4;
       u[k] = v ? __ldcg(reinterpret_cast<const float4*>(a.U + (int64_t)uu * D + off)) : z4;
       it[k] = v ? __ldcg(reinterpret_cast<const float4*>(a.I + (int64_t)ii * D + off)) : z4;
-      if (S0) {
+      if (SL::S0) {
         us0[k] = (fl & 2) ? __ldcg(reinterpret_cast<const float4*>(a.Us0 + (int64_t)uu * D + off)) : z4;
         is0[k] = (fl & 4) ? __ldcg(reinterpret_cast<const float4*>(a.Is0 + (int64_t)ii * D + off)) : z4;
       }
-      if (S1) {
+      if (SL::S1) {
         us1[k] = (fl & 2) ? __ldcg(reinterpret_cast<const float4*>(a.Us1 + (int64_t)uu * D + off)) : z4;
         is1[k] = (fl & 4) ? __ldcg(reinterpret_cast<const float4*>(a.Is1 + (int64_t)ii * D + off)) : z4;
       }
@@ -149,30 +147,16 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
           gwacc[k].x += g * u[k].x * it[k].x; gwacc[k].y += g * u[k].y * it[k].y;
           gwacc[k].z += g * u[k].z * it[k].z; gwacc[k].w += g * u[k].w * it[k].w;
         }
-        if (!STAGE_ONLY && (fl & 2)) {
-          const int64_t o = (int64_t)uu * D + off;
-          __stcg(reinterpret_cast<float4*>(a.U + o), orx_apply4<OPT>(u[k], gu, us0[k], us1[k], a.opt));
-          if (S0) __stcg(reinterpret_cast<float4*>(a.Us0 + o), us0[k]);
-          if (S1) __stcg(reinterpret_cast<float4*>(a.Us1 + o), us1[k]);
-        } else {
-          orx_red4(a.gu + (int64_t)duj * D + off, gu);
-        }
-        if (!STAGE_ONLY && (fl & 4)) {
-          const int64_t o = (int64_t)ii * D + off;
-          __stcg(reinterpret_cast<float4*>(a.I + o), orx_apply4<OPT>(it[k], gi, is0[k], is1[k], a.opt));
-          if (S0) __stcg(reinterpret_cast<float4*>(a.Is0 + o), is0[k]);
-          if (S1) __stcg(reinterpret_cast<float4*>(a.Is1 + o), is1[k]);
-        } else {
-          orx_red4(a.gi + (int64_t)dij * D + off, gi);
-        }
+        orx_own_or_stage4<OPT, false>(fl & 2, a.U, a.Us0, a.Us1, uu, a.gu, duj, D, off, u[k], gu, us0[k], us1[k], a.opt);
+        orx_own_or_stage4<OPT, false>(fl & 4, a.I, a.Is0, a.Is1, ii, a.gi, dij, D, off, it[k], gi, is0[k], is1[k], a.opt);
       }
     }
   }
   if (flags & 1) {
     if (flags & 4) {
       __stcg(a.Bv + i_id, orx_apply<OPT>(bi, g_own, bs0, bs1, a.opt));
-      if (S0) __stcg(a.Bs0 + i_id, bs0);
-      if (S1) __stcg(a.Bs1 + i_id, bs1);
+      if (SL::S0) __stcg(a.Bs0 + i_id, bs0);
+      if (SL::S1) __stcg(a.Bs1 + i_id, bs1);
     } else {
       atomicAdd(a.gb + di, g_own);
     }
@@ -200,9 +184,7 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
 // Any dim; MODE 0 = fused step, 1 = forward / explicit (un-fused) gradients.
 template <int KIND, int OPT, int MODE>
 __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool STAGE_ONLY = (OPT == ORX_OPT_ADAM_DENSE);
+  constexpr bool STAGE_ONLY = OrxOptSlots<OPT>::STAGE_ONLY;
   constexpr bool GMF = (KIND == ORX_POINT_GMF);
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -247,27 +229,11 @@ __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
           gi = g * w * u + c2 * it;
           if (GMF && a.gw) atomicAdd(a.gw + d, g * u * it);
           if (MODE == 0) {
-            float s0v = 0.f, s1v = 0.f;
-            if (fu) {
-              const int64_t o = (int64_t)uu * D + d;
-              if (S0) s0v = a.Us0[o];
-              if (S1) s1v = a.Us1[o];
-              ur[d] = orx_apply<OPT>(u, gu, s0v, s1v, a.opt);
-              if (S0) a.Us0[o] = s0v;
-              if (S1) a.Us1[o] = s1v;
-            } else {
-              atomicAdd(a.gu + (int64_t)du * D + d, gu);
-            }
-            if (fi) {
-              const int64_t o = (int64_t)ii * D + d;
-              if (S0) s0v = a.Is0[o];
-              if (S1) s1v = a.Is1[o];
-              ir[d] = orx_apply<OPT>(it, gi, s0v, s1v, a.opt);
-              if (S0) a.Is0[o] = s0v;
-              if (S1) a.Is1[o] = s1v;
-            } else {
-              atomicAdd(a.gi + (int64_t)di * D + d, gi);
-            }
+            const int64_t ou = (int64_t)uu * D + d, oi = (int64_t)ii * D + d;
+            if (fu) orx_update1<OPT>(ur + d, a.Us0 + ou, a.Us1 + ou, u, gu, a.opt);
+            else atomicAdd(a.gu + (int64_t)du * D + d, gu);
+            if (fi) orx_update1<OPT>(ir + d, a.Is0 + oi, a.Is1 + oi, it, gi, a.opt);
+            else atomicAdd(a.gi + (int64_t)di * D + d, gi);
           }
         }
         if (MODE == 1) {
@@ -279,16 +245,8 @@ __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
     }
     if (lane == 0) {
       if (MODE == 0 && ok) {
-        float s0v = 0.f, s1v = 0.f;
-        if (fi) {
-          if (S0) s0v = a.Bs0[ii];
-          if (S1) s1v = a.Bs1[ii];
-          a.Bv[ii] = orx_apply<OPT>(bi, g, s0v, s1v, a.opt);
-          if (S0) a.Bs0[ii] = s0v;
-          if (S1) a.Bs1[ii] = s1v;
-        } else {
-          atomicAdd(a.gb + di, g);
-        }
+        if (fi) orx_update1<OPT>(a.Bv + ii, a.Bs0 + ii, a.Bs1 + ii, bi, g, a.opt);
+        else atomicAdd(a.gb + di, g);
       }
       if (MODE == 1) {
         if (a.d_bias) a.d_bias[t] = g;
@@ -339,18 +297,6 @@ static int launch_point_kind_opt(const PointArgs& pa, cudaStream_t st, int* n_pa
   }
   ORX_LAUNCH_CHECK();
   return ORX_OK;
-}
-
-template <int KIND>
-static int launch_point_kind(const PointArgs& pa, int opt_kind, cudaStream_t st, int* n_partials, int* variant) {
-  switch (opt_kind) {
-    case ORX_OPT_SGD: return launch_point_kind_opt<KIND, ORX_OPT_SGD>(pa, st, n_partials, variant);
-    case ORX_OPT_ADAGRAD: return launch_point_kind_opt<KIND, ORX_OPT_ADAGRAD>(pa, st, n_partials, variant);
-    case ORX_OPT_ADAM_LAZY: return launch_point_kind_opt<KIND, ORX_OPT_ADAM_LAZY>(pa, st, n_partials, variant);
-    case ORX_OPT_ADAM_DENSE: return launch_point_kind_opt<KIND, ORX_OPT_ADAM_DENSE>(pa, st, n_partials, variant);
-  }
-  orx_set_error("unknown optimizer kind %d", opt_kind);
-  return ORX_ERR_INVALID;
 }
 
 static int check_point(int kind, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
@@ -408,8 +354,11 @@ extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_
   pa.opt = orx_opt_to_dev(opt);
   pa.gw = (kind == ORX_POINT_GMF) ? h->gw : nullptr;
   int n_partials = 0, variant = 0;
-  rc = (kind == ORX_POINT_GMF) ? launch_point_kind<ORX_POINT_GMF>(pa, opt->kind, st, &n_partials, &variant)
-                               : launch_point_kind<ORX_POINT_WRMF>(pa, opt->kind, st, &n_partials, &variant);
+  rc = orx_dispatch<ORX_POINT_GMF, ORX_POINT_WRMF>(kind, [&](auto K) {
+    return orx_dispatch_opt(opt->kind, [&](auto O) {
+      return launch_point_kind_opt<decltype(K)::value, decltype(O)::value>(pa, st, &n_partials, &variant);
+    });
+  });
   if (rc) return rc;
   orx_log_dispatch(h, ORX_OP_POINTWISE_STEP, variant, kind, opt->kind, B, D, 0, 0);   // index set 0 always
   if (dense) {

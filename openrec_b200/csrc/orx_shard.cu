@@ -439,8 +439,7 @@ struct ShCompArgs {
 
 template <int KIND, int OPT, int NQ>
 __global__ void __launch_bounds__(256) k_sh_compute(ShardDev x, ShardWs w, ShCompArgs a, int epoch) {
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
+  typedef OrxOptSlots<OPT> SL;
   constexpr int TPW = NQ == 1 ? 4 : (NQ == 2 ? 2 : 1);     // triplets in flight per warp
   __shared__ int32_t goff[SH_MAX_R], gbase[SH_MAX_R];
   const int R = x.world, me = x.rank, D = x.D, nq = D >> 2;
@@ -504,8 +503,8 @@ __global__ void __launch_bounds__(256) k_sh_compute(ShardDev x, ShardWs w, ShCom
         u[k][q] = on ? __ldcg(reinterpret_cast<const float4*>(a.U + (int64_t)uu[k] * D) + e) : z4;
         p[k][q] = on ? __ldcg(reinterpret_cast<const float4*>(got + (int64_t)pp * D) + e) : z4;
         n[k][q] = on ? __ldcg(reinterpret_cast<const float4*>(got + (int64_t)pn * D) + e) : z4;
-        us0[k][q] = (S0 && on && own) ? __ldcg(reinterpret_cast<const float4*>(a.Us0 + (int64_t)uu[k] * D) + e) : z4;
-        us1[k][q] = (S1 && on && own) ? __ldcg(reinterpret_cast<const float4*>(a.Us1 + (int64_t)uu[k] * D) + e) : z4;
+        us0[k][q] = (SL::S0 && on && own) ? __ldcg(reinterpret_cast<const float4*>(a.Us0 + (int64_t)uu[k] * D) + e) : z4;
+        us1[k][q] = (SL::S1 && on && own) ? __ldcg(reinterpret_cast<const float4*>(a.Us1 + (int64_t)uu[k] * D) + e) : z4;
       }
     }
 #pragma unroll
@@ -543,14 +542,9 @@ __global__ void __launch_bounds__(256) k_sh_compute(ShardDev x, ShardWs w, ShCom
         pair_row_grads<KIND>(g, a.c_l2, u[k][q], p[k][q], n[k][q], &gu, &gp, &gn);
         if (dp) reinterpret_cast<float4*>(dp)[e] = gp;           // peer stores: the item gradient rows
         if (dn) reinterpret_cast<float4*>(dn)[e] = gn;
-        const int64_t o = (int64_t)uu[k] * D + 4 * e;
-        if (own) {                                               // the only reference of this user row in the global batch
-          __stcg(reinterpret_cast<float4*>(a.U + o), orx_apply4<OPT>(u[k][q], gu, us0[k][q], us1[k][q], a.opt));
-          if (S0) __stcg(reinterpret_cast<float4*>(a.Us0 + o), us0[k][q]);
-          if (S1) __stcg(reinterpret_cast<float4*>(a.Us1 + o), us1[k][q]);
-        } else {
-          orx_red4(a.gu + (int64_t)du * D + 4 * e, gu);
-        }
+        // own: the only reference of this user row in the global batch
+        orx_own_or_stage4<OPT, false>(own, a.U, a.Us0, a.Us1, uu[k], a.gu, du, D, 4 * e, u[k][q], gu, us0[k][q],
+                                      us1[k][q], a.opt);
       }
       {                         // bias gradient of the positive item: BPR +g, UCML -g; the negative gets the opposite sign
         float* bdp = reinterpret_cast<float*>(__shfl_sync(ORX_FULL, (unsigned long long)my_bdp, k));
@@ -571,28 +565,13 @@ __global__ void __launch_bounds__(256) k_sh_compute(ShardDev x, ShardWs w, ShCom
     a.partials[2 * gwarp + 1] = l2_acc;
   }
   // The LAST block to finish reduces this rank's (loss, l2) partials, sends the pair to every rank and releases flag 3.
-  __shared__ double sh_red[2][256];
   sh_arrive(x, w.ctl + SH_C_DONE + 3, gridDim.x, 3, epoch, [&]() {
-    double l = 0.0, q = 0.0;                           // deterministic (fixed order, double) reduction of my partials
-    const int np = (int)((gridDim.x * blockDim.x) >> 5);
-    for (int i = threadIdx.x; i < np; i += blockDim.x) {
-      l += (double)__ldcg(a.partials + 2 * i);
-      q += (double)__ldcg(a.partials + 2 * i + 1);
-    }
-    sh_red[0][threadIdx.x] = l;
-    sh_red[1][threadIdx.x] = q;
-    __syncthreads();
-    for (int s = 128; s > 0; s >>= 1) {
-      if ((int)threadIdx.x < s) {
-        sh_red[0][threadIdx.x] += sh_red[0][threadIdx.x + s];
-        sh_red[1][threadIdx.x] += sh_red[1][threadIdx.x + s];
-      }
-      __syncthreads();
-    }
+    double l, q;                                       // deterministic (fixed order, double) reduction of my partials
+    orx_block_sum_partials(a.partials, (int)((gridDim.x * blockDim.x) >> 5), nullptr, 0, &l, &q);
     if ((int)threadIdx.x < R) {
       int32_t* m = x.meta[threadIdx.x] + SH_META * me;
-      m[SH_M_LOSS] = __float_as_int((float)(sh_red[0][0] * (double)a.loss_scale));
-      m[SH_M_L2] = __float_as_int((float)(0.5 * sh_red[1][0]));
+      m[SH_M_LOSS] = __float_as_int((float)(l * (double)a.loss_scale));
+      m[SH_M_L2] = __float_as_int((float)(0.5 * q));
     }
   });
 }
@@ -623,8 +602,7 @@ struct ShProArgs {
 
 template <int OPT, int NQ>
 __global__ void __launch_bounds__(256) k_sh_apply(ShardDev x, ShardWs w, ShApplyArgs a, ShProArgs pro, int epoch) {
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
+  typedef OrxOptSlots<OPT> SL;
   constexpr int GRP = NQ == 1 ? 4 : (NQ == 2 ? 2 : 1);   // rows whose loads are issued together
   const int me = x.rank, D = x.D, nq = D >> 2;
   orx_pdl_wait();
@@ -661,10 +639,10 @@ __global__ void __launch_bounds__(256) k_sh_apply(ShardDev x, ShardWs w, ShApply
         my_own = orx_hash_find(a.hi, my_id, &my_d) == 1u;
         const float gbv = __ldcg(ginb + j0 + lane);
         if (my_own) {            // bias of a row requested once: lane-parallel, straight from the inbox
-          float s0v = S0 ? __ldcg(a.Bs0 + my_id) : 0.f, s1v = S1 ? __ldcg(a.Bs1 + my_id) : 0.f;
+          float s0v = SL::S0 ? __ldcg(a.Bs0 + my_id) : 0.f, s1v = SL::S1 ? __ldcg(a.Bs1 + my_id) : 0.f;
           __stcg(a.Bv + my_id, orx_apply<OPT>(__ldcg(a.Bv + my_id), gbv, s0v, s1v, a.opt));
-          if (S0) __stcg(a.Bs0 + my_id, s0v);
-          if (S1) __stcg(a.Bs1 + my_id, s1v);
+          if (SL::S0) __stcg(a.Bs0 + my_id, s0v);
+          if (SL::S1) __stcg(a.Bs1 + my_id, s1v);
         } else {
           atomicAdd(a.gb + my_d, gbv);
         }
@@ -687,8 +665,8 @@ __global__ void __launch_bounds__(256) k_sh_apply(ShardDev x, ShardWs w, ShApply
           g[k][q] = on ? __ldcg(reinterpret_cast<const float4*>(gin + (int64_t)(j0 + k0 + k) * D) + e) : z4;
           const bool ld = on && own[k];
           wv[k][q] = ld ? __ldcg(reinterpret_cast<const float4*>(a.I + (int64_t)id[k] * D) + e) : z4;
-          s0v[k][q] = (S0 && ld) ? __ldcg(reinterpret_cast<const float4*>(a.Is0 + (int64_t)id[k] * D) + e) : z4;
-          s1v[k][q] = (S1 && ld) ? __ldcg(reinterpret_cast<const float4*>(a.Is1 + (int64_t)id[k] * D) + e) : z4;
+          s0v[k][q] = (SL::S0 && ld) ? __ldcg(reinterpret_cast<const float4*>(a.Is0 + (int64_t)id[k] * D) + e) : z4;
+          s1v[k][q] = (SL::S1 && ld) ? __ldcg(reinterpret_cast<const float4*>(a.Is1 + (int64_t)id[k] * D) + e) : z4;
         }
       }
 #pragma unroll
@@ -698,14 +676,8 @@ __global__ void __launch_bounds__(256) k_sh_apply(ShardDev x, ShardWs w, ShApply
         for (int q = 0; q < NQ; ++q) {
           const int e = q * 32 + lane;
           if (e >= nq) continue;
-          if (own[k]) {
-            const int64_t o = (int64_t)id[k] * D + 4 * e;
-            __stcg(reinterpret_cast<float4*>(a.I + o), orx_apply4<OPT>(wv[k][q], g[k][q], s0v[k][q], s1v[k][q], a.opt));
-            if (S0) __stcg(reinterpret_cast<float4*>(a.Is0 + o), s0v[k][q]);
-            if (S1) __stcg(reinterpret_cast<float4*>(a.Is1 + o), s1v[k][q]);
-          } else {
-            orx_red4(a.gi + (int64_t)d[k] * D + 4 * e, g[k][q]);
-          }
+          orx_own_or_stage4<OPT, false>(own[k], a.I, a.Is0, a.Is1, id[k], a.gi, d[k], D, 4 * e, wv[k][q], g[k][q],
+                                        s0v[k][q], s1v[k][q], a.opt);
         }
       }
     }
@@ -713,70 +685,13 @@ __global__ void __launch_bounds__(256) k_sh_apply(ShardDev x, ShardWs w, ShApply
   orx_pdl_trigger();
 }
 
-// staged (duplicated) user and item rows -> optimizer, once per unique row, staging re-zeroed; global (loss, l2) from the
-// meta mailbox; counters reset.  Two rows per warp iteration so that both rows' loads are in flight together.
-struct ShTailArgs {
-  float *U, *Us0, *Us1;
-  OrxHash hu;
-  float* gu;
-};
-
+// staged (duplicated) user and item rows -> optimizer, once per unique row, staging re-zeroed: the rows of the
+// single-GPU tail (orx_tail_rows); global (loss, l2) from the meta mailbox; counters reset.
 template <int OPT>
-__device__ __forceinline__ void sh_apply_staged2(float* W, float* P0, float* P1, float* G, int D, int lane, int id1, int r1,
-                                                 bool two, int id2, int r2, const OrxOptDev& opt) {
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
-  const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int e = lane * 4; e < D; e += 128) {
-    const int64_t o1 = (int64_t)id1 * D + e, o2 = (int64_t)id2 * D + e;
-    float4* gp1 = reinterpret_cast<float4*>(G + (int64_t)r1 * D + e);
-    float4* gp2 = reinterpret_cast<float4*>(G + (int64_t)r2 * D + e);
-    const float4 g1 = __ldcg(gp1), g2 = two ? __ldcg(gp2) : z;
-    float4 w1 = __ldcg(reinterpret_cast<const float4*>(W + o1)), w2 = two ? __ldcg(reinterpret_cast<const float4*>(W + o2)) : z;
-    float4 p1 = S0 ? __ldcg(reinterpret_cast<const float4*>(P0 + o1)) : z, p2 = (S0 && two) ? __ldcg(reinterpret_cast<const float4*>(P0 + o2)) : z;
-    float4 q1 = S1 ? __ldcg(reinterpret_cast<const float4*>(P1 + o1)) : z, q2 = (S1 && two) ? __ldcg(reinterpret_cast<const float4*>(P1 + o2)) : z;
-    __stcg(reinterpret_cast<float4*>(W + o1), orx_apply4<OPT>(w1, g1, p1, q1, opt));
-    if (S0) __stcg(reinterpret_cast<float4*>(P0 + o1), p1);
-    if (S1) __stcg(reinterpret_cast<float4*>(P1 + o1), q1);
-    __stcg(gp1, z);
-    if (two) {
-      __stcg(reinterpret_cast<float4*>(W + o2), orx_apply4<OPT>(w2, g2, p2, q2, opt));
-      if (S0) __stcg(reinterpret_cast<float4*>(P0 + o2), p2);
-      if (S1) __stcg(reinterpret_cast<float4*>(P1 + o2), q2);
-      __stcg(gp2, z);
-    }
-  }
-}
-
-template <int OPT>
-__global__ void __launch_bounds__(256) k_sh_tail(ShardDev x, ShardWs w, ShTailArgs u, ShApplyArgs a, int32_t* ticket,
-                                                 int par, float* out4) {
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
-  const int D = x.D;
-  const int lane = threadIdx.x & 31;
-  const int gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nw = (gridDim.x * blockDim.x) >> 5;
+__global__ void __launch_bounds__(256) k_sh_tail(ShardDev x, ShardWs w, TailArgs a, int par) {
   orx_pdl_wait();
-  const int nu = *u.hu.counter, ni = *a.hi.counter;
-  for (int r = gwarp; r < nu; r += 2 * nw) {
-    const int r2 = r + nw;
-    const bool two = r2 < nu;
-    sh_apply_staged2<OPT>(u.U, u.Us0, u.Us1, u.gu, D, lane, u.hu.did[r], r, two, two ? u.hu.did[r2] : 0, two ? r2 : r, a.opt);
-  }
-  for (int r = gwarp; r < ni; r += 2 * nw) {
-    const int r2 = r + nw;
-    const bool two = r2 < ni;
-    const int id1 = a.hi.did[r], id2 = two ? a.hi.did[r2] : 0;
-    sh_apply_staged2<OPT>(a.I, a.Is0, a.Is1, a.gi, D, lane, id1, r, two, id2, two ? r2 : r, a.opt);
-    if (lane < (two ? 2 : 1)) {            // lane 0: row r, lane 1: row r2 -- the item bias of the staged row
-      const int id = lane ? id2 : id1, rr = lane ? r2 : r;
-      float s0v = S0 ? a.Bs0[id] : 0.f, s1v = S1 ? a.Bs1[id] : 0.f;
-      a.Bv[id] = orx_apply<OPT>(a.Bv[id], __ldcg(a.gb + rr), s0v, s1v, a.opt);
-      if (S0) a.Bs0[id] = s0v;
-      if (S1) a.Bs1[id] = s1v;
-      a.gb[rr] = 0.f;
-    }
-  }
+  const int nu = *a.hu.counter, ni = *a.hi.counter;
+  orx_tail_rows<OPT>(a, nu, ni);
   if (blockIdx.x == 0 && threadIdx.x == 0) {    // every rank adds the R pairs it holds in rank order: bit-identical totals
     const int32_t* m = x.meta[x.rank];
     float l = 0.f, q = 0.f;
@@ -784,10 +699,10 @@ __global__ void __launch_bounds__(256) k_sh_tail(ShardDev x, ShardWs w, ShTailAr
       l += __int_as_float(__ldcg(m + SH_META * r + SH_M_LOSS));
       q += __int_as_float(__ldcg(m + SH_META * r + SH_M_L2));
     }
-    out4[0] = l;
-    out4[1] = q;
-    out4[2] = (float)w.ctl[SH_C_BAD + par];
-    out4[3] = (float)(nu + ni);
+    a.out4[0] = l;
+    a.out4[1] = q;
+    a.out4[2] = (float)w.ctl[SH_C_BAD + par];
+    a.out4[3] = (float)(nu + ni);
     w.ctl[SH_C_BAD + par] = 0;
     w.ctl[SH_C_ACUR] = 0;
   }
@@ -795,13 +710,13 @@ __global__ void __launch_bounds__(256) k_sh_tail(ShardDev x, ShardWs w, ShTailAr
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence();
-    last = (atomicAdd(ticket, 1) == (int)gridDim.x - 1);
+    last = (atomicAdd(a.counters + 2, 1) == (int)gridDim.x - 1);
   }
   __syncthreads();
   if (last && threadIdx.x == 0) {
-    *u.hu.counter = 0;
+    *a.hu.counter = 0;
     *a.hi.counter = 0;
-    *ticket = 0;
+    a.counters[2] = 0;
   }
 }
 
@@ -944,27 +859,15 @@ extern "C" int orx_shard_sizes(const orx_shard_t* xs, int64_t* n8_host) {
   return ORX_OK;
 }
 
-template <int KIND, int OPT>
-static int launch_compute(int nq, int num_sms, cudaStream_t st, const ShardDev& xd, const ShardWs& w, const ShCompArgs& a, int epoch) {
-#define SH_GO(NQ)                                                                        \
-  {                                                                                      \
-    const int g = num_sms * sh_ctas_per_sm((const void*)k_sh_compute<KIND, OPT, NQ>, 4); \
-    orx_launch_pdl(k_sh_compute<KIND, OPT, NQ>, dim3(g), dim3(256), 0, st, xd, w, a, epoch); \
-    return g;                                                                            \
-  }
-  if (nq <= 32) SH_GO(1) else if (nq <= 64) SH_GO(2) else SH_GO(4)
-#undef SH_GO
+// runtime -> template arguments of the sharded kernels: the optimizers the sharded step supports (it rejects ADAM_DENSE)
+// and the row-width classes NQ (float4 per lane: D <= 128, 256, 512)
+template <typename F>
+static inline auto sh_dispatch_opt(int opt_kind, F&& f) {
+  return orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY>(opt_kind, f);
 }
-template <int OPT>
-static void launch_apply(int nq, int num_sms, cudaStream_t st, const ShardDev& xd, const ShardWs& w, const ShApplyArgs& a,
-                         const ShProArgs& pro, int epoch) {
-#define SH_GO(NQ)                                                                          \
-  {                                                                                        \
-    const int g = num_sms * sh_ctas_per_sm((const void*)k_sh_apply<OPT, NQ>, 4) + pro.n_route + pro.n_request; \
-    orx_launch_pdl(k_sh_apply<OPT, NQ>, dim3(g), dim3(256), 0, st, xd, w, a, pro, epoch);  \
-  }
-  if (nq <= 32) SH_GO(1) else if (nq <= 64) SH_GO(2) else SH_GO(4)
-#undef SH_GO
+template <typename F>
+static inline auto sh_dispatch_nq(int nq, F&& f) {
+  return orx_dispatch<1, 2, 4>(nq <= 32 ? 1 : (nq <= 64 ? 2 : 4), f);
 }
 
 // two fresh index epochs (user set of the step, item set of the step).  A 31-bit wrap empties every table of the handle
@@ -1085,26 +988,23 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
         break;
       case 2:
         ORX_REQUIRE(S->pro_request[par] == epoch, "phase 2 before this step's phases 0 and 1");
-#define SH_SERVE(NQ)                                                                                          \
-  ORX_CUDA(orx_launch_pdl(k_sh_serve<NQ>, dim3(h->num_sms * sh_ctas_per_sm((const void*)k_sh_serve<NQ>, 4)),  \
-                          dim3(256), 0, st, xd, w, (const float*)item->var, (const float*)item_bias->var,    \
-                          (int64_t)item->rows, hi, epoch))
-        if (nq <= 32) SH_SERVE(1); else if (nq <= 64) SH_SERVE(2); else SH_SERVE(4);
-#undef SH_SERVE
+        sh_dispatch_nq(nq, [&](auto Q) {
+          auto kern = k_sh_serve<decltype(Q)::value>;
+          orx_launch_pdl(kern, dim3(h->num_sms * sh_ctas_per_sm((const void*)kern, 4)), dim3(256), 0, st, xd, w,
+                         (const float*)item->var, (const float*)item_bias->var, (int64_t)item->rows, hi, epoch);
+        });
         S->serve_epoch = epoch;
         break;
       case 3:
-#define SH_COMPUTE(K, O) launch_compute<K, O>(nq, h->num_sms, st, xd, w, ca, epoch)
-        if (kind == ORX_PAIR_BPR) {
-          if (opt->kind == ORX_OPT_SGD) SH_COMPUTE(ORX_PAIR_BPR, ORX_OPT_SGD);
-          else if (opt->kind == ORX_OPT_ADAGRAD) SH_COMPUTE(ORX_PAIR_BPR, ORX_OPT_ADAGRAD);
-          else SH_COMPUTE(ORX_PAIR_BPR, ORX_OPT_ADAM_LAZY);
-        } else {
-          if (opt->kind == ORX_OPT_SGD) SH_COMPUTE(ORX_PAIR_UCML, ORX_OPT_SGD);
-          else if (opt->kind == ORX_OPT_ADAGRAD) SH_COMPUTE(ORX_PAIR_UCML, ORX_OPT_ADAGRAD);
-          else SH_COMPUTE(ORX_PAIR_UCML, ORX_OPT_ADAM_LAZY);
-        }
-#undef SH_COMPUTE
+        orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {
+          sh_dispatch_opt(opt->kind, [&](auto O) {
+            sh_dispatch_nq(nq, [&](auto Q) {
+              auto kern = k_sh_compute<decltype(K)::value, decltype(O)::value, decltype(Q)::value>;
+              orx_launch_pdl(kern, dim3(h->num_sms * sh_ctas_per_sm((const void*)kern, 4)), dim3(256), 0, st, xd, w,
+                             ca, epoch);
+            });
+          });
+        });
         break;
       case 4: {
         ShProArgs pro;
@@ -1122,19 +1022,29 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
           S->ids_u[np] = next_uid; S->ids_p[np] = next_pid; S->ids_n[np] = next_nid; S->ids_B[np] = next_B;
           S->pro_route[np] = S->pro_request[np] = epoch + 1;
         }
-        if (opt->kind == ORX_OPT_SGD) launch_apply<ORX_OPT_SGD>(nq, h->num_sms, st, xd, w, aa, pro, epoch);
-        else if (opt->kind == ORX_OPT_ADAGRAD) launch_apply<ORX_OPT_ADAGRAD>(nq, h->num_sms, st, xd, w, aa, pro, epoch);
-        else launch_apply<ORX_OPT_ADAM_LAZY>(nq, h->num_sms, st, xd, w, aa, pro, epoch);
+        sh_dispatch_opt(opt->kind, [&](auto O) {
+          sh_dispatch_nq(nq, [&](auto Q) {
+            auto kern = k_sh_apply<decltype(O)::value, decltype(Q)::value>;
+            const int g = h->num_sms * sh_ctas_per_sm((const void*)kern, 4) + pro.n_route + pro.n_request;
+            orx_launch_pdl(kern, dim3(g), dim3(256), 0, st, xd, w, aa, pro, epoch);
+          });
+        });
         break;
       }
       case 5: {
-        const int g = h->num_sms * 4;
-        ShTailArgs ta;
-        ta.U = user->var; ta.Us0 = user->s0; ta.Us1 = user->s1; ta.hu = hu; ta.gu = h->gu;
-        int32_t* ticket = h->counters + 2;
-        if (opt->kind == ORX_OPT_SGD) ORX_CUDA(orx_launch_pdl(k_sh_tail<ORX_OPT_SGD>, dim3(g), dim3(256), 0, st, xd, w, ta, aa, ticket, par, out4));
-        else if (opt->kind == ORX_OPT_ADAGRAD) ORX_CUDA(orx_launch_pdl(k_sh_tail<ORX_OPT_ADAGRAD>, dim3(g), dim3(256), 0, st, xd, w, ta, aa, ticket, par, out4));
-        else ORX_CUDA(orx_launch_pdl(k_sh_tail<ORX_OPT_ADAM_LAZY>, dim3(g), dim3(256), 0, st, xd, w, ta, aa, ticket, par, out4));
+        const int g = h->num_sms * 4;   // the grid of k_sparse_tail
+        TailArgs ta;
+        memset(&ta, 0, sizeof(ta));
+        ta.U = user->var; ta.Us0 = user->s0; ta.Us1 = user->s1;
+        ta.I = item->var; ta.Is0 = item->s0; ta.Is1 = item->s1;
+        ta.Bv = item_bias->var; ta.Bs0 = item_bias->s0; ta.Bs1 = item_bias->s1;
+        ta.D = x->dim; ta.opt = od; ta.hu = hu; ta.hi = hi;
+        ta.gu = h->gu; ta.gi = h->gi; ta.gb = h->gb;
+        ta.counters = h->counters;   // [2]: the tail's block ticket
+        ta.out4 = out4;
+        sh_dispatch_opt(opt->kind, [&](auto O) {
+          orx_launch_pdl(k_sh_tail<decltype(O)::value>, dim3(g), dim3(256), 0, st, xd, w, ta, par);
+        });
         S->tail_epoch = epoch;
         break;
       }

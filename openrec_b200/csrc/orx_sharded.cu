@@ -3,8 +3,11 @@
 //                        local row r / R) -> send order, per-owner counts, inverse permutation ("K9" bucket half)
 //   * orx_sparse_apply : Keras OptimizerV2 sparse apply of IndexedSlices (ids[n], values[n,D]) to one table:
 //                        dedup by row (batch hash), rows hit once are updated straight from their value row,
-//                        duplicated rows are summed in the staging buffer and updated once ("K8").
+//                        duplicated rows are summed in the staging buffer and updated once by the steps' staged-row
+//                        tail, k_sparse_tail ("K8").
 // The reference has no multi-device code (SURVEY 2.1); the partitioning follows SURVEY 8(e).
+#include <string.h>
+
 #include "orx_common.cuh"
 
 // ---------------------------------------------------------------------------------------
@@ -118,9 +121,7 @@ __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, flo
                                                       const float* __restrict__ vals, int64_t val_ld, int n,
                                                       const int32_t* __restrict__ n_dev, OrxHash hsh, float* gstage,
                                                       OrxOptDev o) {
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool STAGE_ONLY = (OPT == ORX_OPT_ADAM_DENSE);
+  typedef OrxOptSlots<OPT> SL;
   const int lane = threadIdx.x & 31;
   if (n_dev) n = min(n, *n_dev);   // count produced on the device: the grid is capped and strides over it
   const int nw = (gridDim.x * blockDim.x) >> 5;
@@ -143,87 +144,26 @@ __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, flo
   const int d = __shfl_sync(ORX_FULL, my_d, k);
   if (id < 0) continue;
   const float* v = vals + (int64_t)b * val_ld;
-  const bool vec = ((D & 3) == 0) && ((val_ld & 3) == 0);
-  if (!STAGE_ONLY && c == 1u) {
-    float* w = var + (int64_t)id * D;
-    if (vec) {   // 128-bit path: all loads of the row first, then the math, then the stores
-      for (int e = lane * 4; e < D; e += 128) {
-        const int64_t off = (int64_t)id * D + e;
-        const float4 g = __ldcg(reinterpret_cast<const float4*>(v + e));
-        float4 wv = __ldcg(reinterpret_cast<const float4*>(w + e));
-        float4 a = S0 ? __ldcg(reinterpret_cast<const float4*>(s0 + off)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        float4 bb = S1 ? __ldcg(reinterpret_cast<const float4*>(s1 + off)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        __stcg(reinterpret_cast<float4*>(w + e), orx_apply4<OPT>(wv, g, a, bb, o));
-        if (S0) __stcg(reinterpret_cast<float4*>(s0 + off), a);
-        if (S1) __stcg(reinterpret_cast<float4*>(s1 + off), bb);
-      }
-    } else {
-      for (int e = lane; e < D; e += 32) {
-        const int64_t off = (int64_t)id * D + e;
-        float a = S0 ? s0[off] : 0.f, bb = S1 ? s1[off] : 0.f;
-        w[e] = orx_apply<OPT>(w[e], v[e], a, bb, o);
-        if (S0) s0[off] = a;
-        if (S1) s1[off] = bb;
-      }
+  const bool own = !SL::STAGE_ONLY && c == 1u;
+  if (((D & 3) == 0) && ((val_ld & 3) == 0)) {   // 128-bit path: all loads of the row first, then the math, then the stores
+    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int e = lane * 4; e < D; e += 128) {
+      const int64_t off = (int64_t)id * D + e;
+      const float4 g = __ldcg(reinterpret_cast<const float4*>(v + e));
+      const float4 wv = own ? __ldcg(reinterpret_cast<const float4*>(var + off)) : z4;
+      float4 a = (SL::S0 && own) ? __ldcg(reinterpret_cast<const float4*>(s0 + off)) : z4;
+      float4 bb = (SL::S1 && own) ? __ldcg(reinterpret_cast<const float4*>(s1 + off)) : z4;
+      orx_own_or_stage4<OPT, false>(own, var, s0, s1, id, gstage, d, D, e, wv, g, a, bb, o);
     }
-  } else if (vec) {
-    for (int e = lane * 4; e < D; e += 128)
-      orx_red4(gstage + (int64_t)d * D + e, __ldcg(reinterpret_cast<const float4*>(v + e)));
   } else {
-    for (int e = lane; e < D; e += 32) atomicAdd(gstage + (int64_t)d * D + e, v[e]);
-  }
-  }
-  }
-}
-
-// tail for one table: staged rows -> optimizer, staging zeroed, hash cleared, counters reset
-template <int OPT>
-__global__ void __launch_bounds__(256) k_sparse_apply_tail(float* var, float* s0, float* s1, int D, OrxHash hsh,
-                                                           float* gstage, OrxOptDev o, int32_t* counters) {
-  constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
-  constexpr bool ZERO_ONLY = (OPT == ORX_OPT_ADAM_DENSE);
-  const int lane = threadIdx.x & 31;
-  const int gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
-  const int ns = *hsh.counter;
-  for (int r = gwarp; r < ns; r += nwarps) {
-    const int id = hsh.did[r];
-    if ((D & 3) == 0) {   // 128-bit path
-      for (int e = lane * 4; e < D; e += 128) {
-        const int64_t off = (int64_t)id * D + e;
-        float4* gp = reinterpret_cast<float4*>(gstage + (int64_t)r * D + e);
-        if (!ZERO_ONLY) {
-          const float4 g = __ldcg(gp);
-          float4 wv = __ldcg(reinterpret_cast<const float4*>(var + off));
-          float4 a = S0 ? __ldcg(reinterpret_cast<const float4*>(s0 + off)) : make_float4(0.f, 0.f, 0.f, 0.f);
-          float4 bb = S1 ? __ldcg(reinterpret_cast<const float4*>(s1 + off)) : make_float4(0.f, 0.f, 0.f, 0.f);
-          __stcg(reinterpret_cast<float4*>(var + off), orx_apply4<OPT>(wv, g, a, bb, o));
-          if (S0) __stcg(reinterpret_cast<float4*>(s0 + off), a);
-          if (S1) __stcg(reinterpret_cast<float4*>(s1 + off), bb);
-        }
-        __stcg(gp, make_float4(0.f, 0.f, 0.f, 0.f));
-      }
-      continue;
-    }
     for (int e = lane; e < D; e += 32) {
       const int64_t off = (int64_t)id * D + e;
-      if (!ZERO_ONLY) {
-        float a = S0 ? s0[off] : 0.f, bb = S1 ? s1[off] : 0.f;
-        var[off] = orx_apply<OPT>(var[off], gstage[(int64_t)r * D + e], a, bb, o);
-        if (S0) s0[off] = a;
-        if (S1) s1[off] = bb;
-      }
-      gstage[(int64_t)r * D + e] = 0.f;
+      if (own) orx_update1<OPT>(var + off, s0 + off, s1 + off, var[off], v[e], o);
+      else atomicAdd(gstage + (int64_t)d * D + e, v[e]);
     }
   }
-  __shared__ bool last;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    last = (atomicAdd(counters + 2, 1) == (int)gridDim.x - 1);
   }
-  __syncthreads();
-  if (last && threadIdx.x < 4) counters[threadIdx.x] = 0;
+  }
 }
 
 static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
@@ -265,23 +205,19 @@ static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32
     if ((rc = orx_launch_index_build_strided(h, ids, id_stride, tab->rows, n, n_dev, dense, st))) return rc;
     int blocks = (n + 63) / 64;   // 8 warps x 8 pairs per block and iteration
     if (n_dev && blocks > h->num_sms * 8) blocks = h->num_sms * 8;
-    switch (opt->kind) {
-      case ORX_OPT_SGD: k_sparse_apply<ORX_OPT_SGD><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride, values, value_ld, n, n_dev, h->hu, h->gu, o); break;
-      case ORX_OPT_ADAGRAD: k_sparse_apply<ORX_OPT_ADAGRAD><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride, values, value_ld, n, n_dev, h->hu, h->gu, o); break;
-      case ORX_OPT_ADAM_LAZY: k_sparse_apply<ORX_OPT_ADAM_LAZY><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride, values, value_ld, n, n_dev, h->hu, h->gu, o); break;
-      default: k_sparse_apply<ORX_OPT_ADAM_DENSE><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride, values, value_ld, n, n_dev, h->hu, h->gu, o); break;
-    }
+    orx_dispatch_opt(opt->kind, [&](auto O) {
+      k_sparse_apply<decltype(O)::value><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride,
+                                                                 values, value_ld, n, n_dev, h->hu, h->gu, o);
+    });
     ORX_LAUNCH_CHECK();
   }
   if (dense)
     if ((rc = orx_launch_adam_sweep(h, tab->var, tab->s0, tab->s1, tab->rows, D, h->hu, h->gu, o, st))) return rc;
-  const int grid = h->num_sms * 2;
-  switch (opt->kind) {
-    case ORX_OPT_SGD: k_sparse_apply_tail<ORX_OPT_SGD><<<grid, 256, 0, st>>>(tab->var, tab->s0, tab->s1, D, h->hu, h->gu, o, h->counters); break;
-    case ORX_OPT_ADAGRAD: k_sparse_apply_tail<ORX_OPT_ADAGRAD><<<grid, 256, 0, st>>>(tab->var, tab->s0, tab->s1, D, h->hu, h->gu, o, h->counters); break;
-    case ORX_OPT_ADAM_LAZY: k_sparse_apply_tail<ORX_OPT_ADAM_LAZY><<<grid, 256, 0, st>>>(tab->var, tab->s0, tab->s1, D, h->hu, h->gu, o, h->counters); break;
-    default: k_sparse_apply_tail<ORX_OPT_ADAM_DENSE><<<grid, 256, 0, st>>>(tab->var, tab->s0, tab->s1, D, h->hu, h->gu, o, h->counters); break;
-  }
-  ORX_LAUNCH_CHECK();
-  return ORX_OK;
+  // staged rows: the shared tail with no item side and no loss
+  TailArgs ta;
+  memset(&ta, 0, sizeof(ta));
+  ta.U = tab->var; ta.Us0 = tab->s0; ta.Us1 = tab->s1;
+  ta.D = D; ta.opt = o; ta.hu = h->hu; ta.gu = h->gu;
+  ta.counters = h->counters;
+  return orx_launch_tail(h, ta, opt->kind, st);
 }
