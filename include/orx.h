@@ -162,19 +162,12 @@ ORX_API int orx_pairwise_fwd(orx_handle_t h, int32_t kind, const orx_table_t* us
                      int32_t B, float margin, float* out4, orx_stream_t s);
 /* Un-fused gradients in TF IndexedSlices form (values per lookup, NOT deduplicated):
  * d_user[B,D], d_pos[B,D], d_neg[B,D], d_bp[B], d_bn[B]; any may be NULL.  g_out[B] (optional) receives
- * the per-triplet loss-gradient scalar.  orx_pairwise_grad_slots is the compact form used by the sharded
- * step: the "tables" are the rows fetched for this batch (one row per lookup), gradients are written to
- * the lookup's own row (d_user[uid[t]], d_item[pid[t]] / d_item[nid[t]], d_bias likewise), and out4 gets
- * the local (loss, l2_loss) sums. */
+ * the per-triplet loss-gradient scalar.  orx_pairwise_grad_rows (below) is the compact form used by the
+ * NCCL form of the sharded step: gradients are written to the lookup's own fetched row. */
 ORX_API int orx_pairwise_grad(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
                       const orx_table_t* item_bias, const int32_t* uid, const int32_t* pid, const int32_t* nid,
                       int32_t B, float margin, float c_loss, float c_l2, float* d_user, float* d_pos, float* d_neg,
                       float* d_bp, float* d_bn, float* g_out, orx_stream_t s);
-
-ORX_API int orx_pairwise_grad_slots(orx_handle_t h, int32_t kind, const float* user_rows, const float* item_rows,
-                            const float* bias_rows, int32_t dim, const int32_t* uslot, const int32_t* pslot,
-                            const int32_t* nslot, int32_t B, float margin, float c_loss, float c_l2, float inv_B,
-                            float* d_user_rows, float* d_item_rows, float* d_bias_rows, float* out4, orx_stream_t s);
 
 /* ---- pointwise recommenders: GMF (recommenders/gmf.py:22-34) and WRMF (recommenders/wrmf.py:21-34 +
  *      modules/pointwise_mse_loss.py:18-31) ---------------------------------------------------
@@ -205,15 +198,12 @@ ORX_API int orx_sparse_apply(orx_handle_t h, const orx_table_t* tab, const int32
 ORX_API int orx_sparse_apply_strided(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
                                      const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt_host,
                                      orx_stream_t s);
-/* orx_owner_bucket: row r lives on rank r % world at local row r / world.  counts[world] = lookups per owner,
- * send_local[n] = local rows in owner-sorted send order, slot[n] = position of lookup i in that order. */
-ORX_API int orx_owner_bucket(orx_handle_t h, const int32_t* ids, int32_t n, int32_t world, int32_t* counts,
-                             int32_t* send_local, int32_t* slot, orx_stream_t s);
-
 /* Combined form used by openrec_b200/sharded.py: each rank stores ONE local table [user rows | item rows] of
  * width ld = D+4 (item bias in column D), so a lookup is (owner, combined local row) whatever its table.
- * orx_owner_bucket_combined: ids = uid | pid | nid (n_user user ids first); item lookups get the owner's user-row
- *   count added to their local row.
+ * orx_owner_bucket_combined: ids = uid | pid | nid (n_user user ids first).  Row r lives on rank r % world at
+ *   local row r / world; item lookups get the owner's user-row count added to their local row.  counts[world] =
+ *   lookups per owner, send_local[n] = local rows in owner-sorted send order, slot[n] = position of lookup i in
+ *   that order.
  * orx_pairwise_grad_rows: score/loss/gradients on the fetched rows (one row of width ld per lookup; slots index
  *   the same buffer); gradients overwrite d_rows at the lookup's row (bias gradient in column D, padding zero). */
 ORX_API int orx_owner_bucket_combined(orx_handle_t h, const int32_t* ids, int32_t n, int32_t n_user, int64_t total_users,

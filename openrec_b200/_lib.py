@@ -70,8 +70,6 @@ SIGNATURES = {
     "orx_pairwise_prefetch": [_vp, _T, _T, _vp, _vp, _vp, _i32, _i32, _i32, _vp],
     "orx_pairwise_fwd": [_vp, _i32, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _vp, _vp],
     "orx_pairwise_grad": [_vp, _i32, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
-    "orx_pairwise_grad_slots": [_vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i32, _f, _f, _f, _f, _vp, _vp, _vp,
-                                _vp, _vp],
     "orx_sparse_apply": [_vp, _T, _vp, _vp, _i32, _O, _vp],
     "orx_sparse_apply_strided": [_vp, _T, _vp, _i64, _vp, _i64, _i32, _O, _vp],
     "orx_gather_strided": [_vp, _vp, _i64, _i32, _vp, _i64, _i64, _vp, _i64, _vp, _vp],
@@ -90,7 +88,6 @@ SIGNATURES = {
                        _i32, _i32, _i32, _vp, _vp],
     "orx_owner_bucket_combined": [_vp, _vp, _i32, _i32, _i64, _i32, _vp, _vp, _vp, _vp],
     "orx_pairwise_grad_rows": [_vp, _i32, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _f, _f, _f, _f, _vp, _vp, _vp],
-    "orx_owner_bucket": [_vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp],
     "orx_pointwise_step": [_vp, _i32, _T, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _i32, _f, _f, _O, _vp, _vp],
     "orx_pointwise_fwd": [_vp, _i32, _T, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _i32, _vp, _vp],
     "orx_pointwise_grad": [_vp, _i32, _T, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _i32, _f, _f,

@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <initializer_list>
 #include <type_traits>
 
 #include "../../include/orx.h"
@@ -71,7 +72,7 @@ struct orx_ctx {
   cudaEvent_t* prof_ev;  // [prof_cap * ORX_PROF_EV]
   int32_t* bucket_cursor;  // owner-bucket scratch
   cudaStream_t side_stream;  // id upload + index build of the NEXT pairwise batch, beside the running step
-  cudaEvent_t side_ev[2];
+  cudaEvent_t side_ev;       // "ids are final" point of orx_pairwise_prefetch on the caller's ids stream
   cudaEvent_t pf_done[2], pf_free[2], stage_free[2];   // prefetched index k built / handed back; id staging f free
   int pf_free_valid[2], stage_free_valid[2];
   int pf_valid, pf_set, pf_next, pf_B, pf_mode;        // the one outstanding prefetched index and what it was built for
@@ -121,7 +122,7 @@ static inline int orx_current_sms() {
   return sms[dev] > 0 ? sms[dev] : 132;
 }
 
-int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim, bool full_staging);
+int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim);
 int orx_ensure_stage(orx_ctx* c, int64_t n_ints);
 
 // Runtime kind -> template argument: calls f(std::integral_constant<int, V>{}) for the V among Vs equal to v, and for the
@@ -140,6 +141,12 @@ template <typename F>
 static inline auto orx_dispatch_opt(int opt_kind, F&& f) {
   return orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE>(opt_kind, f);
 }
+
+// an orx_opt_kind
+static inline bool orx_opt_kind_ok(int kind) { return kind >= ORX_OPT_SGD && kind <= ORX_OPT_ADAM_DENSE; }
+// The host side of OrxOptSlots: every table carries the slot rows optimizer `kind` keeps -- s0 for every kind but SGD,
+// s1 for both Adams (ADAM_DENSE's sweep keeps m and v there).  Null tables are skipped.
+bool orx_opt_slots_ok(int kind, std::initializer_list<const orx_table_t*> tabs);
 
 // ---------------------------------------------------------------------------------------
 // device helpers
@@ -420,6 +427,17 @@ __device__ __forceinline__ void orx_block_partial(float loss, float l2, float* p
   }
 }
 
+// One (loss, l2) float partial per warp at partials[2 * warp], warp = the global warp index.
+__device__ __forceinline__ void orx_warp_partial(float loss, float l2, float* partials) {
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  loss = orx_group_sum<32>(loss);
+  l2 = orx_group_sum<32>(l2);
+  if ((threadIdx.x & 31) == 0) {
+    partials[2 * warp] = loss;
+    partials[2 * warp + 1] = l2;
+  }
+}
+
 // Deterministic (loss, l2) totals of n float pairs (loss, l2) for one 256-thread block: each thread sums a fixed stride
 // in float64, adds the squares of sq[0..nsq) to its l2 share (GMF weight), then a fixed-order tree.  Every thread of the
 // block calls it and gets the totals in *l / *q.
@@ -539,10 +557,17 @@ __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni)
 
 OrxOptDev orx_opt_to_dev(const orx_opt_t* o);
 int orx_launch_index_build_strided(orx_ctx* c, const int32_t* a, int64_t stride, int64_t rows, int32_t n,
-                                   const int32_t* n_dev, bool stage_all, cudaStream_t st);
+                                   bool stage_all, cudaStream_t st);
+// The tail arguments of a step over user / item / bias (item and bias may be null) with index sets hu / hi, the handle's
+// staging rows and optimizer o; every other field is zero (partials, loss_scale, counters, out4, GMF's W / gw: the
+// caller's).
+TailArgs orx_tail_args(const orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
+                       const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o);
+// ADAM_DENSE: Keras dense Adam over every row of user / item / bias (item and bias may be null), a row's summed gradient
+// taken from its side's index set (hu / hi) and staging rows.  Runs before the tail, which zeroes the staging rows.
+int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
+                           const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o, cudaStream_t st);
 int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st);
-int orx_launch_adam_sweep(orx_ctx* c, float* var, float* m, float* v, int64_t rows, int D, const OrxHash& h,
-                          const float* gstage, const OrxOptDev& o, cudaStream_t st);
 int orx_ensure_partials(orx_ctx* c, int need, cudaStream_t st);
 int orx_launch_reduce_partials(const float* partials, int n, float loss_scale, float* out4, cudaStream_t st);
 // index of n samples (a[t], b0[t]) or (a[t], b0[t], b1[t]); only samples whose ids are all in range are inserted

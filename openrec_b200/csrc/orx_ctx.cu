@@ -82,7 +82,7 @@ static int alloc_hash(OrxHash& t, int64_t lookups, int32_t* counter) {
 
 // Workspace is sized for B lookups on the user side and 2B on the item side; every lookup may be
 // staged (ADAM_DENSE stages all rows), so the staging buffers hold B resp. 2B rows of `dim` floats.
-int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim, bool /*full_staging*/) {
+int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim) {
   if (B <= c->cap_B && dim <= c->g_dim) return ORX_OK;
   int64_t nb = B > c->cap_B ? B : c->cap_B;
   int32_t nd = dim > c->g_dim ? dim : c->g_dim;
@@ -219,8 +219,8 @@ extern "C" int orx_destroy(orx_handle_t h) {
   orx_shard_ws_release(h);
   if (h->side_stream) {
     cudaStreamDestroy(h->side_stream);
+    cudaEventDestroy(h->side_ev);
     for (int i = 0; i < 2; ++i) {
-      cudaEventDestroy(h->side_ev[i]);
       cudaEventDestroy(h->pf_done[i]);
       cudaEventDestroy(h->pf_free[i]);
       cudaEventDestroy(h->stage_free[i]);
@@ -269,6 +269,13 @@ extern "C" int orx_stream_synchronize(orx_handle_t h, orx_stream_t s) {
   ORX_REQUIRE(h != nullptr, "null handle");
   ORX_CUDA(cudaStreamSynchronize((cudaStream_t)s));
   return ORX_OK;
+}
+
+bool orx_opt_slots_ok(int kind, std::initializer_list<const orx_table_t*> tabs) {
+  const bool s0 = kind != ORX_OPT_SGD, s1 = kind == ORX_OPT_ADAM_LAZY || kind == ORX_OPT_ADAM_DENSE;
+  for (const orx_table_t* t : tabs)
+    if (t && ((s0 && !t->s0) || (s1 && !t->s1))) return false;
+  return true;
 }
 
 OrxOptDev orx_opt_to_dev(const orx_opt_t* o) {

@@ -134,7 +134,7 @@ extern "C" int orx_censor(orx_handle_t h, float* tab, int64_t rows, int32_t dim,
   if (n == 0) return ORX_OK;
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
-  int rc = orx_ensure_workspace(h, n, h->g_dim > 0 ? h->g_dim : 1, false);
+  int rc = orx_ensure_workspace(h, n, h->g_dim > 0 ? h->g_dim : 1);
   if (rc) return rc;
   if ((rc = orx_next_epoch(h, st))) return rc;   // the dedup hash needs no clearing: a new epoch empties it
   int blocks = (n + 63) / 64;                 // 8 warps x 8 ids per block and iteration
@@ -165,12 +165,9 @@ extern "C" int orx_dense_apply(orx_handle_t h, float* var, float* s0, float* s1,
   int64_t blocks = (n + 255) / 256;
   if (blocks > (int64_t)h->num_sms * 16) blocks = (int64_t)h->num_sms * 16;
   cudaStream_t st = (cudaStream_t)s;
-  if (opt->kind < ORX_OPT_SGD || opt->kind > ORX_OPT_ADAM_DENSE) {
-    orx_set_error("unknown optimizer kind %d", opt->kind);
-    return ORX_ERR_INVALID;
-  }
-  if (opt->kind == ORX_OPT_ADAGRAD) ORX_REQUIRE(s0, "Adagrad needs s0");
-  if (opt->kind >= ORX_OPT_ADAM_LAZY) ORX_REQUIRE(s0 && s1, "Adam needs s0 and s1");
+  ORX_REQUIRE(orx_opt_kind_ok(opt->kind), "unknown optimizer kind");
+  const orx_table_t t = {var, s0, s1, n, 1};
+  ORX_REQUIRE(orx_opt_slots_ok(opt->kind, {&t}), "optimizer slot rows missing");
   // ADAM_DENSE runs as ADAM_LAZY: identical on a dense variable
   const int kind = opt->kind == ORX_OPT_ADAM_DENSE ? ORX_OPT_ADAM_LAZY : opt->kind;
   orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY>(kind, [&](auto O) {

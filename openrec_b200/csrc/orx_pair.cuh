@@ -37,19 +37,19 @@ __device__ __forceinline__ float4 sa_pcd(float s, float4 a, float c, float4 d) {
 // loss term = -log sigmoid(max(x,-30)), g = -(c_loss/B) sigmoid(-y) [x>=-30]  (pairwise_log_loss.py:19-32).
 // UCML: h = margin - ((-|u-p|^2+bp) - (-|u-n|^2+bn)), loss term = max(h,0), a = c_loss [h>=0] (ucml.py:29-39).
 template <int KIND>
-__device__ __forceinline__ void pair_score(float s1, float s2, float bp, float bn, const PairArgs& a,
-                                           float* loss_term, float* g) {
+__device__ __forceinline__ void pair_score(float s1, float s2, float bp, float bn, float margin, float c_loss,
+                                           float inv_B, float* loss_term, float* g) {
   if (KIND == ORX_PAIR_BPR) {
     const float x = (s1 + bp) - (s2 + bn);
     const float y = fmaxf(x, -30.f);
     float ls, sn;
     orx_logsig(y, &ls, &sn);
     *loss_term = -ls;
-    *g = (x >= -30.f) ? -(a.c_loss * a.inv_B) * sn : 0.f;
+    *g = (x >= -30.f) ? -(c_loss * inv_B) * sn : 0.f;
   } else {
-    const float h = a.margin - (((-s1) + bp) - ((-s2) + bn));
+    const float h = margin - (((-s1) + bp) - ((-s2) + bn));
     *loss_term = fmaxf(h, 0.f);
-    *g = (h >= 0.f) ? a.c_loss : 0.f;
+    *g = (h >= 0.f) ? c_loss : 0.f;
   }
 }
 

@@ -14,6 +14,7 @@
 //   3. k_pair_tail   : optimizer for the staged rows (once per unique row), staging re-zeroed,
 //                      hash cleared, deterministic loss reduction.
 #include <stdlib.h>
+#include <string.h>
 
 #include "orx_common.cuh"
 #include "orx_pair.cuh"
@@ -46,8 +47,7 @@ __global__ void k_index_build(OrxHash hu, OrxHash hi, const int32_t* __restrict_
 }
 
 __global__ void k_index_build_strided(OrxHash hu, const int32_t* __restrict__ a, int64_t stride, int64_t rows, int n,
-                                       const int32_t* __restrict__ n_dev, int stage_all, int32_t* bad) {
-  if (n_dev) n = min(n, *n_dev);   // count produced on the device (mailbox exchange): grid-stride over it
+                                       int stage_all, int32_t* bad) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const int32_t id = a[(int64_t)i * stride];
     if (id >= 0 && (int64_t)id < rows) orx_hash_insert(hu, id, stage_all);
@@ -56,13 +56,11 @@ __global__ void k_index_build_strided(OrxHash hu, const int32_t* __restrict__ a,
 }
 
 int orx_launch_index_build_strided(orx_ctx* c, const int32_t* a, int64_t stride, int64_t rows, int32_t n,
-                                   const int32_t* n_dev, bool stage_all, cudaStream_t st) {
+                                   bool stage_all, cudaStream_t st) {
   if (n <= 0) return ORX_OK;
   int rc = orx_next_epoch(c, st);
   if (rc) return rc;
-  int blocks = (n + 255) / 256;
-  if (n_dev && blocks > c->num_sms * 8) blocks = c->num_sms * 8;
-  k_index_build_strided<<<blocks, 256, 0, st>>>(c->hu, a, stride, rows, n, n_dev, stage_all ? 1 : 0, c->counters + 3);
+  k_index_build_strided<<<(n + 255) / 256, 256, 0, st>>>(c->hu, a, stride, rows, n, stage_all ? 1 : 0, c->counters + 3);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
@@ -210,7 +208,7 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
     s1 = orx_group_sum<G>(s1);
     s2 = orx_group_sum<G>(s2);
     float lt, g;
-    pair_score<KIND>(s1, s2, r.bp, r.bn, a, &lt, &g);
+    pair_score<KIND>(s1, s2, r.bp, r.bn, a.margin, a.c_loss, a.inv_B, &lt, &g);
     const bool v = r.fl & 1;
     if (!v) { lt = 0.f; g = 0.f; }
     if (gl == 0) loss_acc += lt;
@@ -334,7 +332,7 @@ __global__ void __launch_bounds__(256) k_pair_step_generic(const PairArgs a) {
     s2 = orx_group_sum<32>(s2);
     const float bp = a.Bv[pp], bn = a.Bv[nn];
     float lt, g;
-    pair_score<KIND>(s1, s2, bp, bn, a, &lt, &g);
+    pair_score<KIND>(s1, s2, bp, bn, a.margin, a.c_loss, a.inv_B, &lt, &g);
     if (lane == 0) loss_acc += lt;
     for (int d = lane; d < D; d += 32) {
       const float u = ur[d], p = pr[d], n = nr[d];
@@ -431,15 +429,32 @@ int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t s
   return ORX_OK;
 }
 
-int orx_launch_adam_sweep(orx_ctx* c, float* var, float* m, float* v, int64_t rows, int D, const OrxHash& h,
-                          const float* gstage, const OrxOptDev& o, cudaStream_t st) {
-  int64_t blocks = (rows + 7) / 8;
-  const int64_t cap = (int64_t)c->num_sms * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  k_adam_sweep<<<(int)blocks, 256, 0, st>>>(var, m, v, rows, D, h, gstage, o);
-  ORX_LAUNCH_CHECK();
+int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
+                           const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o, cudaStream_t st) {
+  struct { const orx_table_t* t; int D; const OrxHash* h; const float* g; } sw[3] = {
+      {user, user->dim, &hu, c->gu}, {item, user->dim, &hi, c->gi}, {bias, 1, &hi, c->gb}};
+  for (const auto& s : sw) {
+    if (!s.t) continue;
+    int64_t blocks = (s.t->rows + 7) / 8;
+    const int64_t cap = (int64_t)c->num_sms * 16;
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) blocks = 1;
+    k_adam_sweep<<<(int)blocks, 256, 0, st>>>(s.t->var, s.t->s0, s.t->s1, s.t->rows, s.D, *s.h, s.g, o);
+    ORX_LAUNCH_CHECK();
+  }
   return ORX_OK;
+}
+
+TailArgs orx_tail_args(const orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
+                       const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o) {
+  TailArgs ta;
+  memset(&ta, 0, sizeof(ta));
+  ta.U = user->var; ta.Us0 = user->s0; ta.Us1 = user->s1;
+  if (item) { ta.I = item->var; ta.Is0 = item->s0; ta.Is1 = item->s1; }
+  if (bias) { ta.Bv = bias->var; ta.Bs0 = bias->s0; ta.Bs1 = bias->s1; }
+  ta.D = user->dim; ta.opt = o; ta.hu = hu; ta.hi = hi;
+  ta.gu = c->gu; ta.gi = c->gi; ta.gb = c->gb;
+  return ta;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -485,9 +500,7 @@ static int check_tables(const orx_table_t* user, const orx_table_t* item, const 
   ORX_REQUIRE(bias->dim == 1 && bias->rows == item->rows, "item_bias must be [item.rows, 1]");
   ORX_REQUIRE(user->rows > 0 && item->rows > 0 && user->rows <= 0x7fffffffLL && item->rows <= 0x7fffffffLL,
               "row counts must fit int32 ids");
-  if (opt_kind != ORX_OPT_SGD) ORX_REQUIRE(user->s0 && item->s0 && bias->s0, "optimizer slot s0 missing");
-  if (opt_kind == ORX_OPT_ADAM_LAZY || opt_kind == ORX_OPT_ADAM_DENSE)
-    ORX_REQUIRE(user->s1 && item->s1 && bias->s1, "optimizer slot s1 missing");
+  ORX_REQUIRE(orx_opt_slots_ok(opt_kind, {user, item, bias}), "optimizer slot rows missing");
   return ORX_OK;
 }
 
@@ -500,8 +513,8 @@ static int check_tables(const orx_table_t* user, const orx_table_t* item, const 
 static int side_stream_ensure(orx_ctx* c) {
   if (c->side_stream) return ORX_OK;
   ORX_CUDA(cudaStreamCreateWithFlags(&c->side_stream, cudaStreamNonBlocking));
+  ORX_CUDA(cudaEventCreateWithFlags(&c->side_ev, cudaEventDisableTiming));
   for (int i = 0; i < 2; ++i) {
-    ORX_CUDA(cudaEventCreateWithFlags(&c->side_ev[i], cudaEventDisableTiming));
     ORX_CUDA(cudaEventCreateWithFlags(&c->pf_done[i], cudaEventDisableTiming));
     ORX_CUDA(cudaEventCreateWithFlags(&c->pf_free[i], cudaEventDisableTiming));
     ORX_CUDA(cudaEventCreateWithFlags(&c->stage_free[i], cudaEventDisableTiming));
@@ -546,16 +559,16 @@ extern "C" int orx_pairwise_prefetch(orx_handle_t h, const orx_table_t* user, co
                                      const int32_t* pid, const int32_t* nid, int32_t B, int32_t opt_kind, int32_t ids_ready,
                                      orx_stream_t ids_stream) {
   ORX_REQUIRE(h != nullptr && user && item && uid && pid && nid && B > 0, "bad arguments");
-  ORX_REQUIRE(opt_kind >= ORX_OPT_SGD && opt_kind <= ORX_OPT_ADAM_DENSE, "unknown optimizer kind");
+  ORX_REQUIRE(orx_opt_kind_ok(opt_kind), "unknown optimizer kind");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t is = (cudaStream_t)ids_stream;
-  int rc = orx_ensure_workspace(h, B, user->dim, false);
+  int rc = orx_ensure_workspace(h, B, user->dim);
   if (rc) return rc;
   if ((rc = side_stream_ensure(h))) return rc;
   if ((rc = prefetch_drop(h, is))) return rc;
   if (!ids_ready) {   // the ids are final once everything queued on ids_stream so far has run
-    ORX_CUDA(cudaEventRecord(h->side_ev[0], is));
-    ORX_CUDA(cudaStreamWaitEvent(h->side_stream, h->side_ev[0], 0));
+    ORX_CUDA(cudaEventRecord(h->side_ev, is));
+    ORX_CUDA(cudaStreamWaitEvent(h->side_stream, h->side_ev, 0));
   }
   return prefetch_issue(h, uid, pid, nid, B, user->rows, item->rows, opt_kind == ORX_OPT_ADAM_DENSE ? 1 : 0);
 }
@@ -566,12 +579,12 @@ static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, con
                               cudaStream_t st) {
   ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
   ORX_REQUIRE(opt != nullptr && out4 != nullptr, "null opt/out");
-  ORX_REQUIRE(opt->kind >= ORX_OPT_SGD && opt->kind <= ORX_OPT_ADAM_DENSE, "unknown optimizer kind");
+  ORX_REQUIRE(orx_opt_kind_ok(opt->kind), "unknown optimizer kind");
   ORX_REQUIRE(B > 0 && uid && pid && nid, "empty batch or null ids");
   int rc = check_tables(user, item, bias, opt->kind);
   if (rc) return rc;
   const int D = user->dim;
-  if ((rc = orx_ensure_workspace(c, B, D, opt->kind == ORX_OPT_ADAM_DENSE))) return rc;
+  if ((rc = orx_ensure_workspace(c, B, D))) return rc;
   const bool dense = opt->kind == ORX_OPT_ADAM_DENSE;
   PairArgs pa;
   pa.U = user->var; pa.Us0 = user->s0; pa.Us1 = user->s1;
@@ -611,21 +624,11 @@ static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, con
   if (rc) return rc;
   orx_log_dispatch(c, ORX_OP_PAIRWISE_STEP, variant, kind, opt->kind, B, D, minb, set);
   orx_prof_mark(c, 2, st);
-  if (dense) {
-    if ((rc = orx_launch_adam_sweep(c, user->var, user->s0, user->s1, user->rows, D, HU, c->gu, pa.opt, st))) return rc;
-    if ((rc = orx_launch_adam_sweep(c, item->var, item->s0, item->s1, item->rows, D, HI, c->gi, pa.opt, st))) return rc;
-    if ((rc = orx_launch_adam_sweep(c, bias->var, bias->s0, bias->s1, bias->rows, 1, HI, c->gb, pa.opt, st))) return rc;
-  }
-  TailArgs ta;
-  ta.U = user->var; ta.Us0 = user->s0; ta.Us1 = user->s1;
-  ta.I = item->var; ta.Is0 = item->s0; ta.Is1 = item->s1;
-  ta.Bv = bias->var; ta.Bs0 = bias->s0; ta.Bs1 = bias->s1;
-  ta.D = D; ta.opt = pa.opt; ta.hu = HU; ta.hi = HI;
-  ta.gu = c->gu; ta.gi = c->gi; ta.gb = c->gb;
+  if (dense && (rc = orx_launch_adam_sweeps(c, user, item, bias, HU, HI, pa.opt, st))) return rc;
+  TailArgs ta = orx_tail_args(c, user, item, bias, HU, HI, pa.opt);
   ta.partials = c->partials; ta.n_partials = n_partials;
   ta.loss_scale = (kind == ORX_PAIR_BPR) ? pa.inv_B : 1.0f;
   ta.counters = ctr; ta.out4 = out4;
-  ta.W = ta.Ws0 = ta.Ws1 = ta.gw = nullptr; ta.c_l2 = c_l2;
   rc = orx_launch_tail(c, ta, opt->kind, st);
   if (set) {   // the prefetch set is free again once this tail has run
     ORX_CUDA(cudaEventRecord(c->pf_free[set - 1], st));
@@ -659,7 +662,7 @@ extern "C" int orx_pairwise_step_host(orx_handle_t h, int32_t kind, const orx_ta
   cudaStream_t st = (cudaStream_t)s;
   int rc = orx_ensure_stage(h, 3 * (int64_t)B);
   if (rc) return rc;
-  if ((rc = orx_ensure_workspace(h, B, user->dim, false))) return rc;
+  if ((rc = orx_ensure_workspace(h, B, user->dim))) return rc;
   if ((rc = side_stream_ensure(h))) return rc;
   if ((rc = prefetch_drop(h, st))) return rc;
   const uint32_t f = (h->stage_flip++) & 1u;
@@ -694,8 +697,9 @@ struct PairGradArgs {
   float margin, c_loss, c_l2, inv_B;
   float *d_user, *d_pos, *d_neg, *d_bp, *d_bn, *g_out;
   float* partials;
-  int slots;  // 1: outputs are indexed by the lookup's row (compact sharded form) instead of by triplet
-  int64_t ld;  // row stride of U / I / outputs in floats (0 => D); ld > D: item bias lives in column D of the row
+  // 0: table form, outputs indexed by triplet.  > D: row form (orx_pairwise_grad_rows) -- U = I = fetched rows of stride
+  // ld with the item bias in column D, outputs written to the lookup's own row of d_user = d_pos = d_neg.
+  int64_t ld;
 };
 
 template <int KIND>
@@ -703,13 +707,9 @@ __global__ void __launch_bounds__(256) k_pair_fwd_grad(const PairGradArgs a) {
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int D = a.D;
-  const int64_t ld = a.ld ? a.ld : D;
-  const bool bias_in_row = a.ld > D;
+  const bool row_form = a.ld != 0;
+  const int64_t ld = row_form ? a.ld : D;
   float loss_acc = 0.f, l2_acc = 0.f;
-  PairArgs sa;  // only the scalar fields pair_score reads
-  sa.margin = a.margin;
-  sa.c_loss = a.c_loss;
-  sa.inv_B = a.inv_B;
   for (int j = 0; j < 8; ++j) {
     const int t = warp * 8 + j;
     if (t >= a.B) break;
@@ -731,19 +731,19 @@ __global__ void __launch_bounds__(256) k_pair_fwd_grad(const PairGradArgs a) {
         }
         sq += u * u + p * p + n * n;
       }
-      bp = bias_in_row ? pr[D] : a.Bv[pp];
-      bn = bias_in_row ? nr[D] : a.Bv[nn];
+      bp = row_form ? pr[D] : a.Bv[pp];
+      bn = row_form ? nr[D] : a.Bv[nn];
     }
     l2_acc += sq;
     s1 = orx_group_sum<32>(s1);
     s2 = orx_group_sum<32>(s2);
-    if (ok) pair_score<KIND>(s1, s2, bp, bn, sa, &lt, &g);
+    if (ok) pair_score<KIND>(s1, s2, bp, bn, a.margin, a.c_loss, a.inv_B, &lt, &g);
     if (lane == 0) loss_acc += lt;
     if (a.d_user || a.d_pos || a.d_neg) {
       for (int d = lane; d < D; d += 32) {
         float gu = 0.f, gp = 0.f, gn = 0.f;
         if (ok) pair_grads1<KIND>(g, a.c_l2, ur[d], pr[d], nr[d], &gu, &gp, &gn);
-        if (a.slots) {
+        if (row_form) {
           if (ok) {
             a.d_user[(int64_t)uu * ld + d] = gu;
             a.d_pos[(int64_t)pp * ld + d] = gp;
@@ -759,18 +759,13 @@ __global__ void __launch_bounds__(256) k_pair_fwd_grad(const PairGradArgs a) {
     }
     if (lane == 0) {
       const float gbias = (KIND == ORX_PAIR_BPR) ? g : -g;
-      if (a.slots && bias_in_row) {
+      if (row_form) {
         if (ok) {   // column D = bias gradient (items) / 0 (users); remaining padding columns = 0
           for (int64_t c = D; c < ld; ++c) {
             a.d_user[(int64_t)uu * ld + c] = 0.f;
             a.d_pos[(int64_t)pp * ld + c] = c == D ? gbias : 0.f;
             a.d_neg[(int64_t)nn * ld + c] = c == D ? -gbias : 0.f;
           }
-        }
-      } else if (a.slots) {
-        if (ok) {
-          a.d_bp[pp] = gbias;
-          a.d_bn[nn] = -gbias;
         }
       } else {
         if (a.d_bp) a.d_bp[t] = gbias;
@@ -779,12 +774,7 @@ __global__ void __launch_bounds__(256) k_pair_fwd_grad(const PairGradArgs a) {
       if (a.g_out) a.g_out[t] = g;
     }
   }
-  loss_acc = orx_group_sum<32>(loss_acc);
-  l2_acc = orx_group_sum<32>(l2_acc);
-  if (lane == 0) {
-    a.partials[2 * warp] = loss_acc;
-    a.partials[2 * warp + 1] = l2_acc;
-  }
+  orx_warp_partial(loss_acc, l2_acc, a.partials);
 }
 
 __global__ void k_reduce_partials(const float* partials, int n, float loss_scale, float* out4) {
@@ -814,6 +804,21 @@ int orx_ensure_partials(orx_ctx* c, int need, cudaStream_t st) {
   return ORX_OK;
 }
 
+// k_pair_fwd_grad over the batch of `a` (kind already validated; one partial per warp of 8 triplets) and, when out4 is
+// given, its (loss, l2) reduced into out4: the loss scaled by inv_B for BPR (mean), summed for UCML.
+static int launch_pair_fwd_grad(orx_ctx* c, int kind, PairGradArgs a, float* out4, cudaStream_t st) {
+  const int nw = (a.B + 7) / 8, blocks = (nw + 7) / 8;
+  int rc = orx_ensure_partials(c, blocks * 8, st);
+  if (rc) return rc;
+  a.partials = c->partials;
+  orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {
+    k_pair_fwd_grad<decltype(K)::value><<<blocks, 256, 0, st>>>(a);
+  });
+  ORX_LAUNCH_CHECK();
+  if (!out4) return ORX_OK;
+  return orx_launch_reduce_partials(c->partials, blocks * 8, kind == ORX_PAIR_BPR ? a.inv_B : 1.f, out4, st);
+}
+
 static int pair_fwd_grad(orx_ctx* c, int kind, const orx_table_t* user, const orx_table_t* item,
                          const orx_table_t* bias, const int32_t* uid, const int32_t* pid, const int32_t* nid, int B,
                          float margin, float c_loss, float c_l2, float* d_user, float* d_pos, float* d_neg,
@@ -822,22 +827,13 @@ static int pair_fwd_grad(orx_ctx* c, int kind, const orx_table_t* user, const or
   ORX_REQUIRE(B > 0 && uid && pid && nid, "empty batch or null ids");
   int rc = check_tables(user, item, bias, ORX_OPT_SGD);
   if (rc) return rc;
-  const int nw = (B + 7) / 8, blocks = (nw + 7) / 8;
-  if ((rc = orx_ensure_partials(c, blocks * 8, st))) return rc;
-  PairGradArgs a;
+  PairGradArgs a = {};
   a.U = user->var; a.I = item->var; a.Bv = bias->var;
   a.rowsU = user->rows; a.rowsI = item->rows; a.D = user->dim;
   a.uid = uid; a.pid = pid; a.nid = nid; a.B = B;
   a.margin = margin; a.c_loss = c_loss; a.c_l2 = c_l2; a.inv_B = 1.0f / (float)B;
   a.d_user = d_user; a.d_pos = d_pos; a.d_neg = d_neg; a.d_bp = d_bp; a.d_bn = d_bn; a.g_out = g_out;
-  a.partials = c->partials; a.slots = 0; a.ld = 0;
-  if (kind == ORX_PAIR_BPR) k_pair_fwd_grad<ORX_PAIR_BPR><<<blocks, 256, 0, st>>>(a);
-  else k_pair_fwd_grad<ORX_PAIR_UCML><<<blocks, 256, 0, st>>>(a);
-  ORX_LAUNCH_CHECK();
-  if (out4) {
-    return orx_launch_reduce_partials(c->partials, blocks * 8, kind == ORX_PAIR_BPR ? a.inv_B : 1.f, out4, st);
-  }
-  return ORX_OK;
+  return launch_pair_fwd_grad(c, kind, a, out4, st);
 }
 
 extern "C" int orx_pairwise_fwd(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
@@ -859,33 +855,6 @@ extern "C" int orx_pairwise_grad(orx_handle_t h, int32_t kind, const orx_table_t
                        d_bp, d_bn, g_out, nullptr, (cudaStream_t)s);
 }
 
-extern "C" int orx_pairwise_grad_slots(orx_handle_t h, int32_t kind, const float* user_rows, const float* item_rows,
-                                       const float* bias_rows, int32_t dim, const int32_t* uslot, const int32_t* pslot,
-                                       const int32_t* nslot, int32_t B, float margin, float c_loss, float c_l2,
-                                       float inv_B, float* d_user_rows, float* d_item_rows, float* d_bias_rows,
-                                       float* out4, orx_stream_t s) {
-  ORX_REQUIRE(h != nullptr && user_rows && item_rows && bias_rows && uslot && pslot && nslot, "null input");
-  ORX_REQUIRE(d_user_rows && d_item_rows && d_bias_rows && out4, "null output");
-  ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
-  ORX_REQUIRE(B > 0 && dim > 0, "bad sizes");
-  ORX_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = (cudaStream_t)s;
-  const int nw = (B + 7) / 8, blocks = (nw + 7) / 8;
-  int rc = orx_ensure_partials(h, blocks * 8, st);
-  if (rc) return rc;
-  PairGradArgs a;
-  a.U = user_rows; a.I = item_rows; a.Bv = bias_rows;
-  a.rowsU = B; a.rowsI = 2 * (int64_t)B; a.D = dim;
-  a.uid = uslot; a.pid = pslot; a.nid = nslot; a.B = B;
-  a.margin = margin; a.c_loss = c_loss; a.c_l2 = c_l2; a.inv_B = inv_B;
-  a.d_user = d_user_rows; a.d_pos = d_item_rows; a.d_neg = d_item_rows; a.d_bp = d_bias_rows; a.d_bn = d_bias_rows;
-  a.g_out = nullptr; a.partials = h->partials; a.slots = 1; a.ld = 0;
-  if (kind == ORX_PAIR_BPR) k_pair_fwd_grad<ORX_PAIR_BPR><<<blocks, 256, 0, st>>>(a);
-  else k_pair_fwd_grad<ORX_PAIR_UCML><<<blocks, 256, 0, st>>>(a);
-  ORX_LAUNCH_CHECK();
-  return orx_launch_reduce_partials(h->partials, blocks * 8, kind == ORX_PAIR_BPR ? inv_B : 1.f, out4, st);
-}
-
 extern "C" int orx_pairwise_grad_rows(orx_handle_t h, int32_t kind, const float* rows, int64_t ld, int32_t dim,
                                       const int32_t* uslot, const int32_t* pslot, const int32_t* nslot, int32_t B,
                                       float margin, float c_loss, float c_l2, float inv_B, float* d_rows, float* out4,
@@ -894,19 +863,12 @@ extern "C" int orx_pairwise_grad_rows(orx_handle_t h, int32_t kind, const float*
   ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
   ORX_REQUIRE(B > 0 && dim > 0 && ld > dim, "bad sizes (ld must exceed dim: the bias lives in column dim)");
   ORX_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = (cudaStream_t)s;
-  const int nw = (B + 7) / 8, blocks = (nw + 7) / 8;
-  int rc = orx_ensure_partials(h, blocks * 8, st);
-  if (rc) return rc;
-  PairGradArgs a;
-  a.U = rows; a.I = rows; a.Bv = nullptr;
+  PairGradArgs a = {};
+  a.U = rows; a.I = rows;
   a.rowsU = 3 * (int64_t)B; a.rowsI = 3 * (int64_t)B; a.D = dim;
   a.uid = uslot; a.pid = pslot; a.nid = nslot; a.B = B;
   a.margin = margin; a.c_loss = c_loss; a.c_l2 = c_l2; a.inv_B = inv_B;
-  a.d_user = d_rows; a.d_pos = d_rows; a.d_neg = d_rows; a.d_bp = nullptr; a.d_bn = nullptr;
-  a.g_out = nullptr; a.partials = h->partials; a.slots = 1; a.ld = ld;
-  if (kind == ORX_PAIR_BPR) k_pair_fwd_grad<ORX_PAIR_BPR><<<blocks, 256, 0, st>>>(a);
-  else k_pair_fwd_grad<ORX_PAIR_UCML><<<blocks, 256, 0, st>>>(a);
-  ORX_LAUNCH_CHECK();
-  return orx_launch_reduce_partials(h->partials, blocks * 8, kind == ORX_PAIR_BPR ? inv_B : 1.f, out4, st);
+  a.d_user = d_rows; a.d_pos = d_rows; a.d_neg = d_rows;
+  a.ld = ld;
+  return launch_pair_fwd_grad(h, kind, a, out4, (cudaStream_t)s);
 }

@@ -173,12 +173,7 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
     __syncthreads();
     for (int e = threadIdx.x; e < D; e += blockDim.x) atomicAdd(a.gw + e, sgw[e]);
   }
-  loss_acc = orx_group_sum<32>(loss_acc);
-  l2_acc = orx_group_sum<32>(l2_acc);
-  if (lane == 0) {
-    a.partials[2 * warp] = loss_acc;
-    a.partials[2 * warp + 1] = l2_acc;
-  }
+  orx_warp_partial(loss_acc, l2_acc, a.partials);
 }
 
 // Any dim; MODE 0 = fused step, 1 = forward / explicit (un-fused) gradients.
@@ -254,12 +249,7 @@ __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
       }
     }
   }
-  loss_acc = orx_group_sum<32>(loss_acc);
-  l2_acc = orx_group_sum<32>(l2_acc);
-  if (lane == 0) {
-    a.partials[2 * warp] = loss_acc;
-    a.partials[2 * warp + 1] = l2_acc;
-  }
+  orx_warp_partial(loss_acc, l2_acc, a.partials);
 }
 
 // adds 0.5*sum(w^2) to out4[1] (gmf.py:31-32) and, for the explicit-gradient path, c_l2*w to d_w
@@ -308,9 +298,8 @@ static int check_point(int kind, const orx_table_t* user, const orx_table_t* ite
   ORX_REQUIRE(user->rows > 0 && item->rows > 0 && user->rows <= 0x7fffffffLL && item->rows <= 0x7fffffffLL,
               "row counts must fit int32 ids");
   if (kind == ORX_POINT_GMF) ORX_REQUIRE(w && w->var && w->dim == user->dim, "GMF needs w with dim == D");
-  const bool has0 = opt_kind != ORX_OPT_SGD, has1 = opt_kind == ORX_OPT_ADAM_LAZY || opt_kind == ORX_OPT_ADAM_DENSE;
-  if (has0) ORX_REQUIRE(user->s0 && item->s0 && bias->s0 && (kind != ORX_POINT_GMF || w->s0), "slot s0 missing");
-  if (has1) ORX_REQUIRE(user->s1 && item->s1 && bias->s1 && (kind != ORX_POINT_GMF || w->s1), "slot s1 missing");
+  ORX_REQUIRE(orx_opt_slots_ok(opt_kind, {user, item, bias, kind == ORX_POINT_GMF ? w : nullptr}),
+              "optimizer slot rows missing");
   return ORX_OK;
 }
 
@@ -338,7 +327,7 @@ extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_
                                   int32_t use_sigmoid, float c_loss, float c_l2, const orx_opt_t* opt, float* out4,
                                   orx_stream_t s) {
   ORX_REQUIRE(h != nullptr && opt != nullptr && out4 != nullptr, "null handle/opt/out");
-  ORX_REQUIRE(opt->kind >= ORX_OPT_SGD && opt->kind <= ORX_OPT_ADAM_DENSE, "unknown optimizer kind");
+  ORX_REQUIRE(orx_opt_kind_ok(opt->kind), "unknown optimizer kind");
   ORX_REQUIRE(B > 0 && uid && iid && label, "empty batch or null inputs");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
@@ -346,7 +335,7 @@ extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_
   if (rc) return rc;
   const int D = user->dim;
   const bool dense = opt->kind == ORX_OPT_ADAM_DENSE;
-  if ((rc = orx_ensure_workspace(h, B, D, dense))) return rc;
+  if ((rc = orx_ensure_workspace(h, B, D))) return rc;
   if ((rc = orx_ensure_partials(h, (B + 7) / 8 + 8, st))) return rc;
   if ((rc = orx_launch_index_build(h, uid, user->rows, iid, nullptr, item->rows, B, dense, st))) return rc;
   PointArgs pa;
@@ -361,23 +350,13 @@ extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_
   });
   if (rc) return rc;
   orx_log_dispatch(h, ORX_OP_POINTWISE_STEP, variant, kind, opt->kind, B, D, 0, 0);   // index set 0 always
-  if (dense) {
-    if ((rc = orx_launch_adam_sweep(h, user->var, user->s0, user->s1, user->rows, D, h->hu, h->gu, pa.opt, st))) return rc;
-    if ((rc = orx_launch_adam_sweep(h, item->var, item->s0, item->s1, item->rows, D, h->hi, h->gi, pa.opt, st))) return rc;
-    if ((rc = orx_launch_adam_sweep(h, item_bias->var, item_bias->s0, item_bias->s1, item_bias->rows, 1, h->hi, h->gb, pa.opt, st))) return rc;
-  }
-  TailArgs ta;
-  ta.U = user->var; ta.Us0 = user->s0; ta.Us1 = user->s1;
-  ta.I = item->var; ta.Is0 = item->s0; ta.Is1 = item->s1;
-  ta.Bv = item_bias->var; ta.Bs0 = item_bias->s0; ta.Bs1 = item_bias->s1;
-  ta.D = D; ta.opt = pa.opt; ta.hu = h->hu; ta.hi = h->hi;
-  ta.gu = h->gu; ta.gi = h->gi; ta.gb = h->gb;
+  if (dense && (rc = orx_launch_adam_sweeps(h, user, item, item_bias, h->hu, h->hi, pa.opt, st))) return rc;
+  TailArgs ta = orx_tail_args(h, user, item, item_bias, h->hu, h->hi, pa.opt);
   ta.partials = h->partials; ta.n_partials = n_partials;
   ta.loss_scale = (kind == ORX_POINT_GMF) ? pa.inv_B : 1.0f;
   ta.counters = h->counters; ta.out4 = out4;
-  ta.W = ta.Ws0 = ta.Ws1 = ta.gw = nullptr; ta.c_l2 = c_l2;
   if (kind == ORX_POINT_GMF) {
-    ta.W = w->var; ta.Ws0 = w->s0; ta.Ws1 = w->s1; ta.gw = h->gw;
+    ta.W = w->var; ta.Ws0 = w->s0; ta.Ws1 = w->s1; ta.gw = h->gw; ta.c_l2 = c_l2;
   }
   return orx_launch_tail(h, ta, opt->kind, st);
 }

@@ -456,8 +456,6 @@ __global__ void __launch_bounds__(256) k_sh_compute(ShardDev x, ShardWs w, ShCom
   const float* got = x.got[me];
   const float* gotb = x.gotb[me];
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
-  PairArgs sa;
-  sa.margin = a.margin; sa.c_loss = a.c_loss; sa.inv_B = a.inv_B;
   float loss_acc = 0.f, l2_acc = 0.f;
   for (int t0 = gwarp * TPW; t0 < T; t0 += nw * TPW) {
     // lanes 0..TPW-1: ids, positions, destinations and the user-row probe of triplet t0 + lane
@@ -527,7 +525,7 @@ __global__ void __launch_bounds__(256) k_sh_compute(ShardDev x, ShardWs w, ShCom
       s2 = orx_group_sum<32>(s2);
       const float bp = __shfl_sync(ORX_FULL, my_bp, k), bn = __shfl_sync(ORX_FULL, my_bn, k);
       float lt, g;
-      pair_score<KIND>(s1, s2, bp, bn, sa, &lt, &g);
+      pair_score<KIND>(s1, s2, bp, bn, a.margin, a.c_loss, a.inv_B, &lt, &g);
       if (lane == 0) loss_acc += lt;
       const int own = __shfl_sync(ORX_FULL, my_own, k);
       const int du = __shfl_sync(ORX_FULL, my_du, k);
@@ -558,12 +556,7 @@ __global__ void __launch_bounds__(256) k_sh_compute(ShardDev x, ShardWs w, ShCom
     }
   }
   orx_pdl_trigger();
-  loss_acc = orx_group_sum<32>(loss_acc);
-  l2_acc = orx_group_sum<32>(l2_acc);
-  if (lane == 0) {
-    a.partials[2 * gwarp] = loss_acc;
-    a.partials[2 * gwarp + 1] = l2_acc;
-  }
+  orx_warp_partial(loss_acc, l2_acc, a.partials);
   // The LAST block to finish reduces this rank's (loss, l2) partials, sends the pair to every rank and releases flag 3.
   sh_arrive(x, w.ctl + SH_C_DONE + 3, gridDim.x, 3, epoch, [&]() {
     double l, q;                                       // deterministic (fixed order, double) reduction of my partials
@@ -916,13 +909,12 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
   ORX_REQUIRE(phase_lo >= 0 && phase_hi <= 5 && phase_lo <= phase_hi, "bad phase range");
   ORX_REQUIRE(opt->kind == ORX_OPT_SGD || opt->kind == ORX_OPT_ADAGRAD || opt->kind == ORX_OPT_ADAM_LAZY,
               "the sharded step supports SGD, Adagrad and row-sparse Adam");
-  if (opt->kind != ORX_OPT_SGD) ORX_REQUIRE(user->s0 && item->s0 && item_bias->s0, "optimizer slot s0 missing");
-  if (opt->kind == ORX_OPT_ADAM_LAZY) ORX_REQUIRE(user->s1 && item->s1 && item_bias->s1, "optimizer slot s1 missing");
+  ORX_REQUIRE(orx_opt_slots_ok(opt->kind, {user, item, item_bias}), "optimizer slot rows missing");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
   // index hashes + staging: user side <= home_cap lookups, item side <= gin_cap lookups
   const int64_t need = x->home_cap > (x->gin_cap + 1) / 2 ? x->home_cap : (x->gin_cap + 1) / 2;
-  if ((rc = orx_ensure_workspace(h, need, x->dim, false))) return rc;
+  if ((rc = orx_ensure_workspace(h, need, x->dim))) return rc;
   if ((rc = shard_ws_ensure(h, x, st))) return rc;
   orx_shard_ws* S = (orx_shard_ws*)h->shard_ws;
   if (S->owner != x->flags) {        // another model on this handle (each has its own mailboxes): its steps start afresh
@@ -1033,13 +1025,7 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
       }
       case 5: {
         const int g = h->num_sms * 4;   // the grid of k_sparse_tail
-        TailArgs ta;
-        memset(&ta, 0, sizeof(ta));
-        ta.U = user->var; ta.Us0 = user->s0; ta.Us1 = user->s1;
-        ta.I = item->var; ta.Is0 = item->s0; ta.Is1 = item->s1;
-        ta.Bv = item_bias->var; ta.Bs0 = item_bias->s0; ta.Bs1 = item_bias->s1;
-        ta.D = x->dim; ta.opt = od; ta.hu = hu; ta.hi = hi;
-        ta.gu = h->gu; ta.gi = h->gi; ta.gb = h->gb;
+        TailArgs ta = orx_tail_args(h, user, item, item_bias, hu, hi, od);
         ta.counters = h->counters;   // [2]: the tail's block ticket
         ta.out4 = out4;
         sh_dispatch_opt(opt->kind, [&](auto O) {

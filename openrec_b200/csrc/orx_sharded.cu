@@ -1,13 +1,11 @@
 // orx_sharded.cu -- building blocks of the row-sharded (multi-GPU) step and of un-fused sparse applies:
-//   * orx_owner_bucket : counting-sort the lookups of a batch by owner rank (row r lives on rank r % R,
+//   * orx_owner_bucket_combined : counting-sort the lookups of a batch by owner rank (row r lives on rank r % R,
 //                        local row r / R) -> send order, per-owner counts, inverse permutation ("K9" bucket half)
 //   * orx_sparse_apply : Keras OptimizerV2 sparse apply of IndexedSlices (ids[n], values[n,D]) to one table:
 //                        dedup by row (batch hash), rows hit once are updated straight from their value row,
 //                        duplicated rows are summed in the staging buffer and updated once by the steps' staged-row
 //                        tail, k_sparse_tail ("K8").
 // The reference has no multi-device code (SURVEY 2.1); the partitioning follows SURVEY 8(e).
-#include <string.h>
-
 #include "orx_common.cuh"
 
 // ---------------------------------------------------------------------------------------
@@ -39,8 +37,7 @@ __global__ void k_owner_scan(const int32_t* counts, int R, int32_t* cursor) {
 // slot[i] = position of lookup i in the owner-sorted send order; send_local[slot] = local row on the owner.
 // Positions are reserved per BLOCK (shared-memory ranks, one global atomic per block and owner): with only R
 // cursors, one global atomic per lookup serialises (measured 158 us for 196k lookups at R = 2).
-// n_user / U: combined form -- lookups i >= n_user are item lookups whose local row is offset by the owner's
-// user-row count (n_user = n and U = 0 for the plain form).
+// Lookups i >= n_user are item lookups whose local row is offset by the owner's user-row count (U users in all).
 __global__ void __launch_bounds__(256) k_owner_scatter(const int32_t* __restrict__ ids, int n, int n_user, int64_t U,
                                                        int R, int32_t* cursor, int32_t* __restrict__ send_local,
                                                        int32_t* __restrict__ slot) {
@@ -90,28 +87,6 @@ extern "C" int orx_owner_bucket_combined(orx_handle_t h, const int32_t* ids, int
   return ORX_OK;
 }
 
-extern "C" int orx_owner_bucket(orx_handle_t h, const int32_t* ids, int32_t n, int32_t world, int32_t* counts,
-                                int32_t* send_local, int32_t* slot, orx_stream_t s) {
-  ORX_REQUIRE(h != nullptr && ids && counts && send_local && slot, "null pointer");
-  ORX_REQUIRE(n >= 0 && world >= 1 && world <= 1024, "bad sizes");
-  ORX_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = (cudaStream_t)s;
-  ORX_CUDA(cudaMemsetAsync(counts, 0, sizeof(int32_t) * world, st));
-  if (n == 0) return ORX_OK;
-  if (!h->bucket_cursor) ORX_CUDA(cudaMalloc(&h->bucket_cursor, sizeof(int32_t) * 1024));
-  int32_t* cursor = h->bucket_cursor;
-  int blocks = (n + 255) / 256;
-  if (blocks > h->num_sms * 4) blocks = h->num_sms * 4;
-  k_owner_hist<<<blocks, 256, sizeof(int32_t) * world, st>>>(ids, n, world, counts);
-  ORX_LAUNCH_CHECK();
-  k_owner_scan<<<1, 32, 0, st>>>(counts, world, cursor);
-  ORX_LAUNCH_CHECK();
-  k_owner_scatter<<<(n + 255) / 256, 256, 2 * sizeof(int32_t) * world, st>>>(ids, n, n, 0, world, cursor, send_local,
-                                                                             slot);
-  ORX_LAUNCH_CHECK();
-  return ORX_OK;
-}
-
 // ---------------------------------------------------------------------------------------
 // generic sparse apply
 // ---------------------------------------------------------------------------------------
@@ -119,11 +94,9 @@ template <int OPT>
 __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, float* s1, int64_t rows, int D,
                                                       const int32_t* __restrict__ ids, int64_t id_stride,
                                                       const float* __restrict__ vals, int64_t val_ld, int n,
-                                                      const int32_t* __restrict__ n_dev, OrxHash hsh, float* gstage,
-                                                      OrxOptDev o) {
+                                                      OrxHash hsh, float* gstage, OrxOptDev o) {
   typedef OrxOptSlots<OPT> SL;
   const int lane = threadIdx.x & 31;
-  if (n_dev) n = min(n, *n_dev);   // count produced on the device: the grid is capped and strides over it
   const int nw = (gridDim.x * blockDim.x) >> 5;
   // a warp takes 8 consecutive pairs per iteration; lanes 0..7 load the ids and probe the hash in parallel
   for (int b0 = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 8; b0 < n; b0 += nw * 8) {
@@ -167,57 +140,49 @@ __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, flo
 }
 
 static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
-                             const float* values, int64_t value_ld, int32_t n, const int32_t* n_dev,
-                             const orx_opt_t* opt, orx_stream_t s);
+                             const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt, orx_stream_t s);
 
 extern "C" int orx_sparse_apply(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, const float* values,
                                 int32_t n, const orx_opt_t* opt, orx_stream_t s) {
   ORX_REQUIRE(tab != nullptr, "null table");
-  return sparse_apply_impl(h, tab, ids, 1, values, tab->dim, n, nullptr, opt, s);
+  return sparse_apply_impl(h, tab, ids, 1, values, tab->dim, n, opt, s);
 }
 
 extern "C" int orx_sparse_apply_strided(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
                                         const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt,
                                         orx_stream_t s) {
   ORX_REQUIRE(tab != nullptr && id_stride >= 1 && value_ld >= tab->dim, "bad strides");
-  return sparse_apply_impl(h, tab, ids, id_stride, values, value_ld, n, nullptr, opt, s);
+  return sparse_apply_impl(h, tab, ids, id_stride, values, value_ld, n, opt, s);
 }
 
 static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
-                             const float* values, int64_t value_ld, int32_t n, const int32_t* n_dev,
-                             const orx_opt_t* opt, orx_stream_t s) {
+                             const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt, orx_stream_t s) {
   ORX_REQUIRE(h != nullptr && tab && tab->var && opt, "null pointer");
   ORX_REQUIRE(n >= 0 && tab->rows > 0 && tab->dim > 0, "bad sizes");
-  ORX_REQUIRE(opt->kind >= ORX_OPT_SGD && opt->kind <= ORX_OPT_ADAM_DENSE, "unknown optimizer kind");
-  if (opt->kind != ORX_OPT_SGD) ORX_REQUIRE(tab->s0, "optimizer slot s0 missing");
-  if (opt->kind >= ORX_OPT_ADAM_LAZY) ORX_REQUIRE(tab->s1, "optimizer slot s1 missing");
+  ORX_REQUIRE(orx_opt_kind_ok(opt->kind), "unknown optimizer kind");
+  ORX_REQUIRE(orx_opt_slots_ok(opt->kind, {tab}), "optimizer slot rows missing");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
   const bool dense = opt->kind == ORX_OPT_ADAM_DENSE;
   if (n == 0 && !dense) return ORX_OK;
   ORX_REQUIRE(n == 0 || (ids && values), "null ids/values");
   const int D = tab->dim;
-  int rc = orx_ensure_workspace(h, n > 0 ? n : 1, D, dense);
+  int rc = orx_ensure_workspace(h, n > 0 ? n : 1, D);
   if (rc) return rc;
   const OrxOptDev o = orx_opt_to_dev(opt);
   // the user-side hash / staging pair serves as "the" table here
   if (n > 0) {
-    if ((rc = orx_launch_index_build_strided(h, ids, id_stride, tab->rows, n, n_dev, dense, st))) return rc;
-    int blocks = (n + 63) / 64;   // 8 warps x 8 pairs per block and iteration
-    if (n_dev && blocks > h->num_sms * 8) blocks = h->num_sms * 8;
+    if ((rc = orx_launch_index_build_strided(h, ids, id_stride, tab->rows, n, dense, st))) return rc;
+    const int blocks = (n + 63) / 64;   // 8 warps x 8 pairs per block and iteration
     orx_dispatch_opt(opt->kind, [&](auto O) {
       k_sparse_apply<decltype(O)::value><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride,
-                                                                 values, value_ld, n, n_dev, h->hu, h->gu, o);
+                                                                 values, value_ld, n, h->hu, h->gu, o);
     });
     ORX_LAUNCH_CHECK();
   }
-  if (dense)
-    if ((rc = orx_launch_adam_sweep(h, tab->var, tab->s0, tab->s1, tab->rows, D, h->hu, h->gu, o, st))) return rc;
+  if (dense && (rc = orx_launch_adam_sweeps(h, tab, nullptr, nullptr, h->hu, h->hi, o, st))) return rc;
   // staged rows: the shared tail with no item side and no loss
-  TailArgs ta;
-  memset(&ta, 0, sizeof(ta));
-  ta.U = tab->var; ta.Us0 = tab->s0; ta.Us1 = tab->s1;
-  ta.D = D; ta.opt = o; ta.hu = h->hu; ta.gu = h->gu;
+  TailArgs ta = orx_tail_args(h, tab, nullptr, nullptr, h->hu, h->hi, o);
   ta.counters = h->counters;
   return orx_launch_tail(h, ta, opt->kind, st);
 }

@@ -158,29 +158,11 @@ class Engine:
                                               _ptr(d_pos), _ptr(d_neg), _ptr(d_bp), _ptr(d_bn), _ptr(g_out),
                                               self.stream()), "orx_pairwise_grad")
 
-    def pairwise_grad_slots(self, kind, user_rows, item_rows, bias_rows, uslot, pslot, nslot, inv_B, d_user, d_item,
-                            d_bias, out4, margin=0.5, c_loss=1.0, c_l2=1.0):
-        _lib.check(self.lib.orx_pairwise_grad_slots(self.h, kind, _ptr(user_rows), _ptr(item_rows), _ptr(bias_rows),
-                                                    user_rows.shape[1], _ptr(uslot), _ptr(pslot), _ptr(nslot),
-                                                    uslot.numel(), margin, c_loss, c_l2, inv_B, _ptr(d_user),
-                                                    _ptr(d_item), _ptr(d_bias), _ptr(out4), self.stream()),
-                   "orx_pairwise_grad_slots")
-
     # ---- un-fused sparse apply / multi-GPU building blocks ------------------------------
     def sparse_apply(self, tab, ids, values, o):
         n = 0 if ids is None else ids.numel()
         _lib.check(self.lib.orx_sparse_apply(self.h, C.byref(tab), _ptr(ids), _ptr(values), n, C.byref(o),
                                              self.stream()), "orx_sparse_apply")
-
-    def owner_bucket(self, ids, world):
-        """-> (counts[world], send_local[n], slot[n]) device int32 tensors."""
-        n = ids.numel()
-        counts = torch.empty(world, dtype=torch.int32, device=ids.device)
-        send_local = torch.empty(n, dtype=torch.int32, device=ids.device)
-        slot = torch.empty(n, dtype=torch.int32, device=ids.device)
-        _lib.check(self.lib.orx_owner_bucket(self.h, _ptr(ids), n, world, _ptr(counts), _ptr(send_local), _ptr(slot),
-                                             self.stream()), "orx_owner_bucket")
-        return counts, send_local, slot
 
     def sparse_apply_strided(self, tab, ids2d, col, values3d, o):
         """ids = ids2d[:, col] (int32 [n, F]); value rows = values3d[:, col, :] ([n, F, D]) -- no copies."""

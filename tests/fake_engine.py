@@ -41,15 +41,6 @@ class FakeEngine:
     def censor(self, tab, ids, min_norm=0.1):
         O.censor(tab.numpy(), ids.numpy().reshape(-1), min_norm)
 
-    def owner_bucket(self, ids, world):
-        a = ids.numpy()
-        owner = a % world
-        order = np.argsort(owner, kind="stable")
-        slot = np.empty(len(a), dtype=np.int32)
-        slot[order] = np.arange(len(a), dtype=np.int32)
-        return (torch.from_numpy(np.bincount(owner, minlength=world).astype(np.int32)),
-                torch.from_numpy((a // world)[order].astype(np.int32)), torch.from_numpy(slot))
-
     def owner_bucket_combined(self, ids, n_user, total_users, world):
         a = ids.numpy()
         owner = a % world
@@ -79,23 +70,6 @@ class FakeEngine:
         d[gr["user"][0], :dim] = gr["user"][1]
         d[gr["item"][0], :dim] = gr["item"][1]
         d[gr["bias"][0], dim] = gr["bias"][1].reshape(-1)
-        out4[0], out4[1] = float(loss), float(l2)
-
-    def pairwise_grad_slots(self, kind, user_rows, item_rows, bias_rows, uslot, pslot, nslot, inv_B, d_user, d_item,
-                            d_bias, out4, margin=0.5, c_loss=1.0, c_l2=1.0):
-        u, i, b = (t.numpy().astype(np.float64) for t in (user_rows, item_rows, bias_rows))
-        us, ps, ns = (t.numpy() for t in (uslot, pslot, nslot))
-        B = len(us)
-        if kind == 0:
-            loss, l2 = O.bpr_forward(u, i, b, us, ps, ns)
-            gr = O.bpr_grads(u, i, b, us, ps, ns, c_loss * B * inv_B, c_l2)
-            loss = loss * B * inv_B
-        else:
-            loss, l2 = O.ucml_forward(u, i, b, us, ps, ns, margin)
-            gr = O.ucml_grads(u, i, b, us, ps, ns, margin, c_loss, c_l2)
-        d_user.numpy()[gr["user"][0]] = gr["user"][1]
-        d_item.numpy()[gr["item"][0]] = gr["item"][1]
-        d_bias.numpy()[gr["bias"][0]] = gr["bias"][1].reshape(-1, 1)
         out4[0], out4[1] = float(loss), float(l2)
 
     def sparse_apply(self, tab, ids, values, o):

@@ -926,10 +926,13 @@ def test_sparse_apply(eng, optname, D, rows, n):
 
 
 def test_owner_bucket(eng):
+    """Owner bucketing of plain lookups: orx_owner_bucket_combined with every lookup a user lookup (n_user = n) puts row r
+    on rank r % world at local row r / world."""
     rng = np.random.default_rng(8)
     for world in (2, 3, 8):
         ids = rng.integers(0, 100000, 5000).astype(np.int32)
-        counts, send_local, slot = (t.cpu().numpy() for t in eng.owner_bucket(dev(ids, torch.int32), world))
+        counts, send_local, slot = (t.cpu().numpy() for t in eng.owner_bucket_combined(dev(ids, torch.int32), len(ids),
+                                                                                        100000, world))
         assert np.array_equal(counts, np.bincount(ids % world, minlength=world))
         assert sorted(slot.tolist()) == list(range(len(ids)))            # a permutation
         assert np.array_equal(send_local[slot], ids // world)            # lookup i sits at slot[i]
@@ -938,35 +941,37 @@ def test_owner_bucket(eng):
 
 
 @pytest.mark.parametrize("kind", ["bpr", "ucml"])
-def test_pairwise_grad_slots(eng, kind):
+def test_pairwise_grad_rows(eng, kind):
+    """Row-form gradients (the compact form of the NCCL sharded step): every lookup of the batch has its own fetched row
+    of width D+4 (item bias in column D); the gradient overwrites the lookup's row of d_rows, padding included."""
     from openrec_b200 import native as N
     rng = np.random.default_rng(9)
     B, D, R = 300, 64, 4
     sc = 0.05 if kind == "bpr" else 0.4
-    urows, irows, brows = rng.uniform(-sc, sc, (B, D)), rng.uniform(-sc, sc, (2 * B, D)), rng.uniform(-sc, sc, (2 * B, 1))
-    us, ps, ns = rng.permutation(B).astype(np.int32), rng.permutation(2 * B)[:B].astype(np.int32), None
-    rest = np.setdiff1d(np.arange(2 * B), ps)
-    ns = rng.permutation(rest).astype(np.int32)
-    tu, ti, tb = dev(urows), dev(irows), dev(brows)
-    u64, i64, b64 = (t.cpu().numpy().astype(np.float64) for t in (tu, ti, tb))
-    du, di, db = torch.zeros_like(tu), torch.zeros_like(ti), torch.zeros_like(tb)
+    rows = np.zeros((3 * B, D + 4))
+    rows[:, :D + 1] = rng.uniform(-sc, sc, (3 * B, D + 1))
+    perm = rng.permutation(3 * B).astype(np.int32)
+    us, ps, ns = perm[:B], perm[B:2 * B], perm[2 * B:]
+    trows = dev(rows)
+    r64 = trows.cpu().numpy().astype(np.float64)
+    d_rows = torch.full_like(trows, 7.0)       # every touched entry must be overwritten (incl. the padding)
     out4 = torch.zeros(4, device="cuda")
     k = N.ORX_PAIR_BPR if kind == "bpr" else N.ORX_PAIR_UCML
-    eng.pairwise_grad_slots(k, tu, ti, tb, dev(us, torch.int32), dev(ps, torch.int32), dev(ns, torch.int32),
-                            1.0 / (B * R), du, di, db, out4, 0.5, 1.0, 1.0)
+    eng.pairwise_grad_rows(k, trows, D, dev(us, torch.int32), dev(ps, torch.int32), dev(ns, torch.int32),
+                           1.0 / (B * R), d_rows, out4, 0.5, 1.0, 1.0)
+    emb, bias = r64[:, :D], r64[:, D:D + 1]
     if kind == "bpr":
-        loss, l2 = O.bpr_forward(u64, i64, b64, us, ps, ns)
-        gr = O.bpr_grads(u64, i64, b64, us, ps, ns, 1.0 / R, 1.0)
+        loss, l2 = O.bpr_forward(emb, emb, bias, us, ps, ns)
+        gr = O.bpr_grads(emb, emb, bias, us, ps, ns, 1.0 / R, 1.0)
         loss = loss / R
     else:
-        loss, l2 = O.ucml_forward(u64, i64, b64, us, ps, ns, 0.5)
-        gr = O.ucml_grads(u64, i64, b64, us, ps, ns, 0.5)
+        loss, l2 = O.ucml_forward(emb, emb, bias, us, ps, ns, 0.5)
+        gr = O.ucml_grads(emb, emb, bias, us, ps, ns, 0.5)
     close(out4[0], loss, rtol=2e-5), close(out4[1], l2, rtol=2e-5)
-    ref_u, ref_i, ref_b = np.zeros_like(u64), np.zeros_like(i64), np.zeros_like(b64)
-    ref_u[gr["user"][0]], ref_i[gr["item"][0]] = gr["user"][1], gr["item"][1]
-    ref_b[gr["bias"][0]] = gr["bias"][1].reshape(-1, 1)
-    tol = 1e-4 if kind == "ucml" else ATOL
-    close(du, ref_u, atol=tol), close(di, ref_i, atol=tol), close(db, ref_b, atol=tol)
+    ref = np.zeros_like(r64)
+    ref[gr["user"][0], :D], ref[gr["item"][0], :D] = gr["user"][1], gr["item"][1]
+    ref[gr["bias"][0], D] = gr["bias"][1].reshape(-1)
+    close(d_rows, ref, atol=1e-4 if kind == "ucml" else ATOL)
 
 
 def test_owner_bucket_combined_and_grad_rows(eng):
@@ -1004,3 +1009,131 @@ def test_owner_bucket_combined_and_grad_rows(eng):
     ref[gr["bias"][0], D] = gr["bias"][1].reshape(-1)
     close(out4[0], loss / R, rtol=2e-5), close(out4[1], l2, rtol=2e-5)
     close(d_rows, ref)
+
+
+# ---- optimizer kind and slot rows: every entry point that applies an optimizer checks them before it launches -------
+# An optimizer needs slot s0 unless it is SGD, and s1 when it is an Adam (ADAM_DENSE keeps m and v there too).
+MISSING_SLOT = [(opt, j) for opt in (1, 2, 3) for j in (0, 1) if j == 0 or opt >= 2]
+BAD_KINDS = (-1, 4)
+
+
+def _rejected(call):
+    with pytest.raises(RuntimeError, match=r"\(status -1\)"):    # ORX_ERR_INVALID
+        call()
+
+
+class _Tabs:
+    """Tables (var, s0, s1) of the given shapes; .t(i, opt, drop) is table i with the slots `opt` needs minus `drop`."""
+
+    def __init__(self, rng, *shapes):
+        self.v = [tuple(dev(rng.uniform(0.1, 0.3, s)) for _ in range(3)) for s in shapes]
+        self.before = [tuple(x.clone() for x in t) for t in self.v]
+
+    def t(self, i, opt, drop=None):
+        from openrec_b200 import native as N
+        var, s0, s1 = self.v[i]
+        keep0 = opt != 0 and drop != (i, 0)
+        keep1 = opt in (2, 3) and drop != (i, 1)
+        return N.table(var, s0 if keep0 else None, s1 if keep1 else None)
+
+    def unchanged(self):
+        return all(torch.equal(a, b) for t, u in zip(self.v, self.before) for a, b in zip(t, u))
+
+
+@pytest.mark.parametrize("entry", ["pairwise_step", "pairwise_prefetch", "pointwise_step", "sparse_apply",
+                                   "sparse_apply_strided", "dense_apply", "shard_step"])
+def test_optimizer_kind_and_slots_checked(eng, entry):
+    """A table missing a slot row its optimizer keeps, or an unknown optimizer kind, is rejected with ORX_ERR_INVALID
+    and nothing is written; SGD with no slot rows is accepted."""
+    from openrec_b200 import native as N
+    rng = np.random.default_rng(seed_of("slots", entry))
+    U, I, D, B = 40, 50, 32, 64
+    ids = lambda n: dev(rng.integers(0, n, B), torch.int32)
+    uid, pid, nid = ids(U), ids(I), ids(I)
+    out4 = torch.zeros(4, device="cuda")
+    if entry == "shard_step":
+        from openrec_b200.sharded import LoopbackGroup
+        g = LoopbackGroup(1, U, I, D, B, kind=0, opt_kind=2, lr=0.05, seed=1)
+        try:
+            m = g.ranks[0]
+            full = (m._tabs, m.opt_kind)
+            vars_ = [m.user, m.item, m.bias] + [x for x in m.user_slots + m.item_slots + m.bias_slots]
+            before = [x.clone() for x in vars_]
+
+            def shard(opt, drop=None):
+                def tab(i, var, slots):
+                    keep0 = opt != 0 and drop != (i, 0)
+                    keep1 = opt in (2, 3) and drop != (i, 1)
+                    return N.table(var, slots[0] if keep0 else None, slots[1] if keep1 else None)
+                m._tabs = (tab(0, m.user, m.user_slots), tab(1, m.item, m.item_slots), tab(2, m.bias, m.bias_slots))
+                m.opt_kind = opt
+                m.iterations = 1
+                m._call(uid, pid, nid, 1.0, 1.0, 0, 5)
+
+            for opt, j in MISSING_SLOT:
+                if opt == 3:
+                    continue                # the sharded step rejects ADAM_DENSE whatever the slots
+                for i in range(3):
+                    _rejected(lambda: shard(opt, (i, j)))
+            for bad in BAD_KINDS + (3,):
+                _rejected(lambda: shard(bad))
+            torch.cuda.synchronize()
+            assert all(torch.equal(a, b) for a, b in zip(vars_, before))
+            shard(0)                        # SGD, no slot rows
+            g.check()
+            m._tabs, m.opt_kind = full
+        finally:
+            g.close()
+        return
+
+    if entry in ("pairwise_step", "pairwise_prefetch"):
+        T = _Tabs(rng, (U, D), (I, D), (I, 1))
+
+        def call(opt, drop=None):
+            if entry == "pairwise_step":
+                eng.pairwise_step(N.ORX_PAIR_BPR, T.t(0, opt, drop), T.t(1, opt, drop), T.t(2, opt, drop), uid, pid,
+                                  nid, N.opt(opt, 0.05), out4)
+            else:
+                eng.pairwise_prefetch(T.t(0, opt, drop), T.t(1, opt, drop), uid, pid, nid, opt)
+        n_tabs = 3
+    elif entry == "pointwise_step":
+        T = _Tabs(rng, (U, D), (I, D), (I, 1), (1, D))
+        label = dev(rng.integers(0, 2, B))
+
+        def call(opt, drop=None):                   # GMF: the dense weight w is checked like the tables
+            eng.pointwise_step(N.ORX_POINT_GMF, T.t(0, opt, drop), T.t(1, opt, drop), T.t(2, opt, drop),
+                               T.t(3, opt, drop), uid, pid, label, N.opt(opt, 0.05), out4)
+        n_tabs = 4
+    elif entry in ("sparse_apply", "sparse_apply_strided"):
+        T = _Tabs(rng, (U, D))
+        vals = dev(rng.standard_normal((B, 1, D)))
+
+        def call(opt, drop=None):
+            if entry == "sparse_apply":
+                eng.sparse_apply(T.t(0, opt, drop), uid, vals.reshape(B, D), N.opt(opt, 0.05))
+            else:
+                eng.sparse_apply_strided(T.t(0, opt, drop), uid.reshape(B, 1), 0, vals, N.opt(opt, 0.05))
+        n_tabs = 1
+    else:
+        T = _Tabs(rng, (300,))
+        grad = dev(rng.standard_normal(300))
+
+        def call(opt, drop=None):
+            t = T.t(0, opt, drop)
+            var, s0, s1 = T.v[0]
+            eng.dense_apply(var, s0 if t.s0 else None, s1 if t.s1 else None, grad, N.opt(opt, 0.05))
+        n_tabs = 1
+
+    if entry != "pairwise_prefetch":                # the prefetch reads no slot row: the step that consumes it checks
+        for opt, j in MISSING_SLOT:
+            for i in range(n_tabs):
+                _rejected(lambda: call(opt, (i, j)))
+    for bad in BAD_KINDS:
+        _rejected(lambda: call(bad))
+    torch.cuda.synchronize()
+    assert T.unchanged()
+    call(0)                                         # SGD, no slot rows
+    if entry == "pairwise_prefetch":                # consume the prefetched index
+        eng.pairwise_step(N.ORX_PAIR_BPR, T.t(0, 0), T.t(1, 0), T.t(2, 0), uid, pid, nid, N.opt(0, 0.05), out4)
+    torch.cuda.synchronize()
+    eng.debug_dispatch_log()
