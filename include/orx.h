@@ -287,7 +287,8 @@ ORX_API int orx_pred_loss(orx_handle_t h, const float* pred, const float* label,
 
 /* ---- inference: full-catalogue scoring (bpr.py:39-43, wrmf.py:36-40, ucml.py:50-53, gmf.py:36-41)
  * scores[Bu, I] = user_rows . item^T + bias   (DOT; GMF passes user_rows pre-multiplied by w via `scale`)
- *               = -||user_row - item||^2 + bias (NEG_SQDIST).  scale may be NULL. */
+ *               = -||user_row - item||^2 + bias (NEG_SQDIST).  scale may be NULL, and so may item_bias (no bias).
+ * A uid outside [0, U) scores as a zero user row: 0 + bias (DOT), -||item||^2 + bias (NEG_SQDIST). */
 ORX_API int orx_score_all(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid, int32_t Bu,
                   const float* scale, const float* item_tab, const float* item_bias, int64_t I, int32_t dim,
                   float* scores, orx_stream_t s);

@@ -5,6 +5,8 @@
 // ---------------------------------------------------------------------------------------
 // LatentFactor.__init__ initializer (latent_factor.py:8-15): U(lo,hi) from a counter-based hash
 // (TF's RNG stream is not reproducible across frameworks; only the distribution matters).
+// lo + (hi - lo) * u can round up to hi for u < 1 (e.g. [1, 2) at u = 1 - 2^-24): such a value is clamped to the
+// largest float below hi, so the range stays half-open.  Values below hi keep their bits.
 // ---------------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
   x += 0x9E3779B97F4A7C15ull;
@@ -15,10 +17,11 @@ __device__ __forceinline__ uint64_t splitmix64(uint64_t x) {
 
 __global__ void k_fill_uniform(float* dst, int64_t n, float lo, float hi, uint64_t seed) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const float top = nextafterf(hi, lo);   // largest float below hi
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const uint64_t r = splitmix64(seed * 0xD1342543DE82EF95ull + (uint64_t)i);
     const float u = (float)(r >> 40) * (1.0f / 16777216.0f);  // [0,1)
-    dst[i] = lo + (hi - lo) * u;
+    dst[i] = fminf(lo + (hi - lo) * u, top);
   }
 }
 
@@ -60,9 +63,10 @@ __global__ void __launch_bounds__(256) k_gather(const float* __restrict__ tab, i
 
 extern "C" int orx_gather(orx_handle_t h, const float* tab, int64_t rows, int32_t dim, const void* ids,
                           int32_t id_is_i64, int64_t n, float* out, int32_t* n_bad, orx_stream_t s) {
-  ORX_REQUIRE(h != nullptr && tab && ids && out, "null pointer");
+  ORX_REQUIRE(h != nullptr && tab, "null pointer");
   ORX_REQUIRE(rows > 0 && dim > 0 && n >= 0, "bad sizes");
-  if (n == 0) return ORX_OK;
+  if (n == 0) return ORX_OK;                   // an empty lookup: ids and out may be NULL (empty tensors)
+  ORX_REQUIRE(ids && out, "null pointer");
   ORX_CUDA(cudaSetDevice(h->device));
   int64_t blocks = (n + 7) / 8;
   if (blocks > (int64_t)h->num_sms * 32) blocks = (int64_t)h->num_sms * 32;
