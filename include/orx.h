@@ -87,13 +87,15 @@ ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
  * TA = TB = 0, S = 1.  A sparse step (one record per call) has TA = kind (orx_pair_kind / orx_point_kind), TB = optimizer
  * (orx_opt_kind), M = B, N = D, K = the CTAs/SM bound of the fused kernel's __launch_bounds__ (0: none) and S = the batch
  * index set it used: 0 = built on the caller's stream, 1 or 2 = a consumed prefetch (orx_pairwise_prefetch, or the side
- * stream of orx_pairwise_step_host).  Host-side bookkeeping only: no device work, no synchronisation. */
+ * stream of orx_pairwise_step_host).  orx_score_rank writes one record per call (fields at ORX_OP_SCORE_RANK).
+ * Host-side bookkeeping only: no device work, no synchronisation. */
 enum orx_dispatch_op {
   ORX_OP_GEMM = 0,
   ORX_OP_INTERACT_FWD = 1,
   ORX_OP_INTERACT_BWD = 2,
   ORX_OP_PAIRWISE_STEP = 3,  /* orx_pairwise_step, orx_pairwise_step_host */
-  ORX_OP_POINTWISE_STEP = 4  /* orx_pointwise_step */
+  ORX_OP_POINTWISE_STEP = 4, /* orx_pointwise_step */
+  ORX_OP_SCORE_RANK = 5      /* orx_score_rank: TA = orx_score_kind, TB = 0, M = Bu, N = I, K = dim, S = item splits */
 };
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
@@ -102,7 +104,9 @@ enum orx_dispatch_variant {
   ORX_VARIANT_INTERACT = 3,      /* k_interact_{fwd,bwd}: one CTA per sample */
   ORX_VARIANT_STEP = 4,          /* k_pair_step / k_point_step specialised on D (32, 64, 128, 256), one register buffer */
   ORX_VARIANT_STEP_PIPE = 5,     /* k_pair_step with the register double buffer (PIPE) */
-  ORX_VARIANT_STEP_GENERIC = 6   /* k_pair_step_generic / k_point_generic: any D */
+  ORX_VARIANT_STEP_GENERIC = 6,  /* k_pair_step_generic / k_point_generic: any D */
+  ORX_VARIANT_RANK_SMEM = 7,     /* k_score_rank: thresholds and histograms of a user tile in shared memory */
+  ORX_VARIANT_RANK_GLOBAL = 8    /* k_score_rank: thresholds and histograms in the handle's global scratch */
 };
 #define ORX_DISPATCH_LOG_CAP 64
 ORX_API int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec_host, int32_t cap, int32_t* n_host);
@@ -322,9 +326,25 @@ ORX_API int orx_sample_per_positive(orx_handle_t h, const orx_sampler_t* sd_host
 /* ---- ranking metrics (openrec/tf2/metrics/ranking_metrics.py:8-69), one row per user --------
  * pos/excl are uint8 masks [R, I]; at[] (host) the cut-offs; outputs auc[R], ndcg[R,n_at], recall[R,n_at]
  * (any may be NULL). */
+#define ORX_MAX_AT 8 /* cut-offs of orx_rank_metrics / orx_score_rank */
 ORX_API int orx_rank_metrics(orx_handle_t h, const float* pred, const uint8_t* pos, const uint8_t* excl, int32_t R,
                      int64_t I, const int32_t* at_host, int32_t n_at, float* auc, float* ndcg, float* recall,
                      orx_stream_t s);
+
+/* ---- fused catalogue evaluation: orx_score_all + orx_rank_metrics in one call, without the [Bu, I] score matrix or
+ * the dense masks (openrec_b200/tf2/metrics/evaluator.py).
+ * For batch row b, u = uid[b]: positives = pos_items[pos_off[u] .. pos_off[u+1]), excluded = excl_items[excl_off[u] ..
+ * excl_off[u+1]) (excl_off may be NULL = nothing excluded).  Each row sorted and unique; entries outside [0, I) are
+ * ignored.  u outside [0, U): zero user row and empty lists.  Results equal orx_score_all followed by orx_rank_metrics
+ * on the masks these lists describe.  max_pos (host) bounds every positive row length; a row longer than max_pos gets
+ * NaN in all its outputs.  auc / ndcg / recall may each be NULL.  kind, scale, item_bias and the bad-uid rule are those
+ * of orx_score_all; at most ORX_MAX_AT cut-offs.  Scratch of about 20 * Bu * (max_pos + 1) bytes comes from the
+ * handle (its own allocation, grown on demand: a growing call synchronises the device). */
+ORX_API int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
+                           int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
+                           int32_t dim, const int64_t* pos_off, const int32_t* pos_items, const int64_t* excl_off,
+                           const int32_t* excl_items, int32_t max_pos, const int32_t* at_host, int32_t n_at,
+                           float* auc, float* ndcg, float* recall, orx_stream_t s);
 
 #ifdef __cplusplus
 }

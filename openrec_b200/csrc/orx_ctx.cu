@@ -216,6 +216,7 @@ extern "C" int orx_destroy(orx_handle_t h) {
   cudaFree(h->counters);
   cudaFree(h->partials);
   cudaFree(h->bucket_cursor);
+  cudaFree(h->eval_ws);
   orx_shard_ws_release(h);
   if (h->side_stream) {
     cudaStreamDestroy(h->side_stream);

@@ -1,0 +1,592 @@
+// orx_eval.cu -- catalogue-scale evaluation: score a batch of users against the whole item table and count the AUC /
+// NDCG / Recall ranks in the same pass, from per-user CSR lists of positives and exclusions.  No [Bu, I] buffer.
+//
+// Counting identity (orx_rank_metrics' definitions, one batch row, p over its positives, i over all items):
+//   AUC count = sum_{i eval} #{p : pred_p >= s_i}          rank_p = #{i : sp_i > sp_p},  sp = expf(pred) * !excl
+// The main pass counts every item as if it were an eval item and not excluded: its AUC term #{p : pred_p >= s} and,
+// with j = #{p : sp_p < expf(s)} over the ascending sp, one hit in hist[j] (the item ranks above the j smallest sp).
+// The finish recomputes the scores of pos u excl, takes back their AUC terms and the rank hits of the excluded items
+// (an excluded item's sp is 0 or NaN and never ranks above anything), and rank of the q-th smallest sp = sum_{j > q}
+// hist[j].  Every score is computed by the FFMA chain of k_score_all (acc = 0, one fused multiply-add per k in
+// ascending order, user value scaled first, bias added last), so the comparisons, and with them every count, equal
+// those of orx_score_all + orx_rank_metrics exactly.
+#include <cub/device/device_segmented_sort.cuh>
+
+#include "orx_common.cuh"
+
+namespace {
+
+constexpr int EV_TU = 128, EV_TI = 128, EV_KC = 8, EV_NT = 256, EV_LD = EV_TU + 4;
+
+struct EvalArgs {
+  const float* user_tab;
+  int64_t U;
+  const int32_t* uid;
+  int Bu;
+  const float* scale;
+  const float* item_tab;
+  const float* bias;
+  int64_t I;
+  int D;
+  const int64_t *pos_off, *excl_off;
+  const int32_t *pos_items, *excl_items;
+  int max_pos;
+  int P;  // max_pos + 1: row stride of the threshold and histogram rows
+};
+
+// Scratch of one call (handle workspace).  keys_in / keys: [2][Bu][P] -- pred thresholds of row b at b * P, sp
+// thresholds at (Bu + b) * P; keys holds them sorted ascending.  info[2b] = positives of row b (-1: longer than
+// max_pos), info[2b + 1] = those whose pred is not NaN (the pred thresholds searched for AUC).
+struct EvalWs {
+  float *keys_in, *keys;
+  int *seg_begin, *seg_end;
+  unsigned* hist;                 // [Bu][P]
+  unsigned long long* auc_cnt;    // [Bu]
+  int* info;                      // [Bu][2]
+  void* sort_tmp;
+  size_t sort_bytes;
+};
+
+struct EvalOut {
+  int at[ORX_MAX_AT];
+  int n_at;
+  float *auc, *ndcg, *recall;
+};
+
+__device__ __forceinline__ const float* ev_user_row(const EvalArgs& a, int b) {
+  const int32_t id = a.uid[b];
+  return (id >= 0 && (int64_t)id < a.U) ? a.user_tab + (int64_t)id * a.D : nullptr;
+}
+
+// first position in items[lo, hi) holding a value >= v (the row is sorted)
+__device__ __forceinline__ int64_t ev_lower(const int32_t* items, int64_t lo, int64_t hi, int64_t v) {
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if ((int64_t)items[mid] < v) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// The entries of user row `row` of a CSR that lie in [0, I): [*lo, *hi); *raw = the row's full length.
+__device__ __forceinline__ void ev_range(const int64_t* off, const int32_t* items, int32_t row, int64_t rows, int64_t I,
+                                         int64_t* lo, int64_t* hi, int64_t* raw) {
+  *lo = *hi = *raw = 0;
+  if (!off || row < 0 || (int64_t)row >= rows) return;
+  const int64_t b = off[row], e = off[row + 1];
+  *raw = e - b;
+  *lo = ev_lower(items, b, e, 0);
+  *hi = ev_lower(items, *lo, e, I);
+}
+
+__device__ __forceinline__ bool ev_contains(const int32_t* items, int64_t lo, int64_t hi, int32_t v) {
+  const int64_t k = ev_lower(items, lo, hi, v);
+  return k < hi && items[k] == v;
+}
+
+// One score by the chain of k_score_all.
+template <int KIND>
+__device__ __forceinline__ float ev_score1(const EvalArgs& a, const float* urow, int64_t i) {
+  const float* irow = a.item_tab + i * a.D;
+  float acc = 0.f;
+  for (int k = 0; k < a.D; ++k) {
+    float uv = 0.f;
+    if (urow) {   // explicit roundings: u * scale - i must not contract into one fused multiply-add
+      uv = urow[k];
+      if (a.scale) uv = __fmul_rn(uv, a.scale[k]);
+    }
+    if (KIND == ORX_SCORE_DOT) {
+      acc = __fmaf_rn(uv, irow[k], acc);
+    } else {
+      const float d = __fsub_rn(uv, irow[k]);
+      acc = __fmaf_rn(-d, d, acc);
+    }
+  }
+  return acc + (a.bias ? a.bias[i] : 0.f);
+}
+
+// #{q < n_auc : pth[q] >= s} over ascending thresholds with bounds pmin / pmax (n_auc = 0: pmin = +inf, pmax = -inf);
+// a NaN s counts nothing (pred_e <= pred_p is false).
+__device__ __forceinline__ unsigned ev_auc_count(const float* pth, int n_auc, float pmin, float pmax, float s) {
+  if (!(s <= pmax)) return 0u;
+  if (s <= pmin) return (unsigned)n_auc;
+  int lo = 0, hi = n_auc;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (pth[mid] >= s) hi = mid;
+    else lo = mid + 1;
+  }
+  return (unsigned)(n_auc - lo);
+}
+
+// #{q < n : sth[q] < e} over ascending thresholds with bounds smin / smax (n = 0: smin = +inf); NaN e gives 0.
+__device__ __forceinline__ int ev_rank_slot(const float* sth, int n, float smin, float smax, float e) {
+  if (!(e > smin)) return 0;
+  if (e > smax) return n;
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (sth[mid] < e) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// ---------------------------------------------------------------------------------------
+// prep: one CTA per batch row.  pred_p and sp_p of every positive (sp: NaN -> +inf, which ranks 0 like NaN; pred: NaN
+// -> +NaN, which sorts after every number and is left out of the AUC search), zeroed histogram and AUC count, and the
+// two sort segments of the row.
+// ---------------------------------------------------------------------------------------
+template <int KIND>
+__global__ void __launch_bounds__(EV_NT) k_eval_prep(const EvalArgs a, const EvalWs w) {
+  __shared__ int s_nan;
+  const int b = blockIdx.x;
+  const int32_t u = a.uid[b];
+  const float* urow = ev_user_row(a, b);
+  int64_t plo, phi, praw, elo, ehi, eraw;
+  ev_range(a.pos_off, a.pos_items, u, a.U, a.I, &plo, &phi, &praw);
+  ev_range(a.excl_off, a.excl_items, u, a.U, a.I, &elo, &ehi, &eraw);
+  const bool bad = praw > a.max_pos;
+  const int n = bad ? 0 : (int)(phi - plo);
+  float* kp = w.keys_in + (int64_t)b * a.P;
+  float* ks = w.keys_in + (int64_t)(a.Bu + b) * a.P;
+  if (threadIdx.x == 0) s_nan = 0;
+  __syncthreads();
+  for (int q = threadIdx.x; q < n; q += blockDim.x) {
+    const int32_t i = a.pos_items[plo + q];
+    float s = ev_score1<KIND>(a, urow, i);
+    const bool ex = ev_contains(a.excl_items, elo, ehi, i);
+    float sp = expf(s) * (ex ? 0.f : 1.f);
+    if (sp != sp) sp = __int_as_float(0x7f800000);
+    if (s != s) {
+      s = __int_as_float(0x7fffffff);
+      atomicAdd(&s_nan, 1);
+    }
+    kp[q] = s;
+    ks[q] = sp;
+  }
+  for (int j = threadIdx.x; j < a.P; j += blockDim.x) w.hist[(int64_t)b * a.P + j] = 0u;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    w.info[2 * b] = bad ? -1 : n;
+    w.info[2 * b + 1] = n - s_nan;
+    w.auc_cnt[b] = 0ull;
+    w.seg_begin[b] = b * a.P;
+    w.seg_end[b] = b * a.P + n;
+    w.seg_begin[a.Bu + b] = (a.Bu + b) * a.P;
+    w.seg_end[a.Bu + b] = (a.Bu + b) * a.P + n;
+  }
+}
+
+// ---------------------------------------------------------------------------------------
+// main pass: 128 users x 128 items per tile, 8 x 8 scores per thread, D in chunks of 8 through a double-buffered
+// shared tile.  A CTA takes one user tile and walks a contiguous range of item tiles; the thresholds and histograms
+// of its rows sit in shared memory (USE_SMEM) or stay in the global scratch, reached through the same generic pointers.
+// ---------------------------------------------------------------------------------------
+struct RowMeta {
+  const float* urow;
+  const float* pth;
+  const float* sth;
+  unsigned* hist;
+  int n, n_auc;
+  float pmin, pmax, smin, smax;
+};
+
+// rows / columns of a thread's 8 x 8 block: 4 at t * 4 and 4 at 64 + t * 4
+__device__ __forceinline__ int ev_frag(int t, int x) { return (x < 4 ? 0 : 64 - 4) + t * 4 + x; }
+
+template <int KIND, bool TAIL>
+__device__ __forceinline__ void ev_mma_chunk(float (&acc)[8][8], const float (*sa)[EV_LD], const float (*sb)[EV_LD],
+                                             int ty, int tx, int kn) {
+#pragma unroll
+  for (int k = 0; k < EV_KC; ++k) {
+    if (TAIL && k >= kn) break;
+    const float4 a0 = *reinterpret_cast<const float4*>(&sa[k][ty * 4]);
+    const float4 a1 = *reinterpret_cast<const float4*>(&sa[k][64 + ty * 4]);
+    const float4 b0 = *reinterpret_cast<const float4*>(&sb[k][tx * 4]);
+    const float4 b1 = *reinterpret_cast<const float4*>(&sb[k][64 + tx * 4]);
+    const float uu[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
+    const float ii[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+#pragma unroll
+    for (int x = 0; x < 8; ++x)
+#pragma unroll
+      for (int y = 0; y < 8; ++y) {
+        if (KIND == ORX_SCORE_DOT) {
+          acc[x][y] = __fmaf_rn(uu[x], ii[y], acc[x][y]);
+        } else {
+          const float d = __fsub_rn(uu[x], ii[y]);
+          acc[x][y] = __fmaf_rn(-d, d, acc[x][y]);
+        }
+      }
+  }
+}
+
+template <int KIND>
+__global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const EvalWs w, int use_smem) {
+  extern __shared__ float4 ev_dyn4[];
+  __shared__ __align__(16) float sA[2][EV_KC][EV_LD];
+  __shared__ __align__(16) float sB[2][EV_KC][EV_LD];
+  __shared__ RowMeta meta[EV_TU];
+  __shared__ unsigned long long s_auc[EV_TU];
+  float* dyn = reinterpret_cast<float*>(ev_dyn4);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tx = tid & 15, ty = tid >> 4;
+  const int u0 = blockIdx.y * EV_TU;
+  const int rows = min(EV_TU, a.Bu - u0);
+  const int rows_alloc = min(EV_TU, a.Bu);   // rows of the shared threshold region (the host sized it so)
+  const int64_t P = a.P;
+
+  if (tid < EV_TU) {
+    RowMeta m = {};
+    if (tid < rows) {
+      const int b = u0 + tid;
+      m.urow = ev_user_row(a, b);
+      m.n = max(w.info[2 * b], 0);
+      m.n_auc = w.info[2 * b] < 0 ? 0 : w.info[2 * b + 1];
+      if (use_smem) {
+        m.pth = dyn + tid * P;
+        m.sth = dyn + (rows_alloc + tid) * P;
+        m.hist = reinterpret_cast<unsigned*>(dyn + (2 * rows_alloc + tid) * P);
+      } else {
+        m.pth = w.keys + (int64_t)b * P;
+        m.sth = w.keys + (int64_t)(a.Bu + b) * P;
+        m.hist = w.hist + (int64_t)b * P;
+      }
+    }
+    meta[tid] = m;
+    s_auc[tid] = 0ull;
+  }
+  __syncthreads();
+  if (use_smem) {
+    for (int r = warp; r < rows; r += EV_NT / 32) {
+      const int b = u0 + r;
+      const RowMeta& m = meta[r];
+      float* pth = const_cast<float*>(m.pth);
+      float* sth = const_cast<float*>(m.sth);
+      for (int q = lane; q < m.n; q += 32) {
+        pth[q] = w.keys[(int64_t)b * P + q];
+        sth[q] = w.keys[(int64_t)(a.Bu + b) * P + q];
+      }
+      for (int j = lane; j <= m.n; j += 32) m.hist[j] = 0u;
+    }
+    __syncthreads();
+  }
+  if (tid < rows) {
+    RowMeta& m = meta[tid];
+    m.pmin = m.n_auc ? m.pth[0] : __int_as_float(0x7f800000);
+    m.pmax = m.n_auc ? m.pth[m.n_auc - 1] : __int_as_float(0xff800000);
+    m.smin = m.n ? m.sth[0] : __int_as_float(0x7f800000);
+    m.smax = m.n ? m.sth[m.n - 1] : __int_as_float(0x7f800000);
+  }
+  __syncthreads();
+
+  const int64_t n_tiles = (a.I + EV_TI - 1) / EV_TI;
+  const int64_t t_begin = n_tiles * blockIdx.x / gridDim.x, t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
+  const int n_chunks = (a.D + EV_KC - 1) / EV_KC;
+  float ru[4], ri[4];
+  // chunk k0 of this tile into registers: element e = tid + 256 j is row e / 8, k e % 8
+  auto load = [&](int64_t i0, int k0) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int e = tid + EV_NT * j, r = e >> 3, k = k0 + (e & 7);
+      float uv = 0.f, iv = 0.f;
+      if (k < a.D) {
+        const float* urow = meta[r].urow;
+        if (urow) {
+          uv = urow[k];
+          if (a.scale) uv = __fmul_rn(uv, a.scale[k]);
+        }
+        if (i0 + r < a.I) iv = a.item_tab[(i0 + r) * a.D + k];
+      }
+      ru[j] = uv;
+      ri[j] = iv;
+    }
+  };
+  auto store = [&](int buf) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int e = tid + EV_NT * j;
+      sA[buf][e & 7][e >> 3] = ru[j];
+      sB[buf][e & 7][e >> 3] = ri[j];
+    }
+  };
+
+  for (int64_t t = t_begin; t < t_end; ++t) {
+    const int64_t i0 = t * EV_TI;
+    float acc[8][8];
+#pragma unroll
+    for (int x = 0; x < 8; ++x)
+#pragma unroll
+      for (int y = 0; y < 8; ++y) acc[x][y] = 0.f;
+    load(i0, 0);
+    store(0);
+    __syncthreads();
+    for (int c = 0; c < n_chunks; ++c) {
+      if (c + 1 < n_chunks) load(i0, (c + 1) * EV_KC);
+      const int kn = a.D - c * EV_KC;
+      if (kn >= EV_KC) ev_mma_chunk<KIND, false>(acc, sA[c & 1], sB[c & 1], ty, tx, EV_KC);
+      else ev_mma_chunk<KIND, true>(acc, sA[c & 1], sB[c & 1], ty, tx, kn);
+      if (c + 1 < n_chunks) store((c + 1) & 1);
+      __syncthreads();
+    }
+    // epilogue: the AUC terms and rank hits of this tile's scores
+    float bv[8];
+#pragma unroll
+    for (int y = 0; y < 8; ++y) {
+      const int64_t i = i0 + ev_frag(tx, y);
+      bv[y] = (a.bias && i < a.I) ? a.bias[i] : 0.f;
+    }
+#pragma unroll
+    for (int x = 0; x < 8; ++x) {
+      const int r = ev_frag(ty, x);
+      if (r >= rows) continue;
+      const RowMeta& m = meta[r];
+      if (m.n == 0) continue;
+      unsigned long long cnt = 0ull;
+#pragma unroll
+      for (int y = 0; y < 8; ++y) {
+        if (i0 + ev_frag(tx, y) >= a.I) continue;
+        const float s = acc[x][y] + bv[y];
+        cnt += ev_auc_count(m.pth, m.n_auc, m.pmin, m.pmax, s);
+        const int j = ev_rank_slot(m.sth, m.n, m.smin, m.smax, expf(s));
+        if (j) atomicAdd(m.hist + j, 1u);
+      }
+      if (cnt) atomicAdd(&s_auc[r], cnt);
+    }
+  }
+  __syncthreads();
+  for (int r = warp; r < rows; r += EV_NT / 32) {
+    const RowMeta& m = meta[r];
+    if (use_smem)
+      for (int j = 1 + lane; j <= m.n; j += 32) {
+        const unsigned h = m.hist[j];
+        if (h) atomicAdd(w.hist + (int64_t)(u0 + r) * P + j, h);
+      }
+    if (lane == 0 && s_auc[r]) atomicAdd(w.auc_cnt + u0 + r, s_auc[r]);
+  }
+}
+
+// ---------------------------------------------------------------------------------------
+// correction + finish: one CTA per batch row.  Takes back the terms of pos u excl, suffix-sums the histogram into the
+// positives' ranks and writes auc / ndcg / recall with the formulas and conversions of k_rank_metrics.
+// ---------------------------------------------------------------------------------------
+template <int KIND>
+__global__ void __launch_bounds__(EV_NT) k_eval_finish(const EvalArgs a, const EvalWs w, const EvalOut o) {
+  __shared__ unsigned long long s_sub;
+  __shared__ long long s_extra;
+  __shared__ unsigned s_part[EV_NT];
+  __shared__ unsigned s_after[EV_NT];
+  __shared__ double s_dcg[ORX_MAX_AT];
+  __shared__ int s_hit[ORX_MAX_AT];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int info = w.info[2 * b];
+  if (info < 0) {   // a positive row longer than max_pos
+    const float nan = __int_as_float(0x7fffffff);
+    if (tid == 0 && o.auc) o.auc[b] = nan;
+    if (tid < o.n_at) {
+      if (o.ndcg) o.ndcg[(int64_t)b * o.n_at + tid] = nan;
+      if (o.recall) o.recall[(int64_t)b * o.n_at + tid] = nan;
+    }
+    return;
+  }
+  const int n = info, n_auc = w.info[2 * b + 1];
+  const int64_t P = a.P;
+  const float* pth = w.keys + (int64_t)b * P;
+  const float* sth = w.keys + (int64_t)(a.Bu + b) * P;
+  unsigned* hist = w.hist + (int64_t)b * P;
+  const float pmin = n_auc ? pth[0] : __int_as_float(0x7f800000);
+  const float pmax = n_auc ? pth[n_auc - 1] : __int_as_float(0xff800000);
+  const float smin = n ? sth[0] : __int_as_float(0x7f800000);
+  const float smax = n ? sth[n - 1] : __int_as_float(0x7f800000);
+  const int32_t u = a.uid[b];
+  const float* urow = ev_user_row(a, b);
+  int64_t plo, phi, praw, elo, ehi, eraw;
+  ev_range(a.pos_off, a.pos_items, u, a.U, a.I, &plo, &phi, &praw);
+  ev_range(a.excl_off, a.excl_items, u, a.U, a.I, &elo, &ehi, &eraw);
+  if (tid == 0) {
+    s_sub = 0ull;
+    s_extra = 0;
+  }
+  if (tid < ORX_MAX_AT) {
+    s_dcg[tid] = 0.0;
+    s_hit[tid] = 0;
+  }
+  __syncthreads();
+  unsigned long long sub = 0ull;
+  long long extra = 0;
+  for (int64_t q = tid; q < n; q += blockDim.x) {          // positives: not eval items
+    const int32_t i = a.pos_items[plo + q];
+    const float s = ev_score1<KIND>(a, urow, i);
+    sub += ev_auc_count(pth, n_auc, pmin, pmax, s);
+    if (ev_contains(a.excl_items, elo, ehi, i)) {
+      const int j = ev_rank_slot(sth, n, smin, smax, expf(s));
+      if (j) atomicSub(hist + j, 1u);
+    }
+  }
+  for (int64_t q = elo + tid; q < ehi; q += blockDim.x) {  // excluded items that are not positives
+    const int32_t i = a.excl_items[q];
+    if (ev_contains(a.pos_items, plo, phi, i)) continue;
+    ++extra;
+    const float s = ev_score1<KIND>(a, urow, i);
+    sub += ev_auc_count(pth, n_auc, pmin, pmax, s);
+    const int j = ev_rank_slot(sth, n, smin, smax, expf(s));
+    if (j) atomicSub(hist + j, 1u);
+  }
+  if (sub) atomicAdd(&s_sub, sub);
+  if (extra) atomicAdd(reinterpret_cast<unsigned long long*>(&s_extra), (unsigned long long)extra);
+  __syncthreads();
+  // rank of the q-th smallest sp = sum_{j > q} hist[j]: thread t owns hist[1 + t * chunk .. (t + 1) * chunk]
+  const int chunk = (n + EV_NT - 1) / EV_NT;
+  const int jlo = 1 + tid * chunk, jhi = min(n, (tid + 1) * chunk);
+  unsigned part = 0;
+  for (int j = jlo; j <= jhi; ++j) part += hist[j];
+  s_part[tid] = part;
+  __syncthreads();
+  if (tid == 0) {
+    unsigned run = 0;
+    for (int t = EV_NT - 1; t >= 0; --t) {
+      s_after[t] = run;
+      run += s_part[t];
+    }
+  }
+  __syncthreads();
+  double dcg[ORX_MAX_AT];
+  int hit[ORX_MAX_AT];
+#pragma unroll
+  for (int k = 0; k < ORX_MAX_AT; ++k) {
+    dcg[k] = 0.0;
+    hit[k] = 0;
+  }
+  unsigned run = s_after[tid];
+  for (int j = jhi; j >= jlo; --j) {
+    run += hist[j];                       // rank of position q = j - 1
+    const float ra = (float)run;
+    const float rec = 1.f / (logf(ra + 2.f) / logf(2.0f));
+#pragma unroll
+    for (int k = 0; k < ORX_MAX_AT; ++k)
+      if (k < o.n_at && ra < (float)o.at[k]) {
+        dcg[k] += (double)rec;
+        ++hit[k];
+      }
+  }
+#pragma unroll
+  for (int k = 0; k < ORX_MAX_AT; ++k)
+    if (k < o.n_at && hit[k]) {
+      atomicAdd(&s_dcg[k], dcg[k]);
+      atomicAdd(&s_hit[k], hit[k]);
+    }
+  __syncthreads();
+  if (tid == 0 && o.auc) {
+    const unsigned long long cnt = w.auc_cnt[b] - s_sub;
+    const long long n_eval = a.I - (long long)n - s_extra;
+    o.auc[b] = (float)cnt / (float)((long long)n * n_eval);
+  }
+  if (tid < o.n_at) {
+    if (o.ndcg) o.ndcg[(int64_t)b * o.n_at + tid] = (float)s_dcg[tid];
+    if (o.recall) o.recall[(int64_t)b * o.n_at + tid] = (float)s_hit[tid] / (float)n;
+  }
+}
+
+size_t ev_align(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// The call's scratch inside one allocation; with base == nullptr only the size is computed.
+size_t ev_layout(char* base, int Bu, int P, size_t sort_bytes, EvalWs* w) {
+  const size_t nk = (size_t)2 * Bu * P;
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    char* p = base ? base + off : nullptr;
+    off += ev_align(bytes);
+    return p;
+  };
+  w->keys_in = reinterpret_cast<float*>(take(sizeof(float) * nk));
+  w->keys = reinterpret_cast<float*>(take(sizeof(float) * nk));
+  w->seg_begin = reinterpret_cast<int*>(take(sizeof(int) * 2 * (size_t)Bu));
+  w->seg_end = reinterpret_cast<int*>(take(sizeof(int) * 2 * (size_t)Bu));
+  w->hist = reinterpret_cast<unsigned*>(take(sizeof(unsigned) * (size_t)Bu * P));
+  w->auc_cnt = reinterpret_cast<unsigned long long*>(take(sizeof(unsigned long long) * (size_t)Bu));
+  w->info = reinterpret_cast<int*>(take(sizeof(int) * 2 * (size_t)Bu));
+  w->sort_tmp = take(sort_bytes);
+  w->sort_bytes = sort_bytes;
+  return off;
+}
+
+template <int KIND>
+int ev_launch(orx_ctx* h, const EvalArgs& a, const EvalWs& w, const EvalOut& o, cudaStream_t st) {
+  auto kern = k_score_rank<KIND>;
+  int optin = 0;
+  ORX_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
+  cudaFuncAttributes fa;
+  ORX_CUDA(cudaFuncGetAttributes(&fa, kern));
+  const size_t dyn_max = (size_t)optin - fa.sharedSizeBytes;
+  // thresholds (pred, sp) and histogram of every row of a user tile in shared memory when they fit, for every tile
+  const size_t rows_alloc = (size_t)(a.Bu < EV_TU ? a.Bu : EV_TU);
+  const size_t dyn_need = 3 * sizeof(float) * rows_alloc * (size_t)a.P;
+  const int use_smem = dyn_need <= dyn_max ? 1 : 0;
+  const size_t dyn = use_smem ? dyn_need : 0;
+  ORX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_max));
+  int per_sm = 0;
+  ORX_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, EV_NT, dyn));
+  if (per_sm < 1) per_sm = 1;
+  const int64_t user_tiles = (a.Bu + EV_TU - 1) / EV_TU;
+  const int64_t item_tiles = (a.I + EV_TI - 1) / EV_TI;
+  int64_t splits = ((int64_t)h->num_sms * per_sm + user_tiles - 1) / user_tiles;
+  if (splits > item_tiles) splits = item_tiles;
+  if (splits < 1) splits = 1;
+
+  k_eval_prep<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w);
+  ORX_LAUNCH_CHECK();
+  size_t bytes = w.sort_bytes;
+  ORX_CUDA(cub::DeviceSegmentedSort::SortKeys(w.sort_tmp, bytes, (const float*)w.keys_in, w.keys, 2 * a.Bu * a.P,
+                                              2 * a.Bu, (const int*)w.seg_begin, (const int*)w.seg_end, st));
+  kern<<<dim3((unsigned)splits, (unsigned)user_tiles), EV_NT, dyn, st>>>(a, w, use_smem);
+  ORX_LAUNCH_CHECK();
+  k_eval_finish<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w, o);
+  ORX_LAUNCH_CHECK();
+  orx_log_dispatch(h, ORX_OP_SCORE_RANK, use_smem ? ORX_VARIANT_RANK_SMEM : ORX_VARIANT_RANK_GLOBAL, KIND, 0, a.Bu,
+                   (int)(a.I > INT32_MAX ? INT32_MAX : a.I), a.D, (int)splits);
+  return ORX_OK;
+}
+
+}  // namespace
+
+extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
+                              int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
+                              int32_t dim, const int64_t* pos_off, const int32_t* pos_items, const int64_t* excl_off,
+                              const int32_t* excl_items, int32_t max_pos, const int32_t* at_host, int32_t n_at,
+                              float* auc, float* ndcg, float* recall, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr && user_tab && uid && item_tab && pos_off, "null pointer");
+  ORX_REQUIRE(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST, "unknown score kind");
+  ORX_REQUIRE(U > 0 && I > 0 && I <= INT32_MAX && dim > 0 && Bu >= 0 && max_pos >= 0, "bad sizes");
+  ORX_REQUIRE(n_at >= 0 && n_at <= ORX_MAX_AT, "at most 8 cut-offs");
+  ORX_REQUIRE(n_at == 0 || at_host, "null cut-offs");
+  if (Bu == 0) return ORX_OK;
+  const int64_t P = (int64_t)max_pos + 1;
+  ORX_REQUIRE(2 * (int64_t)Bu * P <= INT32_MAX, "Bu * (max_pos + 1) too large for one call: split the batch");
+  ORX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)s;
+
+  EvalWs w;
+  size_t sort_bytes = 0;
+  ORX_CUDA(cub::DeviceSegmentedSort::SortKeys((void*)nullptr, sort_bytes, (const float*)nullptr, (float*)nullptr,
+                                              (int)(2 * Bu * P), 2 * Bu, (const int*)nullptr, (const int*)nullptr, st));
+  const size_t need = ev_layout(nullptr, Bu, (int)P, sort_bytes, &w);
+  if (need > h->eval_cap) {   // grown like the index workspace: drain the device, then replace the allocation
+    ORX_CUDA(cudaDeviceSynchronize());
+    cudaFree(h->eval_ws);
+    h->eval_ws = nullptr;
+    h->eval_cap = 0;
+    ORX_CUDA(cudaMalloc(&h->eval_ws, need));
+    h->eval_cap = need;
+  }
+  ev_layout(static_cast<char*>(h->eval_ws), Bu, (int)P, sort_bytes, &w);
+
+  EvalArgs a;
+  a.user_tab = user_tab; a.U = U; a.uid = uid; a.Bu = Bu; a.scale = scale; a.item_tab = item_tab;
+  a.bias = item_bias; a.I = I; a.D = dim; a.pos_off = pos_off; a.excl_off = excl_off; a.pos_items = pos_items;
+  a.excl_items = excl_items; a.max_pos = max_pos; a.P = (int)P;
+  EvalOut o;
+  for (int k = 0; k < ORX_MAX_AT; ++k) o.at[k] = k < n_at ? at_host[k] : 0;
+  o.n_at = n_at; o.auc = auc; o.ndcg = ndcg; o.recall = recall;
+  return kind == ORX_SCORE_DOT ? ev_launch<ORX_SCORE_DOT>(h, a, w, o, st)
+                               : ev_launch<ORX_SCORE_NEG_SQDIST>(h, a, w, o, st);
+}

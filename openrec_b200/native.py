@@ -9,16 +9,18 @@ import torch
 
 from . import _lib
 from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP,
-                   ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR, ORX_PAIR_UCML,
-                   ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
-                   ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_STEP,
-                   ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE, OrxOpt, OrxTable)
+                   ORX_OP_SCORE_RANK, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
+                   ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
+                   ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
+                   ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE, OrxOpt,
+                   OrxTable)
 
 __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", "ORX_POINT_GMF", "ORX_POINT_WRMF",
            "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_SCORE_DOT",
            "ORX_SCORE_NEG_SQDIST", "ORX_OP_GEMM", "ORX_OP_INTERACT_FWD", "ORX_OP_INTERACT_BWD", "ORX_OP_PAIRWISE_STEP",
            "ORX_OP_POINTWISE_STEP", "ORX_VARIANT_GEMM_TMA", "ORX_VARIANT_GEMM_SIMT", "ORX_VARIANT_INTERACT_WARP",
-           "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC", "Dispatch"]
+           "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC",
+           "ORX_OP_SCORE_RANK", "ORX_VARIANT_RANK_SMEM", "ORX_VARIANT_RANK_GLOBAL", "Dispatch"]
 
 _engines = {}
 
@@ -280,6 +282,41 @@ class Engine:
         rec = torch.empty((R, len(at)), dtype=torch.float32, device=pred.device) if "recall" in want else None
         _lib.check(self.lib.orx_rank_metrics(self.h, _ptr(pred), _ptr(pos), _ptr(excl), R, I, at_arr, len(at),
                                              _ptr(auc), _ptr(ndcg), _ptr(rec), self.stream()), "orx_rank_metrics")
+        return auc, ndcg, rec
+
+    def score_rank(self, kind, user_tab, uid, item_tab, item_bias, pos_off, pos_items, excl_off, excl_items, max_pos,
+                   at=(), scale=None):
+        """score_all + rank_metrics in one pass for the users uid, from CSR lists indexed by user id: positives
+        pos_items[pos_off[u]:pos_off[u + 1]] and exclusions likewise (excl_off / excl_items may be None); int64 offsets,
+        int32 items, rows sorted and unique.  max_pos bounds every positive row length (a longer row gets NaN outputs).
+        -> (auc [Bu], ndcg [Bu, len(at)], recall [Bu, len(at)])."""
+        uid = ids32(uid)
+        Bu, dev = uid.numel(), item_tab.device
+
+        def csr(off, items):
+            if off is None:
+                return None, None
+            if not (off.is_cuda and off.dtype == torch.int64 and off.is_contiguous()):
+                raise ValueError("CSR offsets: expected a contiguous int64 CUDA tensor")
+            if not (items.is_cuda and items.dtype == torch.int32 and items.is_contiguous()):
+                raise ValueError("CSR items: expected a contiguous int32 CUDA tensor")
+            if off.numel() != user_tab.shape[0] + 1:
+                raise ValueError("CSR offsets must have one entry per user row plus one")
+            return off, items if items.numel() else None
+
+        pos_off, pos_items = csr(pos_off, pos_items)
+        excl_off, excl_items = csr(excl_off, excl_items)
+        if pos_off is None:
+            raise ValueError("score_rank needs the positives' CSR")
+        at_arr = (C.c_int32 * max(len(at), 1))(*[int(k) for k in at])
+        auc = torch.empty(Bu, dtype=torch.float32, device=dev)
+        ndcg = torch.empty((Bu, len(at)), dtype=torch.float32, device=dev)
+        rec = torch.empty((Bu, len(at)), dtype=torch.float32, device=dev)
+        _lib.check(self.lib.orx_score_rank(
+            self.h, kind, _ptr(_f32(user_tab, "user_tab")), user_tab.shape[0], _ptr(uid), Bu, _ptr(scale),
+            _ptr(_f32(item_tab, "item_tab")), _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(pos_off),
+            _ptr(pos_items), _ptr(excl_off), _ptr(excl_items), int(max_pos), at_arr, len(at), _ptr(auc), _ptr(ndcg),
+            _ptr(rec), self.stream()), "orx_score_rank")
         return auc, ndcg, rec
 
 

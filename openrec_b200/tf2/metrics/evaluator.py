@@ -1,0 +1,90 @@
+"""RankingEvaluator -- AUC / NDCG / Recall of every warm user of a dataset at catalogue scale, in one fused liborx call
+per batch (orx_score_rank): the users are scored against the whole item table and the ranks counted in the same pass,
+so neither the [users, items] score matrix nor the per-user masks of ``Dataset.evaluation`` are ever built.
+
+The results equal those of the reference example's loop (``Dataset.evaluation`` + ``model.inference`` + ``AUC`` /
+``NDCG`` / ``Recall``) for the same users in the same order.  The positives of ``val_dataset`` and the union of the
+positives of ``excl_datasets`` become two CSR lists over user ids, uploaded once; a batch then only needs its user ids.
+"""
+from __future__ import annotations
+
+import numpy as np
+import torch
+
+from ... import native as N
+from ..._lib import ORX_MAX_AT
+from ...tfshim.core import Tensor
+
+
+def _csr(n_rows, rows):
+    """{user: iterable of items} -> (offsets int64 [n_rows + 1], items int32): each row sorted and unique, users
+    without an entry (or outside [0, n_rows)) empty."""
+    lens = np.zeros(n_rows, dtype=np.int64)
+    parts = {}
+    for u, items in rows.items():
+        u = int(u)
+        if 0 <= u < n_rows:
+            parts[u] = np.unique(np.fromiter(items, dtype=np.int64))
+            lens[u] = len(parts[u])
+    off = np.zeros(n_rows + 1, dtype=np.int64)
+    np.cumsum(lens, out=off[1:])
+    items = np.concatenate([parts[u] for u in sorted(parts)]) if parts else np.zeros(0, dtype=np.int64)
+    return off, items.astype(np.int32)
+
+
+class RankingEvaluator:
+    """``RankingEvaluator(val_dataset, excl_datasets=[train_dataset], at=[50, 100], batch_size=1024).evaluate(model)``
+    -> {'AUC': [n_warm], 'NDCG': [n_warm, len(at)], 'Recall': [n_warm, len(at)]} in ``warm_users()`` order, ready for
+    ``DictMean.update_state``.  Ranks against the whole catalogue, so a dataset with explicit negatives (ranked against
+    its listed items only) is not supported: use ``Dataset.evaluation`` for those."""
+
+    def __init__(self, val_dataset, excl_datasets=[], at=[100], batch_size=1024):
+        store = val_dataset.datastore
+        if store.contain_negatives():
+            raise NotImplementedError("RankingEvaluator ranks against the whole catalogue; a dataset with explicit "
+                                      "negatives ranks against its listed items only (use Dataset.evaluation)")
+        if len(at) > ORX_MAX_AT:
+            raise ValueError(f"at most {ORX_MAX_AT} cut-offs")
+        if batch_size < 1:
+            raise ValueError("batch_size must be positive")
+        self.at = tuple(int(k) for k in at)
+        self.batch_size = int(batch_size)
+        n_users = store.total_users()
+        self.warm_users = np.asarray(store.warm_users(), dtype=np.int64)
+        self.pos_off, self.pos_items = _csr(n_users, {u: store.get_positive_items(u) for u in self.warm_users})
+        excl = {}
+        for ds in excl_datasets:
+            other = ds.datastore
+            for u in other.warm_users():
+                excl.setdefault(int(u), set()).update(other.get_positive_items(u))
+        self.excl_off, self.excl_items = _csr(n_users, excl)
+        self._pos_len = np.diff(self.pos_off)
+        self.max_pos = int(self._pos_len.max()) if n_users else 0
+        self._dev = None
+
+    def _upload(self, device):
+        if self._dev is None or self._dev[0] != device:
+            put = lambda a: torch.from_numpy(a).to(device)                       # noqa: E731
+            self._dev = (device, put(self.warm_users.astype(np.int32)), put(self.pos_off), put(self.pos_items),
+                         put(self.excl_off), put(self.excl_items))
+        return self._dev[1:]
+
+    def evaluate(self, model):
+        ops = getattr(model, "_score_operands", None)
+        if ops is None:
+            raise NotImplementedError(f"{type(model).__name__}: catalogue evaluation needs the model's whole item "
+                                      "table on one device (BPR, UCML, GMF, WRMF)")
+        kind, user, item, bias, scale = ops()
+        uids, pos_off, pos_items, excl_off, excl_items = self._upload(item.device)
+        eng = N.engine()
+        auc, ndcg, rec = [], [], []
+        for b0 in range(0, len(self.warm_users), self.batch_size):
+            b1 = min(b0 + self.batch_size, len(self.warm_users))
+            max_pos = int(self._pos_len[self.warm_users[b0:b1]].max())
+            a, n, r = eng.score_rank(kind, user, uids[b0:b1], item, bias, pos_off, pos_items, excl_off, excl_items,
+                                     max_pos, at=self.at, scale=scale)
+            auc.append(a), ndcg.append(n), rec.append(r)
+        if not auc:
+            empty = torch.zeros((0, len(self.at)), dtype=torch.float32, device=item.device)
+            return {"AUC": Tensor(empty[:, 0]), "NDCG": Tensor(empty), "Recall": Tensor(empty.clone())}
+        return {"AUC": Tensor(torch.cat(auc)), "NDCG": Tensor(torch.cat(ndcg)), "Recall": Tensor(torch.cat(rec))}

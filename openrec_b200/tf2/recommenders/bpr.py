@@ -73,7 +73,12 @@ class BPR(FusedRecommender):
             val = torch.cat([kw["d_bp"], kw["d_bn"]]).reshape(-1, 1)
         return Tensor(idx), Tensor(val)
 
+    def _score_operands(self):
+        """(kind, user table, item table, item bias, scale) of the full-catalogue score (inference, RankingEvaluator)."""
+        return (self._score, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
+                self.item_bias.embeddings.t, None)
+
     def inference(self, user_id):
         """scores [Bu, total_items] = U[user] @ Item^T + bias (bpr.py:39-43)."""
-        return Tensor(N.engine().score_all(self._score, self.user_latent_factor.embeddings.t, ids_of(user_id),
-                                           self.item_latent_factor.embeddings.t, self.item_bias.embeddings.t))
+        kind, user, item, bias, scale = self._score_operands()
+        return Tensor(N.engine().score_all(kind, user, ids_of(user_id), item, bias, scale=scale))

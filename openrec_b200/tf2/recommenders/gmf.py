@@ -2,9 +2,8 @@
 import torch
 
 from ... import native as N
-from ...tfshim.core import Tensor
 from ..modules import MLP, LatentFactor
-from ._base import FusedRecommender, ids_of, w_table
+from ._base import FusedRecommender, w_table
 from .wrmf import WRMF
 
 
@@ -31,8 +30,7 @@ class GMF(WRMF):
         s0, s1 = optimizer.slots(k)
         return w_table(k.t, s0, s1)
 
-    def inference(self, user_id):
-        """(u * w) . item^T + bias (gmf.py:36-41)."""
-        return Tensor(N.engine().score_all(N.ORX_SCORE_DOT, self.user_latent_factor.embeddings.t, ids_of(user_id),
-                                           self.item_latent_factor.embeddings.t, self.item_bias.embeddings.t,
-                                           scale=self.mlp.layers[0].kernel.t.reshape(-1)))
+    def _score_operands(self):
+        """(u * w) . item^T + bias (gmf.py:36-41): WRMF's score with GMF's w as the user-side scale."""
+        return (N.ORX_SCORE_DOT, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
+                self.item_bias.embeddings.t, self.mlp.layers[0].kernel.t.reshape(-1))

@@ -61,7 +61,12 @@ class WRMF(FusedRecommender):
         val = next(iter(kw.values()))
         return Tensor(idx), Tensor(val.reshape(B, -1))
 
+    def _score_operands(self):
+        """(kind, user table, item table, item bias, scale) of the full-catalogue score (inference, RankingEvaluator)."""
+        return (N.ORX_SCORE_DOT, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
+                self.item_bias.embeddings.t, None)
+
     def inference(self, user_id):
         """U[user] @ Item^T + bias (wrmf.py:36-40)."""
-        return Tensor(N.engine().score_all(N.ORX_SCORE_DOT, self.user_latent_factor.embeddings.t, ids_of(user_id),
-                                           self.item_latent_factor.embeddings.t, self.item_bias.embeddings.t))
+        kind, user, item, bias, scale = self._score_operands()
+        return Tensor(N.engine().score_all(kind, user, ids_of(user_id), item, bias, scale=scale))
