@@ -87,7 +87,8 @@ ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
  * TA = TB = 0, S = 1.  A sparse step (one record per call) has TA = kind (orx_pair_kind / orx_point_kind), TB = optimizer
  * (orx_opt_kind), M = B, N = D, K = the CTAs/SM bound of the fused kernel's __launch_bounds__ (0: none) and S = the batch
  * index set it used: 0 = built on the caller's stream, 1 or 2 = a consumed prefetch (orx_pairwise_prefetch, or the side
- * stream of orx_pairwise_step_host).  orx_score_rank writes one record per call (fields at ORX_OP_SCORE_RANK).
+ * stream of orx_pairwise_step_host).  orx_score_rank and orx_score_topk write one record per call (fields at
+ * ORX_OP_SCORE_RANK / ORX_OP_SCORE_TOPK).
  * Host-side bookkeeping only: no device work, no synchronisation. */
 enum orx_dispatch_op {
   ORX_OP_GEMM = 0,
@@ -95,7 +96,8 @@ enum orx_dispatch_op {
   ORX_OP_INTERACT_BWD = 2,
   ORX_OP_PAIRWISE_STEP = 3,  /* orx_pairwise_step, orx_pairwise_step_host */
   ORX_OP_POINTWISE_STEP = 4, /* orx_pointwise_step */
-  ORX_OP_SCORE_RANK = 5      /* orx_score_rank: TA = orx_score_kind, TB = 0, M = Bu, N = I, K = dim, S = item splits */
+  ORX_OP_SCORE_RANK = 5,     /* orx_score_rank: TA = orx_score_kind, TB = 0, M = Bu, N = I, K = dim, S = item splits */
+  ORX_OP_SCORE_TOPK = 6      /* orx_score_topk: TA = orx_score_kind, TB = k, M = Bu, N = I, K = dim, S = item splits */
 };
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
@@ -106,7 +108,8 @@ enum orx_dispatch_variant {
   ORX_VARIANT_STEP_PIPE = 5,     /* k_pair_step with the register double buffer (PIPE) */
   ORX_VARIANT_STEP_GENERIC = 6,  /* k_pair_step_generic / k_point_generic: any D */
   ORX_VARIANT_RANK_SMEM = 7,     /* k_score_rank: thresholds and histograms of a user tile in shared memory */
-  ORX_VARIANT_RANK_GLOBAL = 8    /* k_score_rank: thresholds and histograms in the handle's global scratch */
+  ORX_VARIANT_RANK_GLOBAL = 8,   /* k_score_rank: thresholds and histograms in the handle's global scratch */
+  ORX_VARIANT_TOPK = 9           /* k_score_topk + k_topk_merge: candidate lists in the handle's global scratch */
 };
 #define ORX_DISPATCH_LOG_CAP 64
 ORX_API int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec_host, int32_t cap, int32_t* n_host);
@@ -345,6 +348,34 @@ ORX_API int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_tab, 
                            int32_t dim, const int64_t* pos_off, const int32_t* pos_items, const int64_t* excl_off,
                            const int32_t* excl_items, int32_t max_pos, const int32_t* at_host, int32_t n_at,
                            float* auc, float* ndcg, float* recall, orx_stream_t s);
+
+/* ---- catalogue top-K retrieval: each batch row's k best unseen items in one fused pass, without the [Bu, I] score
+ * matrix (openrec_b200/tf2/recommenders/retriever.py; closest reference: openrec/tf1's FastDotProductServer).
+ * Scores and conventions are those of orx_score_all, unchanged: the score of (b, i) with kind, scale and item_bias as
+ * there; a uid outside [0, U) scores as a zero user row and has an empty exclusion list.  Exclusion lists follow the
+ * CSR conventions of orx_score_rank: row u = excl_items[excl_off[u] .. excl_off[u+1]), sorted and unique, entries
+ * outside [0, I) ignored, excl_off == NULL meaning nothing is excluded.
+ * Eligible items: item i is eligible for row b when 0 <= i < I, i is not in uid[b]'s exclusion row, and its score is
+ * not NaN.
+ * Order: row b of the output is the first k eligible items in the total order "score descending, then item id
+ * ascending".  Scores compare as floats, so -0.0 == +0.0, and -inf is a valid score.
+ * Padding: when fewer than k items are eligible, the remaining slots hold item -1 and score -inf.
+ * Score values: top_scores[b, j] equals the orx_score_all value of (uid[b], top_items[b, j]) bit for bit, except that
+ * a -0.0 may come back as +0.0.  top_scores may be NULL.
+ * Argument limits: 1 <= k <= ORX_MAX_TOPK, and k > I is allowed.  Bu = 0 is a no-op.  The other size checks are those
+ * of orx_score_rank.
+ * Determinism: the result does not depend on the number of item splits, on how many other users share the call, or on
+ * the order of atomics, so the same inputs give the same bits on every call and every handle.
+ * Scratch: 8 * Bu * S * (k + 1024) + 4 * Bu * S bytes (plus 512 bytes of alignment), S = the item splits of the
+ * dispatch record (one wave of CTAs over the SMs divided among the ceil(Bu / 128) user tiles, at least 1 and at most
+ * ceil(I / 128)), from the handle's evaluation scratch of
+ * orx_score_rank: its own allocation, grown on demand (a growing call synchronises the device), so a call between
+ * orx_pairwise_prefetch and its step leaves the prefetched index alone. */
+#define ORX_MAX_TOPK 1024
+ORX_API int orx_score_topk(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
+                           int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
+                           int32_t dim, const int64_t* excl_off, const int32_t* excl_items, int32_t k,
+                           int32_t* top_items /*[Bu, k]*/, float* top_scores /*[Bu, k], may be NULL*/, orx_stream_t s);
 
 #ifdef __cplusplus
 }

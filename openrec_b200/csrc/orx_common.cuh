@@ -82,7 +82,7 @@ struct orx_ctx {
   void* shard_ws;          // orx_shard.cu: local scratch of the row-sharded step (orx_shard_ws*)
   int32_t dispatch[ORX_DISPATCH_LOG_CAP][8];   // orx_debug_dispatch_log: ring of the last DLRM / sparse-step launches
   int64_t dispatch_n;      // records written since the last read
-  void* eval_ws;           // orx_eval.cu: scratch of orx_score_rank (thresholds, histograms, sort), its own allocation
+  void* eval_ws;           // orx_eval.cu: scratch of orx_score_rank / orx_score_topk, its own allocation
   size_t eval_cap;
 };
 

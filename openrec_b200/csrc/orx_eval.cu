@@ -1,5 +1,7 @@
-// orx_eval.cu -- catalogue-scale evaluation: score a batch of users against the whole item table and count the AUC /
-// NDCG / Recall ranks in the same pass, from per-user CSR lists of positives and exclusions.  No [Bu, I] buffer.
+// orx_eval.cu -- catalogue-scale evaluation and retrieval: score a batch of users against the whole item table and
+// count the AUC / NDCG / Recall ranks in the same pass (orx_score_rank), or keep each user's k best items
+// (orx_score_topk), from per-user CSR lists of positives and exclusions.  No [Bu, I] buffer.  Both share one tile loop
+// (ev_tiles) and differ only in its epilogue.
 //
 // Counting identity (orx_rank_metrics' definitions, one batch row, p over its positives, i over all items):
 //   AUC count = sum_{i eval} #{p : pred_p >= s_i}          rank_p = #{i : sp_i > sp_p},  sp = expf(pred) * !excl
@@ -221,6 +223,68 @@ __device__ __forceinline__ void ev_mma_chunk(float (&acc)[8][8], const float (*s
   }
 }
 
+// The main loop of k_score_rank and k_score_topk: the CTA's user tile against its contiguous range of item tiles
+// (blockIdx.x of gridDim.x splits).  Tile row r's user row is urow_of(r) (nullptr: a zero row); D goes in chunks of 8
+// through the double-buffered shared tiles sA / sB.  After each tile every thread calls epi(i0, acc): acc[x][y] is the
+// score of row ev_frag(ty, x) and item i0 + ev_frag(tx, y) before the bias, by the chain of k_score_all.  Every thread
+// passes a __syncthreads after epi returns and before the next tile's scores are read.
+template <int KIND, class UrowOf, class Epi>
+__device__ __forceinline__ void ev_tiles(const EvalArgs& a, float (*sA)[EV_KC][EV_LD], float (*sB)[EV_KC][EV_LD],
+                                         UrowOf urow_of, Epi epi) {
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int64_t n_tiles = (a.I + EV_TI - 1) / EV_TI;
+  const int64_t t_begin = n_tiles * blockIdx.x / gridDim.x, t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
+  const int n_chunks = (a.D + EV_KC - 1) / EV_KC;
+  float ru[4], ri[4];
+  // chunk k0 of this tile into registers: element e = tid + 256 j is row e / 8, k e % 8
+  auto load = [&](int64_t i0, int k0) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int e = tid + EV_NT * j, r = e >> 3, k = k0 + (e & 7);
+      float uv = 0.f, iv = 0.f;
+      if (k < a.D) {
+        const float* urow = urow_of(r);
+        if (urow) {
+          uv = urow[k];
+          if (a.scale) uv = __fmul_rn(uv, a.scale[k]);
+        }
+        if (i0 + r < a.I) iv = a.item_tab[(i0 + r) * a.D + k];
+      }
+      ru[j] = uv;
+      ri[j] = iv;
+    }
+  };
+  auto store = [&](int buf) {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int e = tid + EV_NT * j;
+      sA[buf][e & 7][e >> 3] = ru[j];
+      sB[buf][e & 7][e >> 3] = ri[j];
+    }
+  };
+
+  for (int64_t t = t_begin; t < t_end; ++t) {
+    const int64_t i0 = t * EV_TI;
+    float acc[8][8];
+#pragma unroll
+    for (int x = 0; x < 8; ++x)
+#pragma unroll
+      for (int y = 0; y < 8; ++y) acc[x][y] = 0.f;
+    load(i0, 0);
+    store(0);
+    __syncthreads();
+    for (int c = 0; c < n_chunks; ++c) {
+      if (c + 1 < n_chunks) load(i0, (c + 1) * EV_KC);
+      const int kn = a.D - c * EV_KC;
+      if (kn >= EV_KC) ev_mma_chunk<KIND, false>(acc, sA[c & 1], sB[c & 1], ty, tx, EV_KC);
+      else ev_mma_chunk<KIND, true>(acc, sA[c & 1], sB[c & 1], ty, tx, kn);
+      if (c + 1 < n_chunks) store((c + 1) & 1);
+      __syncthreads();
+    }
+    epi(i0, acc);
+  }
+}
+
 template <int KIND>
 __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const EvalWs w, int use_smem) {
   extern __shared__ float4 ev_dyn4[];
@@ -280,56 +344,8 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
   }
   __syncthreads();
 
-  const int64_t n_tiles = (a.I + EV_TI - 1) / EV_TI;
-  const int64_t t_begin = n_tiles * blockIdx.x / gridDim.x, t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
-  const int n_chunks = (a.D + EV_KC - 1) / EV_KC;
-  float ru[4], ri[4];
-  // chunk k0 of this tile into registers: element e = tid + 256 j is row e / 8, k e % 8
-  auto load = [&](int64_t i0, int k0) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int e = tid + EV_NT * j, r = e >> 3, k = k0 + (e & 7);
-      float uv = 0.f, iv = 0.f;
-      if (k < a.D) {
-        const float* urow = meta[r].urow;
-        if (urow) {
-          uv = urow[k];
-          if (a.scale) uv = __fmul_rn(uv, a.scale[k]);
-        }
-        if (i0 + r < a.I) iv = a.item_tab[(i0 + r) * a.D + k];
-      }
-      ru[j] = uv;
-      ri[j] = iv;
-    }
-  };
-  auto store = [&](int buf) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int e = tid + EV_NT * j;
-      sA[buf][e & 7][e >> 3] = ru[j];
-      sB[buf][e & 7][e >> 3] = ri[j];
-    }
-  };
-
-  for (int64_t t = t_begin; t < t_end; ++t) {
-    const int64_t i0 = t * EV_TI;
-    float acc[8][8];
-#pragma unroll
-    for (int x = 0; x < 8; ++x)
-#pragma unroll
-      for (int y = 0; y < 8; ++y) acc[x][y] = 0.f;
-    load(i0, 0);
-    store(0);
-    __syncthreads();
-    for (int c = 0; c < n_chunks; ++c) {
-      if (c + 1 < n_chunks) load(i0, (c + 1) * EV_KC);
-      const int kn = a.D - c * EV_KC;
-      if (kn >= EV_KC) ev_mma_chunk<KIND, false>(acc, sA[c & 1], sB[c & 1], ty, tx, EV_KC);
-      else ev_mma_chunk<KIND, true>(acc, sA[c & 1], sB[c & 1], ty, tx, kn);
-      if (c + 1 < n_chunks) store((c + 1) & 1);
-      __syncthreads();
-    }
-    // epilogue: the AUC terms and rank hits of this tile's scores
+  // epilogue: the AUC terms and rank hits of each tile's scores
+  ev_tiles<KIND>(a, sA, sB, [&](int r) { return meta[r].urow; }, [&](int64_t i0, const float (&acc)[8][8]) {
     float bv[8];
 #pragma unroll
     for (int y = 0; y < 8; ++y) {
@@ -353,7 +369,7 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
       }
       if (cnt) atomicAdd(&s_auc[r], cnt);
     }
-  }
+  });
   __syncthreads();
   for (int r = warp; r < rows; r += EV_NT / 32) {
     const RowMeta& m = meta[r];
@@ -487,6 +503,254 @@ __global__ void __launch_bounds__(EV_NT) k_eval_finish(const EvalArgs a, const E
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// top-K retrieval (orx_score_topk).  Key of an eligible (score s, item i): the order-preserving bits of s (-0 taken as
+// +0) in the high word, ~i in the low word, so "score descending, then item ascending" is ">" on keys; keys are unique
+// and every real key is > 0, which marks an empty slot.  NaN scores never form a key.
+// ---------------------------------------------------------------------------------------
+// Room of a candidate list beyond k.  A tile appends at most 128 keys to a row's list, so a list is cut back to k only
+// once it holds more than k + TK_ROOM - 128 keys (and once after the CTA's last tile): every few tiles while the
+// threshold warms up or when scores rise with item id, rarely after that.
+constexpr int TK_ROOM = 1024;
+
+struct TopkWs {
+  unsigned long long* cand;   // [Bu][splits][k + TK_ROOM]: the candidate list of (row, item split)
+  int* cnt;                   // [Bu][splits]: its length after the split's last tile (<= k)
+};
+
+__device__ __forceinline__ unsigned long long tk_key(float s, int64_t i) {
+  unsigned u = __float_as_uint(s == 0.f ? 0.f : s);
+  u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  return ((unsigned long long)u << 32) | (unsigned)~(uint32_t)i;
+}
+
+__device__ __forceinline__ float tk_score(unsigned long long key) {
+  const unsigned u = (unsigned)(key >> 32);
+  return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u);
+}
+
+template <int NT>
+__device__ __forceinline__ void tk_sync() {
+  if (NT == 32) __syncwarp();
+  else __syncthreads();
+}
+
+// The k-th largest (1 <= k <= number of keys) of a set of unique keys, found by NT threads (one warp, or the CTA) that
+// visit the keys through each(fn): a radix select, 8 bits per pass from the most significant byte, with the 256-bin
+// histogram hist in shared memory.  t = the thread's index in the group; s_sel: CTA-wide broadcast (NT > 32 only).
+template <int NT, class Each>
+__device__ unsigned long long tk_kth(Each each, int k, unsigned* hist, unsigned long long* s_sel, int t) {
+  unsigned long long prefix = 0ull, mask = 0ull;
+  unsigned kk = (unsigned)k;
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    for (int j = t; j < 256; j += NT) hist[j] = 0u;
+    tk_sync<NT>();
+    each([&](unsigned long long v) {
+      if ((v & mask) == prefix) {
+        const unsigned bin = (unsigned)(v >> shift) & 255u;
+        if (NT == 32) {
+          atomicAdd(&hist[bin], 1u);
+        } else {   // CTA-wide: one atomic per distinct bin of the converged lanes (keys share their leading bytes)
+          const unsigned peers = __match_any_sync(__activemask(), bin);
+          if ((threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&hist[bin], (unsigned)__popc(peers));
+        }
+      }
+    });
+    tk_sync<NT>();
+    if (t < 32) {   // the digit d with fewer than kk keys in the bins above it and at least kk from d up
+      unsigned c[8], sum = 0u;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        c[j] = hist[255 - 8 * t - j];
+        sum += c[j];
+      }
+      unsigned incl = sum;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned v = __shfl_up_sync(ORX_FULL, incl, o);
+        if (t >= o) incl += v;
+      }
+      const int src = __ffs(__ballot_sync(ORX_FULL, incl >= kk)) - 1;
+      unsigned run = incl - sum, above = 0u;
+      int d = 0;
+      if (t == src)
+        for (int j = 0; j < 8; ++j) {
+          if (run + c[j] >= kk) {
+            d = 255 - 8 * t - j;
+            above = run;
+            break;
+          }
+          run += c[j];
+        }
+      d = __shfl_sync(ORX_FULL, d, src);
+      above = __shfl_sync(ORX_FULL, above, src);
+      prefix |= (unsigned long long)d << shift;
+      kk -= above;
+      if (NT > 32 && t == 0) {
+        s_sel[0] = prefix;
+        s_sel[1] = kk;
+      }
+    }
+    if (NT > 32) {
+      __syncthreads();
+      prefix = s_sel[0];
+      kk = (unsigned)s_sel[1];
+    }
+    mask |= 0xffull << shift;
+  }
+  return prefix;
+}
+
+// Main pass: the tile loop of k_score_rank with a top-K epilogue.  Row r of the CTA's user tile keeps a threshold key
+// (0 until its list is first cut) and appends every eligible key above it to its list in the scratch.  Cutting a list
+// (one warp) keeps its exact top k, and the threshold becomes the k-th key.
+struct TkRow {
+  const float* urow;
+  int64_t elo, ehi;   // the row's exclusion entries in [0, I)
+};
+
+template <int KIND>
+__global__ void __launch_bounds__(EV_NT, 2) k_score_topk(const EvalArgs a, const TopkWs w, int k) {
+  __shared__ __align__(16) float sA[2][EV_KC][EV_LD];
+  __shared__ __align__(16) float sB[2][EV_KC][EV_LD];
+  __shared__ TkRow meta[EV_TU];
+  __shared__ unsigned long long s_thr[EV_TU];
+  __shared__ int s_cnt[EV_TU];
+  __shared__ unsigned s_hist[EV_NT / 32][256];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tx = tid & 15, ty = tid >> 4;
+  const int u0 = blockIdx.y * EV_TU;
+  const int rows = min(EV_TU, a.Bu - u0);
+  const int64_t C = (int64_t)k + TK_ROOM;
+  auto list = [&](int r) { return w.cand + ((int64_t)(u0 + r) * gridDim.x + blockIdx.x) * C; };
+  // cut every list of the tile longer than `limit` to its top k (after a __syncthreads that follows the appends); the
+  // CTA's last tile cuts every list longer than k (a CTA has at least one tile: splits <= item tiles)
+  const int64_t n_tiles = (a.I + EV_TI - 1) / EV_TI;
+  const int64_t last_i0 = (n_tiles * (blockIdx.x + 1) / gridDim.x - 1) * EV_TI;
+  auto cut = [&](int limit) {
+    for (int r = warp; r < rows; r += EV_NT / 32) {
+      const int n = s_cnt[r];
+      if (n <= limit) continue;
+      unsigned long long* keys = list(r);
+      const unsigned long long t = tk_kth<32>([&](auto fn) {
+        for (int q = lane; q < n; q += 32) fn(keys[q]);
+      }, k, s_hist[warp], nullptr, lane);
+      // keep the k keys >= t, in place: a chunk is read before any of its slots is written
+      int kept = 0;
+      for (int q0 = 0; q0 < n; q0 += 32) {
+        const unsigned long long v = q0 + lane < n ? keys[q0 + lane] : 0ull;
+        const unsigned keep = __ballot_sync(ORX_FULL, v >= t);
+        if (v >= t) keys[kept + __popc(keep & ((1u << lane) - 1u))] = v;
+        kept += __popc(keep);
+      }
+      __syncwarp();
+      if (lane == 0) {
+        s_thr[r] = t;
+        s_cnt[r] = k;
+      }
+    }
+  };
+
+  if (tid < EV_TU) {
+    TkRow m = {};
+    if (tid < rows) {
+      int64_t raw;
+      m.urow = ev_user_row(a, u0 + tid);
+      ev_range(a.excl_off, a.excl_items, a.uid[u0 + tid], a.U, a.I, &m.elo, &m.ehi, &raw);
+    }
+    meta[tid] = m;
+    s_thr[tid] = 0ull;
+    s_cnt[tid] = 0;
+  }
+  __syncthreads();
+
+  ev_tiles<KIND>(a, sA, sB, [&](int r) { return meta[r].urow; }, [&](int64_t i0, const float (&acc)[8][8]) {
+    float bv[8];
+#pragma unroll
+    for (int y = 0; y < 8; ++y) {
+      const int64_t i = i0 + ev_frag(tx, y);
+      bv[y] = (a.bias && i < a.I) ? a.bias[i] : 0.f;
+    }
+#pragma unroll
+    for (int x = 0; x < 8; ++x) {
+      const int r = ev_frag(ty, x);
+      if (r >= rows) continue;
+      const unsigned long long thr = s_thr[r];
+#pragma unroll
+      for (int y = 0; y < 8; ++y) {
+        const int64_t i = i0 + ev_frag(tx, y);
+        const float s = acc[x][y] + bv[y];
+        if (i >= a.I || s != s) continue;
+        const unsigned long long key = tk_key(s, i);
+        if (key <= thr || ev_contains(a.excl_items, meta[r].elo, meta[r].ehi, (int32_t)i)) continue;
+        list(r)[atomicAdd(&s_cnt[r], 1)] = key;
+      }
+    }
+    __syncthreads();
+    cut(i0 == last_i0 ? k : k + TK_ROOM - EV_TI);
+  });
+  __syncthreads();
+  if (tid < rows) w.cnt[(int64_t)(u0 + tid) * gridDim.x + blockIdx.x] = s_cnt[tid];
+}
+
+// Merge: one CTA per batch row.  The top k of the union of the row's split lists (radix select when the union is
+// larger), sorted descending in shared memory (bitonic), decoded; slots past the eligible items get item -1, -inf.
+__global__ void __launch_bounds__(EV_NT) k_topk_merge(const TopkWs w, int splits, int k, int32_t* top_items,
+                                                      float* top_scores) {
+  __shared__ unsigned long long s_key[ORX_MAX_TOPK];
+  __shared__ unsigned s_hist[256];
+  __shared__ unsigned long long s_sel[2];
+  __shared__ int s_n, s_m;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int C = k + TK_ROOM;
+  const unsigned long long* cand = w.cand + (int64_t)b * splits * C;
+  const int* cnt = w.cnt + (int64_t)b * splits;
+  auto each = [&](auto fn) {   // splits * k <= 2^31: the grid has at most a few thousand CTAs
+    for (int e = tid; e < splits * k; e += EV_NT) {
+      const int s = e / k, q = e - s * k;
+      if (q < cnt[s]) fn(cand[(int64_t)s * C + q]);
+    }
+  };
+  if (tid == 0) {
+    s_n = 0;
+    s_m = 0;
+  }
+  __syncthreads();
+  int part = 0;
+  for (int s = tid; s < splits; s += EV_NT) part += cnt[s];
+  if (part) atomicAdd(&s_n, part);
+  __syncthreads();
+  const int n = s_n;
+  const unsigned long long t = n > k ? tk_kth<EV_NT>(each, k, s_hist, s_sel, tid) : 1ull;
+  each([&](unsigned long long v) {
+    if (v >= t) s_key[atomicAdd(&s_m, 1)] = v;
+  });
+  int p2 = 1;
+  while (p2 < k) p2 <<= 1;
+  const int m = min(n, k);
+  for (int j = m + tid; j < p2; j += EV_NT) s_key[j] = 0ull;
+  __syncthreads();
+  for (int size = 2; size <= p2; size <<= 1)
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int i = tid; i < p2; i += EV_NT) {
+        const int j = i ^ stride;
+        if (j > i) {
+          const unsigned long long x = s_key[i], y = s_key[j];
+          if ((x < y) == ((i & size) == 0)) {
+            s_key[i] = y;
+            s_key[j] = x;
+          }
+        }
+      }
+      __syncthreads();
+    }
+  for (int j = tid; j < k; j += EV_NT) {
+    const unsigned long long key = s_key[j];
+    top_items[(int64_t)b * k + j] = key ? (int32_t)~(uint32_t)key : -1;
+    if (top_scores) top_scores[(int64_t)b * k + j] = key ? tk_score(key) : __int_as_float(0xff800000);
+  }
+}
+
 size_t ev_align(size_t x) { return (x + 255) & ~(size_t)255; }
 
 // The call's scratch inside one allocation; with base == nullptr only the size is computed.
@@ -510,6 +774,35 @@ size_t ev_layout(char* base, int Bu, int P, size_t sort_bytes, EvalWs* w) {
   return off;
 }
 
+// Item splits of a grid of user tiles x item splits for kern at dyn bytes of dynamic shared memory: enough CTAs for one
+// wave over the SMs, at most one item tile per CTA.
+template <class Kern>
+int ev_item_splits(const orx_ctx* h, Kern kern, size_t dyn, int Bu, int64_t I, int64_t* splits) {
+  int per_sm = 0;
+  ORX_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, EV_NT, dyn));
+  if (per_sm < 1) per_sm = 1;
+  const int64_t user_tiles = (Bu + EV_TU - 1) / EV_TU;
+  const int64_t item_tiles = (I + EV_TI - 1) / EV_TI;
+  int64_t s = ((int64_t)h->num_sms * per_sm + user_tiles - 1) / user_tiles;
+  if (s > item_tiles) s = item_tiles;
+  *splits = s < 1 ? 1 : s;
+  return ORX_OK;
+}
+
+// The handle's evaluation scratch, at least `need` bytes.  Grown like the index workspace: drain the device, then
+// replace the allocation.  It is its own allocation, so it never aliases a prefetched batch index.
+int ev_scratch(orx_ctx* h, size_t need) {
+  if (need > h->eval_cap) {
+    ORX_CUDA(cudaDeviceSynchronize());
+    cudaFree(h->eval_ws);
+    h->eval_ws = nullptr;
+    h->eval_cap = 0;
+    ORX_CUDA(cudaMalloc(&h->eval_ws, need));
+    h->eval_cap = need;
+  }
+  return ORX_OK;
+}
+
 template <int KIND>
 int ev_launch(orx_ctx* h, const EvalArgs& a, const EvalWs& w, const EvalOut& o, cudaStream_t st) {
   auto kern = k_score_rank<KIND>;
@@ -524,14 +817,10 @@ int ev_launch(orx_ctx* h, const EvalArgs& a, const EvalWs& w, const EvalOut& o, 
   const int use_smem = dyn_need <= dyn_max ? 1 : 0;
   const size_t dyn = use_smem ? dyn_need : 0;
   ORX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_max));
-  int per_sm = 0;
-  ORX_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, EV_NT, dyn));
-  if (per_sm < 1) per_sm = 1;
+  int64_t splits = 1;
+  const int rc = ev_item_splits(h, kern, dyn, a.Bu, a.I, &splits);
+  if (rc != ORX_OK) return rc;
   const int64_t user_tiles = (a.Bu + EV_TU - 1) / EV_TU;
-  const int64_t item_tiles = (a.I + EV_TI - 1) / EV_TI;
-  int64_t splits = ((int64_t)h->num_sms * per_sm + user_tiles - 1) / user_tiles;
-  if (splits > item_tiles) splits = item_tiles;
-  if (splits < 1) splits = 1;
 
   k_eval_prep<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w);
   ORX_LAUNCH_CHECK();
@@ -544,6 +833,33 @@ int ev_launch(orx_ctx* h, const EvalArgs& a, const EvalWs& w, const EvalOut& o, 
   ORX_LAUNCH_CHECK();
   orx_log_dispatch(h, ORX_OP_SCORE_RANK, use_smem ? ORX_VARIANT_RANK_SMEM : ORX_VARIANT_RANK_GLOBAL, KIND, 0, a.Bu,
                    (int)(a.I > INT32_MAX ? INT32_MAX : a.I), a.D, (int)splits);
+  return ORX_OK;
+}
+
+// The top-K scratch of Bu rows over `splits` item splits inside one allocation; with base == nullptr only the size.
+size_t tk_layout(char* base, int Bu, int64_t splits, int k, TopkWs* w) {
+  const size_t lists = (size_t)Bu * (size_t)splits;
+  const size_t cand = ev_align(sizeof(unsigned long long) * lists * ((size_t)k + TK_ROOM));
+  w->cand = reinterpret_cast<unsigned long long*>(base);
+  w->cnt = base ? reinterpret_cast<int*>(base + cand) : nullptr;
+  return cand + ev_align(sizeof(int) * lists);
+}
+
+template <int KIND>
+int tk_launch(orx_ctx* h, const EvalArgs& a, int k, int32_t* top_items, float* top_scores, cudaStream_t st) {
+  int64_t splits = 1;
+  int rc = ev_item_splits(h, k_score_topk<KIND>, 0, a.Bu, a.I, &splits);
+  if (rc != ORX_OK) return rc;
+  TopkWs w;
+  rc = ev_scratch(h, tk_layout(nullptr, a.Bu, splits, k, &w));
+  if (rc != ORX_OK) return rc;
+  tk_layout(static_cast<char*>(h->eval_ws), a.Bu, splits, k, &w);
+  const int64_t user_tiles = (a.Bu + EV_TU - 1) / EV_TU;
+  k_score_topk<KIND><<<dim3((unsigned)splits, (unsigned)user_tiles), EV_NT, 0, st>>>(a, w, k);
+  ORX_LAUNCH_CHECK();
+  k_topk_merge<<<a.Bu, EV_NT, 0, st>>>(w, (int)splits, k, top_items, top_scores);
+  ORX_LAUNCH_CHECK();
+  orx_log_dispatch(h, ORX_OP_SCORE_TOPK, ORX_VARIANT_TOPK, KIND, k, a.Bu, (int)a.I, a.D, (int)splits);
   return ORX_OK;
 }
 
@@ -569,15 +885,8 @@ extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_ta
   size_t sort_bytes = 0;
   ORX_CUDA(cub::DeviceSegmentedSort::SortKeys((void*)nullptr, sort_bytes, (const float*)nullptr, (float*)nullptr,
                                               (int)(2 * Bu * P), 2 * Bu, (const int*)nullptr, (const int*)nullptr, st));
-  const size_t need = ev_layout(nullptr, Bu, (int)P, sort_bytes, &w);
-  if (need > h->eval_cap) {   // grown like the index workspace: drain the device, then replace the allocation
-    ORX_CUDA(cudaDeviceSynchronize());
-    cudaFree(h->eval_ws);
-    h->eval_ws = nullptr;
-    h->eval_cap = 0;
-    ORX_CUDA(cudaMalloc(&h->eval_ws, need));
-    h->eval_cap = need;
-  }
+  const int rc = ev_scratch(h, ev_layout(nullptr, Bu, (int)P, sort_bytes, &w));
+  if (rc != ORX_OK) return rc;
   ev_layout(static_cast<char*>(h->eval_ws), Bu, (int)P, sort_bytes, &w);
 
   EvalArgs a;
@@ -589,4 +898,22 @@ extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_ta
   o.n_at = n_at; o.auc = auc; o.ndcg = ndcg; o.recall = recall;
   return kind == ORX_SCORE_DOT ? ev_launch<ORX_SCORE_DOT>(h, a, w, o, st)
                                : ev_launch<ORX_SCORE_NEG_SQDIST>(h, a, w, o, st);
+}
+
+extern "C" int orx_score_topk(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
+                              int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
+                              int32_t dim, const int64_t* excl_off, const int32_t* excl_items, int32_t k,
+                              int32_t* top_items, float* top_scores, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr, "null handle");
+  ORX_REQUIRE(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST, "unknown score kind");
+  ORX_REQUIRE(U > 0 && I > 0 && I <= INT32_MAX && dim > 0 && Bu >= 0, "bad sizes");
+  ORX_REQUIRE(k >= 1 && k <= ORX_MAX_TOPK, "k must lie in [1, ORX_MAX_TOPK]");
+  if (Bu == 0) return ORX_OK;   // before the pointer checks: an empty batch may come with NULL buffers
+  ORX_REQUIRE(user_tab && uid && item_tab && top_items, "null pointer");
+  ORX_CUDA(cudaSetDevice(h->device));
+  EvalArgs a = {};
+  a.user_tab = user_tab; a.U = U; a.uid = uid; a.Bu = Bu; a.scale = scale; a.item_tab = item_tab;
+  a.bias = item_bias; a.I = I; a.D = dim; a.excl_off = excl_off; a.excl_items = excl_items;
+  return kind == ORX_SCORE_DOT ? tk_launch<ORX_SCORE_DOT>(h, a, k, top_items, top_scores, (cudaStream_t)s)
+                               : tk_launch<ORX_SCORE_NEG_SQDIST>(h, a, k, top_items, top_scores, (cudaStream_t)s);
 }

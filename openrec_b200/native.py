@@ -9,18 +9,19 @@ import torch
 
 from . import _lib
 from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP,
-                   ORX_OP_SCORE_RANK, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
+                   ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
                    ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
                    ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
-                   ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE, OrxOpt,
-                   OrxTable)
+                   ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE,
+                   ORX_VARIANT_TOPK, OrxOpt, OrxTable)
 
 __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", "ORX_POINT_GMF", "ORX_POINT_WRMF",
            "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_SCORE_DOT",
            "ORX_SCORE_NEG_SQDIST", "ORX_OP_GEMM", "ORX_OP_INTERACT_FWD", "ORX_OP_INTERACT_BWD", "ORX_OP_PAIRWISE_STEP",
            "ORX_OP_POINTWISE_STEP", "ORX_VARIANT_GEMM_TMA", "ORX_VARIANT_GEMM_SIMT", "ORX_VARIANT_INTERACT_WARP",
            "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC",
-           "ORX_OP_SCORE_RANK", "ORX_VARIANT_RANK_SMEM", "ORX_VARIANT_RANK_GLOBAL", "Dispatch"]
+           "ORX_OP_SCORE_RANK", "ORX_VARIANT_RANK_SMEM", "ORX_VARIANT_RANK_GLOBAL", "ORX_OP_SCORE_TOPK",
+           "ORX_VARIANT_TOPK", "Dispatch"]
 
 _engines = {}
 
@@ -60,6 +61,20 @@ def table(var, s0=None, s1=None):
 
 def opt(kind, lr, eps=1e-7, beta1=0.9, beta2=0.999, step=1):
     return OrxOpt(kind, lr, eps, beta1, beta2, step)
+
+
+def _csr(off, items, n_rows):
+    """Check a per-user CSR list (int64 offsets [n_rows + 1], int32 items, on the device) -> (off, items or None when
+    empty); (None, None) when off is None."""
+    if off is None:
+        return None, None
+    if not (off.is_cuda and off.dtype == torch.int64 and off.is_contiguous()):
+        raise ValueError("CSR offsets: expected a contiguous int64 CUDA tensor")
+    if not (items.is_cuda and items.dtype == torch.int32 and items.is_contiguous()):
+        raise ValueError("CSR items: expected a contiguous int32 CUDA tensor")
+    if off.numel() != n_rows + 1:
+        raise ValueError("CSR offsets must have one entry per user row plus one")
+    return off, items if items.numel() else None
 
 
 class Engine:
@@ -292,20 +307,8 @@ class Engine:
         -> (auc [Bu], ndcg [Bu, len(at)], recall [Bu, len(at)])."""
         uid = ids32(uid)
         Bu, dev = uid.numel(), item_tab.device
-
-        def csr(off, items):
-            if off is None:
-                return None, None
-            if not (off.is_cuda and off.dtype == torch.int64 and off.is_contiguous()):
-                raise ValueError("CSR offsets: expected a contiguous int64 CUDA tensor")
-            if not (items.is_cuda and items.dtype == torch.int32 and items.is_contiguous()):
-                raise ValueError("CSR items: expected a contiguous int32 CUDA tensor")
-            if off.numel() != user_tab.shape[0] + 1:
-                raise ValueError("CSR offsets must have one entry per user row plus one")
-            return off, items if items.numel() else None
-
-        pos_off, pos_items = csr(pos_off, pos_items)
-        excl_off, excl_items = csr(excl_off, excl_items)
+        pos_off, pos_items = _csr(pos_off, pos_items, user_tab.shape[0])
+        excl_off, excl_items = _csr(excl_off, excl_items, user_tab.shape[0])
         if pos_off is None:
             raise ValueError("score_rank needs the positives' CSR")
         at_arr = (C.c_int32 * max(len(at), 1))(*[int(k) for k in at])
@@ -318,6 +321,25 @@ class Engine:
             _ptr(pos_items), _ptr(excl_off), _ptr(excl_items), int(max_pos), at_arr, len(at), _ptr(auc), _ptr(ndcg),
             _ptr(rec), self.stream()), "orx_score_rank")
         return auc, ndcg, rec
+
+    def score_topk(self, kind, user_tab, uid, item_tab, item_bias, excl_off, excl_items, k, scale=None):
+        """The k best eligible items of each user uid in one pass over the item table, without the [Bu, I] score
+        matrix: order score descending then item ascending, the user's CSR exclusion row (excl_off / excl_items as in
+        score_rank, may be None) and NaN scores left out, slots past the eligible items padded with item -1 and score
+        -inf.  -> (items int32 [Bu, k], scores float32 [Bu, k]), scores bit-equal to score_all's (-0.0 may read +0.0)."""
+        uid = ids32(uid)
+        Bu, dev = uid.numel(), item_tab.device
+        excl_off, excl_items = _csr(excl_off, excl_items, user_tab.shape[0])
+        k = int(k)
+        if not 1 <= k <= _lib.ORX_MAX_TOPK:
+            raise ValueError(f"k must lie in [1, {_lib.ORX_MAX_TOPK}]")
+        items = torch.empty((Bu, k), dtype=torch.int32, device=dev)
+        scores = torch.empty((Bu, k), dtype=torch.float32, device=dev)
+        _lib.check(self.lib.orx_score_topk(
+            self.h, kind, _ptr(_f32(user_tab, "user_tab")), user_tab.shape[0], _ptr(uid), Bu, _ptr(scale),
+            _ptr(_f32(item_tab, "item_tab")), _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(excl_off),
+            _ptr(excl_items), k, _ptr(items), _ptr(scores), self.stream()), "orx_score_topk")
+        return items, scores
 
 
 def engine(device=None) -> Engine:

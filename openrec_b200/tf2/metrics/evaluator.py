@@ -14,22 +14,7 @@ import torch
 from ... import native as N
 from ..._lib import ORX_MAX_AT
 from ...tfshim.core import Tensor
-
-
-def _csr(n_rows, rows):
-    """{user: iterable of items} -> (offsets int64 [n_rows + 1], items int32): each row sorted and unique, users
-    without an entry (or outside [0, n_rows)) empty."""
-    lens = np.zeros(n_rows, dtype=np.int64)
-    parts = {}
-    for u, items in rows.items():
-        u = int(u)
-        if 0 <= u < n_rows:
-            parts[u] = np.unique(np.fromiter(items, dtype=np.int64))
-            lens[u] = len(parts[u])
-    off = np.zeros(n_rows + 1, dtype=np.int64)
-    np.cumsum(lens, out=off[1:])
-    items = np.concatenate([parts[u] for u in sorted(parts)]) if parts else np.zeros(0, dtype=np.int64)
-    return off, items.astype(np.int32)
+from ..data.user_lists import positives_csr, user_csr
 
 
 class RankingEvaluator:
@@ -51,13 +36,8 @@ class RankingEvaluator:
         self.batch_size = int(batch_size)
         n_users = store.total_users()
         self.warm_users = np.asarray(store.warm_users(), dtype=np.int64)
-        self.pos_off, self.pos_items = _csr(n_users, {u: store.get_positive_items(u) for u in self.warm_users})
-        excl = {}
-        for ds in excl_datasets:
-            other = ds.datastore
-            for u in other.warm_users():
-                excl.setdefault(int(u), set()).update(other.get_positive_items(u))
-        self.excl_off, self.excl_items = _csr(n_users, excl)
+        self.pos_off, self.pos_items = user_csr(n_users, {u: store.get_positive_items(u) for u in self.warm_users})
+        self.excl_off, self.excl_items = positives_csr(n_users, excl_datasets)
         self._pos_len = np.diff(self.pos_off)
         self.max_pos = int(self._pos_len.max()) if n_users else 0
         self._dev = None

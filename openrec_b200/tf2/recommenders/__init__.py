@@ -3,8 +3,9 @@ from .bpr import BPR
 from .wrmf import WRMF
 from .gmf import GMF
 from .ucml import UCML
+from .retriever import Retriever
 
-__all__ = ["BPR", "WRMF", "GMF", "UCML"]
+__all__ = ["BPR", "WRMF", "GMF", "UCML", "Retriever"]
 try:  # DLRM needs the MLP / interaction kernels
     from .dlrm import DLRM  # noqa: F401
     __all__.append("DLRM")

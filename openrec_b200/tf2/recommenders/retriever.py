@@ -1,0 +1,62 @@
+"""Retriever -- each user's k best unseen items at catalogue scale, in one fused liborx call per batch of users
+(orx_score_topk): the users are scored against the whole item table and only the k best items of each are kept, so the
+[users, items] score matrix of ``model.inference`` is never built.
+
+The result equals ``model.inference(users)`` with the users' excluded items left out, ordered by score descending and
+then item id ascending (NaN scores are never returned), cut at k and padded with item -1 / score -inf when fewer items
+remain.  The union of the positives of ``excl_datasets`` becomes one CSR list over user ids, uploaded once per device.
+The reference's tf2 package has no serving path; its tf1 ``FastDotProductServer`` is the closest counterpart."""
+from __future__ import annotations
+
+import torch
+
+from ... import native as N
+from ..._lib import ORX_MAX_TOPK
+from ...tfshim.core import Tensor
+from ..data.user_lists import positives_csr
+from ._base import ids_of
+
+
+class Retriever:
+    """``Retriever(excl_datasets=[train_dataset], k=10, batch_size=1024).recommend(model, user_id)`` -> (items, scores),
+    int32 / float32 ``Tensor``s of shape [n, k] on the model's device, n = the number of ids in ``user_id`` (a host or
+    device array of ints of any shape, flattened).  Models: BPR, UCML, GMF, WRMF."""
+
+    def __init__(self, excl_datasets=[], k=10, batch_size=1024):
+        k = int(k)
+        if not 1 <= k <= ORX_MAX_TOPK:
+            raise ValueError(f"k must lie in [1, {ORX_MAX_TOPK}]")
+        if batch_size < 1:
+            raise ValueError("batch_size must be positive")
+        totals = {int(ds.datastore.total_users()) for ds in excl_datasets}
+        if len(totals) > 1:
+            raise ValueError(f"excl_datasets disagree on total_users: {sorted(totals)}")
+        self.k, self.batch_size = k, int(batch_size)
+        self.excl_off, self.excl_items = positives_csr(totals.pop(), excl_datasets) if totals else (None, None)
+        self._dev = None
+
+    def _upload(self, device):
+        if self.excl_off is None:
+            return None, None
+        if self._dev is None or self._dev[0] != device:
+            self._dev = (device, torch.from_numpy(self.excl_off).to(device), torch.from_numpy(self.excl_items).to(device))
+        return self._dev[1:]
+
+    def recommend(self, model, user_id):
+        ops = getattr(model, "_score_operands", None)
+        if ops is None:
+            raise NotImplementedError(f"{type(model).__name__}: catalogue retrieval needs the model's whole item "
+                                      "table on one device (BPR, UCML, GMF, WRMF)")
+        kind, user, item, bias, scale = ops()
+        uids = ids_of(user_id)
+        excl_off, excl_items = self._upload(item.device)
+        eng = N.engine()
+        items, scores = [], []
+        for b0 in range(0, uids.numel(), self.batch_size):
+            it, sc = eng.score_topk(kind, user, uids[b0:b0 + self.batch_size], item, bias, excl_off, excl_items,
+                                    self.k, scale=scale)
+            items.append(it), scores.append(sc)
+        if not items:
+            return (Tensor(torch.zeros((0, self.k), dtype=torch.int32, device=item.device)),
+                    Tensor(torch.zeros((0, self.k), dtype=torch.float32, device=item.device)))
+        return Tensor(torch.cat(items)), Tensor(torch.cat(scores))
