@@ -84,6 +84,11 @@ static int alloc_hash(OrxHash& t, int64_t lookups, int32_t* counter) {
 // staged (ADAM_DENSE stages all rows), so the staging buffers hold B resp. 2B rows of `dim` floats.
 int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim) {
   if (B <= c->cap_B && dim <= c->g_dim) return ORX_OK;
+  if (orx_shard_holds_index(c)) {
+    orx_set_error("workspace growth to %lld lookups / dim %d refused: a sharded step's announced batch holds this "
+                  "handle's index sets until its orx_shard_step call", (long long)B, dim);
+    return ORX_ERR_INVALID;
+  }
   int64_t nb = B > c->cap_B ? B : c->cap_B;
   int32_t nd = dim > c->g_dim ? dim : c->g_dim;
   ORX_CUDA(cudaDeviceSynchronize());
@@ -124,6 +129,11 @@ static int zero_hash(OrxHash& t) {
 }
 
 int orx_next_epoch(orx_ctx* c, cudaStream_t /*st*/) {
+  if (c->epoch == 0x7fffffffu && orx_shard_holds_index(c)) {
+    orx_set_error("index epoch wrap refused: a sharded step's announced batch holds this handle's index sets until its "
+                  "orx_shard_step call");
+    return ORX_ERR_INVALID;
+  }
   c->epoch = (c->epoch + 1) & 0x7fffffffu;
   if (c->epoch == 0) {
     // 31-bit wrap (once per 2^31 index builds): a stale slot could alias the epochs to come, so every table is emptied.

@@ -560,6 +560,8 @@ extern "C" int orx_pairwise_prefetch(orx_handle_t h, const orx_table_t* user, co
                                      orx_stream_t ids_stream) {
   ORX_REQUIRE(h != nullptr && user && item && uid && pid && nid && B > 0, "bad arguments");
   ORX_REQUIRE(orx_opt_kind_ok(opt_kind), "unknown optimizer kind");
+  ORX_REQUIRE(!orx_shard_holds_index(h), "a sharded step's announced batch holds this handle's index sets (a prefetch "
+                                         "would overwrite one) until its orx_shard_step call");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t is = (cudaStream_t)ids_stream;
   int rc = orx_ensure_workspace(h, B, user->dim);
@@ -658,6 +660,8 @@ extern "C" int orx_pairwise_step_host(orx_handle_t h, int32_t kind, const orx_ta
                                       const orx_opt_t* opt, float* out4_host, orx_stream_t s) {
   ORX_REQUIRE(h != nullptr, "null handle");
   ORX_REQUIRE(B > 0 && uid_host && pid_host && nid_host && out4_host && user && item && opt, "empty batch or null host buffers");
+  ORX_REQUIRE(!orx_shard_holds_index(h), "a sharded step's announced batch holds this handle's index sets (this entry "
+                                         "point prefetches into one) until its orx_shard_step call");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
   int rc = orx_ensure_stage(h, 3 * (int64_t)B);

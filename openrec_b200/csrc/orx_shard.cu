@@ -793,6 +793,12 @@ static void shard_ws_free(orx_ctx* c) {
 
 void orx_shard_ws_release(orx_ctx* c) { shard_ws_free(c); }
 
+// A route issued for a step whose tail has not been issued yet: that step's user index lives in pf_u[its parity]
+bool orx_shard_holds_index(const orx_ctx* c) {
+  const orx_shard_ws* s = (const orx_shard_ws*)c->shard_ws;
+  return s && (s->pro_route[0] > s->tail_epoch || s->pro_route[1] > s->tail_epoch);
+}
+
 static int shard_ws_ensure(orx_ctx* c, const ShardHost* x, cudaStream_t st) {
   orx_shard_ws* s = (orx_shard_ws*)c->shard_ws;
   const int got_rows = sh_got_rows(x->home_cap, x->world);

@@ -390,13 +390,26 @@ class LoopbackGroup:
         for ph in range(6):       # phases 0 / 1 of an announced batch were issued a step ago: the C call skips them
             fused = ph == 4 and next_batches is not None and self.world == 1    # one rank: the real fused launch
             if ph == 4 and next_batches is not None and not fused:
-                for early in (0, 1):
-                    for r, m in enumerate(self.ranks):
-                        m._call(*next_batches[r], c_loss, c_l2, early, early, epoch=m.iterations + 1)
+                self._issue_early(next_batches, c_loss, c_l2)
             for r, m in enumerate(self.ranks):
                 outs[r] = m._call(*batches[r], c_loss, c_l2, ph, ph, nxt=next_batches[r] if fused else None)
         self._announced = [tuple(b) for b in next_batches] if next_batches is not None else None
         return [o[:2] for o in outs]
+
+    def _issue_early(self, next_batches, c_loss, c_l2):
+        """Route (phase 0) of the announced batches for every rank, then request (phase 1).  A rank whose index epochs
+        are about to wrap refuses its route: the wrap empties its index sets, so it must wait for this step's tail.  The
+        fused prologue skips itself in that case; here the request phase is skipped for every rank, and the next step's
+        call issues the routes that are still missing and all requests."""
+        for r, m in enumerate(self.ranks):
+            try:
+                m._call(*next_batches[r], c_loss, c_l2, 0, 0, epoch=m.iterations + 1)
+            except RuntimeError as e:
+                if "about to wrap" not in str(e):
+                    raise
+                return
+        for r, m in enumerate(self.ranks):
+            m._call(*next_batches[r], c_loss, c_l2, 1, 1, epoch=m.iterations + 1)
 
     def load_global(self, user, item, bias):
         for m in self.ranks:
