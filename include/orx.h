@@ -11,7 +11,9 @@
  *    cudaStream_t passed as void*; NULL = the legacy default stream);
  *  - every pointer is a DEVICE pointer unless its name ends in _host;
  *  - the caller owns every buffer; the library allocates only the opaque per-device workspace
- *    held by an orx_handle_t (index hash tables, duplicate-row gradient staging, id staging);
+ *    held by an orx_handle_t (index hash sets and duplicate-row gradient staging, loss partials,
+ *    id staging, evaluation scratch, sharded-step scratch, split-K partials), keeps no device
+ *    state outside it, and orx_destroy frees all of it.  Two handles share nothing;
  *  - all calls are asynchronous w.r.t. the host and ordered on the given stream;
  *  - return value: ORX_OK (0) or a negative orx_status; orx_last_error_string() gives the
  *    thread-local message.  There is no CPU fallback: without a CUDA device every compute

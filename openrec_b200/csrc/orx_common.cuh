@@ -58,19 +58,19 @@ struct orx_ctx {
   float *gu, *gi, *gb, *gw;
   int64_t g_rows_u, g_rows_i;
   int32_t g_dim;
-  // loss partials
-  float* partials;  // [cap_partials*2]
-  int32_t cap_partials;
+  // loss partials: (loss, l2) float pairs
+  float* partials;
+  size_t partials_cap;   // bytes
   // id staging for the *_host entry points (double buffered)
   int32_t* ids_stage[2];
+  size_t stage_cap[2];   // bytes
   float* out_stage[2];
-  int64_t stage_cap;
   uint32_t stage_flip;
   // measurement hook (orx_profile_*)
   int prof_on, prof_n, prof_cap;
   int prof_step;  // steps seen since orx_profile_enable: every 8th one carries the phase events
   cudaEvent_t* prof_ev;  // [prof_cap * ORX_PROF_EV]
-  int32_t* bucket_cursor;  // owner-bucket scratch
+  int32_t* bucket_cursor;  // [1024] owner-bucket scratch
   cudaStream_t side_stream;  // id upload + index build of the NEXT pairwise batch, beside the running step
   cudaEvent_t side_ev;       // "ids are final" point of orx_pairwise_prefetch on the caller's ids stream
   cudaEvent_t pf_done[2], pf_free[2], stage_free[2];   // prefetched index k built / handed back; id staging f free
@@ -79,12 +79,22 @@ struct orx_ctx {
   const int32_t *pf_uid, *pf_pid, *pf_nid;
   int64_t pf_rows_u, pf_rows_i;
   uint32_t epoch;          // hash epoch of the last step, in [1, 2^31)
-  void* shard_ws;          // orx_shard.cu: local scratch of the row-sharded step (orx_shard_ws*)
+  void* shard_ws;          // orx_shard.cu: host bookkeeping of the row-sharded step (orx_shard_ws*)
+  void* shard_scratch;     // orx_shard.cu: its local device scratch, carved by sh_layout
+  size_t shard_cap;
   int32_t dispatch[ORX_DISPATCH_LOG_CAP][8];   // orx_debug_dispatch_log: ring of the last DLRM / sparse-step launches
   int64_t dispatch_n;      // records written since the last read
   void* eval_ws;           // orx_eval.cu: scratch of orx_score_rank / orx_score_topk, its own allocation
   size_t eval_cap;
+  float* splitk;           // split-K partials of the Dense-layer GEMMs and of the split column sum
+  size_t splitk_cap;
 };
+
+// Grow a workspace buffer of the handle to at least `need` bytes (*cap = its size in bytes).  Returns at once when it is
+// large enough; otherwise drains the device (the old buffer may be in use on any stream), frees it and allocates the
+// new one.  A failed allocation leaves *buf null and *cap 0 and returns ORX_ERR_NOMEM; a failed drain returns
+// ORX_ERR_CUDA with the buffer untouched.
+int orx_grow(void** buf, size_t* cap, size_t need);
 
 // append {op, variant, TA, TB, M, N, K, S} to the handle's dispatch ring (host only)
 static inline void orx_log_dispatch(orx_ctx* c, int op, int variant, int TA, int TB, int M, int N, int K, int S) {
@@ -119,17 +129,7 @@ static inline void orx_prof_next(orx_ctx* c) {
   c->prof_step++;
 }
 
-// SM count of the current device (cached per device), for grid sizing where no handle is at hand
-static inline int orx_current_sms() {
-  static int sms[64] = {0};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
-  if (sms[dev] <= 0 && cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms[dev] = 0;
-  return sms[dev] > 0 ? sms[dev] : 132;
-}
-
 int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim);
-int orx_ensure_stage(orx_ctx* c, int64_t n_ints);
 
 // Runtime kind -> template argument: calls f(std::integral_constant<int, V>{}) for the V among Vs equal to v, and for the
 // last of Vs when none is (every entry point validates v, with its own error message, before it dispatches).  Only the
@@ -574,7 +574,6 @@ TailArgs orx_tail_args(const orx_ctx* c, const orx_table_t* user, const orx_tabl
 int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
                            const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o, cudaStream_t st);
 int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st);
-int orx_ensure_partials(orx_ctx* c, int need, cudaStream_t st);
 int orx_launch_reduce_partials(const float* partials, int n, float loss_scale, float* out4, cudaStream_t st);
 // index of n samples (a[t], b0[t]) or (a[t], b0[t], b1[t]); only samples whose ids are all in range are inserted
 int orx_launch_index_build(orx_ctx* c, const int32_t* a, int64_t rows_a, const int32_t* b0, const int32_t* b1,

@@ -170,15 +170,20 @@ extern "C" int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec, int32_t cap,
   return ORX_OK;
 }
 
-int orx_ensure_stage(orx_ctx* c, int64_t n_ints) {
-  if (n_ints <= c->stage_cap) return ORX_OK;
+int orx_grow(void** buf, size_t* cap, size_t need) {
+  if (need <= *cap) return ORX_OK;
   ORX_CUDA(cudaDeviceSynchronize());
-  for (int i = 0; i < 2; ++i) {
-    cudaFree(c->ids_stage[i]);
-    c->ids_stage[i] = nullptr;
-    ORX_CUDA(cudaMalloc(&c->ids_stage[i], sizeof(int32_t) * (size_t)n_ints));
+  cudaFree(*buf);
+  *buf = nullptr;
+  *cap = 0;
+  const cudaError_t e = cudaMalloc(buf, need);
+  if (e != cudaSuccess) {
+    cudaGetLastError();   // not left behind for the next launch check to report
+    *buf = nullptr;
+    orx_set_error("workspace allocation of %zu bytes failed: %s", need, cudaGetErrorString(e));
+    return ORX_ERR_NOMEM;
   }
-  c->stage_cap = n_ints;
+  *cap = need;
   return ORX_OK;
 }
 
@@ -200,13 +205,14 @@ extern "C" int orx_create(int device, orx_handle_t* out) {
   memset(c, 0, sizeof(*c));
   c->device = device;
   c->num_sms = prop.multiProcessorCount;
-  c->cap_partials = c->num_sms * 64;
+  c->partials_cap = sizeof(float) * 2 * (size_t)c->num_sms * 64;
   if (cudaMalloc(&c->counters, sizeof(int32_t) * 16) != cudaSuccess ||
-      cudaMalloc(&c->partials, sizeof(float) * 2 * (size_t)c->cap_partials) != cudaSuccess ||
+      cudaMalloc(&c->bucket_cursor, sizeof(int32_t) * 1024) != cudaSuccess ||
+      cudaMalloc(&c->partials, c->partials_cap) != cudaSuccess ||
       cudaMalloc(&c->out_stage[0], sizeof(float) * 8) != cudaSuccess ||
       cudaMalloc(&c->out_stage[1], sizeof(float) * 8) != cudaSuccess) {
     orx_set_error("orx_create: workspace allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
-    delete c;
+    orx_destroy(c);
     return ORX_ERR_NOMEM;
   }
   cudaMemset(c->counters, 0, sizeof(int32_t) * 16);
@@ -227,6 +233,8 @@ extern "C" int orx_destroy(orx_handle_t h) {
   cudaFree(h->partials);
   cudaFree(h->bucket_cursor);
   cudaFree(h->eval_ws);
+  cudaFree(h->splitk);
+  cudaFree(h->shard_scratch);
   orx_shard_ws_release(h);
   if (h->side_stream) {
     cudaStreamDestroy(h->side_stream);

@@ -307,8 +307,7 @@ extern "C" int orx_interact_fwd(orx_handle_t h, const float* emb, int64_t emb_ld
   ORX_CUDA(cudaSetDevice(h->device));
   if (inter_fast_ok(F, D, mode, emb ? (const void*)emb : (const void*)dense, dense, emb_ld, dense_ld)) {
     const size_t sm = sizeof(float4) * (size_t)INTER_WARPS * F * 32;
-    static bool attr = false;
-    if (!attr) { ORX_CUDA(cudaFuncSetAttribute(k_interact_fwd_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
+    ORX_CUDA(cudaFuncSetAttribute(k_interact_fwd_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     int grid = (B + INTER_WARPS - 1) / INTER_WARPS;
     if (grid > h->num_sms * 4) grid = h->num_sms * 4;
     k_interact_fwd_warp<<<grid, INTER_WARPS * 32, sm, (cudaStream_t)s>>>(emb, emb_ld, dense, dense_ld, B, F, D, self_interaction, out, out_ld);
@@ -336,8 +335,7 @@ extern "C" int orx_interact_bwd(orx_handle_t h, const float* emb, int64_t emb_ld
   if (inter_fast_ok(F, D, mode, emb ? (const void*)emb : (const void*)dense, dense, emb_ld, dense_ld) && (demb_ld & 3) == 0 &&
       (ddense_ld & 3) == 0 && ((((uintptr_t)(demb ? (const void*)demb : (const void*)ddense)) | ((uintptr_t)ddense)) & 15) == 0) {
     const size_t sm = (size_t)INTER_WARPS * (sizeof(float4) * (size_t)F * 32 + sizeof(float) * (size_t)F * 36);
-    static bool attr = false;
-    if (!attr) { ORX_CUDA(cudaFuncSetAttribute(k_interact_bwd_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); attr = true; }
+    ORX_CUDA(cudaFuncSetAttribute(k_interact_bwd_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     int grid = (B + INTER_WARPS - 1) / INTER_WARPS;
     if (grid > h->num_sms * 3) grid = h->num_sms * 3;
     k_interact_bwd_warp<<<grid, INTER_WARPS * 32, sm, (cudaStream_t)s>>>(emb, emb_ld, dense, dense_ld, dout, dout_ld, B, F, D, self_interaction, demb, demb_ld, ddense, ddense_ld);
@@ -428,7 +426,6 @@ __global__ void __launch_bounds__(256) k_gemm(const float* __restrict__ A, int64
 
 int orx_launch_gemm_tc(orx_ctx* h, int TA, int TB, const float* A, int64_t lda, const float* Bm, int64_t ldb, float* C,
                        int64_t ldc, int M, int N, int K, const float* bias, int act, cudaStream_t st);   // orx_mlp_tc.cu
-float* orx_splitk_workspace(size_t floats);                                                  // orx_mlp_tc.cu
 int orx_launch_splitk_reduce(const float* part, int S, int M, int N, float* C, int64_t ldc, const float* bias, int act,
                              cudaStream_t st);
 
@@ -440,7 +437,7 @@ static int launch_gemm(orx_ctx* h, const float* A, int64_t lda, const float* Bm,
   if (rc != ORX_ERR_UNSUPPORTED) return rc;
   const int tiles = ((N + 63) / 64) * ((M + 63) / 64);
   int S = 1;
-  const int sms = orx_current_sms();
+  const int sms = h->num_sms;
   if (tiles < sms && K >= 1024) {   // dw of a narrow layer (13 x 512, 256 x 1): K = batch, a handful of tiles
     S = (2 * sms + tiles - 1) / tiles;
     if (S > K / 256) S = K / 256;
@@ -448,8 +445,9 @@ static int launch_gemm(orx_ctx* h, const float* A, int64_t lda, const float* Bm,
   }
   float* part = nullptr;
   if (S > 1) {
-    part = orx_splitk_workspace((size_t)S * (size_t)M * (size_t)N);
-    if (!part) { orx_set_error("split-K workspace allocation failed"); return ORX_ERR_CUDA; }
+    const int rc2 = orx_grow((void**)&h->splitk, &h->splitk_cap, sizeof(float) * (size_t)S * (size_t)M * (size_t)N);
+    if (rc2) return rc2;
+    part = h->splitk;
   }
   dim3 grid((N + 63) / 64, (M + 63) / 64, S);
   k_gemm<TA, TB><<<grid, 256, 0, st>>>(A, lda, Bm, ldb, C, ldc, M, N, K, bias, act, part);
@@ -524,11 +522,12 @@ extern "C" int orx_mlp_layer_bwd(orx_handle_t h, const float* x, int64_t ldx, co
       if (S > B / 256) S = B / 256;
     }
     if (S > 1) {
-      float* part = orx_splitk_workspace((size_t)S * (size_t)out);
-      if (!part) { orx_set_error("split workspace allocation failed"); return ORX_ERR_CUDA; }
+      int rc2 = orx_grow((void**)&h->splitk, &h->splitk_cap, sizeof(float) * (size_t)S * (size_t)out);
+      if (rc2) return rc2;
+      float* part = h->splitk;
       k_col_sum<<<dim3(cb, S), 256, 0, st>>>(dy, lddy, B, out, part);
       ORX_LAUNCH_CHECK();
-      const int rc2 = orx_launch_splitk_reduce(part, S, 1, out, db, out, nullptr, 0, st);
+      rc2 = orx_launch_splitk_reduce(part, S, 1, out, db, out, nullptr, 0, st);
       if (rc2) return rc2;
     } else {
       k_col_sum<<<cb, 256, 0, st>>>(dy, lddy, B, out, db);
@@ -593,7 +592,7 @@ extern "C" int orx_pred_loss(orx_handle_t h, const float* pred, const float* lab
   cudaStream_t st = (cudaStream_t)s;
   int blocks = (B + 255) / 256;
   if (blocks > 256) blocks = 256;
-  int rc = orx_ensure_partials(h, blocks, st);
+  const int rc = orx_grow((void**)&h->partials, &h->partials_cap, sizeof(float) * 2 * (size_t)blocks);
   if (rc) return rc;
   k_pred_loss<<<blocks, 256, 0, st>>>(pred, label, B, kind, clip_threshold, pred_out, dpred, h->partials);
   ORX_LAUNCH_CHECK();

@@ -789,20 +789,6 @@ int ev_item_splits(const orx_ctx* h, Kern kern, size_t dyn, int Bu, int64_t I, i
   return ORX_OK;
 }
 
-// The handle's evaluation scratch, at least `need` bytes.  Grown like the index workspace: drain the device, then
-// replace the allocation.  It is its own allocation, so it never aliases a prefetched batch index.
-int ev_scratch(orx_ctx* h, size_t need) {
-  if (need > h->eval_cap) {
-    ORX_CUDA(cudaDeviceSynchronize());
-    cudaFree(h->eval_ws);
-    h->eval_ws = nullptr;
-    h->eval_cap = 0;
-    ORX_CUDA(cudaMalloc(&h->eval_ws, need));
-    h->eval_cap = need;
-  }
-  return ORX_OK;
-}
-
 template <int KIND>
 int ev_launch(orx_ctx* h, const EvalArgs& a, const EvalWs& w, const EvalOut& o, cudaStream_t st) {
   auto kern = k_score_rank<KIND>;
@@ -851,7 +837,7 @@ int tk_launch(orx_ctx* h, const EvalArgs& a, int k, int32_t* top_items, float* t
   int rc = ev_item_splits(h, k_score_topk<KIND>, 0, a.Bu, a.I, &splits);
   if (rc != ORX_OK) return rc;
   TopkWs w;
-  rc = ev_scratch(h, tk_layout(nullptr, a.Bu, splits, k, &w));
+  rc = orx_grow(&h->eval_ws, &h->eval_cap, tk_layout(nullptr, a.Bu, splits, k, &w));
   if (rc != ORX_OK) return rc;
   tk_layout(static_cast<char*>(h->eval_ws), a.Bu, splits, k, &w);
   const int64_t user_tiles = (a.Bu + EV_TU - 1) / EV_TU;
@@ -885,7 +871,7 @@ extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_ta
   size_t sort_bytes = 0;
   ORX_CUDA(cub::DeviceSegmentedSort::SortKeys((void*)nullptr, sort_bytes, (const float*)nullptr, (float*)nullptr,
                                               (int)(2 * Bu * P), 2 * Bu, (const int*)nullptr, (const int*)nullptr, st));
-  const int rc = ev_scratch(h, ev_layout(nullptr, Bu, (int)P, sort_bytes, &w));
+  const int rc = orx_grow(&h->eval_ws, &h->eval_cap, ev_layout(nullptr, Bu, (int)P, sort_bytes, &w));
   if (rc != ORX_OK) return rc;
   ev_layout(static_cast<char*>(h->eval_ws), Bu, (int)P, sort_bytes, &w);
 

@@ -365,11 +365,7 @@ int make_map(CUtensorMap* tm, const float* base, int rows, int K, int64_t ld, bo
 template <int TA, int TB>
 int launch_tma(const CUtensorMap& ta, const CUtensorMap& tb, float* C, int64_t ldc, int M, int N, int K, const float* bias,
                int act, float* part, int S, cudaStream_t st) {
-  static bool done = false;
-  if (!done) {
-    ORX_CUDA(cudaFuncSetAttribute(k_gemm_tma<TA, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM + 1024));
-    done = true;
-  }
+  ORX_CUDA(cudaFuncSetAttribute(k_gemm_tma<TA, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM + 1024));
   dim3 grid((N + TN - 1) / TN, (M + TM - 1) / TM, S);
   k_gemm_tma<TA, TB><<<grid, THREADS, SMEM + 1024, st>>>(ta, tb, C, ldc, M, N, K, bias, act, part);
   ORX_LAUNCH_CHECK();
@@ -378,23 +374,6 @@ int launch_tma(const CUtensorMap& ta, const CUtensorMap& tb, float* C, int64_t l
 
 }  // namespace
 
-// split-K workspace: one buffer per device (indexed by the current device), grown on demand, reused by every GEMM /
-// column sum of that device's stream in order
-static float* g_part[64] = {nullptr};
-static size_t g_part_floats[64] = {0};
-float* orx_splitk_workspace(size_t floats) {
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
-  if (floats > g_part_floats[dev]) {
-    cudaDeviceSynchronize();
-    cudaFree(g_part[dev]);
-    g_part[dev] = nullptr;
-    g_part_floats[dev] = 0;
-    if (cudaMalloc(&g_part[dev], sizeof(float) * floats) != cudaSuccess) return nullptr;
-    g_part_floats[dev] = floats;
-  }
-  return g_part[dev];
-}
 int orx_launch_splitk_reduce(const float* part, int S, int M, int N, float* C, int64_t ldc, const float* bias, int act, cudaStream_t st) {
   const int64_t n = (int64_t)M * N;
   k_splitk_reduce<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(part, S, M, N, C, ldc, bias, act);
@@ -414,19 +393,19 @@ int orx_launch_gemm_tc(orx_ctx* h, int TA, int TB, const float* A, int64_t lda, 
   const int tiles = ((N + TN - 1) / TN) * ((M + TM - 1) / TM);
   const int nkb = (K + TK - 1) / TK;
   int S = 1;
-  const int sms = orx_current_sms();
+  const int sms = h->num_sms;
   if (tiles < sms && nkb >= 32) {             // too few tiles for the machine and a long K: split it
     S = (2 * sms + tiles - 1) / tiles;
     if (S > nkb / 8) S = nkb / 8;             // at least 8 k-blocks (two accumulation groups) per split
     if (S < 1) S = 1;
   }
+  int rc;
   float* part = nullptr;
   if (S > 1) {
-    part = orx_splitk_workspace((size_t)S * (size_t)M * (size_t)N);
-    if (!part) { orx_set_error("split-K workspace allocation failed"); return ORX_ERR_CUDA; }
+    if ((rc = orx_grow((void**)&h->splitk, &h->splitk_cap, sizeof(float) * (size_t)S * (size_t)M * (size_t)N))) return rc;
+    part = h->splitk;
   }
   CUtensorMap ta, tb;
-  int rc;
   if ((rc = make_map(&ta, A, M, K, lda, TA == 0, TM))) return rc;
   if ((rc = make_map(&tb, Bm, N, K, ldb, TB == 1, TN))) return rc;
 #define ORX_TMA(a, b) rc = launch_tma<a, b>(ta, tb, C, ldc, M, N, K, bias, act, part, S, st)

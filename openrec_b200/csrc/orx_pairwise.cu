@@ -598,7 +598,8 @@ static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, con
   pa.opt = orx_opt_to_dev(opt);
   pa.gu = c->gu; pa.gi = c->gi; pa.gb = c->gb;
   pa.g_out = nullptr;
-  if ((rc = orx_ensure_partials(c, (B + 63) / 64 + 8 > c->num_sms ? (B + 63) / 64 + 8 : c->num_sms, st))) return rc;
+  const int n_part = (B + 63) / 64 + 8 > c->num_sms ? (B + 63) / 64 + 8 : c->num_sms;
+  if ((rc = orx_grow((void**)&c->partials, &c->partials_cap, sizeof(float) * 2 * (size_t)n_part))) return rc;
   pa.partials = c->partials;
   orx_prof_mark(c, 0, st);
   // index: a matching prefetched one (side stream, possibly still running), else built here on the caller's stream
@@ -664,8 +665,9 @@ extern "C" int orx_pairwise_step_host(orx_handle_t h, int32_t kind, const orx_ta
                                          "point prefetches into one) until its orx_shard_step call");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
-  int rc = orx_ensure_stage(h, 3 * (int64_t)B);
-  if (rc) return rc;
+  int rc;
+  for (int i = 0; i < 2; ++i)
+    if ((rc = orx_grow((void**)&h->ids_stage[i], &h->stage_cap[i], sizeof(int32_t) * 3 * (size_t)B))) return rc;
   if ((rc = orx_ensure_workspace(h, B, user->dim))) return rc;
   if ((rc = side_stream_ensure(h))) return rc;
   if ((rc = prefetch_drop(h, st))) return rc;
@@ -798,21 +800,11 @@ int orx_launch_reduce_partials(const float* partials, int n, float loss_scale, f
   return ORX_OK;
 }
 
-int orx_ensure_partials(orx_ctx* c, int need, cudaStream_t st) {
-  if (need <= c->cap_partials) return ORX_OK;
-  ORX_CUDA(cudaStreamSynchronize(st));
-  cudaFree(c->partials);
-  c->partials = nullptr;
-  c->cap_partials = need * 2;
-  ORX_CUDA(cudaMalloc(&c->partials, sizeof(float) * 2 * (size_t)c->cap_partials));
-  return ORX_OK;
-}
-
 // k_pair_fwd_grad over the batch of `a` (kind already validated; one partial per warp of 8 triplets) and, when out4 is
 // given, its (loss, l2) reduced into out4: the loss scaled by inv_B for BPR (mean), summed for UCML.
 static int launch_pair_fwd_grad(orx_ctx* c, int kind, PairGradArgs a, float* out4, cudaStream_t st) {
   const int nw = (a.B + 7) / 8, blocks = (nw + 7) / 8;
-  int rc = orx_ensure_partials(c, blocks * 8, st);
+  int rc = orx_grow((void**)&c->partials, &c->partials_cap, sizeof(float) * 2 * (size_t)(blocks * 8));
   if (rc) return rc;
   a.partials = c->partials;
   orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {

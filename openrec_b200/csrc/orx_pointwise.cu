@@ -336,7 +336,7 @@ extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_
   const int D = user->dim;
   const bool dense = opt->kind == ORX_OPT_ADAM_DENSE;
   if ((rc = orx_ensure_workspace(h, B, D))) return rc;
-  if ((rc = orx_ensure_partials(h, (B + 7) / 8 + 8, st))) return rc;
+  if ((rc = orx_grow((void**)&h->partials, &h->partials_cap, sizeof(float) * 2 * (size_t)((B + 7) / 8 + 8)))) return rc;
   if ((rc = orx_launch_index_build(h, uid, user->rows, iid, nullptr, item->rows, B, dense, st))) return rc;
   PointArgs pa;
   fill_point_args(pa, h, kind, user, item, item_bias, w, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2);
@@ -370,7 +370,7 @@ static int point_fwd_grad(orx_ctx* h, int kind, const orx_table_t* user, const o
   int rc = check_point(kind, user, item, bias, w, ORX_OPT_SGD);
   if (rc) return rc;
   const int nw = (B + 7) / 8, blocks = (nw + 7) / 8;
-  if ((rc = orx_ensure_partials(h, blocks * 8, st))) return rc;
+  if ((rc = orx_grow((void**)&h->partials, &h->partials_cap, sizeof(float) * 2 * (size_t)(blocks * 8)))) return rc;
   PointArgs pa;
   fill_point_args(pa, h, kind, user, item, bias, w, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2);
   pa.d_user = d_user; pa.d_item = d_item; pa.d_bias = d_bias; pa.g_out = g_out;

@@ -717,8 +717,10 @@ __global__ void __launch_bounds__(256) k_sh_tail(ShardDev x, ShardWs w, TailArgs
 // host side
 // ---------------------------------------------------------------------------------------
 struct orx_shard_ws {
-  ShardWs w;
+  ShardWs w;                         // carved from the handle's shard_scratch by sh_layout
   int home_cap, gin_cap, got_rows;
+  const void* occ_fn[32];            // sh_ctas_per_sm: resident CTAs per SM of each persistent kernel launched so far
+  int occ[32], n_occ;
   // prologue bookkeeping, per step parity: which step's route / request were issued, with which index epochs and ids
   int32_t pro_route[2], pro_request[2];
   uint32_t ep_u[2], ep_i[2];
@@ -767,31 +769,37 @@ extern "C" int orx_peer_free(orx_handle_t h, void* dev_ptr) {
   return ORX_OK;
 }
 
-// resident CTAs per SM of a 256-thread kernel (cached per kernel): persistent grids are sized to exactly one wave
-static int sh_ctas_per_sm(const void* fn, int cap) {
-  static const void* keys[64];
-  static int vals[64];
-  static int n = 0;
-  for (int i = 0; i < n; ++i)
-    if (keys[i] == fn) return vals[i] < cap ? vals[i] : cap;
+// resident CTAs per SM of a 256-thread kernel (cached per kernel in the workspace, i.e. for the handle's device):
+// persistent grids are sized to exactly one wave
+static int sh_ctas_per_sm(orx_shard_ws* s, const void* fn, int cap) {
+  for (int i = 0; i < s->n_occ; ++i)
+    if (s->occ_fn[i] == fn) return s->occ[i] < cap ? s->occ[i] : cap;
   int nb = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fn, 256, 0) != cudaSuccess || nb < 1) nb = 1;
-  if (n < 64) { keys[n] = fn; vals[n] = nb; ++n; }
+  if (s->n_occ < 32) { s->occ_fn[s->n_occ] = fn; s->occ[s->n_occ++] = nb; }
   return nb < cap ? nb : cap;
 }
 
-static void shard_ws_free(orx_ctx* c) {
-  orx_shard_ws* s = (orx_shard_ws*)c->shard_ws;
-  if (!s) return;
-  cudaFree(s->w.trip_u);
-  cudaFree(s->w.slot);
-  cudaFree(s->w.req);
-  cudaFree(s->w.ctl);
-  delete s;
-  c->shard_ws = nullptr;
+// The local scratch (trip_u | slot | req | ctl) inside one allocation; with base == nullptr only the size is computed.
+static size_t sh_layout(char* base, int home_cap, int gin_cap, ShardWs* w) {
+  size_t off = 0;
+  auto take = [&](size_t words) {
+    int32_t* p = base ? reinterpret_cast<int32_t*>(base + off) : nullptr;
+    off += (sizeof(int32_t) * words + 255) & ~(size_t)255;
+    return p;
+  };
+  w->trip_u = take((size_t)home_cap);
+  w->slot = take(2 * (size_t)home_cap);
+  w->req = take((size_t)gin_cap);
+  w->ctl = take(SH_C_WORDS);
+  return off;
 }
 
-void orx_shard_ws_release(orx_ctx* c) { shard_ws_free(c); }
+// the device scratch stays with the handle (shard_scratch, freed by orx_destroy)
+void orx_shard_ws_release(orx_ctx* c) {
+  delete (orx_shard_ws*)c->shard_ws;
+  c->shard_ws = nullptr;
+}
 
 // A route issued for a step whose tail has not been issued yet: that step's user index lives in pf_u[its parity]
 bool orx_shard_holds_index(const orx_ctx* c) {
@@ -803,15 +811,12 @@ static int shard_ws_ensure(orx_ctx* c, const ShardHost* x, cudaStream_t st) {
   orx_shard_ws* s = (orx_shard_ws*)c->shard_ws;
   const int got_rows = sh_got_rows(x->home_cap, x->world);
   if (s && s->home_cap >= x->home_cap && s->gin_cap >= x->gin_cap && s->got_rows >= got_rows) return ORX_OK;
-  ORX_CUDA(cudaStreamSynchronize(st));
-  shard_ws_free(c);
-  s = new orx_shard_ws();
-  memset(s, 0, sizeof(*s));
-  c->shard_ws = s;
-  ORX_CUDA(cudaMalloc(&s->w.trip_u, sizeof(int32_t) * (size_t)x->home_cap));
-  ORX_CUDA(cudaMalloc(&s->w.slot, sizeof(int32_t) * 2 * (size_t)x->home_cap));
-  ORX_CUDA(cudaMalloc(&s->w.req, sizeof(int32_t) * (size_t)x->gin_cap));
-  ORX_CUDA(cudaMalloc(&s->w.ctl, sizeof(int32_t) * SH_C_WORDS));
+  // a new layout starts afresh: zeroed bookkeeping and control words
+  orx_shard_ws_release(c);
+  c->shard_ws = s = new orx_shard_ws();
+  int rc = orx_grow(&c->shard_scratch, &c->shard_cap, sh_layout(nullptr, x->home_cap, x->gin_cap, &s->w));
+  if (rc) return rc;
+  sh_layout(static_cast<char*>(c->shard_scratch), x->home_cap, x->gin_cap, &s->w);
   ORX_CUDA(cudaMemsetAsync(s->w.ctl, 0, sizeof(int32_t) * SH_C_WORDS, st));
   s->home_cap = x->home_cap;
   s->gin_cap = x->gin_cap;
@@ -937,7 +942,8 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
   const int par = epoch & 1;
   const OrxOptDev od = orx_opt_to_dev(opt);
   const int nq = x->dim >> 2;
-  if ((rc = orx_ensure_partials(h, h->num_sms * 4 * 8, st))) return rc;   // compute grid <= 4 CTAs/SM x 8 warps
+  // compute grid <= 4 CTAs/SM x 8 warps, one (loss, l2) pair each
+  if ((rc = orx_grow((void**)&h->partials, &h->partials_cap, sizeof(float) * 2 * (size_t)(h->num_sms * 4 * 8)))) return rc;
   const int route_blocks = (B + 1023) / 1024;
   int request_blocks = (x->home_cap + 511) / 512;
   if (request_blocks > h->num_sms) request_blocks = h->num_sms;
@@ -988,7 +994,7 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
         ORX_REQUIRE(S->pro_request[par] == epoch, "phase 2 before this step's phases 0 and 1");
         sh_dispatch_nq(nq, [&](auto Q) {
           auto kern = k_sh_serve<decltype(Q)::value>;
-          orx_launch_pdl(kern, dim3(h->num_sms * sh_ctas_per_sm((const void*)kern, 4)), dim3(256), 0, st, xd, w,
+          orx_launch_pdl(kern, dim3(h->num_sms * sh_ctas_per_sm(S, (const void*)kern, 4)), dim3(256), 0, st, xd, w,
                          (const float*)item->var, (const float*)item_bias->var, (int64_t)item->rows, hi, epoch);
         });
         S->serve_epoch = epoch;
@@ -998,7 +1004,7 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
           sh_dispatch_opt(opt->kind, [&](auto O) {
             sh_dispatch_nq(nq, [&](auto Q) {
               auto kern = k_sh_compute<decltype(K)::value, decltype(O)::value, decltype(Q)::value>;
-              orx_launch_pdl(kern, dim3(h->num_sms * sh_ctas_per_sm((const void*)kern, 4)), dim3(256), 0, st, xd, w,
+              orx_launch_pdl(kern, dim3(h->num_sms * sh_ctas_per_sm(S, (const void*)kern, 4)), dim3(256), 0, st, xd, w,
                              ca, epoch);
             });
           });
@@ -1023,7 +1029,7 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
         sh_dispatch_opt(opt->kind, [&](auto O) {
           sh_dispatch_nq(nq, [&](auto Q) {
             auto kern = k_sh_apply<decltype(O)::value, decltype(Q)::value>;
-            const int g = h->num_sms * sh_ctas_per_sm((const void*)kern, 4) + pro.n_route + pro.n_request;
+            const int g = h->num_sms * sh_ctas_per_sm(S, (const void*)kern, 4) + pro.n_route + pro.n_request;
             orx_launch_pdl(kern, dim3(g), dim3(256), 0, st, xd, w, aa, pro, epoch);
           });
         });

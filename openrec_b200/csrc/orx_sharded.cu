@@ -74,7 +74,6 @@ extern "C" int orx_owner_bucket_combined(orx_handle_t h, const int32_t* ids, int
   cudaStream_t st = (cudaStream_t)s;
   ORX_CUDA(cudaMemsetAsync(counts, 0, sizeof(int32_t) * world, st));
   if (n == 0) return ORX_OK;
-  if (!h->bucket_cursor) ORX_CUDA(cudaMalloc(&h->bucket_cursor, sizeof(int32_t) * 1024));
   int blocks = (n + 255) / 256;
   if (blocks > h->num_sms * 4) blocks = h->num_sms * 4;
   k_owner_hist<<<blocks, 256, sizeof(int32_t) * world, st>>>(ids, n, world, counts);
