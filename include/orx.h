@@ -108,7 +108,7 @@ enum orx_dispatch_variant {
   ORX_VARIANT_INTERACT = 3,      /* k_interact_{fwd,bwd}: one CTA per sample */
   ORX_VARIANT_STEP = 4,          /* k_pair_step / k_point_step specialised on D (32, 64, 128, 256), one register buffer */
   ORX_VARIANT_STEP_PIPE = 5,     /* k_pair_step with the register double buffer (PIPE) */
-  ORX_VARIANT_STEP_GENERIC = 6,  /* k_pair_step_generic / k_point_generic: any D */
+  ORX_VARIANT_STEP_GENERIC = 6,  /* k_pair_generic / k_point_generic (fused-step mode): any D */
   ORX_VARIANT_RANK_SMEM = 7,     /* k_score_rank: thresholds and histograms of a user tile in shared memory */
   ORX_VARIANT_RANK_GLOBAL = 8,   /* k_score_rank: thresholds and histograms in the handle's global scratch */
   ORX_VARIANT_TOPK = 9           /* k_score_topk + k_topk_merge: candidate lists in the handle's global scratch */
@@ -117,8 +117,9 @@ enum orx_dispatch_variant {
 ORX_API int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec_host, int32_t cap, int32_t* n_host);
 
 /* Measurement hook (bench.py's roofline): while enabled, every 8th *_step call records CUDA events on its launch stream
- * around its launches -- pairwise / pointwise steps: [0] batch index (or the wait for a prefetched one), [1] the fused
- * gather-score-update kernel, [2] tail (+ Adam sweep); orx_shard_step: its six launches [0..5].  orx_profile_read waits
+ * around its launches -- orx_pairwise_step, orx_pairwise_step_host and orx_pointwise_step: [0] batch index (or the wait
+ * for a prefetched one), [1] the fused gather-score-update kernel, [2] tail (ADAM_DENSE: + the Adam sweeps);
+ * orx_shard_step: its six launches [0..5].  orx_profile_read waits
  * for the recorded events, returns the summed device time of the first n_phases phases (ms) and the number of steps
  * recorded since the last read, and resets the counter. */
 ORX_API int orx_profile_enable(orx_handle_t h, int32_t on);

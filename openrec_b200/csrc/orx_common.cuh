@@ -4,6 +4,7 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <functional>
 #include <initializer_list>
 #include <type_traits>
 
@@ -473,15 +474,21 @@ __device__ __forceinline__ void orx_block_sum_partials(const float* partials, in
 
 #endif  // __CUDACC__
 
-// Arguments of the shared tail kernel (staged rows -> optimizer, hash clear, loss reduction).
-struct TailArgs {
+// What every sparse-step kernel (step and tail) reads: the user, item and item-bias tables with their optimizer slots
+// (item and bias null for orx_sparse_apply), the row width, the optimizer, the batch's index sets and the handle's
+// staging rows.  PairArgs, PointArgs and TailArgs derive from it.
+struct SparseArgs {
   float *U, *Us0, *Us1;
   float *I, *Is0, *Is1;
   float *Bv, *Bs0, *Bs1;
-  int D;
-  OrxOptDev opt;
-  OrxHash hu, hi;
   float *gu, *gi, *gb;
+  OrxHash hu, hi;
+  OrxOptDev opt;
+  int D;
+};
+
+// Arguments of the shared tail kernel (staged rows -> optimizer, loss reduction).
+struct TailArgs : SparseArgs {
   const float* partials;
   int n_partials;
   float loss_scale;  // BPR: 1/B (mean), UCML: 1 (sum)
@@ -564,11 +571,38 @@ __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni)
 OrxOptDev orx_opt_to_dev(const orx_opt_t* o);
 int orx_launch_index_build_strided(orx_ctx* c, const int32_t* a, int64_t stride, int64_t rows, int32_t n,
                                    bool stage_all, cudaStream_t st);
-// The tail arguments of a step over user / item / bias (item and bias may be null) with index sets hu / hi, the handle's
-// staging rows and optimizer o; every other field is zero (partials, loss_scale, counters, out4, GMF's W / gw: the
-// caller's).
-TailArgs orx_tail_args(const orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
-                       const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o);
+// The shared arguments of a step over user / item / bias (item and bias may be null) with index sets hu / hi, the
+// handle's staging rows and optimizer o.  A derived block takes them as its first initializer: TailArgs ta = {s};
+// zeroes every other field.
+SparseArgs orx_sparse_args(const orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
+                           const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o);
+// The tables of a pairwise or pointwise step, fused or not: user, item and item bias present, user / item dims that
+// agree, int32 row ids, and the slot rows optimizer opt_kind keeps -- also on w, GMF's dense weight, when it is given.
+int orx_check_step_tables(const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
+                          const orx_table_t* w, int opt_kind);
+// Grid of every sparse-step kernel over B samples: 256 threads, 8 samples per warp.  A kernel writes at most one
+// (loss, l2) partial per warp, so 8 * orx_step_blocks(B) partials hold any step's.
+static inline int orx_step_blocks(int B) { return ((B + 7) / 8 + 7) / 8; }
+// What a family's step kernel launch reports back: the (loss, l2) partials it writes and, for the dispatch record, the
+// orx_dispatch_variant launched and its CTAs/SM bound (0 if none).
+struct OrxStepLaunch {
+  int n_partials, variant, minb;
+};
+// A family's step kernel, launched on the driver's stream with the shared arguments (index sets chosen) and the
+// handle's partials.
+typedef std::function<int(const SparseArgs& s, float* partials, OrxStepLaunch* out)> OrxStepKernel;
+// One fused pairwise or pointwise step on st: validate, workspace, partials, batch index (a pairwise batch, nid != null,
+// takes its prefetched index when one matches), profile marks 0..3, kernel(...), dispatch record {op, variant, kind,
+// opt, B, D, minb, index set}, ADAM_DENSE sweeps, tail (loss scaled by loss_scale into out4; w: GMF's dense weight,
+// updated with c_l2, or null), and the prefetched set handed back.
+int orx_sparse_step(orx_ctx* c, int op, int kind, const orx_table_t* user, const orx_table_t* item,
+                    const orx_table_t* bias, const orx_table_t* w, const int32_t* uid, const int32_t* iid,
+                    const int32_t* nid, int B, const orx_opt_t* opt, float loss_scale, float c_l2, float* out4,
+                    const OrxStepKernel& kernel, cudaStream_t st);
+// The un-fused forward / gradient kernel of a family over B samples: launch(partials, blocks) on st with the handle's
+// partials, then, when out4 is given, the (loss, l2) partials reduced into it, the loss scaled by loss_scale.
+int orx_sparse_unfused(orx_ctx* c, int B, float loss_scale, float* out4,
+                       const std::function<void(float* partials, int blocks)>& launch, cudaStream_t st);
 // ADAM_DENSE: Keras dense Adam over every row of user / item / bias (item and bias may be null), a row's summed gradient
 // taken from its side's index set (hu / hi) and staging rows.  Runs before the tail, which zeroes the staging rows.
 int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,

@@ -2,20 +2,17 @@
 #pragma once
 #include "orx_common.cuh"
 
-struct PairArgs {
-  float *U, *Us0, *Us1;
-  float *I, *Is0, *Is1;
-  float *Bv, *Bs0, *Bs1;
+struct PairArgs : SparseArgs {
   int64_t rowsU, rowsI;
-  int D;
   const int32_t *uid, *pid, *nid;
   int B;
   float margin, c_loss, c_l2, inv_B;
-  OrxOptDev opt;
-  OrxHash hu, hi;
-  float *gu, *gi, *gb;
   float* partials;
-  float* g_out;
+  // un-fused outputs (k_pair_generic MODE 1).  ld = 0: table form, outputs indexed by triplet.  ld > D: row form
+  // (orx_pairwise_grad_rows) -- U = I = fetched rows of stride ld with the item bias in column D, outputs written to the
+  // lookup's own row of d_user = d_pos = d_neg.
+  float *d_user, *d_pos, *d_neg, *d_bp, *d_bn, *g_out;
+  int64_t ld;
 };
 
 __device__ __forceinline__ float dot4(float4 a, float4 b) { return a.x * b.x + a.y * b.y + a.z * b.z + a.w * b.w; }

@@ -1,4 +1,5 @@
-// orx_pairwise.cu -- BPR / UCML fused training step (K1/K2), its batch index (K9) and tail.
+// orx_pairwise.cu -- BPR / UCML fused training step (K1/K2), its batch index (K9), the tail and the step driver shared
+// with orx_pointwise.cu.
 //
 // Reference path replaced (paths relative to the reference repo):
 //   openrec/tf2/recommenders/bpr.py:21-37, ucml.py:21-42, modules/pairwise_log_loss.py:15-34
@@ -11,11 +12,10 @@
 //          in registers, row + slots written back once (read once, written once == algorithmic bytes);
 //        * a row referenced more than once is NEVER written here: its per-sample gradient is
 //          red.global.add'ed into the compact staging buffer (so every gather sees pre-step values).
-//   3. k_pair_tail   : optimizer for the staged rows (once per unique row), staging re-zeroed,
-//                      hash cleared, deterministic loss reduction.
-#include <stdlib.h>
-#include <string.h>
-
+//   3. k_sparse_tail : optimizer for the staged rows (once per unique row), staging re-zeroed, deterministic loss
+//                      reduction.  The hash is not cleared: the next step's index uses a new epoch.
+// k_pair_step is specialised on D = 32, 64, 128, 256; k_pair_generic takes any D, as the fused step (MODE 0) and as the
+// forward / un-fused gradients (MODE 1).
 #include "orx_common.cuh"
 #include "orx_pair.cuh"
 
@@ -279,83 +279,117 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
     } else {
       atomicAdd(a.gb + dn, -g_own);
     }
-    if (a.g_out) a.g_out[t] = (KIND == ORX_PAIR_BPR) ? g_own : -g_own;
-  } else if (a.g_out && lane < CH && t < a.B) {
-    a.g_out[t] = 0.f;
   }
 
   // ---- one (loss, l2) partial per block, fixed order => deterministic
   orx_block_partial(loss_acc, l2_acc, a.partials);
 }
 
-// Any dim (e.g. the example's D=50): one triplet per warp-iteration, lanes stride the row.
-template <int KIND, int OPT>
-__global__ void __launch_bounds__(256) k_pair_step_generic(const PairArgs a) {
+// Any D (e.g. the example's D=50): one triplet per warp-iteration, lanes stride the row.  MODE 0 = fused step (launched
+// with PDL), 1 = forward / explicit (un-fused) gradients into a.d_* / a.g_out (OPT = SGD, unread), table or row form.
+// A skipped triplet (bad id) contributes nothing and, in MODE 1, gets zero gradients and g_out = 0.
+template <int KIND, int OPT, int MODE>
+__global__ void __launch_bounds__(256) k_pair_generic(const PairArgs a) {
   constexpr bool STAGE_ONLY = OrxOptSlots<OPT>::STAGE_ONLY;
-  constexpr int CH = 8;
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int D = a.D;
+  const bool row_form = MODE == 1 && a.ld != 0;
+  const int64_t ld = row_form ? a.ld : D;
   float loss_acc = 0.f, l2_acc = 0.f;
   orx_pdl_wait();
-  for (int j = 0; j < CH; ++j) {
-    const int t = warp * CH + j;
+  for (int j = 0; j < 8; ++j) {
+    const int t = warp * 8 + j;
     if (t >= a.B) break;
     const int uu = a.uid[t], pp = a.pid[t], nn = a.nid[t];
     const bool ok = uu >= 0 && uu < a.rowsU && pp >= 0 && pp < a.rowsI && nn >= 0 && nn < a.rowsI;
-    if (!ok) {
-      if (a.g_out && lane == 0) a.g_out[t] = 0.f;
-      continue;
-    }
-    int du, dp, dn;
-    const uint32_t cu = orx_hash_find<!STAGE_ONLY>(a.hu, uu, &du);
-    const uint32_t cp = orx_hash_find<!STAGE_ONLY>(a.hi, pp, &dp);
-    const uint32_t cn = orx_hash_find<!STAGE_ONLY>(a.hi, nn, &dn);
-    const bool fu = !STAGE_ONLY && cu == 1u, fp = !STAGE_ONLY && cp == 1u, fn = !STAGE_ONLY && cn == 1u;
-    float* ur = a.U + (int64_t)uu * D;
-    float* pr = a.I + (int64_t)pp * D;
-    float* nr = a.I + (int64_t)nn * D;
-    float s1 = 0.f, s2 = 0.f, sq = 0.f;
-    for (int d = lane; d < D; d += 32) {
-      const float u = ur[d], p = pr[d], n = nr[d];
-      if (KIND == ORX_PAIR_BPR) {
-        s1 += u * p;
-        s2 += u * n;
-      } else {
-        s1 += (u - p) * (u - p);
-        s2 += (u - n) * (u - n);
+    float* ur = a.U + (int64_t)uu * ld;
+    float* pr = a.I + (int64_t)pp * ld;
+    float* nr = a.I + (int64_t)nn * ld;
+    float s1 = 0.f, s2 = 0.f, sq = 0.f, bp = 0.f, bn = 0.f, lt = 0.f, g = 0.f;
+    if (ok) {
+      for (int d = lane; d < D; d += 32) {
+        const float u = ur[d], p = pr[d], n = nr[d];
+        if (KIND == ORX_PAIR_BPR) {
+          s1 += u * p;
+          s2 += u * n;
+        } else {
+          s1 += (u - p) * (u - p);
+          s2 += (u - n) * (u - n);
+        }
+        sq += u * u + p * p + n * n;
       }
-      sq += u * u + p * p + n * n;
+      bp = row_form ? pr[D] : a.Bv[pp];
+      bn = row_form ? nr[D] : a.Bv[nn];
     }
     l2_acc += sq;
     s1 = orx_group_sum<32>(s1);
     s2 = orx_group_sum<32>(s2);
-    const float bp = a.Bv[pp], bn = a.Bv[nn];
-    float lt, g;
-    pair_score<KIND>(s1, s2, bp, bn, a.margin, a.c_loss, a.inv_B, &lt, &g);
+    if (ok) pair_score<KIND>(s1, s2, bp, bn, a.margin, a.c_loss, a.inv_B, &lt, &g);
     if (lane == 0) loss_acc += lt;
-    for (int d = lane; d < D; d += 32) {
-      const float u = ur[d], p = pr[d], n = nr[d];
-      float gu, gp, gn;
-      pair_grads1<KIND>(g, a.c_l2, u, p, n, &gu, &gp, &gn);
-      const int64_t ou = (int64_t)uu * D + d, op = (int64_t)pp * D + d, on = (int64_t)nn * D + d;
-      if (fu) orx_update1<OPT>(ur + d, a.Us0 + ou, a.Us1 + ou, u, gu, a.opt);
-      else atomicAdd(a.gu + (int64_t)du * D + d, gu);
-      if (fp) orx_update1<OPT>(pr + d, a.Is0 + op, a.Is1 + op, p, gp, a.opt);
-      else atomicAdd(a.gi + (int64_t)dp * D + d, gp);
-      if (fn) orx_update1<OPT>(nr + d, a.Is0 + on, a.Is1 + on, n, gn, a.opt);
-      else atomicAdd(a.gi + (int64_t)dn * D + d, gn);
+    const float gbias = (KIND == ORX_PAIR_BPR) ? g : -g;
+    if (MODE == 0) {
+      if (!ok) continue;
+      int du, dp, dn;
+      const uint32_t cu = orx_hash_find<!STAGE_ONLY>(a.hu, uu, &du);
+      const uint32_t cp = orx_hash_find<!STAGE_ONLY>(a.hi, pp, &dp);
+      const uint32_t cn = orx_hash_find<!STAGE_ONLY>(a.hi, nn, &dn);
+      const bool fu = !STAGE_ONLY && cu == 1u, fp = !STAGE_ONLY && cp == 1u, fn = !STAGE_ONLY && cn == 1u;
+      for (int d = lane; d < D; d += 32) {
+        const float u = ur[d], p = pr[d], n = nr[d];
+        float gu, gp, gn;
+        pair_grads1<KIND>(g, a.c_l2, u, p, n, &gu, &gp, &gn);
+        const int64_t ou = (int64_t)uu * D + d, op = (int64_t)pp * D + d, on = (int64_t)nn * D + d;
+        if (fu) orx_update1<OPT>(ur + d, a.Us0 + ou, a.Us1 + ou, u, gu, a.opt);
+        else atomicAdd(a.gu + (int64_t)du * D + d, gu);
+        if (fp) orx_update1<OPT>(pr + d, a.Is0 + op, a.Is1 + op, p, gp, a.opt);
+        else atomicAdd(a.gi + (int64_t)dp * D + d, gp);
+        if (fn) orx_update1<OPT>(nr + d, a.Is0 + on, a.Is1 + on, n, gn, a.opt);
+        else atomicAdd(a.gi + (int64_t)dn * D + d, gn);
+      }
+      if (lane == 0) {
+        if (fp) orx_update1<OPT>(a.Bv + pp, a.Bs0 + pp, a.Bs1 + pp, bp, gbias, a.opt);
+        else atomicAdd(a.gb + dp, gbias);
+        if (fn) orx_update1<OPT>(a.Bv + nn, a.Bs0 + nn, a.Bs1 + nn, bn, -gbias, a.opt);
+        else atomicAdd(a.gb + dn, -gbias);
+      }
+      continue;
+    }
+    if (a.d_user || a.d_pos || a.d_neg) {
+      for (int d = lane; d < D; d += 32) {
+        float gu = 0.f, gp = 0.f, gn = 0.f;
+        if (ok) pair_grads1<KIND>(g, a.c_l2, ur[d], pr[d], nr[d], &gu, &gp, &gn);
+        if (row_form) {
+          if (ok) {
+            a.d_user[(int64_t)uu * ld + d] = gu;
+            a.d_pos[(int64_t)pp * ld + d] = gp;
+            a.d_neg[(int64_t)nn * ld + d] = gn;
+          }
+        } else {
+          const int64_t o = (int64_t)t * D + d;
+          if (a.d_user) a.d_user[o] = gu;
+          if (a.d_pos) a.d_pos[o] = gp;
+          if (a.d_neg) a.d_neg[o] = gn;
+        }
+      }
     }
     if (lane == 0) {
-      const float gbias = (KIND == ORX_PAIR_BPR) ? g : -g;
-      if (fp) orx_update1<OPT>(a.Bv + pp, a.Bs0 + pp, a.Bs1 + pp, bp, gbias, a.opt);
-      else atomicAdd(a.gb + dp, gbias);
-      if (fn) orx_update1<OPT>(a.Bv + nn, a.Bs0 + nn, a.Bs1 + nn, bn, -gbias, a.opt);
-      else atomicAdd(a.gb + dn, -gbias);
+      if (row_form) {
+        if (ok) {   // column D = bias gradient (items) / 0 (users); remaining padding columns = 0
+          for (int64_t c = D; c < ld; ++c) {
+            a.d_user[(int64_t)uu * ld + c] = 0.f;
+            a.d_pos[(int64_t)pp * ld + c] = c == D ? gbias : 0.f;
+            a.d_neg[(int64_t)nn * ld + c] = c == D ? -gbias : 0.f;
+          }
+        }
+      } else {
+        if (a.d_bp) a.d_bp[t] = gbias;
+        if (a.d_bn) a.d_bn[t] = -gbias;
+      }
       if (a.g_out) a.g_out[t] = g;
     }
   }
-  orx_block_partial(loss_acc, l2_acc, a.partials);
+  orx_warp_partial(loss_acc, l2_acc, a.partials);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -445,16 +479,28 @@ int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_
   return ORX_OK;
 }
 
-TailArgs orx_tail_args(const orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
-                       const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o) {
-  TailArgs ta;
-  memset(&ta, 0, sizeof(ta));
-  ta.U = user->var; ta.Us0 = user->s0; ta.Us1 = user->s1;
-  if (item) { ta.I = item->var; ta.Is0 = item->s0; ta.Is1 = item->s1; }
-  if (bias) { ta.Bv = bias->var; ta.Bs0 = bias->s0; ta.Bs1 = bias->s1; }
-  ta.D = user->dim; ta.opt = o; ta.hu = hu; ta.hi = hi;
-  ta.gu = c->gu; ta.gi = c->gi; ta.gb = c->gb;
-  return ta;
+SparseArgs orx_sparse_args(const orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
+                           const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o) {
+  SparseArgs s = {};
+  s.U = user->var; s.Us0 = user->s0; s.Us1 = user->s1;
+  if (item) { s.I = item->var; s.Is0 = item->s0; s.Is1 = item->s1; }
+  if (bias) { s.Bv = bias->var; s.Bs0 = bias->s0; s.Bs1 = bias->s1; }
+  s.D = user->dim; s.opt = o; s.hu = hu; s.hi = hi;
+  s.gu = c->gu; s.gi = c->gi; s.gb = c->gb;
+  return s;
+}
+
+int orx_check_step_tables(const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
+                          const orx_table_t* w, int opt_kind) {
+  ORX_REQUIRE(user && item && bias, "null table");
+  ORX_REQUIRE(user->var && item->var && bias->var, "null table storage");
+  ORX_REQUIRE(user->dim == item->dim && user->dim > 0, "user/item dims must match and be positive");
+  ORX_REQUIRE(bias->dim == 1 && bias->rows == item->rows, "item_bias must be [item.rows, 1]");
+  ORX_REQUIRE(user->rows > 0 && item->rows > 0 && user->rows <= 0x7fffffffLL && item->rows <= 0x7fffffffLL,
+              "row counts must fit int32 ids");
+  ORX_REQUIRE(!w || (w->var && w->dim == user->dim), "GMF needs w with dim == D");
+  ORX_REQUIRE(orx_opt_slots_ok(opt_kind, {user, item, bias, w}), "optimizer slot rows missing");
+  return ORX_OK;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -465,42 +511,27 @@ TailArgs orx_tail_args(const orx_ctx* c, const orx_table_t* user, const orx_tabl
 // "last arriver applies" form without the tail launch were all slower and are gone).  Re-checked on H100 SXM (700 W)
 // with the L2 priorities of k_pair_step in place, BPR Adagrad at the bench shape: CH = 16 measured the same as CH = 8,
 // 3 CTAs/SM was 1 % slower, and the register double-buffer (PIPE) 1-2 % slower at 2 or 3 CTAs/SM.
-// *variant / *minb: the orx_dispatch_variant launched and its CTAs/SM bound, for the dispatch record.
 template <int KIND, int OPT>
-static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, int* n_partials, int* variant, int* minb) {
-  const int B = pa.B;
+static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, OrxStepLaunch* out) {
   constexpr bool LAZY = (OPT == ORX_OPT_ADAM_LAZY);  // 9 rows per triplet: no register double-buffer
-  auto go = [&](auto kern, int ch, int v, int mb) {
-    const int nw = (B + ch - 1) / ch;
-    const int blocks = (nw + 7) / 8;
-    *n_partials = blocks;
-    *variant = v;
-    *minb = mb;
+  const int blocks = orx_step_blocks(pa.B);
+  // k_pair_step writes one (loss, l2) partial per block, k_pair_generic one per warp
+  auto go = [&](auto kern, int variant, int minb, int n_partials) {
+    *out = {n_partials, variant, minb};
     orx_launch_pdl(kern, dim3(blocks), dim3(256), 0, st, pa);
   };
   constexpr int PV = LAZY ? ORX_VARIANT_STEP : ORX_VARIANT_STEP_PIPE;
   switch (pa.D) {
-    case 32: go(k_pair_step<KIND, OPT, 32, 8, 2, !LAZY>, 8, PV, 2); break;
-    case 64: go(k_pair_step<KIND, OPT, 64, 8, 2, !LAZY>, 8, PV, 2); break;
+    case 32: go(k_pair_step<KIND, OPT, 32, 8, 2, !LAZY>, PV, 2, blocks); break;
+    case 64: go(k_pair_step<KIND, OPT, 64, 8, 2, !LAZY>, PV, 2, blocks); break;
     case 128:
-      if (LAZY) go(k_pair_step<KIND, OPT, 128, 8, 3, false>, 8, ORX_VARIANT_STEP, 3);
-      else go(k_pair_step<KIND, OPT, 128, 8, 4, false>, 8, ORX_VARIANT_STEP, 4);
+      if constexpr (LAZY) go(k_pair_step<KIND, OPT, 128, 8, 3, false>, ORX_VARIANT_STEP, 3, blocks);
+      else go(k_pair_step<KIND, OPT, 128, 8, 4, false>, ORX_VARIANT_STEP, 4, blocks);
       break;
-    case 256: go(k_pair_step<KIND, OPT, 256, 8, 2, !LAZY>, 8, PV, 2); break;
-    default: go(k_pair_step_generic<KIND, OPT>, 8, ORX_VARIANT_STEP_GENERIC, 0); break;
+    case 256: go(k_pair_step<KIND, OPT, 256, 8, 2, !LAZY>, PV, 2, blocks); break;
+    default: go(k_pair_generic<KIND, OPT, 0>, ORX_VARIANT_STEP_GENERIC, 0, 8 * blocks); break;
   }
   ORX_LAUNCH_CHECK();
-  return ORX_OK;
-}
-
-static int check_tables(const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias, int opt_kind) {
-  ORX_REQUIRE(user && item && bias, "null table");
-  ORX_REQUIRE(user->var && item->var && bias->var, "null table storage");
-  ORX_REQUIRE(user->dim == item->dim && user->dim > 0, "user/item dims must match and be positive");
-  ORX_REQUIRE(bias->dim == 1 && bias->rows == item->rows, "item_bias must be [item.rows, 1]");
-  ORX_REQUIRE(user->rows > 0 && item->rows > 0 && user->rows <= 0x7fffffffLL && item->rows <= 0x7fffffffLL,
-              "row counts must fit int32 ids");
-  ORX_REQUIRE(orx_opt_slots_ok(opt_kind, {user, item, bias}), "optimizer slot rows missing");
   return ORX_OK;
 }
 
@@ -575,63 +606,47 @@ extern "C" int orx_pairwise_prefetch(orx_handle_t h, const orx_table_t* user, co
   return prefetch_issue(h, uid, pid, nid, B, user->rows, item->rows, opt_kind == ORX_OPT_ADAM_DENSE ? 1 : 0);
 }
 
-static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, const orx_table_t* item,
-                              const orx_table_t* bias, const int32_t* uid, const int32_t* pid, const int32_t* nid,
-                              int B, float margin, float c_loss, float c_l2, const orx_opt_t* opt, float* out4,
-                              cudaStream_t st) {
-  ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
+int orx_sparse_step(orx_ctx* c, int op, int kind, const orx_table_t* user, const orx_table_t* item,
+                    const orx_table_t* bias, const orx_table_t* w, const int32_t* uid, const int32_t* iid,
+                    const int32_t* nid, int B, const orx_opt_t* opt, float loss_scale, float c_l2, float* out4,
+                    const OrxStepKernel& kernel, cudaStream_t st) {
   ORX_REQUIRE(opt != nullptr && out4 != nullptr, "null opt/out");
   ORX_REQUIRE(orx_opt_kind_ok(opt->kind), "unknown optimizer kind");
-  ORX_REQUIRE(B > 0 && uid && pid && nid, "empty batch or null ids");
-  int rc = check_tables(user, item, bias, opt->kind);
+  ORX_REQUIRE(B > 0 && uid && iid, "empty batch or null ids");
+  int rc = orx_check_step_tables(user, item, bias, w, opt->kind);
   if (rc) return rc;
   const int D = user->dim;
   if ((rc = orx_ensure_workspace(c, B, D))) return rc;
   const bool dense = opt->kind == ORX_OPT_ADAM_DENSE;
-  PairArgs pa;
-  pa.U = user->var; pa.Us0 = user->s0; pa.Us1 = user->s1;
-  pa.I = item->var; pa.Is0 = item->s0; pa.Is1 = item->s1;
-  pa.Bv = bias->var; pa.Bs0 = bias->s0; pa.Bs1 = bias->s1;
-  pa.rowsU = user->rows; pa.rowsI = item->rows; pa.D = D;
-  pa.uid = uid; pa.pid = pid; pa.nid = nid; pa.B = B;
-  pa.margin = margin; pa.c_loss = c_loss; pa.c_l2 = c_l2; pa.inv_B = 1.0f / (float)B;
-  pa.opt = orx_opt_to_dev(opt);
-  pa.gu = c->gu; pa.gi = c->gi; pa.gb = c->gb;
-  pa.g_out = nullptr;
-  const int n_part = (B + 63) / 64 + 8 > c->num_sms ? (B + 63) / 64 + 8 : c->num_sms;
-  if ((rc = orx_grow((void**)&c->partials, &c->partials_cap, sizeof(float) * 2 * (size_t)n_part))) return rc;
-  pa.partials = c->partials;
+  if ((rc = orx_grow((void**)&c->partials, &c->partials_cap, sizeof(float) * 2 * 8 * (size_t)orx_step_blocks(B))))
+    return rc;
   orx_prof_mark(c, 0, st);
   // index: a matching prefetched one (side stream, possibly still running), else built here on the caller's stream
   int set = 0;
-  if (c->pf_valid && c->pf_uid == uid && c->pf_pid == pid && c->pf_nid == nid && c->pf_B == B &&
+  if (nid && c->pf_valid && c->pf_uid == uid && c->pf_pid == iid && c->pf_nid == nid && c->pf_B == B &&
       c->pf_rows_u == user->rows && c->pf_rows_i == item->rows && c->pf_mode == (dense ? 1 : 0)) {
     set = 1 + c->pf_set;
     ORX_CUDA(cudaStreamWaitEvent(st, c->pf_done[c->pf_set], 0));
     c->pf_valid = 0;
   } else {
-    if ((rc = prefetch_drop(c, st))) return rc;
-    if ((rc = orx_launch_index_build(c, uid, user->rows, pid, nid, item->rows, B, dense ? 1 : 0, st))) return rc;
+    if (nid && (rc = prefetch_drop(c, st))) return rc;
+    if ((rc = orx_launch_index_build(c, uid, user->rows, iid, nid, item->rows, B, dense ? 1 : 0, st))) return rc;
   }
   const OrxHash& HU = set ? c->pf_u[set - 1] : c->hu;
   const OrxHash& HI = set ? c->pf_i[set - 1] : c->hi;
-  int32_t* ctr = c->counters + 4 * set;
   orx_prof_mark(c, 1, st);
-  pa.hu = HU; pa.hi = HI;
-  int n_partials = 0, variant = 0, minb = 0;
-  rc = orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {
-    return orx_dispatch_opt(opt->kind, [&](auto O) {
-      return launch_pair_step_kind_opt<decltype(K)::value, decltype(O)::value>(pa, st, &n_partials, &variant, &minb);
-    });
-  });
-  if (rc) return rc;
-  orx_log_dispatch(c, ORX_OP_PAIRWISE_STEP, variant, kind, opt->kind, B, D, minb, set);
+  const SparseArgs s = orx_sparse_args(c, user, item, bias, HU, HI, orx_opt_to_dev(opt));
+  OrxStepLaunch L = {};
+  if ((rc = kernel(s, c->partials, &L))) return rc;
+  orx_log_dispatch(c, op, L.variant, kind, opt->kind, B, D, L.minb, set);
   orx_prof_mark(c, 2, st);
-  if (dense && (rc = orx_launch_adam_sweeps(c, user, item, bias, HU, HI, pa.opt, st))) return rc;
-  TailArgs ta = orx_tail_args(c, user, item, bias, HU, HI, pa.opt);
-  ta.partials = c->partials; ta.n_partials = n_partials;
-  ta.loss_scale = (kind == ORX_PAIR_BPR) ? pa.inv_B : 1.0f;
-  ta.counters = ctr; ta.out4 = out4;
+  if (dense && (rc = orx_launch_adam_sweeps(c, user, item, bias, HU, HI, s.opt, st))) return rc;
+  TailArgs ta = {s};
+  ta.partials = c->partials; ta.n_partials = L.n_partials; ta.loss_scale = loss_scale;
+  ta.counters = c->counters + 4 * set; ta.out4 = out4;
+  if (w) {
+    ta.W = w->var; ta.Ws0 = w->s0; ta.Ws1 = w->s1; ta.gw = c->gw; ta.c_l2 = c_l2;
+  }
   rc = orx_launch_tail(c, ta, opt->kind, st);
   if (set) {   // the prefetch set is free again once this tail has run
     ORX_CUDA(cudaEventRecord(c->pf_free[set - 1], st));
@@ -640,6 +655,36 @@ static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, con
   orx_prof_mark(c, 3, st);
   orx_prof_next(c);
   return rc;
+}
+
+// The kernel arguments of a pairwise batch (shared part s) over user / item rows rows_u / rows_i; no un-fused outputs.
+static PairArgs pair_args(const SparseArgs& s, int64_t rows_u, int64_t rows_i, const int32_t* uid, const int32_t* pid,
+                          const int32_t* nid, int B, float margin, float c_loss, float c_l2, float inv_B) {
+  PairArgs pa = {s};
+  pa.rowsU = rows_u; pa.rowsI = rows_i;
+  pa.uid = uid; pa.pid = pid; pa.nid = nid; pa.B = B;
+  pa.margin = margin; pa.c_loss = c_loss; pa.c_l2 = c_l2; pa.inv_B = inv_B;
+  return pa;
+}
+
+static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, const orx_table_t* item,
+                              const orx_table_t* bias, const int32_t* uid, const int32_t* pid, const int32_t* nid,
+                              int B, float margin, float c_loss, float c_l2, const orx_opt_t* opt, float* out4,
+                              cudaStream_t st) {
+  ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
+  ORX_REQUIRE(nid != nullptr, "empty batch or null ids");
+  const float inv_B = 1.0f / (float)B;
+  const auto kernel = [&](const SparseArgs& s, float* partials, OrxStepLaunch* out) {
+    PairArgs pa = pair_args(s, user->rows, item->rows, uid, pid, nid, B, margin, c_loss, c_l2, inv_B);
+    pa.partials = partials;
+    return orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {
+      return orx_dispatch_opt(opt->kind, [&](auto O) {
+        return launch_pair_step_kind_opt<decltype(K)::value, decltype(O)::value>(pa, st, out);
+      });
+    });
+  };
+  return orx_sparse_step(c, ORX_OP_PAIRWISE_STEP, kind, user, item, bias, nullptr, uid, pid, nid, B, opt,
+                         kind == ORX_PAIR_BPR ? inv_B : 1.0f, c_l2, out4, kernel, st);
 }
 
 extern "C" int orx_pairwise_step(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
@@ -694,95 +739,6 @@ extern "C" int orx_pairwise_step_host(orx_handle_t h, int32_t kind, const orx_ta
 // ---------------------------------------------------------------------------------------
 // forward only / explicit gradients (un-fused; parity tests and the lazy-handle fallback)
 // ---------------------------------------------------------------------------------------
-struct PairGradArgs {
-  const float *U, *I, *Bv;
-  int64_t rowsU, rowsI;
-  int D;
-  const int32_t *uid, *pid, *nid;
-  int B;
-  float margin, c_loss, c_l2, inv_B;
-  float *d_user, *d_pos, *d_neg, *d_bp, *d_bn, *g_out;
-  float* partials;
-  // 0: table form, outputs indexed by triplet.  > D: row form (orx_pairwise_grad_rows) -- U = I = fetched rows of stride
-  // ld with the item bias in column D, outputs written to the lookup's own row of d_user = d_pos = d_neg.
-  int64_t ld;
-};
-
-template <int KIND>
-__global__ void __launch_bounds__(256) k_pair_fwd_grad(const PairGradArgs a) {
-  const int lane = threadIdx.x & 31;
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int D = a.D;
-  const bool row_form = a.ld != 0;
-  const int64_t ld = row_form ? a.ld : D;
-  float loss_acc = 0.f, l2_acc = 0.f;
-  for (int j = 0; j < 8; ++j) {
-    const int t = warp * 8 + j;
-    if (t >= a.B) break;
-    const int uu = a.uid[t], pp = a.pid[t], nn = a.nid[t];
-    const bool ok = uu >= 0 && uu < a.rowsU && pp >= 0 && pp < a.rowsI && nn >= 0 && nn < a.rowsI;
-    float s1 = 0.f, s2 = 0.f, sq = 0.f, bp = 0.f, bn = 0.f, lt = 0.f, g = 0.f;
-    const float* ur = a.U + (int64_t)uu * ld;
-    const float* pr = a.I + (int64_t)pp * ld;
-    const float* nr = a.I + (int64_t)nn * ld;
-    if (ok) {
-      for (int d = lane; d < D; d += 32) {
-        const float u = ur[d], p = pr[d], n = nr[d];
-        if (KIND == ORX_PAIR_BPR) {
-          s1 += u * p;
-          s2 += u * n;
-        } else {
-          s1 += (u - p) * (u - p);
-          s2 += (u - n) * (u - n);
-        }
-        sq += u * u + p * p + n * n;
-      }
-      bp = row_form ? pr[D] : a.Bv[pp];
-      bn = row_form ? nr[D] : a.Bv[nn];
-    }
-    l2_acc += sq;
-    s1 = orx_group_sum<32>(s1);
-    s2 = orx_group_sum<32>(s2);
-    if (ok) pair_score<KIND>(s1, s2, bp, bn, a.margin, a.c_loss, a.inv_B, &lt, &g);
-    if (lane == 0) loss_acc += lt;
-    if (a.d_user || a.d_pos || a.d_neg) {
-      for (int d = lane; d < D; d += 32) {
-        float gu = 0.f, gp = 0.f, gn = 0.f;
-        if (ok) pair_grads1<KIND>(g, a.c_l2, ur[d], pr[d], nr[d], &gu, &gp, &gn);
-        if (row_form) {
-          if (ok) {
-            a.d_user[(int64_t)uu * ld + d] = gu;
-            a.d_pos[(int64_t)pp * ld + d] = gp;
-            a.d_neg[(int64_t)nn * ld + d] = gn;
-          }
-        } else {
-          const int64_t o = (int64_t)t * D + d;
-          if (a.d_user) a.d_user[o] = gu;
-          if (a.d_pos) a.d_pos[o] = gp;
-          if (a.d_neg) a.d_neg[o] = gn;
-        }
-      }
-    }
-    if (lane == 0) {
-      const float gbias = (KIND == ORX_PAIR_BPR) ? g : -g;
-      if (row_form) {
-        if (ok) {   // column D = bias gradient (items) / 0 (users); remaining padding columns = 0
-          for (int64_t c = D; c < ld; ++c) {
-            a.d_user[(int64_t)uu * ld + c] = 0.f;
-            a.d_pos[(int64_t)pp * ld + c] = c == D ? gbias : 0.f;
-            a.d_neg[(int64_t)nn * ld + c] = c == D ? -gbias : 0.f;
-          }
-        }
-      } else {
-        if (a.d_bp) a.d_bp[t] = gbias;
-        if (a.d_bn) a.d_bn[t] = -gbias;
-      }
-      if (a.g_out) a.g_out[t] = g;
-    }
-  }
-  orx_warp_partial(loss_acc, l2_acc, a.partials);
-}
-
 __global__ void k_reduce_partials(const float* partials, int n, float loss_scale, float* out4) {
   double l, q;
   orx_block_sum_partials(partials, n, nullptr, 0, &l, &q);
@@ -800,19 +756,27 @@ int orx_launch_reduce_partials(const float* partials, int n, float loss_scale, f
   return ORX_OK;
 }
 
-// k_pair_fwd_grad over the batch of `a` (kind already validated; one partial per warp of 8 triplets) and, when out4 is
-// given, its (loss, l2) reduced into out4: the loss scaled by inv_B for BPR (mean), summed for UCML.
-static int launch_pair_fwd_grad(orx_ctx* c, int kind, PairGradArgs a, float* out4, cudaStream_t st) {
-  const int nw = (a.B + 7) / 8, blocks = (nw + 7) / 8;
-  int rc = orx_grow((void**)&c->partials, &c->partials_cap, sizeof(float) * 2 * (size_t)(blocks * 8));
+int orx_sparse_unfused(orx_ctx* c, int B, float loss_scale, float* out4,
+                       const std::function<void(float* partials, int blocks)>& launch, cudaStream_t st) {
+  const int blocks = orx_step_blocks(B);
+  int rc = orx_grow((void**)&c->partials, &c->partials_cap, sizeof(float) * 2 * 8 * (size_t)blocks);
   if (rc) return rc;
-  a.partials = c->partials;
-  orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {
-    k_pair_fwd_grad<decltype(K)::value><<<blocks, 256, 0, st>>>(a);
-  });
+  launch(c->partials, blocks);
   ORX_LAUNCH_CHECK();
   if (!out4) return ORX_OK;
-  return orx_launch_reduce_partials(c->partials, blocks * 8, kind == ORX_PAIR_BPR ? a.inv_B : 1.f, out4, st);
+  return orx_launch_reduce_partials(c->partials, 8 * blocks, loss_scale, out4, st);
+}
+
+// k_pair_generic MODE 1 over the batch of pa (kind already validated) and, when out4 is given, its (loss, l2) reduced
+// into out4: the loss scaled by inv_B for BPR (mean), summed for UCML.
+static int pair_unfused(orx_ctx* c, int kind, PairArgs pa, float* out4, cudaStream_t st) {
+  const auto launch = [&](float* partials, int blocks) {
+    pa.partials = partials;
+    orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {
+      k_pair_generic<decltype(K)::value, ORX_OPT_SGD, 1><<<blocks, 256, 0, st>>>(pa);
+    });
+  };
+  return orx_sparse_unfused(c, pa.B, kind == ORX_PAIR_BPR ? pa.inv_B : 1.f, out4, launch, st);
 }
 
 static int pair_fwd_grad(orx_ctx* c, int kind, const orx_table_t* user, const orx_table_t* item,
@@ -821,15 +785,12 @@ static int pair_fwd_grad(orx_ctx* c, int kind, const orx_table_t* user, const or
                          float* d_bp, float* d_bn, float* g_out, float* out4, cudaStream_t st) {
   ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
   ORX_REQUIRE(B > 0 && uid && pid && nid, "empty batch or null ids");
-  int rc = check_tables(user, item, bias, ORX_OPT_SGD);
+  int rc = orx_check_step_tables(user, item, bias, nullptr, ORX_OPT_SGD);
   if (rc) return rc;
-  PairGradArgs a = {};
-  a.U = user->var; a.I = item->var; a.Bv = bias->var;
-  a.rowsU = user->rows; a.rowsI = item->rows; a.D = user->dim;
-  a.uid = uid; a.pid = pid; a.nid = nid; a.B = B;
-  a.margin = margin; a.c_loss = c_loss; a.c_l2 = c_l2; a.inv_B = 1.0f / (float)B;
+  const SparseArgs s = orx_sparse_args(c, user, item, bias, c->hu, c->hi, OrxOptDev{});
+  PairArgs a = pair_args(s, user->rows, item->rows, uid, pid, nid, B, margin, c_loss, c_l2, 1.0f / (float)B);
   a.d_user = d_user; a.d_pos = d_pos; a.d_neg = d_neg; a.d_bp = d_bp; a.d_bn = d_bn; a.g_out = g_out;
-  return launch_pair_fwd_grad(c, kind, a, out4, st);
+  return pair_unfused(c, kind, a, out4, st);
 }
 
 extern "C" int orx_pairwise_fwd(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
@@ -859,12 +820,11 @@ extern "C" int orx_pairwise_grad_rows(orx_handle_t h, int32_t kind, const float*
   ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
   ORX_REQUIRE(B > 0 && dim > 0 && ld > dim, "bad sizes (ld must exceed dim: the bias lives in column dim)");
   ORX_CUDA(cudaSetDevice(h->device));
-  PairGradArgs a = {};
-  a.U = rows; a.I = rows;
-  a.rowsU = 3 * (int64_t)B; a.rowsI = 3 * (int64_t)B; a.D = dim;
-  a.uid = uslot; a.pid = pslot; a.nid = nslot; a.B = B;
-  a.margin = margin; a.c_loss = c_loss; a.c_l2 = c_l2; a.inv_B = inv_B;
-  a.d_user = d_rows; a.d_pos = d_rows; a.d_neg = d_rows;
+  SparseArgs r = {};
+  r.U = r.I = const_cast<float*>(rows);   // read only in MODE 1
+  r.D = dim;
+  PairArgs a = pair_args(r, 3 * (int64_t)B, 3 * (int64_t)B, uslot, pslot, nslot, B, margin, c_loss, c_l2, inv_B);
+  a.d_user = a.d_pos = a.d_neg = d_rows;
   a.ld = ld;
-  return launch_pair_fwd_grad(h, kind, a, out4, (cudaStream_t)s);
+  return pair_unfused(h, kind, a, out4, (cudaStream_t)s);
 }

@@ -2,27 +2,20 @@
 //
 // Reference path replaced: openrec/tf2/recommenders/gmf.py:22-34, wrmf.py:21-34,
 // modules/pointwise_mse_loss.py:18-31 + tape.gradient + apply_gradients.
-// Same three-launch structure as orx_pairwise.cu (index -> step -> tail); GMF's dense [D] weight
+// Same three launches as the pairwise step (index -> step -> tail), run by orx_sparse_step; GMF's dense [D] weight
 // gets its batch-summed gradient through shared-memory + one global reduction per block and is
 // updated by the tail.
 #include "orx_common.cuh"
 
-struct PointArgs {
-  float *U, *Us0, *Us1;
-  float *I, *Is0, *Is1;
-  float *Bv, *Bs0, *Bs1;
+struct PointArgs : SparseArgs {
   const float* W;  // GMF weight [D] (pre-step) or null
   float* gw;       // staged dense gradient of W
   int64_t rowsU, rowsI;
-  int D;
   const int32_t *uid, *iid;
   const float* label;
   int B;
   float wa, wb, c_loss, c_l2, inv_B;
   int use_sigmoid;
-  OrxOptDev opt;
-  OrxHash hu, hi;
-  float *gu, *gi, *gb;
   float* partials;
   // un-fused outputs (grad kernel only)
   float *d_user, *d_item, *d_bias, *g_out;
@@ -269,19 +262,17 @@ __global__ void k_gmf_w_terms(const float* W, int D, float* out4, float* d_w, fl
   if (threadIdx.x == 0 && out4) out4[1] += 0.5f * sh[0];
 }
 
-// *variant: the orx_dispatch_variant launched, for the dispatch record
 template <int KIND, int OPT>
-static int launch_point_kind_opt(const PointArgs& pa, cudaStream_t st, int* n_partials, int* variant) {
-  const int nw = (pa.B + 7) / 8, blocks = (nw + 7) / 8;
-  *n_partials = blocks * 8;
-  *variant = ORX_VARIANT_STEP;
+static int launch_point_kind_opt(const PointArgs& pa, cudaStream_t st, OrxStepLaunch* out) {
+  const int blocks = orx_step_blocks(pa.B);
+  *out = {8 * blocks, ORX_VARIANT_STEP, 0};
   switch (pa.D) {
     case 32: k_point_step<KIND, OPT, 32, 8><<<blocks, 256, 0, st>>>(pa); break;
     case 64: k_point_step<KIND, OPT, 64, 8><<<blocks, 256, 0, st>>>(pa); break;
     case 128: k_point_step<KIND, OPT, 128, 8><<<blocks, 256, 0, st>>>(pa); break;
     case 256: k_point_step<KIND, OPT, 256, 8><<<blocks, 256, 0, st>>>(pa); break;
     default:
-      *variant = ORX_VARIANT_STEP_GENERIC;
+      out->variant = ORX_VARIANT_STEP_GENERIC;
       k_point_generic<KIND, OPT, 0><<<blocks, 256, 0, st>>>(pa);
       break;
   }
@@ -289,36 +280,17 @@ static int launch_point_kind_opt(const PointArgs& pa, cudaStream_t st, int* n_pa
   return ORX_OK;
 }
 
-static int check_point(int kind, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
-                       const orx_table_t* w, int opt_kind) {
-  ORX_REQUIRE(kind == ORX_POINT_GMF || kind == ORX_POINT_WRMF, "unknown pointwise kind");
-  ORX_REQUIRE(user && item && bias && user->var && item->var && bias->var, "null table");
-  ORX_REQUIRE(user->dim == item->dim && user->dim > 0, "user/item dims must match and be positive");
-  ORX_REQUIRE(bias->dim == 1 && bias->rows == item->rows, "item_bias must be [item.rows, 1]");
-  ORX_REQUIRE(user->rows > 0 && item->rows > 0 && user->rows <= 0x7fffffffLL && item->rows <= 0x7fffffffLL,
-              "row counts must fit int32 ids");
-  if (kind == ORX_POINT_GMF) ORX_REQUIRE(w && w->var && w->dim == user->dim, "GMF needs w with dim == D");
-  ORX_REQUIRE(orx_opt_slots_ok(opt_kind, {user, item, bias, kind == ORX_POINT_GMF ? w : nullptr}),
-              "optimizer slot rows missing");
-  return ORX_OK;
-}
-
-static void fill_point_args(PointArgs& pa, orx_ctx* c, int kind, const orx_table_t* user, const orx_table_t* item,
-                            const orx_table_t* bias, const orx_table_t* w, const int32_t* uid, const int32_t* iid,
-                            const float* label, int B, float a, float b, int use_sigmoid, float c_loss, float c_l2) {
-  pa.U = user->var; pa.Us0 = user->s0; pa.Us1 = user->s1;
-  pa.I = item->var; pa.Is0 = item->s0; pa.Is1 = item->s1;
-  pa.Bv = bias->var; pa.Bs0 = bias->s0; pa.Bs1 = bias->s1;
-  pa.W = (kind == ORX_POINT_GMF) ? w->var : nullptr;
-  pa.gw = nullptr;
-  pa.rowsU = user->rows; pa.rowsI = item->rows; pa.D = user->dim;
+// The kernel arguments of a pointwise batch (shared part s); no gw, partials or un-fused outputs.
+static PointArgs point_args(const SparseArgs& s, const orx_table_t* dense_w, const orx_table_t* user,
+                            const orx_table_t* item, const int32_t* uid, const int32_t* iid, const float* label, int B,
+                            float a, float b, int use_sigmoid, float c_loss, float c_l2) {
+  PointArgs pa = {s};
+  pa.W = dense_w ? dense_w->var : nullptr;
+  pa.rowsU = user->rows; pa.rowsI = item->rows;
   pa.uid = uid; pa.iid = iid; pa.label = label; pa.B = B;
   pa.wa = a; pa.wb = b; pa.c_loss = c_loss; pa.c_l2 = c_l2; pa.inv_B = 1.0f / (float)B;
   pa.use_sigmoid = use_sigmoid;
-  pa.hu = c->hu; pa.hi = c->hi; pa.gu = c->gu; pa.gi = c->gi; pa.gb = c->gb;
-  pa.partials = c->partials;
-  pa.d_user = pa.d_item = pa.d_bias = pa.g_out = nullptr;
-  pa.opt.kind = 0; pa.opt.lr = 0.f; pa.opt.eps = 0.f; pa.opt.beta1 = 0.f; pa.opt.beta2 = 0.f;
+  return pa;
 }
 
 extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
@@ -326,39 +298,25 @@ extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_
                                   const int32_t* iid, const float* label, int32_t B, float a, float b,
                                   int32_t use_sigmoid, float c_loss, float c_l2, const orx_opt_t* opt, float* out4,
                                   orx_stream_t s) {
-  ORX_REQUIRE(h != nullptr && opt != nullptr && out4 != nullptr, "null handle/opt/out");
-  ORX_REQUIRE(orx_opt_kind_ok(opt->kind), "unknown optimizer kind");
-  ORX_REQUIRE(B > 0 && uid && iid && label, "empty batch or null inputs");
+  ORX_REQUIRE(h != nullptr, "null handle");
+  ORX_REQUIRE(label != nullptr, "empty batch or null inputs");
+  ORX_REQUIRE(kind == ORX_POINT_GMF || kind == ORX_POINT_WRMF, "unknown pointwise kind");
+  ORX_REQUIRE(kind == ORX_POINT_WRMF || w, "GMF needs w with dim == D");
+  const orx_table_t* dense_w = (kind == ORX_POINT_GMF) ? w : nullptr;
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
-  int rc = check_point(kind, user, item, item_bias, w, opt->kind);
-  if (rc) return rc;
-  const int D = user->dim;
-  const bool dense = opt->kind == ORX_OPT_ADAM_DENSE;
-  if ((rc = orx_ensure_workspace(h, B, D))) return rc;
-  if ((rc = orx_grow((void**)&h->partials, &h->partials_cap, sizeof(float) * 2 * (size_t)((B + 7) / 8 + 8)))) return rc;
-  if ((rc = orx_launch_index_build(h, uid, user->rows, iid, nullptr, item->rows, B, dense, st))) return rc;
-  PointArgs pa;
-  fill_point_args(pa, h, kind, user, item, item_bias, w, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2);
-  pa.opt = orx_opt_to_dev(opt);
-  pa.gw = (kind == ORX_POINT_GMF) ? h->gw : nullptr;
-  int n_partials = 0, variant = 0;
-  rc = orx_dispatch<ORX_POINT_GMF, ORX_POINT_WRMF>(kind, [&](auto K) {
-    return orx_dispatch_opt(opt->kind, [&](auto O) {
-      return launch_point_kind_opt<decltype(K)::value, decltype(O)::value>(pa, st, &n_partials, &variant);
+  const auto kernel = [&](const SparseArgs& sa, float* partials, OrxStepLaunch* out) {
+    PointArgs pa = point_args(sa, dense_w, user, item, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2);
+    pa.partials = partials;
+    pa.gw = dense_w ? h->gw : nullptr;
+    return orx_dispatch<ORX_POINT_GMF, ORX_POINT_WRMF>(kind, [&](auto K) {
+      return orx_dispatch_opt(opt->kind, [&](auto O) {
+        return launch_point_kind_opt<decltype(K)::value, decltype(O)::value>(pa, st, out);
+      });
     });
-  });
-  if (rc) return rc;
-  orx_log_dispatch(h, ORX_OP_POINTWISE_STEP, variant, kind, opt->kind, B, D, 0, 0);   // index set 0 always
-  if (dense && (rc = orx_launch_adam_sweeps(h, user, item, item_bias, h->hu, h->hi, pa.opt, st))) return rc;
-  TailArgs ta = orx_tail_args(h, user, item, item_bias, h->hu, h->hi, pa.opt);
-  ta.partials = h->partials; ta.n_partials = n_partials;
-  ta.loss_scale = (kind == ORX_POINT_GMF) ? pa.inv_B : 1.0f;
-  ta.counters = h->counters; ta.out4 = out4;
-  if (kind == ORX_POINT_GMF) {
-    ta.W = w->var; ta.Ws0 = w->s0; ta.Ws1 = w->s1; ta.gw = h->gw; ta.c_l2 = c_l2;
-  }
-  return orx_launch_tail(h, ta, opt->kind, st);
+  };
+  return orx_sparse_step(h, ORX_OP_POINTWISE_STEP, kind, user, item, item_bias, dense_w, uid, iid, nullptr, B, opt,
+                         dense_w ? 1.0f / (float)B : 1.0f, c_l2, out4, kernel, st);
 }
 
 static int point_fwd_grad(orx_ctx* h, int kind, const orx_table_t* user, const orx_table_t* item,
@@ -367,25 +325,26 @@ static int point_fwd_grad(orx_ctx* h, int kind, const orx_table_t* user, const o
                           float* d_user, float* d_item, float* d_bias, float* d_w, float* g_out, float* out4,
                           cudaStream_t st) {
   ORX_REQUIRE(B > 0 && uid && iid && label, "empty batch or null inputs");
-  int rc = check_point(kind, user, item, bias, w, ORX_OPT_SGD);
+  ORX_REQUIRE(kind == ORX_POINT_GMF || kind == ORX_POINT_WRMF, "unknown pointwise kind");
+  ORX_REQUIRE(kind == ORX_POINT_WRMF || w, "GMF needs w with dim == D");
+  const orx_table_t* dense_w = (kind == ORX_POINT_GMF) ? w : nullptr;
+  int rc = orx_check_step_tables(user, item, bias, dense_w, ORX_OPT_SGD);
   if (rc) return rc;
-  const int nw = (B + 7) / 8, blocks = (nw + 7) / 8;
-  if ((rc = orx_grow((void**)&h->partials, &h->partials_cap, sizeof(float) * 2 * (size_t)(blocks * 8)))) return rc;
-  PointArgs pa;
-  fill_point_args(pa, h, kind, user, item, bias, w, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2);
+  const SparseArgs s = orx_sparse_args(h, user, item, bias, h->hu, h->hi, OrxOptDev{});
+  PointArgs pa = point_args(s, dense_w, user, item, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2);
   pa.d_user = d_user; pa.d_item = d_item; pa.d_bias = d_bias; pa.g_out = g_out;
-  if (kind == ORX_POINT_GMF && d_w) {
+  if (dense_w && d_w) {
     ORX_CUDA(cudaMemsetAsync(d_w, 0, sizeof(float) * user->dim, st));
     pa.gw = d_w;
   }
-  if (kind == ORX_POINT_GMF) k_point_generic<ORX_POINT_GMF, ORX_OPT_SGD, 1><<<blocks, 256, 0, st>>>(pa);
-  else k_point_generic<ORX_POINT_WRMF, ORX_OPT_SGD, 1><<<blocks, 256, 0, st>>>(pa);
-  ORX_LAUNCH_CHECK();
-  if (out4) {
-    rc = orx_launch_reduce_partials(h->partials, blocks * 8, kind == ORX_POINT_GMF ? pa.inv_B : 1.f, out4, st);
-    if (rc) return rc;
-  }
-  if (kind == ORX_POINT_GMF && (out4 || d_w)) {
+  const auto launch = [&](float* partials, int blocks) {
+    pa.partials = partials;
+    orx_dispatch<ORX_POINT_GMF, ORX_POINT_WRMF>(kind, [&](auto K) {
+      k_point_generic<decltype(K)::value, ORX_OPT_SGD, 1><<<blocks, 256, 0, st>>>(pa);
+    });
+  };
+  if ((rc = orx_sparse_unfused(h, B, dense_w ? pa.inv_B : 1.f, out4, launch, st))) return rc;
+  if (dense_w && (out4 || d_w)) {
     k_gmf_w_terms<<<1, 256, 0, st>>>(w->var, user->dim, out4, d_w, c_l2);
     ORX_LAUNCH_CHECK();
   }

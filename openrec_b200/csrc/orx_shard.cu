@@ -1037,7 +1037,7 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
       }
       case 5: {
         const int g = h->num_sms * 4;   // the grid of k_sparse_tail
-        TailArgs ta = orx_tail_args(h, user, item, item_bias, hu, hi, od);
+        TailArgs ta = {orx_sparse_args(h, user, item, item_bias, hu, hi, od)};
         ta.counters = h->counters;   // [2]: the tail's block ticket
         ta.out4 = out4;
         sh_dispatch_opt(opt->kind, [&](auto O) {

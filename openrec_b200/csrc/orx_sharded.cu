@@ -181,7 +181,7 @@ static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32
   }
   if (dense && (rc = orx_launch_adam_sweeps(h, tab, nullptr, nullptr, h->hu, h->hi, o, st))) return rc;
   // staged rows: the shared tail with no item side and no loss
-  TailArgs ta = orx_tail_args(h, tab, nullptr, nullptr, h->hu, h->hi, o);
+  TailArgs ta = {orx_sparse_args(h, tab, nullptr, nullptr, h->hu, h->hi, o)};
   ta.counters = h->counters;
   return orx_launch_tail(h, ta, opt->kind, st);
 }
