@@ -89,8 +89,8 @@ ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
  * TA = TB = 0, S = 1.  A sparse step (one record per call) has TA = kind (orx_pair_kind / orx_point_kind), TB = optimizer
  * (orx_opt_kind), M = B, N = D, K = the CTAs/SM bound of the fused kernel's __launch_bounds__ (0: none) and S = the batch
  * index set it used: 0 = built on the caller's stream, 1 or 2 = a consumed prefetch (orx_pairwise_prefetch, or the side
- * stream of orx_pairwise_step_host).  orx_score_rank and orx_score_topk write one record per call (fields at
- * ORX_OP_SCORE_RANK / ORX_OP_SCORE_TOPK).
+ * stream of orx_pairwise_step_host).  orx_score_rank and orx_score_topk write one record per call, and
+ * orx_score_rank_shard one per phase-2 call (fields at ORX_OP_SCORE_RANK / ORX_OP_SCORE_TOPK / ORX_OP_SCORE_RANK_SHARD).
  * Host-side bookkeeping only: no device work, no synchronisation. */
 enum orx_dispatch_op {
   ORX_OP_GEMM = 0,
@@ -99,7 +99,10 @@ enum orx_dispatch_op {
   ORX_OP_PAIRWISE_STEP = 3,  /* orx_pairwise_step, orx_pairwise_step_host */
   ORX_OP_POINTWISE_STEP = 4, /* orx_pointwise_step */
   ORX_OP_SCORE_RANK = 5,     /* orx_score_rank: TA = orx_score_kind, TB = 0, M = Bu, N = I, K = dim, S = item splits */
-  ORX_OP_SCORE_TOPK = 6      /* orx_score_topk: TA = orx_score_kind, TB = k, M = Bu, N = I, K = dim, S = item splits */
+  ORX_OP_SCORE_TOPK = 6,     /* orx_score_topk: TA = orx_score_kind, TB = k, M = Bu, N = I, K = dim, S = item splits */
+  ORX_OP_SCORE_RANK_SHARD = 7 /* orx_score_rank_shard, phase 2 only: variant RANK_SMEM / RANK_GLOBAL of the local pass,
+                                 TA = orx_score_kind, TB = rank, M = Bu, N = local items, K = dim, S = item splits
+                                 (0: no local items, no pass launched) */
 };
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
@@ -355,6 +358,47 @@ ORX_API int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_tab, 
                            int32_t dim, const int64_t* pos_off, const int32_t* pos_items, const int64_t* excl_off,
                            const int32_t* excl_items, int32_t max_pos, const int32_t* at_host, int32_t n_at,
                            float* auc, float* ndcg, float* recall, orx_stream_t s);
+
+/* ---- sharded catalogue evaluation: orx_score_rank over row-sharded user / item tables (the layout of orx_shard_step:
+ * row r of every table lives on rank r % world at local row r / world), each rank counting over its own item rows
+ * (openrec_b200/sharded.py score_rank_sharded, RankingEvaluator on ShardedBPR / ShardedUCML).
+ * orx_rowshard_t: the geometry; local_* = ceil((total - rank) / world), which may be 0.
+ * The call runs one phase.  Between phases the caller replaces each exchange buffer with its element-wise integer SUM
+ * over all ranks (an all-reduce on the int32 / int64 words); every phase writes every element of the buffer it
+ * produces, so no buffer needs clearing.  With P = max_pos + 1, and sizes from orx_score_rank_shard_sizes
+ * (n3 = {Bu * dim, Bu * P, Bu * P} elements):
+ *   phase 0 reads the user shard and writes xrows[b] = the bits of user row uid[b] if this rank owns it, else 0;
+ *   phase 1 reads the summed xrows and writes xpred[b, q] = the bits of the score of the q-th positive of uid[b] in
+ *           [0, total_items) if this rank owns that item, else 0 (all 0 for a row longer than max_pos);
+ *   phase 2 reads the summed xrows and xpred, scores this rank's item rows and writes xcnt[b, 0] = its AUC count and
+ *           xcnt[b, 1..n] = its rank-histogram hits, both after taking back its own items of pos u excl (two's
+ *           complement; a partial may be negative), the rest of the row 0;
+ *   phase 3 reads the summed xcnt and writes auc / ndcg / recall (each may be NULL).
+ * Exactly one rank contributes a non-zero word to each element of xrows and xpred, so the integer sum carries the float
+ * bits unchanged (-0.0, NaN payloads, +-inf), which a float sum would not.  uid holds global user ids; the CSR lists are
+ * the global lists of orx_score_rank, present on every rank.  Phase 3's outputs equal orx_score_rank on the global
+ * tables (scale NULL): AUC and Recall bit for bit, NDCG within one float32 ulp; the bad-uid rule, ignored list
+ * entries, max_pos, excl_off == NULL and the cut-offs are those of orx_score_rank.
+ * Item row i is read only at local row i / world on the rank i % world, and only for i < total_items: a rank without
+ * items (local_items == 0) may pass a 1-row dummy shard that is never read, and launches no empty grid.
+ * No handle state crosses a phase boundary: one handle may serve several ranks, with any call between phases.  Phase 2
+ * uses the evaluation scratch of orx_score_rank and writes one dispatch record (ORX_OP_SCORE_RANK_SHARD).
+ * ORX_ERR_INVALID before any device work: local_* that disagree with (total, world, rank), rank outside [0, world),
+ * phase outside [0, 3], the size limits of orx_score_rank, a null buffer the phase reads or writes.  Bu = 0 is a no-op.
+ * There is no scale argument: no sharded model uses one. */
+typedef struct {
+  int32_t world, rank;               /* row r of every table lives on rank r % world at local row r / world */
+  int64_t total_users, total_items;  /* global U, I */
+  int64_t local_users, local_items;  /* rows of this rank's shards */
+} orx_rowshard_t;
+ORX_API int orx_score_rank_shard_sizes(int32_t Bu, int32_t dim, int32_t max_pos, int64_t* n3_host);
+ORX_API int orx_score_rank_shard(orx_handle_t h, int32_t kind, int32_t phase, const orx_rowshard_t* g_host,
+                                 const float* user_shard, const float* item_shard, const float* bias_shard,
+                                 int32_t dim, const int32_t* uid, int32_t Bu, const int64_t* pos_off,
+                                 const int32_t* pos_items, const int64_t* excl_off, const int32_t* excl_items,
+                                 int32_t max_pos, const int32_t* at_host, int32_t n_at, int32_t* xrows /*[Bu, dim]*/,
+                                 int32_t* xpred /*[Bu, P]*/, int64_t* xcnt /*[Bu, P]*/, float* auc, float* ndcg,
+                                 float* recall, orx_stream_t s);
 
 /* ---- catalogue top-K retrieval: each batch row's k best unseen items in one fused pass, without the [Bu, I] score
  * matrix (openrec_b200/tf2/recommenders/retriever.py; closest reference: openrec/tf1's FastDotProductServer).

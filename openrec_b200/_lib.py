@@ -17,7 +17,7 @@ ORX_POINT_GMF, ORX_POINT_WRMF = 0, 1
 ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST = 0, 1
 ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE = 0, 1, 2, 3
 ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP = 0, 1, 2, 3, 4
-ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK = 5, 6
+ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_RANK_SHARD = 5, 6, 7
 ORX_VARIANT_GEMM_TMA, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_INTERACT = 0, 1, 2, 3
 ORX_VARIANT_STEP, ORX_VARIANT_STEP_PIPE, ORX_VARIANT_STEP_GENERIC = 4, 5, 6
 ORX_VARIANT_RANK_SMEM, ORX_VARIANT_RANK_GLOBAL, ORX_VARIANT_TOPK = 7, 8, 9
@@ -41,6 +41,11 @@ class OrxShard(C.Structure):
                 ("home_cap", C.c_int32), ("req_cap", C.c_int32), ("gin_cap", C.c_int32), ("timeout_ms", C.c_int32),
                 ("tripbox", C.c_void_p), ("idbox", C.c_void_p), ("got", C.c_void_p), ("gotb", C.c_void_p),
                 ("gin", C.c_void_p), ("ginb", C.c_void_p), ("meta", C.c_void_p), ("flags", C.c_void_p)]
+
+
+class OrxRowShard(C.Structure):
+    _fields_ = [("world", C.c_int32), ("rank", C.c_int32), ("total_users", C.c_int64), ("total_items", C.c_int64),
+                ("local_users", C.c_int64), ("local_items", C.c_int64)]
 
 
 class OrxSampler(C.Structure):
@@ -105,6 +110,9 @@ SIGNATURES = {
     "orx_score_rank": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _i32,
                        C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp],
     "orx_score_topk": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp],
+    "orx_score_rank_shard_sizes": [_i32, _i32, _i32, C.POINTER(_i64)],
+    "orx_score_rank_shard": [_vp, _i32, _i32, C.POINTER(OrxRowShard), _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp,
+                             _i32, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
 }
 
 _lib = None

@@ -12,6 +12,12 @@
 // hist[j].  Every score is computed by the FFMA chain of k_score_all (acc = 0, one fused multiply-add per k in
 // ascending order, user value scaled first, bias added last), so the comparisons, and with them every count, equal
 // those of orx_score_all + orx_rank_metrics exactly.
+//
+// Every count is a sum over items, so it splits over any partition of the catalogue.  orx_score_rank_shard runs the
+// same kernels on row-sharded tables (item i is row i / world of rank i % world): each rank counts over its own rows
+// and takes back its own items of pos u excl, the callers sum the integer counts over the ranks, and the finish reads
+// the sums.  The user rows and the positives' scores reach every rank the same way, as integer sums in which exactly
+// one rank contributes a non-zero word, so their bits cross unchanged.
 #include <cub/device/device_segmented_sort.cuh>
 
 #include "orx_common.cuh"
@@ -20,6 +26,7 @@ namespace {
 
 constexpr int EV_TU = 128, EV_TI = 128, EV_KC = 8, EV_NT = 256, EV_LD = EV_TU + 4;
 
+// What the tile kernels (k_score_rank, k_score_topk) read.  Kept at this layout: their register allocation is tight.
 struct EvalArgs {
   const float* user_tab;
   int64_t U;
@@ -28,12 +35,20 @@ struct EvalArgs {
   const float* scale;
   const float* item_tab;
   const float* bias;
-  int64_t I;
+  int64_t I;   // item rows the tile loop walks (rows of item_tab / bias)
   int D;
   const int64_t *pos_off, *excl_off;
   const int32_t *pos_items, *excl_items;
   int max_pos;
   int P;  // max_pos + 1: row stride of the threshold and histogram rows
+};
+
+// What the per-row kernels (one CTA per batch row) read on top: the catalogue, the item ownership and the exchange.
+struct EvalRowArgs : EvalArgs {
+  int64_t I_all;        // the catalogue: list entries in [0, I_all) count, n_eval = I_all - n - extra
+  int world, rank;      // row r is local row r / world on rank r % world (1, 0: the whole table)
+  const float* xrows;   // non-null: batch row b's user row is xrows[b * D ..] (uid still decides bad rows)
+  const float* xpred;   // non-null: prep reads the positives' scores from xpred[b * P + q] instead of computing them
 };
 
 // Scratch of one call (handle workspace).  keys_in / keys: [2][Bu][P] -- pred thresholds of row b at b * P, sp
@@ -55,10 +70,23 @@ struct EvalOut {
   float *auc, *ndcg, *recall;
 };
 
+// XROWS: user_tab holds one row per batch position (the summed exchange of the sharded pass), not per user id
+template <bool XROWS>
 __device__ __forceinline__ const float* ev_user_row(const EvalArgs& a, int b) {
   const int32_t id = a.uid[b];
-  return (id >= 0 && (int64_t)id < a.U) ? a.user_tab + (int64_t)id * a.D : nullptr;
+  return (id >= 0 && (int64_t)id < a.U) ? a.user_tab + (int64_t)(XROWS ? b : id) * a.D : nullptr;
 }
+__device__ __forceinline__ const float* ev_urow(const EvalRowArgs& a, int b) {
+  if (!a.xrows) return ev_user_row<false>(a, b);
+  const int32_t id = a.uid[b];
+  return (id >= 0 && (int64_t)id < a.U) ? a.xrows + (int64_t)b * a.D : nullptr;
+}
+
+// ownership of a (user or item) id in [0, 2^31): row r lives on rank r % world at local row r / world
+__device__ __forceinline__ bool ev_owns(const EvalRowArgs& a, int32_t r) {
+  return (uint32_t)r % (uint32_t)a.world == (uint32_t)a.rank;
+}
+__device__ __forceinline__ int64_t ev_local(const EvalRowArgs& a, int32_t r) { return (uint32_t)r / (uint32_t)a.world; }
 
 // first position in items[lo, hi) holding a value >= v (the row is sorted)
 __device__ __forceinline__ int64_t ev_lower(const int32_t* items, int64_t lo, int64_t hi, int64_t v) {
@@ -86,9 +114,10 @@ __device__ __forceinline__ bool ev_contains(const int32_t* items, int64_t lo, in
   return k < hi && items[k] == v;
 }
 
-// One score by the chain of k_score_all.
+// One score by the chain of k_score_all, of an item i this rank owns (ev_owns).
 template <int KIND>
-__device__ __forceinline__ float ev_score1(const EvalArgs& a, const float* urow, int64_t i) {
+__device__ __forceinline__ float ev_score1(const EvalRowArgs& a, const float* urow, int32_t i_global) {
+  const int64_t i = ev_local(a, i_global);
   const float* irow = a.item_tab + i * a.D;
   float acc = 0.f;
   for (int k = 0; k < a.D; ++k) {
@@ -137,26 +166,40 @@ __device__ __forceinline__ int ev_rank_slot(const float* sth, int n, float smin,
 // ---------------------------------------------------------------------------------------
 // prep: one CTA per batch row.  pred_p and sp_p of every positive (sp: NaN -> +inf, which ranks 0 like NaN; pred: NaN
 // -> +NaN, which sorts after every number and is left out of the AUC search), zeroed histogram and AUC count, and the
-// two sort segments of the row.
+// two sort segments of the row.  With a.xpred the scores are read from the summed exchange, not computed.
 // ---------------------------------------------------------------------------------------
+// The positive and exclusion entries of batch row b in [0, I_all), and whether its positive row is longer than max_pos.
+struct EvRow {
+  int64_t plo, phi, elo, ehi;
+  bool bad;
+};
+
+__device__ __forceinline__ EvRow ev_row(const EvalRowArgs& a, int b) {
+  EvRow r;
+  int64_t praw, eraw;
+  const int32_t u = a.uid[b];
+  ev_range(a.pos_off, a.pos_items, u, a.U, a.I_all, &r.plo, &r.phi, &praw);
+  ev_range(a.excl_off, a.excl_items, u, a.U, a.I_all, &r.elo, &r.ehi, &eraw);
+  r.bad = praw > a.max_pos;
+  return r;
+}
+
 template <int KIND>
-__global__ void __launch_bounds__(EV_NT) k_eval_prep(const EvalArgs a, const EvalWs w) {
+__global__ void __launch_bounds__(EV_NT) k_eval_prep(const EvalRowArgs a, const EvalWs w) {
   __shared__ int s_nan;
   const int b = blockIdx.x;
-  const int32_t u = a.uid[b];
-  const float* urow = ev_user_row(a, b);
-  int64_t plo, phi, praw, elo, ehi, eraw;
-  ev_range(a.pos_off, a.pos_items, u, a.U, a.I, &plo, &phi, &praw);
-  ev_range(a.excl_off, a.excl_items, u, a.U, a.I, &elo, &ehi, &eraw);
-  const bool bad = praw > a.max_pos;
-  const int n = bad ? 0 : (int)(phi - plo);
+  const float* urow = ev_urow(a, b);
+  const EvRow r = ev_row(a, b);
+  const int64_t plo = r.plo, elo = r.elo, ehi = r.ehi;
+  const bool bad = r.bad;
+  const int n = bad ? 0 : (int)(r.phi - plo);
   float* kp = w.keys_in + (int64_t)b * a.P;
   float* ks = w.keys_in + (int64_t)(a.Bu + b) * a.P;
   if (threadIdx.x == 0) s_nan = 0;
   __syncthreads();
   for (int q = threadIdx.x; q < n; q += blockDim.x) {
     const int32_t i = a.pos_items[plo + q];
-    float s = ev_score1<KIND>(a, urow, i);
+    float s = a.xpred ? a.xpred[(int64_t)b * a.P + q] : ev_score1<KIND>(a, urow, i);
     const bool ex = ev_contains(a.excl_items, elo, ehi, i);
     float sp = expf(s) * (ex ? 0.f : 1.f);
     if (sp != sp) sp = __int_as_float(0x7f800000);
@@ -177,6 +220,37 @@ __global__ void __launch_bounds__(EV_NT) k_eval_prep(const EvalArgs a, const Eva
     w.seg_end[b] = b * a.P + n;
     w.seg_begin[a.Bu + b] = (a.Bu + b) * a.P;
     w.seg_end[a.Bu + b] = (a.Bu + b) * a.P + n;
+  }
+}
+
+// Sharded phase 0: xrows[b] = the bits of user row uid[b] if this rank owns it, else 0 (every element written).
+__global__ void __launch_bounds__(EV_NT) k_eval_user_rows(const EvalRowArgs a, int32_t* xrows) {
+  const int64_t n = (int64_t)a.Bu * a.D;
+  for (int64_t e = blockIdx.x * (int64_t)EV_NT + threadIdx.x; e < n; e += (int64_t)gridDim.x * EV_NT) {
+    const int b = (int)(e / a.D);
+    const int32_t id = a.uid[b];
+    int32_t v = 0;
+    if (id >= 0 && (int64_t)id < a.U && ev_owns(a, id))
+      v = __float_as_int(a.user_tab[ev_local(a, id) * a.D + (e - (int64_t)b * a.D)]);
+    xrows[e] = v;
+  }
+}
+
+// Sharded phase 1: xpred[b][q] = the bits of the score of row b's q-th positive in [0, I_all) if this rank owns that
+// item, else 0; a row longer than max_pos is all 0 (every element written).
+template <int KIND>
+__global__ void __launch_bounds__(EV_NT) k_eval_pos_scores(const EvalRowArgs a, int32_t* xpred) {
+  const int b = blockIdx.x;
+  const float* urow = ev_urow(a, b);
+  const EvRow r = ev_row(a, b);
+  const int n = r.bad ? 0 : (int)(r.phi - r.plo);
+  for (int q = threadIdx.x; q < a.P; q += blockDim.x) {
+    int32_t v = 0;
+    if (q < n) {
+      const int32_t i = a.pos_items[r.plo + q];
+      if (ev_owns(a, i)) v = __float_as_int(ev_score1<KIND>(a, urow, i));
+    }
+    xpred[(int64_t)b * a.P + q] = v;
   }
 }
 
@@ -285,7 +359,7 @@ __device__ __forceinline__ void ev_tiles(const EvalArgs& a, float (*sA)[EV_KC][E
   }
 }
 
-template <int KIND>
+template <int KIND, bool XROWS>
 __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const EvalWs w, int use_smem) {
   extern __shared__ float4 ev_dyn4[];
   __shared__ __align__(16) float sA[2][EV_KC][EV_LD];
@@ -304,7 +378,7 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
     RowMeta m = {};
     if (tid < rows) {
       const int b = u0 + tid;
-      m.urow = ev_user_row(a, b);
+      m.urow = ev_user_row<XROWS>(a, b);
       m.n = max(w.info[2 * b], 0);
       m.n_auc = w.info[2 * b] < 0 ? 0 : w.info[2 * b + 1];
       if (use_smem) {
@@ -383,79 +457,83 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
 }
 
 // ---------------------------------------------------------------------------------------
-// correction + finish: one CTA per batch row.  Takes back the terms of pos u excl, suffix-sums the histogram into the
-// positives' ranks and writes auc / ndcg / recall with the formulas and conversions of k_rank_metrics.
+// correction + finish: one CTA per batch row.  ev_take_back takes back the terms of pos u excl, ev_finish_row
+// suffix-sums the histogram into the positives' ranks and writes auc / ndcg / recall with the formulas and conversions
+// of k_rank_metrics.  k_eval_finish does both on one device; the sharded phases 2 and 3 split them (k_eval_correct on
+// each rank's own items, k_eval_finish_counts on the summed counts).
 // ---------------------------------------------------------------------------------------
-template <int KIND>
-__global__ void __launch_bounds__(EV_NT) k_eval_finish(const EvalArgs a, const EvalWs w, const EvalOut o) {
-  __shared__ unsigned long long s_sub;
-  __shared__ long long s_extra;
-  __shared__ unsigned s_part[EV_NT];
-  __shared__ unsigned s_after[EV_NT];
-  __shared__ double s_dcg[ORX_MAX_AT];
-  __shared__ int s_hit[ORX_MAX_AT];
-  const int b = blockIdx.x, tid = threadIdx.x;
-  const int info = w.info[2 * b];
-  if (info < 0) {   // a positive row longer than max_pos
-    const float nan = __int_as_float(0x7fffffff);
-    if (tid == 0 && o.auc) o.auc[b] = nan;
-    if (tid < o.n_at) {
-      if (o.ndcg) o.ndcg[(int64_t)b * o.n_at + tid] = nan;
-      if (o.recall) o.recall[(int64_t)b * o.n_at + tid] = nan;
-    }
-    return;
+// Block-wide over the entries of row r: adds to *s_sub the AUC terms of the positives and excluded items this rank
+// owns (the main pass counted them as eval items) and takes their rank hits off hist (excluded items only: an excluded
+// item's sp is 0 or NaN and never ranks above anything); adds to *s_extra the excluded items that are not positives,
+// owned or not.  TAKE = false: *s_extra only (no scores, no thresholds).
+template <int KIND, bool TAKE>
+__device__ __forceinline__ void ev_take_back(const EvalRowArgs& a, int b, const EvRow& r, int n, int n_auc,
+                                             const float* pth, const float* sth, unsigned* hist,
+                                             unsigned long long* s_sub, long long* s_extra) {
+  const int tid = threadIdx.x;
+  const float* urow = TAKE ? ev_urow(a, b) : nullptr;
+  float pmin = 0.f, pmax = 0.f, smin = 0.f, smax = 0.f;
+  if (TAKE) {
+    pmin = n_auc ? pth[0] : __int_as_float(0x7f800000);
+    pmax = n_auc ? pth[n_auc - 1] : __int_as_float(0xff800000);
+    smin = n ? sth[0] : __int_as_float(0x7f800000);
+    smax = n ? sth[n - 1] : __int_as_float(0x7f800000);
   }
-  const int n = info, n_auc = w.info[2 * b + 1];
-  const int64_t P = a.P;
-  const float* pth = w.keys + (int64_t)b * P;
-  const float* sth = w.keys + (int64_t)(a.Bu + b) * P;
-  unsigned* hist = w.hist + (int64_t)b * P;
-  const float pmin = n_auc ? pth[0] : __int_as_float(0x7f800000);
-  const float pmax = n_auc ? pth[n_auc - 1] : __int_as_float(0xff800000);
-  const float smin = n ? sth[0] : __int_as_float(0x7f800000);
-  const float smax = n ? sth[n - 1] : __int_as_float(0x7f800000);
-  const int32_t u = a.uid[b];
-  const float* urow = ev_user_row(a, b);
-  int64_t plo, phi, praw, elo, ehi, eraw;
-  ev_range(a.pos_off, a.pos_items, u, a.U, a.I, &plo, &phi, &praw);
-  ev_range(a.excl_off, a.excl_items, u, a.U, a.I, &elo, &ehi, &eraw);
-  if (tid == 0) {
-    s_sub = 0ull;
-    s_extra = 0;
-  }
-  if (tid < ORX_MAX_AT) {
-    s_dcg[tid] = 0.0;
-    s_hit[tid] = 0;
-  }
-  __syncthreads();
   unsigned long long sub = 0ull;
   long long extra = 0;
-  for (int64_t q = tid; q < n; q += blockDim.x) {          // positives: not eval items
-    const int32_t i = a.pos_items[plo + q];
-    const float s = ev_score1<KIND>(a, urow, i);
-    sub += ev_auc_count(pth, n_auc, pmin, pmax, s);
-    if (ev_contains(a.excl_items, elo, ehi, i)) {
-      const int j = ev_rank_slot(sth, n, smin, smax, expf(s));
-      if (j) atomicSub(hist + j, 1u);
+  if (TAKE)
+    for (int64_t q = tid; q < n; q += blockDim.x) {          // positives: not eval items
+      const int32_t i = a.pos_items[r.plo + q];
+      if (!ev_owns(a, i)) continue;
+      const float s = ev_score1<KIND>(a, urow, i);
+      sub += ev_auc_count(pth, n_auc, pmin, pmax, s);
+      if (ev_contains(a.excl_items, r.elo, r.ehi, i)) {
+        const int j = ev_rank_slot(sth, n, smin, smax, expf(s));
+        if (j) atomicSub(hist + j, 1u);
+      }
     }
-  }
-  for (int64_t q = elo + tid; q < ehi; q += blockDim.x) {  // excluded items that are not positives
+  for (int64_t q = r.elo + tid; q < r.ehi; q += blockDim.x) {  // excluded items that are not positives
     const int32_t i = a.excl_items[q];
-    if (ev_contains(a.pos_items, plo, phi, i)) continue;
+    if (ev_contains(a.pos_items, r.plo, r.phi, i)) continue;
     ++extra;
+    if (!TAKE || !ev_owns(a, i)) continue;
     const float s = ev_score1<KIND>(a, urow, i);
     sub += ev_auc_count(pth, n_auc, pmin, pmax, s);
     const int j = ev_rank_slot(sth, n, smin, smax, expf(s));
     if (j) atomicSub(hist + j, 1u);
   }
-  if (sub) atomicAdd(&s_sub, sub);
-  if (extra) atomicAdd(reinterpret_cast<unsigned long long*>(&s_extra), (unsigned long long)extra);
-  __syncthreads();
+  if (sub) atomicAdd(s_sub, sub);
+  if (extra) atomicAdd(reinterpret_cast<unsigned long long*>(s_extra), (unsigned long long)extra);
+}
+
+__device__ __forceinline__ void ev_nan_row(const EvalOut& o, int b) {   // a positive row longer than max_pos
+  const float nan = __int_as_float(0x7fffffff);
+  if (threadIdx.x == 0 && o.auc) o.auc[b] = nan;
+  if (threadIdx.x < o.n_at) {
+    if (o.ndcg) o.ndcg[(int64_t)b * o.n_at + threadIdx.x] = nan;
+    if (o.recall) o.recall[(int64_t)b * o.n_at + threadIdx.x] = nan;
+  }
+}
+
+// The outputs of row b from its final counts: auc_cnt, and hist_at(j) for j = 1..n (the rank hits).  Block-wide; every
+// thread must call it.
+template <class Hist>
+__device__ __forceinline__ void ev_finish_row(const EvalRowArgs& a, const EvalOut& o, int b, int n, long long extra,
+                                              unsigned long long auc_cnt, Hist hist_at) {
+  __shared__ unsigned s_part[EV_NT];
+  __shared__ unsigned s_after[EV_NT];
+  __shared__ double s_dcg[ORX_MAX_AT];
+  __shared__ int s_hit[ORX_MAX_AT];
+  const int tid = threadIdx.x;
+  if (tid < ORX_MAX_AT) {
+    s_dcg[tid] = 0.0;
+    s_hit[tid] = 0;
+  }
   // rank of the q-th smallest sp = sum_{j > q} hist[j]: thread t owns hist[1 + t * chunk .. (t + 1) * chunk]
   const int chunk = (n + EV_NT - 1) / EV_NT;
   const int jlo = 1 + tid * chunk, jhi = min(n, (tid + 1) * chunk);
   unsigned part = 0;
-  for (int j = jlo; j <= jhi; ++j) part += hist[j];
+  for (int j = jlo; j <= jhi; ++j) part += hist_at(j);
   s_part[tid] = part;
   __syncthreads();
   if (tid == 0) {
@@ -475,7 +553,7 @@ __global__ void __launch_bounds__(EV_NT) k_eval_finish(const EvalArgs a, const E
   }
   unsigned run = s_after[tid];
   for (int j = jhi; j >= jlo; --j) {
-    run += hist[j];                       // rank of position q = j - 1
+    run += hist_at(j);                    // rank of position q = j - 1
     const float ra = (float)run;
     const float rec = 1.f / (logf(ra + 2.f) / logf(2.0f));
 #pragma unroll
@@ -493,14 +571,78 @@ __global__ void __launch_bounds__(EV_NT) k_eval_finish(const EvalArgs a, const E
     }
   __syncthreads();
   if (tid == 0 && o.auc) {
-    const unsigned long long cnt = w.auc_cnt[b] - s_sub;
-    const long long n_eval = a.I - (long long)n - s_extra;
-    o.auc[b] = (float)cnt / (float)((long long)n * n_eval);
+    const long long n_eval = a.I_all - (long long)n - extra;
+    o.auc[b] = (float)auc_cnt / (float)((long long)n * n_eval);
   }
   if (tid < o.n_at) {
     if (o.ndcg) o.ndcg[(int64_t)b * o.n_at + tid] = (float)s_dcg[tid];
     if (o.recall) o.recall[(int64_t)b * o.n_at + tid] = (float)s_hit[tid] / (float)n;
   }
+}
+
+template <int KIND>
+__global__ void __launch_bounds__(EV_NT) k_eval_finish(const EvalRowArgs a, const EvalWs w, const EvalOut o) {
+  __shared__ unsigned long long s_sub;
+  __shared__ long long s_extra;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int info = w.info[2 * b];
+  if (info < 0) {
+    ev_nan_row(o, b);
+    return;
+  }
+  const int n = info;
+  unsigned* hist = w.hist + (int64_t)b * a.P;
+  const EvRow r = ev_row(a, b);
+  if (tid == 0) {
+    s_sub = 0ull;
+    s_extra = 0;
+  }
+  __syncthreads();
+  ev_take_back<KIND, true>(a, b, r, n, w.info[2 * b + 1], w.keys + (int64_t)b * a.P, w.keys + (int64_t)(a.Bu + b) * a.P,
+                           hist, &s_sub, &s_extra);
+  __syncthreads();
+  ev_finish_row(a, o, b, n, s_extra, w.auc_cnt[b] - s_sub, [&](int j) { return hist[j]; });
+}
+
+// Sharded phase 2, after the main pass over this rank's rows: xcnt[b][0] = the row's AUC count and xcnt[b][1..n] its
+// rank hits, both after taking back this rank's own items of pos u excl; the rest of the row 0 (every element written).
+template <int KIND>
+__global__ void __launch_bounds__(EV_NT) k_eval_correct(const EvalRowArgs a, const EvalWs w, int64_t* xcnt) {
+  __shared__ unsigned long long s_sub;
+  __shared__ long long s_extra;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int info = w.info[2 * b];
+  const int n = max(info, 0);
+  unsigned* hist = w.hist + (int64_t)b * a.P;
+  if (tid == 0) {
+    s_sub = 0ull;
+    s_extra = 0;
+  }
+  __syncthreads();
+  if (info >= 0)
+    ev_take_back<KIND, true>(a, b, ev_row(a, b), n, w.info[2 * b + 1], w.keys + (int64_t)b * a.P,
+                             w.keys + (int64_t)(a.Bu + b) * a.P, hist, &s_sub, &s_extra);
+  __syncthreads();
+  for (int j = tid; j < a.P; j += blockDim.x)
+    xcnt[(int64_t)b * a.P + j] = j == 0 ? (int64_t)(w.auc_cnt[b] - s_sub) : j <= n ? (int64_t)hist[j] : 0;
+}
+
+// Sharded phase 3: the outputs from the counts summed over the ranks; n and extra come from the lists alone.
+__global__ void __launch_bounds__(EV_NT) k_eval_finish_counts(const EvalRowArgs a, const int64_t* xcnt, const EvalOut o) {
+  __shared__ long long s_extra;
+  const int b = blockIdx.x;
+  const EvRow r = ev_row(a, b);
+  if (r.bad) {
+    ev_nan_row(o, b);
+    return;
+  }
+  const int n = (int)(r.phi - r.plo);
+  if (threadIdx.x == 0) s_extra = 0;
+  __syncthreads();
+  ev_take_back<ORX_SCORE_DOT, false>(a, b, r, n, 0, nullptr, nullptr, nullptr, nullptr, &s_extra);
+  __syncthreads();
+  const int64_t* cnt = xcnt + (int64_t)b * a.P;
+  ev_finish_row(a, o, b, n, s_extra, (unsigned long long)cnt[0], [&](int j) { return (unsigned)cnt[j]; });
 }
 
 // ---------------------------------------------------------------------------------------
@@ -655,7 +797,7 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_topk(const EvalArgs a, const
     TkRow m = {};
     if (tid < rows) {
       int64_t raw;
-      m.urow = ev_user_row(a, u0 + tid);
+      m.urow = ev_user_row<false>(a, u0 + tid);
       ev_range(a.excl_off, a.excl_items, a.uid[u0 + tid], a.U, a.I, &m.elo, &m.ehi, &raw);
     }
     meta[tid] = m;
@@ -789,9 +931,23 @@ int ev_item_splits(const orx_ctx* h, Kern kern, size_t dyn, int Bu, int64_t I, i
   return ORX_OK;
 }
 
-template <int KIND>
-int ev_launch(orx_ctx* h, const EvalArgs& a, const EvalWs& w, const EvalOut& o, cudaStream_t st) {
-  auto kern = k_score_rank<KIND>;
+// The handle's evaluation scratch for Bu rows of P thresholds each.
+int ev_workspace(orx_ctx* h, int Bu, int P, cudaStream_t st, EvalWs* w) {
+  size_t sort_bytes = 0;
+  ORX_CUDA(cub::DeviceSegmentedSort::SortKeys((void*)nullptr, sort_bytes, (const float*)nullptr, (float*)nullptr,
+                                              2 * Bu * P, 2 * Bu, (const int*)nullptr, (const int*)nullptr, st));
+  const int rc = orx_grow(&h->eval_ws, &h->eval_cap, ev_layout(nullptr, Bu, P, sort_bytes, w));
+  if (rc != ORX_OK) return rc;
+  ev_layout(static_cast<char*>(h->eval_ws), Bu, P, sort_bytes, w);
+  return ORX_OK;
+}
+
+// prep, sort and the main pass over the a.I item rows (no main pass when a.I == 0): the thresholds, AUC counts and
+// rank histograms of every batch row in w, before the take-back.  *variant / *splits: the main pass's dispatch fields
+// (splits 0: not launched).
+template <int KIND, bool XROWS>
+int ev_count(orx_ctx* h, const EvalRowArgs& a, const EvalWs& w, cudaStream_t st, int* variant, int64_t* splits) {
+  auto kern = k_score_rank<KIND, XROWS>;
   int optin = 0;
   ORX_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
   cudaFuncAttributes fa;
@@ -803,9 +959,12 @@ int ev_launch(orx_ctx* h, const EvalArgs& a, const EvalWs& w, const EvalOut& o, 
   const int use_smem = dyn_need <= dyn_max ? 1 : 0;
   const size_t dyn = use_smem ? dyn_need : 0;
   ORX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_max));
-  int64_t splits = 1;
-  const int rc = ev_item_splits(h, kern, dyn, a.Bu, a.I, &splits);
-  if (rc != ORX_OK) return rc;
+  *variant = use_smem ? ORX_VARIANT_RANK_SMEM : ORX_VARIANT_RANK_GLOBAL;
+  *splits = 0;
+  if (a.I > 0) {
+    const int rc = ev_item_splits(h, kern, dyn, a.Bu, a.I, splits);
+    if (rc != ORX_OK) return rc;
+  }
   const int64_t user_tiles = (a.Bu + EV_TU - 1) / EV_TU;
 
   k_eval_prep<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w);
@@ -813,12 +972,53 @@ int ev_launch(orx_ctx* h, const EvalArgs& a, const EvalWs& w, const EvalOut& o, 
   size_t bytes = w.sort_bytes;
   ORX_CUDA(cub::DeviceSegmentedSort::SortKeys(w.sort_tmp, bytes, (const float*)w.keys_in, w.keys, 2 * a.Bu * a.P,
                                               2 * a.Bu, (const int*)w.seg_begin, (const int*)w.seg_end, st));
-  kern<<<dim3((unsigned)splits, (unsigned)user_tiles), EV_NT, dyn, st>>>(a, w, use_smem);
-  ORX_LAUNCH_CHECK();
+  if (*splits > 0) {
+    EvalArgs t = a;
+    if (XROWS) t.user_tab = a.xrows;
+    kern<<<dim3((unsigned)*splits, (unsigned)user_tiles), EV_NT, dyn, st>>>(t, w, use_smem);
+    ORX_LAUNCH_CHECK();
+  }
+  return ORX_OK;
+}
+
+template <int KIND>
+int ev_launch(orx_ctx* h, const EvalRowArgs& a, const EvalWs& w, const EvalOut& o, cudaStream_t st) {
+  int variant = 0;
+  int64_t splits = 0;
+  const int rc = ev_count<KIND, false>(h, a, w, st, &variant, &splits);
+  if (rc != ORX_OK) return rc;
   k_eval_finish<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w, o);
   ORX_LAUNCH_CHECK();
-  orx_log_dispatch(h, ORX_OP_SCORE_RANK, use_smem ? ORX_VARIANT_RANK_SMEM : ORX_VARIANT_RANK_GLOBAL, KIND, 0, a.Bu,
-                   (int)(a.I > INT32_MAX ? INT32_MAX : a.I), a.D, (int)splits);
+  orx_log_dispatch(h, ORX_OP_SCORE_RANK, variant, KIND, 0, a.Bu, (int)(a.I > INT32_MAX ? INT32_MAX : a.I), a.D,
+                   (int)splits);
+  return ORX_OK;
+}
+
+// One phase of orx_score_rank_shard (arguments checked by the caller).
+template <int KIND>
+int ev_shard_phase(orx_ctx* h, int phase, const EvalRowArgs& a, const EvalOut& o, int32_t* xrows, int32_t* xpred,
+                   int64_t* xcnt, cudaStream_t st) {
+  if (phase == 0) {
+    const int64_t blocks = ((int64_t)a.Bu * a.D + EV_NT - 1) / EV_NT;
+    k_eval_user_rows<<<(unsigned)(blocks < 4096 ? blocks : 4096), EV_NT, 0, st>>>(a, xrows);
+  } else if (phase == 1) {
+    k_eval_pos_scores<KIND><<<a.Bu, EV_NT, 0, st>>>(a, xpred);
+  } else if (phase == 2) {
+    EvalWs w;
+    int rc = ev_workspace(h, a.Bu, a.P, st, &w);
+    if (rc != ORX_OK) return rc;
+    int variant = 0;
+    int64_t splits = 0;
+    rc = ev_count<KIND, true>(h, a, w, st, &variant, &splits);
+    if (rc != ORX_OK) return rc;
+    k_eval_correct<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w, xcnt);
+    ORX_LAUNCH_CHECK();
+    orx_log_dispatch(h, ORX_OP_SCORE_RANK_SHARD, variant, KIND, a.rank, a.Bu, (int)a.I, a.D, (int)splits);
+    return ORX_OK;
+  } else {
+    k_eval_finish_counts<<<a.Bu, EV_NT, 0, st>>>(a, xcnt, o);
+  }
+  ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
 
@@ -849,6 +1049,13 @@ int tk_launch(orx_ctx* h, const EvalArgs& a, int k, int32_t* top_items, float* t
   return ORX_OK;
 }
 
+EvalOut ev_out(const int32_t* at_host, int n_at, float* auc, float* ndcg, float* recall) {
+  EvalOut o;
+  for (int k = 0; k < ORX_MAX_AT; ++k) o.at[k] = k < n_at ? at_host[k] : 0;
+  o.n_at = n_at; o.auc = auc; o.ndcg = ndcg; o.recall = recall;
+  return o;
+}
+
 }  // namespace
 
 extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
@@ -868,20 +1075,14 @@ extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_ta
   cudaStream_t st = (cudaStream_t)s;
 
   EvalWs w;
-  size_t sort_bytes = 0;
-  ORX_CUDA(cub::DeviceSegmentedSort::SortKeys((void*)nullptr, sort_bytes, (const float*)nullptr, (float*)nullptr,
-                                              (int)(2 * Bu * P), 2 * Bu, (const int*)nullptr, (const int*)nullptr, st));
-  const int rc = orx_grow(&h->eval_ws, &h->eval_cap, ev_layout(nullptr, Bu, (int)P, sort_bytes, &w));
+  const int rc = ev_workspace(h, Bu, (int)P, st, &w);
   if (rc != ORX_OK) return rc;
-  ev_layout(static_cast<char*>(h->eval_ws), Bu, (int)P, sort_bytes, &w);
 
-  EvalArgs a;
+  EvalRowArgs a = {};
   a.user_tab = user_tab; a.U = U; a.uid = uid; a.Bu = Bu; a.scale = scale; a.item_tab = item_tab;
-  a.bias = item_bias; a.I = I; a.D = dim; a.pos_off = pos_off; a.excl_off = excl_off; a.pos_items = pos_items;
-  a.excl_items = excl_items; a.max_pos = max_pos; a.P = (int)P;
-  EvalOut o;
-  for (int k = 0; k < ORX_MAX_AT; ++k) o.at[k] = k < n_at ? at_host[k] : 0;
-  o.n_at = n_at; o.auc = auc; o.ndcg = ndcg; o.recall = recall;
+  a.bias = item_bias; a.I = I; a.I_all = I; a.world = 1; a.rank = 0; a.D = dim; a.pos_off = pos_off;
+  a.excl_off = excl_off; a.pos_items = pos_items; a.excl_items = excl_items; a.max_pos = max_pos; a.P = (int)P;
+  const EvalOut o = ev_out(at_host, n_at, auc, ndcg, recall);
   return kind == ORX_SCORE_DOT ? ev_launch<ORX_SCORE_DOT>(h, a, w, o, st)
                                : ev_launch<ORX_SCORE_NEG_SQDIST>(h, a, w, o, st);
 }
@@ -902,4 +1103,55 @@ extern "C" int orx_score_topk(orx_handle_t h, int32_t kind, const float* user_ta
   a.bias = item_bias; a.I = I; a.D = dim; a.excl_off = excl_off; a.excl_items = excl_items;
   return kind == ORX_SCORE_DOT ? tk_launch<ORX_SCORE_DOT>(h, a, k, top_items, top_scores, (cudaStream_t)s)
                                : tk_launch<ORX_SCORE_NEG_SQDIST>(h, a, k, top_items, top_scores, (cudaStream_t)s);
+}
+
+extern "C" int orx_score_rank_shard_sizes(int32_t Bu, int32_t dim, int32_t max_pos, int64_t* n3_host) {
+  ORX_REQUIRE(n3_host != nullptr, "null pointer");
+  ORX_REQUIRE(Bu >= 0 && dim > 0 && max_pos >= 0, "bad sizes");
+  const int64_t P = (int64_t)max_pos + 1;
+  ORX_REQUIRE(2 * (int64_t)Bu * P <= INT32_MAX, "Bu * (max_pos + 1) too large for one call: split the batch");
+  n3_host[0] = (int64_t)Bu * dim;
+  n3_host[1] = n3_host[2] = (int64_t)Bu * P;
+  return ORX_OK;
+}
+
+extern "C" int orx_score_rank_shard(orx_handle_t h, int32_t kind, int32_t phase, const orx_rowshard_t* g_host,
+                                    const float* user_shard, const float* item_shard, const float* bias_shard,
+                                    int32_t dim, const int32_t* uid, int32_t Bu, const int64_t* pos_off,
+                                    const int32_t* pos_items, const int64_t* excl_off, const int32_t* excl_items,
+                                    int32_t max_pos, const int32_t* at_host, int32_t n_at, int32_t* xrows,
+                                    int32_t* xpred, int64_t* xcnt, float* auc, float* ndcg, float* recall,
+                                    orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr && g_host != nullptr, "null pointer");
+  ORX_REQUIRE(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST, "unknown score kind");
+  ORX_REQUIRE(phase >= 0 && phase <= 3, "phase must lie in [0, 3]");
+  const orx_rowshard_t g = *g_host;
+  ORX_REQUIRE(g.world >= 1 && g.rank >= 0 && g.rank < g.world, "rank must lie in [0, world)");
+  ORX_REQUIRE(g.total_users > 0 && g.total_items > 0 && g.total_items <= INT32_MAX, "bad table sizes");
+  ORX_REQUIRE(g.local_users == (g.total_users - g.rank + g.world - 1) / g.world &&
+                  g.local_items == (g.total_items - g.rank + g.world - 1) / g.world,
+              "local_users / local_items disagree with (total, world, rank)");
+  ORX_REQUIRE(dim > 0 && Bu >= 0 && max_pos >= 0, "bad sizes");
+  ORX_REQUIRE(n_at >= 0 && n_at <= ORX_MAX_AT, "at most 8 cut-offs");
+  ORX_REQUIRE(n_at == 0 || at_host, "null cut-offs");
+  if (Bu == 0) return ORX_OK;
+  const int64_t P = (int64_t)max_pos + 1;
+  ORX_REQUIRE(2 * (int64_t)Bu * P <= INT32_MAX, "Bu * (max_pos + 1) too large for one call: split the batch");
+  ORX_REQUIRE(uid && pos_off, "null pointer");
+  ORX_REQUIRE(phase != 0 || (user_shard && xrows), "phase 0 needs user_shard and xrows");
+  ORX_REQUIRE(phase != 1 || (item_shard && xrows && xpred), "phase 1 needs item_shard, xrows and xpred");
+  ORX_REQUIRE(phase != 2 || (item_shard && xrows && xpred && xcnt), "phase 2 needs item_shard, xrows, xpred, xcnt");
+  ORX_REQUIRE(phase != 3 || xcnt, "phase 3 needs xcnt");
+  ORX_CUDA(cudaSetDevice(h->device));
+
+  EvalRowArgs a = {};
+  a.user_tab = user_shard; a.U = g.total_users; a.uid = uid; a.Bu = Bu; a.item_tab = item_shard; a.bias = bias_shard;
+  a.I = g.local_items; a.I_all = g.total_items; a.world = g.world; a.rank = g.rank; a.D = dim; a.pos_off = pos_off;
+  a.excl_off = excl_off; a.pos_items = pos_items; a.excl_items = excl_items; a.max_pos = max_pos; a.P = (int)P;
+  a.xrows = phase >= 1 ? reinterpret_cast<const float*>(xrows) : nullptr;
+  a.xpred = phase == 2 ? reinterpret_cast<const float*>(xpred) : nullptr;
+  const EvalOut o = ev_out(at_host, n_at, auc, ndcg, recall);
+  cudaStream_t st = (cudaStream_t)s;
+  return kind == ORX_SCORE_DOT ? ev_shard_phase<ORX_SCORE_DOT>(h, phase, a, o, xrows, xpred, xcnt, st)
+                               : ev_shard_phase<ORX_SCORE_NEG_SQDIST>(h, phase, a, o, xrows, xpred, xcnt, st);
 }

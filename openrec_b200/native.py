@@ -9,7 +9,7 @@ import torch
 
 from . import _lib
 from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP,
-                   ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
+                   ORX_OP_SCORE_RANK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
                    ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
                    ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
                    ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE,
@@ -21,13 +21,22 @@ __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", 
            "ORX_OP_POINTWISE_STEP", "ORX_VARIANT_GEMM_TMA", "ORX_VARIANT_GEMM_SIMT", "ORX_VARIANT_INTERACT_WARP",
            "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC",
            "ORX_OP_SCORE_RANK", "ORX_VARIANT_RANK_SMEM", "ORX_VARIANT_RANK_GLOBAL", "ORX_OP_SCORE_TOPK",
-           "ORX_VARIANT_TOPK", "Dispatch"]
+           "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "Dispatch", "RowShard", "rowshard"]
 
 _engines = {}
 
 # one record of orx_debug_dispatch_log: which kernel an orx_mlp_layer_* / orx_interact_* call or a sparse step launched
 # (the field meanings per op are in include/orx.h)
 Dispatch = namedtuple("Dispatch", "op variant ta tb m n k s")
+
+# geometry of a row-sharded table pair: row r of every table lives on rank r % world at local row r // world
+RowShard = namedtuple("RowShard", "world rank total_users total_items local_users local_items")
+
+
+def rowshard(world, rank, total_users, total_items):
+    """RowShard of `rank`: local_* = ceil((total - rank) / world) (0 for a rank past the table's end)."""
+    return RowShard(world, rank, total_users, total_items, (total_users - rank + world - 1) // world,
+                    (total_items - rank + world - 1) // world)
 
 
 def _ptr(t):
@@ -321,6 +330,43 @@ class Engine:
             _ptr(pos_items), _ptr(excl_off), _ptr(excl_items), int(max_pos), at_arr, len(at), _ptr(auc), _ptr(ndcg),
             _ptr(rec), self.stream()), "orx_score_rank")
         return auc, ndcg, rec
+
+    @staticmethod
+    def score_rank_shard_sizes(Bu, dim, max_pos):
+        """-> element counts of the exchange buffers (xrows int32, xpred int32, xcnt int64) of score_rank_shard."""
+        n3 = (C.c_int64 * 3)()
+        _lib.check(_lib.lib().orx_score_rank_shard_sizes(int(Bu), int(dim), int(max_pos), n3),
+                   "orx_score_rank_shard_sizes")
+        return tuple(n3)
+
+    def score_rank_shard(self, kind, phase, g, user_shard, item_shard, bias_shard, uid, pos_off, pos_items, excl_off,
+                         excl_items, max_pos, xrows, xpred, xcnt, at=()):
+        """One phase of score_rank over row-sharded tables (orx_score_rank_shard in include/orx.h).  g: RowShard;
+        the shards are this rank's rows (bias_shard flat [local_items] or None); uid and the CSR lists are global.  The
+        caller sums each exchange buffer over the ranks between phases (openrec_b200.sharded.score_rank_sharded).
+        Phase 3 -> (auc [Bu], ndcg [Bu, len(at)], recall [Bu, len(at)]); other phases -> None."""
+        uid = ids32(uid)
+        Bu, dev = uid.numel(), xrows.device
+        pos_off, pos_items = _csr(pos_off, pos_items, g.total_users)
+        excl_off, excl_items = _csr(excl_off, excl_items, g.total_users)
+        if pos_off is None:
+            raise ValueError("score_rank_shard needs the positives' CSR")
+        if xrows.dtype != torch.int32 or xpred.dtype != torch.int32 or xcnt.dtype != torch.int64:
+            raise ValueError("exchange buffers: xrows / xpred int32, xcnt int64")
+        at_arr = (C.c_int32 * max(len(at), 1))(*[int(k) for k in at])
+        out = [None] * 3
+        if phase == 3:
+            out = [torch.empty(Bu, dtype=torch.float32, device=dev),
+                   torch.empty((Bu, len(at)), dtype=torch.float32, device=dev),
+                   torch.empty((Bu, len(at)), dtype=torch.float32, device=dev)]
+        geo = _lib.OrxRowShard(*[int(x) for x in g])
+        _lib.check(self.lib.orx_score_rank_shard(
+            self.h, kind, int(phase), C.byref(geo), _ptr(_f32(user_shard, "user_shard")),
+            _ptr(_f32(item_shard, "item_shard")), _ptr(_f32(bias_shard, "bias_shard")), user_shard.shape[1],
+            _ptr(uid), Bu, _ptr(pos_off), _ptr(pos_items), _ptr(excl_off), _ptr(excl_items), int(max_pos), at_arr,
+            len(at), _ptr(xrows), _ptr(xpred), _ptr(xcnt), *[_ptr(t) for t in out], self.stream()),
+            "orx_score_rank_shard")
+        return tuple(out) if phase == 3 else None
 
     def score_topk(self, kind, user_tab, uid, item_tab, item_bias, excl_off, excl_items, k, scale=None):
         """The k best eligible items of each user uid in one pass over the item table, without the [Bu, I] score

@@ -123,6 +123,47 @@ class ShardedPairwise:
         return outs
 
 
+def score_rank_sharded(parts, reduce, uid, pos_off, pos_items, excl_off, excl_items, max_pos, at=()):
+    """Catalogue evaluation (AUC / NDCG / Recall, as native.Engine.score_rank on the global tables) of row-sharded
+    tables, each rank counting over its own item rows: the four phases of orx_score_rank_shard, with ``reduce`` between
+    them.  parts[k] = (eng, kind, user_shard, item_shard, bias_shard or None, g) for each rank this process drives
+    (g: native.RowShard); uid (global user ids) and the global CSR lists live on every part's device.
+    ``reduce(tensors)`` replaces each tensor (one per part) in place by its element-wise integer sum over ALL ranks:
+    all_reduce_sum(group) when each process is one rank, loopback_sum for virtual ranks on one device.
+    -> [(auc, ndcg, recall)] per part, identical on every rank."""
+    bufs = []
+    for eng, kind, user, item, bias, g in parts:
+        n3 = eng.score_rank_shard_sizes(uid.numel(), user.shape[1], max_pos)
+        dev = item.device
+        bufs.append((torch.empty(n3[0], dtype=torch.int32, device=dev), torch.empty(n3[1], dtype=torch.int32, device=dev),
+                     torch.empty(n3[2], dtype=torch.int64, device=dev)))
+    outs = [None] * len(parts)
+    for phase in range(4):   # every part's phase k is issued before any part's phase k + 1
+        for k, ((eng, kind, user, item, bias, g), b) in enumerate(zip(parts, bufs)):
+            outs[k] = eng.score_rank_shard(kind, phase, g, user, item, bias, uid, pos_off, pos_items, excl_off,
+                                           excl_items, max_pos, *b, at=at)
+        if phase < 3:
+            reduce([b[phase] for b in bufs])
+    return outs
+
+
+def all_reduce_sum(group=None):
+    """reduce for score_rank_sharded with one rank per process: an all-reduce (SUM) on torch's current stream."""
+    def reduce(tensors):
+        for t in tensors:
+            dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
+    return reduce
+
+
+def loopback_sum(tensors):
+    """reduce for score_rank_sharded with every rank in this process (virtual ranks on one device)."""
+    total = tensors[0].clone()
+    for t in tensors[1:]:
+        total += t
+    for t in tensors:
+        t.copy_(total)
+
+
 class _PeerBuf:
     """A cudaMalloc'd, IPC-exportable device buffer viewed as a torch tensor (orx_peer_alloc)."""
 

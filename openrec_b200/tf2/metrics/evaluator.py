@@ -13,6 +13,7 @@ import torch
 
 from ... import native as N
 from ..._lib import ORX_MAX_AT
+from ...sharded import all_reduce_sum, score_rank_sharded
 from ...tfshim.core import Tensor
 from ..data.user_lists import positives_csr, user_csr
 
@@ -50,6 +51,11 @@ class RankingEvaluator:
         return self._dev[1:]
 
     def evaluate(self, model):
+        """A row-sharded model (ShardedBPR / ShardedUCML) is evaluated collectively: every rank builds the same
+        evaluator and calls evaluate; each rank counts over its own item rows and every rank gets the same result."""
+        sharded = getattr(model, "_sharded_score_operands", None)
+        if sharded is not None:
+            return self._evaluate_sharded(*sharded())
         ops = getattr(model, "_score_operands", None)
         if ops is None:
             raise NotImplementedError(f"{type(model).__name__}: catalogue evaluation needs the model's whole item "
@@ -64,7 +70,23 @@ class RankingEvaluator:
             a, n, r = eng.score_rank(kind, user, uids[b0:b1], item, bias, pos_off, pos_items, excl_off, excl_items,
                                      max_pos, at=self.at, scale=scale)
             auc.append(a), ndcg.append(n), rec.append(r)
+        return self._result(auc, ndcg, rec, item.device)
+
+    def _evaluate_sharded(self, kind, user, item, bias, g, group):
+        uids, pos_off, pos_items, excl_off, excl_items = self._upload(item.device)
+        part = (N.engine(), kind, user, item, bias, g)
+        reduce = all_reduce_sum(group)
+        auc, ndcg, rec = [], [], []
+        for b0 in range(0, len(self.warm_users), self.batch_size):
+            b1 = min(b0 + self.batch_size, len(self.warm_users))
+            max_pos = int(self._pos_len[self.warm_users[b0:b1]].max())
+            (a, n, r), = score_rank_sharded([part], reduce, uids[b0:b1], pos_off, pos_items, excl_off, excl_items,
+                                            max_pos, at=self.at)
+            auc.append(a), ndcg.append(n), rec.append(r)
+        return self._result(auc, ndcg, rec, item.device)
+
+    def _result(self, auc, ndcg, rec, device):
         if not auc:
-            empty = torch.zeros((0, len(self.at)), dtype=torch.float32, device=item.device)
+            empty = torch.zeros((0, len(self.at)), dtype=torch.float32, device=device)
             return {"AUC": Tensor(empty[:, 0]), "NDCG": Tensor(empty), "Recall": Tensor(empty.clone())}
         return {"AUC": Tensor(torch.cat(auc)), "NDCG": Tensor(torch.cat(ndcg)), "Recall": Tensor(torch.cat(rec))}

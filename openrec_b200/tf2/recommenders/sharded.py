@@ -32,6 +32,7 @@ class _Shard:
 
 class ShardedBPR(Model):
     _kind = N.ORX_PAIR_BPR
+    _score = N.ORX_SCORE_DOT
 
     def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items, seed=0):
         super().__init__()
@@ -114,6 +115,13 @@ class ShardedBPR(Model):
         node.stepped = True
         node.ids = None
 
+    def _sharded_score_operands(self):
+        """(score kind, user shard, item shard, item bias shard as a flat [rows] view, native.RowShard, process group)
+        of the catalogue evaluation over the shards (RankingEvaluator: one collective call on every rank)."""
+        g = N.rowshard(self._world, self._rank, self._U, self._I)
+        return (self._score, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
+                self.item_bias.embeddings.t.reshape(-1), g, None)
+
     def inference(self, user_id):
         raise NotImplementedError("full-catalogue scoring needs the whole item table on one device")
 
@@ -125,6 +133,7 @@ class ShardedBPR(Model):
 
 class ShardedUCML(ShardedBPR):
     _kind = N.ORX_PAIR_UCML
+    _score = N.ORX_SCORE_NEG_SQDIST
 
     def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items, margin=0.5, seed=0):
         super().__init__(dim_user_embed, dim_item_embed, total_users, total_items, seed=seed)
