@@ -118,6 +118,13 @@ enum orx_dispatch_variant {
 };
 #define ORX_DISPATCH_LOG_CAP 64
 ORX_API int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec_host, int32_t cap, int32_t* n_host);
+/* Test hook: the per-triplet records a prefetch resolved for index set `set` (1 or 2, as in a dispatch record), copied
+ * to the device int32[B][4] rec on `stream` once that prefetch is complete: {flags, du, dp, dn} of triplet t, flags bit 0
+ * = its three ids are in range, bits 1/2/3 = the user / positive / negative row is referenced once in the batch; du /
+ * dp / dn = the row's staging index, -1 for such a row (ADAM_DENSE: every row has one, bits 1-3 are 0).  The records
+ * of a set last until the second prefetch after it.  ORX_ERR_INVALID when the handle has none (ORX_PAIR_RESOLVE=0 at
+ * orx_create, or no prefetch yet). */
+ORX_API int orx_debug_pair_records(orx_handle_t h, int32_t set, int32_t* rec, int32_t B, orx_stream_t stream);
 
 /* Measurement hook (bench.py's roofline): while enabled, every 8th *_step call records CUDA events on its launch stream
  * around its launches -- orx_pairwise_step, orx_pairwise_step_host and orx_pointwise_step: [0] batch index (or the wait

@@ -69,6 +69,7 @@ SIGNATURES = {
     "orx_stream_synchronize": [_vp, _vp],
     "orx_debug_set_epoch": [_vp, C.c_uint32],
     "orx_debug_dispatch_log": [_vp, C.POINTER(_i32), _i32, C.POINTER(_i32)],
+    "orx_debug_pair_records": [_vp, _i32, _vp, _i32, _vp],
     "orx_profile_enable": [_vp, _i32],
     "orx_profile_read": [_vp, C.POINTER(C.c_float), _i32, C.POINTER(_i32)],
     "orx_fill_uniform": [_vp, _vp, _i64, _f, _f, _u64, _vp],

@@ -79,6 +79,9 @@ struct orx_ctx {
   int pf_valid, pf_set, pf_next, pf_B, pf_mode;        // the one outstanding prefetched index and what it was built for
   const int32_t *pf_uid, *pf_pid, *pf_nid;
   int64_t pf_rows_u, pf_rows_i;
+  int4* pf_res[2];         // per-triplet records {flags, du, dp, dn} of prefetched set k (k_index_resolve, orx_pairwise.cu)
+  size_t pf_res_cap[2];    // bytes
+  int pair_resolve;        // ORX_PAIR_RESOLVE, read at orx_create: 0 = no records, a prefetched step probes the index
   uint32_t epoch;          // hash epoch of the last step, in [1, 2^31)
   void* shard_ws;          // orx_shard.cu: host bookkeeping of the row-sharded step (orx_shard_ws*)
   void* shard_scratch;     // orx_shard.cu: its local device scratch, carved by sh_layout
@@ -589,8 +592,8 @@ struct OrxStepLaunch {
   int n_partials, variant, minb;
 };
 // A family's step kernel, launched on the driver's stream with the shared arguments (index sets chosen) and the
-// handle's partials.
-typedef std::function<int(const SparseArgs& s, float* partials, OrxStepLaunch* out)> OrxStepKernel;
+// handle's partials; res = the per-triplet records of a consumed prefetch (k_index_resolve), else null.
+typedef std::function<int(const SparseArgs& s, const int4* res, float* partials, OrxStepLaunch* out)> OrxStepKernel;
 // One fused pairwise or pointwise step on st: validate, workspace, partials, batch index (a pairwise batch, nid != null,
 // takes its prefetched index when one matches), profile marks 0..3, kernel(...), dispatch record {op, variant, kind,
 // opt, B, D, minb, index set}, ADAM_DENSE sweeps, tail (loss scaled by loss_scale into out4; w: GMF's dense weight,

@@ -102,6 +102,8 @@ int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim) {
   }
   c->pf_valid = 0;
   c->pf_free_valid[0] = c->pf_free_valid[1] = 0;
+  for (int k = 0; k < 2 && c->pair_resolve; ++k)
+    if ((rc = orx_grow((void**)&c->pf_res[k], &c->pf_res_cap[k], sizeof(int4) * (size_t)nb)) != ORX_OK) return rc;
   c->g_rows_u = nb;
   c->g_rows_i = 2 * nb;
   size_t bu = sizeof(float) * (size_t)c->g_rows_u * nd, bi = sizeof(float) * (size_t)c->g_rows_i * nd;
@@ -206,6 +208,8 @@ extern "C" int orx_create(int device, orx_handle_t* out) {
   c->device = device;
   c->num_sms = prop.multiProcessorCount;
   c->partials_cap = sizeof(float) * 2 * (size_t)c->num_sms * 64;
+  const char* pr = getenv("ORX_PAIR_RESOLVE");   // 0: prefetched pairwise steps probe the index (A/B measurements)
+  c->pair_resolve = (pr && atoi(pr) == 0) ? 0 : 1;
   if (cudaMalloc(&c->counters, sizeof(int32_t) * 16) != cudaSuccess ||
       cudaMalloc(&c->bucket_cursor, sizeof(int32_t) * 1024) != cudaSuccess ||
       cudaMalloc(&c->partials, c->partials_cap) != cudaSuccess ||
@@ -228,6 +232,7 @@ extern "C" int orx_destroy(orx_handle_t h) {
   for (int i = 0; i < 2; ++i) {
     cudaFree(h->ids_stage[i]);
     cudaFree(h->out_stage[i]);
+    cudaFree(h->pf_res[i]);
   }
   cudaFree(h->counters);
   cudaFree(h->partials);

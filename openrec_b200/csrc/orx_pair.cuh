@@ -8,6 +8,9 @@ struct PairArgs : SparseArgs {
   int B;
   float margin, c_loss, c_l2, inv_B;
   float* partials;
+  // k_pair_step of a prefetched batch: record t = {flags, du, dp, dn} of triplet t (k_index_resolve), read in place of the
+  // id bounds check and the three index probes.  Null: probe the index.
+  const int4* res;
   // un-fused outputs (k_pair_generic MODE 1).  ld = 0: table form, outputs indexed by triplet.  ld > D: row form
   // (orx_pairwise_grad_rows) -- U = I = fetched rows of stride ld with the item bias in column D, outputs written to the
   // lookup's own row of d_user = d_pos = d_neg.

@@ -7,6 +7,9 @@
 //
 // Synchronous-batch semantics in three launches on one stream:
 //   1. k_index_build : hash every id of the batch's valid triplets; rows hit more than once get a "staging" slot.
+//      A batch prefetched on the side stream (orx_pairwise_prefetch, orx_pairwise_step_host) is also resolved there:
+//      k_index_resolve writes each triplet's probe answers as one record {flags, du, dp, dn}, which k_pair_step
+//      reads in place of probing the index.
 //   2. k_pair_step   : per triplet gather u,p,n (128-bit loads), score, loss, per-sample gradient.
 //        * a row referenced exactly once in the batch is owned by its triplet: optimizer applied
 //          in registers, row + slots written back once (read once, written once == algorithmic bytes);
@@ -44,6 +47,34 @@ __global__ void k_index_build(OrxHash hu, OrxHash hi, const int32_t* __restrict_
     if (!g) atomicAdd(bad, 1);
     else if (all) orx_hash_insert(hi, i < 2 * n ? ib0 : ib1, stage_all);
   }
+}
+
+// The probe answers of a prefetched pairwise batch, once its index (hu, hi) is complete: one thread per triplet writes
+// res[t] = {flags, du, dp, dn} exactly as k_pair_step's probes would find them -- flags bit 0: the three ids are in range;
+// bits 1/2/3: the user / pos / neg row is referenced once in the batch (owned by this triplet); du / dp / dn: staging
+// index, -1 for an owned row.  Mode 1 (ADAM_DENSE) stages every row: all three indices, no owned bits.  An invalid
+// triplet gets {0, -1, -1, -1}.
+__global__ void k_index_resolve(OrxHash hu, OrxHash hi, const int32_t* __restrict__ uid, const int32_t* __restrict__ pid,
+                                const int32_t* __restrict__ nid, int64_t rows_u, int64_t rows_i, int n, int mode,
+                                int4* __restrict__ res) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const int32_t u = uid[t], p = pid[t], q = nid[t];
+  int4 r = make_int4(0, -1, -1, -1);
+  if (u >= 0 && (int64_t)u < rows_u && p >= 0 && (int64_t)p < rows_i && q >= 0 && (int64_t)q < rows_i) {
+    if (mode == 1) {
+      orx_hash_find(hu, u, &r.y);
+      orx_hash_find(hi, p, &r.z);
+      orx_hash_find(hi, q, &r.w);
+      r.x = 1;
+    } else {
+      const uint32_t cu = orx_hash_find<true>(hu, u, &r.y);
+      const uint32_t cp = orx_hash_find<true>(hi, p, &r.z);
+      const uint32_t cn = orx_hash_find<true>(hi, q, &r.w);
+      r.x = 1 | (cu == 1u ? 2 : 0) | (cp == 1u ? 4 : 0) | (cn == 1u ? 8 : 0);
+    }
+  }
+  res[t] = r;
 }
 
 __global__ void k_index_build_strided(OrxHash hu, const int32_t* __restrict__ a, int64_t stride, int64_t rows, int n,
@@ -85,7 +116,6 @@ struct TripRegs {
   float4 us0[K], ps0[K], ns0[K];  // dead arrays are eliminated when the optimizer has no such slot
   float4 us1[K], ps1[K], ns1[K];
   int fl, uu, pp, nn, du, dp, dn;
-  float bp, bn;
 };
 
 // flags: bit0 triplet valid, bit1/2/3 user/pos/neg row owned by this triplet (fast path)
@@ -94,6 +124,8 @@ struct TripRegs {
 //   ids (coalesced, lanes < CH) -> variable rows of the first one/two triplet groups (they need only
 //   the ids) -> hash probes + bias loads (lanes < CH, overlap the row loads) -> slot rows of the first
 //   groups -> steady state: process one register buffer while the other's 128-bit loads are in flight.
+//   With a.res (a prefetched batch) the ids come with their record, so there are no probes: the slot rows of the first
+//   groups follow their variable rows and the bias loads without waiting for anything.
 // L2 priority: table and slot rows are loaded and stored evict-first (orx_ld4_stream / orx_st4_stream); the probes and
 // the item bias + slot loads are evict-last (orx_ld_keep), the staging red.adds and the bias stores normal, so that the
 // index, the bias and the staging rows are still in L2 when they are reused.
@@ -113,13 +145,21 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
   const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
   orx_pdl_wait();
 
-  // ---- ids of triplet t (lanes < CH)
+  // ---- ids of triplet t (lanes < CH), and its record when the index was resolved ahead (a.res)
   int u_id = 0, p_id = 0, n_id = 0, du = -1, dp = -1, dn = -1, flags = 0;
   if (lane < CH && t < a.B) {
     u_id = a.uid[t];
     p_id = a.pid[t];
     n_id = a.nid[t];
-    flags = (u_id >= 0 && u_id < a.rowsU && p_id >= 0 && p_id < a.rowsI && n_id >= 0 && n_id < a.rowsI) ? 1 : 0;
+    if (a.res) {
+      const int4 r = __ldcs(a.res + t);
+      flags = r.x;
+      du = r.y;
+      dp = r.z;
+      dn = r.w;
+    } else {
+      flags = (u_id >= 0 && u_id < a.rowsU && p_id >= 0 && p_id < a.rowsI && n_id >= 0 && n_id < a.rowsI) ? 1 : 0;
+    }
   }
 
   // variable rows: need ids + the valid bit only
@@ -141,16 +181,19 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
   load_var(0, ra);
   if (PIPE && TPW < CH) load_var(TPW, rb);
 
-  // ---- hash probes + item_bias (lanes < CH), overlapping the row loads above; L2 evict-last (orx_ld_keep)
+  // ---- hash probes (no a.res) + item_bias (lanes < CH), overlapping the row loads above; L2 evict-last (orx_ld_keep)
   float bp = 0.f, bn = 0.f, bps0 = 0.f, bps1 = 0.f, bns0 = 0.f, bns1 = 0.f;
   if (flags & 1) {
-    const uint32_t cu = orx_hash_find<!SL::STAGE_ONLY, true>(a.hu, u_id, &du);
-    const uint32_t cp = orx_hash_find<!SL::STAGE_ONLY, true>(a.hi, p_id, &dp);
-    const uint32_t cn = orx_hash_find<!SL::STAGE_ONLY, true>(a.hi, n_id, &dn);
+    uint32_t cu = 0, cp = 0, cn = 0;
+    if (!a.res) {
+      cu = orx_hash_find<!SL::STAGE_ONLY, true>(a.hu, u_id, &du);
+      cp = orx_hash_find<!SL::STAGE_ONLY, true>(a.hi, p_id, &dp);
+      cn = orx_hash_find<!SL::STAGE_ONLY, true>(a.hi, n_id, &dn);
+    }
     bp = orx_ld_keep(a.Bv + p_id);
     bn = orx_ld_keep(a.Bv + n_id);
     if (!SL::STAGE_ONLY) {
-      flags |= (cu == 1u ? 2 : 0) | (cp == 1u ? 4 : 0) | (cn == 1u ? 8 : 0);
+      if (!a.res) flags |= (cu == 1u ? 2 : 0) | (cp == 1u ? 4 : 0) | (cn == 1u ? 8 : 0);
       if (SL::S0) {
         if (flags & 4) bps0 = orx_ld_keep(a.Bs0 + p_id);
         if (flags & 8) bns0 = orx_ld_keep(a.Bs0 + n_id);
@@ -162,15 +205,14 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
     }
   }
 
-  // optimizer-slot rows + staging indices: need the probe results
+  // optimizer-slot rows + staging indices: need the probe results (or the record).  The item bias is shuffled only where
+  // the score needs it, so that no row load waits for a bias load.
   auto load_slots = [&](int j, Regs& r) {
     const int src = j + grp;
     r.fl = __shfl_sync(ORX_FULL, flags, src);
     r.du = __shfl_sync(ORX_FULL, du, src);
     r.dp = __shfl_sync(ORX_FULL, dp, src);
     r.dn = __shfl_sync(ORX_FULL, dn, src);
-    r.bp = __shfl_sync(ORX_FULL, bp, src);
-    r.bn = __shfl_sync(ORX_FULL, bn, src);
 #pragma unroll
     for (int k = 0; k < K; ++k) {
       const int off = (k * G + gl) * 4;
@@ -208,7 +250,8 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
     s1 = orx_group_sum<G>(s1);
     s2 = orx_group_sum<G>(s2);
     float lt, g;
-    pair_score<KIND>(s1, s2, r.bp, r.bn, a.margin, a.c_loss, a.inv_B, &lt, &g);
+    pair_score<KIND>(s1, s2, __shfl_sync(ORX_FULL, bp, j + grp), __shfl_sync(ORX_FULL, bn, j + grp), a.margin, a.c_loss,
+                     a.inv_B, &lt, &g);
     const bool v = r.fl & 1;
     if (!v) { lt = 0.f; g = 0.f; }
     if (gl == 0) loss_acc += lt;
@@ -580,6 +623,11 @@ static int prefetch_issue(orx_ctx* c, const int32_t* uid, const int32_t* pid, co
   k_index_build<<<(3 * B + 255) / 256, 256, 0, ss>>>(c->pf_u[k], c->pf_i[k], uid, rows_u, pid, nid, rows_i, B, mode,
                                                      c->counters + 4 * (1 + k) + 3);
   ORX_LAUNCH_CHECK();
+  if (c->pair_resolve) {   // the probe answers too: the step then reads one record per triplet (pf_done follows them)
+    k_index_resolve<<<(B + 255) / 256, 256, 0, ss>>>(c->pf_u[k], c->pf_i[k], uid, pid, nid, rows_u, rows_i, B, mode,
+                                                      c->pf_res[k]);
+    ORX_LAUNCH_CHECK();
+  }
   ORX_CUDA(cudaEventRecord(c->pf_done[k], ss));
   c->pf_valid = 1; c->pf_set = k; c->pf_uid = uid; c->pf_pid = pid; c->pf_nid = nid; c->pf_B = B;
   c->pf_rows_u = rows_u; c->pf_rows_i = rows_i; c->pf_mode = mode;
@@ -604,6 +652,18 @@ extern "C" int orx_pairwise_prefetch(orx_handle_t h, const orx_table_t* user, co
     ORX_CUDA(cudaStreamWaitEvent(h->side_stream, h->side_ev, 0));
   }
   return prefetch_issue(h, uid, pid, nid, B, user->rows, item->rows, opt_kind == ORX_OPT_ADAM_DENSE ? 1 : 0);
+}
+
+// test hook: the first B records k_index_resolve wrote for prefetch set `set` (1 or 2), copied to rec on s once that
+// set's prefetch is complete
+extern "C" int orx_debug_pair_records(orx_handle_t h, int32_t set, int32_t* rec, int32_t B, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr && rec && (set == 1 || set == 2) && B > 0, "bad arguments");
+  ORX_REQUIRE(h->pair_resolve && h->side_stream && sizeof(int4) * (size_t)B <= h->pf_res_cap[set - 1],
+              "no records of that many triplets (ORX_PAIR_RESOLVE=0, no prefetch yet, or B beyond the workspace)");
+  ORX_CUDA(cudaSetDevice(h->device));
+  ORX_CUDA(cudaStreamWaitEvent((cudaStream_t)s, h->pf_done[set - 1], 0));
+  ORX_CUDA(cudaMemcpyAsync(rec, h->pf_res[set - 1], sizeof(int4) * (size_t)B, cudaMemcpyDeviceToDevice, (cudaStream_t)s));
+  return ORX_OK;
 }
 
 int orx_sparse_step(orx_ctx* c, int op, int kind, const orx_table_t* user, const orx_table_t* item,
@@ -637,7 +697,7 @@ int orx_sparse_step(orx_ctx* c, int op, int kind, const orx_table_t* user, const
   orx_prof_mark(c, 1, st);
   const SparseArgs s = orx_sparse_args(c, user, item, bias, HU, HI, orx_opt_to_dev(opt));
   OrxStepLaunch L = {};
-  if ((rc = kernel(s, c->partials, &L))) return rc;
+  if ((rc = kernel(s, set && c->pair_resolve ? c->pf_res[set - 1] : nullptr, c->partials, &L))) return rc;
   orx_log_dispatch(c, op, L.variant, kind, opt->kind, B, D, L.minb, set);
   orx_prof_mark(c, 2, st);
   if (dense && (rc = orx_launch_adam_sweeps(c, user, item, bias, HU, HI, s.opt, st))) return rc;
@@ -674,9 +734,10 @@ static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, con
   ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
   ORX_REQUIRE(nid != nullptr, "empty batch or null ids");
   const float inv_B = 1.0f / (float)B;
-  const auto kernel = [&](const SparseArgs& s, float* partials, OrxStepLaunch* out) {
+  const auto kernel = [&](const SparseArgs& s, const int4* res, float* partials, OrxStepLaunch* out) {
     PairArgs pa = pair_args(s, user->rows, item->rows, uid, pid, nid, B, margin, c_loss, c_l2, inv_B);
     pa.partials = partials;
+    pa.res = res;   // k_pair_generic probes the index whatever res is
     return orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {
       return orx_dispatch_opt(opt->kind, [&](auto O) {
         return launch_pair_step_kind_opt<decltype(K)::value, decltype(O)::value>(pa, st, out);

@@ -305,7 +305,7 @@ extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_
   const orx_table_t* dense_w = (kind == ORX_POINT_GMF) ? w : nullptr;
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
-  const auto kernel = [&](const SparseArgs& sa, float* partials, OrxStepLaunch* out) {
+  const auto kernel = [&](const SparseArgs& sa, const int4* /*res: pairwise only*/, float* partials, OrxStepLaunch* out) {
     PointArgs pa = point_args(sa, dense_w, user, item, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2);
     pa.partials = partials;
     pa.gw = dense_w ? h->gw : nullptr;

@@ -172,6 +172,13 @@ class Engine:
                    "orx_debug_dispatch_log")
         return [Dispatch(*rec[8 * i:8 * i + 8]) for i in range(n.value)]
 
+    def debug_pair_records(self, index_set, B):
+        """-> int32 [B, 4] CUDA tensor: the records {flags, du, dp, dn} a prefetch resolved for index set 1 or 2."""
+        rec = torch.empty((B, 4), dtype=torch.int32, device=self.device)
+        _lib.check(self.lib.orx_debug_pair_records(self.h, index_set, _ptr(rec), B, self.stream()),
+                   "orx_debug_pair_records")
+        return rec
+
     def pairwise_fwd(self, kind, user, item, bias, uid, pid, nid, out4, margin=0.5):
         _lib.check(self.lib.orx_pairwise_fwd(self.h, kind, C.byref(user), C.byref(item), C.byref(bias), _ptr(uid),
                                              _ptr(pid), _ptr(nid), uid.numel(), margin, _ptr(out4), self.stream()),
