@@ -79,7 +79,8 @@ ORX_API int orx_destroy(orx_handle_t h);
 ORX_API int orx_device_count(int* n_out_host);
 /* Blocks the host until `stream` has drained (cudaStreamSynchronize). */
 ORX_API int orx_stream_synchronize(orx_handle_t h, orx_stream_t stream);
-/* Test hook: place the handle's batch-index epoch counter (31 bits; the wrap path empties the hash tables). */
+/* Test hook: place the handle's batch-index epoch counter, and those of the index sets of orx_shard_step once it has
+ * run (31 bits; the wrap path empties the hash tables). */
 ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
 /* Test hook: the kernel variants launched by this handle's DLRM entry points (orx_mlp_layer_*, orx_interact_*) and
  * sparse steps (orx_pairwise_step, orx_pairwise_step_host, orx_pointwise_step) since the last call, oldest first, at
@@ -252,11 +253,7 @@ ORX_API int orx_pairwise_grad_rows(orx_handle_t h, int32_t kind, const float* ro
  *   next_uid / next_pid / next_nid / next_B (all NULL / 0, or all set: device pointers that stay valid until that step
  *   ran) announce the batch of step epoch + 1: its route and request then ride inside this step's apply launch, and the
  *   call for epoch + 1 -- which must pass exactly these pointers as uid / pid / nid -- issues four launches instead of six.
- *   All ranks announce, or none.  The announced step's user index lives in the handle's index sets until that call:
- *   meanwhile (and between the phases of a step issued phase by phase) any call on the handle that would grow its
- *   workspace, orx_pairwise_prefetch / orx_pairwise_step_host, and an index-epoch take that would wrap return
- *   ORX_ERR_INVALID before any device work.  Calls that need none of these (orx_pairwise_step within the workspace,
- *   scoring, sampling) are accepted.
+ *   All ranks announce, or none.  Other calls on the handle may come between steps and between phases.
  *   out4 = { loss, l2_loss (GLOBAL batch, identical on every rank), skipped triplets of this rank, staged rows }.
  *   The sticky error word flags[4*64] is 0 or: 1 a peer never arrived within timeout_ms, 2 more triplets routed to this
  *   home than home_cap, 3 / 4 request / gradient inbox too small.  SGD, Adagrad and row-sparse Adam. */

@@ -47,6 +47,10 @@ struct OrxHash {
   uint32_t epoch;  // current epoch, >= 1
 };
 
+// Shape of an index set for `lookups` ids: sets t.mask and t.shift, returns the slot count, the least power of two
+// (>= 1024) that holds 4x the lookups.  did takes lookups + 1 entries.
+uint32_t orx_hash_shape(OrxHash& t, int64_t lookups);
+
 struct orx_ctx {
   int device;
   int num_sms;
@@ -111,10 +115,8 @@ static inline void orx_log_dispatch(orx_ctx* c, int op, int variant, int TA, int
 // slot can never alias the current epoch (about 65 h of back-to-back steps between wraps).
 int orx_next_epoch(orx_ctx* c, cudaStream_t st);
 void orx_shard_ws_release(orx_ctx* c);
-// true while a row-sharded step on this handle has an index that must survive until its next orx_shard_step call (an
-// announced batch's user index, built inside the previous step's apply launch; or a step issued phase by phase).
-// Workspace growth, a prefetch and an epoch wrap are refused meanwhile: each would empty or overwrite that index.
-bool orx_shard_holds_index(const orx_ctx* c);
+// orx_debug_set_epoch: place the epoch counters of the row-sharded step's own index sets too, once they exist
+void orx_shard_set_epoch(orx_ctx* c, uint32_t epoch);
 
 #define ORX_PROF_EV 8   // event slots per sampled step: up to 7 phases (the sharded step has seven launches)
 // record phase boundary k (0..7) of the current step on `st` when profiling is enabled

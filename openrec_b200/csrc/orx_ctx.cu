@@ -58,20 +58,20 @@ static void free_workspace(orx_ctx* c) {
   c->g_dim = 0;
 }
 
-static uint32_t pow2_at_least(int64_t n) {
-  uint32_t p = 1024;
-  while ((int64_t)p < n) p <<= 1;
-  return p;
-}
-
-static int alloc_hash(OrxHash& t, int64_t lookups, int32_t* counter) {
+uint32_t orx_hash_shape(OrxHash& t, int64_t lookups) {
   // load factor <= 0.25: with linear probing the slowest of a warp's 32 inserts/probes sets the pace
   // (profile r1b: ~7 serialized L2 round trips per warp at 0.5)
-  uint32_t cap = pow2_at_least(4 * lookups);
+  uint32_t cap = 1024;
+  while ((int64_t)cap < 4 * lookups) cap <<= 1;
   int lg = 0;
   while ((1u << lg) < cap) ++lg;
   t.mask = cap - 1;
   t.shift = 32 - lg;
+  return cap;
+}
+
+static int alloc_hash(OrxHash& t, int64_t lookups, int32_t* counter) {
+  const uint32_t cap = orx_hash_shape(t, lookups);
   t.counter = counter;
   ORX_CUDA(cudaMalloc(&t.slots, sizeof(unsigned long long) * cap));
   ORX_CUDA(cudaMalloc(&t.didx, sizeof(int32_t) * cap));
@@ -84,11 +84,6 @@ static int alloc_hash(OrxHash& t, int64_t lookups, int32_t* counter) {
 // staged (ADAM_DENSE stages all rows), so the staging buffers hold B resp. 2B rows of `dim` floats.
 int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim) {
   if (B <= c->cap_B && dim <= c->g_dim) return ORX_OK;
-  if (orx_shard_holds_index(c)) {
-    orx_set_error("workspace growth to %lld lookups / dim %d refused: a sharded step's announced batch holds this "
-                  "handle's index sets until its orx_shard_step call", (long long)B, dim);
-    return ORX_ERR_INVALID;
-  }
   int64_t nb = B > c->cap_B ? B : c->cap_B;
   int32_t nd = dim > c->g_dim ? dim : c->g_dim;
   ORX_CUDA(cudaDeviceSynchronize());
@@ -131,11 +126,6 @@ static int zero_hash(OrxHash& t) {
 }
 
 int orx_next_epoch(orx_ctx* c, cudaStream_t /*st*/) {
-  if (c->epoch == 0x7fffffffu && orx_shard_holds_index(c)) {
-    orx_set_error("index epoch wrap refused: a sharded step's announced batch holds this handle's index sets until its "
-                  "orx_shard_step call");
-    return ORX_ERR_INVALID;
-  }
   c->epoch = (c->epoch + 1) & 0x7fffffffu;
   if (c->epoch == 0) {
     // 31-bit wrap (once per 2^31 index builds): a stale slot could alias the epochs to come, so every table is emptied.
@@ -152,10 +142,11 @@ int orx_next_epoch(orx_ctx* c, cudaStream_t /*st*/) {
   return ORX_OK;
 }
 
-// test hook: place the epoch counter (tests/test_gpu_kernels.py::test_epoch_wrap starts it just below 2^31)
+// test hook: place the epoch counters (tests/test_gpu_kernels.py::test_epoch_wrap starts them just below 2^31)
 extern "C" int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch) {
   ORX_REQUIRE(h != nullptr && epoch < 0x80000000u, "null handle / epoch must be < 2^31");
   h->epoch = epoch;
+  orx_shard_set_epoch(h, epoch);
   return ORX_OK;
 }
 

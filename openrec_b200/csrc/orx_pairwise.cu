@@ -581,9 +581,9 @@ static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, OrxSte
 // ---- pipelined batch index ------------------------------------------------------------------------------------------
 // The index of a batch depends only on its ids, so it can be built while the PREVIOUS step's kernels still run: on the
 // context's side stream, into one of two "prefetch" index sets (hash tables + counters) that alternate -- set 0 stays
-// with everything that builds its index on the caller's stream (pointwise / DLRM / censor / sharded / un-prefetched
-// pairwise steps).  The step that consumes a prefetched index waits for it with an event; the set is handed back with
-// an event recorded behind that step's tail.
+// with everything that builds its index on the caller's stream (pointwise / DLRM / censor / un-prefetched pairwise
+// steps; the row-sharded step keeps index sets of its own, orx_shard.cu).  The step that consumes a prefetched index
+// waits for it with an event; the set is handed back with an event recorded behind that step's tail.
 static int side_stream_ensure(orx_ctx* c) {
   if (c->side_stream) return ORX_OK;
   ORX_CUDA(cudaStreamCreateWithFlags(&c->side_stream, cudaStreamNonBlocking));
@@ -639,8 +639,6 @@ extern "C" int orx_pairwise_prefetch(orx_handle_t h, const orx_table_t* user, co
                                      orx_stream_t ids_stream) {
   ORX_REQUIRE(h != nullptr && user && item && uid && pid && nid && B > 0, "bad arguments");
   ORX_REQUIRE(orx_opt_kind_ok(opt_kind), "unknown optimizer kind");
-  ORX_REQUIRE(!orx_shard_holds_index(h), "a sharded step's announced batch holds this handle's index sets (a prefetch "
-                                         "would overwrite one) until its orx_shard_step call");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t is = (cudaStream_t)ids_stream;
   int rc = orx_ensure_workspace(h, B, user->dim);
@@ -767,8 +765,6 @@ extern "C" int orx_pairwise_step_host(orx_handle_t h, int32_t kind, const orx_ta
                                       const orx_opt_t* opt, float* out4_host, orx_stream_t s) {
   ORX_REQUIRE(h != nullptr, "null handle");
   ORX_REQUIRE(B > 0 && uid_host && pid_host && nid_host && out4_host && user && item && opt, "empty batch or null host buffers");
-  ORX_REQUIRE(!orx_shard_holds_index(h), "a sharded step's announced batch holds this handle's index sets (this entry "
-                                         "point prefetches into one) until its orx_shard_step call");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
   int rc;

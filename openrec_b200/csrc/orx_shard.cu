@@ -57,10 +57,11 @@ enum { SH_M_TRIPS = 0,    // triplets r routed to X                             
        SH_M_GINBASE = 3,  // first row of owner r's `gin` that home X fills, -1 = overflow (k_sh_serve)
        SH_M_LOSS = 4, SH_M_L2 = 5 };   // r's partial sums, float bits                (k_sh_compute)
 
-// local control words (ShardWs::ctl)
+// local control words (ShardWs::ctl).  SH_C_CNT + p: staged rows of user index set p (p = step parity), + 2: the block
+// ticket of k_sh_tail (TailArgs::counters[2]), + 3: staged rows of the item index set.
 enum { SH_C_CURH = 0, SH_C_CURO = SH_MAX_R, SH_C_GOFF = 2 * SH_MAX_R, SH_C_RCO = 3 * SH_MAX_R + 1,
        SH_C_DONE = 4 * SH_MAX_R + 1, SH_C_T = SH_C_DONE + 8, SH_C_NREQ = SH_C_T + 1, SH_C_ACUR = SH_C_T + 2,
-       SH_C_BAD = SH_C_T + 4 /* + step parity */, SH_C_WORDS = SH_C_T + 8 };
+       SH_C_BAD = SH_C_T + 4 /* + step parity */, SH_C_CNT = SH_C_T + 8, SH_C_WORDS = SH_C_CNT + 4 };
 
 struct ShardHost {   // mirrors orx_shard_t (include/orx.h)
   int32_t world, rank, dim, batch_cap, home_cap, req_cap, gin_cap, timeout_ms;
@@ -717,11 +718,15 @@ __global__ void __launch_bounds__(256) k_sh_tail(ShardDev x, ShardWs w, TailArgs
 // host side
 // ---------------------------------------------------------------------------------------
 struct orx_shard_ws {
-  ShardWs w;                         // carved from the handle's shard_scratch by sh_layout
-  int home_cap, gin_cap, got_rows;
+  // carved from the handle's shard_scratch by sh_layout
+  ShardWs w;
+  OrxHash hu[2], hi;                 // the step's index sets: users by step parity, items; .epoch = the last epoch taken
+  float *gu, *gi, *gb;               // their staging rows: user [nb][dim], item [2 nb][dim], item bias [2 nb]
+  int home_cap, gin_cap, got_rows, dim;
   const void* occ_fn[32];            // sh_ctas_per_sm: resident CTAs per SM of each persistent kernel launched so far
   int occ[32], n_occ;
   // prologue bookkeeping, per step parity: which step's route / request were issued, with which index epochs and ids
+  // (a step's user epoch is taken with its route, its item epoch with its serve)
   int32_t pro_route[2], pro_request[2];
   uint32_t ep_u[2], ep_i[2];
   const int32_t *ids_u[2], *ids_p[2], *ids_n[2];
@@ -780,18 +785,36 @@ static int sh_ctas_per_sm(orx_shard_ws* s, const void* fn, int cap) {
   return nb < cap ? nb : cap;
 }
 
-// The local scratch (trip_u | slot | req | ctl) inside one allocation; with base == nullptr only the size is computed.
-static size_t sh_layout(char* base, int home_cap, int gin_cap, ShardWs* w) {
+// The local scratch inside one allocation: trip_u | slot | req | ctl, the index sets hu[0], hu[1], hi (slots | didx |
+// did each) and the staging rows gu | gi | gb.  The sets and staging rows are sized as a handle's workspace for
+// nb = max(home_cap, ceil(gin_cap / 2)) lookups: home_cap user rows, gin_cap item rows.  With base == nullptr only the
+// size is computed.
+static size_t sh_layout(char* base, int home_cap, int gin_cap, int dim, orx_shard_ws* s) {
   size_t off = 0;
-  auto take = [&](size_t words) {
-    int32_t* p = base ? reinterpret_cast<int32_t*>(base + off) : nullptr;
-    off += (sizeof(int32_t) * words + 255) & ~(size_t)255;
+  auto take = [&](size_t bytes) {
+    char* p = base ? base + off : nullptr;
+    off += (bytes + 255) & ~(size_t)255;
     return p;
   };
-  w->trip_u = take((size_t)home_cap);
-  w->slot = take(2 * (size_t)home_cap);
-  w->req = take((size_t)gin_cap);
-  w->ctl = take(SH_C_WORDS);
+  ShardWs& w = s->w;
+  w.trip_u = (int32_t*)take(sizeof(int32_t) * home_cap);
+  w.slot = (int32_t*)take(sizeof(int32_t) * 2 * (size_t)home_cap);
+  w.req = (int32_t*)take(sizeof(int32_t) * gin_cap);
+  w.ctl = (int32_t*)take(sizeof(int32_t) * SH_C_WORDS);
+  const int64_t nb = home_cap > (gin_cap + 1) / 2 ? home_cap : (gin_cap + 1) / 2;
+  auto hash = [&](OrxHash& t, int64_t lookups, int counter_word) {
+    const uint32_t cap = orx_hash_shape(t, lookups);
+    t.slots = (unsigned long long*)take(sizeof(unsigned long long) * cap);
+    t.didx = (int32_t*)take(sizeof(int32_t) * cap);
+    t.did = (int32_t*)take(sizeof(int32_t) * (size_t)(lookups + 1));
+    t.counter = base ? w.ctl + counter_word : nullptr;
+  };
+  hash(s->hu[0], nb, SH_C_CNT + 0);
+  hash(s->hu[1], nb, SH_C_CNT + 1);
+  hash(s->hi, 2 * nb, SH_C_CNT + 3);
+  s->gu = (float*)take(sizeof(float) * (size_t)nb * dim);
+  s->gi = (float*)take(sizeof(float) * 2 * (size_t)nb * dim);
+  s->gb = (float*)take(sizeof(float) * 2 * (size_t)nb);
   return off;
 }
 
@@ -801,26 +824,37 @@ void orx_shard_ws_release(orx_ctx* c) {
   c->shard_ws = nullptr;
 }
 
-// A route issued for a step whose tail has not been issued yet: that step's user index lives in pf_u[its parity]
-bool orx_shard_holds_index(const orx_ctx* c) {
-  const orx_shard_ws* s = (const orx_shard_ws*)c->shard_ws;
-  return s && (s->pro_route[0] > s->tail_epoch || s->pro_route[1] > s->tail_epoch);
+void orx_shard_set_epoch(orx_ctx* c, uint32_t epoch) {
+  orx_shard_ws* s = (orx_shard_ws*)c->shard_ws;
+  if (s) s->hu[0].epoch = s->hu[1].epoch = s->hi.epoch = epoch;
 }
 
 static int shard_ws_ensure(orx_ctx* c, const ShardHost* x, cudaStream_t st) {
   orx_shard_ws* s = (orx_shard_ws*)c->shard_ws;
   const int got_rows = sh_got_rows(x->home_cap, x->world);
-  if (s && s->home_cap >= x->home_cap && s->gin_cap >= x->gin_cap && s->got_rows >= got_rows) return ORX_OK;
-  // a new layout starts afresh: zeroed bookkeeping and control words
+  if (s && s->home_cap >= x->home_cap && s->gin_cap >= x->gin_cap && s->got_rows >= got_rows && s->dim >= x->dim)
+    return ORX_OK;
+  // a new layout starts afresh: zeroed bookkeeping, epochs, control words, index slots and staging rows
   orx_shard_ws_release(c);
   c->shard_ws = s = new orx_shard_ws();
-  int rc = orx_grow(&c->shard_scratch, &c->shard_cap, sh_layout(nullptr, x->home_cap, x->gin_cap, &s->w));
+  const size_t bytes = sh_layout(nullptr, x->home_cap, x->gin_cap, x->dim, s);
+  int rc = orx_grow(&c->shard_scratch, &c->shard_cap, bytes);
   if (rc) return rc;
-  sh_layout(static_cast<char*>(c->shard_scratch), x->home_cap, x->gin_cap, &s->w);
-  ORX_CUDA(cudaMemsetAsync(s->w.ctl, 0, sizeof(int32_t) * SH_C_WORDS, st));
+  sh_layout(static_cast<char*>(c->shard_scratch), x->home_cap, x->gin_cap, x->dim, s);
+  ORX_CUDA(cudaMemsetAsync(c->shard_scratch, 0, bytes, st));
   s->home_cap = x->home_cap;
   s->gin_cap = x->gin_cap;
   s->got_rows = got_rows;
+  s->dim = x->dim;
+  return ORX_OK;
+}
+
+// The next epoch of one of the step's index sets (31 bits, like the handle's).  On the wrap the set is emptied on st:
+// every launch that reads or writes it runs on st and was issued before, so no stale slot aliases the epochs to come.
+static int sh_take_epoch(OrxHash& t, cudaStream_t st, uint32_t* ep) {
+  const uint32_t e = (t.epoch + 1) & 0x7fffffffu;
+  if (e == 0) ORX_CUDA(cudaMemsetAsync(t.slots, 0, sizeof(unsigned long long) * ((size_t)t.mask + 1), st));
+  *ep = t.epoch = e ? e : 1;
   return ORX_OK;
 }
 
@@ -874,22 +908,6 @@ static inline auto sh_dispatch_nq(int nq, F&& f) {
   return orx_dispatch<1, 2, 4>(nq <= 32 ? 1 : (nq <= 64 ? 2 : 4), f);
 }
 
-// two fresh index epochs (user set of the step, item set of the step).  A 31-bit wrap empties every table of the handle
-// after draining the device (orx_next_epoch), which must not happen while another step's index is live: `may_drain` says
-// whether it may; returns 1 (and takes nothing) when it may not and the wrap is near.
-static int shard_take_epochs(orx_ctx* c, cudaStream_t st, bool may_drain, uint32_t* eu, uint32_t* ei) {
-  if (c->epoch >= 0x7ffffff0u) {
-    if (!may_drain) return 1;
-    c->epoch = 0x7fffffffu;      // wrap now, at a step boundary: both epochs come from after the wrap
-  }
-  int rc;
-  if ((rc = orx_next_epoch(c, st))) return rc;
-  *eu = c->epoch;
-  if ((rc = orx_next_epoch(c, st))) return rc;
-  *ei = c->epoch;
-  return ORX_OK;
-}
-
 // One step (or a sub-range of its six launches: phases 0 route, 1 request, 2 serve, 3 compute, 4 apply, 5 tail); see the
 // file header.  out4 = { loss, l2_loss, skipped triplets (ids out of range), staged rows }, the first two GLOBAL and
 // identical on every rank.
@@ -923,9 +941,6 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
   ORX_REQUIRE(orx_opt_slots_ok(opt->kind, {user, item, item_bias}), "optimizer slot rows missing");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
-  // index hashes + staging: user side <= home_cap lookups, item side <= gin_cap lookups
-  const int64_t need = x->home_cap > (x->gin_cap + 1) / 2 ? x->home_cap : (x->gin_cap + 1) / 2;
-  if ((rc = orx_ensure_workspace(h, need, x->dim))) return rc;
   if ((rc = shard_ws_ensure(h, x, st))) return rc;
   orx_shard_ws* S = (orx_shard_ws*)h->shard_ws;
   if (S->owner != x->flags) {        // another model on this handle (each has its own mailboxes): its steps start afresh
@@ -936,7 +951,6 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
     S->serve_epoch = S->tail_epoch = 0;
     S->owner = x->flags;
   }
-  ORX_REQUIRE(!h->pf_valid, "this handle has an index prefetched by orx_pairwise_prefetch outstanding (the sharded step uses the same index sets)");
   const ShardWs& w = S->w;
   const ShardDev xd = shard_to_dev(x);
   const int par = epoch & 1;
@@ -950,28 +964,21 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
 
   // phases 0 / 1: unless this step's prologue was already issued (announced in the previous call, or explicitly)
   if (phase_lo == 0 && S->pro_route[par] != epoch) {
-    if ((rc = shard_take_epochs(h, st, S->serve_epoch == S->tail_epoch, &S->ep_u[par], &S->ep_i[par])) != ORX_OK) {
-      if (rc == 1) { orx_set_error("orx_shard_step: index epochs are about to wrap; issue this step's route after the previous step's tail"); return ORX_ERR_INVALID; }
-      return rc;
-    }
+    if ((rc = sh_take_epoch(S->hu[par], st, &S->ep_u[par]))) return rc;
     S->ids_u[par] = uid; S->ids_p[par] = pid; S->ids_n[par] = nid; S->ids_B[par] = B;
   }
   if (S->pro_route[par] == epoch || phase_lo == 0)      // whichever way the prologue was issued: it must be for THIS batch
     ORX_REQUIRE(S->ids_u[par] == uid && S->ids_p[par] == pid && S->ids_n[par] == nid && S->ids_B[par] == B,
                 "this step's batch differs from the one its route was issued for (announced as next_* in the previous call)");
-  OrxHash hu = h->pf_u[par];
+  OrxHash hu = S->hu[par];
   hu.epoch = S->ep_u[par];
-  OrxHash hi = h->hi;
-  hi.epoch = S->ep_i[par];
+  OrxHash hi = S->hi;
+  hi.epoch = S->ep_i[par];   // taken below when this call issues the serve
 
   ShCompArgs ca;
-  ca.U = user->var; ca.Us0 = user->s0; ca.Us1 = user->s1; ca.hu = hu; ca.gu = h->gu;
+  ca.U = user->var; ca.Us0 = user->s0; ca.Us1 = user->s1; ca.hu = hu; ca.gu = S->gu;
   ca.margin = margin; ca.c_loss = c_loss; ca.c_l2 = c_l2; ca.inv_B = inv_B; ca.opt = od; ca.partials = h->partials;
   ca.loss_scale = kind == ORX_PAIR_BPR ? inv_B : 1.f;
-  ShApplyArgs aa;
-  aa.I = item->var; aa.Is0 = item->s0; aa.Is1 = item->s1;
-  aa.Bv = item_bias->var; aa.Bs0 = item_bias->s0; aa.Bs1 = item_bias->s1;
-  aa.hi = hi; aa.gi = h->gi; aa.gb = h->gb; aa.opt = od;
   const bool whole = phase_lo == 0 && phase_hi == 5;     // the measurement hook follows whole steps only
   for (int ph = phase_lo; ph <= phase_hi; ++ph) {
     if (whole) orx_prof_mark(h, ph, st);
@@ -992,6 +999,9 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
         break;
       case 2:
         ORX_REQUIRE(S->pro_request[par] == epoch, "phase 2 before this step's phases 0 and 1");
+        // the item set's epoch: apply and tail of the previous step, its last readers, were issued before this
+        if ((rc = sh_take_epoch(S->hi, st, &S->ep_i[par]))) return rc;
+        hi.epoch = S->ep_i[par];
         sh_dispatch_nq(nq, [&](auto Q) {
           auto kern = k_sh_serve<decltype(Q)::value>;
           orx_launch_pdl(kern, dim3(h->num_sms * sh_ctas_per_sm(S, (const void*)kern, 4)), dim3(256), 0, st, xd, w,
@@ -1014,18 +1024,21 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
         ShProArgs pro;
         memset(&pro, 0, sizeof(pro));
         const int np = par ^ 1;
-        if (announce && S->pro_route[np] != epoch + 1 &&
-            shard_take_epochs(h, st, false, &S->ep_u[np], &S->ep_i[np]) == ORX_OK) {
+        if (announce && S->pro_route[np] != epoch + 1) {
+          if ((rc = sh_take_epoch(S->hu[np], st, &S->ep_u[np]))) return rc;
           pro.n_route = (next_B + 1023) / 1024;
           pro.n_request = request_blocks;
           pro.epoch = epoch + 1;
           pro.r.uid = next_uid; pro.r.pid = next_pid; pro.r.nid = next_nid; pro.r.B = next_B;
           pro.r.U = total_users; pro.r.I = total_items;
-          pro.hu = h->pf_u[np];
-          pro.hu.epoch = S->ep_u[np];
+          pro.hu = S->hu[np];
           S->ids_u[np] = next_uid; S->ids_p[np] = next_pid; S->ids_n[np] = next_nid; S->ids_B[np] = next_B;
           S->pro_route[np] = S->pro_request[np] = epoch + 1;
         }
+        ShApplyArgs aa;
+        aa.I = item->var; aa.Is0 = item->s0; aa.Is1 = item->s1;
+        aa.Bv = item_bias->var; aa.Bs0 = item_bias->s0; aa.Bs1 = item_bias->s1;
+        aa.hi = hi; aa.gi = S->gi; aa.gb = S->gb; aa.opt = od;
         sh_dispatch_opt(opt->kind, [&](auto O) {
           sh_dispatch_nq(nq, [&](auto Q) {
             auto kern = k_sh_apply<decltype(O)::value, decltype(Q)::value>;
@@ -1037,8 +1050,13 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
       }
       case 5: {
         const int g = h->num_sms * 4;   // the grid of k_sparse_tail
-        TailArgs ta = {orx_sparse_args(h, user, item, item_bias, hu, hi, od)};
-        ta.counters = h->counters;   // [2]: the tail's block ticket
+        TailArgs ta = {};
+        ta.U = user->var; ta.Us0 = user->s0; ta.Us1 = user->s1;
+        ta.I = item->var; ta.Is0 = item->s0; ta.Is1 = item->s1;
+        ta.Bv = item_bias->var; ta.Bs0 = item_bias->s0; ta.Bs1 = item_bias->s1;
+        ta.gu = S->gu; ta.gi = S->gi; ta.gb = S->gb;
+        ta.hu = hu; ta.hi = hi; ta.opt = od; ta.D = x->dim;
+        ta.counters = w.ctl + SH_C_CNT;
         ta.out4 = out4;
         sh_dispatch_opt(opt->kind, [&](auto O) {
           orx_launch_pdl(k_sh_tail<decltype(O)::value>, dim3(g), dim3(256), 0, st, xd, w, ta, par);

@@ -438,17 +438,9 @@ class LoopbackGroup:
         return [o[:2] for o in outs]
 
     def _issue_early(self, next_batches, c_loss, c_l2):
-        """Route (phase 0) of the announced batches for every rank, then request (phase 1).  A rank whose index epochs
-        are about to wrap refuses its route: the wrap empties its index sets, so it must wait for this step's tail.  The
-        fused prologue skips itself in that case; here the request phase is skipped for every rank, and the next step's
-        call issues the routes that are still missing and all requests."""
+        """Route (phase 0) of the announced batches for every rank, then request (phase 1)."""
         for r, m in enumerate(self.ranks):
-            try:
-                m._call(*next_batches[r], c_loss, c_l2, 0, 0, epoch=m.iterations + 1)
-            except RuntimeError as e:
-                if "about to wrap" not in str(e):
-                    raise
-                return
+            m._call(*next_batches[r], c_loss, c_l2, 0, 0, epoch=m.iterations + 1)
         for r, m in enumerate(self.ranks):
             m._call(*next_batches[r], c_loss, c_l2, 1, 1, epoch=m.iterations + 1)
 

@@ -119,8 +119,9 @@ def test_announced_batch_must_match():
 
 
 def test_loopback_index_epoch_wrap():
-    """Index epochs of the sharded step wrap at 2^31 (two per step): tables are emptied at a step boundary, and a batch
-    is not hoisted across the wrap."""
+    """The epochs of the sharded step's index sets wrap at 2^31 (the item set takes one a step, each user set one every
+    other step): a set is emptied on the step's stream when its epoch wraps, also while an announced batch is in
+    flight."""
     from openrec_b200.sharded import LoopbackGroup
     rng = np.random.default_rng(3)
     U, I, D, B = 97, 131, 32, 256
@@ -133,7 +134,7 @@ def test_loopback_index_epoch_wrap():
         g.step(batches[0])      # builds the workspace
         O.pairwise_train_step("bpr", user, item, bias, *[t.cpu().numpy() for t in batches[0][0]], O.OPT_ADAGRAD, st, 1, 0.05)
         m = g.ranks[0]
-        m.eng.debug_set_epoch(0x7fffffff - 24)
+        m.eng.debug_set_epoch(0x7fffffff - 4)      # the item set wraps at the 5th step, the user sets at the 9th / 10th
         for k in range(1, 13):
             g.step(batches[k], next_batches=batches[k + 1])
             O.pairwise_train_step("bpr", user, item, bias, *[t.cpu().numpy() for t in batches[k][0]], O.OPT_ADAGRAD, st, k + 1, 0.05)

@@ -6,7 +6,7 @@
 * exactly on, and one triplet past, each mailbox capacity (home_cap, the padded gradient inbox gin_cap, req_cap);
 * at batch tails (plain and announced), loss / l2 scales other than 1, bad ids in a tail;
 * over kind x optimizer x row width, at 16 and 64 ranks, across the index-epoch wrap with announced batches;
-* beside the other entry points of a rank's handle while an announced batch holds its index sets.
+* beside the other entry points of a rank's handle while an announced batch is outstanding.
 
 Each step compares the global (loss, l2) of every rank (bit-identical across ranks), all three tables, every optimizer
 slot, and out4[2] (skipped triplets) / out4[3] (staged rows) of each rank against counts taken from the ids."""
@@ -445,14 +445,14 @@ def test_large_worlds(world):
 
 # ---- epoch wrap ------------------------------------------------------------------------------------------------------
 def test_epoch_wrap_announced_world3():
-    """Every rank's index epoch starts just below 2^31; announced steps cross the wrap (a route that cannot be hoisted
-    across it is issued by its own step instead)."""
+    """The epoch counters of every rank's index sets start 4 below 2^31 - 1; announced steps cross the wrap of the item
+    set (one epoch a step, at the 5th step) and of both user sets (one epoch every other step, at the 9th / 10th)."""
     run = Run(3, 0, 1, 97, 131, 32, 256, seed=71)
     try:
         cur = run.prep(run.uniform(256))
         cur = run.step(cur, lambda: run.uniform(256))
         for m in run.g.ranks:
-            m.eng.debug_set_epoch(0x7fffffff - 24)
+            m.eng.debug_set_epoch(0x7fffffff - 4)
         for k in range(12):
             cur = run.step(cur, lambda: run.uniform(256), announce=True)
         run.step(cur)
@@ -467,77 +467,85 @@ def _shared_run():
 
 def _cap_B(run):
     m = run.g.ranks[0]
-    return max(m.home_cap, (m.gin_cap + 1) // 2)      # what orx_shard_step sized the handle's workspace for
+    return max(m.home_cap, (m.gin_cap + 1) // 2)      # lookups the sharded step's user index sets are sized for
 
 
-def _small_pairwise(eng, rng, B):
-    """A pairwise_step on its own tables of `eng`, compared with the oracle."""
-    U, I, D = 50, 60, 64
-    user, item, bias = (rng.uniform(-0.05, 0.05, s).astype(np.float32) for s in ((U, D), (I, D), (I, 1)))
-    uid, pid, nid = (rng.integers(0, n, B).astype(np.int32) for n in (U, I, I))
-    t = [torch.from_numpy(a).cuda() for a in (user, item, bias)]
-    acc = [torch.full_like(x, 0.1) for x in t]
-    out4 = torch.zeros(4, device="cuda")
-    eng.pairwise_step(N.ORX_PAIR_BPR, *(N.table(x, s) for x, s in zip(t, acc)),
-                      *(torch.from_numpy(a).cuda() for a in (uid, pid, nid)), N.opt(N.ORX_OPT_ADAGRAD, 0.05), out4)
-    ref = [a.astype(np.float64) for a in (user, item, bias)]
-    st = {k: (np.full_like(v, 0.1), None) for k, v in zip(("user", "item", "bias"), ref)}
-    loss, l2 = O.pairwise_train_step("bpr", *ref, uid, pid, nid, O.OPT_ADAGRAD, st, 1, 0.05)
-    np.testing.assert_allclose(out4[:2].cpu().numpy(), [loss, l2], rtol=3e-5, atol=1e-6)
-    for x, r in zip(t, ref):
-        np.testing.assert_allclose(x.cpu().numpy(), r, atol=1e-5)
+class _SmallPairwise:
+    """A BPR x Adagrad pairwise_step on tables of its own on `eng`, compared with the oracle.  prefetch() builds its
+    batch index ahead on the handle's side stream; step() then checks in the dispatch record that it consumed it."""
+
+    def __init__(self, eng, rng, B):
+        U, I, D = 50, 60, 64
+        self.eng, self.prefetched = eng, False
+        self.host = [rng.uniform(-0.05, 0.05, s).astype(np.float32) for s in ((U, D), (I, D), (I, 1))]
+        self.ids = [rng.integers(0, n, B).astype(np.int32) for n in (U, I, I)]
+        self.t = [torch.from_numpy(a).cuda() for a in self.host]
+        self.acc = [torch.full_like(x, 0.1) for x in self.t]
+        self.tabs = [N.table(x, s) for x, s in zip(self.t, self.acc)]
+        self.dids = [torch.from_numpy(a).cuda() for a in self.ids]
+
+    def prefetch(self):
+        self.eng.pairwise_prefetch(self.tabs[0], self.tabs[1], *self.dids, N.ORX_OPT_ADAGRAD)
+        self.prefetched = True
+
+    def step(self):
+        self.eng.debug_dispatch_log()
+        out4 = torch.zeros(4, device="cuda")
+        self.eng.pairwise_step(N.ORX_PAIR_BPR, *self.tabs, *self.dids, N.opt(N.ORX_OPT_ADAGRAD, 0.05), out4)
+        rec = self.eng.debug_dispatch_log()
+        assert len(rec) == 1 and (rec[0].s != 0) == self.prefetched, rec
+        ref = [a.astype(np.float64) for a in self.host]
+        st = {k: (np.full_like(v, 0.1), None) for k, v in zip(("user", "item", "bias"), ref)}
+        loss, l2 = O.pairwise_train_step("bpr", *ref, *self.ids, O.OPT_ADAGRAD, st, 1, 0.05)
+        np.testing.assert_allclose(out4[:2].cpu().numpy(), [loss, l2], rtol=3e-5, atol=1e-6)
+        for x, r in zip(self.t, ref):
+            np.testing.assert_allclose(x.cpu().numpy(), r, atol=1e-5)
 
 
-REFUSED = ["censor_grow", "prefetch", "epoch_wrap"]
-ACCEPTED = ["pairwise_step", "score_topk", "score_rank", "sample_pairwise"]
+def _censor(eng, rng, n):
+    """A censor of n ids on a table of its own on `eng` (it grows the handle's workspace to n lookups), compared with
+    the oracle."""
+    tab = rng.uniform(-1, 1, (5000, 64)).astype(np.float32)
+    ids = rng.integers(0, 5000, n).astype(np.int32)
+    t = torch.from_numpy(tab).cuda()
+    eng.censor(t, torch.from_numpy(ids).cuda())
+    ref = tab.astype(np.float64)
+    O.censor(ref, ids)
+    np.testing.assert_allclose(t.cpu().numpy(), ref, atol=1e-6)
 
 
-@pytest.mark.parametrize("call", REFUSED)
-def test_shared_handle_refuses_while_announced(call):
-    """While a rank's handle holds an announced batch's user index (built in the previous step's apply launch), calls
-    that would free, overwrite or empty its index sets are refused before any device work -- and the announced step
-    then matches the oracle."""
-    run = _shared_run()
-    try:
-        a = run.prep(run.uniform(256))
-        b = run.step(a, lambda: run.uniform(256), announce=True)
-        eng = run.g.ranks[0].eng
-        rng = np.random.default_rng(5)
-        if call == "censor_grow":
-            tab = torch.from_numpy(rng.uniform(-1, 1, (5000, 64)).astype(np.float32)).cuda()
-            keep = tab.clone()
-            ids = torch.from_numpy(rng.integers(0, 5000, _cap_B(run) + 100).astype(np.int32)).cuda()
-            with pytest.raises(RuntimeError, match=r"status -1\).*workspace growth"):
-                eng.censor(tab, ids)
-            assert torch.equal(tab, keep)
-        elif call == "prefetch":
-            t = [torch.zeros(50, 64, device="cuda"), torch.zeros(60, 64, device="cuda")]
-            ids = [torch.zeros(64, dtype=torch.int32, device="cuda") for _ in range(3)]
-            with pytest.raises(RuntimeError, match=r"status -1\).*announced batch"):
-                eng.pairwise_prefetch(N.table(t[0]), N.table(t[1]), *ids, N.ORX_OPT_ADAGRAD)
-            _small_pairwise(eng, rng, 64)            # a pairwise_step of its own is still accepted
-        else:
-            eng.debug_set_epoch(0x7fffffff)         # the next epoch take wraps
-            with pytest.raises(RuntimeError, match=r"status -1\).*wrap"):
-                _small_pairwise(eng, rng, 64)
-        run.step(b, lambda: run.uniform(256))       # the announced step, then a plain one (wraps in "epoch_wrap")
-        run.step(run.prep(run.uniform(256)))
-    finally:
-        run.close()
+ACCEPTED = ["pairwise_step", "score_topk", "score_rank", "sample_pairwise", "censor_grow", "prefetch", "epoch_wrap",
+            "prefetch_across_step"]
 
 
 @pytest.mark.parametrize("call", ACCEPTED)
 def test_shared_handle_accepts_while_announced(call):
-    """Calls that leave the announced index alone are accepted between the two steps, match their own reference, and
-    leave the announced step matching the oracle."""
+    """Calls on a rank's handle between an announced step and its successor -- a workspace growth, a pairwise prefetch
+    consumed by its step, a wrap of the handle's index epoch included -- match their own reference, and the announced
+    step and a plain one after it match the oracle.  prefetch_across_step: the announced step runs while a pairwise
+    prefetch is outstanding, and the pairwise step consumes it after."""
     run = _shared_run()
     try:
         a = run.prep(run.uniform(256))
         b = run.step(a, lambda: run.uniform(256), announce=True)
         eng = run.g.ranks[0].eng
         rng = np.random.default_rng(6)
+        after = None
         if call == "pairwise_step":
-            _small_pairwise(eng, rng, 200)
+            _SmallPairwise(eng, rng, 200).step()
+        elif call == "censor_grow":
+            _censor(eng, rng, _cap_B(run) + 100)
+        elif call in ("prefetch", "prefetch_across_step"):
+            sp = _SmallPairwise(eng, rng, 64)
+            sp.prefetch()
+            if call == "prefetch":
+                sp.step()
+            else:
+                after = sp
+        elif call == "epoch_wrap":
+            # the small step wraps the handle's epoch; then the announced step wraps its item set, the plain one a user set
+            eng.debug_set_epoch(0x7fffffff)
+            _SmallPairwise(eng, rng, 64).step()
         elif call in ("score_topk", "score_rank"):
             # same call on a fresh handle: bit-identical (the evaluation suites hold it to the oracle)
             Uq, I, D = 40, 300, 64
@@ -566,27 +574,22 @@ def test_shared_handle_accepts_while_announced(call):
                                                 *(C.c_void_p(t.data_ptr()) for t in out), eng.stream()))
             for g, w in zip(out, S.sample_pairwise(st.sd, 99, 12345, 500)):
                 assert np.array_equal(g.cpu().numpy(), w)
-        run.step(b, lambda: run.uniform(256))
+        c = run.step(b, lambda: run.uniform(256))
+        if after is not None:
+            after.step()
+        run.step(c)
     finally:
         run.close()
 
 
 def test_shared_handle_grows_after_plain_step():
-    """With nothing announced, a workspace-growing call between two steps is accepted, and the next step rebuilds its
-    index sets in the new workspace."""
+    """With nothing announced, a workspace-growing call between two steps is accepted, and the steps after it match
+    the oracle."""
     run = _shared_run()
     try:
         run.step(run.prep(run.uniform(256)))
         eng = run.g.ranks[0].eng
-        rng = np.random.default_rng(7)
-        D = 64
-        tab = rng.uniform(-1, 1, (5000, D)).astype(np.float32)
-        ids = rng.integers(0, 5000, _cap_B(run) + 100).astype(np.int32)
-        t = torch.from_numpy(tab).cuda()
-        eng.censor(t, torch.from_numpy(ids).cuda())
-        ref = tab.astype(np.float64)
-        O.censor(ref, ids)
-        np.testing.assert_allclose(t.cpu().numpy(), ref, atol=1e-6)
+        _censor(eng, np.random.default_rng(7), _cap_B(run) + 100)
         run.step(run.prep(run.uniform(256)), lambda: run.uniform(256))
         run.step(run.prep(run.uniform(256)))
     finally:
