@@ -15,6 +15,10 @@
  *    id staging, evaluation scratch, sharded-step scratch, split-K partials), keeps no device
  *    state outside it, and orx_destroy frees all of it.  Two handles share nothing;
  *  - all calls are asynchronous w.r.t. the host and ordered on the given stream;
+ *  - the calls of one handle that build or use its own batch index (the pairwise and pointwise steps, orx_sparse_apply*,
+ *    orx_censor; not orx_pairwise_prefetch's side-stream build) share its index set 0 and staging rows, so they must be
+ *    ordered among themselves: one stream, or streams the caller orders with events.  A table's epoch wrap then empties
+ *    it on that stream, behind every launch that used it;
  *  - return value: ORX_OK (0) or a negative orx_status; orx_last_error_string() gives the
  *    thread-local message.  There is no CPU fallback: without a CUDA device every compute
  *    entry point fails with ORX_ERR_CUDA.
@@ -79,8 +83,9 @@ ORX_API int orx_destroy(orx_handle_t h);
 ORX_API int orx_device_count(int* n_out_host);
 /* Blocks the host until `stream` has drained (cudaStreamSynchronize). */
 ORX_API int orx_stream_synchronize(orx_handle_t h, orx_stream_t stream);
-/* Test hook: place the handle's batch-index epoch counter, and those of the index sets of orx_shard_step once it has
- * run (31 bits; the wrap path empties the hash tables). */
+/* Test hook: place the epoch of every batch-index table of the handle (index sets 0, 1 and 2) and, once it has run, of
+ * orx_shard_step's own index sets (31 bits; each table takes its next epoch at its next build, and the one whose epoch
+ * wraps is emptied on the stream of that build). */
 ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
 /* Test hook: the kernel variants launched by this handle's DLRM entry points (orx_mlp_layer_*, orx_interact_*) and
  * sparse steps (orx_pairwise_step, orx_pairwise_step_host, orx_pointwise_step) since the last call, oldest first, at

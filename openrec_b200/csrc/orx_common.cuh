@@ -51,18 +51,53 @@ struct OrxHash {
 // (>= 1024) that holds 4x the lookups.  did takes lookups + 1 entries.
 uint32_t orx_hash_shape(OrxHash& t, int64_t lookups);
 
+// 256-byte aligned bump allocation inside one buffer.  With a null base it only counts bytes (off = the size so far).
+struct OrxCarve {
+  char* base;
+  size_t off;
+  void* take(size_t bytes) {
+    char* p = base ? base + off : nullptr;
+    off += (bytes + 255) & ~(size_t)255;
+    return p;
+  }
+};
+
+// slots | didx | did of a table for `lookups` ids (orx_hash_shape); counter and epoch are the caller's
+void orx_hash_carve(OrxCarve& m, OrxHash& t, int64_t lookups);
+
+// Start the next epoch of table t (31 bits, skipping 0), for an index build into t on `st`.  On the wrap only t's slots
+// are emptied, on `st`: every launch that writes or probes t runs on `st` or is ordered before this point, so no stale
+// slot can alias the epochs to come (about 65 h of back-to-back steps between wraps).
+int orx_take_epoch(OrxHash& t, cudaStream_t st);
+
+// One batch index set of the handle: user / item tables, the control words of the steps that use it and, for the
+// prefetch sets 1 and 2 (pairwise batches indexed ahead on the side stream, orx_pairwise.cu), their records, events
+// and what the outstanding prefetch was built for.
+struct OrxIndexSet {
+  OrxHash u, i;
+  int32_t* ctl;   // [4] staged_u (u.counter), staged_i (i.counter), tail block ticket, bad ids: TailArgs::counters
+  int4* res;      // sets 1, 2 with ORX_PAIR_RESOLVE: per-triplet records {flags, du, dp, dn} (k_index_resolve)
+  cudaEvent_t done, free;   // index built / handed back by the step that consumed it
+  int free_valid;
+  const int32_t *uid, *pid, *nid;
+  int B, mode;
+  int64_t rows_u, rows_i;
+};
+
 struct orx_ctx {
   int device;
   int num_sms;
-  // index workspace (sized for cap_B lookups per table side)
-  int64_t cap_B;  // largest batch the workspace is sized for
-  OrxHash hu, hi;      // index set 0: everything that builds its index on the caller's stream
-  OrxHash pf_u[2], pf_i[2];  // index sets 1, 2: pairwise batches indexed ahead on the side stream (orx_pairwise.cu)
-  int32_t* counters;  // [16]: per index set k at 4k: staged_u, staged_i, ticket, bad ids; 12.. spare
+  // index workspace, one allocation (sized for cap_B lookups per table side, staging rows of g_dim floats): set 0 for
+  // everything that builds its index on the caller's stream, sets 1 and 2 for prefetched pairwise batches, then the
   // staged-row gradient buffers
-  float *gu, *gi, *gb, *gw;
-  int64_t g_rows_u, g_rows_i;
+  int64_t cap_B;  // largest batch the workspace is sized for
   int32_t g_dim;
+  void* index_ws;
+  size_t index_cap;
+  OrxIndexSet set[3];
+  int pf_set;     // the outstanding prefetched set (1 or 2), 0 = none
+  int pf_next;    // the next prefetch builds into set 1 + pf_next
+  float *gu, *gi, *gb, *gw;
   // loss partials: (loss, l2) float pairs
   float* partials;
   size_t partials_cap;   // bytes
@@ -78,16 +113,10 @@ struct orx_ctx {
   int32_t* bucket_cursor;  // [1024] owner-bucket scratch
   cudaStream_t side_stream;  // id upload + index build of the NEXT pairwise batch, beside the running step
   cudaEvent_t side_ev;       // "ids are final" point of orx_pairwise_prefetch on the caller's ids stream
-  cudaEvent_t pf_done[2], pf_free[2], stage_free[2];   // prefetched index k built / handed back; id staging f free
-  int pf_free_valid[2], stage_free_valid[2];
-  int pf_valid, pf_set, pf_next, pf_B, pf_mode;        // the one outstanding prefetched index and what it was built for
-  const int32_t *pf_uid, *pf_pid, *pf_nid;
-  int64_t pf_rows_u, pf_rows_i;
-  int4* pf_res[2];         // per-triplet records {flags, du, dp, dn} of prefetched set k (k_index_resolve, orx_pairwise.cu)
-  size_t pf_res_cap[2];    // bytes
+  cudaEvent_t stage_free[2];   // id staging f free
+  int stage_free_valid[2];
   int pair_resolve;        // ORX_PAIR_RESOLVE, read at orx_create: 0 = no records, a prefetched step probes the index
-  uint32_t epoch;          // hash epoch of the last step, in [1, 2^31)
-  void* shard_ws;          // orx_shard.cu: host bookkeeping of the row-sharded step (orx_shard_ws*)
+  void* shard_ws;         // orx_shard.cu: host bookkeeping of the row-sharded step (orx_shard_ws*)
   void* shard_scratch;     // orx_shard.cu: its local device scratch, carved by sh_layout
   size_t shard_cap;
   int32_t dispatch[ORX_DISPATCH_LOG_CAP][8];   // orx_debug_dispatch_log: ring of the last DLRM / sparse-step launches
@@ -110,10 +139,6 @@ static inline void orx_log_dispatch(orx_ctx* c, int op, int variant, int TA, int
   r[0] = op; r[1] = variant; r[2] = TA; r[3] = TB; r[4] = M; r[5] = N; r[6] = K; r[7] = S;
 }
 
-// Start a new hash epoch (once per step, before the index build; `st` = the stream the step runs on).
-// A slot word holds 31 epoch bits: epochs live in [1, 2^31) and on wrap every table is zeroed on `st`, so a stale
-// slot can never alias the current epoch (about 65 h of back-to-back steps between wraps).
-int orx_next_epoch(orx_ctx* c, cudaStream_t st);
 void orx_shard_ws_release(orx_ctx* c);
 // orx_debug_set_epoch: place the epoch counters of the row-sharded step's own index sets too, once they exist
 void orx_shard_set_epoch(orx_ctx* c, uint32_t epoch);
@@ -576,11 +601,11 @@ __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni)
 OrxOptDev orx_opt_to_dev(const orx_opt_t* o);
 int orx_launch_index_build_strided(orx_ctx* c, const int32_t* a, int64_t stride, int64_t rows, int32_t n,
                                    bool stage_all, cudaStream_t st);
-// The shared arguments of a step over user / item / bias (item and bias may be null) with index sets hu / hi, the
-// handle's staging rows and optimizer o.  A derived block takes them as its first initializer: TailArgs ta = {s};
-// zeroes every other field.
+// The shared arguments of a step over user / item / bias (item and bias may be null) with index set ix, the handle's
+// staging rows and optimizer o.  A derived block takes them as its first initializer: TailArgs ta = {s}; zeroes every
+// other field.
 SparseArgs orx_sparse_args(const orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
-                           const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o);
+                           const OrxIndexSet& ix, const OrxOptDev& o);
 // The tables of a pairwise or pointwise step, fused or not: user, item and item bias present, user / item dims that
 // agree, int32 row ids, and the slot rows optimizer opt_kind keeps -- also on w, GMF's dense weight, when it is given.
 int orx_check_step_tables(const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
@@ -609,9 +634,9 @@ int orx_sparse_step(orx_ctx* c, int op, int kind, const orx_table_t* user, const
 int orx_sparse_unfused(orx_ctx* c, int B, float loss_scale, float* out4,
                        const std::function<void(float* partials, int blocks)>& launch, cudaStream_t st);
 // ADAM_DENSE: Keras dense Adam over every row of user / item / bias (item and bias may be null), a row's summed gradient
-// taken from its side's index set (hu / hi) and staging rows.  Runs before the tail, which zeroes the staging rows.
+// taken from its side's table of index set ix and staging rows.  Runs before the tail, which zeroes the staging rows.
 int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
-                           const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o, cudaStream_t st);
+                           const OrxIndexSet& ix, const OrxOptDev& o, cudaStream_t st);
 int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st);
 int orx_launch_reduce_partials(const float* partials, int n, float loss_scale, float* out4, cudaStream_t st);
 // index of n samples (a[t], b0[t]) or (a[t], b0[t], b1[t]); only samples whose ids are all in range are inserted

@@ -33,31 +33,6 @@ extern "C" int orx_device_count(int* n) {
   return ORX_OK;
 }
 
-static void free_hash(OrxHash& t) {
-  cudaFree(t.slots);
-  cudaFree(t.didx);
-  cudaFree(t.did);
-  t.slots = nullptr;
-  t.didx = nullptr;
-  t.did = nullptr;
-}
-
-static void free_workspace(orx_ctx* c) {
-  free_hash(c->hu);
-  free_hash(c->hi);
-  for (int k = 0; k < 2; ++k) {
-    free_hash(c->pf_u[k]);
-    free_hash(c->pf_i[k]);
-  }
-  cudaFree(c->gu);
-  cudaFree(c->gi);
-  cudaFree(c->gb);
-  cudaFree(c->gw);
-  c->gu = c->gi = c->gb = c->gw = nullptr;
-  c->cap_B = 0;
-  c->g_dim = 0;
-}
-
 uint32_t orx_hash_shape(OrxHash& t, int64_t lookups) {
   // load factor <= 0.25: with linear probing the slowest of a warp's 32 inserts/probes sets the pace
   // (profile r1b: ~7 serialized L2 round trips per warp at 0.5)
@@ -70,82 +45,73 @@ uint32_t orx_hash_shape(OrxHash& t, int64_t lookups) {
   return cap;
 }
 
-static int alloc_hash(OrxHash& t, int64_t lookups, int32_t* counter) {
+void orx_hash_carve(OrxCarve& m, OrxHash& t, int64_t lookups) {
   const uint32_t cap = orx_hash_shape(t, lookups);
-  t.counter = counter;
-  ORX_CUDA(cudaMalloc(&t.slots, sizeof(unsigned long long) * cap));
-  ORX_CUDA(cudaMalloc(&t.didx, sizeof(int32_t) * cap));
-  ORX_CUDA(cudaMalloc(&t.did, sizeof(int32_t) * (lookups + 1)));
-  ORX_CUDA(cudaMemset(t.slots, 0, sizeof(unsigned long long) * cap));
-  return ORX_OK;
+  t.slots = (unsigned long long*)m.take(sizeof(unsigned long long) * cap);
+  t.didx = (int32_t*)m.take(sizeof(int32_t) * cap);
+  t.did = (int32_t*)m.take(sizeof(int32_t) * (size_t)(lookups + 1));
 }
 
-// Workspace is sized for B lookups on the user side and 2B on the item side; every lookup may be
-// staged (ADAM_DENSE stages all rows), so the staging buffers hold B resp. 2B rows of `dim` floats.
+// The index workspace for nb lookups on the user side and 2 nb on the item side: the control words of the three index
+// sets side by side, their tables and the records of sets 1 and 2, then the staging rows gu | gi | gb | gw.  Every
+// lookup may be staged (ADAM_DENSE stages all rows), so the staging rows hold nb resp. 2 nb rows of nd floats.  With
+// base == nullptr only the size is computed, and every pointer is left null.
+static size_t index_ws_layout(char* base, int64_t nb, int32_t nd, orx_ctx* c) {
+  OrxCarve m = {base, 0};
+  int32_t* ctl = (int32_t*)m.take(sizeof(int32_t) * 4 * 3);
+  for (int k = 0; k < 3; ++k) {
+    OrxIndexSet& s = c->set[k];
+    s.ctl = base ? ctl + 4 * k : nullptr;
+    s.u.counter = s.ctl;
+    s.i.counter = base ? s.ctl + 1 : nullptr;
+    orx_hash_carve(m, s.u, nb);
+    orx_hash_carve(m, s.i, 2 * nb);
+    s.res = k > 0 && c->pair_resolve ? (int4*)m.take(sizeof(int4) * (size_t)nb) : nullptr;
+  }
+  c->gu = (float*)m.take(sizeof(float) * (size_t)nb * nd);
+  c->gi = (float*)m.take(sizeof(float) * 2 * (size_t)nb * nd);
+  c->gb = (float*)m.take(sizeof(float) * 2 * (size_t)nb);
+  c->gw = (float*)m.take(sizeof(float) * (size_t)nd);
+  return m.off;
+}
+
 int orx_ensure_workspace(orx_ctx* c, int64_t B, int32_t dim) {
   if (B <= c->cap_B && dim <= c->g_dim) return ORX_OK;
-  int64_t nb = B > c->cap_B ? B : c->cap_B;
-  int32_t nd = dim > c->g_dim ? dim : c->g_dim;
+  const int64_t nb = B > c->cap_B ? B : c->cap_B;
+  const int32_t nd = dim > c->g_dim ? dim : c->g_dim;
+  ORX_CUDA(cudaDeviceSynchronize());   // the old layout may be in use on any stream
+  // until the new layout is in place: no set points into the old buffer, and a failed allocation is retried next call
+  c->cap_B = 0;
+  c->g_dim = 0;
+  const size_t bytes = index_ws_layout(nullptr, nb, nd, c);
+  int rc = orx_grow(&c->index_ws, &c->index_cap, bytes);
+  if (rc) return rc;
+  index_ws_layout(static_cast<char*>(c->index_ws), nb, nd, c);
+  ORX_CUDA(cudaMemset(c->index_ws, 0, bytes));
+  // the memset ran on the legacy default stream; the caller's stream may be a non-blocking one
   ORX_CUDA(cudaDeviceSynchronize());
-  free_workspace(c);
-  int rc;
-  if ((rc = alloc_hash(c->hu, nb, c->counters + 0)) != ORX_OK) return rc;
-  if ((rc = alloc_hash(c->hi, 2 * nb, c->counters + 1)) != ORX_OK) return rc;
-  for (int k = 0; k < 2; ++k) {
-    if ((rc = alloc_hash(c->pf_u[k], nb, c->counters + 4 * (1 + k))) != ORX_OK) return rc;
-    if ((rc = alloc_hash(c->pf_i[k], 2 * nb, c->counters + 4 * (1 + k) + 1)) != ORX_OK) return rc;
+  for (OrxIndexSet& s : c->set) {
+    s.u.epoch = s.i.epoch = 0;  // fresh (zeroed) tables: epochs restart at 1
+    s.free_valid = 0;
   }
-  c->pf_valid = 0;
-  c->pf_free_valid[0] = c->pf_free_valid[1] = 0;
-  for (int k = 0; k < 2 && c->pair_resolve; ++k)
-    if ((rc = orx_grow((void**)&c->pf_res[k], &c->pf_res_cap[k], sizeof(int4) * (size_t)nb)) != ORX_OK) return rc;
-  c->g_rows_u = nb;
-  c->g_rows_i = 2 * nb;
-  size_t bu = sizeof(float) * (size_t)c->g_rows_u * nd, bi = sizeof(float) * (size_t)c->g_rows_i * nd;
-  ORX_CUDA(cudaMalloc(&c->gu, bu));
-  ORX_CUDA(cudaMalloc(&c->gi, bi));
-  ORX_CUDA(cudaMalloc(&c->gb, sizeof(float) * (size_t)c->g_rows_i));
-  ORX_CUDA(cudaMalloc(&c->gw, sizeof(float) * (size_t)nd));
-  ORX_CUDA(cudaMemset(c->gu, 0, bu));
-  ORX_CUDA(cudaMemset(c->gi, 0, bi));
-  ORX_CUDA(cudaMemset(c->gb, 0, sizeof(float) * (size_t)c->g_rows_i));
-  ORX_CUDA(cudaMemset(c->gw, 0, sizeof(float) * (size_t)nd));
-  ORX_CUDA(cudaMemset(c->counters, 0, sizeof(int32_t) * 16));
-  // the memsets above ran on the legacy default stream; the caller's stream may be a non-blocking one
-  ORX_CUDA(cudaDeviceSynchronize());
+  c->pf_set = 0;
   c->cap_B = nb;
   c->g_dim = nd;
-  c->epoch = 0;  // fresh (zeroed) tables: epochs restart at 1
   return ORX_OK;
 }
 
-static int zero_hash(OrxHash& t) {
-  if (!t.slots) return ORX_OK;
-  ORX_CUDA(cudaMemset(t.slots, 0, sizeof(unsigned long long) * ((size_t)t.mask + 1)));
+int orx_take_epoch(OrxHash& t, cudaStream_t st) {
+  const uint32_t e = (t.epoch + 1) & 0x7fffffffu;
+  if (e == 0) ORX_CUDA(cudaMemsetAsync(t.slots, 0, sizeof(unsigned long long) * ((size_t)t.mask + 1), st));
+  t.epoch = e ? e : 1;
   return ORX_OK;
 }
 
-int orx_next_epoch(orx_ctx* c, cudaStream_t /*st*/) {
-  c->epoch = (c->epoch + 1) & 0x7fffffffu;
-  if (c->epoch == 0) {
-    // 31-bit wrap (once per 2^31 index builds): a stale slot could alias the epochs to come, so every table is emptied.
-    // Index builds may be in flight on two streams: drain the device around the memsets.
-    ORX_CUDA(cudaDeviceSynchronize());
-    int rc;
-    if ((rc = zero_hash(c->hu)) || (rc = zero_hash(c->hi))) return rc;
-    for (int k = 0; k < 2; ++k)
-      if ((rc = zero_hash(c->pf_u[k])) || (rc = zero_hash(c->pf_i[k]))) return rc;
-    ORX_CUDA(cudaDeviceSynchronize());
-    c->epoch = 1;
-  }
-  c->hu.epoch = c->hi.epoch = c->epoch;
-  return ORX_OK;
-}
-
-// test hook: place the epoch counters (tests/test_gpu_kernels.py::test_epoch_wrap starts them just below 2^31)
+// test hook: place the epoch of every index table, the handle's and the sharded step's (the wrap tests start them just
+// below 2^31)
 extern "C" int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch) {
   ORX_REQUIRE(h != nullptr && epoch < 0x80000000u, "null handle / epoch must be < 2^31");
-  h->epoch = epoch;
+  for (OrxIndexSet& s : h->set) s.u.epoch = s.i.epoch = epoch;
   orx_shard_set_epoch(h, epoch);
   return ORX_OK;
 }
@@ -201,8 +167,7 @@ extern "C" int orx_create(int device, orx_handle_t* out) {
   c->partials_cap = sizeof(float) * 2 * (size_t)c->num_sms * 64;
   const char* pr = getenv("ORX_PAIR_RESOLVE");   // 0: prefetched pairwise steps probe the index (A/B measurements)
   c->pair_resolve = (pr && atoi(pr) == 0) ? 0 : 1;
-  if (cudaMalloc(&c->counters, sizeof(int32_t) * 16) != cudaSuccess ||
-      cudaMalloc(&c->bucket_cursor, sizeof(int32_t) * 1024) != cudaSuccess ||
+  if (cudaMalloc(&c->bucket_cursor, sizeof(int32_t) * 1024) != cudaSuccess ||
       cudaMalloc(&c->partials, c->partials_cap) != cudaSuccess ||
       cudaMalloc(&c->out_stage[0], sizeof(float) * 8) != cudaSuccess ||
       cudaMalloc(&c->out_stage[1], sizeof(float) * 8) != cudaSuccess) {
@@ -210,7 +175,6 @@ extern "C" int orx_create(int device, orx_handle_t* out) {
     orx_destroy(c);
     return ORX_ERR_NOMEM;
   }
-  cudaMemset(c->counters, 0, sizeof(int32_t) * 16);
   *out = c;
   return ORX_OK;
 }
@@ -219,13 +183,11 @@ extern "C" int orx_destroy(orx_handle_t h) {
   if (!h) return ORX_OK;
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();
-  free_workspace(h);
+  cudaFree(h->index_ws);
   for (int i = 0; i < 2; ++i) {
     cudaFree(h->ids_stage[i]);
     cudaFree(h->out_stage[i]);
-    cudaFree(h->pf_res[i]);
   }
-  cudaFree(h->counters);
   cudaFree(h->partials);
   cudaFree(h->bucket_cursor);
   cudaFree(h->eval_ws);
@@ -236,8 +198,8 @@ extern "C" int orx_destroy(orx_handle_t h) {
     cudaStreamDestroy(h->side_stream);
     cudaEventDestroy(h->side_ev);
     for (int i = 0; i < 2; ++i) {
-      cudaEventDestroy(h->pf_done[i]);
-      cudaEventDestroy(h->pf_free[i]);
+      cudaEventDestroy(h->set[1 + i].done);
+      cudaEventDestroy(h->set[1 + i].free);
       cudaEventDestroy(h->stage_free[i]);
     }
   }

@@ -893,27 +893,20 @@ __global__ void __launch_bounds__(EV_NT) k_topk_merge(const TopkWs w, int splits
   }
 }
 
-size_t ev_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
 // The call's scratch inside one allocation; with base == nullptr only the size is computed.
 size_t ev_layout(char* base, int Bu, int P, size_t sort_bytes, EvalWs* w) {
   const size_t nk = (size_t)2 * Bu * P;
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    char* p = base ? base + off : nullptr;
-    off += ev_align(bytes);
-    return p;
-  };
-  w->keys_in = reinterpret_cast<float*>(take(sizeof(float) * nk));
-  w->keys = reinterpret_cast<float*>(take(sizeof(float) * nk));
-  w->seg_begin = reinterpret_cast<int*>(take(sizeof(int) * 2 * (size_t)Bu));
-  w->seg_end = reinterpret_cast<int*>(take(sizeof(int) * 2 * (size_t)Bu));
-  w->hist = reinterpret_cast<unsigned*>(take(sizeof(unsigned) * (size_t)Bu * P));
-  w->auc_cnt = reinterpret_cast<unsigned long long*>(take(sizeof(unsigned long long) * (size_t)Bu));
-  w->info = reinterpret_cast<int*>(take(sizeof(int) * 2 * (size_t)Bu));
-  w->sort_tmp = take(sort_bytes);
+  OrxCarve m = {base, 0};
+  w->keys_in = reinterpret_cast<float*>(m.take(sizeof(float) * nk));
+  w->keys = reinterpret_cast<float*>(m.take(sizeof(float) * nk));
+  w->seg_begin = reinterpret_cast<int*>(m.take(sizeof(int) * 2 * (size_t)Bu));
+  w->seg_end = reinterpret_cast<int*>(m.take(sizeof(int) * 2 * (size_t)Bu));
+  w->hist = reinterpret_cast<unsigned*>(m.take(sizeof(unsigned) * (size_t)Bu * P));
+  w->auc_cnt = reinterpret_cast<unsigned long long*>(m.take(sizeof(unsigned long long) * (size_t)Bu));
+  w->info = reinterpret_cast<int*>(m.take(sizeof(int) * 2 * (size_t)Bu));
+  w->sort_tmp = m.take(sort_bytes);
   w->sort_bytes = sort_bytes;
-  return off;
+  return m.off;
 }
 
 // Item splits of a grid of user tiles x item splits for kern at dyn bytes of dynamic shared memory: enough CTAs for one
@@ -1025,10 +1018,10 @@ int ev_shard_phase(orx_ctx* h, int phase, const EvalRowArgs& a, const EvalOut& o
 // The top-K scratch of Bu rows over `splits` item splits inside one allocation; with base == nullptr only the size.
 size_t tk_layout(char* base, int Bu, int64_t splits, int k, TopkWs* w) {
   const size_t lists = (size_t)Bu * (size_t)splits;
-  const size_t cand = ev_align(sizeof(unsigned long long) * lists * ((size_t)k + TK_ROOM));
-  w->cand = reinterpret_cast<unsigned long long*>(base);
-  w->cnt = base ? reinterpret_cast<int*>(base + cand) : nullptr;
-  return cand + ev_align(sizeof(int) * lists);
+  OrxCarve m = {base, 0};
+  w->cand = reinterpret_cast<unsigned long long*>(m.take(sizeof(unsigned long long) * lists * ((size_t)k + TK_ROOM)));
+  w->cnt = reinterpret_cast<int*>(m.take(sizeof(int) * lists));
+  return m.off;
 }
 
 template <int KIND>

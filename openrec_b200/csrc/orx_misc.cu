@@ -140,10 +140,11 @@ extern "C" int orx_censor(orx_handle_t h, float* tab, int64_t rows, int32_t dim,
   cudaStream_t st = (cudaStream_t)s;
   int rc = orx_ensure_workspace(h, n, h->g_dim > 0 ? h->g_dim : 1);
   if (rc) return rc;
-  if ((rc = orx_next_epoch(h, st))) return rc;   // the dedup hash needs no clearing: a new epoch empties it
+  OrxIndexSet& ix = h->set[0];
+  if ((rc = orx_take_epoch(ix.u, st))) return rc;   // the dedup hash needs no clearing: a new epoch empties it
   int blocks = (n + 63) / 64;                 // 8 warps x 8 ids per block and iteration
   if (blocks > h->num_sms * 8) blocks = h->num_sms * 8;
-  k_censor<<<blocks, 256, 0, st>>>(tab, rows, dim, ids, n, min_norm, h->hu);
+  k_censor<<<blocks, 256, 0, st>>>(tab, rows, dim, ids, n, min_norm, ix.u);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }

@@ -89,9 +89,10 @@ __global__ void k_index_build_strided(OrxHash hu, const int32_t* __restrict__ a,
 int orx_launch_index_build_strided(orx_ctx* c, const int32_t* a, int64_t stride, int64_t rows, int32_t n,
                                    bool stage_all, cudaStream_t st) {
   if (n <= 0) return ORX_OK;
-  int rc = orx_next_epoch(c, st);
+  OrxIndexSet& s = c->set[0];
+  int rc = orx_take_epoch(s.u, st);
   if (rc) return rc;
-  k_index_build_strided<<<(n + 255) / 256, 256, 0, st>>>(c->hu, a, stride, rows, n, stage_all ? 1 : 0, c->counters + 3);
+  k_index_build_strided<<<(n + 255) / 256, 256, 0, st>>>(s.u, a, stride, rows, n, stage_all ? 1 : 0, s.ctl + 3);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
@@ -100,9 +101,10 @@ int orx_launch_index_build(orx_ctx* c, const int32_t* a, int64_t rows_a, const i
                            int64_t rows_b, int32_t n, int mode, cudaStream_t st) {
   const int total = (b1 ? 3 : 2) * n;
   if (total <= 0) return ORX_OK;
-  int rc = orx_next_epoch(c, st);
-  if (rc) return rc;
-  k_index_build<<<(total + 255) / 256, 256, 0, st>>>(c->hu, c->hi, a, rows_a, b0, b1, rows_b, n, mode, c->counters + 3);
+  OrxIndexSet& s = c->set[0];
+  int rc;
+  if ((rc = orx_take_epoch(s.u, st)) || (rc = orx_take_epoch(s.i, st))) return rc;
+  k_index_build<<<(total + 255) / 256, 256, 0, st>>>(s.u, s.i, a, rows_a, b0, b1, rows_b, n, mode, s.ctl + 3);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
@@ -507,9 +509,9 @@ int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t s
 }
 
 int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
-                           const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o, cudaStream_t st) {
+                           const OrxIndexSet& ix, const OrxOptDev& o, cudaStream_t st) {
   struct { const orx_table_t* t; int D; const OrxHash* h; const float* g; } sw[3] = {
-      {user, user->dim, &hu, c->gu}, {item, user->dim, &hi, c->gi}, {bias, 1, &hi, c->gb}};
+      {user, user->dim, &ix.u, c->gu}, {item, user->dim, &ix.i, c->gi}, {bias, 1, &ix.i, c->gb}};
   for (const auto& s : sw) {
     if (!s.t) continue;
     int64_t blocks = (s.t->rows + 7) / 8;
@@ -523,12 +525,12 @@ int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_
 }
 
 SparseArgs orx_sparse_args(const orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
-                           const OrxHash& hu, const OrxHash& hi, const OrxOptDev& o) {
+                           const OrxIndexSet& ix, const OrxOptDev& o) {
   SparseArgs s = {};
   s.U = user->var; s.Us0 = user->s0; s.Us1 = user->s1;
   if (item) { s.I = item->var; s.Is0 = item->s0; s.Is1 = item->s1; }
   if (bias) { s.Bv = bias->var; s.Bs0 = bias->s0; s.Bs1 = bias->s1; }
-  s.D = user->dim; s.opt = o; s.hu = hu; s.hi = hi;
+  s.D = user->dim; s.opt = o; s.hu = ix.u; s.hi = ix.i;
   s.gu = c->gu; s.gi = c->gi; s.gb = c->gb;
   return s;
 }
@@ -580,32 +582,34 @@ static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, OrxSte
 
 // ---- pipelined batch index ------------------------------------------------------------------------------------------
 // The index of a batch depends only on its ids, so it can be built while the PREVIOUS step's kernels still run: on the
-// context's side stream, into one of two "prefetch" index sets (hash tables + counters) that alternate -- set 0 stays
-// with everything that builds its index on the caller's stream (pointwise / DLRM / censor / un-prefetched pairwise
-// steps; the row-sharded step keeps index sets of its own, orx_shard.cu).  The step that consumes a prefetched index
-// waits for it with an event; the set is handed back with an event recorded behind that step's tail.
+// context's side stream, into one of the handle's two prefetch index sets (1 and 2, alternating) -- set 0 stays with
+// everything that builds its index on the caller's stream (pointwise / censor / sparse apply / un-prefetched pairwise
+// steps; the row-sharded step keeps index sets of its own, orx_shard.cu).  The step that consumes a prefetched set waits
+// for its `done` event; the set is handed back with its `free` event, recorded behind that step's tail.  A set's epoch
+// is taken on the side stream after that wait, so a wrap empties its tables behind every step that used them.
 static int side_stream_ensure(orx_ctx* c) {
   if (c->side_stream) return ORX_OK;
   ORX_CUDA(cudaStreamCreateWithFlags(&c->side_stream, cudaStreamNonBlocking));
   ORX_CUDA(cudaEventCreateWithFlags(&c->side_ev, cudaEventDisableTiming));
   for (int i = 0; i < 2; ++i) {
-    ORX_CUDA(cudaEventCreateWithFlags(&c->pf_done[i], cudaEventDisableTiming));
-    ORX_CUDA(cudaEventCreateWithFlags(&c->pf_free[i], cudaEventDisableTiming));
+    OrxIndexSet& s = c->set[1 + i];
+    ORX_CUDA(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
+    ORX_CUDA(cudaEventCreateWithFlags(&s.free, cudaEventDisableTiming));
     ORX_CUDA(cudaEventCreateWithFlags(&c->stage_free[i], cudaEventDisableTiming));
-    c->pf_free_valid[i] = c->stage_free_valid[i] = 0;
+    s.free_valid = c->stage_free_valid[i] = 0;
   }
   return ORX_OK;
 }
 
-// a prefetched index nobody consumed: wait for it, reset its counters (the hash itself dies with its epoch)
+// a prefetched index nobody consumed: wait for it, reset its control words (the hash itself dies with its epoch)
 static int prefetch_drop(orx_ctx* c, cudaStream_t st) {
-  if (!c->pf_valid) return ORX_OK;
-  const int k = c->pf_set;
-  ORX_CUDA(cudaStreamWaitEvent(st, c->pf_done[k], 0));
-  ORX_CUDA(cudaMemsetAsync(c->counters + 4 * (1 + k), 0, sizeof(int32_t) * 4, st));
-  ORX_CUDA(cudaEventRecord(c->pf_free[k], st));
-  c->pf_free_valid[k] = 1;
-  c->pf_valid = 0;
+  if (!c->pf_set) return ORX_OK;
+  OrxIndexSet& s = c->set[c->pf_set];
+  ORX_CUDA(cudaStreamWaitEvent(st, s.done, 0));
+  ORX_CUDA(cudaMemsetAsync(s.ctl, 0, sizeof(int32_t) * 4, st));
+  ORX_CUDA(cudaEventRecord(s.free, st));
+  s.free_valid = 1;
+  c->pf_set = 0;
   return ORX_OK;
 }
 
@@ -613,24 +617,22 @@ static int prefetch_drop(orx_ctx* c, cudaStream_t st) {
 // (the caller's "ids are final" point); the ids themselves may also be produced on the side stream (host upload).
 static int prefetch_issue(orx_ctx* c, const int32_t* uid, const int32_t* pid, const int32_t* nid, int B, int64_t rows_u,
                           int64_t rows_i, int mode) {
-  const int k = c->pf_next;
+  const int k = 1 + c->pf_next;
   c->pf_next ^= 1;
+  OrxIndexSet& s = c->set[k];
   cudaStream_t ss = c->side_stream;
-  if (c->pf_free_valid[k]) ORX_CUDA(cudaStreamWaitEvent(ss, c->pf_free[k], 0));   // the step that last used set k is done
-  int rc = orx_next_epoch(c, ss);
-  if (rc) return rc;
-  c->pf_u[k].epoch = c->pf_i[k].epoch = c->epoch;
-  k_index_build<<<(3 * B + 255) / 256, 256, 0, ss>>>(c->pf_u[k], c->pf_i[k], uid, rows_u, pid, nid, rows_i, B, mode,
-                                                     c->counters + 4 * (1 + k) + 3);
+  if (s.free_valid) ORX_CUDA(cudaStreamWaitEvent(ss, s.free, 0));   // the step that last used set k is done
+  int rc;
+  if ((rc = orx_take_epoch(s.u, ss)) || (rc = orx_take_epoch(s.i, ss))) return rc;
+  k_index_build<<<(3 * B + 255) / 256, 256, 0, ss>>>(s.u, s.i, uid, rows_u, pid, nid, rows_i, B, mode, s.ctl + 3);
   ORX_LAUNCH_CHECK();
-  if (c->pair_resolve) {   // the probe answers too: the step then reads one record per triplet (pf_done follows them)
-    k_index_resolve<<<(B + 255) / 256, 256, 0, ss>>>(c->pf_u[k], c->pf_i[k], uid, pid, nid, rows_u, rows_i, B, mode,
-                                                      c->pf_res[k]);
+  if (s.res) {   // the probe answers too: the step then reads one record per triplet (done follows them)
+    k_index_resolve<<<(B + 255) / 256, 256, 0, ss>>>(s.u, s.i, uid, pid, nid, rows_u, rows_i, B, mode, s.res);
     ORX_LAUNCH_CHECK();
   }
-  ORX_CUDA(cudaEventRecord(c->pf_done[k], ss));
-  c->pf_valid = 1; c->pf_set = k; c->pf_uid = uid; c->pf_pid = pid; c->pf_nid = nid; c->pf_B = B;
-  c->pf_rows_u = rows_u; c->pf_rows_i = rows_i; c->pf_mode = mode;
+  ORX_CUDA(cudaEventRecord(s.done, ss));
+  c->pf_set = k;
+  s.uid = uid; s.pid = pid; s.nid = nid; s.B = B; s.rows_u = rows_u; s.rows_i = rows_i; s.mode = mode;
   return ORX_OK;
 }
 
@@ -656,11 +658,12 @@ extern "C" int orx_pairwise_prefetch(orx_handle_t h, const orx_table_t* user, co
 // set's prefetch is complete
 extern "C" int orx_debug_pair_records(orx_handle_t h, int32_t set, int32_t* rec, int32_t B, orx_stream_t s) {
   ORX_REQUIRE(h != nullptr && rec && (set == 1 || set == 2) && B > 0, "bad arguments");
-  ORX_REQUIRE(h->pair_resolve && h->side_stream && sizeof(int4) * (size_t)B <= h->pf_res_cap[set - 1],
+  const OrxIndexSet& x = h->set[set];
+  ORX_REQUIRE(x.res && h->side_stream && B <= h->cap_B,
               "no records of that many triplets (ORX_PAIR_RESOLVE=0, no prefetch yet, or B beyond the workspace)");
   ORX_CUDA(cudaSetDevice(h->device));
-  ORX_CUDA(cudaStreamWaitEvent((cudaStream_t)s, h->pf_done[set - 1], 0));
-  ORX_CUDA(cudaMemcpyAsync(rec, h->pf_res[set - 1], sizeof(int4) * (size_t)B, cudaMemcpyDeviceToDevice, (cudaStream_t)s));
+  ORX_CUDA(cudaStreamWaitEvent((cudaStream_t)s, x.done, 0));
+  ORX_CUDA(cudaMemcpyAsync(rec, x.res, sizeof(int4) * (size_t)B, cudaMemcpyDeviceToDevice, (cudaStream_t)s));
   return ORX_OK;
 }
 
@@ -680,35 +683,35 @@ int orx_sparse_step(orx_ctx* c, int op, int kind, const orx_table_t* user, const
     return rc;
   orx_prof_mark(c, 0, st);
   // index: a matching prefetched one (side stream, possibly still running), else built here on the caller's stream
+  const OrxIndexSet& pf = c->set[c->pf_set];
   int set = 0;
-  if (nid && c->pf_valid && c->pf_uid == uid && c->pf_pid == iid && c->pf_nid == nid && c->pf_B == B &&
-      c->pf_rows_u == user->rows && c->pf_rows_i == item->rows && c->pf_mode == (dense ? 1 : 0)) {
-    set = 1 + c->pf_set;
-    ORX_CUDA(cudaStreamWaitEvent(st, c->pf_done[c->pf_set], 0));
-    c->pf_valid = 0;
+  if (nid && c->pf_set && pf.uid == uid && pf.pid == iid && pf.nid == nid && pf.B == B && pf.rows_u == user->rows &&
+      pf.rows_i == item->rows && pf.mode == (dense ? 1 : 0)) {
+    set = c->pf_set;
+    ORX_CUDA(cudaStreamWaitEvent(st, pf.done, 0));
+    c->pf_set = 0;
   } else {
     if (nid && (rc = prefetch_drop(c, st))) return rc;
     if ((rc = orx_launch_index_build(c, uid, user->rows, iid, nid, item->rows, B, dense ? 1 : 0, st))) return rc;
   }
-  const OrxHash& HU = set ? c->pf_u[set - 1] : c->hu;
-  const OrxHash& HI = set ? c->pf_i[set - 1] : c->hi;
+  OrxIndexSet& ix = c->set[set];
   orx_prof_mark(c, 1, st);
-  const SparseArgs s = orx_sparse_args(c, user, item, bias, HU, HI, orx_opt_to_dev(opt));
+  const SparseArgs s = orx_sparse_args(c, user, item, bias, ix, orx_opt_to_dev(opt));
   OrxStepLaunch L = {};
-  if ((rc = kernel(s, set && c->pair_resolve ? c->pf_res[set - 1] : nullptr, c->partials, &L))) return rc;
+  if ((rc = kernel(s, ix.res, c->partials, &L))) return rc;   // set 0 has no records
   orx_log_dispatch(c, op, L.variant, kind, opt->kind, B, D, L.minb, set);
   orx_prof_mark(c, 2, st);
-  if (dense && (rc = orx_launch_adam_sweeps(c, user, item, bias, HU, HI, s.opt, st))) return rc;
+  if (dense && (rc = orx_launch_adam_sweeps(c, user, item, bias, ix, s.opt, st))) return rc;
   TailArgs ta = {s};
   ta.partials = c->partials; ta.n_partials = L.n_partials; ta.loss_scale = loss_scale;
-  ta.counters = c->counters + 4 * set; ta.out4 = out4;
+  ta.counters = ix.ctl; ta.out4 = out4;
   if (w) {
     ta.W = w->var; ta.Ws0 = w->s0; ta.Ws1 = w->s1; ta.gw = c->gw; ta.c_l2 = c_l2;
   }
   rc = orx_launch_tail(c, ta, opt->kind, st);
   if (set) {   // the prefetch set is free again once this tail has run
-    ORX_CUDA(cudaEventRecord(c->pf_free[set - 1], st));
-    c->pf_free_valid[set - 1] = 1;
+    ORX_CUDA(cudaEventRecord(ix.free, st));
+    ix.free_valid = 1;
   }
   orx_prof_mark(c, 3, st);
   orx_prof_next(c);
@@ -844,7 +847,7 @@ static int pair_fwd_grad(orx_ctx* c, int kind, const orx_table_t* user, const or
   ORX_REQUIRE(B > 0 && uid && pid && nid, "empty batch or null ids");
   int rc = orx_check_step_tables(user, item, bias, nullptr, ORX_OPT_SGD);
   if (rc) return rc;
-  const SparseArgs s = orx_sparse_args(c, user, item, bias, c->hu, c->hi, OrxOptDev{});
+  const SparseArgs s = orx_sparse_args(c, user, item, bias, c->set[0], OrxOptDev{});
   PairArgs a = pair_args(s, user->rows, item->rows, uid, pid, nid, B, margin, c_loss, c_l2, 1.0f / (float)B);
   a.d_user = d_user; a.d_pos = d_pos; a.d_neg = d_neg; a.d_bp = d_bp; a.d_bn = d_bn; a.g_out = g_out;
   return pair_unfused(c, kind, a, out4, st);

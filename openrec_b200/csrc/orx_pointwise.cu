@@ -330,7 +330,7 @@ static int point_fwd_grad(orx_ctx* h, int kind, const orx_table_t* user, const o
   const orx_table_t* dense_w = (kind == ORX_POINT_GMF) ? w : nullptr;
   int rc = orx_check_step_tables(user, item, bias, dense_w, ORX_OPT_SGD);
   if (rc) return rc;
-  const SparseArgs s = orx_sparse_args(h, user, item, bias, h->hu, h->hi, OrxOptDev{});
+  const SparseArgs s = orx_sparse_args(h, user, item, bias, h->set[0], OrxOptDev{});
   PointArgs pa = point_args(s, dense_w, user, item, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2);
   pa.d_user = d_user; pa.d_item = d_item; pa.d_bias = d_bias; pa.g_out = g_out;
   if (dense_w && d_w) {

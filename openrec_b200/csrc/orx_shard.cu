@@ -790,32 +790,23 @@ static int sh_ctas_per_sm(orx_shard_ws* s, const void* fn, int cap) {
 // nb = max(home_cap, ceil(gin_cap / 2)) lookups: home_cap user rows, gin_cap item rows.  With base == nullptr only the
 // size is computed.
 static size_t sh_layout(char* base, int home_cap, int gin_cap, int dim, orx_shard_ws* s) {
-  size_t off = 0;
-  auto take = [&](size_t bytes) {
-    char* p = base ? base + off : nullptr;
-    off += (bytes + 255) & ~(size_t)255;
-    return p;
-  };
+  OrxCarve m = {base, 0};
   ShardWs& w = s->w;
-  w.trip_u = (int32_t*)take(sizeof(int32_t) * home_cap);
-  w.slot = (int32_t*)take(sizeof(int32_t) * 2 * (size_t)home_cap);
-  w.req = (int32_t*)take(sizeof(int32_t) * gin_cap);
-  w.ctl = (int32_t*)take(sizeof(int32_t) * SH_C_WORDS);
+  w.trip_u = (int32_t*)m.take(sizeof(int32_t) * home_cap);
+  w.slot = (int32_t*)m.take(sizeof(int32_t) * 2 * (size_t)home_cap);
+  w.req = (int32_t*)m.take(sizeof(int32_t) * gin_cap);
+  w.ctl = (int32_t*)m.take(sizeof(int32_t) * SH_C_WORDS);
   const int64_t nb = home_cap > (gin_cap + 1) / 2 ? home_cap : (gin_cap + 1) / 2;
-  auto hash = [&](OrxHash& t, int64_t lookups, int counter_word) {
-    const uint32_t cap = orx_hash_shape(t, lookups);
-    t.slots = (unsigned long long*)take(sizeof(unsigned long long) * cap);
-    t.didx = (int32_t*)take(sizeof(int32_t) * cap);
-    t.did = (int32_t*)take(sizeof(int32_t) * (size_t)(lookups + 1));
-    t.counter = base ? w.ctl + counter_word : nullptr;
-  };
-  hash(s->hu[0], nb, SH_C_CNT + 0);
-  hash(s->hu[1], nb, SH_C_CNT + 1);
-  hash(s->hi, 2 * nb, SH_C_CNT + 3);
-  s->gu = (float*)take(sizeof(float) * (size_t)nb * dim);
-  s->gi = (float*)take(sizeof(float) * 2 * (size_t)nb * dim);
-  s->gb = (float*)take(sizeof(float) * 2 * (size_t)nb);
-  return off;
+  orx_hash_carve(m, s->hu[0], nb);
+  orx_hash_carve(m, s->hu[1], nb);
+  orx_hash_carve(m, s->hi, 2 * nb);
+  s->hu[0].counter = base ? w.ctl + SH_C_CNT + 0 : nullptr;
+  s->hu[1].counter = base ? w.ctl + SH_C_CNT + 1 : nullptr;
+  s->hi.counter = base ? w.ctl + SH_C_CNT + 3 : nullptr;
+  s->gu = (float*)m.take(sizeof(float) * (size_t)nb * dim);
+  s->gi = (float*)m.take(sizeof(float) * 2 * (size_t)nb * dim);
+  s->gb = (float*)m.take(sizeof(float) * 2 * (size_t)nb);
+  return m.off;
 }
 
 // the device scratch stays with the handle (shard_scratch, freed by orx_destroy)
@@ -846,15 +837,6 @@ static int shard_ws_ensure(orx_ctx* c, const ShardHost* x, cudaStream_t st) {
   s->gin_cap = x->gin_cap;
   s->got_rows = got_rows;
   s->dim = x->dim;
-  return ORX_OK;
-}
-
-// The next epoch of one of the step's index sets (31 bits, like the handle's).  On the wrap the set is emptied on st:
-// every launch that reads or writes it runs on st and was issued before, so no stale slot aliases the epochs to come.
-static int sh_take_epoch(OrxHash& t, cudaStream_t st, uint32_t* ep) {
-  const uint32_t e = (t.epoch + 1) & 0x7fffffffu;
-  if (e == 0) ORX_CUDA(cudaMemsetAsync(t.slots, 0, sizeof(unsigned long long) * ((size_t)t.mask + 1), st));
-  *ep = t.epoch = e ? e : 1;
   return ORX_OK;
 }
 
@@ -964,7 +946,8 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
 
   // phases 0 / 1: unless this step's prologue was already issued (announced in the previous call, or explicitly)
   if (phase_lo == 0 && S->pro_route[par] != epoch) {
-    if ((rc = sh_take_epoch(S->hu[par], st, &S->ep_u[par]))) return rc;
+    if ((rc = orx_take_epoch(S->hu[par], st))) return rc;   // every launch that uses the step's sets runs on st
+    S->ep_u[par] = S->hu[par].epoch;
     S->ids_u[par] = uid; S->ids_p[par] = pid; S->ids_n[par] = nid; S->ids_B[par] = B;
   }
   if (S->pro_route[par] == epoch || phase_lo == 0)      // whichever way the prologue was issued: it must be for THIS batch
@@ -1000,8 +983,8 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
       case 2:
         ORX_REQUIRE(S->pro_request[par] == epoch, "phase 2 before this step's phases 0 and 1");
         // the item set's epoch: apply and tail of the previous step, its last readers, were issued before this
-        if ((rc = sh_take_epoch(S->hi, st, &S->ep_i[par]))) return rc;
-        hi.epoch = S->ep_i[par];
+        if ((rc = orx_take_epoch(S->hi, st))) return rc;
+        hi.epoch = S->ep_i[par] = S->hi.epoch;
         sh_dispatch_nq(nq, [&](auto Q) {
           auto kern = k_sh_serve<decltype(Q)::value>;
           orx_launch_pdl(kern, dim3(h->num_sms * sh_ctas_per_sm(S, (const void*)kern, 4)), dim3(256), 0, st, xd, w,
@@ -1025,7 +1008,8 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
         memset(&pro, 0, sizeof(pro));
         const int np = par ^ 1;
         if (announce && S->pro_route[np] != epoch + 1) {
-          if ((rc = sh_take_epoch(S->hu[np], st, &S->ep_u[np]))) return rc;
+          if ((rc = orx_take_epoch(S->hu[np], st))) return rc;
+          S->ep_u[np] = S->hu[np].epoch;
           pro.n_route = (next_B + 1023) / 1024;
           pro.n_request = request_blocks;
           pro.epoch = epoch + 1;

@@ -175,13 +175,13 @@ static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32
     const int blocks = (n + 63) / 64;   // 8 warps x 8 pairs per block and iteration
     orx_dispatch_opt(opt->kind, [&](auto O) {
       k_sparse_apply<decltype(O)::value><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride,
-                                                                 values, value_ld, n, h->hu, h->gu, o);
+                                                                 values, value_ld, n, h->set[0].u, h->gu, o);
     });
     ORX_LAUNCH_CHECK();
   }
-  if (dense && (rc = orx_launch_adam_sweeps(h, tab, nullptr, nullptr, h->hu, h->hi, o, st))) return rc;
+  if (dense && (rc = orx_launch_adam_sweeps(h, tab, nullptr, nullptr, h->set[0], o, st))) return rc;
   // staged rows: the shared tail with no item side and no loss
-  TailArgs ta = {orx_sparse_args(h, tab, nullptr, nullptr, h->hu, h->hi, o)};
-  ta.counters = h->counters;
+  TailArgs ta = {orx_sparse_args(h, tab, nullptr, nullptr, h->set[0], o)};
+  ta.counters = h->set[0].ctl;
   return orx_launch_tail(h, ta, opt->kind, st);
 }

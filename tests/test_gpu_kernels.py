@@ -537,6 +537,73 @@ def test_epoch_wrap():
         e.close()
 
 
+@pytest.mark.parametrize("case", ["prefetch", "host", "set0_under_prefetch", "apply_censor"])
+def test_epoch_wrap_per_set(case):
+    """Every index table takes its own epoch, and a wrap empties only that table, on the stream that builds into it.
+    Every table starts 3 below 2^31 (its third build wraps), with few rows so that every row is hit many times:
+      prefetch            -- prefetched steps, sets 1 and 2 alternating, each set wrapping;
+      host                -- orx_pairwise_step_host run ahead, its side-stream sets wrapping under the previous step;
+      set0_under_prefetch -- set 0 wraps under pointwise steps and censors while a prefetch is outstanding, and the
+                             pairwise step then consumes that prefetch;
+      apply_censor        -- orx_sparse_apply_strided and orx_censor, which use set 0's user table only.
+    Each step matches the oracle, with its dispatch record."""
+    e = N.Engine(0)
+    try:
+        rng = np.random.default_rng(seed_of("wrap", case))
+        U, I, D, B = 50, 70, 64, 512
+        if case == "apply_censor":
+            ok, lr = OPTS["adagrad"]
+            var = rng.uniform(-0.3, 0.3, (U, D))
+            st, dv = slots(ok, ("v", var))
+            tv = dev(var)
+            var, s0 = tv.cpu().numpy().astype(np.float64), dv["v"][0].cpu().numpy().astype(np.float64)
+            tc = dev(rng.uniform(-0.3, 0.3, (U, D)))
+            cref = tc.cpu().numpy().astype(np.float64)
+            for k in range(5):                       # the user table's epochs: k = 0 allocates, then 2^31-2 ... wrap
+                ids = rng.integers(0, U, B).astype(np.int32)
+                vals = rng.standard_normal((B, 2, D)).astype(np.float32)
+                e.sparse_apply_strided(N.table(tv, dv["v"][0]), dev(np.stack([ids, ids[::-1]], 1), torch.int32), 1,
+                                       dev(vals), N.opt(ok, lr, step=k + 1))
+                O.apply_sparse(ok, var, s0, None, ids[::-1], vals[:, 1].astype(np.float64), k + 1, lr)
+                e.censor(tc, dev(ids, torch.int32))
+                O.censor(cref, ids)
+                close(tv, var, atol=2e-5, what=f"sparse apply {k}")
+                close(dv["v"][0], s0, atol=2e-5, what=f"accumulator {k}")
+                close(tc, cref, what=f"censor {k}")
+                if k == 0:
+                    e.debug_set_epoch(2 ** 31 - 3)
+            return
+        p = PairProb("bpr", "adagrad", D, U, I, seed_of("wrap-tabs", case), scale=0.05)
+        p.step(e, _ids(rng, "mixed", U, I, B))       # allocates the workspace (epochs restart there)
+        e.debug_set_epoch(2 ** 31 - 3)
+        ids = [_ids(rng, "mixed", U, I, B) for _ in range(8)]
+        if case == "host":
+            runs = [p.run(e, x, host=True, index_set="prefetch") for x in ids]
+            for x, (out, n, _) in zip(ids, runs):
+                p.verify(out, x, n, tables=False)
+            p.check_tables()
+            sets = [r[2] for r in runs]
+        else:
+            if case == "set0_under_prefetch":
+                q = PointProb("gmf", "adagrad", D, U, I, seed_of("wrap-point"))
+                tc = dev(rng.uniform(-0.3, 0.3, (U, D)))
+                cref = tc.cpu().numpy().astype(np.float64)
+            sets = []
+            for x in ids:
+                dids = [dev(a, torch.int32) for a in x]
+                torch.cuda.synchronize()             # the id tensors are complete: ids_ready=True is honest
+                e.pairwise_prefetch(p.tt[0], p.tt[1], *dids, p.opt, ids_ready=True)
+                if case == "set0_under_prefetch":    # set 0: two user-table and one item-table epochs per batch
+                    q.step(e, _point_ids(rng, "mixed", U, I, B), (rng.random(B) < 0.4).astype(np.float32))
+                    e.censor(tc, dids[0])
+                    O.censor(cref, x[0])
+                    close(tc, cref, what="censor")
+                sets.append(p.step(e, x, dids=dids, index_set="prefetch")[1])
+        assert all(a != b for a, b in zip(sets, sets[1:])), sets   # sets 1 and 2 alternate
+    finally:
+        e.close()
+
+
 # ---------------------------------------------------------------------------------------
 @pytest.mark.parametrize("kind", ["gmf", "wrmf"])
 def test_pointwise_golden_fwd_grad(eng, golden_dir, kind):
