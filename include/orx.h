@@ -95,8 +95,9 @@ ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
  * TA = TB = 0, S = 1.  A sparse step (one record per call) has TA = kind (orx_pair_kind / orx_point_kind), TB = optimizer
  * (orx_opt_kind), M = B, N = D, K = the CTAs/SM bound of the fused kernel's __launch_bounds__ (0: none) and S = the batch
  * index set it used: 0 = built on the caller's stream, 1 or 2 = a consumed prefetch (orx_pairwise_prefetch, or the side
- * stream of orx_pairwise_step_host).  orx_score_rank and orx_score_topk write one record per call, and
- * orx_score_rank_shard one per phase-2 call (fields at ORX_OP_SCORE_RANK / ORX_OP_SCORE_TOPK / ORX_OP_SCORE_RANK_SHARD).
+ * stream of orx_pairwise_step_host).  orx_score_rank and orx_score_topk write one record per call, orx_score_rank_shard
+ * one per phase-2 call and orx_score_topk_shard one per phase-1 call (fields at ORX_OP_SCORE_RANK / ORX_OP_SCORE_TOPK /
+ * ORX_OP_SCORE_RANK_SHARD / ORX_OP_SCORE_TOPK_SHARD).
  * Host-side bookkeeping only: no device work, no synchronisation. */
 enum orx_dispatch_op {
   ORX_OP_GEMM = 0,
@@ -106,9 +107,11 @@ enum orx_dispatch_op {
   ORX_OP_POINTWISE_STEP = 4, /* orx_pointwise_step */
   ORX_OP_SCORE_RANK = 5,     /* orx_score_rank: TA = orx_score_kind, TB = 0, M = Bu, N = I, K = dim, S = item splits */
   ORX_OP_SCORE_TOPK = 6,     /* orx_score_topk: TA = orx_score_kind, TB = k, M = Bu, N = I, K = dim, S = item splits */
-  ORX_OP_SCORE_RANK_SHARD = 7 /* orx_score_rank_shard, phase 2 only: variant RANK_SMEM / RANK_GLOBAL of the local pass,
-                                 TA = orx_score_kind, TB = rank, M = Bu, N = local items, K = dim, S = item splits
-                                 (0: no local items, no pass launched) */
+  ORX_OP_SCORE_RANK_SHARD = 7, /* orx_score_rank_shard, phase 2 only: variant RANK_SMEM / RANK_GLOBAL of the local
+                                  pass, TA = orx_score_kind, TB = rank, M = Bu, N = local items, K = dim, S = item
+                                  splits (0: no local items, no pass launched) */
+  ORX_OP_SCORE_TOPK_SHARD = 8  /* orx_score_topk_shard, phase 1 only: variant TOPK, TA = orx_score_kind, TB = rank,
+                                  M = Bu, N = local items, K = dim, S = item splits (0: no local items, no pass) */
 };
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
@@ -436,6 +439,36 @@ ORX_API int orx_score_topk(orx_handle_t h, int32_t kind, const float* user_tab, 
                            int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
                            int32_t dim, const int64_t* excl_off, const int32_t* excl_items, int32_t k,
                            int32_t* top_items /*[Bu, k]*/, float* top_scores /*[Bu, k], may be NULL*/, orx_stream_t s);
+
+/* ---- sharded top-K retrieval: orx_score_topk over row-sharded user / item tables (orx_rowshard_t, the layout of
+ * orx_score_rank_shard), each rank keeping the k best of its own item rows (openrec_b200/sharded.py score_topk_sharded,
+ * Retriever on ShardedBPR / ShardedUCML).
+ * The call runs one phase; between phases the caller replaces each exchange buffer with its element-wise integer SUM
+ * over all ranks.  Buffers: xrows int32 [Bu, dim], xkeys int64 [Bu, world, k], top_items int32 [Bu, k], top_scores
+ * float [Bu, k] (may be NULL).
+ *   phase 0 reads the user shard and writes xrows[b] = the bits of user row uid[b] if this rank owns it, else 0 (the
+ *           phase 0 of orx_score_rank_shard);
+ *   phase 1 reads the summed xrows, scores this rank's item rows and writes xkeys[b, rank] = the 64-bit keys of its k
+ *           best eligible items of row b (score bits high, ~global item id low), sorted descending and padded with 0,
+ *           and 0 into every other rank's slot of xkeys (every element written);
+ *   phase 2 reads the summed xkeys and writes top_items / top_scores: the top k of the union of the ranks' keys.
+ * Exactly one rank contributes a non-zero word to each element of xrows and xkeys, so the sum carries them unchanged.
+ * Phase 2's outputs equal orx_score_topk on the global tables (scale NULL) bit for bit, whatever world is: the
+ * eligibility, order, padding, bad-uid and exclusion-list rules are those of orx_score_topk, applied to global item
+ * ids.  uid holds global user ids; the exclusion CSR is the global one, present on every rank.
+ * A rank without items (local_items == 0) may pass a 1-row dummy shard: phase 1 then writes an all-zero xkeys and
+ * launches no main pass.  No handle state crosses a phase boundary: phase 1 uses the scratch of orx_score_topk for its
+ * own pass and merge only, so one handle may serve several ranks, with any call between phases.
+ * The exchange moves 4 * Bu * dim + 8 * Bu * world * k bytes per call.
+ * ORX_ERR_INVALID before any device work: the geometry checks of orx_score_rank_shard, phase outside [0, 2], k outside
+ * [1, ORX_MAX_TOPK] (k > total_items is allowed), Bu * world * k > 2^31 - 1, a null buffer the phase reads or writes.
+ * Bu = 0 is a no-op.  There is no scale argument: no sharded model uses one. */
+ORX_API int orx_score_topk_shard(orx_handle_t h, int32_t kind, int32_t phase, const orx_rowshard_t* g_host,
+                                 const float* user_shard, const float* item_shard, const float* bias_shard,
+                                 int32_t dim, const int32_t* uid, int32_t Bu, const int64_t* excl_off,
+                                 const int32_t* excl_items, int32_t k, int32_t* xrows /*[Bu, dim]*/,
+                                 int64_t* xkeys /*[Bu, world, k]*/, int32_t* top_items /*[Bu, k]*/,
+                                 float* top_scores /*[Bu, k], may be NULL*/, orx_stream_t s);
 
 #ifdef __cplusplus
 }

@@ -17,7 +17,7 @@ ORX_POINT_GMF, ORX_POINT_WRMF = 0, 1
 ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST = 0, 1
 ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE = 0, 1, 2, 3
 ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP = 0, 1, 2, 3, 4
-ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_RANK_SHARD = 5, 6, 7
+ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK_SHARD = 5, 6, 7, 8
 ORX_VARIANT_GEMM_TMA, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_INTERACT = 0, 1, 2, 3
 ORX_VARIANT_STEP, ORX_VARIANT_STEP_PIPE, ORX_VARIANT_STEP_GENERIC = 4, 5, 6
 ORX_VARIANT_RANK_SMEM, ORX_VARIANT_RANK_GLOBAL, ORX_VARIANT_TOPK = 7, 8, 9
@@ -114,6 +114,8 @@ SIGNATURES = {
     "orx_score_rank_shard_sizes": [_i32, _i32, _i32, C.POINTER(_i64)],
     "orx_score_rank_shard": [_vp, _i32, _i32, C.POINTER(OrxRowShard), _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp,
                              _i32, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "orx_score_topk_shard": [_vp, _i32, _i32, C.POINTER(OrxRowShard), _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _i32,
+                             _vp, _vp, _vp, _vp, _vp],
 }
 
 _lib = None

@@ -18,6 +18,10 @@
 // and takes back its own items of pos u excl, the callers sum the integer counts over the ranks, and the finish reads
 // the sums.  The user rows and the positives' scores reach every rank the same way, as integer sums in which exactly
 // one rank contributes a non-zero word, so their bits cross unchanged.
+//
+// orx_score_topk_shard does the same for retrieval: each rank keeps the exact top k of its own rows (keys built from the
+// global item ids), the ranks' lists cross as a summed exchange, and the merge of k_score_topk takes the top k of their
+// union, which holds the global top k.
 #include <cub/device/device_segmented_sort.cuh>
 
 #include "orx_common.cuh"
@@ -751,8 +755,11 @@ struct TkRow {
   int64_t elo, ehi;   // the row's exclusion entries in [0, I)
 };
 
-template <int KIND>
-__global__ void __launch_bounds__(EV_NT, 2) k_score_topk(const EvalArgs a, const TopkWs w, int k) {
+// SHARD: the tile loop walks this rank's a.I local rows of a row-sharded table (local row i is item i * world + rank of
+// [0, I_all)) and takes user rows by batch position (a.user_tab = the summed exchange); keys and the exclusion lookup
+// use the global item id, so keys stay unique across ranks and equal scores order by global id as on one device.
+template <int KIND, bool SHARD>
+__device__ __forceinline__ void tk_main(const EvalArgs& a, const TopkWs& w, int k, int world, int rank, int64_t I_all) {
   __shared__ __align__(16) float sA[2][EV_KC][EV_LD];
   __shared__ __align__(16) float sB[2][EV_KC][EV_LD];
   __shared__ TkRow meta[EV_TU];
@@ -797,8 +804,8 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_topk(const EvalArgs a, const
     TkRow m = {};
     if (tid < rows) {
       int64_t raw;
-      m.urow = ev_user_row<false>(a, u0 + tid);
-      ev_range(a.excl_off, a.excl_items, a.uid[u0 + tid], a.U, a.I, &m.elo, &m.ehi, &raw);
+      m.urow = ev_user_row<SHARD>(a, u0 + tid);
+      ev_range(a.excl_off, a.excl_items, a.uid[u0 + tid], a.U, SHARD ? I_all : a.I, &m.elo, &m.ehi, &raw);
     }
     meta[tid] = m;
     s_thr[tid] = 0ull;
@@ -823,8 +830,9 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_topk(const EvalArgs a, const
         const int64_t i = i0 + ev_frag(tx, y);
         const float s = acc[x][y] + bv[y];
         if (i >= a.I || s != s) continue;
-        const unsigned long long key = tk_key(s, i);
-        if (key <= thr || ev_contains(a.excl_items, meta[r].elo, meta[r].ehi, (int32_t)i)) continue;
+        const int64_t ig = SHARD ? (int32_t)i * world + rank : i;   // a global id is < 2^31
+        const unsigned long long key = tk_key(s, ig);
+        if (key <= thr || ev_contains(a.excl_items, meta[r].elo, meta[r].ehi, (int32_t)ig)) continue;
         list(r)[atomicAdd(&s_cnt[r], 1)] = key;
       }
     }
@@ -835,20 +843,37 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_topk(const EvalArgs a, const
   if (tid < rows) w.cnt[(int64_t)(u0 + tid) * gridDim.x + blockIdx.x] = s_cnt[tid];
 }
 
-// Merge: one CTA per batch row.  The top k of the union of the row's split lists (radix select when the union is
-// larger), sorted descending in shared memory (bitonic), decoded; slots past the eligible items get item -1, -inf.
-__global__ void __launch_bounds__(EV_NT) k_topk_merge(const TopkWs w, int splits, int k, int32_t* top_items,
-                                                      float* top_scores) {
-  __shared__ unsigned long long s_key[ORX_MAX_TOPK];
+template <int KIND>
+__global__ void __launch_bounds__(EV_NT, 2) k_score_topk(const EvalArgs a, const TopkWs w, int k) {
+  tk_main<KIND, false>(a, w, k, 1, 0, a.I);
+}
+
+// Sharded phase 1's main pass (a.user_tab: the summed user rows of phase 0, by batch position).
+template <int KIND>
+__global__ void __launch_bounds__(EV_NT, 2) k_score_topk_shard(const EvalArgs a, const TopkWs w, int k, int world,
+                                                               int rank, int64_t I_all) {
+  tk_main<KIND, true>(a, w, k, world, rank, I_all);
+}
+
+// Merge of one batch row (the CTA): the top k of the union of its lists (radix select when the union is larger), sorted
+// descending into s_key[0, k) (bitonic), 0 past the keys.  The lists: the row's split lists of k_score_topk (stride
+// k + TK_ROOM, cnt[s] keys each), or with XIN the summed exchange of the sharded phase 1 (`lists` ranks' lists of stride
+// k, each sorted descending and padded with 0).  Only real keys are counted and visited, never padding: keys are
+// unique (global item ids), so at most k of them are >= the k-th and s_key cannot overflow.
+template <bool XIN>
+__device__ __forceinline__ void tk_merge(const unsigned long long* cand, const int* cnt, int lists, int k,
+                                         unsigned long long* s_key) {
   __shared__ unsigned s_hist[256];
   __shared__ unsigned long long s_sel[2];
   __shared__ int s_n, s_m;
-  const int b = blockIdx.x, tid = threadIdx.x;
+  const int tid = threadIdx.x;
   const int C = k + TK_ROOM;
-  const unsigned long long* cand = w.cand + (int64_t)b * splits * C;
-  const int* cnt = w.cnt + (int64_t)b * splits;
-  auto each = [&](auto fn) {   // splits * k <= 2^31: the grid has at most a few thousand CTAs
-    for (int e = tid; e < splits * k; e += EV_NT) {
+  auto each = [&](auto fn) {   // lists * k <= 2^31: the grid has at most a few thousand CTAs; the caller checks world
+    for (int e = tid; e < lists * k; e += EV_NT) {
+      if (XIN) {
+        if (cand[e]) fn(cand[e]);
+        continue;
+      }
       const int s = e / k, q = e - s * k;
       if (q < cnt[s]) fn(cand[(int64_t)s * C + q]);
     }
@@ -859,7 +884,10 @@ __global__ void __launch_bounds__(EV_NT) k_topk_merge(const TopkWs w, int splits
   }
   __syncthreads();
   int part = 0;
-  for (int s = tid; s < splits; s += EV_NT) part += cnt[s];
+  if (XIN)
+    for (int e = tid; e < lists * k; e += EV_NT) part += cand[e] != 0ull;
+  else
+    for (int s = tid; s < lists; s += EV_NT) part += cnt[s];
   if (part) atomicAdd(&s_n, part);
   __syncthreads();
   const int n = s_n;
@@ -886,11 +914,44 @@ __global__ void __launch_bounds__(EV_NT) k_topk_merge(const TopkWs w, int splits
       }
       __syncthreads();
     }
-  for (int j = tid; j < k; j += EV_NT) {
+}
+
+// Row b's merged keys decoded; slots past the eligible items get item -1, -inf.
+__device__ __forceinline__ void tk_decode(const unsigned long long* s_key, int b, int k, int32_t* top_items,
+                                          float* top_scores) {
+  for (int j = threadIdx.x; j < k; j += EV_NT) {
     const unsigned long long key = s_key[j];
     top_items[(int64_t)b * k + j] = key ? (int32_t)~(uint32_t)key : -1;
     if (top_scores) top_scores[(int64_t)b * k + j] = key ? tk_score(key) : __int_as_float(0xff800000);
   }
+}
+
+// Merge: one CTA per batch row, over the row's split lists.
+__global__ void __launch_bounds__(EV_NT) k_topk_merge(const TopkWs w, int splits, int k, int32_t* top_items,
+                                                      float* top_scores) {
+  __shared__ unsigned long long s_key[ORX_MAX_TOPK];
+  const int b = blockIdx.x;
+  tk_merge<false>(w.cand + (int64_t)b * splits * (k + TK_ROOM), w.cnt + (int64_t)b * splits, splits, k, s_key);
+  tk_decode(s_key, b, k, top_items, top_scores);
+}
+
+// Sharded phase 1's local merge: this rank's top k of row b, as raw keys, into slot [b][rank] of xkeys[Bu][world][k].
+__global__ void __launch_bounds__(EV_NT) k_topk_merge_local(const TopkWs w, int splits, int k, int world, int rank,
+                                                            unsigned long long* xkeys) {
+  __shared__ unsigned long long s_key[ORX_MAX_TOPK];
+  const int b = blockIdx.x;
+  tk_merge<false>(w.cand + (int64_t)b * splits * (k + TK_ROOM), w.cnt + (int64_t)b * splits, splits, k, s_key);
+  unsigned long long* slot = xkeys + ((int64_t)b * world + rank) * k;
+  for (int j = threadIdx.x; j < k; j += EV_NT) slot[j] = s_key[j];
+}
+
+// Sharded phase 2: row b's top k over the world ranks' lists of the summed xkeys, decoded.
+__global__ void __launch_bounds__(EV_NT) k_topk_merge_ranks(const unsigned long long* xkeys, int world, int k,
+                                                            int32_t* top_items, float* top_scores) {
+  __shared__ unsigned long long s_key[ORX_MAX_TOPK];
+  const int b = blockIdx.x;
+  tk_merge<true>(xkeys + (int64_t)b * world * k, nullptr, world, k, s_key);
+  tk_decode(s_key, b, k, top_items, top_scores);
 }
 
 // The call's scratch inside one allocation; with base == nullptr only the size is computed.
@@ -987,13 +1048,18 @@ int ev_launch(orx_ctx* h, const EvalRowArgs& a, const EvalWs& w, const EvalOut& 
   return ORX_OK;
 }
 
+// Phase 0 of orx_score_rank_shard and orx_score_topk_shard: the bits of this rank's user rows of the batch.
+void ev_user_rows(const EvalRowArgs& a, int32_t* xrows, cudaStream_t st) {
+  const int64_t blocks = ((int64_t)a.Bu * a.D + EV_NT - 1) / EV_NT;
+  k_eval_user_rows<<<(unsigned)(blocks < 4096 ? blocks : 4096), EV_NT, 0, st>>>(a, xrows);
+}
+
 // One phase of orx_score_rank_shard (arguments checked by the caller).
 template <int KIND>
 int ev_shard_phase(orx_ctx* h, int phase, const EvalRowArgs& a, const EvalOut& o, int32_t* xrows, int32_t* xpred,
                    int64_t* xcnt, cudaStream_t st) {
   if (phase == 0) {
-    const int64_t blocks = ((int64_t)a.Bu * a.D + EV_NT - 1) / EV_NT;
-    k_eval_user_rows<<<(unsigned)(blocks < 4096 ? blocks : 4096), EV_NT, 0, st>>>(a, xrows);
+    ev_user_rows(a, xrows, st);
   } else if (phase == 1) {
     k_eval_pos_scores<KIND><<<a.Bu, EV_NT, 0, st>>>(a, xpred);
   } else if (phase == 2) {
@@ -1024,21 +1090,51 @@ size_t tk_layout(char* base, int Bu, int64_t splits, int k, TopkWs* w) {
   return m.off;
 }
 
+// The item splits of kern over a.I rows and the top-K scratch for them, from the handle's evaluation scratch.
+template <class Kern>
+int tk_workspace(orx_ctx* h, Kern kern, const EvalArgs& a, int k, int64_t* splits, TopkWs* w) {
+  int rc = ev_item_splits(h, kern, 0, a.Bu, a.I, splits);
+  if (rc != ORX_OK) return rc;
+  rc = orx_grow(&h->eval_ws, &h->eval_cap, tk_layout(nullptr, a.Bu, *splits, k, w));
+  if (rc != ORX_OK) return rc;
+  tk_layout(static_cast<char*>(h->eval_ws), a.Bu, *splits, k, w);
+  return ORX_OK;
+}
+
 template <int KIND>
 int tk_launch(orx_ctx* h, const EvalArgs& a, int k, int32_t* top_items, float* top_scores, cudaStream_t st) {
   int64_t splits = 1;
-  int rc = ev_item_splits(h, k_score_topk<KIND>, 0, a.Bu, a.I, &splits);
-  if (rc != ORX_OK) return rc;
   TopkWs w;
-  rc = orx_grow(&h->eval_ws, &h->eval_cap, tk_layout(nullptr, a.Bu, splits, k, &w));
+  const int rc = tk_workspace(h, k_score_topk<KIND>, a, k, &splits, &w);
   if (rc != ORX_OK) return rc;
-  tk_layout(static_cast<char*>(h->eval_ws), a.Bu, splits, k, &w);
   const int64_t user_tiles = (a.Bu + EV_TU - 1) / EV_TU;
   k_score_topk<KIND><<<dim3((unsigned)splits, (unsigned)user_tiles), EV_NT, 0, st>>>(a, w, k);
   ORX_LAUNCH_CHECK();
   k_topk_merge<<<a.Bu, EV_NT, 0, st>>>(w, (int)splits, k, top_items, top_scores);
   ORX_LAUNCH_CHECK();
   orx_log_dispatch(h, ORX_OP_SCORE_TOPK, ORX_VARIANT_TOPK, KIND, k, a.Bu, (int)a.I, a.D, (int)splits);
+  return ORX_OK;
+}
+
+// Phase 1 of orx_score_topk_shard (arguments checked by the caller): xkeys all 0, then, when this rank has item rows,
+// the main pass over them and the local merge into slot [b][rank].  Only the scratch of this call is used.
+template <int KIND>
+int tk_shard_local(orx_ctx* h, const EvalArgs& a, int k, int world, int rank, int64_t I_all,
+                   unsigned long long* xkeys, cudaStream_t st) {
+  ORX_CUDA(cudaMemsetAsync(xkeys, 0, sizeof(unsigned long long) * (size_t)a.Bu * world * k, st));
+  int64_t splits = 0;
+  if (a.I > 0) {
+    TopkWs w;
+    const int rc = tk_workspace(h, k_score_topk_shard<KIND>, a, k, &splits, &w);
+    if (rc != ORX_OK) return rc;
+    const int64_t user_tiles = (a.Bu + EV_TU - 1) / EV_TU;
+    k_score_topk_shard<KIND><<<dim3((unsigned)splits, (unsigned)user_tiles), EV_NT, 0, st>>>(a, w, k, world, rank,
+                                                                                             I_all);
+    ORX_LAUNCH_CHECK();
+    k_topk_merge_local<<<a.Bu, EV_NT, 0, st>>>(w, (int)splits, k, world, rank, xkeys);
+    ORX_LAUNCH_CHECK();
+  }
+  orx_log_dispatch(h, ORX_OP_SCORE_TOPK_SHARD, ORX_VARIANT_TOPK, KIND, rank, a.Bu, (int)a.I, a.D, (int)splits);
   return ORX_OK;
 }
 
@@ -1147,4 +1243,49 @@ extern "C" int orx_score_rank_shard(orx_handle_t h, int32_t kind, int32_t phase,
   cudaStream_t st = (cudaStream_t)s;
   return kind == ORX_SCORE_DOT ? ev_shard_phase<ORX_SCORE_DOT>(h, phase, a, o, xrows, xpred, xcnt, st)
                                : ev_shard_phase<ORX_SCORE_NEG_SQDIST>(h, phase, a, o, xrows, xpred, xcnt, st);
+}
+
+extern "C" int orx_score_topk_shard(orx_handle_t h, int32_t kind, int32_t phase, const orx_rowshard_t* g_host,
+                                    const float* user_shard, const float* item_shard, const float* bias_shard,
+                                    int32_t dim, const int32_t* uid, int32_t Bu, const int64_t* excl_off,
+                                    const int32_t* excl_items, int32_t k, int32_t* xrows, int64_t* xkeys,
+                                    int32_t* top_items, float* top_scores, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr && g_host != nullptr, "null pointer");
+  ORX_REQUIRE(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST, "unknown score kind");
+  ORX_REQUIRE(phase >= 0 && phase <= 2, "phase must lie in [0, 2]");
+  const orx_rowshard_t g = *g_host;
+  ORX_REQUIRE(g.world >= 1 && g.rank >= 0 && g.rank < g.world, "rank must lie in [0, world)");
+  ORX_REQUIRE(g.total_users > 0 && g.total_items > 0 && g.total_items <= INT32_MAX, "bad table sizes");
+  ORX_REQUIRE(g.local_users == (g.total_users - g.rank + g.world - 1) / g.world &&
+                  g.local_items == (g.total_items - g.rank + g.world - 1) / g.world,
+              "local_users / local_items disagree with (total, world, rank)");
+  ORX_REQUIRE(dim > 0 && Bu >= 0, "bad sizes");
+  ORX_REQUIRE(k >= 1 && k <= ORX_MAX_TOPK, "k must lie in [1, ORX_MAX_TOPK]");
+  if (Bu == 0) return ORX_OK;
+  ORX_REQUIRE((int64_t)Bu * g.world * k <= INT32_MAX, "Bu * world * k too large for one call: split the batch");
+  ORX_REQUIRE(uid != nullptr, "null pointer");
+  ORX_REQUIRE(phase != 0 || (user_shard && xrows), "phase 0 needs user_shard and xrows");
+  ORX_REQUIRE(phase != 1 || (item_shard && xrows && xkeys), "phase 1 needs item_shard, xrows and xkeys");
+  ORX_REQUIRE(phase != 2 || (xkeys && top_items), "phase 2 needs xkeys and top_items");
+  ORX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)s;
+  unsigned long long* keys = reinterpret_cast<unsigned long long*>(xkeys);
+  if (phase == 0) {
+    EvalRowArgs a = {};
+    a.user_tab = user_shard; a.U = g.total_users; a.uid = uid; a.Bu = Bu; a.D = dim; a.world = g.world;
+    a.rank = g.rank;
+    ev_user_rows(a, xrows, st);
+  } else if (phase == 1) {
+    EvalArgs a = {};
+    a.user_tab = reinterpret_cast<const float*>(xrows); a.U = g.total_users; a.uid = uid; a.Bu = Bu;
+    a.item_tab = item_shard; a.bias = bias_shard; a.I = g.local_items; a.D = dim; a.excl_off = excl_off;
+    a.excl_items = excl_items;
+    return kind == ORX_SCORE_DOT
+               ? tk_shard_local<ORX_SCORE_DOT>(h, a, k, g.world, g.rank, g.total_items, keys, st)
+               : tk_shard_local<ORX_SCORE_NEG_SQDIST>(h, a, k, g.world, g.rank, g.total_items, keys, st);
+  } else {
+    k_topk_merge_ranks<<<Bu, EV_NT, 0, st>>>(keys, g.world, k, top_items, top_scores);
+  }
+  ORX_LAUNCH_CHECK();
+  return ORX_OK;
 }

@@ -9,7 +9,7 @@ import torch
 
 from . import _lib
 from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP,
-                   ORX_OP_SCORE_RANK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
+                   ORX_OP_SCORE_RANK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_TOPK_SHARD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
                    ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
                    ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
                    ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE,
@@ -21,7 +21,7 @@ __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", 
            "ORX_OP_POINTWISE_STEP", "ORX_VARIANT_GEMM_TMA", "ORX_VARIANT_GEMM_SIMT", "ORX_VARIANT_INTERACT_WARP",
            "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC",
            "ORX_OP_SCORE_RANK", "ORX_VARIANT_RANK_SMEM", "ORX_VARIANT_RANK_GLOBAL", "ORX_OP_SCORE_TOPK",
-           "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "Dispatch", "RowShard", "rowshard"]
+           "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "ORX_OP_SCORE_TOPK_SHARD", "Dispatch", "RowShard", "rowshard"]
 
 _engines = {}
 
@@ -393,6 +393,33 @@ class Engine:
             _ptr(_f32(item_tab, "item_tab")), _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(excl_off),
             _ptr(excl_items), k, _ptr(items), _ptr(scores), self.stream()), "orx_score_topk")
         return items, scores
+
+    def score_topk_shard(self, kind, phase, g, user_shard, item_shard, bias_shard, uid, excl_off, excl_items, k, xrows,
+                         xkeys):
+        """One phase of score_topk over row-sharded tables (orx_score_topk_shard in include/orx.h).  g: RowShard; the
+        shards are this rank's rows (bias_shard flat [local_items] or None); uid and the exclusion CSR are global.
+        Exchange buffers: xrows int32 [Bu * dim], xkeys int64 [Bu * world * k], summed over the ranks by the caller
+        between phases (openrec_b200.sharded.score_topk_sharded).  Phase 2 -> (items int32 [Bu, k], scores float32
+        [Bu, k]); other phases -> None."""
+        uid = ids32(uid)
+        Bu, dev = uid.numel(), xrows.device
+        excl_off, excl_items = _csr(excl_off, excl_items, g.total_users)
+        k = int(k)
+        if not 1 <= k <= _lib.ORX_MAX_TOPK:
+            raise ValueError(f"k must lie in [1, {_lib.ORX_MAX_TOPK}]")
+        if xrows.dtype != torch.int32 or xkeys.dtype != torch.int64:
+            raise ValueError("exchange buffers: xrows int32, xkeys int64")
+        out = [None, None]
+        if phase == 2:
+            out = [torch.empty((Bu, k), dtype=torch.int32, device=dev),
+                   torch.empty((Bu, k), dtype=torch.float32, device=dev)]
+        geo = _lib.OrxRowShard(*[int(x) for x in g])
+        _lib.check(self.lib.orx_score_topk_shard(
+            self.h, kind, int(phase), C.byref(geo), _ptr(_f32(user_shard, "user_shard")),
+            _ptr(_f32(item_shard, "item_shard")), _ptr(_f32(bias_shard, "bias_shard")), user_shard.shape[1],
+            _ptr(uid), Bu, _ptr(excl_off), _ptr(excl_items), k, _ptr(xrows), _ptr(xkeys), *[_ptr(t) for t in out],
+            self.stream()), "orx_score_topk_shard")
+        return tuple(out) if phase == 2 else None
 
 
 def engine(device=None) -> Engine:

@@ -147,8 +147,27 @@ def score_rank_sharded(parts, reduce, uid, pos_off, pos_items, excl_off, excl_it
     return outs
 
 
+def score_topk_sharded(parts, reduce, uid, excl_off, excl_items, k):
+    """Top-K retrieval (the k best unseen items of each user uid, as native.Engine.score_topk on the global tables) of
+    row-sharded tables, each rank keeping the k best of its own item rows: the three phases of orx_score_topk_shard,
+    with ``reduce`` between them.  ``parts``, ``reduce``, uid and the global exclusion CSR are as in
+    score_rank_sharded.  -> [(items int32 [Bu, k], scores float32 [Bu, k])] per part, identical on every rank."""
+    Bu, k = uid.numel(), int(k)
+    bufs = [(torch.empty(Bu * user.shape[1], dtype=torch.int32, device=item.device),
+             torch.empty(Bu * g.world * k, dtype=torch.int64, device=item.device))
+            for _, _, user, item, _, g in parts]
+    outs = [None] * len(parts)
+    for phase in range(3):   # every part's phase p is issued before any part's phase p + 1
+        for j, ((eng, kind, user, item, bias, g), b) in enumerate(zip(parts, bufs)):
+            outs[j] = eng.score_topk_shard(kind, phase, g, user, item, bias, uid, excl_off, excl_items, k, *b)
+        if phase < 2:
+            reduce([b[phase] for b in bufs])
+    return outs
+
+
 def all_reduce_sum(group=None):
-    """reduce for score_rank_sharded with one rank per process: an all-reduce (SUM) on torch's current stream."""
+    """reduce for score_rank_sharded / score_topk_sharded with one rank per process: an all-reduce (SUM) on torch's
+    current stream."""
     def reduce(tensors):
         for t in tensors:
             dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
@@ -156,7 +175,8 @@ def all_reduce_sum(group=None):
 
 
 def loopback_sum(tensors):
-    """reduce for score_rank_sharded with every rank in this process (virtual ranks on one device)."""
+    """reduce for score_rank_sharded / score_topk_sharded with every rank in this process (virtual ranks on one
+    device)."""
     total = tensors[0].clone()
     for t in tensors[1:]:
         total += t

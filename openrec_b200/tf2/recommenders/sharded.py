@@ -117,13 +117,15 @@ class ShardedBPR(Model):
 
     def _sharded_score_operands(self):
         """(score kind, user shard, item shard, item bias shard as a flat [rows] view, native.RowShard, process group)
-        of the catalogue evaluation over the shards (RankingEvaluator: one collective call on every rank)."""
+        of the catalogue evaluation and retrieval over the shards (RankingEvaluator.evaluate, Retriever.recommend: one
+        collective call on every rank)."""
         g = N.rowshard(self._world, self._rank, self._U, self._I)
         return (self._score, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
                 self.item_bias.embeddings.t.reshape(-1), g, None)
 
     def inference(self, user_id):
-        raise NotImplementedError("full-catalogue scoring needs the whole item table on one device")
+        raise NotImplementedError("full-catalogue scoring needs the whole item table on one device; a sharded model's "
+                                  "top-k items come from Retriever.recommend")
 
     def check(self):
         """Raise if the sharded step flagged an error (peer timeout, mailbox overflow)."""
