@@ -242,6 +242,31 @@ ORX_API int orx_pairwise_grad_rows(orx_handle_t h, int32_t kind, const float* ro
                                    float margin, float c_loss, float c_l2, float inv_B, float* d_rows, float* out4,
                                    orx_stream_t s);
 
+/* ---- row-sharded DLRM (openrec_b200/csrc/orx_dlrm_shard.cu, openrec_b200/sharded.py ShardedDLRMStep) ----------
+ * The T embedding tables form one row space: row_off[k] = sum of the vocabularies of tables 0..k-1, G = row_off[T] <=
+ * 2^31 - 1.  Lookup i = b*T + k (id = sparse[i]) is valid iff 0 <= id < row_off[k+1] - row_off[k]; its global row
+ * g = row_off[k] + id lives on rank g % world at local row g / world.
+ * orx_lookup_bucket: sparse [B, T] int32 row-major (device), row_off_host int64 [T + 1] (host).  The unique valid
+ *   global rows of the batch, in ascending (owner, local row) order -- the send order, n_uniq rows:
+ *     counts[world]      unique rows owned by each rank (sum = n_uniq)
+ *     send_local[j]      local row of unique row j on its owner                          (j < n_uniq; rest unspecified)
+ *     slot[i]            send-order index of lookup i, or -1 for an invalid id           (all B*T entries)
+ *     grp_idx[grp_off[j] .. grp_off[j+1])  the lookups of unique row j, ascending i       (rest unspecified)
+ *     grp_off[n_uniq]    the number of valid lookups                                     (grp_off needs B*T + 1 entries)
+ *   Limits: B*T <= 2^31 - 1, T >= 1, 1 <= world <= 1024, row_off[0] == 0 and non-decreasing (ORX_ERR_INVALID
+ *   otherwise, before any device work).  B = 0 writes zero counts and grp_off[0] = 0 and launches nothing.  Scratch:
+ *   the handle's own lookup buffer (about 16 bytes per lookup plus the radix sort's storage), grown on demand; the
+ *   batch index sets are not touched, so an orx_sparse_apply later in the same step keeps them.
+ * orx_rows_segment_sum: out[j, :] = sum of src[grp_idx[p], :] for p in [grp_off[j], grp_off[j+1]), added in that
+ *   order, so repeated calls give the same bits.  src rows have stride src_ld >= dim; out is [n_uniq, dim]
+ *   contiguous; float4 loads when dim, src_ld and both pointers allow, a scalar path for any dim >= 1.  grp_idx entries
+ *   must index rows of src.  n_uniq = 0 is a no-op. */
+ORX_API int orx_lookup_bucket(orx_handle_t h, const int32_t* sparse, int32_t B, int32_t T, const int64_t* row_off_host,
+                              int32_t world, int32_t* counts, int32_t* send_local, int32_t* slot, int32_t* grp_off,
+                              int32_t* grp_idx, orx_stream_t s);
+ORX_API int orx_rows_segment_sum(orx_handle_t h, const float* src, int64_t src_ld, int32_t dim, const int32_t* grp_off,
+                                 const int32_t* grp_idx, int32_t n_uniq, float* out, orx_stream_t s);
+
 /* ---- row-sharded BPR / UCML step over the GPUs of one box, "home-routed" (openrec_b200/csrc/orx_shard.cu,
  * openrec_b200/sharded.py).  The reference is single-device: this is the scale-out of the same synchronous step
  * (tf2_examples/bpr_citeulike.py:33-39) and replaces the NCCL all-to-alls named in SURVEY 8(e) with peer STORES into

@@ -98,6 +98,8 @@ SIGNATURES = {
                        _i32, _i32, _i32, _vp, _vp],
     "orx_owner_bucket_combined": [_vp, _vp, _i32, _i32, _i64, _i32, _vp, _vp, _vp, _vp],
     "orx_pairwise_grad_rows": [_vp, _i32, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _f, _f, _f, _f, _vp, _vp, _vp],
+    "orx_lookup_bucket": [_vp, _vp, _i32, _i32, C.POINTER(_i64), _i32, _vp, _vp, _vp, _vp, _vp, _vp],
+    "orx_rows_segment_sum": [_vp, _vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp],
     "orx_pointwise_step": [_vp, _i32, _T, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _i32, _f, _f, _O, _vp, _vp],
     "orx_pointwise_fwd": [_vp, _i32, _T, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _i32, _vp, _vp],
     "orx_pointwise_grad": [_vp, _i32, _T, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _i32, _f, _f,

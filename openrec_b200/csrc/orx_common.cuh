@@ -123,6 +123,8 @@ struct orx_ctx {
   int64_t dispatch_n;      // records written since the last read
   void* eval_ws;           // orx_eval.cu: scratch of orx_score_rank / orx_score_topk, its own allocation
   size_t eval_cap;
+  void* lookup_ws;         // orx_dlrm_shard.cu: scratch of orx_lookup_bucket (keys, scan, sort storage)
+  size_t lookup_cap;
   float* splitk;           // split-K partials of the Dense-layer GEMMs and of the split column sum
   size_t splitk_cap;
 };

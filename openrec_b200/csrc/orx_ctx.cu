@@ -191,6 +191,7 @@ extern "C" int orx_destroy(orx_handle_t h) {
   cudaFree(h->partials);
   cudaFree(h->bucket_cursor);
   cudaFree(h->eval_ws);
+  cudaFree(h->lookup_ws);
   cudaFree(h->splitk);
   cudaFree(h->shard_scratch);
   orx_shard_ws_release(h);

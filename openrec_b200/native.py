@@ -258,6 +258,38 @@ class Engine:
                    "orx_owner_bucket_combined")
         return counts, send_local, slot
 
+    def lookup_bucket(self, sparse, row_off, world):
+        """sparse int32 [B, T] on the device, row_off [T + 1] host ints (the tables' offsets in the concatenated row
+        space) -> (counts [world], send_local, slot [B*T], grp_off [B*T + 1], grp_idx [B*T]): the batch's unique valid
+        rows in (owner, local row) order and each one's lookups (orx_lookup_bucket in include/orx.h)."""
+        if sparse.dtype != torch.int32 or sparse.dim() != 2 or not sparse.is_contiguous():
+            raise ValueError("sparse: expected a contiguous int32 [B, T] tensor")
+        B, T = sparse.shape
+        if len(row_off) != T + 1:
+            raise ValueError("row_off must have T + 1 entries")
+        dev, n = sparse.device, B * T
+        counts = torch.empty(world, dtype=torch.int32, device=dev)
+        send_local, slot, grp_idx = (torch.empty(n, dtype=torch.int32, device=dev) for _ in range(3))
+        grp_off = torch.empty(n + 1, dtype=torch.int32, device=dev)
+        off = (C.c_int64 * (T + 1))(*[int(x) for x in row_off])
+        _lib.check(self.lib.orx_lookup_bucket(self.h, _ptr(sparse), B, T, off, world, _ptr(counts), _ptr(send_local),
+                                              _ptr(slot), _ptr(grp_off), _ptr(grp_idx), self.stream()),
+                   "orx_lookup_bucket")
+        return counts, send_local, slot, grp_off, grp_idx
+
+    def rows_segment_sum(self, src, grp_off, grp_idx, n_uniq, out=None):
+        """src [n, dim] (any row stride) -> out [n_uniq, dim]: row j = the sum of src rows grp_idx[grp_off[j] ..
+        grp_off[j+1]), in that order (orx_rows_segment_sum)."""
+        n_uniq = int(n_uniq)
+        if n_uniq < 0 or n_uniq + 1 > grp_off.numel():
+            raise ValueError("n_uniq must lie in [0, grp_off.numel() - 1]")
+        if out is None:
+            out = torch.empty((n_uniq, src.shape[1]), dtype=torch.float32, device=src.device)
+        _lib.check(self.lib.orx_rows_segment_sum(self.h, _ptr(src), self._ld(src), src.shape[1], _ptr(grp_off),
+                                                 _ptr(grp_idx), n_uniq, _ptr(out), self.stream()),
+                   "orx_rows_segment_sum")
+        return out
+
     def pairwise_grad_rows(self, kind, rows, dim, uslot, pslot, nslot, inv_B, d_rows, out4, margin=0.5, c_loss=1.0,
                            c_l2=1.0):
         _lib.check(self.lib.orx_pairwise_grad_rows(self.h, kind, _ptr(rows), rows.shape[1], dim, _ptr(uslot),

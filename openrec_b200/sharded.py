@@ -184,6 +184,209 @@ def loopback_sum(tensors):
         t.copy_(total)
 
 
+# ---------------------------------------------------------------------------------------
+# row-sharded DLRM: embedding rows on their owners, Dense layers replicated
+# ---------------------------------------------------------------------------------------
+def row_offsets(vocab):
+    """[T + 1] offsets of T tables of the given vocabularies in one concatenated row space; ValueError when the space
+    exceeds 2^31 - 1 rows (global rows are int32)."""
+    off = [0]
+    for v in vocab:
+        if int(v) < 0:
+            raise ValueError("a vocabulary size is negative")
+        off.append(off[-1] + int(v))
+    if off[-1] > 2 ** 31 - 1:
+        raise ValueError(f"the {len(vocab)} tables hold {off[-1]} rows in all; the sharded layout allows 2^31 - 1")
+    return off
+
+
+class DistExchange:
+    """The collectives of the sharded DLRM step with one rank per process (torch.distributed: NCCL, or gloo on CPU).
+    Every method takes lists with one entry, this rank's."""
+
+    def __init__(self, group=None):
+        self.group = group
+
+    def all_to_all(self, outs, ins, out_splits, in_splits):
+        for o, i, os_, is_ in zip(outs, ins, out_splits, in_splits):
+            dist.all_to_all_single(o, i, output_split_sizes=os_, input_split_sizes=is_, group=self.group)
+
+    def all_reduce(self, tensors):
+        for t in tensors:
+            dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
+
+
+class LoopbackExchange:
+    """The same collectives for R virtual ranks in this process (one entry per rank, all on one device): the 1-GPU
+    test of the multi-GPU code path, same kernels.  The sum adds the ranks in rank order and hands every rank the same
+    tensor, as an all-reduce does."""
+
+    @staticmethod
+    def all_to_all(outs, ins, out_splits, in_splits):
+        R = len(ins)
+        ioff = [np.concatenate([[0], np.cumsum(s)]).astype(np.int64) for s in in_splits]
+        ooff = [np.concatenate([[0], np.cumsum(s)]).astype(np.int64) for s in out_splits]
+        for q in range(R):
+            for r in range(R):
+                n = int(in_splits[q][r])
+                if n != int(out_splits[r][q]):
+                    raise ValueError("all_to_all: send and receive splits disagree")
+                if n:
+                    outs[r][ooff[r][q]:ooff[r][q] + n].copy_(ins[q][ioff[q][r]:ioff[q][r] + n])
+
+    all_reduce = staticmethod(loopback_sum)
+
+
+class DLRMShard:
+    """One rank's part of a row-sharded DLRM.  The T tables are one row space (row_offsets); global row g lives on rank
+    g % world at local row g // world of ``table`` ([max(rows, 1), dim]: a rank without rows keeps a 1-row dummy that
+    is never read), with its optimizer slots ``slots`` (s0, s1, None when the optimizer has fewer).  ``bot`` / ``top``
+    are this rank's Dense replicas as (kernel, bias or None, act) triples, ``dense_slots`` the (s0, s1) of every kernel
+    and bias in that order (biases that are None skipped)."""
+
+    def __init__(self, eng, rank, world, vocab, dim, bot, top, table, slots, dense_slots, *, self_interaction=False,
+                 mode="reference", loss_kind=0, clip=0.0):
+        from .tf2.mlp_ops import DLRMGraph
+        self.eng, self.rank, self.world, self.D = eng, rank, world, int(dim)
+        self.row_off = row_offsets(vocab)
+        self.T, self.G = len(vocab), self.row_off[-1]
+        self.rows = (self.G - rank + world - 1) // world
+        if tuple(table.shape) != (max(self.rows, 1), self.D):
+            raise ValueError(f"shard shape {tuple(table.shape)} != {(max(self.rows, 1), self.D)}")
+        self.table, self.slots = table, tuple(slots)
+        self.bot, self.top, self.dense_slots = bot, top, list(dense_slots)
+        if len(self.dense_slots) != len(self.dense_vars()):
+            raise ValueError("dense_slots needs one (s0, s1) pair per Dense kernel and bias")
+        self.graph = DLRMGraph([None] * self.T, bot, top, self.D, self_interaction, mode, loss_kind, clip)
+        self.last = {}          # sizes of the last step: unique rows fetched, rows served to the other ranks
+
+    def dense_vars(self):
+        return [t for w, b, _ in self.bot + self.top for t in (w, b) if t is not None]
+
+    # ---- global <-> shard (tests, checkpoints)
+    def load_global(self, table):
+        """table: the concatenated [G, D] tables (host or device); keeps this rank's rows."""
+        t = torch.as_tensor(np.ascontiguousarray(np.asarray(table)[self.rank::self.world]), dtype=torch.float32)
+        self.table[:self.rows] = t.to(self.table.device)
+
+
+def _dlrm_fetch(parts, xchg, sparses, equal_batches, timer=None):
+    """Steps 1-3 of the sharded DLRM step for every part: bucket, counts / ids / rows exchanges, Z.  -> per part
+    (Z [B, T, D], bucket tuple, send counts, receive counts, requested local rows)."""
+    R = parts[0].world
+    n = len(parts)
+    bk = [p.eng.lookup_bucket(s, p.row_off, R) for p, s in zip(parts, sparses)]
+    if timer:
+        timer("bucket")
+    send = [torch.stack([b[0], torch.full_like(b[0], s.shape[0])], 1) for b, s in zip(bk, sparses)]   # (count, B)
+    recv = [torch.empty_like(x) for x in send]
+    xchg.all_to_all(recv, send, [[1] * R] * n, [[1] * R] * n)
+    host = torch.stack([torch.stack(send), torch.stack(recv)]).cpu()          # the step's one host sync
+    sc = [host[0, k, :, 0].tolist() for k in range(n)]
+    rc = [host[1, k, :, 0].tolist() for k in range(n)]
+    if equal_batches and any(set(host[1, k, :, 1].tolist()) != {sparses[k].shape[0]} for k in range(n)):
+        raise ValueError("every rank must pass the same local batch size to the sharded DLRM step "
+                         f"(got {sorted(set(host[1, :, :, 1].reshape(-1).tolist()))})")
+    if timer:
+        timer("counts")
+    dev = [s.device for s in sparses]
+    req = [torch.empty(sum(r), dtype=torch.int32, device=d) for r, d in zip(rc, dev)]
+    xchg.all_to_all(req, [b[1][:sum(s)] for b, s in zip(bk, sc)], rc, sc)
+    if timer:
+        timer("ids")
+    rows = [p.eng.gather(p.table, q) for p, q in zip(parts, req)]
+    if timer:
+        timer("owner_gather")
+    got = [torch.empty(sum(s), p.D, dtype=torch.float32, device=d) for p, s, d in zip(parts, sc, dev)]
+    xchg.all_to_all(got, rows, sc, rc)
+    if timer:
+        timer("rows")
+    Zs = []
+    for p, b, g, s in zip(parts, bk, got, sparses):
+        B = s.shape[0]
+        if g.shape[0]:
+            Zs.append(p.eng.gather(g, b[2]).view(B, p.T, p.D))     # slot -1 (a bad id) -> the zero row
+        else:
+            Zs.append(torch.zeros(B, p.T, p.D, dtype=torch.float32, device=s.device))
+    for p, s, r in zip(parts, sc, rc):
+        p.last = {"uniq": sum(s), "served": sum(r)}
+    return Zs, bk, sc, rc, req
+
+
+def dlrm_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, timer=None):
+    """One synchronous training step of a row-sharded DLRM on the global batch (the union of every rank's batch; every
+    rank passes the same local batch size).  parts: the DLRMShard of each rank this process drives; xchg: DistExchange
+    or LoopbackExchange; batches[k] = (dense [B, n_dense] f32, sparse [B, T] int32, label [B] f32) of parts[k];
+    opt_args = (kind, lr, eps, beta1, beta2, step).  ``timer(name)``, when given, is called after each phase (the
+    benchmark's per-phase split).  -> per part a [4] device tensor whose [0] is the GLOBAL loss, identical on every rank.
+
+    The embedding rows of the batch are deduplicated before they travel (orx_lookup_bucket), the per-lookup gradient
+    rows are folded onto those unique rows in a fixed order (orx_rows_segment_sum) and each owner's orx_sparse_apply
+    dedups across all ranks' requests -- Keras' sparse apply on the global batch.  The Dense gradients and the loss
+    travel in one all-reduce; every replica then applies the same summed gradient."""
+    R = parts[0].world
+    for p, (dense, sparse, _) in zip(parts, batches):
+        if sparse.dim() != 2 or sparse.shape[1] != p.T:
+            raise ValueError(f"sparse features must be [B, {p.T}]")
+        if sparse.shape[0] < 1 or dense.shape[0] != sparse.shape[0]:
+            raise ValueError("the sharded DLRM step needs B >= 1 samples, with as many dense rows as sparse rows")
+    Zs, bk, sc, rc, req = _dlrm_fetch(parts, xchg, [b[1] for b in batches], True, timer)
+    caches, grads = [], []
+    for p, (dense, sparse, label), Z in zip(parts, batches, Zs):
+        c = p.graph.forward(dense, sparse, label, want_grad=True, Z=Z)
+        c["dpred"].mul_(c_loss / R)                         # Keras' MSE / BCE: a mean over the GLOBAL batch
+        caches.append(c)
+        grads.append(p.graph.backward(c))
+    if timer:
+        timer("fwd_bwd")
+    g_uniq = [p.eng.rows_segment_sum(dZ.view(-1, p.D), b[3], b[4], sum(s))
+              for p, (dZ, _, _), b, s in zip(parts, grads, bk, sc)]
+    if timer:
+        timer("segment_sum")
+    g_rows = [torch.empty(sum(r), p.D, dtype=torch.float32, device=g.device) for p, r, g in zip(parts, rc, g_uniq)]
+    xchg.all_to_all(g_rows, g_uniq, rc, sc)
+    if timer:
+        timer("grad_rows")
+    for p, q, g in zip(parts, req, g_rows):
+        o = p.eng.make_opt(*opt_args)
+        p.eng.sparse_apply(p.eng.make_table(p.table, *p.slots), q, g, o)    # ADAM_DENSE: the owner sweeps its shard
+    if timer:
+        timer("owner_apply")
+    flats = []
+    for (_, bot_g, top_g), c in zip(grads, caches):
+        flats.append(torch.cat([t.reshape(-1) for dw, db in bot_g + top_g for t in (dw, db) if t is not None]
+                               + [c["out4"][:1]]))
+    xchg.all_reduce(flats)
+    outs = []
+    for p, flat, c in zip(parts, flats, caches):
+        o, off = p.eng.make_opt(*opt_args), 0
+        for var, (s0, s1) in zip(p.dense_vars(), p.dense_slots):
+            p.eng.dense_apply(var, s0, s1, flat[off:off + var.numel()].view_as(var), o)
+            off += var.numel()
+        out = c["out4"].clone()
+        out[0] = flat[-1] / R
+        outs.append(out)
+    if timer:
+        timer("dense_allreduce")
+    return outs
+
+
+def dlrm_inference_sharded(parts, xchg, batches):
+    """DLRM.inference of row-sharded tables, a collective call: batches[k] = (dense, sparse) of parts[k], any B >= 0
+    per rank.  -> per part its predictions [B]."""
+    for p, (dense, sparse) in zip(parts, batches):
+        if sparse.dim() != 2 or sparse.shape[1] != p.T or dense.shape[0] != sparse.shape[0]:
+            raise ValueError(f"sparse features must be [B, {p.T}] with as many dense rows")
+    Zs = _dlrm_fetch(parts, xchg, [b[1] for b in batches], False)[0]
+    out = []
+    for p, (dense, sparse), Z in zip(parts, batches, Zs):
+        if dense.shape[0] == 0:
+            out.append(torch.empty(0, dtype=torch.float32, device=dense.device))
+        else:
+            out.append(p.graph.forward(dense, sparse, Z=Z)["pred"])
+    return out
+
+
 class _PeerBuf:
     """A cudaMalloc'd, IPC-exportable device buffer viewed as a torch tensor (orx_peer_alloc)."""
 

@@ -100,15 +100,19 @@ class DLRMGraph:
         self.D, self.self_int, self.mode = m_spa, self_interaction, 0 if mode == "reference" else 1
         self.loss_kind, self.clip = loss_kind, clip
 
-    def forward(self, dense, sparse, label=None, want_grad=False):
+    def forward(self, dense, sparse, label=None, want_grad=False, Z=None):
+        """Z: the embeddings [B, T, D] when the caller has gathered them already (the row-sharded step: rows fetched
+        from their owners); the per-table gathers of ``sparse`` are then skipped."""
         eng = N.engine()
         dev = dense.device
         B, T, D = dense.shape[0], len(self.tables), self.D
         P = interaction_width(T + 1, self.self_int)
         c = {"dense": dense, "sparse": sparse}
-        Z = c["Z"] = torch.empty(B, T, D, dtype=torch.float32, device=dev)
-        for k, tab in enumerate(self.tables):                        # dlrm.py:83-85
-            eng.gather_strided(tab, sparse, k, Z[:, k, :])
+        if Z is None:
+            Z = torch.empty(B, T, D, dtype=torch.float32, device=dev)
+            for k, tab in enumerate(self.tables):                    # dlrm.py:83-85
+                eng.gather_strided(tab, sparse, k, Z[:, k, :])
+        c["Z"] = Z
         top_in = c["top_in"] = _rows(B, D + P, dev)
         x, acts = dense, []
         for l, (w, b, act) in enumerate(self.bot):                   # dlrm.py:87

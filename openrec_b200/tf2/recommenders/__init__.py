@@ -13,8 +13,11 @@ except ImportError:  # pragma: no cover
     pass
 
 
-def __getattr__(name):   # row-sharded BPR / UCML (torch.distributed): imported on demand
+def __getattr__(name):   # row-sharded BPR / UCML / DLRM (torch.distributed): imported on demand
     if name in ("ShardedBPR", "ShardedUCML"):
         from . import sharded
         return getattr(sharded, name)
+    if name == "ShardedDLRM":
+        from .sharded_dlrm import ShardedDLRM
+        return ShardedDLRM
     raise AttributeError(name)

@@ -1,0 +1,126 @@
+"""ShardedDLRM -- the DLRM class surface (openrec/tf2/recommenders/dlrm.py:6-100: same constructor arguments, same
+``model(dense, sparse, label) -> loss``, same GradientTape / ``optimizer.apply_gradients`` step protocol) with the
+embedding tables ROW-SHARDED over the GPUs of a box: one process per GPU under ``torch.distributed``.
+
+The T tables are one concatenated row space (table k starts at row_off[k] = the sum of the vocabularies before it);
+global row g lives on rank ``g % world_size``.  Each rank holds one embedding shard with its optimizer slots, and a
+replica of every Dense layer.  Every rank calls the model with ITS part of the global batch (the same local batch size
+on every rank); ``apply_gradients`` runs one sharded step (openrec_b200.sharded.dlrm_step_sharded) and the loss is that
+of the GLOBAL batch, identical on every rank.  SGD, Adagrad, LazyAdam and Keras ``Adam()`` (each owner sweeps its own
+shard, which is the whole-table sweep).  ``openrec_b200.tf2.checkpoint`` saves one rank's shard and replicas (one file
+per rank)."""
+from __future__ import annotations
+
+import sys
+
+import torch
+import torch.distributed as dist
+
+from ... import native as N
+from ...sharded import DistExchange, DLRMShard, dlrm_inference_sharded, dlrm_step_sharded, row_offsets
+from ...tfshim.core import LazyScalar, StepNode, Tensor, Variable
+from ...tfshim.keras import Model
+from ..mlp_ops import ACT, interaction_width
+from ..modules import MLP
+from .dlrm import DLRM
+
+
+class ShardedDLRM(Model):
+    def __init__(self, m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op="dot", arch_interaction_itself=False,
+                 sigmoid_bot=False, sigmoid_top=True, loss_func="mse", loss_threshold=0.0,
+                 interaction_mode="reference", seed=0):
+        super().__init__()
+        if not dist.is_initialized():
+            raise RuntimeError("ShardedDLRM needs torch.distributed (one process per GPU; world size 1 is allowed)")
+        if arch_interaction_op != "dot" and self._arch_interaction_op != "cat":   # as DLRM: AttributeError (SURVEY Q2)
+            sys.exit("ERROR: arch_interaction_op=" + self._arch_interaction_op + " is not supported")
+        if loss_func not in ("mse", "bce"):
+            sys.exit("ERROR: loss_func=" + loss_func + " is not supported")
+        self._m_spa = int(m_spa)
+        self._vocab = [int(v) for v in ln_emb]
+        self._row_off = row_offsets(self._vocab)
+        self._loss_threshold, self._loss_func = loss_threshold, loss_func
+        self._self_interaction, self._interaction_mode = bool(arch_interaction_itself), interaction_mode
+        self._rank, self._world = dist.get_rank(), dist.get_world_size()
+        eng = self._eng = N.engine()
+        rows = (self._row_off[-1] - self._rank + self._world - 1) // self._world
+        t = torch.empty(max(rows, 1), self._m_spa, dtype=torch.float32, device=eng.device)
+        eng.fill_uniform(t, -0.05, 0.05, seed * 1000003 + self._rank * 17)     # LatentFactor's 'uniform' initializer
+        v = Variable.__new__(Variable)
+        v.t, v.trainable, v.name = t, True, "embedding_shard"
+        self.embedding_shard = v
+        self._mlp_bot = MLP(units_list=ln_bot, out_activation="sigmoid" if sigmoid_bot else "relu")
+        self._mlp_top = MLP(units_list=ln_top, out_activation="sigmoid" if sigmoid_top else "relu")
+        self._xchg = DistExchange()
+
+    def _own_variables(self):
+        return [self.embedding_shard]
+
+    def _orx_step_variables(self):
+        return self.trainable_variables
+
+    def _build(self, n_dense):
+        """Create the Dense layers (keras builds them during the first call) and make every rank's replicas rank 0's."""
+        if self._mlp_bot.layers[0].kernel is not None:
+            return
+        self._mlp_bot.build(n_dense)
+        self._mlp_top.build(self._m_spa + interaction_width(len(self._vocab) + 1, self._self_interaction))
+        for mlp in (self._mlp_bot, self._mlp_top):
+            for layer in mlp.layers:
+                for var in (layer.kernel, layer.bias):
+                    if var is not None:
+                        dist.broadcast(var.t, 0)
+
+    def _part(self, optimizer=None):
+        def layers(mlp):
+            return [(l.kernel.t, None if l.bias is None else l.bias.t, ACT[l.activation]) for l in mlp.layers]
+        dense = [var for mlp in (self._mlp_bot, self._mlp_top) for l in mlp.layers for var in (l.kernel, l.bias)
+                 if var is not None]
+        slots = optimizer.slots(self.embedding_shard) if optimizer is not None else (None, None)
+        dense_slots = [optimizer.slots(var) if optimizer is not None else (None, None) for var in dense]
+        clip = float(self._loss_threshold) if 0.0 < self._loss_threshold < 1.0 else 0.0
+        return DLRMShard(self._eng, self._rank, self._world, self._vocab, self._m_spa, layers(self._mlp_bot),
+                         layers(self._mlp_top), self.embedding_shard.t, slots, dense_slots,
+                         self_interaction=self._self_interaction, mode=self._interaction_mode,
+                         loss_kind=0 if self._loss_func == "mse" else 1, clip=clip)
+
+    def _inputs(self, dense_features, sparse_features, label=None):
+        dense, sparse, lab = DLRM._inputs(dense_features, sparse_features, label)
+        if sparse.dim() != 2 or sparse.shape[1] != len(self._vocab):
+            raise ValueError(f"sparse features must be [B, {len(self._vocab)}] (one id per table)")
+        return dense, sparse, lab
+
+    def call(self, dense_features, sparse_features, label):
+        """-> the loss of the GLOBAL batch (a lazy scalar); this rank contributes the samples it was given."""
+        node = StepNode(self, 1)
+        node.inputs = self._inputs(dense_features, sparse_features, label)
+        self._build(node.inputs[0].shape[1])
+        return LazyScalar(node, {0: 1.0})
+
+    def inference(self, dense_features, sparse_features):
+        """-> this rank's predictions [B].  A collective call: every rank calls it with its own samples (any B >= 0)."""
+        dense, sparse, _ = self._inputs(dense_features, sparse_features)
+        self._build(dense.shape[1])
+        return Tensor(dlrm_inference_sharded([self._part()], self._xchg, [(dense, sparse)])[0])
+
+    def _orx_forward(self, node):
+        raise NotImplementedError("a sharded model's loss exists only as part of the training step "
+                                  "(read it after optimizer.apply_gradients)")
+
+    def _orx_materialize_grad(self, node, var, coef):
+        raise NotImplementedError("explicit IndexedSlices are not available for row-sharded tables")
+
+    def _orx_apply(self, node, grads_and_vars, optimizer):
+        if node.stepped:
+            raise RuntimeError("this model call's gradients were already applied")
+        want = {id(v) for v in self.trainable_variables}
+        coefs = [g.coef for g, _ in grads_and_vars]
+        if {id(v) for _, v in grads_and_vars} != want or any(c != coefs[0] for c in coefs):
+            raise NotImplementedError("apply_gradients: the sharded step needs the gradients of ALL trainable "
+                                      "variables w.r.t. one objective")
+        opt_args = (optimizer._kind, optimizer.learning_rate, optimizer.epsilon, optimizer.beta_1, optimizer.beta_2,
+                    optimizer.iterations)
+        node.out = dlrm_step_sharded([self._part(optimizer)], self._xchg, [node.inputs], opt_args,
+                                     c_loss=float(coefs[0].get(0, 0.0)))[0]
+        node.stepped = True
+        node.inputs = None
