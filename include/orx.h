@@ -110,8 +110,11 @@ enum orx_dispatch_op {
   ORX_OP_SCORE_RANK_SHARD = 7, /* orx_score_rank_shard, phase 2 only: variant RANK_SMEM / RANK_GLOBAL of the local
                                   pass, TA = orx_score_kind, TB = rank, M = Bu, N = local items, K = dim, S = item
                                   splits (0: no local items, no pass launched) */
-  ORX_OP_SCORE_TOPK_SHARD = 8  /* orx_score_topk_shard, phase 1 only: variant TOPK, TA = orx_score_kind, TB = rank,
+  ORX_OP_SCORE_TOPK_SHARD = 8, /* orx_score_topk_shard, phase 1 only: variant TOPK, TA = orx_score_kind, TB = rank,
                                   M = Bu, N = local items, K = dim, S = item splits (0: no local items, no pass) */
+  ORX_OP_POINTWISE_GRAD_ROWS = 9 /* orx_pointwise_grad_rows: variant STEP (k_pgr_step, specialised on D) or
+                                    STEP_GENERIC (k_pgr_generic), TA = orx_point_kind, TB = 0, M = B, N = dim, K = ld,
+                                    S = 1 */
 };
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
@@ -223,7 +226,9 @@ ORX_API int orx_pointwise_grad(orx_handle_t h, int32_t kind, const orx_table_t* 
 ORX_API int orx_sparse_apply(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, const float* values,
                              int32_t n, const orx_opt_t* opt_host, orx_stream_t s);
 /* Same with strided inputs: id i = ids[i*id_stride], value row i = values + i*value_ld (DLRM: ids = sparse[:,k],
- * values = dZ[:,k,:]). */
+ * values = dZ[:,k,:]; the row-sharded pointwise step: one column block of its exchange rows).  Value rows may start at
+ * any float: 128-bit loads are used only when dim, value_ld and values allow them.  Ids outside [0, rows), such as
+ * the -1 of orx_pointwise_serve, are skipped and never enter the batch index. */
 ORX_API int orx_sparse_apply_strided(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
                                      const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt_host,
                                      orx_stream_t s);
@@ -266,6 +271,55 @@ ORX_API int orx_lookup_bucket(orx_handle_t h, const int32_t* sparse, int32_t B, 
                               int32_t* grp_idx, orx_stream_t s);
 ORX_API int orx_rows_segment_sum(orx_handle_t h, const float* src, int64_t src_ld, int32_t dim, const int32_t* grp_off,
                                  const int32_t* grp_idx, int32_t n_uniq, float* out, orx_stream_t s);
+
+/* ---- row-sharded GMF / WRMF (openrec_b200/csrc/orx_pointwise_shard.cu, openrec_b200/sharded.py
+ * pointwise_step_sharded): the user table, the item table and the item bias are row-sharded per table (row r on rank
+ * r % world at local row r / world, as orx_score_rank_shard reads them); GMF's w is replicated.  The step's exchange
+ * runs over one row space built so that ownership matches that layout: with Lu = ceil(U / world), user u is global row
+ * u and item i is global row world*Lu + i, i.e. orx_lookup_bucket with T = 2 and row_off = {0, world*Lu, world*Lu + I};
+ * an owner's local rows < Lu are user rows, the others item rows (item local row + Lu).
+ * orx_pointwise_shard_lookups: lookups [B, 2] int32 (8-byte aligned) = (uid[b], iid[b]) when 0 <= uid[b] < U and
+ *   0 <= iid[b] < I, else (-1, -1) for the whole sample -- the single-device step's rule (a sample with a bad id is
+ *   skipped, and none of its rows is touched), and the rejection of ids in [U, world*Lu), which orx_lookup_bucket
+ *   would accept.  ORX_ERR_INVALID: B < 0, U or I outside [0, 2^31 - 1], a null pointer with B > 0.  B = 0 is a no-op.
+ * orx_pointwise_serve (owner side): for each requested local row req[r], r < n, writes rows[r, 0 .. ld) = the user row
+ *   req[r] (req[r] < local_users) or the item row req[r] - Lu with its bias in column dim (Lu <= req[r] < Lu +
+ *   local_items), zeros elsewhere; user_local[r] / item_local[r] = the row in its own table, -1 where the request
+ *   belongs to the other table (both -1 for a request outside both ranges, with a zero row).  Lu = user_rows_per_rank.
+ *   ORX_ERR_INVALID: dim < 1, ld <= dim, n < 0, Lu < local_users, Lu + local_items > 2^31 - 1, a null pointer with n > 0
+ *   (a shard may be null when its local row count is 0).  n = 0 is a no-op.
+ * orx_pointwise_grad_rows: GMF's BCE-with-logits (kind GMF: the score (u * w) . i + bias) or WRMF's weighted squared
+ *   error (kind WRMF: a, b, use_sigmoid as in orx_pointwise_step) of B samples over fetched rows: sample b reads row
+ *   slot[2b] (user) and row slot[2b+1] (item, its bias in column dim) of `rows` (stride ld); a sample with a negative
+ *   slot is skipped.  Writes, in lookup order, d_rows[2b] = the gradient of c_loss*loss + c_l2*l2_loss w.r.t. the user
+ *   row and d_rows[2b+1] = that w.r.t. the item row with the bias gradient in column dim; padding columns and the rows
+ *   of a skipped sample are zero.  out2 = {loss, l2}: the loss terms summed (GMF: times inv_B, the mean over a batch of
+ *   1 / inv_B samples; the gradient is scaled alike) and 0.5 * the squares of every fetched row of a valid sample
+ *   (duplicates included).  GMF: gw[dim] = this batch's part of w's gradient; with add_w_terms, c_l2 * w is added to gw
+ *   and 0.5 * sum(w^2) to out2[1] -- the sharded step sets it on exactly one rank, so the sum over the ranks holds each
+ *   once.  The arithmetic order is that of orx_pointwise_step's kernels; no atomics: the same inputs give the same bits.
+ *   One dispatch record per call (ORX_OP_POINTWISE_GRAD_ROWS): variant STEP for dim 32 / 64 / 128 / 256 with ld % 4 == 0
+ *   and 16-byte aligned rows, d_rows and w, else STEP_GENERIC.  Scratch: the handle's loss partials buffer, grown to
+ *   (16 + 4 * dim (GMF)) bytes per 64 samples (a growing call synchronises the device).  ORX_ERR_INVALID: unknown kind,
+ *   B < 1, dim outside [1, 1024], ld <= dim, a null rows / slot / label / d_rows / out2, GMF without w or gw, slot not
+ *   8-byte aligned.
+ * orx_rows_scale: x[r, k] = x[r, k] * scale[k] for r < rows, k < dim (x contiguous), one rounding per element -- the
+ *   u * w of orx_score_rank / orx_score_topk with scale = w, so orx_score_rank_shard / orx_score_topk_shard on scaled
+ *   xrows after phase 0's sum give GMF's scores.  rows = 0 is a no-op; ORX_ERR_INVALID: rows < 0, dim < 1, null x /
+ *   scale with rows > 0. */
+ORX_API int orx_pointwise_shard_lookups(orx_handle_t h, const int32_t* uid, const int32_t* iid, int32_t B,
+                                        int64_t total_users, int64_t total_items, int32_t* lookups /*[B, 2]*/,
+                                        orx_stream_t s);
+ORX_API int orx_pointwise_serve(orx_handle_t h, const float* user_shard, const float* item_shard,
+                                const float* bias_shard, int32_t dim, int64_t local_users, int64_t local_items,
+                                int64_t user_rows_per_rank, const int32_t* req, int32_t n, int64_t ld,
+                                float* rows /*[n, ld]*/, int32_t* user_local, int32_t* item_local, orx_stream_t s);
+ORX_API int orx_pointwise_grad_rows(orx_handle_t h, int32_t kind, const float* rows, int64_t ld, int32_t dim,
+                                    const int32_t* slot /*[2B]*/, const float* label, const float* w, int32_t B,
+                                    float a, float b, int32_t use_sigmoid, float c_loss, float c_l2, float inv_B,
+                                    int32_t add_w_terms, float* d_rows /*[2B, ld]*/, float* gw /*[dim]*/,
+                                    float* out2, orx_stream_t s);
+ORX_API int orx_rows_scale(orx_handle_t h, float* x, int64_t rows, int32_t dim, const float* scale, orx_stream_t s);
 
 /* ---- row-sharded BPR / UCML step over the GPUs of one box, "home-routed" (openrec_b200/csrc/orx_shard.cu,
  * openrec_b200/sharded.py).  The reference is single-device: this is the scale-out of the same synchronous step
@@ -422,7 +476,8 @@ ORX_API int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_tab, 
  * uses the evaluation scratch of orx_score_rank and writes one dispatch record (ORX_OP_SCORE_RANK_SHARD).
  * ORX_ERR_INVALID before any device work: local_* that disagree with (total, world, rank), rank outside [0, world),
  * phase outside [0, 3], the size limits of orx_score_rank, a null buffer the phase reads or writes.  Bu = 0 is a no-op.
- * There is no scale argument: no sharded model uses one. */
+ * There is no scale argument: a scaled score (GMF) scales the summed xrows in place with orx_rows_scale between phase 0
+ * and phase 1, which gives orx_score_rank's scores with scale = w bit for bit. */
 typedef struct {
   int32_t world, rank;               /* row r of every table lives on rank r % world at local row r / world */
   int64_t total_users, total_items;  /* global U, I */
@@ -487,7 +542,8 @@ ORX_API int orx_score_topk(orx_handle_t h, int32_t kind, const float* user_tab, 
  * The exchange moves 4 * Bu * dim + 8 * Bu * world * k bytes per call.
  * ORX_ERR_INVALID before any device work: the geometry checks of orx_score_rank_shard, phase outside [0, 2], k outside
  * [1, ORX_MAX_TOPK] (k > total_items is allowed), Bu * world * k > 2^31 - 1, a null buffer the phase reads or writes.
- * Bu = 0 is a no-op.  There is no scale argument: no sharded model uses one. */
+ * Bu = 0 is a no-op.  There is no scale argument: GMF scales the summed xrows with orx_rows_scale between phase 0 and
+ * phase 1, as for orx_score_rank_shard. */
 ORX_API int orx_score_topk_shard(orx_handle_t h, int32_t kind, int32_t phase, const orx_rowshard_t* g_host,
                                  const float* user_shard, const float* item_shard, const float* bias_shard,
                                  int32_t dim, const int32_t* uid, int32_t Bu, const int64_t* excl_off,

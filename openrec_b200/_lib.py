@@ -18,6 +18,7 @@ ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST = 0, 1
 ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE = 0, 1, 2, 3
 ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP = 0, 1, 2, 3, 4
 ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK_SHARD = 5, 6, 7, 8
+ORX_OP_POINTWISE_GRAD_ROWS = 9
 ORX_VARIANT_GEMM_TMA, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_INTERACT = 0, 1, 2, 3
 ORX_VARIANT_STEP, ORX_VARIANT_STEP_PIPE, ORX_VARIANT_STEP_GENERIC = 4, 5, 6
 ORX_VARIANT_RANK_SMEM, ORX_VARIANT_RANK_GLOBAL, ORX_VARIANT_TOPK = 7, 8, 9
@@ -100,6 +101,11 @@ SIGNATURES = {
     "orx_pairwise_grad_rows": [_vp, _i32, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _f, _f, _f, _f, _vp, _vp, _vp],
     "orx_lookup_bucket": [_vp, _vp, _i32, _i32, C.POINTER(_i64), _i32, _vp, _vp, _vp, _vp, _vp, _vp],
     "orx_rows_segment_sum": [_vp, _vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp],
+    "orx_pointwise_shard_lookups": [_vp, _vp, _vp, _i32, _i64, _i64, _vp, _vp],
+    "orx_pointwise_serve": [_vp, _vp, _vp, _vp, _i32, _i64, _i64, _i64, _vp, _i32, _i64, _vp, _vp, _vp, _vp],
+    "orx_pointwise_grad_rows": [_vp, _i32, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _f, _f, _i32, _f, _f, _f, _i32, _vp,
+                                _vp, _vp, _vp],
+    "orx_rows_scale": [_vp, _vp, _i64, _i32, _vp, _vp],
     "orx_pointwise_step": [_vp, _i32, _T, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _i32, _f, _f, _O, _vp, _vp],
     "orx_pointwise_fwd": [_vp, _i32, _T, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _i32, _vp, _vp],
     "orx_pointwise_grad": [_vp, _i32, _T, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _i32, _f, _f,

@@ -117,7 +117,9 @@ __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, flo
   if (id < 0) continue;
   const float* v = vals + (int64_t)b * val_ld;
   const bool own = !SL::STAGE_ONLY && c == 1u;
-  if (((D & 3) == 0) && ((val_ld & 3) == 0)) {   // 128-bit path: all loads of the row first, then the math, then the stores
+  // 128-bit path (value rows 16-byte aligned: a strided view may start mid-row): all loads of the row first, then the
+  // math, then the stores
+  if (((D & 3) == 0) && ((val_ld & 3) == 0) && (((uintptr_t)vals & 15) == 0)) {
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int e = lane * 4; e < D; e += 128) {
       const int64_t off = (int64_t)id * D + e;

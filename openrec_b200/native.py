@@ -9,6 +9,7 @@ import torch
 
 from . import _lib
 from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP,
+                   ORX_OP_POINTWISE_GRAD_ROWS,
                    ORX_OP_SCORE_RANK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_TOPK_SHARD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
                    ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
                    ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
@@ -21,7 +22,8 @@ __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", 
            "ORX_OP_POINTWISE_STEP", "ORX_VARIANT_GEMM_TMA", "ORX_VARIANT_GEMM_SIMT", "ORX_VARIANT_INTERACT_WARP",
            "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC",
            "ORX_OP_SCORE_RANK", "ORX_VARIANT_RANK_SMEM", "ORX_VARIANT_RANK_GLOBAL", "ORX_OP_SCORE_TOPK",
-           "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "ORX_OP_SCORE_TOPK_SHARD", "Dispatch", "RowShard", "rowshard"]
+           "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "ORX_OP_SCORE_TOPK_SHARD", "ORX_OP_POINTWISE_GRAD_ROWS",
+           "Dispatch", "RowShard", "rowshard"]
 
 _engines = {}
 
@@ -296,6 +298,68 @@ class Engine:
                                                    _ptr(pslot), _ptr(nslot), uslot.numel(), margin, c_loss, c_l2,
                                                    inv_B, _ptr(d_rows), _ptr(out4), self.stream()),
                    "orx_pairwise_grad_rows")
+
+    def sparse_apply_rows(self, tab, ids, values, o):
+        """orx_sparse_apply_strided with id i = ids[i] and value row i = values[i] (a 2-D view of any row stride: the
+        row-sharded pointwise step applies the bias column of its exchange rows in place)."""
+        n = ids.numel()
+        if values.shape[0] != n:
+            raise ValueError("one value row per id")
+        _lib.check(self.lib.orx_sparse_apply_strided(self.h, C.byref(tab), _ptr(ids) if n else None, 1,
+                                                     _ptr(values) if n else None, self._ld(values), n, C.byref(o),
+                                                     self.stream()), "orx_sparse_apply_strided")
+
+    # ---- row-sharded pointwise step (orx_pointwise_shard.cu) -------------------------------
+    def pointwise_shard_lookups(self, uid, iid, total_users, total_items):
+        """-> int32 [B, 2] lookups (uid, iid) for orx_lookup_bucket, (-1, -1) for a sample with an id out of range."""
+        B = uid.numel()
+        if iid.numel() != B:
+            raise ValueError("uid and iid must have the same length")
+        out = torch.empty((B, 2), dtype=torch.int32, device=uid.device)
+        _lib.check(self.lib.orx_pointwise_shard_lookups(self.h, _ptr(uid), _ptr(iid), B, int(total_users),
+                                                        int(total_items), _ptr(out), self.stream()),
+                   "orx_pointwise_shard_lookups")
+        return out
+
+    def pointwise_serve(self, user, item, bias, local_users, local_items, user_rows_per_rank, req, ld):
+        """Owner side: -> (rows [n, ld], user_local [n], item_local [n]) for the requested local rows req
+        (orx_pointwise_serve in include/orx.h).  user / item / bias are this rank's shards (bias [rows] or [rows, 1])."""
+        n = req.numel()
+        dev = req.device
+        rows = torch.empty((n, ld), dtype=torch.float32, device=dev)
+        ul = torch.empty(n, dtype=torch.int32, device=dev)
+        il = torch.empty(n, dtype=torch.int32, device=dev)
+        _lib.check(self.lib.orx_pointwise_serve(self.h, _ptr(_f32(user, "user")), _ptr(_f32(item, "item")),
+                                                _ptr(_f32(bias, "bias")), user.shape[1], int(local_users),
+                                                int(local_items), int(user_rows_per_rank), _ptr(req), n, int(ld),
+                                                _ptr(rows), _ptr(ul), _ptr(il), self.stream()), "orx_pointwise_serve")
+        return rows, ul, il
+
+    def pointwise_grad_rows(self, kind, rows, dim, slot, label, w, inv_B, a=1.0, b=1.0, use_sigmoid=False,
+                            c_loss=1.0, c_l2=1.0, add_w_terms=False):
+        """Score, loss and per-lookup gradient rows over fetched rows (orx_pointwise_grad_rows in include/orx.h): rows
+        [*, ld] with the bias in column dim, slot int32 [2B] -> (d_rows [2B, ld], gw [dim] (GMF) or None, out2 [2])."""
+        B = label.numel()
+        if slot.numel() != 2 * B:
+            raise ValueError("slot needs two entries (user, item) per sample")
+        dev, ld = label.device, rows.shape[1]
+        d_rows = torch.empty((2 * B, ld), dtype=torch.float32, device=dev)
+        gw = torch.empty(dim, dtype=torch.float32, device=dev) if kind == ORX_POINT_GMF else None
+        out2 = torch.empty(2, dtype=torch.float32, device=dev)
+        _lib.check(self.lib.orx_pointwise_grad_rows(self.h, kind, _ptr(_f32(rows, "rows")), ld, dim, _ptr(slot),
+                                                    _ptr(_f32(label, "label")), _ptr(w), B, a, b, int(use_sigmoid),
+                                                    c_loss, c_l2, inv_B, int(add_w_terms), _ptr(d_rows), _ptr(gw),
+                                                    _ptr(out2), self.stream()), "orx_pointwise_grad_rows")
+        return d_rows, gw, out2
+
+    def rows_scale(self, x, scale):
+        """In place: x[r, k] *= scale[k], one rounding (orx_rows_scale).  x: contiguous [rows, dim] float32, or an int32
+        tensor holding float bits (the xrows exchange buffer of the shard phases)."""
+        dim = scale.numel()
+        if not x.is_contiguous() or x.numel() % dim:
+            raise ValueError("x must be contiguous with a multiple of scale.numel() elements")
+        _lib.check(self.lib.orx_rows_scale(self.h, _ptr(x), x.numel() // dim, dim, _ptr(_f32(scale, "scale")),
+                                           self.stream()), "orx_rows_scale")
 
     # ---- pointwise ---------------------------------------------------------------------
     def pointwise_step(self, kind, user, item, bias, w, uid, iid, label, o, out4, a=1.0, b=1.0, use_sigmoid=False,

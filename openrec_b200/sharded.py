@@ -123,13 +123,25 @@ class ShardedPairwise:
         return outs
 
 
-def score_rank_sharded(parts, reduce, uid, pos_off, pos_items, excl_off, excl_items, max_pos, at=()):
+def _scale_rows(parts, scale, bufs):
+    """GMF: each part's summed xrows (bufs[k][0], float bits) times its w replica scale[k], in place (orx_rows_scale:
+    the rounding of u * w in orx_score_rank / orx_score_topk)."""
+    if scale is None:
+        return
+    for (eng, *_), sc, b in zip(parts, scale, bufs):
+        if sc is not None:
+            eng.rows_scale(b[0], sc.reshape(-1))
+
+
+def score_rank_sharded(parts, reduce, uid, pos_off, pos_items, excl_off, excl_items, max_pos, at=(), scale=None):
     """Catalogue evaluation (AUC / NDCG / Recall, as native.Engine.score_rank on the global tables) of row-sharded
     tables, each rank counting over its own item rows: the four phases of orx_score_rank_shard, with ``reduce`` between
     them.  parts[k] = (eng, kind, user_shard, item_shard, bias_shard or None, g) for each rank this process drives
     (g: native.RowShard); uid (global user ids) and the global CSR lists live on every part's device.
     ``reduce(tensors)`` replaces each tensor (one per part) in place by its element-wise integer sum over ALL ranks:
     all_reduce_sum(group) when each process is one rank, loopback_sum for virtual ranks on one device.
+    ``scale`` (GMF): one [dim] tensor (or None) per part, the score_rank ``scale`` of the global call; the summed user
+    rows are scaled after phase 0's reduce.
     -> [(auc, ndcg, recall)] per part, identical on every rank."""
     bufs = []
     for eng, kind, user, item, bias, g in parts:
@@ -144,13 +156,15 @@ def score_rank_sharded(parts, reduce, uid, pos_off, pos_items, excl_off, excl_it
                                            excl_items, max_pos, *b, at=at)
         if phase < 3:
             reduce([b[phase] for b in bufs])
+        if phase == 0:
+            _scale_rows(parts, scale, bufs)
     return outs
 
 
-def score_topk_sharded(parts, reduce, uid, excl_off, excl_items, k):
+def score_topk_sharded(parts, reduce, uid, excl_off, excl_items, k, scale=None):
     """Top-K retrieval (the k best unseen items of each user uid, as native.Engine.score_topk on the global tables) of
     row-sharded tables, each rank keeping the k best of its own item rows: the three phases of orx_score_topk_shard,
-    with ``reduce`` between them.  ``parts``, ``reduce``, uid and the global exclusion CSR are as in
+    with ``reduce`` between them.  ``parts``, ``reduce``, uid, the global exclusion CSR and ``scale`` are as in
     score_rank_sharded.  -> [(items int32 [Bu, k], scores float32 [Bu, k])] per part, identical on every rank."""
     Bu, k = uid.numel(), int(k)
     bufs = [(torch.empty(Bu * user.shape[1], dtype=torch.int32, device=item.device),
@@ -162,6 +176,8 @@ def score_topk_sharded(parts, reduce, uid, excl_off, excl_items, k):
             outs[j] = eng.score_topk_shard(kind, phase, g, user, item, bias, uid, excl_off, excl_items, k, *b)
         if phase < 2:
             reduce([b[phase] for b in bufs])
+        if phase == 0:
+            _scale_rows(parts, scale, bufs)
     return outs
 
 
@@ -385,6 +401,139 @@ def dlrm_inference_sharded(parts, xchg, batches):
         else:
             out.append(p.graph.forward(dense, sparse, Z=Z)["pred"])
     return out
+
+
+# ---------------------------------------------------------------------------------------
+# row-sharded GMF / WRMF: user / item / bias rows on their owners, GMF's w replicated
+# ---------------------------------------------------------------------------------------
+class PointwiseShard:
+    """One rank's part of a row-sharded GMF (kind ORX_POINT_GMF) / WRMF (ORX_POINT_WRMF).  Row r of the user table,
+    the item table and the item bias lives on rank r % world at local row r // world: ``user`` [max(ru, 1), dim],
+    ``item`` [max(ri, 1), dim], ``bias`` [max(ri, 1), 1] (a rank without rows keeps a 1-row dummy that is never read),
+    with their optimizer slots (s0, s1 per table, None where the optimizer has fewer).  GMF: ``w`` is this rank's [dim, 1]
+    replica of the Dense(1) kernel with its slots ``w_slots``.  (a, b, use_sigmoid): WRMF's PointwiseMSELoss.
+
+    The exchange runs over one row space whose ownership matches that layout (orx.h, row-sharded GMF / WRMF): user u is
+    global row u, item i is global row world * Lu + i with Lu = ceil(U / world), so one orx_lookup_bucket call over the
+    [B, 2] (user, item) lookups gives every owner one request list."""
+
+    def __init__(self, eng, rank, world, total_users, total_items, dim, kind, user, item, bias, slots, w=None,
+                 w_slots=(None, None), a=1.0, b=1.0, use_sigmoid=False):
+        from . import native as N
+        self.eng, self.rank, self.world, self.kind = eng, rank, world, kind
+        self.U, self.I, self.D = int(total_users), int(total_items), int(dim)
+        self.W = self.D + 4                     # exchange row: D values, the item bias, 3 zeros (16-byte aligned rows)
+        self.Lu = (self.U + world - 1) // world
+        self.row_off = row_offsets([world * self.Lu, self.I])
+        self.ru = (self.U - rank + world - 1) // world
+        self.ri = (self.I - rank + world - 1) // world
+        want = ((max(self.ru, 1), self.D), (max(self.ri, 1), self.D), (max(self.ri, 1), 1))
+        if tuple(tuple(t.shape) for t in (user, item, bias)) != want:
+            raise ValueError(f"shard shapes {[tuple(t.shape) for t in (user, item, bias)]} != {want}")
+        if (kind == N.ORX_POINT_GMF) != (w is not None):
+            raise ValueError("GMF needs its w replica, WRMF has none")
+        self.user, self.item, self.bias = user, item, bias
+        self.user_slots, self.item_slots, self.bias_slots = (tuple(x) for x in slots)
+        self.w, self.w_slots = w, tuple(w_slots)
+        self.a, self.b, self.use_sigmoid = float(a), float(b), bool(use_sigmoid)
+        self.last = {}          # sizes of the last step: unique rows fetched, rows served to the other ranks
+
+    def local_shards(self):
+        return self.user[:self.ru], self.item[:self.ri], self.bias[:self.ri]
+
+    def load_global(self, user, item, bias):
+        """user [U, D], item [I, D], bias [I] or [I, 1] (host or device): keep this rank's rows."""
+        r, R, dev = self.rank, self.world, self.user.device
+        for t, g in zip(self.local_shards(), (user, item, bias)):
+            t.copy_(torch.as_tensor(np.ascontiguousarray(np.asarray(g)[r::R]), dtype=torch.float32)
+                    .reshape(t.shape).to(dev))
+
+
+def pointwise_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, c_l2=1.0, timer=None):
+    """One synchronous training step of a row-sharded GMF / WRMF on the global batch (the union of every rank's batch;
+    every rank passes the same local batch size B >= 1).  parts: the PointwiseShard of each rank this process drives;
+    xchg: DistExchange or LoopbackExchange; batches[k] = (uid int32 [B], iid int32 [B], label f32 [B]) of parts[k],
+    global ids on the device; opt_args = (kind, lr, eps, beta1, beta2, step); (c_loss, c_l2) the coefficients of
+    tape.gradient(c_loss * loss + c_l2 * l2_loss).  ``timer(name)``, when given, is called after each phase.
+    -> per part a [2] device tensor = the GLOBAL (loss, l2_loss), identical on every rank.
+
+    A sample with an id out of range is skipped whole (orx_pointwise_shard_lookups), as orx_pointwise_step skips it; GMF's
+    loss is still the mean over the B * R samples of the global batch.  The batch's rows are deduplicated before they
+    travel (orx_lookup_bucket), the owners pack user / item rows with the item bias in one exchange row
+    (orx_pointwise_serve), the per-lookup gradient rows (orx_pointwise_grad_rows) are folded onto the unique rows in a
+    fixed order (orx_rows_segment_sum), and each owner applies the optimizer to its user, item and bias shards once per
+    row over ALL ranks' requests (orx_sparse_apply_strided; Keras Adam() sweeps each shard).  GMF's w gradient, the loss
+    and l2 travel in one all-reduce, with c_l2 * w and 0.5 * |w|^2 contributed by rank 0 only; every replica then
+    applies the same summed gradient."""
+    from . import native as N
+    R = parts[0].world
+    n = len(parts)
+    for p, (uid, iid, label) in zip(parts, batches):
+        if uid.dim() != 1 or uid.shape != iid.shape or label.shape != uid.shape:
+            raise ValueError("uid, iid and label must be 1-D tensors of one length")
+        if uid.numel() < 1:
+            raise ValueError("the sharded pointwise step needs B >= 1 samples per rank")
+    lks = [p.eng.pointwise_shard_lookups(uid, iid, p.U, p.I) for p, (uid, iid, _) in zip(parts, batches)]
+    bk = [p.eng.lookup_bucket(lk, p.row_off, R) for p, lk in zip(parts, lks)]
+    if timer:
+        timer("bucket")
+    send = [torch.stack([b[0], torch.full_like(b[0], lk.shape[0])], 1) for b, lk in zip(bk, lks)]   # (count, B)
+    recv = [torch.empty_like(x) for x in send]
+    xchg.all_to_all(recv, send, [[1] * R] * n, [[1] * R] * n)
+    host = torch.stack([torch.stack(send), torch.stack(recv)]).cpu()          # the step's one host sync
+    sc = [host[0, k, :, 0].tolist() for k in range(n)]
+    rc = [host[1, k, :, 0].tolist() for k in range(n)]
+    if any(set(host[1, k, :, 1].tolist()) != {lks[k].shape[0]} for k in range(n)):
+        raise ValueError("every rank must pass the same local batch size to the sharded pointwise step "
+                         f"(got {sorted(set(host[1, :, :, 1].reshape(-1).tolist()))})")
+    if timer:
+        timer("counts")
+    dev = [lk.device for lk in lks]
+    req = [torch.empty(sum(r), dtype=torch.int32, device=d) for r, d in zip(rc, dev)]
+    xchg.all_to_all(req, [b[1][:sum(s)] for b, s in zip(bk, sc)], rc, sc)
+    if timer:
+        timer("ids")
+    served = [p.eng.pointwise_serve(p.user, p.item, p.bias, p.ru, p.ri, p.Lu, q, p.W) for p, q in zip(parts, req)]
+    if timer:
+        timer("owner_serve")
+    got = [torch.empty(max(sum(s), 1), p.W, dtype=torch.float32, device=d) for p, s, d in zip(parts, sc, dev)]
+    xchg.all_to_all([g[:sum(s)] for g, s in zip(got, sc)], [x[0] for x in served], sc, rc)
+    if timer:
+        timer("rows")
+    grads = []
+    for p, (_, _, label), b, g in zip(parts, batches, bk, got):
+        grads.append(p.eng.pointwise_grad_rows(p.kind, g, p.D, b[2], label, p.w, 1.0 / (label.numel() * R), p.a, p.b,
+                                               p.use_sigmoid, c_loss, c_l2, add_w_terms=p.rank == 0))
+    if timer:
+        timer("grad_rows")
+    g_uniq = [p.eng.rows_segment_sum(gr[0], b[3], b[4], sum(s)) for p, gr, b, s in zip(parts, grads, bk, sc)]
+    if timer:
+        timer("segment_sum")
+    g_rows = [torch.empty(sum(r), p.W, dtype=torch.float32, device=d) for p, r, d in zip(parts, rc, dev)]
+    xchg.all_to_all(g_rows, g_uniq, rc, sc)
+    if timer:
+        timer("grad_xchg")
+    for p, g, (_, ul, il) in zip(parts, g_rows, served):
+        o = p.eng.make_opt(*opt_args)
+        D = p.D
+        p.eng.sparse_apply_rows(p.eng.make_table(p.user, *p.user_slots), ul, g[:, :D], o)
+        p.eng.sparse_apply_rows(p.eng.make_table(p.item, *p.item_slots), il, g[:, :D], o)
+        p.eng.sparse_apply_rows(p.eng.make_table(p.bias, *p.bias_slots), il, g[:, D:D + 1], o)
+    if timer:
+        timer("owner_apply")
+    gmf = parts[0].kind == N.ORX_POINT_GMF
+    flats = [torch.cat([gr[1], gr[2]]) if gmf else gr[2].clone() for gr in grads]
+    xchg.all_reduce(flats)
+    outs = []
+    for p, flat in zip(parts, flats):
+        if gmf:
+            p.eng.dense_apply(p.w, *p.w_slots, flat[:p.D].view_as(p.w), p.eng.make_opt(*opt_args))
+        outs.append(flat[-2:].clone())
+    if timer:
+        timer("dense_allreduce")
+    for p, s, r in zip(parts, sc, rc):
+        p.last = {"uniq": sum(s), "served": sum(r)}
+    return outs
 
 
 class _PeerBuf:

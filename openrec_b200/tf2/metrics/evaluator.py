@@ -51,15 +51,17 @@ class RankingEvaluator:
         return self._dev[1:]
 
     def evaluate(self, model):
-        """A row-sharded model (ShardedBPR / ShardedUCML) is evaluated collectively: every rank builds the same
-        evaluator and calls evaluate; each rank counts over its own item rows and every rank gets the same result."""
+        """A row-sharded model (ShardedBPR / ShardedUCML / ShardedGMF / ShardedWRMF) is evaluated collectively: every
+        rank builds the same evaluator and calls evaluate; each rank counts over its own item rows and every rank gets
+        the same result."""
         sharded = getattr(model, "_sharded_score_operands", None)
         if sharded is not None:
             return self._evaluate_sharded(*sharded())
         ops = getattr(model, "_score_operands", None)
         if ops is None:
             raise NotImplementedError(f"{type(model).__name__}: catalogue evaluation needs the model's whole item "
-                                      "table on one device (BPR, UCML, GMF, WRMF)")
+                                      "table on one device (BPR, UCML, GMF, WRMF) or its row shards (ShardedBPR, "
+                                      "ShardedUCML, ShardedGMF, ShardedWRMF)")
         kind, user, item, bias, scale = ops()
         uids, pos_off, pos_items, excl_off, excl_items = self._upload(item.device)
         eng = N.engine()
@@ -72,7 +74,7 @@ class RankingEvaluator:
             auc.append(a), ndcg.append(n), rec.append(r)
         return self._result(auc, ndcg, rec, item.device)
 
-    def _evaluate_sharded(self, kind, user, item, bias, g, group):
+    def _evaluate_sharded(self, kind, user, item, bias, g, group, scale=None):
         uids, pos_off, pos_items, excl_off, excl_items = self._upload(item.device)
         part = (N.engine(), kind, user, item, bias, g)
         reduce = all_reduce_sum(group)
@@ -81,7 +83,7 @@ class RankingEvaluator:
             b1 = min(b0 + self.batch_size, len(self.warm_users))
             max_pos = int(self._pos_len[self.warm_users[b0:b1]].max())
             (a, n, r), = score_rank_sharded([part], reduce, uids[b0:b1], pos_off, pos_items, excl_off, excl_items,
-                                            max_pos, at=self.at)
+                                            max_pos, at=self.at, scale=[scale])
             auc.append(a), ndcg.append(n), rec.append(r)
         return self._result(auc, ndcg, rec, item.device)
 

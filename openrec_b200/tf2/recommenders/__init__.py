@@ -13,10 +13,13 @@ except ImportError:  # pragma: no cover
     pass
 
 
-def __getattr__(name):   # row-sharded BPR / UCML / DLRM (torch.distributed): imported on demand
+def __getattr__(name):   # row-sharded BPR / UCML / GMF / WRMF / DLRM (torch.distributed): imported on demand
     if name in ("ShardedBPR", "ShardedUCML"):
         from . import sharded
         return getattr(sharded, name)
+    if name in ("ShardedGMF", "ShardedWRMF"):
+        from . import sharded_pointwise
+        return getattr(sharded_pointwise, name)
     if name == "ShardedDLRM":
         from .sharded_dlrm import ShardedDLRM
         return ShardedDLRM

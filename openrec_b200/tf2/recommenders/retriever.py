@@ -7,9 +7,10 @@ then item id ascending (NaN scores are never returned), cut at k and padded with
 remain.  The union of the positives of ``excl_datasets`` becomes one CSR list over user ids, uploaded once per device.
 The reference's tf2 package has no serving path; its tf1 ``FastDotProductServer`` is the closest counterpart.
 
-A row-sharded model (ShardedBPR / ShardedUCML) is served where its rows live: ``recommend`` is then a collective call
-(orx_score_topk_shard) in which each rank keeps the k best of its own item rows and one merge over the ranks' lists gives
-every rank the result of the single-device call on the gathered tables.  No table row crosses the interconnect."""
+A row-sharded model (ShardedBPR / ShardedUCML / ShardedGMF / ShardedWRMF) is served where its rows live: ``recommend``
+is then a collective call (orx_score_topk_shard) in which each rank keeps the k best of its own item rows and one merge
+over the ranks' lists gives every rank the result of the single-device call on the gathered tables (GMF: the summed
+user rows are scaled by w first, orx_rows_scale).  No table row crosses the interconnect."""
 from __future__ import annotations
 
 import torch
@@ -26,8 +27,8 @@ from ._base import ids_of
 class Retriever:
     """``Retriever(excl_datasets=[train_dataset], k=10, batch_size=1024).recommend(model, user_id)`` -> (items, scores),
     int32 / float32 ``Tensor``s of shape [n, k] on the model's device, n = the number of ids in ``user_id`` (a host or
-    device array of ints of any shape, flattened).  Models: BPR, UCML, GMF, WRMF, and ShardedBPR / ShardedUCML, on which
-    every rank must call ``recommend`` with the same ids and gets the same result."""
+    device array of ints of any shape, flattened).  Models: BPR, UCML, GMF, WRMF, and ShardedBPR / ShardedUCML /
+    ShardedGMF / ShardedWRMF, on which every rank must call ``recommend`` with the same ids and gets the same result."""
 
     def __init__(self, excl_datasets=[], k=10, batch_size=1024):
         k = int(k)
@@ -57,7 +58,7 @@ class Retriever:
         if ops is None:
             raise NotImplementedError(f"{type(model).__name__}: catalogue retrieval needs the model's whole item "
                                       "table on one device (BPR, UCML, GMF, WRMF) or its row shards (ShardedBPR, "
-                                      "ShardedUCML)")
+                                      "ShardedUCML, ShardedGMF, ShardedWRMF)")
         kind, user, item, bias, scale = ops()
         uids = ids_of(user_id)
         excl_off, excl_items = self._upload(item.device)
@@ -69,7 +70,7 @@ class Retriever:
             items.append(it), scores.append(sc)
         return self._result(items, scores, item.device)
 
-    def _recommend_sharded(self, uids, kind, user, item, bias, g, group):
+    def _recommend_sharded(self, uids, kind, user, item, bias, g, group, scale=None):
         # every rank must issue the same batches: unequal id counts would leave some ranks waiting in the exchange
         n = torch.tensor([uids.numel(), -uids.numel()], dtype=torch.int64, device=item.device)
         dist.all_reduce(n, op=dist.ReduceOp.MIN, group=group)
@@ -82,7 +83,8 @@ class Retriever:
         reduce = all_reduce_sum(group)
         items, scores = [], []
         for b0 in range(0, uids.numel(), self.batch_size):
-            (it, sc), = score_topk_sharded([part], reduce, uids[b0:b0 + self.batch_size], excl_off, excl_items, self.k)
+            (it, sc), = score_topk_sharded([part], reduce, uids[b0:b0 + self.batch_size], excl_off, excl_items, self.k,
+                                           scale=[scale])
             items.append(it), scores.append(sc)
         return self._result(items, scores, item.device)
 
