@@ -12,7 +12,7 @@
  *  - every pointer is a DEVICE pointer unless its name ends in _host;
  *  - the caller owns every buffer; the library allocates only the opaque per-device workspace
  *    held by an orx_handle_t (index hash sets and duplicate-row gradient staging, loss partials,
- *    id staging, evaluation scratch, sharded-step scratch, split-K partials), keeps no device
+ *    id staging, evaluation scratch, sharded-step scratch, split-K partials, the sharded censor's dedup hash), keeps no device
  *    state outside it, and orx_destroy frees all of it.  Two handles share nothing;
  *  - all calls are asynchronous w.r.t. the host and ordered on the given stream;
  *  - the calls of one handle that build or use its own batch index (the pairwise and pointwise steps, orx_sparse_apply*,
@@ -83,8 +83,8 @@ ORX_API int orx_destroy(orx_handle_t h);
 ORX_API int orx_device_count(int* n_out_host);
 /* Blocks the host until `stream` has drained (cudaStreamSynchronize). */
 ORX_API int orx_stream_synchronize(orx_handle_t h, orx_stream_t stream);
-/* Test hook: place the epoch of every batch-index table of the handle (index sets 0, 1 and 2) and, once it has run, of
- * orx_shard_step's own index sets (31 bits; each table takes its next epoch at its next build, and the one whose epoch
+/* Test hook: place the epoch of every batch-index table of the handle (index sets 0, 1 and 2), of orx_censor_shard's
+ * dedup hash and, once it has run, of orx_shard_step's own index sets (31 bits; each table takes its next epoch at its next build, and the one whose epoch
  * wraps is emptied on the stream of that build). */
 ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
 /* Test hook: the kernel variants launched by this handle's DLRM entry points (orx_mlp_layer_*, orx_interact_*) and
@@ -112,9 +112,11 @@ enum orx_dispatch_op {
                                   splits (0: no local items, no pass launched) */
   ORX_OP_SCORE_TOPK_SHARD = 8, /* orx_score_topk_shard, phase 1 only: variant TOPK, TA = orx_score_kind, TB = rank,
                                   M = Bu, N = local items, K = dim, S = item splits (0: no local items, no pass) */
-  ORX_OP_POINTWISE_GRAD_ROWS = 9 /* orx_pointwise_grad_rows: variant STEP (k_pgr_step, specialised on D) or
+  ORX_OP_POINTWISE_GRAD_ROWS = 9, /* orx_pointwise_grad_rows: variant STEP (k_pgr_step, specialised on D) or
                                     STEP_GENERIC (k_pgr_generic), TA = orx_point_kind, TB = 0, M = B, N = dim, K = ld,
                                     S = 1 */
+  ORX_OP_CENSOR_SHARD = 10 /* orx_censor_shard, one per call: variant CENSOR_VEC / CENSOR_SCALAR, TA = rank, TB = 0,
+                              M = total ids (n_per_block * n_blocks), N = local_rows, K = dim, S = world */
 };
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
@@ -126,7 +128,9 @@ enum orx_dispatch_variant {
   ORX_VARIANT_STEP_GENERIC = 6,  /* k_pair_generic / k_point_generic (fused-step mode): any D */
   ORX_VARIANT_RANK_SMEM = 7,     /* k_score_rank: thresholds and histograms of a user tile in shared memory */
   ORX_VARIANT_RANK_GLOBAL = 8,   /* k_score_rank: thresholds and histograms in the handle's global scratch */
-  ORX_VARIANT_TOPK = 9           /* k_score_topk + k_topk_merge: candidate lists in the handle's global scratch */
+  ORX_VARIANT_TOPK = 9,          /* k_score_topk + k_topk_merge: candidate lists in the handle's global scratch */
+  ORX_VARIANT_CENSOR_VEC = 10,   /* k_censor_shard, one float4 per lane (dim % 4 == 0 && dim <= 128) */
+  ORX_VARIANT_CENSOR_SCALAR = 11 /* k_censor_shard, lane-strided scalar rows (any other dim) */
 };
 #define ORX_DISPATCH_LOG_CAP 64
 ORX_API int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec_host, int32_t cap, int32_t* n_host);
@@ -159,6 +163,23 @@ ORX_API int orx_gather(orx_handle_t h, const float* tab, int64_t rows, int32_t d
 /* LatentFactor.censor (latent_factor.py:17-23): for the UNIQUE ids, row /= max(||row||_2, min_norm). */
 ORX_API int orx_censor(orx_handle_t h, float* tab, int64_t rows, int32_t dim, const int32_t* ids, int32_t n,
                float min_norm, orx_stream_t s);
+/* LatentFactor.censor (latent_factor.py:17-23) of a ROW-SHARDED table, the kernel of UCML.censor_vec (ucml.py:44-48) on
+ * sharded tables (openrec_b200.sharded.censor_vec_sharded).  Row r of the global [total_rows, dim] table lives on rank
+ * r % world at local row r / world of this rank's shard tab [local_rows, dim].
+ *   ids: n_blocks blocks of n_per_block GLOBAL ids, block b at ids + b * block_stride -- an all-gather of every rank's
+ *        ids: censor_vec packs (u, p, n) as [3][B] per rank, so call c uses ids + c * B with n_per_block = B,
+ *        block_stride = 3B, n_blocks = world; one table's censor uses [world][n] with block_stride = n.
+ *   This rank censors the ids it owns, 0 <= id < total_rows and id % world == rank: over all n_per_block * n_blocks
+ *   ids, each such row once, row /= max(||row||_2, min_norm) with the arithmetic of orx_censor, so the rows of every
+ *   rank together equal orx_censor on the global table and the concatenated ids, bit for bit.  Other ids are skipped.
+ *   local_rows may exceed the rows this rank owns (a 1-row dummy shard of a rank past the table's end is not touched).
+ *   Scratch: the handle's own dedup hash (not index set 0), grown to the largest call; orx_censor_shard calls of one
+ *   handle are ordered among themselves as the index-set calls are.  At most ORX_CENSOR_SHARD_MAX_IDS ids per call.
+ *   One dispatch record per call (ORX_OP_CENSOR_SHARD); a call without ids or owned rows launches nothing. */
+#define ORX_CENSOR_SHARD_MAX_IDS (1 << 28)
+ORX_API int orx_censor_shard(orx_handle_t h, float* tab, int64_t local_rows, int32_t dim, int64_t total_rows,
+                             int32_t world, int32_t rank, const int32_t* ids, int32_t n_per_block, int64_t block_stride,
+                             int32_t n_blocks, float min_norm, orx_stream_t s);
 
 /* ---- pairwise recommenders: BPR (recommenders/bpr.py:21-37 + modules/pairwise_log_loss.py:15-34)
  *      and UCML (recommenders/ucml.py:21-42) ------------------------------------------------

@@ -18,10 +18,12 @@ ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST = 0, 1
 ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE = 0, 1, 2, 3
 ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP = 0, 1, 2, 3, 4
 ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK_SHARD = 5, 6, 7, 8
-ORX_OP_POINTWISE_GRAD_ROWS = 9
+ORX_OP_POINTWISE_GRAD_ROWS, ORX_OP_CENSOR_SHARD = 9, 10
 ORX_VARIANT_GEMM_TMA, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_INTERACT = 0, 1, 2, 3
 ORX_VARIANT_STEP, ORX_VARIANT_STEP_PIPE, ORX_VARIANT_STEP_GENERIC = 4, 5, 6
 ORX_VARIANT_RANK_SMEM, ORX_VARIANT_RANK_GLOBAL, ORX_VARIANT_TOPK = 7, 8, 9
+ORX_VARIANT_CENSOR_VEC, ORX_VARIANT_CENSOR_SCALAR = 10, 11
+ORX_CENSOR_SHARD_MAX_IDS = 1 << 28
 ORX_MAX_AT = 8
 ORX_MAX_TOPK = 1024
 ORX_DISPATCH_LOG_CAP = 64
@@ -76,6 +78,7 @@ SIGNATURES = {
     "orx_fill_uniform": [_vp, _vp, _i64, _f, _f, _u64, _vp],
     "orx_gather": [_vp, _vp, _i64, _i32, _vp, _i32, _i64, _vp, _vp, _vp],
     "orx_censor": [_vp, _vp, _i64, _i32, _vp, _i32, _f, _vp],
+    "orx_censor_shard": [_vp, _vp, _i64, _i32, _i64, _i32, _i32, _vp, _i32, _i64, _i32, _f, _vp],
     "orx_pairwise_step": [_vp, _i32, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _f, _O, _vp, _vp],
     "orx_pairwise_step_host": [_vp, _i32, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _f, _O, _vp, _vp],
     "orx_pairwise_prefetch": [_vp, _T, _T, _vp, _vp, _vp, _i32, _i32, _i32, _vp],

@@ -127,6 +127,9 @@ struct orx_ctx {
   size_t lookup_cap;
   float* splitk;           // split-K partials of the Dense-layer GEMMs and of the split column sum
   size_t splitk_cap;
+  void* censor_ws;         // orx_misc.cu: the dedup hash of orx_censor_shard (slots only), its own allocation
+  size_t censor_cap;
+  OrxHash censor_hash;     // its slots, shape and epoch
 };
 
 // Grow a workspace buffer of the handle to at least `need` bytes (*cap = its size in bytes).  Returns at once when it is

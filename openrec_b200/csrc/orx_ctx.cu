@@ -107,11 +107,12 @@ int orx_take_epoch(OrxHash& t, cudaStream_t st) {
   return ORX_OK;
 }
 
-// test hook: place the epoch of every index table, the handle's and the sharded step's (the wrap tests start them just
-// below 2^31)
+// test hook: place the epoch of every index table, the handle's, orx_censor_shard's and the sharded step's (the wrap
+// tests start them just below 2^31)
 extern "C" int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch) {
   ORX_REQUIRE(h != nullptr && epoch < 0x80000000u, "null handle / epoch must be < 2^31");
   for (OrxIndexSet& s : h->set) s.u.epoch = s.i.epoch = epoch;
+  h->censor_hash.epoch = epoch;
   orx_shard_set_epoch(h, epoch);
   return ORX_OK;
 }
@@ -193,6 +194,7 @@ extern "C" int orx_destroy(orx_handle_t h) {
   cudaFree(h->eval_ws);
   cudaFree(h->lookup_ws);
   cudaFree(h->splitk);
+  cudaFree(h->censor_ws);
   cudaFree(h->shard_scratch);
   orx_shard_ws_release(h);
   if (h->side_stream) {

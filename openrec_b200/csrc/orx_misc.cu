@@ -82,6 +82,46 @@ extern "C" int orx_gather(orx_handle_t h, const float* tab, int64_t rows, int32_
 // LatentFactor.censor (latent_factor.py:17-23), "K10": unique ids via the batch hash (the first
 // warp to insert an id owns the row), row <- row / max(||row||, min_norm).
 // ---------------------------------------------------------------------------------------
+// The censor of up to 8 rows of one warp: lane k < 8 holds row k in my_id (-1: none; other lanes' values are not read).
+// D % 4 == 0 && D <= 128: one float4 per lane, all 8 rows loaded before the first norm is reduced; otherwise one row at
+// a time, lane-strided.  Every lane of the warp calls it.  (The row shape is tested here rather than passed in: so
+// k_censor compiles to the same SASS as before the function was factored out of it.)
+__device__ __forceinline__ void orx_censor_rows8(float* tab, int D, int32_t my_id, float min_norm) {
+  const int lane = threadIdx.x & 31;
+  if ((D & 3) == 0 && D <= 128) {
+    const int nq = D >> 2;
+    float4 v[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int32_t id = __shfl_sync(ORX_FULL, my_id, k);
+      v[k] = (id >= 0 && lane < nq) ? __ldcg(reinterpret_cast<const float4*>(tab + (int64_t)id * D) + lane)
+                                    : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int32_t id = __shfl_sync(ORX_FULL, my_id, k);
+      if (id < 0) continue;
+      float sq = v[k].x * v[k].x + v[k].y * v[k].y + v[k].z * v[k].z + v[k].w * v[k].w;
+      sq = orx_group_sum<32>(sq);
+      const float den = fmaxf(sqrtf(sq), min_norm);
+      if (lane < nq)
+        __stcg(reinterpret_cast<float4*>(tab + (int64_t)id * D) + lane,
+               make_float4(v[k].x / den, v[k].y / den, v[k].z / den, v[k].w / den));
+    }
+  } else {
+    for (int k = 0; k < 8; ++k) {
+      const int32_t id = __shfl_sync(ORX_FULL, my_id, k);
+      if (id < 0) continue;
+      float* row = tab + (int64_t)id * D;
+      float sq = 0.f;
+      for (int e = lane; e < D; e += 32) sq += row[e] * row[e];
+      sq = orx_group_sum<32>(sq);
+      const float den = fmaxf(sqrtf(sq), min_norm);
+      for (int e = lane; e < D; e += 32) row[e] = row[e] / den;
+    }
+  }
+}
+
 // A warp takes 8 ids per iteration: lanes 0..7 load the ids and claim the rows in the hash in parallel, then (128-bit path)
 // all 8 rows are loaded before the first norm is reduced -- one row per warp left the kernel latency-bound (id -> hash ->
 // row -> reduce -> divide -> store: 23 us for 65 536 ids at D = 128, three of them per UCML step).
@@ -89,46 +129,52 @@ __global__ void __launch_bounds__(256) k_censor(float* tab, int64_t rows, int D,
                                                 int n, float min_norm, OrxHash hsh) {
   const int lane = threadIdx.x & 31;
   const int nw = (gridDim.x * blockDim.x) >> 5;
-  const bool vec = (D & 3) == 0 && D <= 128;
   for (int b0 = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 8; b0 < n; b0 += nw * 8) {
     int32_t my_id = -1;
     if (lane < 8 && b0 + lane < n) {
       const int32_t id = ids[b0 + lane];
       if (id >= 0 && (int64_t)id < rows && orx_hash_insert(hsh, id, 2) == 0u) my_id = id;   // first claim owns the row
     }
-    if (vec) {
-      const int nq = D >> 2;
-      float4 v[8];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const int32_t id = __shfl_sync(ORX_FULL, my_id, k);
-        v[k] = (id >= 0 && lane < nq) ? __ldcg(reinterpret_cast<const float4*>(tab + (int64_t)id * D) + lane)
-                                      : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const int32_t id = __shfl_sync(ORX_FULL, my_id, k);
-        if (id < 0) continue;
-        float sq = v[k].x * v[k].x + v[k].y * v[k].y + v[k].z * v[k].z + v[k].w * v[k].w;
-        sq = orx_group_sum<32>(sq);
-        const float den = fmaxf(sqrtf(sq), min_norm);
-        if (lane < nq)
-          __stcg(reinterpret_cast<float4*>(tab + (int64_t)id * D) + lane,
-                 make_float4(v[k].x / den, v[k].y / den, v[k].z / den, v[k].w / den));
-      }
-    } else {
-      for (int k = 0; k < 8; ++k) {
-        const int32_t id = __shfl_sync(ORX_FULL, my_id, k);
-        if (id < 0) continue;
-        float* row = tab + (int64_t)id * D;
-        float sq = 0.f;
-        for (int e = lane; e < D; e += 32) sq += row[e] * row[e];
-        sq = orx_group_sum<32>(sq);
-        const float den = fmaxf(sqrtf(sq), min_norm);
-        for (int e = lane; e < D; e += 32) row[e] = row[e] / den;
-      }
-    }
+    orx_censor_rows8(tab, D, my_id, min_norm);
   }
+}
+
+// LatentFactor.censor on a row-sharded table: this rank censors the ids it owns (id % world == rank, local row
+// id / world) among n GLOBAL ids laid out in blocks of n_per_block, block b at ids + b * block_stride (an all-gather of
+// every rank's ids).  Only about one id in `world` is owned, so a warp reads `chunk` = min(32, 8 world) consecutive ids
+// at once (coalesced; about 8 owned ones, and k_censor's 8 ids per warp at world 1), the owned lanes claim their local
+// row in the dedup hash, and the first claims are compacted into a per-warp queue; every 8 queued rows, and once at the
+// end, go through orx_censor_rows8, the arithmetic of k_censor.
+__global__ void __launch_bounds__(256) k_censor_shard(float* tab, int D, int64_t total_rows, int world, int rank,
+                                                      const int32_t* __restrict__ ids, int n_per_block,
+                                                      int64_t block_stride, int n, int chunk, float min_norm,
+                                                      OrxHash hsh) {
+  __shared__ int32_t queue[8][40];   // < 8 rows left over + up to 32 new claims
+  int32_t* q = queue[threadIdx.x >> 5];
+  const int lane = threadIdx.x & 31;
+  const int nw = (gridDim.x * blockDim.x) >> 5;
+  int qn = 0;
+  for (int t0 = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * chunk; t0 < n; t0 += nw * chunk) {
+    const int t = t0 + lane;
+    int32_t row = -1;
+    if (lane < chunk && t < n) {
+      const int32_t id = ids[(int64_t)(t / n_per_block) * block_stride + t % n_per_block];
+      if (id >= 0 && (int64_t)id < total_rows && id % world == rank && orx_hash_insert(hsh, id / world, 2) == 0u)
+        row = id / world;                                                          // first claim owns the row
+    }
+    const unsigned claim = __ballot_sync(ORX_FULL, row >= 0);
+    if (row >= 0) q[qn + __popc(claim & ((1u << lane) - 1u))] = row;
+    __syncwarp();
+    const int queued = qn + __popc(claim);
+    int head = 0;
+    for (; queued - head >= 8; head += 8) orx_censor_rows8(tab, D, lane < 8 ? q[head + lane] : -1, min_norm);
+    const int32_t rest = lane < queued - head ? q[head + lane] : -1;   // the < 8 rows left move to the queue's front
+    __syncwarp();
+    if (lane < queued - head) q[lane] = rest;
+    __syncwarp();
+    qn = queued - head;
+  }
+  if (qn > 0) orx_censor_rows8(tab, D, lane < qn ? q[lane] : -1, min_norm);
 }
 
 extern "C" int orx_censor(orx_handle_t h, float* tab, int64_t rows, int32_t dim, const int32_t* ids, int32_t n,
@@ -145,6 +191,56 @@ extern "C" int orx_censor(orx_handle_t h, float* tab, int64_t rows, int32_t dim,
   int blocks = (n + 63) / 64;                 // 8 warps x 8 ids per block and iteration
   if (blocks > h->num_sms * 8) blocks = h->num_sms * 8;
   k_censor<<<blocks, 256, 0, st>>>(tab, rows, dim, ids, n, min_norm, ix.u);
+  ORX_LAUNCH_CHECK();
+  return ORX_OK;
+}
+
+// The dedup hash of orx_censor_shard is the handle's censor_ws: slots only (mode-2 inserts stage nothing), as many as
+// orx_hash_shape gives for the largest call so far, all of them in use (so the epoch wrap's clear covers every slot that
+// may hold an old epoch).  It grows on the caller's stream; its epoch carries over, a zeroed slot being empty in any.
+static int censor_hash_for(orx_ctx* c, int64_t lookups, cudaStream_t st) {
+  OrxHash shape;
+  const uint32_t cap = orx_hash_shape(shape, lookups);
+  OrxCarve m = {nullptr, 0};
+  m.take(sizeof(unsigned long long) * cap);
+  if (m.off <= c->censor_cap) return ORX_OK;
+  c->censor_hash.slots = nullptr;
+  int rc = orx_grow(&c->censor_ws, &c->censor_cap, m.off);
+  if (rc) return rc;
+  m = {static_cast<char*>(c->censor_ws), 0};
+  c->censor_hash.slots = (unsigned long long*)m.take(sizeof(unsigned long long) * cap);
+  c->censor_hash.mask = shape.mask;
+  c->censor_hash.shift = shape.shift;
+  ORX_CUDA(cudaMemsetAsync(c->censor_ws, 0, c->censor_cap, st));
+  return ORX_OK;
+}
+
+extern "C" int orx_censor_shard(orx_handle_t h, float* tab, int64_t local_rows, int32_t dim, int64_t total_rows,
+                                int32_t world, int32_t rank, const int32_t* ids, int32_t n_per_block,
+                                int64_t block_stride, int32_t n_blocks, float min_norm, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr, "null handle");
+  ORX_REQUIRE(world >= 1 && rank >= 0 && rank < world, "need world >= 1 and 0 <= rank < world");
+  ORX_REQUIRE(dim > 0 && total_rows >= 0 && local_rows >= 0 && n_per_block >= 0 && n_blocks >= 0, "bad sizes");
+  const int64_t owned = total_rows > rank ? (total_rows - rank + world - 1) / world : 0;
+  ORX_REQUIRE(local_rows >= owned, "local_rows is below the number of rows this rank owns");
+  ORX_REQUIRE(n_blocks <= 1 || block_stride >= n_per_block, "blocks overlap (block_stride < n_per_block)");
+  const int64_t n = (int64_t)n_per_block * n_blocks;
+  ORX_REQUIRE(n <= ORX_CENSOR_SHARD_MAX_IDS, "more than ORX_CENSOR_SHARD_MAX_IDS ids in one call");
+  ORX_REQUIRE((n == 0 || ids) && (owned == 0 || tab), "null pointer");
+  const bool vec = (dim & 3) == 0 && dim <= 128;
+  orx_log_dispatch(h, ORX_OP_CENSOR_SHARD, vec ? ORX_VARIANT_CENSOR_VEC : ORX_VARIANT_CENSOR_SCALAR, rank, 0, (int)n,
+                   (int)(local_rows < INT32_MAX ? local_rows : INT32_MAX), dim, world);
+  if (n == 0 || owned == 0) return ORX_OK;
+  ORX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)s;
+  int rc = censor_hash_for(h, n, st);
+  if (rc) return rc;
+  if ((rc = orx_take_epoch(h->censor_hash, st))) return rc;
+  const int chunk = world >= 4 ? 32 : 8 * world;   // ids per warp and iteration: about 8 of them owned
+  int64_t blocks = (n + 8 * chunk - 1) / (8 * chunk);
+  if (blocks > (int64_t)h->num_sms * 8) blocks = (int64_t)h->num_sms * 8;
+  k_censor_shard<<<(int)blocks, 256, 0, st>>>(tab, dim, total_rows, world, rank, ids, n_per_block, block_stride, (int)n,
+                                              chunk, min_norm, h->censor_hash);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }

@@ -9,7 +9,7 @@ import torch
 
 from . import _lib
 from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP,
-                   ORX_OP_POINTWISE_GRAD_ROWS,
+                   ORX_OP_POINTWISE_GRAD_ROWS, ORX_OP_CENSOR_SHARD, ORX_VARIANT_CENSOR_SCALAR, ORX_VARIANT_CENSOR_VEC,
                    ORX_OP_SCORE_RANK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_TOPK_SHARD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
                    ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
                    ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
@@ -23,7 +23,7 @@ __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", 
            "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC",
            "ORX_OP_SCORE_RANK", "ORX_VARIANT_RANK_SMEM", "ORX_VARIANT_RANK_GLOBAL", "ORX_OP_SCORE_TOPK",
            "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "ORX_OP_SCORE_TOPK_SHARD", "ORX_OP_POINTWISE_GRAD_ROWS",
-           "Dispatch", "RowShard", "rowshard"]
+           "ORX_OP_CENSOR_SHARD", "ORX_VARIANT_CENSOR_VEC", "ORX_VARIANT_CENSOR_SCALAR", "Dispatch", "RowShard", "rowshard"]
 
 _engines = {}
 
@@ -139,6 +139,25 @@ class Engine:
         ids = ids32(ids)
         _lib.check(self.lib.orx_censor(self.h, _ptr(_f32(tab, "tab")), tab.shape[0], tab.shape[1], _ptr(ids),
                                        ids.numel(), min_norm, self.stream()))
+
+    def censor_shard(self, tab, total_rows, world, rank, ids, n_per_block, block_stride, n_blocks, first=0,
+                     min_norm=0.1):
+        """censor of a row-sharded table (orx_censor_shard in include/orx.h): tab is this rank's shard (row r of the
+        global table at local row r // world of rank r % world; a rank without rows passes its 1-row dummy), ids a flat
+        int32 tensor of GLOBAL ids holding n_blocks blocks of n_per_block, block b from element first + b * block_stride.
+        This rank censors each row it owns once."""
+        if not (ids.is_cuda and ids.dtype == torch.int32 and ids.is_contiguous()):
+            raise ValueError("ids: expected a contiguous int32 CUDA tensor")
+        if n_per_block * n_blocks and first + (n_blocks - 1) * block_stride + n_per_block > ids.numel():
+            raise ValueError("the id blocks run past the end of ids")
+        local = max((int(total_rows) - rank + world - 1) // world, 0)
+        if tab.shape[0] < max(local, 1):
+            raise ValueError(f"the shard has {tab.shape[0]} rows; rank {rank} of {world} owns {local}")
+        _lib.check(self.lib.orx_censor_shard(self.h, _ptr(_f32(tab, "tab")), tab.shape[0], tab.shape[1],
+                                             int(total_rows), int(world), int(rank),
+                                             C.c_void_p(ids.data_ptr() + 4 * int(first)), int(n_per_block),
+                                             int(block_stride), int(n_blocks), min_norm, self.stream()),
+                   "orx_censor_shard")
 
     # ---- pairwise ----------------------------------------------------------------------
     def pairwise_step(self, kind, user, item, bias, uid, pid, nid, o, out4, margin=0.5, c_loss=1.0, c_l2=1.0):

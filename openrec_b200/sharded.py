@@ -201,6 +201,42 @@ def loopback_sum(tensors):
 
 
 # ---------------------------------------------------------------------------------------
+# UCML.censor_vec on row-sharded tables
+# ---------------------------------------------------------------------------------------
+def censor_gathered(eng, user, item, total_users, total_items, world, rank, ids, B, min_norm=0.1):
+    """The three censors of UCML.censor_vec (ucml.py:44-48) on one rank's shards, from the all-gathered ids: ids is the
+    flat [world][3][B] int32 block of every rank's (u, p, n).  The user table is censored over every rank's u, then the
+    item table over every p, then over every n (orx_censor_shard, on eng's stream).  user / item: this rank's shards."""
+    for c, (tab, total) in enumerate(((user, total_users), (item, total_items), (item, total_items))):
+        eng.censor_shard(tab, total, world, rank, ids, B, 3 * B, world, first=c * B, min_norm=min_norm)
+
+
+def censor_vec_sharded(eng, user, item, total_users, total_items, world, rank, uid, pid, nid, group=None,
+                       min_norm=0.1):
+    """UCML.censor_vec of row-sharded tables (row r on rank r % world at local row r // world), a COLLECTIVE call: every
+    rank passes its part (uid, pid, nid) of the global batch, int32 GLOBAL ids on the device, and afterwards the shards
+    of all ranks together equal the single-device censor_vec on the concatenation of every rank's ids, bit for bit.
+    Each of the three censors deduplicates over the global ids of that call; an item row in both p and n is censored
+    twice, p first; ids out of range are skipped.
+
+    This rank packs its ids as [3][B], one all-gather (group, torch's current stream) gives every rank the [world][3][B]
+    block, and each rank censors the rows it owns (censor_gathered): 12 B bytes in, 12 world B bytes out, no host sync.
+    Every rank must pass the same B, as in the step; this is not checked (a mismatch leaves the collective hanging)."""
+    B = uid.numel()
+    if pid.numel() != B or nid.numel() != B:
+        raise ValueError("uid, pid and nid must have the same length")
+    if B == 0:
+        return
+    packed = torch.stack([uid.reshape(-1), pid.reshape(-1), nid.reshape(-1)]).to(torch.int32).reshape(-1)
+    if world == 1:
+        ids = packed
+    else:
+        ids = torch.empty(world * 3 * B, dtype=torch.int32, device=packed.device)
+        dist.all_gather_into_tensor(ids, packed, group=group)    # flat [world * 3B]: gloo takes no [world, 3, B] output
+    censor_gathered(eng, user, item, total_users, total_items, world, rank, ids, B, min_norm)
+
+
+# ---------------------------------------------------------------------------------------
 # row-sharded DLRM: embedding rows on their owners, Dense layers replicated
 # ---------------------------------------------------------------------------------------
 def row_offsets(vocab):
@@ -691,6 +727,14 @@ class HomeRoutedPairwise:
         self._announced = tuple(next_ids) if next_ids is not None else None     # also keeps the tensors alive
         return out
 
+    def censor_vec(self, uid, pid, nid):
+        """UCML.censor_vec (ucml.py:44-48) on this model's shards, a collective call (censor_vec_sharded).  Safe after
+        a step that announced the next batch: the announced route / request read no table row, and every later read of
+        a row runs on its owner's stream, behind the owner's censor."""
+        if self._loop is not None:
+            raise RuntimeError("loopback ranks are censored by their LoopbackGroup")
+        censor_vec_sharded(self.eng, self.user, self.item, self.U, self.I, self.world, self.rank, uid, pid, nid)
+
     def check(self):
         """Raise if a flag wait timed out or a mailbox overflowed (sticky device word; one tiny D2H read)."""
         code = int(self._flags()[4 * 64].item())
@@ -815,6 +859,19 @@ class LoopbackGroup:
             m._call(*next_batches[r], c_loss, c_l2, 0, 0, epoch=m.iterations + 1)
         for r, m in enumerate(self.ranks):
             m._call(*next_batches[r], c_loss, c_l2, 1, 1, epoch=m.iterations + 1)
+
+    def censor_vec(self, batches):
+        """UCML.censor_vec of the global batch, batches[r] = (uid, pid, nid) of rank r (the same B for every rank): the
+        [R][3][B] block an all-gather would give, built on the device, then each rank's three orx_censor_shard calls
+        on its own engine and shards -- the kernels of HomeRoutedPairwise.censor_vec."""
+        B = batches[0][0].numel()
+        if any(x.numel() != B for b in batches for x in b):
+            raise ValueError("every rank passes uid, pid and nid of one length B")
+        if B == 0:
+            return
+        ids = torch.cat([torch.stack([x.reshape(-1) for x in b]).to(torch.int32).reshape(-1) for b in batches])
+        for m in self.ranks:
+            censor_gathered(m.eng, m.user, m.item, m.U, m.I, self.world, m.rank, ids, B)
 
     def load_global(self, user, item, bias):
         for m in self.ranks:

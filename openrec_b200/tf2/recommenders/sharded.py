@@ -8,14 +8,20 @@ Every rank calls the model with ITS part of the global batch (any user / item id
 sharded step; the (loss, l2_loss) it returns are those of the GLOBAL batch, identical on every rank.  The model's
 variables are the local shards; the keras optimizer owns the slot tensors, so ``openrec_b200.tf2.checkpoint`` saves and
 restores a rank's shard like any other model (one file per rank).  SGD, Adagrad and LazyAdam (row-sparse Adam; Keras'
-``Adam()`` sweeps whole tables every step and is not offered sharded)."""
+``Adam()`` sweeps whole tables every step and is not offered sharded).
+
+``ShardedUCML.censor_vec(u, p, n)`` -- UCML's training loop is "step, then censor_vec" -- is a collective call too:
+every rank passes its part of the global batch, and each rank censors the rows it owns among every rank's ids, as the
+single-device censor_vec does on the concatenated batch.  ``user_latent_factor.censor(ids)`` / ``item_latent_factor
+.censor(ids)`` (LatentFactor.censor on one sharded table) are collective as well and accept a different number of ids
+per rank."""
 from __future__ import annotations
 
 import torch
 import torch.distributed as dist
 
 from ... import native as N
-from ...sharded import HomeRoutedPairwise
+from ...sharded import HomeRoutedPairwise, censor_vec_sharded
 from ...tfshim.core import LazyScalar, StepNode, Variable
 from ...tfshim.keras import Model
 from ._base import ids_of
@@ -23,11 +29,30 @@ from ._base import ids_of
 
 class _Shard:
     """Stand-in for the LatentFactor attribute of the reference models: ``.embeddings`` / ``.variables[0]`` is this rank's
-    shard ([rows r with r % world == rank, dim])."""
+    shard ([rows r with r % world == rank, dim]) of a table split over the default process group."""
 
     def __init__(self, var, total, dim):
         self.embeddings, self.input_dim, self.output_dim = var, total, dim
         self.variables = self.trainable_variables = [var]
+
+    def censor(self, censor_id):
+        """LatentFactor.censor (latent_factor.py:17-23) of the sharded table, a COLLECTIVE call: the rows of the unique
+        ids of every rank's censor_id <- row / max(||row||, 0.1), in place, each on its owner.  The ranks may pass
+        different numbers of ids: the counts are all-gathered first (one host read) and every rank's ids padded to the
+        largest count with -1, then one all-gather of the ids.  Returns ``embeddings``, as LatentFactor.censor does."""
+        world, rank = dist.get_world_size(), dist.get_rank()
+        ids = ids_of(censor_id)
+        t = self.embeddings.t
+        counts = torch.empty(world, dtype=torch.int32, device=t.device)
+        dist.all_gather_into_tensor(counts, torch.tensor([ids.numel()], dtype=torch.int32, device=t.device))
+        n = int(counts.max().item())
+        if n:
+            padded = torch.full((n,), -1, dtype=torch.int32, device=t.device)
+            padded[:ids.numel()] = ids.to(t.device)
+            gathered = torch.empty(world * n, dtype=torch.int32, device=t.device)
+            dist.all_gather_into_tensor(gathered, padded)
+            N.engine().censor_shard(t, self.input_dim, world, rank, gathered, n, n, world)
+        return self.embeddings
 
 
 class ShardedBPR(Model):
@@ -143,3 +168,13 @@ class ShardedUCML(ShardedBPR):
 
     def _get_margin(self):
         return float(self.margin)
+
+    def censor_vec(self, user_id, p_item_id, n_item_id):
+        """UCML.censor_vec (ucml.py:44-48) on the shards, a COLLECTIVE call: every rank passes its part of the global
+        batch, the same number of ids on every rank, as in the step (not checked: a mismatch leaves the all-gather
+        hanging).  The tables end as the single-device censor_vec leaves them on the concatenation of every rank's ids
+        (openrec_b200.sharded.censor_vec_sharded: one all-gather of the ids, no host sync)."""
+        ids = [ids_of(x) for x in (user_id, p_item_id, n_item_id)]
+        user, item = self.user_latent_factor.embeddings, self.item_latent_factor.embeddings
+        censor_vec_sharded(self._eng, user.t, item.t, self._U, self._I, self._world, self._rank, *ids)
+        return user, item, item
