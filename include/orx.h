@@ -12,7 +12,7 @@
  *  - every pointer is a DEVICE pointer unless its name ends in _host;
  *  - the caller owns every buffer; the library allocates only the opaque per-device workspace
  *    held by an orx_handle_t (index hash sets and duplicate-row gradient staging, loss partials,
- *    id staging, evaluation scratch, sharded-step scratch, split-K partials, the sharded censor's dedup hash), keeps no device
+ *    id staging, evaluation scratch, sharded-step scratch, split-K partials, the sharded censor's dedup hash, the bag apply's compacted ids), keeps no device
  *    state outside it, and orx_destroy frees all of it.  Two handles share nothing;
  *  - all calls are asynchronous w.r.t. the host and ordered on the given stream;
  *  - the calls of one handle that build or use its own batch index (the pairwise and pointwise steps, orx_sparse_apply*,
@@ -253,6 +253,20 @@ ORX_API int orx_sparse_apply(orx_handle_t h, const orx_table_t* tab, const int32
 ORX_API int orx_sparse_apply_strided(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
                                      const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt_host,
                                      orx_stream_t s);
+/* orx_bag_sparse_apply: optimizer.apply_gradients for ONE table of a multi-hot DLRM feature.  Bag b of the table is
+ * sparse[b*ld + col_lo .. b*ld + col_lo + L) (sparse row-major [B, ld] int32); dZ + b*dz_ld is its pooled gradient row.
+ * The IndexedSlices applied hold, for every valid id (0 <= id < rows) of every bag, in (b, l) order, the row
+ * (id, dZ[b]) (mode 0, sum) or (id, dZ[b] / n_b) (mode 1, mean; n_b = the bag's valid ids, IEEE division); padding
+ * (id < 0) and out-of-range ids contribute nothing.  Then Keras sparse semantics as orx_sparse_apply: dedup-then-apply
+ * for SGD / Adagrad / row-sparse Adam, the whole-table sweep for ADAM_DENSE.  With L = 1 and mode 0 this is
+ * orx_sparse_apply_strided(ids = sparse + col_lo, id_stride = ld, values = dZ, value_ld = dz_ld).
+ * Scratch: the index workspace for B*L lookups (the handle's index sets and staging rows, sized per lookup) and the
+ * handle's bag buffer (4 bytes per lookup + 4 per bag).  ORX_ERR_INVALID: null handle / table / opt, a null sparse / dZ
+ * with B > 0, B < 0, L < 1, col_lo < 0, col_lo + L > ld, dz_ld < dim, mode outside {0, 1}, B*L > 2^31 - 1, unknown
+ * optimizer kind or missing slot rows.  B = 0 is a no-op except for the ADAM_DENSE sweep. */
+ORX_API int orx_bag_sparse_apply(orx_handle_t h, const orx_table_t* tab, const int32_t* sparse, int64_t ld,
+                                 int32_t col_lo, int32_t L, int32_t B, const float* dZ, int64_t dz_ld, int32_t mode,
+                                 const orx_opt_t* opt_host, orx_stream_t s);
 /* Combined form used by openrec_b200/sharded.py: each rank stores ONE local table [user rows | item rows] of
  * width ld = D+4 (item bias in column D), so a lookup is (owner, combined local row) whatever its table.
  * orx_owner_bucket_combined: ids = uid | pid | nid (n_user user ids first).  Row r lives on rank r % world at
@@ -399,6 +413,21 @@ ORX_API int orx_dense_apply(orx_handle_t h, float* var, float* s0, float* s1, co
 ORX_API int orx_gather_strided(orx_handle_t h, const float* tab, int64_t rows, int32_t dim, const int32_t* ids,
                                int64_t id_stride, int64_t n, float* out, int64_t out_ld, int32_t* n_bad,
                                orx_stream_t s);
+/* orx_bag_gather: the multi-hot form of the T gathers in ONE launch -- each sparse feature is a bag of ids pooled by a sum
+ *   (mode 0) or a mean (mode 1).  sparse [B, ld] int32 row-major (device); tabs_host[k] / rows_host[k] (host arrays) =
+ *   table k [rows, dim]; col_off_host[T + 1] (host): table k's bag for sample b is sparse[b*ld + col_off[k] ..
+ *   b*ld + col_off[k+1]).  Writes Z[b, k, :] at out + b*out_ld + k*dim.  An id < 0 is padding; an id >= rows[k] is
+ *   counted in *n_bad (device, optional) and adds nothing.  Sum: the valid rows added in column order in fp32, starting
+ *   from the first valid row (a one-id bag copies its row bit for bit, as orx_gather_strided); mean: that sum / the
+ *   bag's valid ids (IEEE division); a bag without a valid id pools to the zero row.  float4 accesses when dim, out_ld,
+ *   out and every table allow them, a scalar path for any dim >= 1.  No atomics on Z: the same inputs give the same bits.
+ *   ORX_ERR_INVALID before any device work: null handle / host arrays / table, a null sparse / out with B > 0, T outside
+ *   [1, ORX_BAG_MAX_TABLES], dim < 1, B < 0, ld < 1, rows[k] < 1, col_off decreasing or outside [0, ld], out_ld < T*dim,
+ *   mode outside {0, 1}.  B = 0 is a no-op. */
+#define ORX_BAG_MAX_TABLES 63   /* T + 1 features (the dense vector last) must fit orx_interact_* (64) */
+ORX_API int orx_bag_gather(orx_handle_t h, const float* const* tabs_host, const int64_t* rows_host, int32_t T,
+                           int32_t dim, const int32_t* sparse, int64_t ld, const int32_t* col_off_host, int32_t B,
+                           int32_t mode, float* out, int64_t out_ld, int32_t* n_bad, orx_stream_t s);
 ORX_API int orx_mlp_layer_fwd(orx_handle_t h, const float* x, int64_t ldx, int32_t B, int32_t in, const float* w,
                               const float* bias, int32_t out, int32_t act, float* y, int64_t ldy, orx_stream_t s);
 ORX_API int orx_mlp_layer_bwd(orx_handle_t h, const float* x, int64_t ldx, const float* y, int64_t ldy, const float* w,

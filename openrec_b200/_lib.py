@@ -25,6 +25,7 @@ ORX_VARIANT_RANK_SMEM, ORX_VARIANT_RANK_GLOBAL, ORX_VARIANT_TOPK = 7, 8, 9
 ORX_VARIANT_CENSOR_VEC, ORX_VARIANT_CENSOR_SCALAR = 10, 11
 ORX_CENSOR_SHARD_MAX_IDS = 1 << 28
 ORX_MAX_AT = 8
+ORX_BAG_MAX_TABLES = 63
 ORX_MAX_TOPK = 1024
 ORX_DISPATCH_LOG_CAP = 64
 
@@ -87,6 +88,9 @@ SIGNATURES = {
     "orx_sparse_apply": [_vp, _T, _vp, _vp, _i32, _O, _vp],
     "orx_sparse_apply_strided": [_vp, _T, _vp, _i64, _vp, _i64, _i32, _O, _vp],
     "orx_gather_strided": [_vp, _vp, _i64, _i32, _vp, _i64, _i64, _vp, _i64, _vp, _vp],
+    "orx_bag_gather": [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _i64, C.POINTER(_i32), _i32, _i32, _vp,
+                       _i64, _vp, _vp],
+    "orx_bag_sparse_apply": [_vp, _T, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _i32, _O, _vp],
     "orx_mlp_layer_fwd": [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _i32, _i32, _vp, _i64, _vp],
     "orx_mlp_layer_bwd": [_vp, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _vp, _vp, _vp],
     "orx_interact_fwd": [_vp, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp],

@@ -130,6 +130,8 @@ struct orx_ctx {
   void* censor_ws;         // orx_misc.cu: the dedup hash of orx_censor_shard (slots only), its own allocation
   size_t censor_cap;
   OrxHash censor_hash;     // its slots, shape and epoch
+  void* bag_ws;            // orx_sharded.cu: orx_bag_sparse_apply's compacted ids and bag counts, its own allocation
+  size_t bag_cap;
 };
 
 // Grow a workspace buffer of the handle to at least `need` bytes (*cap = its size in bytes).  Returns at once when it is

@@ -195,6 +195,7 @@ extern "C" int orx_destroy(orx_handle_t h) {
   cudaFree(h->lookup_ws);
   cudaFree(h->splitk);
   cudaFree(h->censor_ws);
+  cudaFree(h->bag_ws);
   cudaFree(h->shard_scratch);
   orx_shard_ws_release(h);
   if (h->side_stream) {

@@ -598,3 +598,124 @@ extern "C" int orx_pred_loss(orx_handle_t h, const float* pred, const float* lab
   ORX_LAUNCH_CHECK();
   return orx_launch_reduce_partials(h->partials, blocks, 1.0f / (float)B, out4, st);
 }
+
+// ---------------------------------------------------------------------------------------
+// Multi-hot features: Z[b, k, :] = the pooled bag of table k for sample b, all T tables in one launch.  Bag (b, k) is
+// sparse[b*ld + col_off[k] .. col_off[k+1]); an id < 0 is padding, an id >= rows[k] is counted in n_bad; both add nothing.
+// Sum: the valid rows added in column order, starting from the first valid row (so a bag of one id copies its row bit
+// for bit, -0.0 included, like k_gather_strided); mean: that sum / the number of valid ids; no valid id: the zero row.
+// ---------------------------------------------------------------------------------------
+static_assert(ORX_BAG_MAX_TABLES + 1 <= ORX_MAX_F, "the pooled features and the dense vector must fit the interaction");
+
+struct BagTables {   // kernel parameter block: ~1.3 KB, read with register-indexed constant loads
+  const float* tab[ORX_BAG_MAX_TABLES];
+  int64_t rows[ORX_BAG_MAX_TABLES];
+  int32_t col_off[ORX_BAG_MAX_TABLES + 1];
+};
+
+template <bool VEC>
+__device__ __forceinline__ float4 bag_ld(const float* p) {
+  if (VEC) return __ldg(reinterpret_cast<const float4*>(p));
+  return make_float4(__ldg(p), 0.f, 0.f, 0.f);
+}
+
+__device__ __forceinline__ float4 bag_add(float4 a, float4 b) {
+  return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
+}
+
+// One warp per bag, w = b*T + k (consecutive warps fill consecutive Z rows).  VEC: a lane holds one float4 of a
+// 128-float column chunk, else one float of a 32-float chunk; wider rows take several chunks, each re-reading the ids.
+// The ids are read 32 at a time (coalesced); a ballot gives the valid ones, which are taken four at a time: four row
+// loads are issued before they are added, in column order.
+template <bool VEC>
+__global__ void __launch_bounds__(256) k_bag_gather(const __grid_constant__ BagTables bt, int T, int D,
+                                                    const int32_t* __restrict__ sparse, int64_t ld, int64_t B,
+                                                    int mean, float* __restrict__ out, int64_t out_ld,
+                                                    int32_t* n_bad) {
+  constexpr int W = VEC ? 4 : 1;
+  const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < B * T; w += nw) {
+    const int64_t b = w / T;
+    const int k = (int)(w - b * T);
+    const float* tab = bt.tab[k];
+    const int64_t rows = bt.rows[k];
+    const int L = bt.col_off[k + 1] - bt.col_off[k];
+    const int32_t* ids = sparse + b * ld + bt.col_off[k];
+    float* dst = out + b * out_ld + (int64_t)k * D;
+    for (int e0 = 0; e0 < D; e0 += 32 * W) {
+      const int e = e0 + lane * W;
+      const bool on = e < D;
+      float4 acc = z4;
+      int n = 0, bad = 0;
+      for (int c = 0; c < L; c += 32) {
+        const int32_t id = c + lane < L ? __ldg(ids + c + lane) : -1;
+        uint32_t m = __ballot_sync(ORX_FULL, id >= 0 && id < rows);
+        if (e0 == 0) bad += __popc(__ballot_sync(ORX_FULL, id >= rows));
+        while (m) {   // warp-uniform
+          int src[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            src[q] = m ? __ffs(m) - 1 : -1;
+            m &= m - 1;
+          }
+          float4 v[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int64_t r = __shfl_sync(ORX_FULL, id, src[q] & 31);
+            v[q] = (src[q] >= 0 && on) ? bag_ld<VEC>(tab + r * D + e) : z4;
+          }
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            if (src[q] < 0) break;
+            acc = n ? bag_add(acc, v[q]) : v[q];
+            ++n;
+          }
+        }
+      }
+      if (e0 == 0 && lane == 0 && bad && n_bad) atomicAdd(n_bad, bad);
+      if (mean && n) {
+        const float fn = (float)n;
+        acc = make_float4(acc.x / fn, acc.y / fn, acc.z / fn, acc.w / fn);
+      }
+      if (!on) continue;
+      if (VEC) *reinterpret_cast<float4*>(dst + e) = acc;
+      else dst[e] = acc.x;
+    }
+  }
+}
+
+extern "C" int orx_bag_gather(orx_handle_t h, const float* const* tabs_host, const int64_t* rows_host, int32_t T,
+                              int32_t dim, const int32_t* sparse, int64_t ld, const int32_t* col_off_host, int32_t B,
+                              int32_t mode, float* out, int64_t out_ld, int32_t* n_bad, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr && tabs_host && rows_host && col_off_host, "null pointer");
+  ORX_REQUIRE(B == 0 || (sparse && out), "null sparse / out");
+  ORX_REQUIRE(T >= 1 && T <= ORX_BAG_MAX_TABLES, "T outside [1, ORX_BAG_MAX_TABLES]");
+  ORX_REQUIRE(dim >= 1 && B >= 0 && ld >= 1 && (mode == 0 || mode == 1), "bad sizes / mode");
+  ORX_REQUIRE(out_ld >= (int64_t)T * dim, "out_ld < T * dim");
+  ORX_REQUIRE(col_off_host[0] >= 0 && col_off_host[T] <= ld, "col_off outside [0, ld]");
+  BagTables bt;
+  bool aligned = ((uintptr_t)out & 15) == 0;
+  for (int k = 0; k < T; ++k) {
+    ORX_REQUIRE(tabs_host[k] != nullptr && rows_host[k] > 0, "null table / empty vocabulary");
+    ORX_REQUIRE(col_off_host[k + 1] >= col_off_host[k], "col_off decreasing");
+    bt.tab[k] = tabs_host[k];
+    bt.rows[k] = rows_host[k];
+    bt.col_off[k] = col_off_host[k];
+    aligned = aligned && ((uintptr_t)tabs_host[k] & 15) == 0;
+  }
+  bt.col_off[T] = col_off_host[T];
+  if (B == 0) return ORX_OK;
+  ORX_CUDA(cudaSetDevice(h->device));
+  const int64_t bags = (int64_t)B * T;
+  int64_t blocks = (bags + 7) / 8;
+  if (blocks > (int64_t)h->num_sms * 32) blocks = (int64_t)h->num_sms * 32;
+  cudaStream_t st = (cudaStream_t)s;
+  if ((dim & 3) == 0 && (out_ld & 3) == 0 && aligned)
+    k_bag_gather<true><<<(int)blocks, 256, 0, st>>>(bt, T, dim, sparse, ld, B, mode, out, out_ld, n_bad);
+  else
+    k_bag_gather<false><<<(int)blocks, 256, 0, st>>>(bt, T, dim, sparse, ld, B, mode, out, out_ld, n_bad);
+  ORX_LAUNCH_CHECK();
+  return ORX_OK;
+}

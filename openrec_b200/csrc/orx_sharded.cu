@@ -5,6 +5,8 @@
 //                        dedup by row (batch hash), rows hit once are updated straight from their value row,
 //                        duplicated rows are summed in the staging buffer and updated once by the steps' staged-row
 //                        tail, k_sparse_tail ("K8").
+//   * orx_bag_sparse_apply : the same for one table's multi-hot bag lookups (the bag's pooled gradient row, / its valid
+//                        id count for a mean, as each valid id's value row).
 // The reference has no multi-device code (SURVEY 2.1); the partitioning follows SURVEY 8(e).
 #include "orx_common.cuh"
 
@@ -156,29 +158,28 @@ extern "C" int orx_sparse_apply_strided(orx_handle_t h, const orx_table_t* tab, 
   return sparse_apply_impl(h, tab, ids, id_stride, values, value_ld, n, opt, s);
 }
 
-static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
-                             const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt, orx_stream_t s) {
+// The checks every un-fused sparse apply makes before any device work.
+static int sparse_apply_check(orx_handle_t h, const orx_table_t* tab, int64_t n, const orx_opt_t* opt) {
   ORX_REQUIRE(h != nullptr && tab && tab->var && opt, "null pointer");
   ORX_REQUIRE(n >= 0 && tab->rows > 0 && tab->dim > 0, "bad sizes");
   ORX_REQUIRE(orx_opt_kind_ok(opt->kind), "unknown optimizer kind");
   ORX_REQUIRE(orx_opt_slots_ok(opt->kind, {tab}), "optimizer slot rows missing");
-  ORX_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = (cudaStream_t)s;
+  return ORX_OK;
+}
+
+// The rest of an un-fused sparse apply of n lookups whose ids are ids[i * id_stride]: the batch index (mode 1 under
+// ADAM_DENSE), apply(o) -- the launch that updates the rows seen once and stages the others --, the ADAM_DENSE sweeps
+// and the staged-row tail.  The caller has checked the arguments and made the workspace hold n lookups.
+template <typename Apply>
+static int sparse_apply_run(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride, int32_t n,
+                            const orx_opt_t* opt, cudaStream_t st, Apply&& apply) {
   const bool dense = opt->kind == ORX_OPT_ADAM_DENSE;
-  if (n == 0 && !dense) return ORX_OK;
-  ORX_REQUIRE(n == 0 || (ids && values), "null ids/values");
-  const int D = tab->dim;
-  int rc = orx_ensure_workspace(h, n > 0 ? n : 1, D);
-  if (rc) return rc;
   const OrxOptDev o = orx_opt_to_dev(opt);
+  int rc;
   // the user-side hash / staging pair serves as "the" table here
   if (n > 0) {
     if ((rc = orx_launch_index_build_strided(h, ids, id_stride, tab->rows, n, dense, st))) return rc;
-    const int blocks = (n + 63) / 64;   // 8 warps x 8 pairs per block and iteration
-    orx_dispatch_opt(opt->kind, [&](auto O) {
-      k_sparse_apply<decltype(O)::value><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride,
-                                                                 values, value_ld, n, h->set[0].u, h->gu, o);
-    });
+    apply(o);
     ORX_LAUNCH_CHECK();
   }
   if (dense && (rc = orx_launch_adam_sweeps(h, tab, nullptr, nullptr, h->set[0], o, st))) return rc;
@@ -186,4 +187,145 @@ static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32
   TailArgs ta = {orx_sparse_args(h, tab, nullptr, nullptr, h->set[0], o)};
   ta.counters = h->set[0].ctl;
   return orx_launch_tail(h, ta, opt->kind, st);
+}
+
+static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
+                             const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt, orx_stream_t s) {
+  int rc = sparse_apply_check(h, tab, n, opt);
+  if (rc) return rc;
+  ORX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)s;
+  if (n == 0 && opt->kind != ORX_OPT_ADAM_DENSE) return ORX_OK;
+  ORX_REQUIRE(n == 0 || (ids && values), "null ids/values");
+  const int D = tab->dim;
+  if ((rc = orx_ensure_workspace(h, n > 0 ? n : 1, D))) return rc;
+  return sparse_apply_run(h, tab, ids, id_stride, n, opt, st, [&](const OrxOptDev& o) {
+    const int blocks = (n + 63) / 64;   // 8 warps x 8 pairs per block and iteration
+    orx_dispatch_opt(opt->kind, [&](auto O) {
+      k_sparse_apply<decltype(O)::value><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride,
+                                                                 values, value_ld, n, h->set[0].u, h->gu, o);
+    });
+  });
+}
+
+// ---------------------------------------------------------------------------------------
+// bag-aware sparse apply (multi-hot DLRM features): lookup i = (b, l) = (i / L, i % L) of one table
+// ---------------------------------------------------------------------------------------
+// ids_c[b*L + l] = sparse[b*ld + col_lo + l] when it is a valid row, else -1; cnt[b] = the bag's valid ids (mean only).
+// One warp per bag, 32 ids at a time.
+__global__ void __launch_bounds__(256) k_bag_ids(const int32_t* __restrict__ sparse, int64_t ld, int col_lo, int L,
+                                                 int B, int64_t rows, int32_t* __restrict__ ids_c,
+                                                 float* __restrict__ cnt) {
+  const int lane = threadIdx.x & 31;
+  const int nw = (gridDim.x * blockDim.x) >> 5;
+  for (int b = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < B; b += nw) {
+    int n = 0;
+    for (int c = 0; c < L; c += 32) {
+      int32_t id = -1;
+      if (c + lane < L) {
+        id = sparse[(int64_t)b * ld + col_lo + c + lane];
+        if (id >= rows) id = -1;
+        ids_c[(int64_t)b * L + c + lane] = id < 0 ? -1 : id;
+      }
+      n += __popc(__ballot_sync(ORX_FULL, id >= 0));
+    }
+    if (cnt && lane == 0) cnt[b] = (float)n;
+  }
+}
+
+// k_sparse_apply's update over compacted bag lookups: value row i / L, divided by cnt[i / L] for a mean (cnt != null).
+// A separate kernel so that k_sparse_apply's parameter block, and with it its register allocation, stays as it is.
+template <int OPT>
+__global__ void __launch_bounds__(256) k_bag_apply(float* var, float* s0, float* s1, int D,
+                                                   const int32_t* __restrict__ ids, int L,
+                                                   const float* __restrict__ vals, int64_t val_ld,
+                                                   const float* __restrict__ cnt, int n, OrxHash hsh, float* gstage,
+                                                   OrxOptDev o) {
+  typedef OrxOptSlots<OPT> SL;
+  const int lane = threadIdx.x & 31;
+  const int nw = (gridDim.x * blockDim.x) >> 5;
+  const bool vec = ((D & 3) == 0) && ((val_ld & 3) == 0) && (((uintptr_t)vals & 15) == 0);
+  for (int b0 = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 8; b0 < n; b0 += nw * 8) {
+  int32_t my_id = -1;
+  int my_d = -1;
+  uint32_t my_c = 0;
+  float my_nb = 1.f;
+  if (lane < 8 && b0 + lane < n) {
+    my_id = ids[b0 + lane];
+    if (my_id >= 0) {
+      my_c = orx_hash_find(hsh, my_id, &my_d);
+      if (cnt) my_nb = cnt[(b0 + lane) / L];
+    }
+  }
+#pragma unroll 2
+  for (int k = 0; k < 8; ++k) {
+  const int b = b0 + k;
+  if (b >= n) break;
+  const int32_t id = __shfl_sync(ORX_FULL, my_id, k);
+  const uint32_t c = __shfl_sync(ORX_FULL, my_c, k);
+  const int d = __shfl_sync(ORX_FULL, my_d, k);
+  const float nb = __shfl_sync(ORX_FULL, my_nb, k);
+  if (id < 0) continue;
+  const float* v = vals + (int64_t)(b / L) * val_ld;
+  const bool own = !SL::STAGE_ONLY && c == 1u;
+  if (vec) {
+    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int e = lane * 4; e < D; e += 128) {
+      const int64_t off = (int64_t)id * D + e;
+      float4 g = __ldcg(reinterpret_cast<const float4*>(v + e));
+      if (cnt) g = make_float4(g.x / nb, g.y / nb, g.z / nb, g.w / nb);
+      const float4 wv = own ? __ldcg(reinterpret_cast<const float4*>(var + off)) : z4;
+      float4 a = (SL::S0 && own) ? __ldcg(reinterpret_cast<const float4*>(s0 + off)) : z4;
+      float4 bb = (SL::S1 && own) ? __ldcg(reinterpret_cast<const float4*>(s1 + off)) : z4;
+      orx_own_or_stage4<OPT, false>(own, var, s0, s1, id, gstage, d, D, e, wv, g, a, bb, o);
+    }
+  } else {
+    for (int e = lane; e < D; e += 32) {
+      const int64_t off = (int64_t)id * D + e;
+      const float g = cnt ? v[e] / nb : v[e];
+      if (own) orx_update1<OPT>(var + off, s0 + off, s1 + off, var[off], g, o);
+      else atomicAdd(gstage + (int64_t)d * D + e, g);
+    }
+  }
+  }
+  }
+}
+
+extern "C" int orx_bag_sparse_apply(orx_handle_t h, const orx_table_t* tab, const int32_t* sparse, int64_t ld,
+                                    int32_t col_lo, int32_t L, int32_t B, const float* dZ, int64_t dz_ld, int32_t mode,
+                                    const orx_opt_t* opt, orx_stream_t s) {
+  const int64_t n64 = (int64_t)B * L;
+  int rc = sparse_apply_check(h, tab, B, opt);
+  if (rc) return rc;
+  ORX_REQUIRE(L >= 1 && col_lo >= 0 && (int64_t)col_lo + L <= ld, "bag columns outside [0, ld)");
+  ORX_REQUIRE(dz_ld >= tab->dim && (mode == 0 || mode == 1), "dz_ld < dim / unknown mode");
+  ORX_REQUIRE(n64 <= 0x7fffffff, "B * L > 2^31 - 1");
+  ORX_REQUIRE(B == 0 || (sparse && dZ), "null sparse / dZ");
+  ORX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)s;
+  if (B == 0 && opt->kind != ORX_OPT_ADAM_DENSE) return ORX_OK;
+  const int n = (int)n64, D = tab->dim;
+  if ((rc = orx_ensure_workspace(h, n > 0 ? n : 1, D))) return rc;
+  int32_t* ids_c = nullptr;
+  float* cnt = nullptr;
+  if (n > 0) {
+    OrxCarve m = {nullptr, 0};
+    m.take(sizeof(int32_t) * (size_t)n);
+    m.take(sizeof(float) * (size_t)B);
+    if ((rc = orx_grow(&h->bag_ws, &h->bag_cap, m.off))) return rc;
+    m = {static_cast<char*>(h->bag_ws), 0};
+    ids_c = (int32_t*)m.take(sizeof(int32_t) * (size_t)n);
+    cnt = mode == 1 ? (float*)m.take(sizeof(float) * (size_t)B) : nullptr;
+    int blocks = (B + 7) / 8;
+    if (blocks > h->num_sms * 32) blocks = h->num_sms * 32;
+    k_bag_ids<<<blocks, 256, 0, st>>>(sparse, ld, col_lo, L, B, tab->rows, ids_c, cnt);
+    ORX_LAUNCH_CHECK();
+  }
+  return sparse_apply_run(h, tab, ids_c, 1, n, opt, st, [&](const OrxOptDev& o) {
+    const int blocks = (n + 63) / 64;
+    orx_dispatch_opt(opt->kind, [&](auto O) {
+      k_bag_apply<decltype(O)::value><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, D, ids_c, L, dZ, dz_ld, cnt,
+                                                              n, h->set[0].u, h->gu, o);
+    });
+  });
 }

@@ -240,6 +240,37 @@ class Engine:
                                                C.c_void_p(ids2d.data_ptr() + 4 * col), F, n, _ptr(out2d),
                                                self._ld(out2d), None, self.stream()), "orx_gather_strided")
 
+    def bag_gather(self, tabs, sparse, col_off, mode, out2d, n_bad=None):
+        """Multi-hot lookup of every table in one launch (orx_bag_gather in include/orx.h): sparse int32 [B, C] on the
+        device, col_off [T + 1] host ints (table k's bag = columns col_off[k] .. col_off[k+1]), mode 0 sum / 1 mean;
+        out2d [B, >= T*D] (any row stride) gets Z[b, k, :] at columns k*D .. (k+1)*D."""
+        T = len(tabs)
+        if sparse.dtype != torch.int32 or sparse.dim() != 2 or sparse.stride(1) != 1:
+            raise ValueError("sparse: expected an int32 [B, C] tensor with unit inner stride")
+        if len(col_off) != T + 1:
+            raise ValueError("col_off must have T + 1 entries")
+        B = sparse.shape[0]
+        ptrs = (C.c_void_p * T)(*[t.data_ptr() for t in tabs])
+        rows = (C.c_int64 * T)(*[t.shape[0] for t in tabs])
+        off = (C.c_int32 * (T + 1))(*[int(x) for x in col_off])
+        _lib.check(self.lib.orx_bag_gather(self.h, ptrs, rows, T, tabs[0].shape[1] if T else 0,
+                                           _ptr(sparse) if B else None, max(sparse.stride(0), 1), off, B, int(mode),
+                                           _ptr(out2d) if B else None, self._ld(out2d), _ptr(n_bad), self.stream()),
+                   "orx_bag_gather")
+
+    def bag_sparse_apply(self, tab, sparse, col_lo, L, dz2d, mode, o):
+        """optimizer.apply_gradients of one table's bag lookups (orx_bag_sparse_apply): bag b = sparse[b, col_lo :
+        col_lo + L], its pooled gradient row dz2d[b] ([B, D], any row stride), mode 0 sum / 1 mean."""
+        B = sparse.shape[0]
+        if sparse.dtype != torch.int32 or sparse.dim() != 2 or sparse.stride(1) != 1:
+            raise ValueError("sparse: expected an int32 [B, C] tensor with unit inner stride")
+        if dz2d.shape[0] != B:
+            raise ValueError("one gradient row per bag")
+        _lib.check(self.lib.orx_bag_sparse_apply(self.h, C.byref(tab), _ptr(sparse) if B else None,
+                                                 max(sparse.stride(0), 1), int(col_lo), int(L), B,
+                                                 _ptr(dz2d) if B else None, self._ld(dz2d), int(mode), C.byref(o),
+                                                 self.stream()), "orx_bag_sparse_apply")
+
     def mlp_fwd(self, x, w, bias, act, y):
         _lib.check(self.lib.orx_mlp_layer_fwd(self.h, _ptr(x), self._ld(x), x.shape[0], w.shape[0], _ptr(w), _ptr(bias),
                                               w.shape[1], act, _ptr(y), self._ld(y), self.stream()),

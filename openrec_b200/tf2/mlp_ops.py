@@ -1,6 +1,6 @@
 """Dense / interaction operators behind keras Dense, MLP and SecondOrderFeatureInteraction, and the
 DLRM forward/backward composition -- all arithmetic in liborx (orx_mlp_layer_*, orx_interact_*,
-orx_gather_strided, orx_pred_loss); this module only sequences launches and owns activations."""
+orx_gather_strided / orx_bag_gather, orx_pred_loss); this module only sequences launches and owns activations."""
 from __future__ import annotations
 
 import torch
@@ -95,10 +95,13 @@ class DLRMGraph:
     Z [B,T,D] embeddings, top_in [B, D+P] = (dense_vec | interactions) written in place by the last
     bottom layer and the interaction kernel."""
 
-    def __init__(self, tables, bot, top, m_spa, self_interaction, mode, loss_kind, clip):
+    def __init__(self, tables, bot, top, m_spa, self_interaction, mode, loss_kind, clip, col_off=None, pooling=0):
+        """col_off: the multi-hot bag layout (table k's bag = sparse columns col_off[k] .. col_off[k+1]), pooled by a
+        sum (pooling 0) or a mean (1); None: one id per table, sparse [B, T]."""
         self.tables, self.bot, self.top = tables, bot, top          # lists of tensors / (w, b, act) triples
         self.D, self.self_int, self.mode = m_spa, self_interaction, 0 if mode == "reference" else 1
         self.loss_kind, self.clip = loss_kind, clip
+        self.col_off, self.pooling = col_off, pooling
 
     def forward(self, dense, sparse, label=None, want_grad=False, Z=None):
         """Z: the embeddings [B, T, D] when the caller has gathered them already (the row-sharded step: rows fetched
@@ -110,8 +113,11 @@ class DLRMGraph:
         c = {"dense": dense, "sparse": sparse}
         if Z is None:
             Z = torch.empty(B, T, D, dtype=torch.float32, device=dev)
-            for k, tab in enumerate(self.tables):                    # dlrm.py:83-85
-                eng.gather_strided(tab, sparse, k, Z[:, k, :])
+            if self.col_off is not None:                             # dlrm.py:83-85, one pooled bag per table
+                eng.bag_gather(self.tables, sparse, self.col_off, self.pooling, Z.view(B, T * D))
+            else:
+                for k, tab in enumerate(self.tables):                # dlrm.py:83-85
+                    eng.gather_strided(tab, sparse, k, Z[:, k, :])
         c["Z"] = Z
         top_in = c["top_in"] = _rows(B, D + P, dev)
         x, acts = dense, []

@@ -1,10 +1,12 @@
 """DLRM -- mirrors openrec/tf2/recommenders/dlrm.py:6-100 on liborx (gathers, interaction, Dense layers,
-loss, sparse + dense optimizer applies); same lazy step protocol as the other recommenders."""
+loss, sparse + dense optimizer applies); same lazy step protocol as the other recommenders.  ``bag_sizes`` adds
+multi-hot sparse features (a pooled bag of ids per table), which the reference does not have."""
 import sys
 
 import torch
 
 from ... import native as N
+from ..._lib import ORX_BAG_MAX_TABLES
 from ...tfshim.core import LazyScalar, StepNode, Tensor, convert
 from ...tfshim.keras import Model
 from ..mlp_ops import ACT, DLRMGraph
@@ -14,10 +16,31 @@ from ..modules import MLP, LatentFactor, SecondOrderFeatureInteraction
 class DLRM(Model):
     def __init__(self, m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op="dot", arch_interaction_itself=False,
                  sigmoid_bot=False, sigmoid_top=True, loss_func="mse", loss_threshold=0.0,
-                 interaction_mode="reference"):
+                 interaction_mode="reference", bag_sizes=None, pooling="sum"):
         """Reference signature (dlrm.py:8-19) + ``interaction_mode``: 'reference' reproduces the reference's
-        dot interaction bit for bit (identically zero, SURVEY Q1), 'dlrm' is the strictly-lower triangle."""
+        dot interaction bit for bit (identically zero, SURVEY Q1), 'dlrm' is the strictly-lower triangle.
+
+        ``bag_sizes = [L_0 .. L_{T-1}]`` makes every sparse feature multi-hot: ``sparse_features`` is then [B, sum(L)],
+        table k's bag for sample b being columns sum(L[:k]) .. sum(L[:k+1]) - 1 of row b, pooled by ``pooling`` ('sum'
+        or 'mean' over the bag's valid ids).  An id < 0 is padding; an id >= the vocabulary adds nothing and gets no
+        gradient; a bag without a valid id pools to the zero row.  None (the default): one id per table, [B, T]."""
         super().__init__()
+        if pooling not in ("sum", "mean"):
+            raise ValueError(f"pooling must be 'sum' or 'mean', got {pooling!r}")
+        self._col_off = None
+        if bag_sizes is not None:
+            sizes = [int(L) for L in bag_sizes]
+            if len(sizes) != len(ln_emb):
+                raise ValueError(f"bag_sizes has {len(sizes)} entries for {len(ln_emb)} embedding tables")
+            if any(L < 1 for L in sizes):
+                raise ValueError("every bag size must be >= 1")
+            if len(sizes) > ORX_BAG_MAX_TABLES:
+                raise ValueError(f"multi-hot DLRM takes at most {ORX_BAG_MAX_TABLES} tables")
+            self._col_off = [0]
+            for L in sizes:
+                self._col_off.append(self._col_off[-1] + L)
+        self._bag_sizes = None if bag_sizes is None else sizes
+        self._pooling = 0 if pooling == "sum" else 1
         self._m_spa = int(m_spa)
         self._loss_threshold = loss_threshold
         self._loss_func = loss_func
@@ -48,7 +71,14 @@ class DLRM(Model):
         clip = float(self._loss_threshold) if 0.0 < self._loss_threshold < 1.0 else 0.0
         return DLRMGraph([lf.embeddings.t for lf in self._latent_factors], layers(self._mlp_bot),
                          layers(self._mlp_top), self._m_spa, self._self_interaction, self._interaction_mode,
-                         0 if self._loss_func == "mse" else 1, clip)
+                         0 if self._loss_func == "mse" else 1, clip, self._col_off, self._pooling)
+
+    def _checked_inputs(self, dense_features, sparse_features, label=None):
+        dense, sparse, lab = self._inputs(dense_features, sparse_features, label)
+        if self._col_off is not None and (sparse.dim() != 2 or sparse.shape[1] != self._col_off[-1]):
+            raise ValueError(f"sparse_features must be [B, {self._col_off[-1]}] (the sum of bag_sizes), got "
+                             f"{tuple(sparse.shape)}")
+        return dense, sparse, lab
 
     @staticmethod
     def _inputs(dense_features, sparse_features, label=None):
@@ -60,13 +90,13 @@ class DLRM(Model):
     def call(self, dense_features, sparse_features, label):
         """-> loss (a single lazy scalar, dlrm.py:63-74)."""
         node = StepNode(self, 1)
-        node.inputs = self._inputs(dense_features, sparse_features, label)
+        node.inputs = self._checked_inputs(dense_features, sparse_features, label)
         self._graph(node.inputs[0].shape[1])   # keras builds the Dense layers during the first call
         return LazyScalar(node, {0: 1.0})
 
     def inference(self, dense_features, sparse_features):
         """-> predictions [B] (dlrm.py:76-100)."""
-        dense, sparse, _ = self._inputs(dense_features, sparse_features)
+        dense, sparse, _ = self._checked_inputs(dense_features, sparse_features)
         return Tensor(self._graph(dense.shape[1]).forward(dense, sparse)["pred"])
 
     # ---- step protocol hooks (openrec_b200/tfshim/core.py)
@@ -99,7 +129,11 @@ class DLRM(Model):
         c, (dZ, bot_g, top_g) = self._fwd_bwd(node, float(coefs[0].get(0, 0.0)))
         eng, o = N.engine(), optimizer.opt_struct()
         for k, lf in enumerate(self._latent_factors):                 # IndexedSlices(ids = sparse[:,k], dZ[:,k,:])
-            eng.sparse_apply_strided(optimizer.table(lf.embeddings), sparse, k, dZ, o)
+            if self._col_off is None:
+                eng.sparse_apply_strided(optimizer.table(lf.embeddings), sparse, k, dZ, o)
+            else:                                                     # ... of every valid id of table k's bags
+                eng.bag_sparse_apply(optimizer.table(lf.embeddings), sparse, self._col_off[k], self._bag_sizes[k],
+                                     dZ[:, k, :], self._pooling, o)
         for mlp, grads in ((self._mlp_bot, bot_g), (self._mlp_top, top_g)):
             for layer, (dw, db) in zip(mlp.layers, grads):
                 eng.dense_apply(layer.kernel.t, *optimizer.slots(layer.kernel), dw, o)
@@ -112,10 +146,11 @@ class DLRM(Model):
     def _launches_per_step(self):
         """liborx kernel launches of one training step (bench.py's gpu_launches): per table gather + index / apply / tail,
         per Dense layer forward (1) + backward (activation, column sum, dgrad, wgrad; split-K adds a reduce) + 2 dense
-        applies, 2 interaction kernels, 1 loss kernel."""
+        applies, 2 interaction kernels, 1 loss kernel.  Multi-hot: one gather launch for all tables, and per table id
+        compaction / index / apply / tail."""
         T = len(self._latent_factors)
         n_dense = len(self._mlp_bot.layers) + len(self._mlp_top.layers)
-        return 4 * T + n_dense * (1 + 4 + 2) + 2 + 1
+        return (4 * T if self._col_off is None else 1 + 4 * T) + n_dense * (1 + 4 + 2) + 2 + 1
 
     def _orx_materialize_grad(self, node, var, coef):
         if node.stepped:
@@ -123,7 +158,9 @@ class DLRM(Model):
         _, (dZ, bot_g, top_g) = self._fwd_bwd(node, float(coef.get(0, 0.0)))
         for k, lf in enumerate(self._latent_factors):
             if var is lf.embeddings:
-                return Tensor(node.inputs[1][:, k].contiguous()), Tensor(dZ[:, k, :].contiguous())
+                if self._col_off is None:
+                    return Tensor(node.inputs[1][:, k].contiguous()), Tensor(dZ[:, k, :].contiguous())
+                return self._bag_slices(node.inputs[1], k, dZ[:, k, :])
         for mlp, grads in ((self._mlp_bot, bot_g), (self._mlp_top, top_g)):
             for layer, (dw, db) in zip(mlp.layers, grads):
                 if var is layer.kernel:
@@ -131,3 +168,14 @@ class DLRM(Model):
                 if var is layer.bias:
                     return None, Tensor(db)
         raise KeyError("variable does not belong to this model")
+
+    def _bag_slices(self, sparse, k, dz):
+        """IndexedSlices of table k's bags: the valid ids in (b, l) order, each with its bag's gradient row dz[b]
+        (divided by the bag's valid-id count for a mean) -- what orx_bag_sparse_apply applies."""
+        lo, L = self._col_off[k], self._bag_sizes[k]
+        ids = sparse[:, lo:lo + L]
+        valid = (ids >= 0) & (ids < self._latent_factors[k].embeddings.t.shape[0])
+        rows = dz.unsqueeze(1).expand(-1, L, -1)
+        if self._pooling == 1:
+            rows = rows / valid.sum(1).clamp_min(1).to(torch.float32).view(-1, 1, 1)
+        return Tensor(ids[valid].contiguous()), Tensor(rows[valid].contiguous())
