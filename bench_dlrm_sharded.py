@@ -27,7 +27,7 @@ from bench_eval import card  # noqa: E402
 from bench_eval_sharded import slowest, timed  # noqa: E402
 from openrec_b200.sharded import dlrm_step_sharded  # noqa: E402
 
-PHASES = ["bucket", "counts", "ids", "owner_gather", "rows", "fwd_bwd", "segment_sum", "grad_rows", "owner_apply",
+PHASES = ["bucket", "counts", "ids", "owner_serve", "rows", "fwd_bwd", "segment_sum", "grad_xchg", "owner_apply",
           "dense_allreduce"]
 
 

@@ -192,6 +192,13 @@ static inline bool orx_opt_kind_ok(int kind) { return kind >= ORX_OPT_SGD && kin
 // s1 for both Adams (ADAM_DENSE's sweep keeps m and v there).  Null tables are skipped.
 bool orx_opt_slots_ok(int kind, std::initializer_list<const orx_table_t*> tabs);
 
+// Grid of a grid-stride loop over n items: one thread per item, at most 32 blocks per SM, at least one block.
+static inline int orx_grid_for(int64_t n, int threads, int num_sms) {
+  const int64_t b = (n + threads - 1) / threads;
+  const int64_t cap = (int64_t)num_sms * 32;
+  return (int)(b < 1 ? 1 : (b < cap ? b : cap));
+}
+
 // ---------------------------------------------------------------------------------------
 // device helpers
 // ---------------------------------------------------------------------------------------

@@ -36,12 +36,6 @@ size_t lookup_layout(char* base, int64_t n, int T, int R, size_t tmp_bytes, Look
   return m.off;
 }
 
-int grid_for(int64_t n, int threads, int num_sms) {
-  int64_t b = (n + threads - 1) / threads;
-  const int64_t cap = (int64_t)num_sms * 32;
-  return (int)(b < cap ? b : cap);
-}
-
 }  // namespace
 
 // key of lookup i = b * T + k: a valid id maps to owner * L + local row (L = ceil(G / R) local rows at most per rank), so
@@ -145,7 +139,7 @@ extern "C" int orx_lookup_bucket(orx_handle_t h, const int32_t* sparse, int32_t 
   lookup_layout(static_cast<char*>(h->lookup_ws), n, T, world, tmp_bytes, &w);
   ORX_CUDA(cudaMemcpyAsync(w.row_off, row_off_host, sizeof(int64_t) * (size_t)(T + 1), cudaMemcpyHostToDevice, st));
 
-  const int grid = grid_for(n, 256, h->num_sms);
+  const int grid = orx_grid_for(n, 256, h->num_sms);
   k_lb_keys<<<grid, 256, 0, st>>>(sparse, n, T, w.row_off, world, L, w.keys_in, w.iota);
   ORX_LAUNCH_CHECK();
   size_t bytes = w.tmp_bytes;   // radix sort is stable: a unique row's lookups stay in ascending i

@@ -11,16 +11,6 @@
 // rows < Lu are user rows, the rest item rows (item local row + Lu).
 #include "orx_common.cuh"
 
-namespace {
-
-int pgr_grid(int64_t n, int threads, int num_sms) {
-  int64_t b = (n + threads - 1) / threads;
-  const int64_t cap = (int64_t)num_sms * 32;
-  return (int)(b < 1 ? 1 : (b < cap ? b : cap));
-}
-
-}  // namespace
-
 __global__ void __launch_bounds__(256) k_pw_lookups(const int32_t* __restrict__ uid, const int32_t* __restrict__ iid,
                                                     int B, int64_t U, int64_t I, int32_t* __restrict__ out) {
   for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < B; t += gridDim.x * blockDim.x) {
@@ -40,8 +30,8 @@ extern "C" int orx_pointwise_shard_lookups(orx_handle_t h, const int32_t* uid, c
   ORX_REQUIRE(uid && iid && lookups, "null pointer");
   ORX_REQUIRE(((uintptr_t)lookups & 7) == 0, "lookups must be 8-byte aligned");
   ORX_CUDA(cudaSetDevice(h->device));
-  k_pw_lookups<<<pgr_grid(B, 256, h->num_sms), 256, 0, (cudaStream_t)s>>>(uid, iid, B, total_users, total_items,
-                                                                          lookups);
+  k_pw_lookups<<<orx_grid_for(B, 256, h->num_sms), 256, 0, (cudaStream_t)s>>>(uid, iid, B, total_users,
+                                                                              total_items, lookups);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
@@ -97,7 +87,7 @@ extern "C" int orx_pointwise_serve(orx_handle_t h, const float* user_shard, cons
   cudaStream_t st = (cudaStream_t)s;
   const bool vec = (ld & 3) == 0 && ((uintptr_t)rows & 15) == 0;
   const int64_t work = (int64_t)n * (vec ? ld / 4 : ld);
-  const int grid = pgr_grid(work, 256, h->num_sms);
+  const int grid = orx_grid_for(work, 256, h->num_sms);
   if (vec)
     k_pw_serve<4><<<grid, 256, 0, st>>>(user_shard, item_shard, bias_shard, dim, local_users, local_items,
                                         user_rows_per_rank, req, n, ld, rows, user_local, item_local);
@@ -403,7 +393,7 @@ extern "C" int orx_rows_scale(orx_handle_t h, float* x, int64_t rows, int32_t di
   ORX_REQUIRE(x && scale, "null pointer");
   ORX_CUDA(cudaSetDevice(h->device));
   const int64_t n = rows * dim;
-  k_rows_scale<<<pgr_grid(n, 256, h->num_sms), 256, 0, (cudaStream_t)s>>>(x, n, dim, scale);
+  k_rows_scale<<<orx_grid_for(n, 256, h->num_sms), 256, 0, (cudaStream_t)s>>>(x, n, dim, scale);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }

@@ -23,7 +23,8 @@ __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", 
            "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC",
            "ORX_OP_SCORE_RANK", "ORX_VARIANT_RANK_SMEM", "ORX_VARIANT_RANK_GLOBAL", "ORX_OP_SCORE_TOPK",
            "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "ORX_OP_SCORE_TOPK_SHARD", "ORX_OP_POINTWISE_GRAD_ROWS",
-           "ORX_OP_CENSOR_SHARD", "ORX_VARIANT_CENSOR_VEC", "ORX_VARIANT_CENSOR_SCALAR", "Dispatch", "RowShard", "rowshard"]
+           "ORX_OP_CENSOR_SHARD", "ORX_VARIANT_CENSOR_VEC", "ORX_VARIANT_CENSOR_SCALAR", "Dispatch", "RowShard", "rowshard",
+           "shard_rows"]
 
 _engines = {}
 
@@ -35,10 +36,16 @@ Dispatch = namedtuple("Dispatch", "op variant ta tb m n k s")
 RowShard = namedtuple("RowShard", "world rank total_users total_items local_users local_items")
 
 
+def shard_rows(total, rank, world):
+    """The local row count of `rank` in the row-sharded layout of a `total`-row table: ceil((total - rank) / world),
+    0 for a rank past the table's end.  A rank without rows stores a 1-row dummy: its shard has max(rows, 1) rows."""
+    return max((int(total) - rank + world - 1) // world, 0)
+
+
 def rowshard(world, rank, total_users, total_items):
-    """RowShard of `rank`: local_* = ceil((total - rank) / world) (0 for a rank past the table's end)."""
-    return RowShard(world, rank, total_users, total_items, (total_users - rank + world - 1) // world,
-                    (total_items - rank + world - 1) // world)
+    """RowShard of `rank` (local_* from shard_rows)."""
+    return RowShard(world, rank, total_users, total_items, shard_rows(total_users, rank, world),
+                    shard_rows(total_items, rank, world))
 
 
 def _ptr(t):
@@ -150,7 +157,7 @@ class Engine:
             raise ValueError("ids: expected a contiguous int32 CUDA tensor")
         if n_per_block * n_blocks and first + (n_blocks - 1) * block_stride + n_per_block > ids.numel():
             raise ValueError("the id blocks run past the end of ids")
-        local = max((int(total_rows) - rank + world - 1) // world, 0)
+        local = shard_rows(total_rows, rank, world)
         if tab.shape[0] < max(local, 1):
             raise ValueError(f"the shard has {tab.shape[0]} rows; rank {rank} of {world} owns {local}")
         _lib.check(self.lib.orx_censor_shard(self.h, _ptr(_f32(tab, "tab")), tab.shape[0], tab.shape[1],

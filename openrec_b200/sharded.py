@@ -25,16 +25,37 @@ import json
 import os
 import sys
 import time
+from collections import namedtuple
 
 import numpy as np
 import torch
 import torch.distributed as dist
 
 from . import _lib
+from .native import shard_rows
 
 
 def _a2a(out, inp, out_splits, in_splits):
     dist.all_to_all_single(out, inp, output_split_sizes=out_splits, input_split_sizes=in_splits)
+
+
+def take_shard(global_rows, rank, world):
+    """Rows rank, rank + world, ... of a global table (numpy or torch, host or device): the shard_rows(total, rank,
+    world) rows `rank` owns in the row-sharded layout, as a float32 tensor where the input lives."""
+    if isinstance(global_rows, torch.Tensor):
+        return global_rows[rank::world].to(torch.float32)
+    return torch.as_tensor(np.ascontiguousarray(np.asarray(global_rows)[rank::world]), dtype=torch.float32)
+
+
+def gather_shards(t, total, world, group=None):
+    """The global [total, cols] table on every rank from each rank's local rows t ([shard_rows(total, rank, world),
+    cols]), a collective call over ``group`` (test and checkpoint helper; sizes must be small)."""
+    per = (total + world - 1) // world
+    pad = torch.zeros(per, t.shape[1], dtype=t.dtype, device=t.device)
+    pad[:t.shape[0]] = t
+    parts = [torch.empty_like(pad) for _ in range(world)]
+    dist.all_gather(parts, pad, group=group)
+    return torch.stack(parts, 1).reshape(per * world, t.shape[1])[:total]     # row = local * world + rank
 
 
 class ShardedPairwise:
@@ -55,8 +76,7 @@ class ShardedPairwise:
         self.kind, self.opt_kind, self.lr, self.eps, self.b1, self.b2, self.margin = kind, opt_kind, lr, eps, beta1, beta2, margin
         self.iterations = 0
         dev = eng.device
-        self.ru = (total_users - rank + world - 1) // world     # rows r with r % world == rank
-        self.ri = (total_items - rank + world - 1) // world
+        self.ru, self.ri = shard_rows(total_users, rank, world), shard_rows(total_items, rank, world)
         self.table = torch.zeros(self.ru + self.ri, self.W, dtype=torch.float32, device=dev)
         if init:
             tmp = torch.empty(self.ru + self.ri, dim + 1, dtype=torch.float32, device=dev)
@@ -104,23 +124,16 @@ class ShardedPairwise:
     # ---- helpers for tests: assemble / scatter the global tables
     def load_global(self, user, item, bias):
         r, R, D = self.rank, self.world, self.D
-        self.table[:self.ru, :D] = torch.as_tensor(user[r::R], dtype=torch.float32)
-        self.table[self.ru:, :D] = torch.as_tensor(item[r::R], dtype=torch.float32)
-        self.table[self.ru:, D] = torch.as_tensor(bias[r::R], dtype=torch.float32).reshape(-1)
+        self.table[:self.ru, :D] = take_shard(user, r, R)
+        self.table[self.ru:, :D] = take_shard(item, r, R)
+        self.table[self.ru:, D] = take_shard(bias, r, R).reshape(-1)
 
     def gather_global(self):
         """-> (user, item, bias) full tables on every rank (test helper; sizes must be small)."""
         D = self.D
-        outs = []
-        for t, total in ((self.table[:self.ru, :D], self.U), (self.table[self.ru:, :D], self.I),
-                         (self.table[self.ru:, D:D + 1], self.I)):
-            per = (total + self.world - 1) // self.world
-            pad = torch.zeros(per, t.shape[1], dtype=t.dtype, device=t.device)
-            pad[:t.shape[0]] = t
-            parts = [torch.empty_like(pad) for _ in range(self.world)]
-            dist.all_gather(parts, pad)
-            outs.append(torch.stack(parts, 1).reshape(per * self.world, t.shape[1])[:total])   # row = local*R + rank
-        return outs
+        return [gather_shards(t, total, self.world) for t, total in
+                ((self.table[:self.ru, :D], self.U), (self.table[self.ru:, :D], self.I),
+                 (self.table[self.ru:, D:D + 1], self.I))]
 
 
 def _scale_rows(parts, scale, bufs):
@@ -302,7 +315,7 @@ class DLRMShard:
         self.eng, self.rank, self.world, self.D = eng, rank, world, int(dim)
         self.row_off = row_offsets(vocab)
         self.T, self.G = len(vocab), self.row_off[-1]
-        self.rows = (self.G - rank + world - 1) // world
+        self.rows = shard_rows(self.G, rank, world)
         if tuple(table.shape) != (max(self.rows, 1), self.D):
             raise ValueError(f"shard shape {tuple(table.shape)} != {(max(self.rows, 1), self.D)}")
         self.table, self.slots = table, tuple(slots)
@@ -318,51 +331,83 @@ class DLRMShard:
     # ---- global <-> shard (tests, checkpoints)
     def load_global(self, table):
         """table: the concatenated [G, D] tables (host or device); keeps this rank's rows."""
-        t = torch.as_tensor(np.ascontiguousarray(np.asarray(table)[self.rank::self.world]), dtype=torch.float32)
-        self.table[:self.rows] = t.to(self.table.device)
+        self.table[:self.rows] = take_shard(table, self.rank, self.world)
 
 
-def _dlrm_fetch(parts, xchg, sparses, equal_batches, timer=None):
-    """Steps 1-3 of the sharded DLRM step for every part: bucket, counts / ids / rows exchanges, Z.  -> per part
-    (Z [B, T, D], bucket tuple, send counts, receive counts, requested local rows)."""
+# ---- the deduplicated row exchange of the sharded DLRM and GMF / WRMF steps
+_Fetched = namedtuple("_Fetched", "bucket send recv req served got")
+
+
+def _untimed(name):
+    pass
+
+
+def _fetch_rows(parts, xchg, lookups, serve, width, equal_batches, timer=None):
+    """Fetch every part's unique rows from their owners.  parts[k] has .eng, .world and .row_off; lookups[k] is its
+    int32 [B, T] global-row lookups; serve(part, req) is the owner's reply to the requested local rows req: the rows
+    [len(req), width] first, then whatever the caller keeps.  Runs orx_lookup_bucket, the (count, B) exchange with the
+    step's one host sync (and, with equal_batches, the check that every rank passed the same B), the ids exchange,
+    serve and the rows exchange.  -> per part a _Fetched: the lookup_bucket tuple, the send / receive counts per rank,
+    req, serve's result and got [max(n, 1), width], whose first n = sum(send) rows are the unique rows in bucket order
+    (never empty: orx_pointwise_grad_rows needs a rows pointer)."""
+    timer = timer or _untimed
     R = parts[0].world
     n = len(parts)
-    bk = [p.eng.lookup_bucket(s, p.row_off, R) for p, s in zip(parts, sparses)]
-    if timer:
-        timer("bucket")
-    send = [torch.stack([b[0], torch.full_like(b[0], s.shape[0])], 1) for b, s in zip(bk, sparses)]   # (count, B)
+    bk = [p.eng.lookup_bucket(lk, p.row_off, R) for p, lk in zip(parts, lookups)]
+    timer("bucket")
+    send = [torch.stack([b[0], torch.full_like(b[0], lk.shape[0])], 1) for b, lk in zip(bk, lookups)]   # (count, B)
     recv = [torch.empty_like(x) for x in send]
     xchg.all_to_all(recv, send, [[1] * R] * n, [[1] * R] * n)
     host = torch.stack([torch.stack(send), torch.stack(recv)]).cpu()          # the step's one host sync
     sc = [host[0, k, :, 0].tolist() for k in range(n)]
     rc = [host[1, k, :, 0].tolist() for k in range(n)]
-    if equal_batches and any(set(host[1, k, :, 1].tolist()) != {sparses[k].shape[0]} for k in range(n)):
-        raise ValueError("every rank must pass the same local batch size to the sharded DLRM step "
+    if equal_batches and any(set(host[1, k, :, 1].tolist()) != {lookups[k].shape[0]} for k in range(n)):
+        raise ValueError("every rank must pass the same local batch size to a sharded step "
                          f"(got {sorted(set(host[1, :, :, 1].reshape(-1).tolist()))})")
-    if timer:
-        timer("counts")
-    dev = [s.device for s in sparses]
+    timer("counts")
+    dev = [lk.device for lk in lookups]
     req = [torch.empty(sum(r), dtype=torch.int32, device=d) for r, d in zip(rc, dev)]
     xchg.all_to_all(req, [b[1][:sum(s)] for b, s in zip(bk, sc)], rc, sc)
-    if timer:
-        timer("ids")
-    rows = [p.eng.gather(p.table, q) for p, q in zip(parts, req)]
-    if timer:
-        timer("owner_gather")
-    got = [torch.empty(sum(s), p.D, dtype=torch.float32, device=d) for p, s, d in zip(parts, sc, dev)]
-    xchg.all_to_all(got, rows, sc, rc)
-    if timer:
-        timer("rows")
+    timer("ids")
+    served = [serve(p, q) for p, q in zip(parts, req)]
+    timer("owner_serve")
+    got = [torch.empty(max(sum(s), 1), width, dtype=torch.float32, device=d) for s, d in zip(sc, dev)]
+    xchg.all_to_all([g[:sum(s)] for g, s in zip(got, sc)], [x[0] for x in served], sc, rc)
+    timer("rows")
+    return [_Fetched(*f) for f in zip(bk, sc, rc, req, served, got)]
+
+
+def _return_grads(parts, xchg, fetched, d_rows, timer=None):
+    """Send the gradients of fetched rows back to their owners: d_rows[k] holds parts[k]'s per-lookup gradient rows
+    (row i for lookup i); orx_rows_segment_sum folds them onto the unique rows in a fixed order, and one exchange takes
+    those to the owners.  Sets each part's .last.  -> per part the gradient rows [len(req), width] of the rows it
+    served, in req's order."""
+    timer = timer or _untimed
+    g_uniq = [p.eng.rows_segment_sum(d, f.bucket[3], f.bucket[4], sum(f.send))
+              for p, d, f in zip(parts, d_rows, fetched)]
+    timer("segment_sum")
+    g_rows = [torch.empty(sum(f.recv), g.shape[1], dtype=torch.float32, device=g.device)
+              for f, g in zip(fetched, g_uniq)]
+    xchg.all_to_all(g_rows, g_uniq, [f.recv for f in fetched], [f.send for f in fetched])
+    timer("grad_xchg")
+    for p, f in zip(parts, fetched):
+        p.last = {"uniq": sum(f.send), "served": sum(f.recv)}
+    return g_rows
+
+
+def _dlrm_fetch(parts, xchg, sparses, equal_batches, timer=None):
+    """The row fetch of the sharded DLRM step and inference: _fetch_rows with the owners gathering the requested rows
+    of their shard, then Z = the fetched rows of every lookup.  -> (Z [B, T, D] per part, the _Fetched per part)."""
+    fetched = _fetch_rows(parts, xchg, sparses, lambda p, req: (p.eng.gather(p.table, req),), parts[0].D,
+                          equal_batches, timer)
     Zs = []
-    for p, b, g, s in zip(parts, bk, got, sparses):
+    for p, f, s in zip(parts, fetched, sparses):
         B = s.shape[0]
-        if g.shape[0]:
-            Zs.append(p.eng.gather(g, b[2]).view(B, p.T, p.D))     # slot -1 (a bad id) -> the zero row
+        if sum(f.send):
+            Zs.append(p.eng.gather(f.got, f.bucket[2]).view(B, p.T, p.D))     # slot -1 (a bad id) -> the zero row
         else:
             Zs.append(torch.zeros(B, p.T, p.D, dtype=torch.float32, device=s.device))
-    for p, s, r in zip(parts, sc, rc):
-        p.last = {"uniq": sum(s), "served": sum(r)}
-    return Zs, bk, sc, rc, req
+    return Zs, fetched
 
 
 def dlrm_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, timer=None):
@@ -376,34 +421,26 @@ def dlrm_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, timer=None):
     rows are folded onto those unique rows in a fixed order (orx_rows_segment_sum) and each owner's orx_sparse_apply
     dedups across all ranks' requests -- Keras' sparse apply on the global batch.  The Dense gradients and the loss
     travel in one all-reduce; every replica then applies the same summed gradient."""
+    timer = timer or _untimed
     R = parts[0].world
     for p, (dense, sparse, _) in zip(parts, batches):
         if sparse.dim() != 2 or sparse.shape[1] != p.T:
             raise ValueError(f"sparse features must be [B, {p.T}]")
         if sparse.shape[0] < 1 or dense.shape[0] != sparse.shape[0]:
             raise ValueError("the sharded DLRM step needs B >= 1 samples, with as many dense rows as sparse rows")
-    Zs, bk, sc, rc, req = _dlrm_fetch(parts, xchg, [b[1] for b in batches], True, timer)
+    Zs, fetched = _dlrm_fetch(parts, xchg, [b[1] for b in batches], True, timer)
     caches, grads = [], []
     for p, (dense, sparse, label), Z in zip(parts, batches, Zs):
         c = p.graph.forward(dense, sparse, label, want_grad=True, Z=Z)
         c["dpred"].mul_(c_loss / R)                         # Keras' MSE / BCE: a mean over the GLOBAL batch
         caches.append(c)
         grads.append(p.graph.backward(c))
-    if timer:
-        timer("fwd_bwd")
-    g_uniq = [p.eng.rows_segment_sum(dZ.view(-1, p.D), b[3], b[4], sum(s))
-              for p, (dZ, _, _), b, s in zip(parts, grads, bk, sc)]
-    if timer:
-        timer("segment_sum")
-    g_rows = [torch.empty(sum(r), p.D, dtype=torch.float32, device=g.device) for p, r, g in zip(parts, rc, g_uniq)]
-    xchg.all_to_all(g_rows, g_uniq, rc, sc)
-    if timer:
-        timer("grad_rows")
-    for p, q, g in zip(parts, req, g_rows):
+    timer("fwd_bwd")
+    g_rows = _return_grads(parts, xchg, fetched, [dZ.view(-1, p.D) for p, (dZ, _, _) in zip(parts, grads)], timer)
+    for p, f, g in zip(parts, fetched, g_rows):
         o = p.eng.make_opt(*opt_args)
-        p.eng.sparse_apply(p.eng.make_table(p.table, *p.slots), q, g, o)    # ADAM_DENSE: the owner sweeps its shard
-    if timer:
-        timer("owner_apply")
+        p.eng.sparse_apply(p.eng.make_table(p.table, *p.slots), f.req, g, o)    # ADAM_DENSE: the owner sweeps its shard
+    timer("owner_apply")
     flats = []
     for (_, bot_g, top_g), c in zip(grads, caches):
         flats.append(torch.cat([t.reshape(-1) for dw, db in bot_g + top_g for t in (dw, db) if t is not None]
@@ -418,8 +455,7 @@ def dlrm_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, timer=None):
         out = c["out4"].clone()
         out[0] = flat[-1] / R
         outs.append(out)
-    if timer:
-        timer("dense_allreduce")
+    timer("dense_allreduce")
     return outs
 
 
@@ -461,8 +497,7 @@ class PointwiseShard:
         self.W = self.D + 4                     # exchange row: D values, the item bias, 3 zeros (16-byte aligned rows)
         self.Lu = (self.U + world - 1) // world
         self.row_off = row_offsets([world * self.Lu, self.I])
-        self.ru = (self.U - rank + world - 1) // world
-        self.ri = (self.I - rank + world - 1) // world
+        self.ru, self.ri = shard_rows(self.U, rank, world), shard_rows(self.I, rank, world)
         want = ((max(self.ru, 1), self.D), (max(self.ri, 1), self.D), (max(self.ri, 1), 1))
         if tuple(tuple(t.shape) for t in (user, item, bias)) != want:
             raise ValueError(f"shard shapes {[tuple(t.shape) for t in (user, item, bias)]} != {want}")
@@ -479,10 +514,8 @@ class PointwiseShard:
 
     def load_global(self, user, item, bias):
         """user [U, D], item [I, D], bias [I] or [I, 1] (host or device): keep this rank's rows."""
-        r, R, dev = self.rank, self.world, self.user.device
         for t, g in zip(self.local_shards(), (user, item, bias)):
-            t.copy_(torch.as_tensor(np.ascontiguousarray(np.asarray(g)[r::R]), dtype=torch.float32)
-                    .reshape(t.shape).to(dev))
+            t.copy_(take_shard(g, self.rank, self.world).reshape(t.shape))
 
 
 def pointwise_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, c_l2=1.0, timer=None):
@@ -502,61 +535,31 @@ def pointwise_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, c_l2=1.0,
     and l2 travel in one all-reduce, with c_l2 * w and 0.5 * |w|^2 contributed by rank 0 only; every replica then
     applies the same summed gradient."""
     from . import native as N
+    timer = timer or _untimed
     R = parts[0].world
-    n = len(parts)
     for p, (uid, iid, label) in zip(parts, batches):
         if uid.dim() != 1 or uid.shape != iid.shape or label.shape != uid.shape:
             raise ValueError("uid, iid and label must be 1-D tensors of one length")
         if uid.numel() < 1:
             raise ValueError("the sharded pointwise step needs B >= 1 samples per rank")
     lks = [p.eng.pointwise_shard_lookups(uid, iid, p.U, p.I) for p, (uid, iid, _) in zip(parts, batches)]
-    bk = [p.eng.lookup_bucket(lk, p.row_off, R) for p, lk in zip(parts, lks)]
-    if timer:
-        timer("bucket")
-    send = [torch.stack([b[0], torch.full_like(b[0], lk.shape[0])], 1) for b, lk in zip(bk, lks)]   # (count, B)
-    recv = [torch.empty_like(x) for x in send]
-    xchg.all_to_all(recv, send, [[1] * R] * n, [[1] * R] * n)
-    host = torch.stack([torch.stack(send), torch.stack(recv)]).cpu()          # the step's one host sync
-    sc = [host[0, k, :, 0].tolist() for k in range(n)]
-    rc = [host[1, k, :, 0].tolist() for k in range(n)]
-    if any(set(host[1, k, :, 1].tolist()) != {lks[k].shape[0]} for k in range(n)):
-        raise ValueError("every rank must pass the same local batch size to the sharded pointwise step "
-                         f"(got {sorted(set(host[1, :, :, 1].reshape(-1).tolist()))})")
-    if timer:
-        timer("counts")
-    dev = [lk.device for lk in lks]
-    req = [torch.empty(sum(r), dtype=torch.int32, device=d) for r, d in zip(rc, dev)]
-    xchg.all_to_all(req, [b[1][:sum(s)] for b, s in zip(bk, sc)], rc, sc)
-    if timer:
-        timer("ids")
-    served = [p.eng.pointwise_serve(p.user, p.item, p.bias, p.ru, p.ri, p.Lu, q, p.W) for p, q in zip(parts, req)]
-    if timer:
-        timer("owner_serve")
-    got = [torch.empty(max(sum(s), 1), p.W, dtype=torch.float32, device=d) for p, s, d in zip(parts, sc, dev)]
-    xchg.all_to_all([g[:sum(s)] for g, s in zip(got, sc)], [x[0] for x in served], sc, rc)
-    if timer:
-        timer("rows")
+    fetched = _fetch_rows(parts, xchg, lks,
+                          lambda p, req: p.eng.pointwise_serve(p.user, p.item, p.bias, p.ru, p.ri, p.Lu, req, p.W),
+                          parts[0].W, True, timer)
     grads = []
-    for p, (_, _, label), b, g in zip(parts, batches, bk, got):
-        grads.append(p.eng.pointwise_grad_rows(p.kind, g, p.D, b[2], label, p.w, 1.0 / (label.numel() * R), p.a, p.b,
-                                               p.use_sigmoid, c_loss, c_l2, add_w_terms=p.rank == 0))
-    if timer:
-        timer("grad_rows")
-    g_uniq = [p.eng.rows_segment_sum(gr[0], b[3], b[4], sum(s)) for p, gr, b, s in zip(parts, grads, bk, sc)]
-    if timer:
-        timer("segment_sum")
-    g_rows = [torch.empty(sum(r), p.W, dtype=torch.float32, device=d) for p, r, d in zip(parts, rc, dev)]
-    xchg.all_to_all(g_rows, g_uniq, rc, sc)
-    if timer:
-        timer("grad_xchg")
-    for p, g, (_, ul, il) in zip(parts, g_rows, served):
+    for p, (_, _, label), f in zip(parts, batches, fetched):
+        grads.append(p.eng.pointwise_grad_rows(p.kind, f.got, p.D, f.bucket[2], label, p.w, 1.0 / (label.numel() * R),
+                                               p.a, p.b, p.use_sigmoid, c_loss, c_l2, add_w_terms=p.rank == 0))
+    timer("grad_rows")
+    g_rows = _return_grads(parts, xchg, fetched, [gr[0] for gr in grads], timer)
+    for p, g, f in zip(parts, g_rows, fetched):
+        _, ul, il = f.served
         o = p.eng.make_opt(*opt_args)
         D = p.D
         p.eng.sparse_apply_rows(p.eng.make_table(p.user, *p.user_slots), ul, g[:, :D], o)
         p.eng.sparse_apply_rows(p.eng.make_table(p.item, *p.item_slots), il, g[:, :D], o)
         p.eng.sparse_apply_rows(p.eng.make_table(p.bias, *p.bias_slots), il, g[:, D:D + 1], o)
-    if timer:
-        timer("owner_apply")
+    timer("owner_apply")
     gmf = parts[0].kind == N.ORX_POINT_GMF
     flats = [torch.cat([gr[1], gr[2]]) if gmf else gr[2].clone() for gr in grads]
     xchg.all_reduce(flats)
@@ -565,10 +568,7 @@ def pointwise_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, c_l2=1.0,
         if gmf:
             p.eng.dense_apply(p.w, *p.w_slots, flat[:p.D].view_as(p.w), p.eng.make_opt(*opt_args))
         outs.append(flat[-2:].clone())
-    if timer:
-        timer("dense_allreduce")
-    for p, s, r in zip(parts, sc, rc):
-        p.last = {"uniq": sum(s), "served": sum(r)}
+    timer("dense_allreduce")
     return outs
 
 
@@ -625,8 +625,7 @@ class HomeRoutedPairwise:
         self.kind, self.opt_kind, self.lr, self.eps, self.b1, self.b2, self.margin = kind, opt_kind, lr, eps, beta1, beta2, margin
         self.iterations = 0
         dev = eng.device
-        self.ru = (total_users - rank + world - 1) // world     # rows r with r % world == rank
-        self.ri = (total_items - rank + world - 1) // world
+        self.ru, self.ri = shard_rows(total_users, rank, world), shard_rows(total_items, rank, world)
         if tables is not None:          # shards owned by the caller (openrec.tf2.recommenders.ShardedBPR: keras variables)
             self.user, self.item, self.bias = tables
             want = ((max(self.ru, 1), dim), (max(self.ri, 1), dim), (max(self.ri, 1), 1))
@@ -743,26 +742,15 @@ class HomeRoutedPairwise:
 
     # ---- global <-> shard (tests, checkpoints)
     def load_global(self, user, item, bias):
-        r, R = self.rank, self.world
-        dev = self.eng.device
-        self.user[:self.ru] = torch.as_tensor(np.ascontiguousarray(user[r::R]), dtype=torch.float32).to(dev)
-        self.item[:self.ri] = torch.as_tensor(np.ascontiguousarray(item[r::R]), dtype=torch.float32).to(dev)
-        self.bias[:self.ri] = torch.as_tensor(np.ascontiguousarray(bias[r::R]), dtype=torch.float32).reshape(-1, 1).to(dev)
+        for t, g in zip(self.local_shards(), (user, item, bias)):
+            t.copy_(take_shard(g, self.rank, self.world).reshape(t.shape))
 
     def local_shards(self):
         return self.user[:self.ru], self.item[:self.ri], self.bias[:self.ri]
 
     def gather_global(self):
         """-> (user, item, bias) full tables on every rank (test helper; sizes must be small)."""
-        outs = []
-        for t, total in zip(self.local_shards(), (self.U, self.I, self.I)):
-            per = (total + self.world - 1) // self.world
-            pad = torch.zeros(per, t.shape[1], dtype=t.dtype, device=t.device)
-            pad[:t.shape[0]] = t
-            parts = [torch.empty_like(pad) for _ in range(self.world)]
-            dist.all_gather(parts, pad)
-            outs.append(torch.stack(parts, 1).reshape(per * self.world, t.shape[1])[:total])   # row = local*R + rank
-        return outs
+        return [gather_shards(t, total, self.world) for t, total in zip(self.local_shards(), (self.U, self.I, self.I))]
 
     # ---- per-rank shard checkpoint (SURVEY 8f N4 for tables that only exist sharded)
     def save_shard(self, path):

@@ -14,7 +14,10 @@ restores a rank's shard like any other model (one file per rank).  SGD, Adagrad 
 every rank passes its part of the global batch, and each rank censors the rows it owns among every rank's ids, as the
 single-device censor_vec does on the concatenated batch.  ``user_latent_factor.censor(ids)`` / ``item_latent_factor
 .censor(ids)`` (LatentFactor.censor on one sharded table) are collective as well and accept a different number of ids
-per rank."""
+per rank.
+
+The bases of every sharded Keras model live here too: ``_ShardedModel`` (process group, engine, the step protocol's
+checks; ShardedDLRM) and ``_ShardedFactors`` (the user / item / item-bias shards; ShardedWRMF / ShardedGMF as well)."""
 from __future__ import annotations
 
 import torch
@@ -55,53 +58,25 @@ class _Shard:
         return self.embeddings
 
 
-class ShardedBPR(Model):
-    _kind = N.ORX_PAIR_BPR
-    _score = N.ORX_SCORE_DOT
+class _ShardedModel(Model):
+    """What every row-sharded model shares: one process per GPU under ``torch.distributed`` (world size 1 allowed), this
+    rank's engine, and the checks of the step protocol -- the loss exists only inside the step, which takes the
+    gradients of all of the model's step variables w.r.t. one objective."""
 
-    def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items, seed=0):
+    def __init__(self):
         super().__init__()
         if not dist.is_initialized():
-            raise RuntimeError("ShardedBPR needs torch.distributed (one process per GPU; world size 1 is allowed)")
-        if dim_user_embed != dim_item_embed:
-            raise ValueError("user and item embedding dims must match (the reference multiplies them elementwise)")
+            raise RuntimeError(f"{type(self).__name__} needs torch.distributed (one process per GPU; world size 1 is "
+                               "allowed)")
         self._rank, self._world = dist.get_rank(), dist.get_world_size()
-        self._U, self._I, self._D = int(total_users), int(total_items), int(dim_user_embed)
-        eng = self._eng = N.engine()
-        r, R = self._rank, self._world
-        ru, ri = (self._U - r + R - 1) // R, (self._I - r + R - 1) // R
-        mk = lambda rows, cols, k, name: self._new_var(eng, rows, cols, seed * 1000003 + r * 17 + k, name)
-        self.user_latent_factor = _Shard(mk(max(ru, 1), self._D, 0, "user_latent_factor"), self._U, self._D)
-        self.item_latent_factor = _Shard(mk(max(ri, 1), self._D, 1, "item_latent_factor"), self._I, self._D)
-        self.item_bias = _Shard(mk(max(ri, 1), 1, 2, "item_bias"), self._I, 1)
-        self._impl = None
-        self._impl_key = None
+        self._eng = N.engine()
 
-    @staticmethod
-    def _new_var(eng, rows, cols, seed, name):
-        t = torch.empty(rows, cols, dtype=torch.float32, device=eng.device)
-        eng.fill_uniform(t, -0.05, 0.05, seed)                       # LatentFactor's 'uniform' initializer
+    def _new_var(self, rows, cols, seed, name):
+        t = torch.empty(rows, cols, dtype=torch.float32, device=self._eng.device)
+        self._eng.fill_uniform(t, -0.05, 0.05, seed)                 # LatentFactor's 'uniform' initializer
         v = Variable.__new__(Variable)
         v.t, v.trainable, v.name = t, True, name
         return v
-
-    def _get_margin(self):
-        return 0.0
-
-    @property
-    def variables(self):
-        return [self.user_latent_factor.embeddings, self.item_latent_factor.embeddings, self.item_bias.embeddings]
-
-    trainable_variables = variables
-
-    def _orx_step_variables(self):
-        return self.variables
-
-    def call(self, user_id, p_item_id, n_item_id):
-        """-> (loss, l2_loss) of the GLOBAL batch as lazy scalars; this rank contributes the triplets it was given."""
-        node = StepNode(self, 2)
-        node.ids = tuple(ids_of(x) for x in (user_id, p_item_id, n_item_id))
-        return LazyScalar(node, {0: 1.0}), LazyScalar(node, {1: 1.0})
 
     def _orx_forward(self, node):
         raise NotImplementedError("a sharded model's loss exists only as part of the training step "
@@ -110,14 +85,93 @@ class ShardedBPR(Model):
     def _orx_materialize_grad(self, node, var, coef):
         raise NotImplementedError("explicit IndexedSlices are not available for row-sharded tables")
 
-    def _orx_apply(self, node, grads_and_vars, optimizer):
+    def _step_args(self, node, grads_and_vars, optimizer):
+        """-> (coef, opt_args) of one sharded step: the objective's {output: coefficient} and (kind, lr, eps, beta1,
+        beta2, step) of ``optimizer``, after refusing a node already stepped or a gradient set that is not ALL of the
+        step variables w.r.t. one objective."""
         if node.stepped:
             raise RuntimeError("this model call's gradients were already applied")
-        want = {id(v) for v in self.variables}
+        want = {id(v) for v in self._orx_step_variables()}
         coefs = [g.coef for g, _ in grads_and_vars]
         if {id(v) for _, v in grads_and_vars} != want or any(c != coefs[0] for c in coefs):
             raise NotImplementedError("apply_gradients: the sharded step needs the gradients of ALL of the model's "
-                                      "variables w.r.t. one objective")
+                                      "trainable variables w.r.t. one objective")
+        return coefs[0], (optimizer._kind, optimizer.learning_rate, optimizer.epsilon, optimizer.beta_1,
+                          optimizer.beta_2, optimizer.iterations)
+
+
+class _ShardedFactors(_ShardedModel):
+    """The user / item / item-bias layout of the sharded factor models (ShardedBPR / ShardedUCML, ShardedWRMF /
+    ShardedGMF): row r of each table on rank r % world at local row r // world, a 1-row dummy on a rank without rows;
+    the tables are ``variables`` in that order, seeded per rank and table."""
+    _score = N.ORX_SCORE_DOT
+
+    def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items, seed):
+        super().__init__()
+        if dim_user_embed != dim_item_embed:
+            raise ValueError("user and item embedding dims must match (the reference multiplies them elementwise)")
+        self._U, self._I, self._D = int(total_users), int(total_items), int(dim_user_embed)
+        self._check_sizes()
+        r, R = self._rank, self._world
+
+        def shard(total, cols, k, name):
+            var = self._new_var(max(N.shard_rows(total, r, R), 1), cols, seed * 1000003 + r * 17 + k, name)
+            return _Shard(var, total, cols)
+        self.user_latent_factor = shard(self._U, self._D, 0, "user_latent_factor")
+        self.item_latent_factor = shard(self._I, self._D, 1, "item_latent_factor")
+        self.item_bias = shard(self._I, 1, 2, "item_bias")
+
+    def _check_sizes(self):
+        """Refuse sizes the model cannot shard (called before any table is allocated)."""
+
+    def _w(self):
+        """GMF's w (the scale of the score), else None."""
+        return None
+
+    @property
+    def variables(self):
+        vs = [self.user_latent_factor.embeddings, self.item_latent_factor.embeddings, self.item_bias.embeddings]
+        w = self._w()
+        return vs + ([w] if w is not None else [])
+
+    trainable_variables = variables
+
+    def _orx_step_variables(self):
+        return self.variables
+
+    def _sharded_score_operands(self):
+        """(score kind, user shard, item shard, item bias shard as a flat [rows] view, native.RowShard, process group,
+        scale: GMF's w as a flat [dim] view, else None) of the catalogue evaluation and retrieval over the shards
+        (RankingEvaluator.evaluate, Retriever.recommend: one collective call on every rank)."""
+        g = N.rowshard(self._world, self._rank, self._U, self._I)
+        w = self._w()
+        return (self._score, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
+                self.item_bias.embeddings.t.reshape(-1), g, None, None if w is None else w.t.reshape(-1))
+
+    def inference(self, user_id):
+        raise NotImplementedError("full-catalogue scoring needs the whole item table on one device; a sharded model's "
+                                  "top-k items come from Retriever.recommend")
+
+
+class ShardedBPR(_ShardedFactors):
+    _kind = N.ORX_PAIR_BPR
+
+    def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items, seed=0):
+        super().__init__(dim_user_embed, dim_item_embed, total_users, total_items, seed)
+        self._impl = None
+        self._impl_key = None
+
+    def _get_margin(self):
+        return 0.0
+
+    def call(self, user_id, p_item_id, n_item_id):
+        """-> (loss, l2_loss) of the GLOBAL batch as lazy scalars; this rank contributes the triplets it was given."""
+        node = StepNode(self, 2)
+        node.ids = tuple(ids_of(x) for x in (user_id, p_item_id, n_item_id))
+        return LazyScalar(node, {0: 1.0}), LazyScalar(node, {1: 1.0})
+
+    def _orx_apply(self, node, grads_and_vars, optimizer):
+        coef, _ = self._step_args(node, grads_and_vars, optimizer)
         kind = optimizer._kind
         if kind not in (N.ORX_OPT_SGD, N.ORX_OPT_ADAGRAD, N.ORX_OPT_ADAM_LAZY):
             raise NotImplementedError("sharded tables: use SGD, Adagrad or LazyAdam (Keras Adam() sweeps whole tables)")
@@ -135,22 +189,10 @@ class ShardedBPR(Model):
         m.lr, m.eps, m.b1, m.b2 = optimizer.learning_rate, optimizer.epsilon, optimizer.beta_1, optimizer.beta_2
         m.margin = self._get_margin()
         m.iterations = optimizer.iterations - 1                      # HomeRoutedPairwise.step increments it
-        out = m.step(*node.ids, c_loss=float(coefs[0].get(0, 0.0)), c_l2=float(coefs[0].get(1, 0.0)))
+        out = m.step(*node.ids, c_loss=float(coef.get(0, 0.0)), c_l2=float(coef.get(1, 0.0)))
         node.out = m._out[m.iterations % 16]
         node.stepped = True
         node.ids = None
-
-    def _sharded_score_operands(self):
-        """(score kind, user shard, item shard, item bias shard as a flat [rows] view, native.RowShard, process group)
-        of the catalogue evaluation and retrieval over the shards (RankingEvaluator.evaluate, Retriever.recommend: one
-        collective call on every rank)."""
-        g = N.rowshard(self._world, self._rank, self._U, self._I)
-        return (self._score, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
-                self.item_bias.embeddings.t.reshape(-1), g, None)
-
-    def inference(self, user_id):
-        raise NotImplementedError("full-catalogue scoring needs the whole item table on one device; a sharded model's "
-                                  "top-k items come from Retriever.recommend")
 
     def check(self):
         """Raise if the sharded step flagged an error (peer timeout, mailbox overflow)."""

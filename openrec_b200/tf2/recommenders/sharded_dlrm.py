@@ -13,25 +13,22 @@ from __future__ import annotations
 
 import sys
 
-import torch
 import torch.distributed as dist
 
 from ... import native as N
 from ...sharded import DistExchange, DLRMShard, dlrm_inference_sharded, dlrm_step_sharded, row_offsets
-from ...tfshim.core import LazyScalar, StepNode, Tensor, Variable
-from ...tfshim.keras import Model
+from ...tfshim.core import LazyScalar, StepNode, Tensor
 from ..mlp_ops import ACT, interaction_width
 from ..modules import MLP
 from .dlrm import DLRM
+from .sharded import _ShardedModel
 
 
-class ShardedDLRM(Model):
+class ShardedDLRM(_ShardedModel):
     def __init__(self, m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op="dot", arch_interaction_itself=False,
                  sigmoid_bot=False, sigmoid_top=True, loss_func="mse", loss_threshold=0.0,
                  interaction_mode="reference", seed=0):
         super().__init__()
-        if not dist.is_initialized():
-            raise RuntimeError("ShardedDLRM needs torch.distributed (one process per GPU; world size 1 is allowed)")
         if arch_interaction_op != "dot" and self._arch_interaction_op != "cat":   # as DLRM: AttributeError (SURVEY Q2)
             sys.exit("ERROR: arch_interaction_op=" + self._arch_interaction_op + " is not supported")
         if loss_func not in ("mse", "bce"):
@@ -41,14 +38,9 @@ class ShardedDLRM(Model):
         self._row_off = row_offsets(self._vocab)
         self._loss_threshold, self._loss_func = loss_threshold, loss_func
         self._self_interaction, self._interaction_mode = bool(arch_interaction_itself), interaction_mode
-        self._rank, self._world = dist.get_rank(), dist.get_world_size()
-        eng = self._eng = N.engine()
-        rows = (self._row_off[-1] - self._rank + self._world - 1) // self._world
-        t = torch.empty(max(rows, 1), self._m_spa, dtype=torch.float32, device=eng.device)
-        eng.fill_uniform(t, -0.05, 0.05, seed * 1000003 + self._rank * 17)     # LatentFactor's 'uniform' initializer
-        v = Variable.__new__(Variable)
-        v.t, v.trainable, v.name = t, True, "embedding_shard"
-        self.embedding_shard = v
+        rows = N.shard_rows(self._row_off[-1], self._rank, self._world)
+        self.embedding_shard = self._new_var(max(rows, 1), self._m_spa, seed * 1000003 + self._rank * 17,
+                                             "embedding_shard")
         self._mlp_bot = MLP(units_list=ln_bot, out_activation="sigmoid" if sigmoid_bot else "relu")
         self._mlp_top = MLP(units_list=ln_top, out_activation="sigmoid" if sigmoid_top else "relu")
         self._xchg = DistExchange()
@@ -103,24 +95,9 @@ class ShardedDLRM(Model):
         self._build(dense.shape[1])
         return Tensor(dlrm_inference_sharded([self._part()], self._xchg, [(dense, sparse)])[0])
 
-    def _orx_forward(self, node):
-        raise NotImplementedError("a sharded model's loss exists only as part of the training step "
-                                  "(read it after optimizer.apply_gradients)")
-
-    def _orx_materialize_grad(self, node, var, coef):
-        raise NotImplementedError("explicit IndexedSlices are not available for row-sharded tables")
-
     def _orx_apply(self, node, grads_and_vars, optimizer):
-        if node.stepped:
-            raise RuntimeError("this model call's gradients were already applied")
-        want = {id(v) for v in self.trainable_variables}
-        coefs = [g.coef for g, _ in grads_and_vars]
-        if {id(v) for _, v in grads_and_vars} != want or any(c != coefs[0] for c in coefs):
-            raise NotImplementedError("apply_gradients: the sharded step needs the gradients of ALL trainable "
-                                      "variables w.r.t. one objective")
-        opt_args = (optimizer._kind, optimizer.learning_rate, optimizer.epsilon, optimizer.beta_1, optimizer.beta_2,
-                    optimizer.iterations)
+        coef, opt_args = self._step_args(node, grads_and_vars, optimizer)
         node.out = dlrm_step_sharded([self._part(optimizer)], self._xchg, [node.inputs], opt_args,
-                                     c_loss=float(coefs[0].get(0, 0.0)))[0]
+                                     c_loss=float(coef.get(0, 0.0)))[0]
         node.stepped = True
         node.inputs = None

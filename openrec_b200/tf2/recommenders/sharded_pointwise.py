@@ -18,34 +18,22 @@ import torch.distributed as dist
 from ... import native as N
 from ...sharded import DistExchange, PointwiseShard, pointwise_step_sharded, row_offsets
 from ...tfshim.core import LazyScalar, StepNode, convert
-from ...tfshim.keras import Model
 from ..modules import MLP, PointwiseMSELoss
 from ._base import ids_of
-from .sharded import ShardedBPR, _Shard
+from .sharded import _ShardedFactors
 
 
-class ShardedWRMF(Model):
+class ShardedWRMF(_ShardedFactors):
     _kind = N.ORX_POINT_WRMF
 
     def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items, a=1.0, b=1.0, seed=0):
-        super().__init__()
-        if not dist.is_initialized():
-            raise RuntimeError(f"{type(self).__name__} needs torch.distributed (one process per GPU; world size 1 is "
-                               "allowed)")
-        if dim_user_embed != dim_item_embed:
-            raise ValueError("user and item embedding dims must match (the reference multiplies them elementwise)")
-        self._rank, self._world = dist.get_rank(), dist.get_world_size()
-        self._U, self._I, self._D = int(total_users), int(total_items), int(dim_user_embed)
-        r, R = self._rank, self._world
-        row_offsets([R * ((self._U + R - 1) // R), self._I])    # the exchange's row space must fit int32: refuse now
-        eng = self._eng = N.engine()
-        ru, ri = (self._U - r + R - 1) // R, (self._I - r + R - 1) // R
-        mk = lambda rows, cols, k, name: ShardedBPR._new_var(eng, rows, cols, seed * 1000003 + r * 17 + k, name)
-        self.user_latent_factor = _Shard(mk(max(ru, 1), self._D, 0, "user_latent_factor"), self._U, self._D)
-        self.item_latent_factor = _Shard(mk(max(ri, 1), self._D, 1, "item_latent_factor"), self._I, self._D)
-        self.item_bias = _Shard(mk(max(ri, 1), 1, 2, "item_bias"), self._I, 1)
+        super().__init__(dim_user_embed, dim_item_embed, total_users, total_items, seed)
         self._init_head(a, b)
         self._xchg = DistExchange()
+
+    def _check_sizes(self):
+        R = self._world
+        row_offsets([R * ((self._U + R - 1) // R), self._I])    # the exchange's row space must fit int32: refuse now
 
     def _init_head(self, a, b):
         self.pointwise_mse_loss = PointwiseMSELoss(a=a, b=b)
@@ -53,20 +41,6 @@ class ShardedWRMF(Model):
     def _point_params(self):
         l = self.pointwise_mse_loss
         return float(l._a), float(l._b), bool(l._sigmoid)
-
-    def _w(self):
-        return None
-
-    @property
-    def variables(self):
-        vs = [self.user_latent_factor.embeddings, self.item_latent_factor.embeddings, self.item_bias.embeddings]
-        w = self._w()
-        return vs + ([w] if w is not None else [])
-
-    trainable_variables = variables
-
-    def _orx_step_variables(self):
-        return self.variables
 
     def call(self, user_id, item_id, label):
         """-> (loss, l2_loss) of the GLOBAL batch as lazy scalars; this rank contributes the samples it was given."""
@@ -84,40 +58,12 @@ class ShardedWRMF(Model):
                               w=None if w is None else w.t, w_slots=optimizer.slots(w) if w is not None else (None, None),
                               a=a, b=b, use_sigmoid=sig)
 
-    def _orx_forward(self, node):
-        raise NotImplementedError("a sharded model's loss exists only as part of the training step "
-                                  "(read it after optimizer.apply_gradients)")
-
-    def _orx_materialize_grad(self, node, var, coef):
-        raise NotImplementedError("explicit IndexedSlices are not available for row-sharded tables")
-
     def _orx_apply(self, node, grads_and_vars, optimizer):
-        if node.stepped:
-            raise RuntimeError("this model call's gradients were already applied")
-        want = {id(v) for v in self.variables}
-        coefs = [g.coef for g, _ in grads_and_vars]
-        if {id(v) for _, v in grads_and_vars} != want or any(c != coefs[0] for c in coefs):
-            raise NotImplementedError("apply_gradients: the sharded step needs the gradients of ALL of the model's "
-                                      "variables w.r.t. one objective")
-        opt_args = (optimizer._kind, optimizer.learning_rate, optimizer.epsilon, optimizer.beta_1, optimizer.beta_2,
-                    optimizer.iterations)
+        coef, opt_args = self._step_args(node, grads_and_vars, optimizer)
         node.out = pointwise_step_sharded([self._part(optimizer)], self._xchg, [node.inputs], opt_args,
-                                          c_loss=float(coefs[0].get(0, 0.0)), c_l2=float(coefs[0].get(1, 0.0)))[0]
+                                          c_loss=float(coef.get(0, 0.0)), c_l2=float(coef.get(1, 0.0)))[0]
         node.stepped = True
         node.inputs = None
-
-    def _sharded_score_operands(self):
-        """(score kind, user shard, item shard, item bias shard as a flat [rows] view, native.RowShard, process group,
-        scale: GMF's w as a flat [dim] view, else None) of the catalogue evaluation and retrieval over the shards
-        (RankingEvaluator.evaluate, Retriever.recommend: one collective call on every rank)."""
-        g = N.rowshard(self._world, self._rank, self._U, self._I)
-        w = self._w()
-        return (N.ORX_SCORE_DOT, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
-                self.item_bias.embeddings.t.reshape(-1), g, None, None if w is None else w.t.reshape(-1))
-
-    def inference(self, user_id):
-        raise NotImplementedError("full-catalogue scoring needs the whole item table on one device; a sharded model's "
-                                  "top-k items come from Retriever.recommend")
 
 
 class ShardedGMF(ShardedWRMF):

@@ -4,12 +4,11 @@ tables and the concatenation of every rank's ids.  The engine is the oracle-back
 test-local censor_shard that restates orx_censor_shard in numpy (each rank censors the ids it owns), so this checks the
 decomposition and the collective plumbing; the kernel is checked in tests/test_gpu_censor_shard.py."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
+from _ranks import run_ranks
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -81,15 +80,8 @@ def _worker(world):
 
 @pytest.mark.parametrize("world", [2, 3])
 def test_sharded_censor_equals_oracle(world):
-    port = 28300 + (os.getpid() + world * 7) % 1500
     paths = [os.path.join(ROOT, "compat"), ROOT, os.path.join(ROOT, "tests")]
     code = (f"import sys; sys.path[:0] = {paths!r}\n"
             f"import test_censor_shard_cpu as t\nt._worker({world})\nprint('rank ok')\n")
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        procs.append(subprocess.Popen([sys.executable, "-c", code], env=env, stdout=subprocess.PIPE,
-                                      stderr=subprocess.STDOUT, text=True))
-    for p in procs:
-        out, _ = p.communicate(timeout=300)
-        assert p.returncode == 0 and "rank ok" in out, out
+    for rc, out in run_ranks(world, code, "censor_shard_cpu"):
+        assert rc == 0 and "rank ok" in out, out

@@ -4,35 +4,21 @@ tests/_dlrm_shard_worker.py), with the oracle-backed engine of tests/fake_engine
 exchanges and the step's arithmetic plan; the kernels are checked in tests/test_gpu_dlrm_shard.py.  Also: the numpy
 restatement of orx_lookup_bucket against a direct definition, and the argument checks."""
 import os
-import subprocess
 import sys
 
 import numpy as np
 import pytest
+from _ranks import run_ranks
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WORKER = os.path.join(ROOT, "tests", "_dlrm_shard_worker.py")
-
-
-def _spawn(world, args, code=None):
-    port = 29100 + (os.getpid() * 7 + world * 13 + sum(map(ord, "".join(args)))) % 1500
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        cmd = [sys.executable, WORKER, *args] if code is None else [sys.executable, "-c", code]
-        procs.append(subprocess.Popen(cmd, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    outs = []
-    for p in procs:
-        out, _ = p.communicate(timeout=300)
-        outs.append((p.returncode, out))
-    return outs
 
 
 @pytest.mark.parametrize("world", [2, 3])
 @pytest.mark.parametrize("opt,mode,loss", [("adagrad", "dlrm", "mse"), ("adam", "reference", "bce"),
                                            ("sgd", "dlrm", "bce"), ("lazyadam", "dlrm", "mse")])
 def test_sharded_dlrm_equals_oracle(world, opt, mode, loss):
-    for rc, out in _spawn(world, ["gloo", opt, mode, loss]):
+    for rc, out in run_ranks(world, [WORKER, "gloo", opt, mode, loss], f"dlrm_shard_cpu {opt} {mode} {loss}"):
         assert rc == 0 and "rank ok" in out, out
 
 
@@ -74,7 +60,7 @@ print("rank ok")
 
 
 def test_sharded_dlrm_refusals():
-    for rc, out in _spawn(2, ["errors"], code=_ERRORS.format(root=ROOT)):
+    for rc, out in run_ranks(2, _ERRORS.format(root=ROOT), "dlrm_shard_cpu errors"):
         assert rc == 0 and "rank ok" in out, out
 
 

@@ -6,8 +6,6 @@ among every rank's ids.  Reassembled, the shards must equal orx_censor on the gl
 the kernel shares k_censor's row arithmetic.  A rank past the table's end keeps a 1-row dummy shard of sentinel values
 that must stay untouched."""
 import os
-import subprocess
-import sys
 import zlib
 
 import numpy as np
@@ -18,6 +16,7 @@ from oracle import openrec_oracle as O
 from openrec_b200 import _lib as L
 from openrec_b200 import native as N
 from openrec_b200.sharded import LoopbackGroup, censor_gathered
+from _ranks import run_ranks
 from test_gpu_shard_loopback import _oracle_state
 
 pytestmark = pytest.mark.gpu
@@ -278,18 +277,10 @@ def test_ucml_loop_loopback(world, opt_kind, announce):
 
 
 def _run_workers(world):
-    port = 29400 + (os.getpid() + world) % 2000
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "tests", "_censor_shard_worker.py")],
-                                      env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    outs = []
-    for p in procs:
-        o, _ = p.communicate(timeout=600)
-        assert p.returncode == 0, o
-        outs.append(o)
-    assert "censor ok" in outs[0], outs[0]
+    outs = run_ranks(world, [os.path.join(ROOT, "tests", "_censor_shard_worker.py")], "gpu_censor_shard", timeout=600)
+    for rc, o in outs:
+        assert rc == 0, o
+    assert "censor ok" in outs[0][1], outs[0][1]
 
 
 def test_end_to_end_world_one():

@@ -3,7 +3,6 @@ ranks on one device (LoopbackExchange: every rank its own liborx handle, the mul
 single-GPU DLRM on the global batch; sharded inference; ShardedDLRM in a one-rank NCCL group with the reference
 example's train_step and Keras Adam(), and a checkpoint round trip; and a worker-process job on >= 2 GPUs."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -14,6 +13,7 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [os.path.join(ROOT, "compat"), os.path.join(ROOT, "tests")]
 
+from _ranks import run_ranks  # noqa: E402
 from dlrm_shard_np import lookup_bucket_np  # noqa: E402
 
 
@@ -279,22 +279,12 @@ print("class ok")
 
 
 def test_sharded_dlrm_class_one_rank():
-    env = dict(os.environ, MASTER_ADDR="127.0.0.1", MASTER_PORT=str(29700 + os.getpid() % 500), RANK="0", WORLD_SIZE="1")
-    p = subprocess.run([sys.executable, "-c", _CLASS.format(root=ROOT)], env=env, capture_output=True, text=True,
-                       timeout=600)
-    assert p.returncode == 0 and "class ok" in p.stdout, p.stdout + p.stderr
+    [(rc, out)] = run_ranks(1, _CLASS.format(root=ROOT), "gpu_dlrm_shard class", timeout=600)
+    assert rc == 0 and "class ok" in out, out
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
 def test_sharded_dlrm_multi_gpu():
-    world = torch.cuda.device_count()
-    port = 29800 + os.getpid() % 500
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "tests", "_dlrm_shard_worker.py"), "nccl",
-                                       "adagrad", "dlrm", "mse"], env=env, stdout=subprocess.PIPE,
-                                      stderr=subprocess.STDOUT, text=True))
-    for p in procs:
-        out, _ = p.communicate(timeout=600)
-        assert p.returncode == 0 and "rank ok" in out, out
+    for rc, out in run_ranks(torch.cuda.device_count(), [os.path.join(ROOT, "tests", "_dlrm_shard_worker.py"), "nccl",
+                                                         "adagrad", "dlrm", "mse"], "gpu_dlrm_shard multi", timeout=600):
+        assert rc == 0 and "rank ok" in out, out

@@ -6,7 +6,6 @@ orx_score_rank / orx_score_topk on the gathered tables; ShardedGMF / ShardedWRMF
 WRMF, with a checkpoint round trip and RankingEvaluator / Retriever; and a worker-process job on >= 2 GPUs."""
 import ctypes as C
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -17,6 +16,7 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [os.path.join(ROOT, "compat"), os.path.join(ROOT, "tests")]
 
+from _ranks import run_ranks  # noqa: E402
 from pointwise_shard_np import grad_rows_np, serve_np, shard_lookups_np  # noqa: E402
 
 GMF, WRMF = 0, 1
@@ -390,22 +390,14 @@ print("class ok")
 
 
 def test_sharded_pointwise_classes_one_rank():
-    env = dict(os.environ, MASTER_ADDR="127.0.0.1", MASTER_PORT=str(28700 + os.getpid() % 500), RANK="0", WORLD_SIZE="1")
-    p = subprocess.run([sys.executable, "-c", _CLASS.format(root=ROOT)], env=env, capture_output=True, text=True,
-                       timeout=600)
-    assert p.returncode == 0 and "class ok" in p.stdout, p.stdout + p.stderr
+    [(rc, out)] = run_ranks(1, _CLASS.format(root=ROOT), "gpu_pointwise_shard class", timeout=600)
+    assert rc == 0 and "class ok" in out, out
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
 @pytest.mark.parametrize("model,opt", [("gmf", "adagrad"), ("wrmf_sigmoid", "adam")])
 def test_sharded_pointwise_multi_gpu(model, opt):
-    world = torch.cuda.device_count()
-    port = 28200 + os.getpid() % 400 + len(model)
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "tests", "_pointwise_shard_worker.py"), "nccl",
-                                       model, opt], env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    for p in procs:
-        out, _ = p.communicate(timeout=600)
-        assert p.returncode == 0 and "rank ok" in out, out
+    for rc, out in run_ranks(torch.cuda.device_count(), [os.path.join(ROOT, "tests", "_pointwise_shard_worker.py"),
+                                                         "nccl", model, opt], f"gpu_pointwise_shard {model} {opt}",
+                             timeout=600):
+        assert rc == 0 and "rank ok" in out, out

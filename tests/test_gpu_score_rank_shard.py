@@ -7,8 +7,6 @@ one float32 ulp, the bar of tests/test_gpu_score_rank.py.  The dummy row of an e
 shows up in the outputs."""
 import ctypes as C
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -17,6 +15,7 @@ import torch
 from openrec_b200 import _lib as L
 from openrec_b200 import native as N
 from openrec_b200.sharded import loopback_sum, score_rank_sharded
+from _ranks import run_ranks
 from test_gpu_score_rank import SHAPES, Problem, check_equal, dev, make_problem, seed_of
 
 pytestmark = pytest.mark.gpu
@@ -251,18 +250,10 @@ def test_argument_refusals(eng):
 
 
 def _run_workers(world):
-    port = 29600 + (os.getpid() + world) % 2000
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "tests", "_score_rank_shard_worker.py")],
-                                      env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    outs = []
-    for p in procs:
-        o, _ = p.communicate(timeout=600)
-        assert p.returncode == 0, o
-        outs.append(o)
-    assert "evaluation ok" in outs[0], outs[0]
+    outs = run_ranks(world, [os.path.join(ROOT, "tests", "_score_rank_shard_worker.py")], "gpu_score_rank_shard", timeout=600)
+    for rc, o in outs:
+        assert rc == 0, o
+    assert "evaluation ok" in outs[0][1], outs[0][1]
 
 
 def test_end_to_end_world_one():

@@ -7,8 +7,6 @@ bits must equal rank 0's, and rank 0's must equal orx_score_topk on the global t
 an empty item shard is a zero row with bias +inf instead: a read of it would put an item id >= I first in the list."""
 import ctypes as C
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -17,6 +15,7 @@ import torch
 from openrec_b200 import _lib as L
 from openrec_b200 import native as N
 from openrec_b200.sharded import loopback_sum, score_topk_sharded
+from _ranks import run_ranks
 from test_gpu_score_topk import F32, SHAPES, Problem, dev, make_problem, seed_of
 
 pytestmark = pytest.mark.gpu
@@ -234,18 +233,10 @@ def test_catalogue_shape(eng):
 
 # ---- end to end through openrec.tf2 over NCCL ------------------------------------------------------------------------
 def _run_workers(world):
-    port = 29600 + (os.getpid() + world + 7) % 2000
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "tests", "_score_topk_shard_worker.py")],
-                                      env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    outs = []
-    for p in procs:
-        o, _ = p.communicate(timeout=600)
-        assert p.returncode == 0, o
-        outs.append(o)
-    assert "retrieval ok" in outs[0], outs[0]
+    outs = run_ranks(world, [os.path.join(ROOT, "tests", "_score_topk_shard_worker.py")], "gpu_score_topk_shard", timeout=600)
+    for rc, o in outs:
+        assert rc == 0, o
+    assert "retrieval ok" in outs[0][1], outs[0][1]
 
 
 def test_end_to_end_world_one():

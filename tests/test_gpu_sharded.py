@@ -1,12 +1,11 @@
 """GPU, >= 2 devices: the row-sharded step on the real kernels over NCCL equals the single-process oracle
 step on the same global batch (cross-rank duplicates included)."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
+from _ranks import run_ranks
 
 from oracle import openrec_oracle as O
 
@@ -22,16 +21,9 @@ def test_sharded_step_on_gpus(tmp_path, kind, opt_kind, mode):
     if world < 2:
         pytest.skip("needs >= 2 GPUs")
     out = str(tmp_path / "res.npz")
-    port = 29600 + (os.getpid() + kind * 3 + opt_kind) % 1000
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "tests", "_sharded_worker.py"), out,
-                                       str(kind), str(opt_kind), mode], env=env, stdout=subprocess.PIPE,
-                                      stderr=subprocess.STDOUT, text=True))
-    for p in procs:
-        o, _ = p.communicate(timeout=600)
-        assert p.returncode == 0, o
+    for rc, o in run_ranks(world, [os.path.join(ROOT, "tests", "_sharded_worker.py"), out, str(kind), str(opt_kind),
+                                   mode], f"gpu_sharded {kind} {opt_kind} {mode}", timeout=600):
+        assert rc == 0, o
     got = np.load(out)
     rng = np.random.default_rng(99)
     U, I, D, B = 1501, 2003, 128, 1024

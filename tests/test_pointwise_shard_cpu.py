@@ -5,28 +5,14 @@ numpy restatements of tests/pointwise_shard_np.py.  This checks the layout, the 
 plan; the kernels are checked in tests/test_gpu_pointwise_shard.py.  Also: the numpy restatements against their
 contracts written out sample by sample, and the refusals."""
 import os
-import subprocess
 import sys
 
 import numpy as np
 import pytest
+from _ranks import run_ranks
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WORKER = os.path.join(ROOT, "tests", "_pointwise_shard_worker.py")
-
-
-def _spawn(world, args, code=None):
-    port = 27100 + (os.getpid() * 7 + world * 13 + sum(map(ord, "".join(args)))) % 1500
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        cmd = [sys.executable, WORKER, *args] if code is None else [sys.executable, "-c", code]
-        procs.append(subprocess.Popen(cmd, env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True))
-    outs = []
-    for p in procs:
-        out, _ = p.communicate(timeout=300)
-        outs.append((p.returncode, out))
-    return outs
 
 
 @pytest.mark.parametrize("world", [2, 3])
@@ -34,7 +20,7 @@ def _spawn(world, args, code=None):
                                        ("wrmf", "adagrad"), ("wrmf_sigmoid", "adam"), ("wrmf", "sgd"),
                                        ("wrmf_sigmoid", "lazyadam")])
 def test_sharded_pointwise_equals_oracle(world, model, opt):
-    for rc, out in _spawn(world, ["gloo", model, opt]):
+    for rc, out in run_ranks(world, [WORKER, "gloo", model, opt], f"pointwise_shard_cpu {model} {opt}"):
         assert rc == 0 and "rank ok" in out, out
 
 
@@ -84,7 +70,7 @@ print("rank ok")
 
 
 def test_sharded_pointwise_refusals():
-    for rc, out in _spawn(2, ["errors"], code=_ERRORS.format(root=ROOT)):
+    for rc, out in run_ranks(2, _ERRORS.format(root=ROOT), "pointwise_shard_cpu errors"):
         assert rc == 0 and "rank ok" in out, out
 
 

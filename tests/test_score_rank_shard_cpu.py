@@ -4,12 +4,11 @@ Recall on the gathered tables.  The engine is the oracle-backed one of tests/fak
 score_rank_shard that restates the phases in numpy (each rank counts over its own item rows only), so this checks the
 counting decomposition and the collective plumbing; the kernels are checked in tests/test_gpu_score_rank_shard.py."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 import torch
+from _ranks import run_ranks
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F32 = np.float32
@@ -172,15 +171,8 @@ def _worker(world, ucml):
 @pytest.mark.parametrize("world", [2, 3])
 @pytest.mark.parametrize("ucml", [False, True], ids=["bpr", "ucml"])
 def test_sharded_evaluation_equals_oracle(world, ucml):
-    port = 29800 + (os.getpid() + world * 3 + ucml) % 1500
     paths = [os.path.join(ROOT, "compat"), ROOT, os.path.join(ROOT, "tests")]
     code = (f"import sys; sys.path[:0] = {paths!r}\n"
             f"import test_score_rank_shard_cpu as t\nt._worker({world}, {ucml})\nprint('rank ok')\n")
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        procs.append(subprocess.Popen([sys.executable, "-c", code], env=env, stdout=subprocess.PIPE,
-                                      stderr=subprocess.STDOUT, text=True))
-    for p in procs:
-        out, _ = p.communicate(timeout=300)
-        assert p.returncode == 0 and "rank ok" in out, out
+    for rc, out in run_ranks(world, code, f"score_rank_shard_cpu {ucml}"):
+        assert rc == 0 and "rank ok" in out, out

@@ -3,11 +3,10 @@ all-to-all exchanges, slot permutations, cross-rank duplicate handling) reproduc
 oracle step on the same global batch.  Arithmetic = oracle via tests/fake_engine.py; the CUDA kernels
 behind the same calls are checked in tests/test_gpu_kernels.py / test_gpu_sharded.py."""
 import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
+from _ranks import run_ranks
 
 from oracle import openrec_oracle as O
 
@@ -17,16 +16,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 @pytest.mark.parametrize("world,kind,opt_kind", [(2, 0, 1), (3, 0, 0), (2, 1, 1), (2, 0, 2)])
 def test_sharded_step_equals_single_process(tmp_path, world, kind, opt_kind):
     out = str(tmp_path / "res.npz")
-    port = 29500 + (os.getpid() + world * 7 + kind * 3 + opt_kind) % 2000
-    procs = []
-    for r in range(world):
-        env = dict(os.environ, RANK=str(r), WORLD_SIZE=str(world), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
-        procs.append(subprocess.Popen([sys.executable, os.path.join(ROOT, "tests", "_sharded_worker.py"), out,
-                                       str(kind), str(opt_kind)], env=env, stdout=subprocess.PIPE,
-                                      stderr=subprocess.STDOUT, text=True))
-    for p in procs:
-        o, _ = p.communicate(timeout=300)
-        assert p.returncode == 0, o
+    for rc, o in run_ranks(world, [os.path.join(ROOT, "tests", "_sharded_worker.py"), out, str(kind), str(opt_kind)],
+                           f"sharded_gloo {kind} {opt_kind}"):
+        assert rc == 0, o
     got = np.load(out)
     rng = np.random.default_rng(99)
     U, I, D, B = 61, 83, 16, 40
