@@ -306,6 +306,31 @@ ORX_API int orx_lookup_bucket(orx_handle_t h, const int32_t* sparse, int32_t B, 
                               int32_t* grp_idx, orx_stream_t s);
 ORX_API int orx_rows_segment_sum(orx_handle_t h, const float* src, int64_t src_ld, int32_t dim, const int32_t* grp_off,
                                  const int32_t* grp_idx, int32_t n_uniq, float* out, orx_stream_t s);
+/* Multi-hot (bag) form of the row-sharded DLRM step.  sparse [B, C] int32 row-major holds T bags per sample: table k's
+ * bag is columns col_off[k] .. col_off[k+1] (col_off_host int32 [T + 1], host, col_off[0] = 0, C = col_off[T]); lookup
+ * i = b*C + c.  An id < 0 is padding; an id >= the table's vocabulary is bad; neither is pooled nor gets a gradient.
+ * orx_bag_shard_lookups: rows[i] = row_off[k] + sparse[i] (the global row) for a valid id of column c in table k's bag,
+ *   else -1.  rows [B, C] is the input of orx_lookup_bucket as [B*C, 1] with row_off = {0, G}: the buckets are those
+ *   of the T-table call.  ORX_ERR_INVALID before any device work: null handle / host arrays, B < 0, T outside [1,
+ *   ORX_BAG_MAX_TABLES], col_off[0] or row_off[0] != 0, either decreasing, C = 0, G > 2^31 - 1, B*C > 2^31 - 1, a null
+ *   sparse / rows with B > 0.  B = 0 is a no-op.
+ * orx_bag_segment_sum: the pooled gradient folded onto the unique rows of that bucket call: out[j, :] = the sum over p
+ *   in [grp_off[j], grp_off[j+1]) of v(grp_idx[p]), added in ascending p, where v(b*C + c) = dZ[b, k(c), :] (mode 0,
+ *   sum) or that row divided element-wise by n[b, k(c)] (mode 1, mean; IEEE division before the add), n being the bag's
+ *   valid lookups (slot >= 0, slot from the bucket call, [B*C]; read in mode 1 only).  dZ[b, k, :] is at dZ + b*dz_ld +
+ *   k*dim (dz_ld >= T*dim); out is [n_uniq, dim] contiguous.  One warp per unique row, float4 loads when dim, dz_ld and
+ *   both pointers allow, a scalar path for any dim >= 1, no atomics: repeated calls give the same bits.  Scratch: the
+ *   mean's B*T counts in the handle's own buffer, grown on demand.  ORX_ERR_INVALID before any device work: null handle
+ *   / col_off, T outside [1, ORX_BAG_MAX_TABLES], dim < 1, B < 0, n_uniq < 0 or > B*C, mode outside {0, 1}, dz_ld <
+ *   T*dim, col_off[0] != 0 or decreasing, C = 0, B*C > 2^31 - 1, and with n_uniq > 0 a null dZ / grp_off / grp_idx /
+ *   out, or a null slot in mode 1.  n_uniq = 0 is a no-op. */
+ORX_API int orx_bag_shard_lookups(orx_handle_t h, const int32_t* sparse, int32_t B, int32_t T,
+                                  const int32_t* col_off_host, const int64_t* row_off_host, int32_t* rows,
+                                  orx_stream_t s);
+ORX_API int orx_bag_segment_sum(orx_handle_t h, const float* dZ, int64_t dz_ld, int32_t T, int32_t dim,
+                                const int32_t* col_off_host, int32_t mode, const int32_t* slot, int32_t B,
+                                const int32_t* grp_off, const int32_t* grp_idx, int32_t n_uniq, float* out,
+                                orx_stream_t s);
 
 /* ---- row-sharded GMF / WRMF (openrec_b200/csrc/orx_pointwise_shard.cu, openrec_b200/sharded.py
  * pointwise_step_sharded): the user table, the item table and the item bias are row-sharded per table (row r on rank

@@ -108,6 +108,8 @@ SIGNATURES = {
     "orx_pairwise_grad_rows": [_vp, _i32, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _f, _f, _f, _f, _vp, _vp, _vp],
     "orx_lookup_bucket": [_vp, _vp, _i32, _i32, C.POINTER(_i64), _i32, _vp, _vp, _vp, _vp, _vp, _vp],
     "orx_rows_segment_sum": [_vp, _vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp],
+    "orx_bag_shard_lookups": [_vp, _vp, _i32, _i32, C.POINTER(_i32), C.POINTER(_i64), _vp, _vp],
+    "orx_bag_segment_sum": [_vp, _vp, _i64, _i32, _i32, C.POINTER(_i32), _i32, _vp, _i32, _vp, _vp, _i32, _vp, _vp],
     "orx_pointwise_shard_lookups": [_vp, _vp, _vp, _i32, _i64, _i64, _vp, _vp],
     "orx_pointwise_serve": [_vp, _vp, _vp, _vp, _i32, _i64, _i64, _i64, _vp, _i32, _i64, _vp, _vp, _vp, _vp],
     "orx_pointwise_grad_rows": [_vp, _i32, _vp, _i64, _i32, _vp, _vp, _vp, _i32, _f, _f, _i32, _f, _f, _f, _i32, _vp,

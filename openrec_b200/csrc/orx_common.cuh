@@ -132,6 +132,8 @@ struct orx_ctx {
   OrxHash censor_hash;     // its slots, shape and epoch
   void* bag_ws;            // orx_sharded.cu: orx_bag_sparse_apply's compacted ids and bag counts, its own allocation
   size_t bag_cap;
+  void* bag_cnt_ws;        // orx_dlrm_shard.cu: orx_bag_segment_sum's per-bag valid-id counts, its own allocation
+  size_t bag_cnt_cap;
 };
 
 // Grow a workspace buffer of the handle to at least `need` bytes (*cap = its size in bytes).  Returns at once when it is

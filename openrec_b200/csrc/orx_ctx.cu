@@ -196,6 +196,7 @@ extern "C" int orx_destroy(orx_handle_t h) {
   cudaFree(h->splitk);
   cudaFree(h->censor_ws);
   cudaFree(h->bag_ws);
+  cudaFree(h->bag_cnt_ws);
   cudaFree(h->shard_scratch);
   orx_shard_ws_release(h);
   if (h->side_stream) {

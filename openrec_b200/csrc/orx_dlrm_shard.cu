@@ -222,3 +222,203 @@ extern "C" int orx_rows_segment_sum(orx_handle_t h, const float* src, int64_t sr
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
+
+// ---------------------------------------------------------------------------------------
+// Multi-hot (bag) form of the sharded DLRM step.  sparse [B, C] holds T bags per sample, table k's bag being columns
+// col_off[k] .. col_off[k+1]; lookup i = b*C + c.  orx_bag_shard_lookups maps every id to its global row (the input of
+// an orx_lookup_bucket call with one column and row_off = {0, G}), orx_bag_segment_sum folds the pooled gradient rows
+// onto the unique rows that bucket call found.
+// ---------------------------------------------------------------------------------------
+struct BagShardCols {   // kernel parameter block, copied to shared memory by each block
+  int32_t col_off[ORX_BAG_MAX_TABLES + 1];
+  int64_t row_off[ORX_BAG_MAX_TABLES + 1];
+};
+
+// the table of column c: the largest k < T with col_off[k] <= c (an empty bag is never chosen)
+__device__ __forceinline__ int bag_table_of(const int32_t* s_col, int T, int c) {
+  int lo = 0, hi = T - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (s_col[mid] <= c) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(256) k_bag_shard_lookups(const __grid_constant__ BagShardCols bc, int T, int C,
+                                                           const int32_t* __restrict__ sparse, int64_t n,
+                                                           int32_t* __restrict__ rows) {
+  __shared__ int32_t s_col[ORX_BAG_MAX_TABLES + 1];
+  __shared__ int64_t s_row[ORX_BAG_MAX_TABLES + 1];
+  for (int t = threadIdx.x; t <= T; t += blockDim.x) {
+    s_col[t] = bc.col_off[t];
+    s_row[t] = bc.row_off[t];
+  }
+  __syncthreads();
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int k = bag_table_of(s_col, T, (int)(i % C));
+    const int32_t id = sparse[i];
+    const int64_t lo = s_row[k];
+    rows[i] = id >= 0 && lo + id < s_row[k + 1] ? (int32_t)(lo + id) : -1;
+  }
+}
+
+extern "C" int orx_bag_shard_lookups(orx_handle_t h, const int32_t* sparse, int32_t B, int32_t T,
+                                     const int32_t* col_off_host, const int64_t* row_off_host, int32_t* rows,
+                                     orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr && col_off_host && row_off_host, "null pointer");
+  ORX_REQUIRE(B >= 0 && T >= 1 && T <= ORX_BAG_MAX_TABLES, "B < 0 or T outside [1, ORX_BAG_MAX_TABLES]");
+  ORX_REQUIRE(col_off_host[0] == 0 && row_off_host[0] == 0, "col_off[0] and row_off[0] must be 0");
+  BagShardCols bc;
+  for (int k = 0; k < T; ++k) {
+    ORX_REQUIRE(col_off_host[k + 1] >= col_off_host[k] && row_off_host[k + 1] >= row_off_host[k],
+                "col_off / row_off must be non-decreasing");
+    bc.col_off[k] = col_off_host[k];
+    bc.row_off[k] = row_off_host[k];
+  }
+  bc.col_off[T] = col_off_host[T];
+  bc.row_off[T] = row_off_host[T];
+  const int32_t C = col_off_host[T];
+  ORX_REQUIRE(C >= 1, "no bag columns");
+  ORX_REQUIRE(row_off_host[T] <= INT32_MAX, "the concatenated tables exceed 2^31 - 1 rows");
+  ORX_REQUIRE((int64_t)B * C <= INT32_MAX, "B * C exceeds 2^31 - 1 lookups");
+  if (B == 0) return ORX_OK;
+  ORX_REQUIRE(sparse && rows, "null sparse / rows");
+  ORX_CUDA(cudaSetDevice(h->device));
+  const int64_t n = (int64_t)B * C;
+  k_bag_shard_lookups<<<orx_grid_for(n, 256, h->num_sms), 256, 0, (cudaStream_t)s>>>(bc, T, C, sparse, n, rows);
+  ORX_LAUNCH_CHECK();
+  return ORX_OK;
+}
+
+// cnt[b*T + k] = the valid lookups (slot >= 0) of bag (b, k), as a float.  One warp per bag, 32 columns at a time.
+__global__ void __launch_bounds__(256) k_bag_counts(const __grid_constant__ BagShardCols bc, int T, int C,
+                                                    const int32_t* __restrict__ slot, int64_t bags,
+                                                    float* __restrict__ cnt) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  for (int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < bags; w += nw) {
+    const int64_t b = w / T;
+    const int k = (int)(w - b * T);
+    const int32_t* sl = slot + b * C;
+    int n = 0;
+    for (int c = bc.col_off[k]; c < bc.col_off[k + 1]; c += 32)
+      n += __popc(__ballot_sync(ORX_FULL, c + lane < bc.col_off[k + 1] && __ldg(sl + c + lane) >= 0));
+    if (lane == 0) cnt[w] = (float)n;
+  }
+}
+
+template <bool VEC>
+__device__ __forceinline__ float4 seg_ld(const float* p) {
+  if (VEC) return __ldg(reinterpret_cast<const float4*>(p));
+  return make_float4(__ldg(p), 0.f, 0.f, 0.f);
+}
+
+// One warp per unique row j: out[j] = the sum over p in [grp_off[j], grp_off[j+1]) of lookup grp_idx[p]'s gradient row,
+// dZ[b, k(c), :] (divided by the bag's valid count for a mean, before the add), added in ascending p.  The lookups are
+// decoded 32 at a time, one per lane, and handed out by shuffle; U row loads are issued before they are added.
+// VEC: a lane holds one float4 of a 128-float column chunk, else one float of a 32-float chunk; wider rows take several
+// chunks, each decoding the lookups again.  No atomics: every call gives the same bits.
+template <bool VEC>
+__global__ void __launch_bounds__(256) k_bag_segment_sum(const __grid_constant__ BagShardCols bc, int T, int C,
+                                                         const float* __restrict__ dz, int64_t dz_ld, int dim,
+                                                         const float* __restrict__ cnt,
+                                                         const int32_t* __restrict__ grp_off,
+                                                         const int32_t* __restrict__ grp_idx, int n_uniq,
+                                                         float* __restrict__ out) {
+  constexpr int U = 4, W = VEC ? 4 : 1;
+  const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  __shared__ int32_t s_col[ORX_BAG_MAX_TABLES + 1];
+  for (int t = threadIdx.x; t <= T; t += blockDim.x) s_col[t] = bc.col_off[t];
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const int64_t warps = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t j = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < n_uniq; j += warps) {
+    const int32_t p0 = grp_off[j], p1 = grp_off[j + 1];
+    float* o = out + j * (int64_t)dim;
+    for (int e0 = 0; e0 < dim; e0 += 32 * W) {
+      const int e = e0 + lane * W;
+      const bool on = e < dim;
+      float4 acc = z4;
+      for (int32_t pb = p0; pb < p1; pb += 32) {
+        const int m = min(32, p1 - pb);
+        int64_t src = 0;
+        float nb = 1.f;
+        if (lane < m) {
+          const int32_t i = __ldg(grp_idx + pb + lane);
+          const int32_t b = i / C;
+          const int c = i - b * C;
+          const int k = bag_table_of(s_col, T, c);
+          src = (int64_t)b * dz_ld + (int64_t)k * dim;
+          if (cnt) nb = __ldg(cnt + (int64_t)b * T + k);
+        }
+        for (int q = 0; q < m; q += U) {   // warp-uniform
+          float4 v[U];
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            const int64_t r = __shfl_sync(ORX_FULL, src, (q + u) & 31);
+            v[u] = (q + u < m && on) ? seg_ld<VEC>(dz + r + e) : z4;
+          }
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            const float d = __shfl_sync(ORX_FULL, nb, (q + u) & 31);
+            if (q + u >= m) break;
+            if (cnt) v[u] = make_float4(v[u].x / d, v[u].y / d, v[u].z / d, v[u].w / d);
+            acc.x += v[u].x; acc.y += v[u].y; acc.z += v[u].z; acc.w += v[u].w;
+          }
+        }
+      }
+      if (!on) continue;
+      if (VEC) *reinterpret_cast<float4*>(o + e) = acc;
+      else o[e] = acc.x;
+    }
+  }
+}
+
+extern "C" int orx_bag_segment_sum(orx_handle_t h, const float* dZ, int64_t dz_ld, int32_t T, int32_t dim,
+                                   const int32_t* col_off_host, int32_t mode, const int32_t* slot, int32_t B,
+                                   const int32_t* grp_off, const int32_t* grp_idx, int32_t n_uniq, float* out,
+                                   orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr && col_off_host, "null pointer");
+  ORX_REQUIRE(T >= 1 && T <= ORX_BAG_MAX_TABLES, "T outside [1, ORX_BAG_MAX_TABLES]");
+  ORX_REQUIRE(dim >= 1 && B >= 0 && n_uniq >= 0 && (mode == 0 || mode == 1), "bad sizes / mode");
+  ORX_REQUIRE(dz_ld >= (int64_t)T * dim, "dz_ld < T * dim");
+  ORX_REQUIRE(col_off_host[0] == 0, "col_off[0] must be 0");
+  BagShardCols bc;
+  for (int k = 0; k < T; ++k) {
+    ORX_REQUIRE(col_off_host[k + 1] >= col_off_host[k], "col_off must be non-decreasing");
+    bc.col_off[k] = col_off_host[k];
+    bc.row_off[k] = 0;
+  }
+  bc.col_off[T] = col_off_host[T];
+  bc.row_off[T] = 0;
+  const int32_t C = col_off_host[T];
+  ORX_REQUIRE(C >= 1, "no bag columns");
+  ORX_REQUIRE((int64_t)B * C <= INT32_MAX, "B * C exceeds 2^31 - 1 lookups");
+  ORX_REQUIRE(n_uniq <= (int64_t)B * C, "more unique rows than lookups");
+  if (n_uniq == 0) return ORX_OK;
+  ORX_REQUIRE(dZ && grp_off && grp_idx && out && (mode == 0 || slot), "null pointer");
+  ORX_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)s;
+  float* cnt = nullptr;
+  if (mode == 1) {
+    const int64_t bags = (int64_t)B * T;
+    const int rc = orx_grow(&h->bag_cnt_ws, &h->bag_cnt_cap, sizeof(float) * (size_t)bags);
+    if (rc != ORX_OK) return rc;
+    cnt = static_cast<float*>(h->bag_cnt_ws);
+    int64_t blocks = (bags + 7) / 8;
+    if (blocks > (int64_t)h->num_sms * 32) blocks = (int64_t)h->num_sms * 32;
+    k_bag_counts<<<(int)blocks, 256, 0, st>>>(bc, T, C, slot, bags, cnt);
+    ORX_LAUNCH_CHECK();
+  }
+  const bool vec = (dim & 3) == 0 && (dz_ld & 3) == 0 && (((uintptr_t)dZ | (uintptr_t)out) & 15) == 0;
+  int64_t blocks = ((int64_t)n_uniq + 7) / 8;
+  const int64_t cap = (int64_t)h->num_sms * 64;
+  if (blocks > cap) blocks = cap;
+  if (vec)
+    k_bag_segment_sum<true><<<(int)blocks, 256, 0, st>>>(bc, T, C, dZ, dz_ld, dim, cnt, grp_off, grp_idx, n_uniq, out);
+  else
+    k_bag_segment_sum<false><<<(int)blocks, 256, 0, st>>>(bc, T, C, dZ, dz_ld, dim, cnt, grp_off, grp_idx, n_uniq, out);
+  ORX_LAUNCH_CHECK();
+  return ORX_OK;
+}

@@ -349,6 +349,44 @@ class Engine:
                    "orx_rows_segment_sum")
         return out
 
+    def bag_shard_lookups(self, sparse, col_off, row_off):
+        """sparse int32 [B, C] on the device (table k's bag = columns col_off[k] .. col_off[k+1]), row_off [T + 1] host
+        ints -> int32 [B, C] global rows, -1 for padding and bad ids (orx_bag_shard_lookups in include/orx.h)."""
+        if sparse.dtype != torch.int32 or sparse.dim() != 2 or not sparse.is_contiguous():
+            raise ValueError("sparse: expected a contiguous int32 [B, C] tensor")
+        T = len(col_off) - 1
+        if len(row_off) != T + 1 or sparse.shape[1] != col_off[-1]:
+            raise ValueError("col_off and row_off need T + 1 entries, and sparse col_off[-1] columns")
+        B = sparse.shape[0]
+        out = torch.empty_like(sparse)
+        co = (C.c_int32 * (T + 1))(*[int(x) for x in col_off])
+        ro = (C.c_int64 * (T + 1))(*[int(x) for x in row_off])
+        _lib.check(self.lib.orx_bag_shard_lookups(self.h, _ptr(sparse) if B else None, B, T, co, ro,
+                                                  _ptr(out) if B else None, self.stream()), "orx_bag_shard_lookups")
+        return out
+
+    def bag_segment_sum(self, dz3d, col_off, mode, slot, grp_off, grp_idx, n_uniq, out=None):
+        """dz3d [B, T, D] pooled gradient (any batch stride, rows contiguous), the bag layout col_off [T + 1] and the
+        bucket of the [B*C, 1] lookups (slot, grp_off, grp_idx, n_uniq) -> out [n_uniq, D]: row j = the sum of its
+        lookups' bag gradient rows, each divided by its bag's valid count for a mean (mode 1), in ascending grp_idx
+        position (orx_bag_segment_sum)."""
+        B, T, D = dz3d.shape
+        n_uniq = int(n_uniq)
+        if len(col_off) != T + 1 or dz3d.stride(2) != 1 or dz3d.stride(1) != D:
+            raise ValueError("col_off needs T + 1 entries, and dz3d contiguous [T, D] rows per sample")
+        if n_uniq < 0 or n_uniq + 1 > grp_off.numel():
+            raise ValueError("n_uniq must lie in [0, grp_off.numel() - 1]")
+        if slot.numel() != B * int(col_off[-1]):
+            raise ValueError("slot needs one entry per lookup")
+        if out is None:
+            out = torch.empty((n_uniq, D), dtype=torch.float32, device=dz3d.device)
+        co = (C.c_int32 * (T + 1))(*[int(x) for x in col_off])
+        ld = dz3d.stride(0) if B > 1 else T * D
+        _lib.check(self.lib.orx_bag_segment_sum(self.h, _ptr(dz3d), ld, T, D, co, int(mode), _ptr(slot), B,
+                                                _ptr(grp_off), _ptr(grp_idx), n_uniq, _ptr(out), self.stream()),
+                   "orx_bag_segment_sum")
+        return out
+
     def pairwise_grad_rows(self, kind, rows, dim, uslot, pslot, nslot, inv_B, d_rows, out4, margin=0.5, c_loss=1.0,
                            c_l2=1.0):
         _lib.check(self.lib.orx_pairwise_grad_rows(self.h, kind, _ptr(rows), rows.shape[1], dim, _ptr(uslot),

@@ -307,14 +307,20 @@ class DLRMShard:
     g % world at local row g // world of ``table`` ([max(rows, 1), dim]: a rank without rows keeps a 1-row dummy that
     is never read), with its optimizer slots ``slots`` (s0, s1, None when the optimizer has fewer).  ``bot`` / ``top``
     are this rank's Dense replicas as (kernel, bias or None, act) triples, ``dense_slots`` the (s0, s1) of every kernel
-    and bias in that order (biases that are None skipped)."""
+    and bias in that order (biases that are None skipped).  ``col_off`` ([T + 1], table k's bag = sparse columns
+    col_off[k] .. col_off[k+1]) makes every feature multi-hot, pooled by a sum (``pooling`` 0) or a mean (1); None: one
+    id per table."""
 
     def __init__(self, eng, rank, world, vocab, dim, bot, top, table, slots, dense_slots, *, self_interaction=False,
-                 mode="reference", loss_kind=0, clip=0.0):
+                 mode="reference", loss_kind=0, clip=0.0, col_off=None, pooling=0):
         from .tf2.mlp_ops import DLRMGraph
         self.eng, self.rank, self.world, self.D = eng, rank, world, int(dim)
         self.row_off = row_offsets(vocab)
         self.T, self.G = len(vocab), self.row_off[-1]
+        if col_off is not None and len(col_off) != self.T + 1:
+            raise ValueError("col_off needs T + 1 entries")
+        self.col_off, self.pooling = (None, 0) if col_off is None else ([int(c) for c in col_off], int(pooling))
+        self.C = self.T if col_off is None else self.col_off[-1]      # sparse columns per sample
         self.rows = shard_rows(self.G, rank, world)
         if tuple(table.shape) != (max(self.rows, 1), self.D):
             raise ValueError(f"shard shape {tuple(table.shape)} != {(max(self.rows, 1), self.D)}")
@@ -342,18 +348,27 @@ def _untimed(name):
     pass
 
 
-def _fetch_rows(parts, xchg, lookups, serve, width, equal_batches, timer=None):
+def _bucket(part, lookups):
+    return part.eng.lookup_bucket(lookups, part.row_off, part.world)
+
+
+def _fold(part, d_rows, f):
+    return part.eng.rows_segment_sum(d_rows, f.bucket[3], f.bucket[4], sum(f.send))
+
+
+def _fetch_rows(parts, xchg, lookups, serve, width, equal_batches, timer=None, bucket=_bucket):
     """Fetch every part's unique rows from their owners.  parts[k] has .eng, .world and .row_off; lookups[k] is its
-    int32 [B, T] global-row lookups; serve(part, req) is the owner's reply to the requested local rows req: the rows
-    [len(req), width] first, then whatever the caller keeps.  Runs orx_lookup_bucket, the (count, B) exchange with the
-    step's one host sync (and, with equal_batches, the check that every rank passed the same B), the ids exchange,
-    serve and the rows exchange.  -> per part a _Fetched: the lookup_bucket tuple, the send / receive counts per rank,
-    req, serve's result and got [max(n, 1), width], whose first n = sum(send) rows are the unique rows in bucket order
-    (never empty: orx_pointwise_grad_rows needs a rows pointer)."""
+    int32 [B, T] lookups (B is the batch size that equal_batches compares); serve(part, req) is the owner's reply to
+    the requested local rows req: the rows [len(req), width] first, then whatever the caller keeps.  bucket(part,
+    lookups) is the part's orx_lookup_bucket call (default: over the part's row_off).  Runs the bucket, the (count, B)
+    exchange with the step's one host sync (and, with equal_batches, the check that every rank passed the same B), the
+    ids exchange, serve and the rows exchange.  -> per part a _Fetched: the lookup_bucket tuple, the send / receive
+    counts per rank, req, serve's result and got [max(n, 1), width], whose first n = sum(send) rows are the unique rows
+    in bucket order (never empty: orx_pointwise_grad_rows needs a rows pointer)."""
     timer = timer or _untimed
     R = parts[0].world
     n = len(parts)
-    bk = [p.eng.lookup_bucket(lk, p.row_off, R) for p, lk in zip(parts, lookups)]
+    bk = [bucket(p, lk) for p, lk in zip(parts, lookups)]
     timer("bucket")
     send = [torch.stack([b[0], torch.full_like(b[0], lk.shape[0])], 1) for b, lk in zip(bk, lookups)]   # (count, B)
     recv = [torch.empty_like(x) for x in send]
@@ -377,14 +392,13 @@ def _fetch_rows(parts, xchg, lookups, serve, width, equal_batches, timer=None):
     return [_Fetched(*f) for f in zip(bk, sc, rc, req, served, got)]
 
 
-def _return_grads(parts, xchg, fetched, d_rows, timer=None):
-    """Send the gradients of fetched rows back to their owners: d_rows[k] holds parts[k]'s per-lookup gradient rows
-    (row i for lookup i); orx_rows_segment_sum folds them onto the unique rows in a fixed order, and one exchange takes
-    those to the owners.  Sets each part's .last.  -> per part the gradient rows [len(req), width] of the rows it
-    served, in req's order."""
+def _return_grads(parts, xchg, fetched, d_rows, timer=None, fold=_fold):
+    """Send the gradients of fetched rows back to their owners: fold(part, d_rows[k], fetched[k]) folds parts[k]'s
+    gradients onto its unique rows in a fixed order (default: d_rows[k] holds the per-lookup gradient rows, row i for
+    lookup i, summed by orx_rows_segment_sum), and one exchange takes those to the owners.  Sets each part's .last.
+    -> per part the gradient rows [len(req), width] of the rows it served, in req's order."""
     timer = timer or _untimed
-    g_uniq = [p.eng.rows_segment_sum(d, f.bucket[3], f.bucket[4], sum(f.send))
-              for p, d, f in zip(parts, d_rows, fetched)]
+    g_uniq = [fold(p, d, f) for p, d, f in zip(parts, d_rows, fetched)]
     timer("segment_sum")
     g_rows = [torch.empty(sum(f.recv), g.shape[1], dtype=torch.float32, device=g.device)
               for f, g in zip(fetched, g_uniq)]
@@ -395,15 +409,36 @@ def _return_grads(parts, xchg, fetched, d_rows, timer=None):
     return g_rows
 
 
+def _bag_bucket(part, rows):
+    return part.eng.lookup_bucket(rows.view(-1, 1), [0, part.G], part.world)
+
+
+def _bag_fold(part, dZ, f):
+    return part.eng.bag_segment_sum(dZ, part.col_off, part.pooling, f.bucket[2], f.bucket[3], f.bucket[4], sum(f.send))
+
+
 def _dlrm_fetch(parts, xchg, sparses, equal_batches, timer=None):
     """The row fetch of the sharded DLRM step and inference: _fetch_rows with the owners gathering the requested rows
-    of their shard, then Z = the fetched rows of every lookup.  -> (Z [B, T, D] per part, the _Fetched per part)."""
-    fetched = _fetch_rows(parts, xchg, sparses, lambda p, req: (p.eng.gather(p.table, req),), parts[0].D,
-                          equal_batches, timer)
+    of their shard, then Z = the fetched rows of every lookup, pooled per bag for a multi-hot model.  -> (Z [B, T, D]
+    per part, the _Fetched per part).
+
+    Multi-hot: orx_bag_shard_lookups maps the [B, C] bags to global rows (-1 for padding and bad ids), bucketed as
+    [B*C, 1] lookups of one row space; orx_bag_gather then pools the fetched rows with slot as the bag ids, skipping
+    slot -1, in column order -- the single-GPU pooling of bit copies of the same rows, so the same Z bit for bit."""
+    serve = lambda p, req: (p.eng.gather(p.table, req),)
+    if parts[0].col_off is None:
+        fetched = _fetch_rows(parts, xchg, sparses, serve, parts[0].D, equal_batches, timer)
+    else:
+        rows = [p.eng.bag_shard_lookups(s, p.col_off, p.row_off) for p, s in zip(parts, sparses)]
+        fetched = _fetch_rows(parts, xchg, rows, serve, parts[0].D, equal_batches, timer, bucket=_bag_bucket)
     Zs = []
     for p, f, s in zip(parts, fetched, sparses):
         B = s.shape[0]
-        if sum(f.send):
+        if p.col_off is not None:
+            Z = torch.empty(B, p.T, p.D, dtype=torch.float32, device=s.device)
+            p.eng.bag_gather([f.got] * p.T, f.bucket[2].view(B, p.C), p.col_off, p.pooling, Z.view(B, p.T * p.D))
+            Zs.append(Z)
+        elif sum(f.send):
             Zs.append(p.eng.gather(f.got, f.bucket[2]).view(B, p.T, p.D))     # slot -1 (a bad id) -> the zero row
         else:
             Zs.append(torch.zeros(B, p.T, p.D, dtype=torch.float32, device=s.device))
@@ -413,19 +448,21 @@ def _dlrm_fetch(parts, xchg, sparses, equal_batches, timer=None):
 def dlrm_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, timer=None):
     """One synchronous training step of a row-sharded DLRM on the global batch (the union of every rank's batch; every
     rank passes the same local batch size).  parts: the DLRMShard of each rank this process drives; xchg: DistExchange
-    or LoopbackExchange; batches[k] = (dense [B, n_dense] f32, sparse [B, T] int32, label [B] f32) of parts[k];
+    or LoopbackExchange; batches[k] = (dense [B, n_dense] f32, sparse [B, T] int32 -- [B, C] bags for a multi-hot
+    model --, label [B] f32) of parts[k];
     opt_args = (kind, lr, eps, beta1, beta2, step).  ``timer(name)``, when given, is called after each phase (the
     benchmark's per-phase split).  -> per part a [4] device tensor whose [0] is the GLOBAL loss, identical on every rank.
 
     The embedding rows of the batch are deduplicated before they travel (orx_lookup_bucket), the per-lookup gradient
-    rows are folded onto those unique rows in a fixed order (orx_rows_segment_sum) and each owner's orx_sparse_apply
-    dedups across all ranks' requests -- Keras' sparse apply on the global batch.  The Dense gradients and the loss
-    travel in one all-reduce; every replica then applies the same summed gradient."""
+    rows are folded onto those unique rows in a fixed order (orx_rows_segment_sum; orx_bag_segment_sum reads a
+    multi-hot model's pooled gradient rows directly, divided by the bag's valid count for a mean) and each owner's
+    orx_sparse_apply dedups across all ranks' requests -- Keras' sparse apply on the global batch.  The Dense gradients
+    and the loss travel in one all-reduce; every replica then applies the same summed gradient."""
     timer = timer or _untimed
     R = parts[0].world
     for p, (dense, sparse, _) in zip(parts, batches):
-        if sparse.dim() != 2 or sparse.shape[1] != p.T:
-            raise ValueError(f"sparse features must be [B, {p.T}]")
+        if sparse.dim() != 2 or sparse.shape[1] != p.C:
+            raise ValueError(f"sparse features must be [B, {p.C}]")
         if sparse.shape[0] < 1 or dense.shape[0] != sparse.shape[0]:
             raise ValueError("the sharded DLRM step needs B >= 1 samples, with as many dense rows as sparse rows")
     Zs, fetched = _dlrm_fetch(parts, xchg, [b[1] for b in batches], True, timer)
@@ -436,7 +473,10 @@ def dlrm_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, timer=None):
         caches.append(c)
         grads.append(p.graph.backward(c))
     timer("fwd_bwd")
-    g_rows = _return_grads(parts, xchg, fetched, [dZ.view(-1, p.D) for p, (dZ, _, _) in zip(parts, grads)], timer)
+    if parts[0].col_off is None:
+        g_rows = _return_grads(parts, xchg, fetched, [dZ.view(-1, p.D) for p, (dZ, _, _) in zip(parts, grads)], timer)
+    else:
+        g_rows = _return_grads(parts, xchg, fetched, [dZ for dZ, _, _ in grads], timer, fold=_bag_fold)
     for p, f, g in zip(parts, fetched, g_rows):
         o = p.eng.make_opt(*opt_args)
         p.eng.sparse_apply(p.eng.make_table(p.table, *p.slots), f.req, g, o)    # ADAM_DENSE: the owner sweeps its shard
@@ -463,8 +503,8 @@ def dlrm_inference_sharded(parts, xchg, batches):
     """DLRM.inference of row-sharded tables, a collective call: batches[k] = (dense, sparse) of parts[k], any B >= 0
     per rank.  -> per part its predictions [B]."""
     for p, (dense, sparse) in zip(parts, batches):
-        if sparse.dim() != 2 or sparse.shape[1] != p.T or dense.shape[0] != sparse.shape[0]:
-            raise ValueError(f"sparse features must be [B, {p.T}] with as many dense rows")
+        if sparse.dim() != 2 or sparse.shape[1] != p.C or dense.shape[0] != sparse.shape[0]:
+            raise ValueError(f"sparse features must be [B, {p.C}] with as many dense rows")
     Zs = _dlrm_fetch(parts, xchg, [b[1] for b in batches], False)[0]
     out = []
     for p, (dense, sparse), Z in zip(parts, batches, Zs):

@@ -13,6 +13,28 @@ from ..mlp_ops import ACT, DLRMGraph
 from ..modules import MLP, LatentFactor, SecondOrderFeatureInteraction
 
 
+def bag_layout(bag_sizes, pooling, n_tables):
+    """The checked multi-hot layout of DLRM / ShardedDLRM: -> (bag sizes, col_off [T + 1] with table k's bag at columns
+    col_off[k] .. col_off[k+1], pooling 0 for 'sum' / 1 for 'mean'); the first two are None when bag_sizes is None.
+    ValueError for an unknown pooling, a bag_sizes length other than n_tables, a size < 1 or more than
+    ORX_BAG_MAX_TABLES tables."""
+    if pooling not in ("sum", "mean"):
+        raise ValueError(f"pooling must be 'sum' or 'mean', got {pooling!r}")
+    sizes = col_off = None
+    if bag_sizes is not None:
+        sizes = [int(L) for L in bag_sizes]
+        if len(sizes) != n_tables:
+            raise ValueError(f"bag_sizes has {len(sizes)} entries for {n_tables} embedding tables")
+        if any(L < 1 for L in sizes):
+            raise ValueError("every bag size must be >= 1")
+        if len(sizes) > ORX_BAG_MAX_TABLES:
+            raise ValueError(f"multi-hot DLRM takes at most {ORX_BAG_MAX_TABLES} tables")
+        col_off = [0]
+        for L in sizes:
+            col_off.append(col_off[-1] + L)
+    return sizes, col_off, 0 if pooling == "sum" else 1
+
+
 class DLRM(Model):
     def __init__(self, m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op="dot", arch_interaction_itself=False,
                  sigmoid_bot=False, sigmoid_top=True, loss_func="mse", loss_threshold=0.0,
@@ -25,22 +47,7 @@ class DLRM(Model):
         or 'mean' over the bag's valid ids).  An id < 0 is padding; an id >= the vocabulary adds nothing and gets no
         gradient; a bag without a valid id pools to the zero row.  None (the default): one id per table, [B, T]."""
         super().__init__()
-        if pooling not in ("sum", "mean"):
-            raise ValueError(f"pooling must be 'sum' or 'mean', got {pooling!r}")
-        self._col_off = None
-        if bag_sizes is not None:
-            sizes = [int(L) for L in bag_sizes]
-            if len(sizes) != len(ln_emb):
-                raise ValueError(f"bag_sizes has {len(sizes)} entries for {len(ln_emb)} embedding tables")
-            if any(L < 1 for L in sizes):
-                raise ValueError("every bag size must be >= 1")
-            if len(sizes) > ORX_BAG_MAX_TABLES:
-                raise ValueError(f"multi-hot DLRM takes at most {ORX_BAG_MAX_TABLES} tables")
-            self._col_off = [0]
-            for L in sizes:
-                self._col_off.append(self._col_off[-1] + L)
-        self._bag_sizes = None if bag_sizes is None else sizes
-        self._pooling = 0 if pooling == "sum" else 1
+        self._bag_sizes, self._col_off, self._pooling = bag_layout(bag_sizes, pooling, len(ln_emb))
         self._m_spa = int(m_spa)
         self._loss_threshold = loss_threshold
         self._loss_func = loss_func

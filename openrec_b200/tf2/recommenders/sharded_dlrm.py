@@ -8,7 +8,12 @@ replica of every Dense layer.  Every rank calls the model with ITS part of the g
 on every rank); ``apply_gradients`` runs one sharded step (openrec_b200.sharded.dlrm_step_sharded) and the loss is that
 of the GLOBAL batch, identical on every rank.  SGD, Adagrad, LazyAdam and Keras ``Adam()`` (each owner sweeps its own
 shard, which is the whole-table sweep).  ``openrec_b200.tf2.checkpoint`` saves one rank's shard and replicas (one file
-per rank)."""
+per rank).
+
+``bag_sizes`` / ``pooling`` make every sparse feature multi-hot, exactly as in DLRM: ``sparse_features`` is [B, sum(L)],
+table k's bag being its column block, pooled by a sum or a mean over the bag's valid ids.  The bags' rows are
+deduplicated over this rank's batch before they travel, and each owner applies every row once per step.  The shard
+layout, and so a checkpoint, does not depend on the bags."""
 from __future__ import annotations
 
 import sys
@@ -20,15 +25,16 @@ from ...sharded import DistExchange, DLRMShard, dlrm_inference_sharded, dlrm_ste
 from ...tfshim.core import LazyScalar, StepNode, Tensor
 from ..mlp_ops import ACT, interaction_width
 from ..modules import MLP
-from .dlrm import DLRM
+from .dlrm import DLRM, bag_layout
 from .sharded import _ShardedModel
 
 
 class ShardedDLRM(_ShardedModel):
     def __init__(self, m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op="dot", arch_interaction_itself=False,
                  sigmoid_bot=False, sigmoid_top=True, loss_func="mse", loss_threshold=0.0,
-                 interaction_mode="reference", seed=0):
+                 interaction_mode="reference", seed=0, bag_sizes=None, pooling="sum"):
         super().__init__()
+        self._bag_sizes, self._col_off, self._pooling = bag_layout(bag_sizes, pooling, len(ln_emb))
         if arch_interaction_op != "dot" and self._arch_interaction_op != "cat":   # as DLRM: AttributeError (SURVEY Q2)
             sys.exit("ERROR: arch_interaction_op=" + self._arch_interaction_op + " is not supported")
         if loss_func not in ("mse", "bce"):
@@ -74,11 +80,16 @@ class ShardedDLRM(_ShardedModel):
         return DLRMShard(self._eng, self._rank, self._world, self._vocab, self._m_spa, layers(self._mlp_bot),
                          layers(self._mlp_top), self.embedding_shard.t, slots, dense_slots,
                          self_interaction=self._self_interaction, mode=self._interaction_mode,
-                         loss_kind=0 if self._loss_func == "mse" else 1, clip=clip)
+                         loss_kind=0 if self._loss_func == "mse" else 1, clip=clip, col_off=self._col_off,
+                         pooling=self._pooling)
 
     def _inputs(self, dense_features, sparse_features, label=None):
         dense, sparse, lab = DLRM._inputs(dense_features, sparse_features, label)
-        if sparse.dim() != 2 or sparse.shape[1] != len(self._vocab):
+        if self._col_off is not None:
+            if sparse.dim() != 2 or sparse.shape[1] != self._col_off[-1]:
+                raise ValueError(f"sparse_features must be [B, {self._col_off[-1]}] (the sum of bag_sizes), got "
+                                 f"{tuple(sparse.shape)}")
+        elif sparse.dim() != 2 or sparse.shape[1] != len(self._vocab):
             raise ValueError(f"sparse features must be [B, {len(self._vocab)}] (one id per table)")
         return dense, sparse, lab
 
