@@ -23,6 +23,12 @@
  *    thread-local message.  There is no CPU fallback: without a CUDA device every compute
  *    entry point fails with ORX_ERR_CUDA.
  *  - tables are row-major float32 [rows, dim] with 64-bit row offsets; ids are int32.
+ *  - alignment: a table, its slot rows s0 / s1, GMF's w and a gather's output may start at any 4-byte-aligned address
+ *    (a view into one flat parameter buffer, say).  A call moves rows as 128-bit float4 only when every caller pointer
+ *    that path reads or writes through is 16-byte aligned; otherwise it takes the entry point's scalar or generic path,
+ *    with the same results (a sparse step then records STEP_GENERIC, orx_censor_shard CENSOR_SCALAR).  The one
+ *    exception is orx_shard_step, which has no scalar path: it refuses local shards or slot rows off a 16-byte boundary
+ *    with ORX_ERR_INVALID before any device work.
  */
 #ifndef ORX_H_
 #define ORX_H_
@@ -123,14 +129,17 @@ enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_SIMT = 1,     /* k_gemm: fp32 SIMT tiles */
   ORX_VARIANT_INTERACT_WARP = 2, /* k_interact_{fwd,bwd}_warp: one warp per sample */
   ORX_VARIANT_INTERACT = 3,      /* k_interact_{fwd,bwd}: one CTA per sample */
-  ORX_VARIANT_STEP = 4,          /* k_pair_step / k_point_step specialised on D (32, 64, 128, 256), one register buffer */
+  ORX_VARIANT_STEP = 4,          /* k_pair_step / k_point_step specialised on D (32, 64, 128, 256), one register buffer;
+                                    tables, slot rows and w 16-byte aligned */
   ORX_VARIANT_STEP_PIPE = 5,     /* k_pair_step with the register double buffer (PIPE) */
-  ORX_VARIANT_STEP_GENERIC = 6,  /* k_pair_generic / k_point_generic (fused-step mode): any D */
+  ORX_VARIANT_STEP_GENERIC = 6,  /* k_pair_generic / k_point_generic (fused-step mode): any D, any 4-byte-aligned table */
   ORX_VARIANT_RANK_SMEM = 7,     /* k_score_rank: thresholds and histograms of a user tile in shared memory */
   ORX_VARIANT_RANK_GLOBAL = 8,   /* k_score_rank: thresholds and histograms in the handle's global scratch */
   ORX_VARIANT_TOPK = 9,          /* k_score_topk + k_topk_merge: candidate lists in the handle's global scratch */
-  ORX_VARIANT_CENSOR_VEC = 10,   /* k_censor_shard, one float4 per lane (dim % 4 == 0 && dim <= 128) */
-  ORX_VARIANT_CENSOR_SCALAR = 11 /* k_censor_shard, lane-strided scalar rows (any other dim) */
+  ORX_VARIANT_CENSOR_VEC = 10,   /* k_censor_shard, one float4 per lane (dim % 4 == 0 && dim <= 128, tab 16-byte
+                                    aligned) */
+  ORX_VARIANT_CENSOR_SCALAR = 11 /* k_censor_shard, lane-strided scalar rows (any other dim, or tab off a 16-byte
+                                    boundary) */
 };
 #define ORX_DISPATCH_LOG_CAP 64
 ORX_API int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec_host, int32_t cap, int32_t* n_host);
@@ -403,7 +412,9 @@ ORX_API int orx_rows_scale(orx_handle_t h, float* x, int64_t rows, int32_t dim, 
  *   All ranks announce, or none.  Other calls on the handle may come between steps and between phases.
  *   out4 = { loss, l2_loss (GLOBAL batch, identical on every rank), skipped triplets of this rank, staged rows }.
  *   The sticky error word flags[4*64] is 0 or: 1 a peer never arrived within timeout_ms, 2 more triplets routed to this
- *   home than home_cap, 3 / 4 request / gradient inbox too small.  SGD, Adagrad and row-sparse Adam. */
+ *   home than home_cap, 3 / 4 request / gradient inbox too small.  SGD, Adagrad and row-sparse Adam.
+ *   user / item var, s0 and s1 must be 16-byte aligned (every launch moves them as float4): a base off a 16-byte
+ *   boundary returns ORX_ERR_INVALID, naming the pointer, before any device work. */
 typedef struct {
   int32_t world, rank, dim, batch_cap, home_cap, req_cap, gin_cap, timeout_ms;
   void *tripbox, *idbox, *got, *gotb, *gin, *ginb, *meta, *flags;   /* DEVICE arrays of `world` pointers */

@@ -194,6 +194,15 @@ static inline bool orx_opt_kind_ok(int kind) { return kind >= ORX_OPT_SGD && kin
 // s1 for both Adams (ADAM_DENSE's sweep keeps m and v there).  Null tables are skipped.
 bool orx_opt_slots_ok(int kind, std::initializer_list<const orx_table_t*> tabs);
 
+// True when every pointer is 16-byte aligned (a null pointer, an absent slot row, counts as aligned).  The one rule of
+// the 128-bit paths on caller memory (orx.h, Conventions): a table, slot row, dense weight or output buffer may start at
+// any 4-byte-aligned address, and a call takes a float4 path only when this holds for every caller pointer that path
+// reads or writes through.  Buffers the library carves itself (OrxCarve: 256-byte aligned) need no check.
+template <typename... P>
+static inline bool orx_aligned16(const P*... p) {
+  return (((uintptr_t)0 | ... | (uintptr_t)p) & 15) == 0;
+}
+
 // Grid of a grid-stride loop over n items: one thread per item, at most 32 blocks per SM, at least one block.
 static inline int orx_grid_for(int64_t n, int threads, int num_sms) {
   const int64_t b = (n + threads - 1) / threads;
@@ -554,7 +563,9 @@ struct TailArgs : SparseArgs {
 // 128 contiguous bytes per access), and issues all of a row's loads before the first use: 12 independent 128-bit
 // loads per lane in flight at D = 128.  Table and slot rows evict-first, staging rows (G) at normal priority: the
 // step's red.adds left them in L2.
-template <int OPT>
+// VEC: the table and slot rows of a are 16-byte aligned (orx_aligned16, decided by the launcher); with D % 4 == 0 the rows
+// then move as float4, else lane-strided scalars.
+template <int OPT, bool VEC>
 __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni) {
   typedef OrxOptSlots<OPT> SL;
   constexpr bool ZERO_ONLY = SL::STAGE_ONLY;
@@ -574,7 +585,7 @@ __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni)
     float* W = (is_u ? a.U : a.I) + (int64_t)id * D;
     float* P0 = (is_u ? a.Us0 : a.Is0) + (int64_t)id * D;
     float* P1 = (is_u ? a.Us1 : a.Is1) + (int64_t)id * D;
-    if ((D & 3) == 0) {  // 128-bit path: float4 index sl + 8k
+    if (VEC && (D & 3) == 0) {  // 128-bit path: float4 index sl + 8k
       const int nq = D >> 2;
       for (int e0 = 0; e0 < nq; e0 += 32) {
         float4 g[4], w[4], s0v[4], s1v[4];
@@ -653,6 +664,7 @@ int orx_sparse_unfused(orx_ctx* c, int B, float loss_scale, float* out4,
 // taken from its side's table of index set ix and staging rows.  Runs before the tail, which zeroes the staging rows.
 int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
                            const OrxIndexSet& ix, const OrxOptDev& o, cudaStream_t st);
+// k_sparse_tail over ta, its 128-bit row path chosen by the alignment of ta's table and slot rows (orx_aligned16).
 int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st);
 int orx_launch_reduce_partials(const float* partials, int n, float loss_scale, float* out4, cudaStream_t st);
 // index of n samples (a[t], b0[t]) or (a[t], b0[t], b1[t]); only samples whose ids are all in range are inserted

@@ -9,12 +9,15 @@
 // ---------------------------------------------------------------------------------------
 // K5: out[b*out_ld + :D] = tab[ids[b*id_stride], :D]   (dlrm.py:83-85, one call per sparse feature)
 // ---------------------------------------------------------------------------------------
+// VEC: tab and out are 16-byte aligned (orx_gather_strided decides); with D and out_ld multiples of 4 the rows then move
+// as float4 (the row shape is tested here, as in k_gather)
+template <bool VEC>
 __global__ void __launch_bounds__(256) k_gather_strided(const float* __restrict__ tab, int64_t rows, int D,
                                                         const int32_t* __restrict__ ids, int64_t id_stride, int64_t n,
                                                         float* __restrict__ out, int64_t out_ld, int32_t* n_bad) {
   const int lane = threadIdx.x & 31;
   const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const bool vec = ((D & 3) == 0) && ((out_ld & 3) == 0);
+  const bool vec = VEC && ((D & 3) == 0) && ((out_ld & 3) == 0);
   for (int64_t b = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < n; b += nw) {
     const int64_t id = ids[b * id_stride];
     const bool ok = id >= 0 && id < rows;
@@ -38,7 +41,11 @@ extern "C" int orx_gather_strided(orx_handle_t h, const float* tab, int64_t rows
   ORX_CUDA(cudaSetDevice(h->device));
   int64_t blocks = (n + 7) / 8;
   if (blocks > (int64_t)h->num_sms * 32) blocks = (int64_t)h->num_sms * 32;
-  k_gather_strided<<<(int)blocks, 256, 0, (cudaStream_t)s>>>(tab, rows, dim, ids, id_stride, n, out, out_ld, n_bad);
+  cudaStream_t st = (cudaStream_t)s;
+  if (orx_aligned16(tab, out))
+    k_gather_strided<true><<<(int)blocks, 256, 0, st>>>(tab, rows, dim, ids, id_stride, n, out, out_ld, n_bad);
+  else
+    k_gather_strided<false><<<(int)blocks, 256, 0, st>>>(tab, rows, dim, ids, id_stride, n, out, out_ld, n_bad);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
@@ -295,7 +302,7 @@ __global__ void __launch_bounds__(INTER_WARPS * 32) k_interact_bwd_warp(const fl
 
 static bool inter_fast_ok(int F, int D, int mode, const void* a, const void* b, int64_t lda, int64_t ldb) {
   return mode == 1 && F >= 2 && F <= 32 && (D & 3) == 0 && D <= 128 && (lda & 3) == 0 && (ldb & 3) == 0 &&
-         ((((uintptr_t)a) | ((uintptr_t)b)) & 15) == 0;
+         orx_aligned16(a, b);
 }
 
 extern "C" int orx_interact_fwd(orx_handle_t h, const float* emb, int64_t emb_ld, const float* dense,
@@ -333,7 +340,7 @@ extern "C" int orx_interact_bwd(orx_handle_t h, const float* emb, int64_t emb_ld
   if (B == 0) return ORX_OK;
   ORX_CUDA(cudaSetDevice(h->device));
   if (inter_fast_ok(F, D, mode, emb ? (const void*)emb : (const void*)dense, dense, emb_ld, dense_ld) && (demb_ld & 3) == 0 &&
-      (ddense_ld & 3) == 0 && ((((uintptr_t)(demb ? (const void*)demb : (const void*)ddense)) | ((uintptr_t)ddense)) & 15) == 0) {
+      (ddense_ld & 3) == 0 && orx_aligned16(demb ? (const void*)demb : (const void*)ddense, ddense)) {
     const size_t sm = (size_t)INTER_WARPS * (sizeof(float4) * (size_t)F * 32 + sizeof(float) * (size_t)F * 36);
     ORX_CUDA(cudaFuncSetAttribute(k_interact_bwd_warp, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     int grid = (B + INTER_WARPS - 1) / INTER_WARPS;
@@ -696,14 +703,14 @@ extern "C" int orx_bag_gather(orx_handle_t h, const float* const* tabs_host, con
   ORX_REQUIRE(out_ld >= (int64_t)T * dim, "out_ld < T * dim");
   ORX_REQUIRE(col_off_host[0] >= 0 && col_off_host[T] <= ld, "col_off outside [0, ld]");
   BagTables bt;
-  bool aligned = ((uintptr_t)out & 15) == 0;
+  bool aligned = orx_aligned16(out);
   for (int k = 0; k < T; ++k) {
     ORX_REQUIRE(tabs_host[k] != nullptr && rows_host[k] > 0, "null table / empty vocabulary");
     ORX_REQUIRE(col_off_host[k + 1] >= col_off_host[k], "col_off decreasing");
     bt.tab[k] = tabs_host[k];
     bt.rows[k] = rows_host[k];
     bt.col_off[k] = col_off_host[k];
-    aligned = aligned && ((uintptr_t)tabs_host[k] & 15) == 0;
+    aligned = aligned && orx_aligned16(tabs_host[k]);
   }
   bt.col_off[T] = col_off_host[T];
   if (B == 0) return ORX_OK;

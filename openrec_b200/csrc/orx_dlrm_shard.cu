@@ -213,7 +213,7 @@ extern "C" int orx_rows_segment_sum(orx_handle_t h, const float* src, int64_t sr
   ORX_REQUIRE(src && grp_off && grp_idx && out, "null pointer");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
-  const bool vec = (dim & 3) == 0 && (src_ld & 3) == 0 && (((uintptr_t)src | (uintptr_t)out) & 15) == 0;
+  const bool vec = (dim & 3) == 0 && (src_ld & 3) == 0 && orx_aligned16(src, out);
   int64_t blocks = ((int64_t)n_uniq + 7) / 8;
   const int64_t cap = (int64_t)h->num_sms * 64;
   if (blocks > cap) blocks = cap;
@@ -411,7 +411,7 @@ extern "C" int orx_bag_segment_sum(orx_handle_t h, const float* dZ, int64_t dz_l
     k_bag_counts<<<(int)blocks, 256, 0, st>>>(bc, T, C, slot, bags, cnt);
     ORX_LAUNCH_CHECK();
   }
-  const bool vec = (dim & 3) == 0 && (dz_ld & 3) == 0 && (((uintptr_t)dZ | (uintptr_t)out) & 15) == 0;
+  const bool vec = (dim & 3) == 0 && (dz_ld & 3) == 0 && orx_aligned16(dZ, out);
   int64_t blocks = ((int64_t)n_uniq + 7) / 8;
   const int64_t cap = (int64_t)h->num_sms * 64;
   if (blocks > cap) blocks = cap;

@@ -40,13 +40,15 @@ extern "C" int orx_fill_uniform(orx_handle_t h, float* dst, int64_t n, float lo,
 // ---------------------------------------------------------------------------------------
 // LatentFactor.__call__ (Embedding.call): out[b,:] = tab[ids[b],:]
 // ---------------------------------------------------------------------------------------
-template <typename IdT>
+// VEC: tab and out are 16-byte aligned (orx_gather decides); with D % 4 == 0 the rows then move as float4.  The row
+// shape is tested here, so that the VEC instance compiles to what the kernel was before the pointer gate.
+template <typename IdT, bool VEC>
 __global__ void __launch_bounds__(256) k_gather(const float* __restrict__ tab, int64_t rows, int D,
                                                 const IdT* __restrict__ ids, int64_t n, float* __restrict__ out,
                                                 int32_t* n_bad) {
   const int lane = threadIdx.x & 31;
   const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const bool vec = (D & 3) == 0;
+  const bool vec = VEC && (D & 3) == 0;
   for (int64_t b = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; b < n; b += nw) {
     const int64_t id = (int64_t)ids[b];
     const bool ok = id >= 0 && id < rows;
@@ -70,10 +72,12 @@ extern "C" int orx_gather(orx_handle_t h, const float* tab, int64_t rows, int32_
   ORX_CUDA(cudaSetDevice(h->device));
   int64_t blocks = (n + 7) / 8;
   if (blocks > (int64_t)h->num_sms * 32) blocks = (int64_t)h->num_sms * 32;
-  if (id_is_i64)
-    k_gather<int64_t><<<(int)blocks, 256, 0, (cudaStream_t)s>>>(tab, rows, dim, (const int64_t*)ids, n, out, n_bad);
-  else
-    k_gather<int32_t><<<(int)blocks, 256, 0, (cudaStream_t)s>>>(tab, rows, dim, (const int32_t*)ids, n, out, n_bad);
+  orx_dispatch<0, 1>(orx_aligned16(tab, out) ? 1 : 0, [&](auto V) {
+    constexpr bool VEC = decltype(V)::value == 1;
+    cudaStream_t st = (cudaStream_t)s;
+    if (id_is_i64) k_gather<int64_t, VEC><<<(int)blocks, 256, 0, st>>>(tab, rows, dim, (const int64_t*)ids, n, out, n_bad);
+    else k_gather<int32_t, VEC><<<(int)blocks, 256, 0, st>>>(tab, rows, dim, (const int32_t*)ids, n, out, n_bad);
+  });
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
@@ -83,12 +87,14 @@ extern "C" int orx_gather(orx_handle_t h, const float* tab, int64_t rows, int32_
 // warp to insert an id owns the row), row <- row / max(||row||, min_norm).
 // ---------------------------------------------------------------------------------------
 // The censor of up to 8 rows of one warp: lane k < 8 holds row k in my_id (-1: none; other lanes' values are not read).
-// D % 4 == 0 && D <= 128: one float4 per lane, all 8 rows loaded before the first norm is reduced; otherwise one row at
-// a time, lane-strided.  Every lane of the warp calls it.  (The row shape is tested here rather than passed in: so
-// k_censor compiles to the same SASS as before the function was factored out of it.)
+// VEC (tab 16-byte aligned, decided by the launcher) && D % 4 == 0 && D <= 128: one float4 per lane, all 8 rows loaded
+// before the first norm is reduced; otherwise one row at a time, lane-strided.  Every lane of the warp calls it.  (The
+// row shape is tested here rather than passed in: so k_censor<true> compiles to the same SASS as k_censor did before
+// the function was factored out of it.)
+template <bool VEC>
 __device__ __forceinline__ void orx_censor_rows8(float* tab, int D, int32_t my_id, float min_norm) {
   const int lane = threadIdx.x & 31;
-  if ((D & 3) == 0 && D <= 128) {
+  if (VEC && (D & 3) == 0 && D <= 128) {
     const int nq = D >> 2;
     float4 v[8];
 #pragma unroll
@@ -125,6 +131,7 @@ __device__ __forceinline__ void orx_censor_rows8(float* tab, int D, int32_t my_i
 // A warp takes 8 ids per iteration: lanes 0..7 load the ids and claim the rows in the hash in parallel, then (128-bit path)
 // all 8 rows are loaded before the first norm is reduced -- one row per warp left the kernel latency-bound (id -> hash ->
 // row -> reduce -> divide -> store: 23 us for 65 536 ids at D = 128, three of them per UCML step).
+template <bool VEC>
 __global__ void __launch_bounds__(256) k_censor(float* tab, int64_t rows, int D, const int32_t* __restrict__ ids,
                                                 int n, float min_norm, OrxHash hsh) {
   const int lane = threadIdx.x & 31;
@@ -135,7 +142,7 @@ __global__ void __launch_bounds__(256) k_censor(float* tab, int64_t rows, int D,
       const int32_t id = ids[b0 + lane];
       if (id >= 0 && (int64_t)id < rows && orx_hash_insert(hsh, id, 2) == 0u) my_id = id;   // first claim owns the row
     }
-    orx_censor_rows8(tab, D, my_id, min_norm);
+    orx_censor_rows8<VEC>(tab, D, my_id, min_norm);
   }
 }
 
@@ -145,6 +152,7 @@ __global__ void __launch_bounds__(256) k_censor(float* tab, int64_t rows, int D,
 // at once (coalesced; about 8 owned ones, and k_censor's 8 ids per warp at world 1), the owned lanes claim their local
 // row in the dedup hash, and the first claims are compacted into a per-warp queue; every 8 queued rows, and once at the
 // end, go through orx_censor_rows8, the arithmetic of k_censor.
+template <bool VEC>
 __global__ void __launch_bounds__(256) k_censor_shard(float* tab, int D, int64_t total_rows, int world, int rank,
                                                       const int32_t* __restrict__ ids, int n_per_block,
                                                       int64_t block_stride, int n, int chunk, float min_norm,
@@ -167,15 +175,16 @@ __global__ void __launch_bounds__(256) k_censor_shard(float* tab, int D, int64_t
     __syncwarp();
     const int queued = qn + __popc(claim);
     int head = 0;
-    for (; queued - head >= 8; head += 8) orx_censor_rows8(tab, D, lane < 8 ? q[head + lane] : -1, min_norm);
+    for (; queued - head >= 8; head += 8) orx_censor_rows8<VEC>(tab, D, lane < 8 ? q[head + lane] : -1, min_norm);
     const int32_t rest = lane < queued - head ? q[head + lane] : -1;   // the < 8 rows left move to the queue's front
     __syncwarp();
     if (lane < queued - head) q[lane] = rest;
     __syncwarp();
     qn = queued - head;
   }
-  if (qn > 0) orx_censor_rows8(tab, D, lane < qn ? q[lane] : -1, min_norm);
+  if (qn > 0) orx_censor_rows8<VEC>(tab, D, lane < qn ? q[lane] : -1, min_norm);
 }
+
 
 extern "C" int orx_censor(orx_handle_t h, float* tab, int64_t rows, int32_t dim, const int32_t* ids, int32_t n,
                           float min_norm, orx_stream_t s) {
@@ -190,7 +199,8 @@ extern "C" int orx_censor(orx_handle_t h, float* tab, int64_t rows, int32_t dim,
   if ((rc = orx_take_epoch(ix.u, st))) return rc;   // the dedup hash needs no clearing: a new epoch empties it
   int blocks = (n + 63) / 64;                 // 8 warps x 8 ids per block and iteration
   if (blocks > h->num_sms * 8) blocks = h->num_sms * 8;
-  k_censor<<<blocks, 256, 0, st>>>(tab, rows, dim, ids, n, min_norm, ix.u);
+  if (orx_aligned16(tab)) k_censor<true><<<blocks, 256, 0, st>>>(tab, rows, dim, ids, n, min_norm, ix.u);
+  else k_censor<false><<<blocks, 256, 0, st>>>(tab, rows, dim, ids, n, min_norm, ix.u);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }
@@ -227,7 +237,8 @@ extern "C" int orx_censor_shard(orx_handle_t h, float* tab, int64_t local_rows, 
   const int64_t n = (int64_t)n_per_block * n_blocks;
   ORX_REQUIRE(n <= ORX_CENSOR_SHARD_MAX_IDS, "more than ORX_CENSOR_SHARD_MAX_IDS ids in one call");
   ORX_REQUIRE((n == 0 || ids) && (owned == 0 || tab), "null pointer");
-  const bool vec = (dim & 3) == 0 && dim <= 128;
+  const bool aligned = orx_aligned16(tab);
+  const bool vec = aligned && (dim & 3) == 0 && dim <= 128;   // orx_censor_rows8's 128-bit path
   orx_log_dispatch(h, ORX_OP_CENSOR_SHARD, vec ? ORX_VARIANT_CENSOR_VEC : ORX_VARIANT_CENSOR_SCALAR, rank, 0, (int)n,
                    (int)(local_rows < INT32_MAX ? local_rows : INT32_MAX), dim, world);
   if (n == 0 || owned == 0) return ORX_OK;
@@ -239,8 +250,10 @@ extern "C" int orx_censor_shard(orx_handle_t h, float* tab, int64_t local_rows, 
   const int chunk = world >= 4 ? 32 : 8 * world;   // ids per warp and iteration: about 8 of them owned
   int64_t blocks = (n + 8 * chunk - 1) / (8 * chunk);
   if (blocks > (int64_t)h->num_sms * 8) blocks = (int64_t)h->num_sms * 8;
-  k_censor_shard<<<(int)blocks, 256, 0, st>>>(tab, dim, total_rows, world, rank, ids, n_per_block, block_stride, (int)n,
-                                              chunk, min_norm, h->censor_hash);
+  orx_dispatch<0, 1>(aligned ? 1 : 0, [&](auto V) {
+    k_censor_shard<decltype(V)::value == 1><<<(int)blocks, 256, 0, st>>>(
+        tab, dim, total_rows, world, rank, ids, n_per_block, block_stride, (int)n, chunk, min_norm, h->censor_hash);
+  });
   ORX_LAUNCH_CHECK();
   return ORX_OK;
 }

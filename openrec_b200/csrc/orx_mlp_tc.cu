@@ -389,7 +389,7 @@ int orx_launch_gemm_tc(orx_ctx* h, int TA, int TB, const float* A, int64_t lda, 
                        int64_t ldc, int M, int N, int K, const float* bias, int act, cudaStream_t st) {
   if (TA == 1 && TB == 1) return ORX_ERR_UNSUPPORTED;
   if (N < 16 || K < 8 || M < 64) return ORX_ERR_UNSUPPORTED;
-  if ((lda & 3) || (ldb & 3) || (((uintptr_t)A | (uintptr_t)Bm) & 15)) return ORX_ERR_UNSUPPORTED;
+  if ((lda & 3) || (ldb & 3) || !orx_aligned16(A, Bm)) return ORX_ERR_UNSUPPORTED;
   const int tiles = ((N + TN - 1) / TN) * ((M + TM - 1) / TM);
   const int nkb = (K + TK - 1) / TK;
   int S = 1;

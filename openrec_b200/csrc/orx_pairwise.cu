@@ -461,12 +461,12 @@ __global__ void __launch_bounds__(256) k_adam_sweep(float* var, float* m, float*
 // ---------------------------------------------------------------------------------------
 
 // ta.I == nullptr: no item side (orx_sparse_apply: one table, in the user-side index set); ta.out4 == nullptr: no loss.
-template <int OPT>
+template <int OPT, bool VEC>
 __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
   __shared__ bool last;
   orx_pdl_wait();
   const int nu = *a.hu.counter, ni = a.I ? *a.hi.counter : 0;
-  orx_tail_rows<OPT>(a, nu, ni);
+  orx_tail_rows<OPT, VEC>(a, nu, ni);
 
   if (blockIdx.x == 0 && a.out4) {
     // deterministic loss reduction; GMF: l2_loss also holds 0.5*sum(w^2) of the PRE-step weight (gmf.py:31-32)
@@ -501,8 +501,11 @@ __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
 
 int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st) {
   const int grid = c->num_sms * 4;  // ~1-2 staged rows per warp: the tail is a latency chain, not bandwidth
+  const bool vec = orx_aligned16(ta.U, ta.Us0, ta.Us1, ta.I, ta.Is0, ta.Is1);
   orx_dispatch_opt(opt_kind, [&](auto O) {
-    orx_launch_pdl(k_sparse_tail<decltype(O)::value>, dim3(grid), dim3(256), 0, st, ta);
+    orx_dispatch<0, 1>(vec ? 1 : 0, [&](auto V) {
+      orx_launch_pdl(k_sparse_tail<decltype(O)::value, decltype(V)::value == 1>, dim3(grid), dim3(256), 0, st, ta);
+    });
   });
   ORX_LAUNCH_CHECK();
   return ORX_OK;
@@ -566,7 +569,9 @@ static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, OrxSte
     orx_launch_pdl(kern, dim3(blocks), dim3(256), 0, st, pa);
   };
   constexpr int PV = LAZY ? ORX_VARIANT_STEP : ORX_VARIANT_STEP_PIPE;
-  switch (pa.D) {
+  // k_pair_step moves table and slot rows as float4: a table or slot base off a 16-byte boundary takes k_pair_generic
+  const bool vec = orx_aligned16(pa.U, pa.Us0, pa.Us1, pa.I, pa.Is0, pa.Is1);
+  switch (vec ? pa.D : 0) {
     case 32: go(k_pair_step<KIND, OPT, 32, 8, 2, !LAZY>, PV, 2, blocks); break;
     case 64: go(k_pair_step<KIND, OPT, 64, 8, 2, !LAZY>, PV, 2, blocks); break;
     case 128:

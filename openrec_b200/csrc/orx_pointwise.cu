@@ -266,7 +266,9 @@ template <int KIND, int OPT>
 static int launch_point_kind_opt(const PointArgs& pa, cudaStream_t st, OrxStepLaunch* out) {
   const int blocks = orx_step_blocks(pa.B);
   *out = {8 * blocks, ORX_VARIANT_STEP, 0};
-  switch (pa.D) {
+  // k_point_step moves table rows, slot rows and GMF's w as float4: a base off a 16-byte boundary takes k_point_generic
+  const bool vec = orx_aligned16(pa.U, pa.Us0, pa.Us1, pa.I, pa.Is0, pa.Is1, pa.W);
+  switch (vec ? pa.D : 0) {
     case 32: k_point_step<KIND, OPT, 32, 8><<<blocks, 256, 0, st>>>(pa); break;
     case 64: k_point_step<KIND, OPT, 64, 8><<<blocks, 256, 0, st>>>(pa); break;
     case 128: k_point_step<KIND, OPT, 128, 8><<<blocks, 256, 0, st>>>(pa); break;

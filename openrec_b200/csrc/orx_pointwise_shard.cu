@@ -85,7 +85,7 @@ extern "C" int orx_pointwise_serve(orx_handle_t h, const float* user_shard, cons
   ORX_REQUIRE((local_users == 0 || user_shard) && (local_items == 0 || (item_shard && bias_shard)), "null shard");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
-  const bool vec = (ld & 3) == 0 && ((uintptr_t)rows & 15) == 0;
+  const bool vec = (ld & 3) == 0 && orx_aligned16(rows);
   const int64_t work = (int64_t)n * (vec ? ld / 4 : ld);
   const int grid = orx_grid_for(work, 256, h->num_sms);
   if (vec)
@@ -352,7 +352,7 @@ extern "C" int orx_pointwise_grad_rows(orx_handle_t h, int32_t kind, const float
   pa.use_sigmoid = use_sigmoid; pa.d_rows = d_rows; pa.partials = h->partials;
   pa.gw_part = gmf ? h->partials + 2 * 8 * (size_t)blocks : nullptr;
   const bool vec = (dim == 32 || dim == 64 || dim == 128 || dim == 256) && (ld & 3) == 0 &&
-                   (((uintptr_t)rows | (uintptr_t)d_rows | (uintptr_t)(gmf ? w : nullptr)) & 15) == 0;
+                   orx_aligned16(rows, d_rows, gmf ? w : nullptr);
   const int variant = vec ? ORX_VARIANT_STEP : ORX_VARIANT_STEP_GENERIC;
   orx_dispatch<ORX_POINT_GMF, ORX_POINT_WRMF>(kind, [&](auto K) {
     constexpr int KD = decltype(K)::value;

@@ -685,7 +685,7 @@ template <int OPT>
 __global__ void __launch_bounds__(256) k_sh_tail(ShardDev x, ShardWs w, TailArgs a, int par) {
   orx_pdl_wait();
   const int nu = *a.hu.counter, ni = *a.hi.counter;
-  orx_tail_rows<OPT>(a, nu, ni);
+  orx_tail_rows<OPT, true>(a, nu, ni);   // orx_shard_step refuses tables off a 16-byte boundary
   if (blockIdx.x == 0 && threadIdx.x == 0) {    // every rank adds the R pairs it holds in rank order: bit-identical totals
     const int32_t* m = x.meta[x.rank];
     float l = 0.f, q = 0.f;
@@ -921,6 +921,17 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
   ORX_REQUIRE(opt->kind == ORX_OPT_SGD || opt->kind == ORX_OPT_ADAGRAD || opt->kind == ORX_OPT_ADAM_LAZY,
               "the sharded step supports SGD, Adagrad and row-sparse Adam");
   ORX_REQUIRE(orx_opt_slots_ok(opt->kind, {user, item, item_bias}), "optimizer slot rows missing");
+  {   // every launch moves local table and slot rows as float4 and there is no scalar form: refuse a misaligned base
+    const struct { const float* p; const char* name; } bases[6] = {
+        {user->var, "user->var"}, {user->s0, "user->s0"}, {user->s1, "user->s1"},
+        {item->var, "item->var"}, {item->s0, "item->s0"}, {item->s1, "item->s1"}};
+    for (const auto& b : bases)
+      if (!orx_aligned16(b.p)) {
+        orx_set_error("%s: %s is not 16-byte aligned (the sharded step takes 16-byte-aligned local shards)", __func__,
+                      b.name);
+        return ORX_ERR_INVALID;
+      }
+  }
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
   if ((rc = shard_ws_ensure(h, x, st))) return rc;

@@ -91,7 +91,9 @@ extern "C" int orx_owner_bucket_combined(orx_handle_t h, const int32_t* ids, int
 // ---------------------------------------------------------------------------------------
 // generic sparse apply
 // ---------------------------------------------------------------------------------------
-template <int OPT>
+// VEC: var, s0 and s1 are 16-byte aligned (sparse_apply_impl decides); the row shape and the value rows are tested here,
+// so that the VEC instance compiles to what the kernel was before the table gate.
+template <int OPT, bool VEC>
 __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, float* s1, int64_t rows, int D,
                                                       const int32_t* __restrict__ ids, int64_t id_stride,
                                                       const float* __restrict__ vals, int64_t val_ld, int n,
@@ -121,7 +123,7 @@ __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, flo
   const bool own = !SL::STAGE_ONLY && c == 1u;
   // 128-bit path (value rows 16-byte aligned: a strided view may start mid-row): all loads of the row first, then the
   // math, then the stores
-  if (((D & 3) == 0) && ((val_ld & 3) == 0) && (((uintptr_t)vals & 15) == 0)) {
+  if (VEC && ((D & 3) == 0) && ((val_ld & 3) == 0) && (((uintptr_t)vals & 15) == 0)) {
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int e = lane * 4; e < D; e += 128) {
       const int64_t off = (int64_t)id * D + e;
@@ -199,11 +201,14 @@ static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32
   ORX_REQUIRE(n == 0 || (ids && values), "null ids/values");
   const int D = tab->dim;
   if ((rc = orx_ensure_workspace(h, n > 0 ? n : 1, D))) return rc;
+  const bool vec = orx_aligned16(tab->var, tab->s0, tab->s1);   // a table may start anywhere (orx.h)
   return sparse_apply_run(h, tab, ids, id_stride, n, opt, st, [&](const OrxOptDev& o) {
     const int blocks = (n + 63) / 64;   // 8 warps x 8 pairs per block and iteration
     orx_dispatch_opt(opt->kind, [&](auto O) {
-      k_sparse_apply<decltype(O)::value><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride,
-                                                                 values, value_ld, n, h->set[0].u, h->gu, o);
+      orx_dispatch<0, 1>(vec ? 1 : 0, [&](auto V) {
+        k_sparse_apply<decltype(O)::value, decltype(V)::value == 1><<<blocks, 256, 0, st>>>(
+            tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride, values, value_ld, n, h->set[0].u, h->gu, o);
+      });
     });
   });
 }
@@ -235,7 +240,9 @@ __global__ void __launch_bounds__(256) k_bag_ids(const int32_t* __restrict__ spa
 
 // k_sparse_apply's update over compacted bag lookups: value row i / L, divided by cnt[i / L] for a mean (cnt != null).
 // A separate kernel so that k_sparse_apply's parameter block, and with it its register allocation, stays as it is.
-template <int OPT>
+// VEC: var, s0 and s1 are 16-byte aligned (orx_bag_sparse_apply decides); the row shape and the value rows are tested
+// here, as in k_sparse_apply.
+template <int OPT, bool VEC>
 __global__ void __launch_bounds__(256) k_bag_apply(float* var, float* s0, float* s1, int D,
                                                    const int32_t* __restrict__ ids, int L,
                                                    const float* __restrict__ vals, int64_t val_ld,
@@ -244,7 +251,7 @@ __global__ void __launch_bounds__(256) k_bag_apply(float* var, float* s0, float*
   typedef OrxOptSlots<OPT> SL;
   const int lane = threadIdx.x & 31;
   const int nw = (gridDim.x * blockDim.x) >> 5;
-  const bool vec = ((D & 3) == 0) && ((val_ld & 3) == 0) && (((uintptr_t)vals & 15) == 0);
+  const bool vec = VEC && ((D & 3) == 0) && ((val_ld & 3) == 0) && (((uintptr_t)vals & 15) == 0);
   for (int b0 = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * 8; b0 < n; b0 += nw * 8) {
   int32_t my_id = -1;
   int my_d = -1;
@@ -321,11 +328,14 @@ extern "C" int orx_bag_sparse_apply(orx_handle_t h, const orx_table_t* tab, cons
     k_bag_ids<<<blocks, 256, 0, st>>>(sparse, ld, col_lo, L, B, tab->rows, ids_c, cnt);
     ORX_LAUNCH_CHECK();
   }
+  const bool vec = orx_aligned16(tab->var, tab->s0, tab->s1);   // a table may start anywhere (orx.h)
   return sparse_apply_run(h, tab, ids_c, 1, n, opt, st, [&](const OrxOptDev& o) {
     const int blocks = (n + 63) / 64;
     orx_dispatch_opt(opt->kind, [&](auto O) {
-      k_bag_apply<decltype(O)::value><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, D, ids_c, L, dZ, dz_ld, cnt,
-                                                              n, h->set[0].u, h->gu, o);
+      orx_dispatch<0, 1>(vec ? 1 : 0, [&](auto V) {
+        k_bag_apply<decltype(O)::value, decltype(V)::value == 1><<<blocks, 256, 0, st>>>(
+            tab->var, tab->s0, tab->s1, D, ids_c, L, dZ, dz_ld, cnt, n, h->set[0].u, h->gu, o);
+      });
     });
   });
 }
