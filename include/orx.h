@@ -578,6 +578,48 @@ ORX_API int orx_score_rank_shard(orx_handle_t h, int32_t kind, int32_t phase, co
                                  int32_t* xpred /*[Bu, P]*/, int64_t* xcnt /*[Bu, P]*/, float* auc, float* ndcg,
                                  float* recall, orx_stream_t s);
 
+/* ---- listed-candidate evaluation: AUC / NDCG / Recall of datasets with explicit negatives, each user ranked against
+ * its listed items only (the sampled-metrics protocol: a user's held-out positives against about 100 listed negatives;
+ * openrec_b200/tf2/metrics/evaluator.py CandidateEvaluator).  No pass over the catalogue: the work is one item row per
+ * listed entry and positive.
+ * For batch row b, u = uid[b]: three CSR rows indexed by user id, positives P (pos_off / pos_items), listed items L
+ * (neg_off / neg_items) and exclusions E (excl_off / excl_items; excl_off may be NULL = E empty), each sorted and
+ * unique, entries outside [0, I) ignored.  Results equal orx_score_all followed by orx_rank_metrics on the masks
+ * Dataset.evaluation builds for such a dataset: pos = P, excl = ~(P u L) u E.  So:
+ *   AUC    = sum over the eval items i in L \ P \ E of #{p in P : pred_p >= s_i}, over |P| * |L \ P \ E| (a row with no
+ *            eval item gets 0 / 0 = NaN);
+ *   sp     = expf(score) on (P u L) \ E and 0 elsewhere; rank_p = #{i : sp_i > sp_p}; NDCG / Recall from rank_p;
+ *   a positive in E keeps its pred for AUC and has sp 0; a listed item that is also a positive is a positive.
+ * AUC and Recall are bit-equal to those of orx_score_all + orx_rank_metrics, and to orx_score_rank called with the
+ * exclusion rows ~(P u L) u E; NDCG equals them within one float32 ulp (float64 sums in another order).  kind, scale,
+ * item_bias, the bad-uid rule, max_pos, the cut-offs, the scratch and the size limits are those of orx_score_rank; the
+ * call writes no dispatch record.
+ * ORX_ERR_INVALID before any device work: the refusals of orx_score_rank, and neg_off NULL.  Bu = 0 is a no-op.  The
+ * scratch is orx_score_rank's own allocation, so a call between orx_pairwise_prefetch and its step leaves the
+ * prefetched index alone. */
+ORX_API int orx_score_rank_listed(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
+                                  int32_t Bu, const float* scale, const float* item_tab, const float* item_bias,
+                                  int64_t I, int32_t dim, const int64_t* pos_off, const int32_t* pos_items,
+                                  const int64_t* neg_off, const int32_t* neg_items, const int64_t* excl_off,
+                                  const int32_t* excl_items, int32_t max_pos, const int32_t* at_host, int32_t n_at,
+                                  float* auc, float* ndcg, float* recall, orx_stream_t s);
+/* orx_score_rank_listed over row-sharded tables: the four phases, buffers (sizes from orx_score_rank_shard_sizes),
+ * exchange and geometry rules of orx_score_rank_shard.  Phases 0 and 1 are its phases 0 and 1; phase 2 writes
+ * xcnt[b, 0] = the AUC count of the eval items this rank owns and xcnt[b, 1..n] the rank hits of the listed items and
+ * positives outside E that it owns; phase 3 reads the summed xcnt and writes auc / ndcg / recall, counting the eval
+ * items from the global lists.  Phase 3's outputs equal orx_score_rank_listed on the global tables (scale NULL): AUC and
+ * Recall bit for bit, NDCG within one float32 ulp.  No handle state crosses a phase boundary.  ORX_ERR_INVALID before
+ * any device work: the refusals of orx_score_rank_shard, and (Bu > 0) neg_off NULL.  Bu = 0 is a no-op.  GMF scales the
+ * summed xrows with orx_rows_scale between phase 0 and phase 1. */
+ORX_API int orx_score_rank_listed_shard(orx_handle_t h, int32_t kind, int32_t phase, const orx_rowshard_t* g_host,
+                                        const float* user_shard, const float* item_shard, const float* bias_shard,
+                                        int32_t dim, const int32_t* uid, int32_t Bu, const int64_t* pos_off,
+                                        const int32_t* pos_items, const int64_t* neg_off, const int32_t* neg_items,
+                                        const int64_t* excl_off, const int32_t* excl_items, int32_t max_pos,
+                                        const int32_t* at_host, int32_t n_at, int32_t* xrows /*[Bu, dim]*/,
+                                        int32_t* xpred /*[Bu, P]*/, int64_t* xcnt /*[Bu, P]*/, float* auc,
+                                        float* ndcg, float* recall, orx_stream_t s);
+
 /* ---- catalogue top-K retrieval: each batch row's k best unseen items in one fused pass, without the [Bu, I] score
  * matrix (openrec_b200/tf2/recommenders/retriever.py; closest reference: openrec/tf1's FastDotProductServer).
  * Scores and conventions are those of orx_score_all, unchanged: the score of (b, i) with kind, scale and item_bias as

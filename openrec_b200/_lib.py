@@ -131,6 +131,10 @@ SIGNATURES = {
     "orx_score_rank_shard_sizes": [_i32, _i32, _i32, C.POINTER(_i64)],
     "orx_score_rank_shard": [_vp, _i32, _i32, C.POINTER(OrxRowShard), _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp,
                              _i32, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "orx_score_rank_listed": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                              _i32, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp],
+    "orx_score_rank_listed_shard": [_vp, _i32, _i32, C.POINTER(OrxRowShard), _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp,
+                                    _vp, _vp, _vp, _vp, _i32, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "orx_score_topk_shard": [_vp, _i32, _i32, C.POINTER(OrxRowShard), _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _i32,
                              _vp, _vp, _vp, _vp, _vp],
 }

@@ -53,6 +53,8 @@ struct EvalRowArgs : EvalArgs {
   int world, rank;      // row r is local row r / world on rank r % world (1, 0: the whole table)
   const float* xrows;   // non-null: batch row b's user row is xrows[b * D ..] (uid still decides bad rows)
   const float* xpred;   // non-null: prep reads the positives' scores from xpred[b * P + q] instead of computing them
+  const int64_t* neg_off;      // orx_score_rank_listed: the listed items' CSR (unused by the catalogue pass)
+  const int32_t* neg_items;
 };
 
 // Scratch of one call (handle workspace).  keys_in / keys: [2][Bu][P] -- pred thresholds of row b at b * P, sp
@@ -118,25 +120,32 @@ __device__ __forceinline__ bool ev_contains(const int32_t* items, int64_t lo, in
   return k < hi && items[k] == v;
 }
 
+// The user value at k of the chain of k_score_all (urow nullptr: a zero row).  Explicit roundings: u * scale - i must
+// not contract into one fused multiply-add.
+__device__ __forceinline__ float ev_uval(const EvalArgs& a, const float* urow, int k) {
+  float uv = 0.f;
+  if (urow) {
+    uv = urow[k];
+    if (a.scale) uv = __fmul_rn(uv, a.scale[k]);
+  }
+  return uv;
+}
+
+// One step of the chain of k_score_all: acc after the term of (user value uv, item value iv).
+template <int KIND>
+__device__ __forceinline__ float ev_step(float acc, float uv, float iv) {
+  if (KIND == ORX_SCORE_DOT) return __fmaf_rn(uv, iv, acc);
+  const float d = __fsub_rn(uv, iv);
+  return __fmaf_rn(-d, d, acc);
+}
+
 // One score by the chain of k_score_all, of an item i this rank owns (ev_owns).
 template <int KIND>
 __device__ __forceinline__ float ev_score1(const EvalRowArgs& a, const float* urow, int32_t i_global) {
   const int64_t i = ev_local(a, i_global);
   const float* irow = a.item_tab + i * a.D;
   float acc = 0.f;
-  for (int k = 0; k < a.D; ++k) {
-    float uv = 0.f;
-    if (urow) {   // explicit roundings: u * scale - i must not contract into one fused multiply-add
-      uv = urow[k];
-      if (a.scale) uv = __fmul_rn(uv, a.scale[k]);
-    }
-    if (KIND == ORX_SCORE_DOT) {
-      acc = __fmaf_rn(uv, irow[k], acc);
-    } else {
-      const float d = __fsub_rn(uv, irow[k]);
-      acc = __fmaf_rn(-d, d, acc);
-    }
-  }
+  for (int k = 0; k < a.D; ++k) acc = ev_step<KIND>(acc, ev_uval(a, urow, k), irow[k]);
   return acc + (a.bias ? a.bias[i] : 0.f);
 }
 
@@ -168,9 +177,10 @@ __device__ __forceinline__ int ev_rank_slot(const float* sth, int n, float smin,
 }
 
 // ---------------------------------------------------------------------------------------
-// prep: one CTA per batch row.  pred_p and sp_p of every positive (sp: NaN -> +inf, which ranks 0 like NaN; pred: NaN
-// -> +NaN, which sorts after every number and is left out of the AUC search), zeroed histogram and AUC count, and the
-// two sort segments of the row.  With a.xpred the scores are read from the summed exchange, not computed.
+// prep: one CTA per batch row.  pred_p and sp_p of every positive (sp: NaN -> +inf, which ranks 0 like NaN; a NaN pred
+// is left out of the AUC search and out of the pred segment, which a comparison sort could not order), zeroed
+// histogram and AUC count, and the two sort segments of the row.  With a.xpred the scores are read from the summed
+// exchange, not computed.
 // ---------------------------------------------------------------------------------------
 // The positive and exclusion entries of batch row b in [0, I_all), and whether its positive row is longer than max_pos.
 struct EvRow {
@@ -190,7 +200,7 @@ __device__ __forceinline__ EvRow ev_row(const EvalRowArgs& a, int b) {
 
 template <int KIND>
 __global__ void __launch_bounds__(EV_NT) k_eval_prep(const EvalRowArgs a, const EvalWs w) {
-  __shared__ int s_nan;
+  __shared__ int s_nan, s_kp;
   const int b = blockIdx.x;
   const float* urow = ev_urow(a, b);
   const EvRow r = ev_row(a, b);
@@ -199,19 +209,16 @@ __global__ void __launch_bounds__(EV_NT) k_eval_prep(const EvalRowArgs a, const 
   const int n = bad ? 0 : (int)(r.phi - plo);
   float* kp = w.keys_in + (int64_t)b * a.P;
   float* ks = w.keys_in + (int64_t)(a.Bu + b) * a.P;
-  if (threadIdx.x == 0) s_nan = 0;
+  if (threadIdx.x == 0) s_nan = s_kp = 0;
   __syncthreads();
   for (int q = threadIdx.x; q < n; q += blockDim.x) {
     const int32_t i = a.pos_items[plo + q];
-    float s = a.xpred ? a.xpred[(int64_t)b * a.P + q] : ev_score1<KIND>(a, urow, i);
+    const float s = a.xpred ? a.xpred[(int64_t)b * a.P + q] : ev_score1<KIND>(a, urow, i);
     const bool ex = ev_contains(a.excl_items, elo, ehi, i);
     float sp = expf(s) * (ex ? 0.f : 1.f);
     if (sp != sp) sp = __int_as_float(0x7f800000);
-    if (s != s) {
-      s = __int_as_float(0x7fffffff);
-      atomicAdd(&s_nan, 1);
-    }
-    kp[q] = s;
+    if (s != s) atomicAdd(&s_nan, 1);
+    else kp[atomicAdd(&s_kp, 1)] = s;   // the pred segment holds the non-NaN preds only, in any order
     ks[q] = sp;
   }
   for (int j = threadIdx.x; j < a.P; j += blockDim.x) w.hist[(int64_t)b * a.P + j] = 0u;
@@ -221,7 +228,7 @@ __global__ void __launch_bounds__(EV_NT) k_eval_prep(const EvalRowArgs a, const 
     w.info[2 * b + 1] = n - s_nan;
     w.auc_cnt[b] = 0ull;
     w.seg_begin[b] = b * a.P;
-    w.seg_end[b] = b * a.P + n;
+    w.seg_end[b] = b * a.P + n - s_nan;
     w.seg_begin[a.Bu + b] = (a.Bu + b) * a.P;
     w.seg_end[a.Bu + b] = (a.Bu + b) * a.P + n;
   }
@@ -650,6 +657,152 @@ __global__ void __launch_bounds__(EV_NT) k_eval_finish_counts(const EvalRowArgs 
 }
 
 // ---------------------------------------------------------------------------------------
+// listed-candidate evaluation (orx_score_rank_listed): each row ranked against its listed items only.  On the masks of
+// Dataset.evaluation for explicit negatives (pos = P, excl = ~(P u L) u E) an item outside (P u L) \ E has sp = 0,
+// never ranks above anything and is no eval item, so every count of the catalogue pass is a sum over the lists: the
+// eval items are L \ P \ E, each adding its AUC term and one rank hit, and each positive outside E adds its rank hit.
+// The finish is ev_finish_row's with extra = I - n - n_eval (every item that is neither a positive nor an eval item).
+// One CTA per batch row; prep and the threshold sort are those of orx_score_rank.
+// ---------------------------------------------------------------------------------------
+constexpr int EL_KS = 32;    // D columns of one staged slab: one 128-byte segment per item row
+constexpr int EL_LD = 33;    // slab row stride, odd: thread t reading row t meets no bank conflict
+constexpr int EL_UNR = 4;    // rows each warp has in flight while staging a slab
+
+// Whether listed entry q of row r (an entry in [0, I_all)) is an eval item: neither a positive nor excluded.
+__device__ __forceinline__ bool el_eval_item(const EvalRowArgs& a, const EvRow& r, int64_t q) {
+  const int32_t i = a.neg_items[q];
+  return !ev_contains(a.pos_items, r.plo, r.phi, i) && !ev_contains(a.excl_items, r.elo, r.ehi, i);
+}
+
+// The listed entries of batch row b in [0, I_all): [*lo, *hi).
+__device__ __forceinline__ void el_range(const EvalRowArgs& a, int b, int64_t* lo, int64_t* hi) {
+  int64_t raw;
+  ev_range(a.neg_off, a.neg_items, a.uid[b], a.U, a.I_all, lo, hi, &raw);
+}
+
+// The counts of row b over the items this rank owns.  Positives outside E: one rank hit each, scored by ev_score1.
+// Eval items: scored in chunks of
+// EV_NT entries, thread t taking entry t; D goes in slabs of EL_KS columns staged in shared memory, one warp-wide
+// 128-byte load per item row, and each thread runs the chain of ev_score1 (ascending k) over the slabs.
+// xcnt == nullptr: the outputs by ev_finish_row.  Else (sharded phase 2): xcnt[b][0] = the AUC count, xcnt[b][1..n]
+// the rank hits, the rest of the row 0 (every element written).
+template <int KIND>
+__global__ void __launch_bounds__(EV_NT, 3) k_eval_listed(const EvalRowArgs a, const EvalWs w, const EvalOut o,
+                                                       int64_t* xcnt) {
+  __shared__ float s_rows[EV_NT * EL_LD];
+  __shared__ float s_u[EL_KS];
+  __shared__ int32_t s_row[EV_NT];     // local item row of chunk entry t, -1: not scored on this rank
+  __shared__ unsigned long long s_auc;
+  __shared__ long long s_eval;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t P = a.P;
+  const int info = w.info[2 * b];
+  if (info < 0) {                      // a positive row longer than max_pos
+    if (xcnt)
+      for (int j = tid; j < a.P; j += EV_NT) xcnt[b * P + j] = 0;
+    else
+      ev_nan_row(o, b);
+    return;
+  }
+  const int n = info, n_auc = w.info[2 * b + 1];
+  const float* pth = w.keys + b * P;
+  const float* sth = w.keys + (a.Bu + b) * P;
+  unsigned* hist = w.hist + b * P;
+  const float pmin = n_auc ? pth[0] : __int_as_float(0x7f800000);
+  const float pmax = n_auc ? pth[n_auc - 1] : __int_as_float(0xff800000);
+  const float smin = n ? sth[0] : __int_as_float(0x7f800000);
+  const float smax = n ? sth[n - 1] : __int_as_float(0x7f800000);
+  const EvRow r = ev_row(a, b);
+  int64_t lo, hi;
+  el_range(a, b, &lo, &hi);
+  const float* urow = ev_urow(a, b);
+  if (tid == 0) {
+    s_auc = 0ull;
+    s_eval = 0;
+  }
+  for (int q = tid; q < n; q += EV_NT) {
+    const int32_t i = a.pos_items[r.plo + q];
+    if (!ev_owns(a, i) || ev_contains(a.excl_items, r.elo, r.ehi, i)) continue;
+    const int j = ev_rank_slot(sth, n, smin, smax, expf(ev_score1<KIND>(a, urow, i)));
+    if (j) atomicAdd(hist + j, 1u);
+  }
+  unsigned long long auc = 0ull;
+  long long n_eval = 0;
+  for (int64_t c0 = lo; c0 < hi; c0 += EV_NT) {
+    const int nc = (int)min((int64_t)EV_NT, hi - c0);
+    int32_t row = -1;
+    if (tid < nc && el_eval_item(a, r, c0 + tid)) {
+      ++n_eval;
+      const int32_t i = a.neg_items[c0 + tid];
+      if (ev_owns(a, i)) row = (int32_t)ev_local(a, i);
+    }
+    s_row[tid] = row;
+    float acc = 0.f;
+    for (int k0 = 0; k0 < a.D; k0 += EL_KS) {
+      const int ks = min(EL_KS, a.D - k0);
+      __syncthreads();                 // s_row written; the previous slab consumed
+      if (tid < ks) s_u[tid] = ev_uval(a, urow, k0 + tid);
+      for (int t0 = warp; t0 < nc; t0 += (EV_NT / 32) * EL_UNR) {
+        float v[EL_UNR];
+#pragma unroll
+        for (int x = 0; x < EL_UNR; ++x) {
+          const int t = t0 + (EV_NT / 32) * x;
+          const int32_t rt = t < nc ? s_row[t] : -1;
+          v[x] = rt >= 0 && lane < ks ? a.item_tab[(int64_t)rt * a.D + k0 + lane] : 0.f;
+        }
+#pragma unroll
+        for (int x = 0; x < EL_UNR; ++x) {
+          const int t = t0 + (EV_NT / 32) * x;
+          if (t < nc) s_rows[t * EL_LD + lane] = v[x];
+        }
+      }
+      __syncthreads();
+      if (row >= 0)
+        for (int k = 0; k < ks; ++k) acc = ev_step<KIND>(acc, s_u[k], s_rows[tid * EL_LD + k]);
+    }
+    if (row >= 0) {
+      const float s = acc + (a.bias ? a.bias[row] : 0.f);
+      auc += ev_auc_count(pth, n_auc, pmin, pmax, s);
+      const int j = ev_rank_slot(sth, n, smin, smax, expf(s));
+      if (j) atomicAdd(hist + j, 1u);
+    }
+  }
+  __syncthreads();                     // s_auc / s_eval initialised (a row without listed items has no chunk)
+  if (auc) atomicAdd(&s_auc, auc);
+  if (n_eval) atomicAdd(reinterpret_cast<unsigned long long*>(&s_eval), (unsigned long long)n_eval);
+  __syncthreads();
+  if (xcnt) {
+    for (int j = tid; j < a.P; j += EV_NT) xcnt[b * P + j] = j == 0 ? (int64_t)s_auc : j <= n ? (int64_t)hist[j] : 0;
+    return;
+  }
+  ev_finish_row(a, o, b, n, a.I_all - n - s_eval, s_auc, [&](int j) { return hist[j]; });
+}
+
+// Sharded phase 3 of orx_score_rank_listed_shard: the outputs from the counts summed over the ranks; n and n_eval come
+// from the lists alone.
+__global__ void __launch_bounds__(EV_NT) k_eval_listed_finish_counts(const EvalRowArgs a, const int64_t* xcnt,
+                                                                     const EvalOut o) {
+  __shared__ long long s_eval;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const EvRow r = ev_row(a, b);
+  if (r.bad) {
+    ev_nan_row(o, b);
+    return;
+  }
+  const int n = (int)(r.phi - r.plo);
+  int64_t lo, hi;
+  el_range(a, b, &lo, &hi);
+  if (tid == 0) s_eval = 0;
+  __syncthreads();
+  long long n_eval = 0;
+  for (int64_t q = lo + tid; q < hi; q += EV_NT) n_eval += el_eval_item(a, r, q) ? 1 : 0;
+  if (n_eval) atomicAdd(reinterpret_cast<unsigned long long*>(&s_eval), (unsigned long long)n_eval);
+  __syncthreads();
+  const int64_t* cnt = xcnt + (int64_t)b * a.P;
+  ev_finish_row(a, o, b, n, a.I_all - n - s_eval, (unsigned long long)cnt[0], [&](int j) { return (unsigned)cnt[j]; });
+}
+
+// ---------------------------------------------------------------------------------------
 // top-K retrieval (orx_score_topk).  Key of an eligible (score s, item i): the order-preserving bits of s (-0 taken as
 // +0) in the high word, ~i in the low word, so "score descending, then item ascending" is ">" on keys; keys are unique
 // and every real key is > 0, which marks an empty slot.  NaN scores never form a key.
@@ -996,6 +1149,17 @@ int ev_workspace(orx_ctx* h, int Bu, int P, cudaStream_t st, EvalWs* w) {
   return ORX_OK;
 }
 
+// prep and the segmented sort: every batch row's sorted thresholds, zeroed histogram and AUC count in w.
+template <int KIND>
+int ev_prep_sort(const EvalRowArgs& a, const EvalWs& w, cudaStream_t st) {
+  k_eval_prep<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w);
+  ORX_LAUNCH_CHECK();
+  size_t bytes = w.sort_bytes;
+  ORX_CUDA(cub::DeviceSegmentedSort::SortKeys(w.sort_tmp, bytes, (const float*)w.keys_in, w.keys, 2 * a.Bu * a.P,
+                                              2 * a.Bu, (const int*)w.seg_begin, (const int*)w.seg_end, st));
+  return ORX_OK;
+}
+
 // prep, sort and the main pass over the a.I item rows (no main pass when a.I == 0): the thresholds, AUC counts and
 // rank histograms of every batch row in w, before the take-back.  *variant / *splits: the main pass's dispatch fields
 // (splits 0: not launched).
@@ -1021,11 +1185,8 @@ int ev_count(orx_ctx* h, const EvalRowArgs& a, const EvalWs& w, cudaStream_t st,
   }
   const int64_t user_tiles = (a.Bu + EV_TU - 1) / EV_TU;
 
-  k_eval_prep<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w);
-  ORX_LAUNCH_CHECK();
-  size_t bytes = w.sort_bytes;
-  ORX_CUDA(cub::DeviceSegmentedSort::SortKeys(w.sort_tmp, bytes, (const float*)w.keys_in, w.keys, 2 * a.Bu * a.P,
-                                              2 * a.Bu, (const int*)w.seg_begin, (const int*)w.seg_end, st));
+  const int rc = ev_prep_sort<KIND>(a, w, st);
+  if (rc != ORX_OK) return rc;
   if (*splits > 0) {
     EvalArgs t = a;
     if (XROWS) t.user_tab = a.xrows;
@@ -1054,14 +1215,33 @@ void ev_user_rows(const EvalRowArgs& a, int32_t* xrows, cudaStream_t st) {
   k_eval_user_rows<<<(unsigned)(blocks < 4096 ? blocks : 4096), EV_NT, 0, st>>>(a, xrows);
 }
 
-// One phase of orx_score_rank_shard (arguments checked by the caller).
+// orx_score_rank_listed's counts of every batch row from the handle's evaluation scratch: its outputs (xcnt nullptr),
+// or phase 2 of orx_score_rank_listed_shard (the counts into xcnt).
 template <int KIND>
-int ev_shard_phase(orx_ctx* h, int phase, const EvalRowArgs& a, const EvalOut& o, int32_t* xrows, int32_t* xpred,
-                   int64_t* xcnt, cudaStream_t st) {
+int el_launch(orx_ctx* h, const EvalRowArgs& a, const EvalOut& o, int64_t* xcnt, cudaStream_t st) {
+  EvalWs w;
+  int rc = ev_workspace(h, a.Bu, a.P, st, &w);
+  if (rc != ORX_OK) return rc;
+  rc = ev_prep_sort<KIND>(a, w, st);
+  if (rc != ORX_OK) return rc;
+  k_eval_listed<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w, o, xcnt);
+  ORX_LAUNCH_CHECK();
+  return ORX_OK;
+}
+
+// One phase of orx_score_rank_shard, or with `listed` of orx_score_rank_listed_shard (arguments checked by the
+// caller).  Phases 0 and 1 are the same for both.
+template <int KIND>
+int ev_shard_phase(orx_ctx* h, int phase, bool listed, const EvalRowArgs& a, const EvalOut& o, int32_t* xrows,
+                   int32_t* xpred, int64_t* xcnt, cudaStream_t st) {
   if (phase == 0) {
     ev_user_rows(a, xrows, st);
   } else if (phase == 1) {
     k_eval_pos_scores<KIND><<<a.Bu, EV_NT, 0, st>>>(a, xpred);
+  } else if (phase == 2 && listed) {
+    return el_launch<KIND>(h, a, o, xcnt, st);
+  } else if (phase == 3 && listed) {
+    k_eval_listed_finish_counts<<<a.Bu, EV_NT, 0, st>>>(a, xcnt, o);
   } else if (phase == 2) {
     EvalWs w;
     int rc = ev_workspace(h, a.Bu, a.P, st, &w);
@@ -1145,6 +1325,78 @@ EvalOut ev_out(const int32_t* at_host, int n_at, float* auc, float* ndcg, float*
   return o;
 }
 
+// Why orx_score_rank / orx_score_rank_listed refuse their arguments, or nullptr (the size limit only for Bu > 0).
+const char* ev_rank_refusal(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
+                            int32_t Bu, const float* item_tab, int64_t I, int32_t dim, const int64_t* pos_off,
+                            int32_t max_pos, const int32_t* at_host, int32_t n_at) {
+  if (!(h != nullptr && user_tab && uid && item_tab && pos_off)) return "null pointer";
+  if (!(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST)) return "unknown score kind";
+  if (!(U > 0 && I > 0 && I <= INT32_MAX && dim > 0 && Bu >= 0 && max_pos >= 0)) return "bad sizes";
+  if (!(n_at >= 0 && n_at <= ORX_MAX_AT)) return "at most 8 cut-offs";
+  if (!(n_at == 0 || at_host)) return "null cut-offs";
+  if (Bu > 0 && 2 * (int64_t)Bu * ((int64_t)max_pos + 1) > INT32_MAX)
+    return "Bu * (max_pos + 1) too large for one call: split the batch";
+  return nullptr;
+}
+
+// The row arguments of a checked orx_score_rank / orx_score_rank_listed call (neg_off nullptr for the former).
+EvalRowArgs ev_rank_args(const float* user_tab, int64_t U, const int32_t* uid, int32_t Bu, const float* scale,
+                         const float* item_tab, const float* item_bias, int64_t I, int32_t dim, const int64_t* pos_off,
+                         const int32_t* pos_items, const int64_t* neg_off, const int32_t* neg_items,
+                         const int64_t* excl_off, const int32_t* excl_items, int32_t max_pos) {
+  EvalRowArgs a = {};
+  a.user_tab = user_tab; a.U = U; a.uid = uid; a.Bu = Bu; a.scale = scale; a.item_tab = item_tab;
+  a.bias = item_bias; a.I = I; a.I_all = I; a.world = 1; a.rank = 0; a.D = dim; a.pos_off = pos_off;
+  a.excl_off = excl_off; a.pos_items = pos_items; a.excl_items = excl_items; a.max_pos = max_pos; a.P = max_pos + 1;
+  a.neg_off = neg_off; a.neg_items = neg_items;
+  return a;
+}
+
+// Why orx_score_rank_shard / orx_score_rank_listed_shard refuse their arguments, or nullptr (the size limit and the
+// buffer checks only for Bu > 0).
+const char* ev_shard_refusal(orx_handle_t h, int32_t kind, int32_t phase, const orx_rowshard_t* g_host,
+                             const float* user_shard, const float* item_shard, int32_t dim, const int32_t* uid,
+                             int32_t Bu, const int64_t* pos_off, int32_t max_pos, const int32_t* at_host, int32_t n_at,
+                             const int32_t* xrows, const int32_t* xpred, const int64_t* xcnt) {
+  if (!(h != nullptr && g_host != nullptr)) return "null pointer";
+  if (!(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST)) return "unknown score kind";
+  if (!(phase >= 0 && phase <= 3)) return "phase must lie in [0, 3]";
+  const orx_rowshard_t g = *g_host;
+  if (!(g.world >= 1 && g.rank >= 0 && g.rank < g.world)) return "rank must lie in [0, world)";
+  if (!(g.total_users > 0 && g.total_items > 0 && g.total_items <= INT32_MAX)) return "bad table sizes";
+  if (!(g.local_users == (g.total_users - g.rank + g.world - 1) / g.world &&
+        g.local_items == (g.total_items - g.rank + g.world - 1) / g.world))
+    return "local_users / local_items disagree with (total, world, rank)";
+  if (!(dim > 0 && Bu >= 0 && max_pos >= 0)) return "bad sizes";
+  if (!(n_at >= 0 && n_at <= ORX_MAX_AT)) return "at most 8 cut-offs";
+  if (!(n_at == 0 || at_host)) return "null cut-offs";
+  if (Bu == 0) return nullptr;
+  if (2 * (int64_t)Bu * ((int64_t)max_pos + 1) > INT32_MAX)
+    return "Bu * (max_pos + 1) too large for one call: split the batch";
+  if (!(uid && pos_off)) return "null pointer";
+  if (!(phase != 0 || (user_shard && xrows))) return "phase 0 needs user_shard and xrows";
+  if (!(phase != 1 || (item_shard && xrows && xpred))) return "phase 1 needs item_shard, xrows and xpred";
+  if (!(phase != 2 || (item_shard && xrows && xpred && xcnt))) return "phase 2 needs item_shard, xrows, xpred, xcnt";
+  if (!(phase != 3 || xcnt)) return "phase 3 needs xcnt";
+  return nullptr;
+}
+
+// The row arguments of a checked sharded phase (neg_off nullptr for orx_score_rank_shard).
+EvalRowArgs ev_shard_args(int32_t phase, const orx_rowshard_t& g, const float* user_shard, const float* item_shard,
+                          const float* bias_shard, int32_t dim, const int32_t* uid, int32_t Bu,
+                          const int64_t* pos_off, const int32_t* pos_items, const int64_t* neg_off,
+                          const int32_t* neg_items, const int64_t* excl_off, const int32_t* excl_items,
+                          int32_t max_pos, const int32_t* xrows, const int32_t* xpred) {
+  EvalRowArgs a = {};
+  a.user_tab = user_shard; a.U = g.total_users; a.uid = uid; a.Bu = Bu; a.item_tab = item_shard; a.bias = bias_shard;
+  a.I = g.local_items; a.I_all = g.total_items; a.world = g.world; a.rank = g.rank; a.D = dim; a.pos_off = pos_off;
+  a.excl_off = excl_off; a.pos_items = pos_items; a.excl_items = excl_items; a.max_pos = max_pos; a.P = max_pos + 1;
+  a.xrows = phase >= 1 ? reinterpret_cast<const float*>(xrows) : nullptr;
+  a.xpred = phase == 2 ? reinterpret_cast<const float*>(xpred) : nullptr;
+  a.neg_off = neg_off; a.neg_items = neg_items;
+  return a;
+}
+
 }  // namespace
 
 extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
@@ -1152,28 +1404,41 @@ extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_ta
                               int32_t dim, const int64_t* pos_off, const int32_t* pos_items, const int64_t* excl_off,
                               const int32_t* excl_items, int32_t max_pos, const int32_t* at_host, int32_t n_at,
                               float* auc, float* ndcg, float* recall, orx_stream_t s) {
-  ORX_REQUIRE(h != nullptr && user_tab && uid && item_tab && pos_off, "null pointer");
-  ORX_REQUIRE(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST, "unknown score kind");
-  ORX_REQUIRE(U > 0 && I > 0 && I <= INT32_MAX && dim > 0 && Bu >= 0 && max_pos >= 0, "bad sizes");
-  ORX_REQUIRE(n_at >= 0 && n_at <= ORX_MAX_AT, "at most 8 cut-offs");
-  ORX_REQUIRE(n_at == 0 || at_host, "null cut-offs");
+  const char* why = ev_rank_refusal(h, kind, user_tab, U, uid, Bu, item_tab, I, dim, pos_off, max_pos, at_host, n_at);
+  ORX_REQUIRE(why == nullptr, why);
   if (Bu == 0) return ORX_OK;
-  const int64_t P = (int64_t)max_pos + 1;
-  ORX_REQUIRE(2 * (int64_t)Bu * P <= INT32_MAX, "Bu * (max_pos + 1) too large for one call: split the batch");
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
 
   EvalWs w;
-  const int rc = ev_workspace(h, Bu, (int)P, st, &w);
+  const int rc = ev_workspace(h, Bu, max_pos + 1, st, &w);
   if (rc != ORX_OK) return rc;
 
-  EvalRowArgs a = {};
-  a.user_tab = user_tab; a.U = U; a.uid = uid; a.Bu = Bu; a.scale = scale; a.item_tab = item_tab;
-  a.bias = item_bias; a.I = I; a.I_all = I; a.world = 1; a.rank = 0; a.D = dim; a.pos_off = pos_off;
-  a.excl_off = excl_off; a.pos_items = pos_items; a.excl_items = excl_items; a.max_pos = max_pos; a.P = (int)P;
+  const EvalRowArgs a = ev_rank_args(user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, pos_off, pos_items,
+                                     nullptr, nullptr, excl_off, excl_items, max_pos);
   const EvalOut o = ev_out(at_host, n_at, auc, ndcg, recall);
   return kind == ORX_SCORE_DOT ? ev_launch<ORX_SCORE_DOT>(h, a, w, o, st)
                                : ev_launch<ORX_SCORE_NEG_SQDIST>(h, a, w, o, st);
+}
+
+extern "C" int orx_score_rank_listed(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U,
+                                     const int32_t* uid, int32_t Bu, const float* scale, const float* item_tab,
+                                     const float* item_bias, int64_t I, int32_t dim, const int64_t* pos_off,
+                                     const int32_t* pos_items, const int64_t* neg_off, const int32_t* neg_items,
+                                     const int64_t* excl_off, const int32_t* excl_items, int32_t max_pos,
+                                     const int32_t* at_host, int32_t n_at, float* auc, float* ndcg, float* recall,
+                                     orx_stream_t s) {
+  const char* why = ev_rank_refusal(h, kind, user_tab, U, uid, Bu, item_tab, I, dim, pos_off, max_pos, at_host, n_at);
+  ORX_REQUIRE(why == nullptr, why);
+  ORX_REQUIRE(neg_off != nullptr, "null pointer");
+  if (Bu == 0) return ORX_OK;
+  ORX_CUDA(cudaSetDevice(h->device));
+  const EvalRowArgs a = ev_rank_args(user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, pos_off, pos_items,
+                                     neg_off, neg_items, excl_off, excl_items, max_pos);
+  const EvalOut o = ev_out(at_host, n_at, auc, ndcg, recall);
+  cudaStream_t st = (cudaStream_t)s;
+  return kind == ORX_SCORE_DOT ? el_launch<ORX_SCORE_DOT>(h, a, o, nullptr, st)
+                               : el_launch<ORX_SCORE_NEG_SQDIST>(h, a, o, nullptr, st);
 }
 
 extern "C" int orx_score_topk(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
@@ -1211,38 +1476,38 @@ extern "C" int orx_score_rank_shard(orx_handle_t h, int32_t kind, int32_t phase,
                                     int32_t max_pos, const int32_t* at_host, int32_t n_at, int32_t* xrows,
                                     int32_t* xpred, int64_t* xcnt, float* auc, float* ndcg, float* recall,
                                     orx_stream_t s) {
-  ORX_REQUIRE(h != nullptr && g_host != nullptr, "null pointer");
-  ORX_REQUIRE(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST, "unknown score kind");
-  ORX_REQUIRE(phase >= 0 && phase <= 3, "phase must lie in [0, 3]");
-  const orx_rowshard_t g = *g_host;
-  ORX_REQUIRE(g.world >= 1 && g.rank >= 0 && g.rank < g.world, "rank must lie in [0, world)");
-  ORX_REQUIRE(g.total_users > 0 && g.total_items > 0 && g.total_items <= INT32_MAX, "bad table sizes");
-  ORX_REQUIRE(g.local_users == (g.total_users - g.rank + g.world - 1) / g.world &&
-                  g.local_items == (g.total_items - g.rank + g.world - 1) / g.world,
-              "local_users / local_items disagree with (total, world, rank)");
-  ORX_REQUIRE(dim > 0 && Bu >= 0 && max_pos >= 0, "bad sizes");
-  ORX_REQUIRE(n_at >= 0 && n_at <= ORX_MAX_AT, "at most 8 cut-offs");
-  ORX_REQUIRE(n_at == 0 || at_host, "null cut-offs");
+  const char* why = ev_shard_refusal(h, kind, phase, g_host, user_shard, item_shard, dim, uid, Bu, pos_off, max_pos,
+                                     at_host, n_at, xrows, xpred, xcnt);
+  ORX_REQUIRE(why == nullptr, why);
   if (Bu == 0) return ORX_OK;
-  const int64_t P = (int64_t)max_pos + 1;
-  ORX_REQUIRE(2 * (int64_t)Bu * P <= INT32_MAX, "Bu * (max_pos + 1) too large for one call: split the batch");
-  ORX_REQUIRE(uid && pos_off, "null pointer");
-  ORX_REQUIRE(phase != 0 || (user_shard && xrows), "phase 0 needs user_shard and xrows");
-  ORX_REQUIRE(phase != 1 || (item_shard && xrows && xpred), "phase 1 needs item_shard, xrows and xpred");
-  ORX_REQUIRE(phase != 2 || (item_shard && xrows && xpred && xcnt), "phase 2 needs item_shard, xrows, xpred, xcnt");
-  ORX_REQUIRE(phase != 3 || xcnt, "phase 3 needs xcnt");
   ORX_CUDA(cudaSetDevice(h->device));
-
-  EvalRowArgs a = {};
-  a.user_tab = user_shard; a.U = g.total_users; a.uid = uid; a.Bu = Bu; a.item_tab = item_shard; a.bias = bias_shard;
-  a.I = g.local_items; a.I_all = g.total_items; a.world = g.world; a.rank = g.rank; a.D = dim; a.pos_off = pos_off;
-  a.excl_off = excl_off; a.pos_items = pos_items; a.excl_items = excl_items; a.max_pos = max_pos; a.P = (int)P;
-  a.xrows = phase >= 1 ? reinterpret_cast<const float*>(xrows) : nullptr;
-  a.xpred = phase == 2 ? reinterpret_cast<const float*>(xpred) : nullptr;
+  const EvalRowArgs a = ev_shard_args(phase, *g_host, user_shard, item_shard, bias_shard, dim, uid, Bu, pos_off,
+                                      pos_items, nullptr, nullptr, excl_off, excl_items, max_pos, xrows, xpred);
   const EvalOut o = ev_out(at_host, n_at, auc, ndcg, recall);
   cudaStream_t st = (cudaStream_t)s;
-  return kind == ORX_SCORE_DOT ? ev_shard_phase<ORX_SCORE_DOT>(h, phase, a, o, xrows, xpred, xcnt, st)
-                               : ev_shard_phase<ORX_SCORE_NEG_SQDIST>(h, phase, a, o, xrows, xpred, xcnt, st);
+  return kind == ORX_SCORE_DOT ? ev_shard_phase<ORX_SCORE_DOT>(h, phase, false, a, o, xrows, xpred, xcnt, st)
+                               : ev_shard_phase<ORX_SCORE_NEG_SQDIST>(h, phase, false, a, o, xrows, xpred, xcnt, st);
+}
+
+extern "C" int orx_score_rank_listed_shard(orx_handle_t h, int32_t kind, int32_t phase, const orx_rowshard_t* g_host,
+                                           const float* user_shard, const float* item_shard, const float* bias_shard,
+                                           int32_t dim, const int32_t* uid, int32_t Bu, const int64_t* pos_off,
+                                           const int32_t* pos_items, const int64_t* neg_off, const int32_t* neg_items,
+                                           const int64_t* excl_off, const int32_t* excl_items, int32_t max_pos,
+                                           const int32_t* at_host, int32_t n_at, int32_t* xrows, int32_t* xpred,
+                                           int64_t* xcnt, float* auc, float* ndcg, float* recall, orx_stream_t s) {
+  const char* why = ev_shard_refusal(h, kind, phase, g_host, user_shard, item_shard, dim, uid, Bu, pos_off, max_pos,
+                                     at_host, n_at, xrows, xpred, xcnt);
+  ORX_REQUIRE(why == nullptr, why);
+  if (Bu == 0) return ORX_OK;
+  ORX_REQUIRE(neg_off != nullptr, "null pointer");
+  ORX_CUDA(cudaSetDevice(h->device));
+  const EvalRowArgs a = ev_shard_args(phase, *g_host, user_shard, item_shard, bias_shard, dim, uid, Bu, pos_off,
+                                      pos_items, neg_off, neg_items, excl_off, excl_items, max_pos, xrows, xpred);
+  const EvalOut o = ev_out(at_host, n_at, auc, ndcg, recall);
+  cudaStream_t st = (cudaStream_t)s;
+  return kind == ORX_SCORE_DOT ? ev_shard_phase<ORX_SCORE_DOT>(h, phase, true, a, o, xrows, xpred, xcnt, st)
+                               : ev_shard_phase<ORX_SCORE_NEG_SQDIST>(h, phase, true, a, o, xrows, xpred, xcnt, st);
 }
 
 extern "C" int orx_score_topk_shard(orx_handle_t h, int32_t kind, int32_t phase, const orx_rowshard_t* g_host,

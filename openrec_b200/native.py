@@ -566,6 +566,59 @@ class Engine:
             "orx_score_rank_shard")
         return tuple(out) if phase == 3 else None
 
+    def score_rank_listed(self, kind, user_tab, uid, item_tab, item_bias, pos_off, pos_items, neg_off, neg_items,
+                          excl_off, excl_items, max_pos, at=(), scale=None):
+        """score_rank with each user ranked against its listed items only (orx_score_rank_listed in include/orx.h):
+        positives, listed items (neg_off / neg_items) and exclusions as CSR lists indexed by user id, as in score_rank
+        (excl_off / excl_items may be None).  Equals score_all + rank_metrics on the masks pos = P,
+        excl = ~(P | L) | E.  -> (auc [Bu], ndcg [Bu, len(at)], recall [Bu, len(at)])."""
+        uid = ids32(uid)
+        Bu, dev = uid.numel(), item_tab.device
+        pos_off, pos_items = _csr(pos_off, pos_items, user_tab.shape[0])
+        neg_off, neg_items = _csr(neg_off, neg_items, user_tab.shape[0])
+        excl_off, excl_items = _csr(excl_off, excl_items, user_tab.shape[0])
+        if pos_off is None or neg_off is None:
+            raise ValueError("score_rank_listed needs the positives' and the listed items' CSR")
+        at_arr = (C.c_int32 * max(len(at), 1))(*[int(k) for k in at])
+        auc = torch.empty(Bu, dtype=torch.float32, device=dev)
+        ndcg = torch.empty((Bu, len(at)), dtype=torch.float32, device=dev)
+        rec = torch.empty((Bu, len(at)), dtype=torch.float32, device=dev)
+        _lib.check(self.lib.orx_score_rank_listed(
+            self.h, kind, _ptr(_f32(user_tab, "user_tab")), user_tab.shape[0], _ptr(uid), Bu, _ptr(scale),
+            _ptr(_f32(item_tab, "item_tab")), _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(pos_off),
+            _ptr(pos_items), _ptr(neg_off), _ptr(neg_items), _ptr(excl_off), _ptr(excl_items), int(max_pos), at_arr,
+            len(at), _ptr(auc), _ptr(ndcg), _ptr(rec), self.stream()), "orx_score_rank_listed")
+        return auc, ndcg, rec
+
+    def score_rank_listed_shard(self, kind, phase, g, user_shard, item_shard, bias_shard, uid, pos_off, pos_items,
+                                neg_off, neg_items, excl_off, excl_items, max_pos, xrows, xpred, xcnt, at=()):
+        """One phase of score_rank_listed over row-sharded tables (orx_score_rank_listed_shard in include/orx.h); the
+        shards, exchange buffers and phases are those of score_rank_shard, the listed items' CSR is global.
+        Phase 3 -> (auc [Bu], ndcg [Bu, len(at)], recall [Bu, len(at)]); other phases -> None."""
+        uid = ids32(uid)
+        Bu, dev = uid.numel(), xrows.device
+        pos_off, pos_items = _csr(pos_off, pos_items, g.total_users)
+        neg_off, neg_items = _csr(neg_off, neg_items, g.total_users)
+        excl_off, excl_items = _csr(excl_off, excl_items, g.total_users)
+        if pos_off is None or neg_off is None:
+            raise ValueError("score_rank_listed_shard needs the positives' and the listed items' CSR")
+        if xrows.dtype != torch.int32 or xpred.dtype != torch.int32 or xcnt.dtype != torch.int64:
+            raise ValueError("exchange buffers: xrows / xpred int32, xcnt int64")
+        at_arr = (C.c_int32 * max(len(at), 1))(*[int(k) for k in at])
+        out = [None] * 3
+        if phase == 3:
+            out = [torch.empty(Bu, dtype=torch.float32, device=dev),
+                   torch.empty((Bu, len(at)), dtype=torch.float32, device=dev),
+                   torch.empty((Bu, len(at)), dtype=torch.float32, device=dev)]
+        geo = _lib.OrxRowShard(*[int(x) for x in g])
+        _lib.check(self.lib.orx_score_rank_listed_shard(
+            self.h, kind, int(phase), C.byref(geo), _ptr(_f32(user_shard, "user_shard")),
+            _ptr(_f32(item_shard, "item_shard")), _ptr(_f32(bias_shard, "bias_shard")), user_shard.shape[1],
+            _ptr(uid), Bu, _ptr(pos_off), _ptr(pos_items), _ptr(neg_off), _ptr(neg_items), _ptr(excl_off),
+            _ptr(excl_items), int(max_pos), at_arr, len(at), _ptr(xrows), _ptr(xpred), _ptr(xcnt),
+            *[_ptr(t) for t in out], self.stream()), "orx_score_rank_listed_shard")
+        return tuple(out) if phase == 3 else None
+
     def score_topk(self, kind, user_tab, uid, item_tab, item_bias, excl_off, excl_items, k, scale=None):
         """The k best eligible items of each user uid in one pass over the item table, without the [Bu, I] score
         matrix: order score descending then item ascending, the user's CSR exclusion row (excl_off / excl_items as in

@@ -146,6 +146,26 @@ def _scale_rows(parts, scale, bufs):
             eng.rows_scale(b[0], sc.reshape(-1))
 
 
+def _rank_phases(parts, reduce, Bu, max_pos, scale, phase_call):
+    """The four phases of a sharded evaluation (orx_score_rank_shard / orx_score_rank_listed_shard) with ``reduce``
+    between them; phase_call(part, phase, bufs) runs one phase on one part.  -> the phase-3 outputs per part."""
+    bufs = []
+    for eng, kind, user, item, bias, g in parts:
+        n3 = eng.score_rank_shard_sizes(Bu, user.shape[1], max_pos)
+        dev = item.device
+        bufs.append((torch.empty(n3[0], dtype=torch.int32, device=dev), torch.empty(n3[1], dtype=torch.int32, device=dev),
+                     torch.empty(n3[2], dtype=torch.int64, device=dev)))
+    outs = [None] * len(parts)
+    for phase in range(4):   # every part's phase k is issued before any part's phase k + 1
+        for k, (part, b) in enumerate(zip(parts, bufs)):
+            outs[k] = phase_call(part, phase, b)
+        if phase < 3:
+            reduce([b[phase] for b in bufs])
+        if phase == 0:
+            _scale_rows(parts, scale, bufs)
+    return outs
+
+
 def score_rank_sharded(parts, reduce, uid, pos_off, pos_items, excl_off, excl_items, max_pos, at=(), scale=None):
     """Catalogue evaluation (AUC / NDCG / Recall, as native.Engine.score_rank on the global tables) of row-sharded
     tables, each rank counting over its own item rows: the four phases of orx_score_rank_shard, with ``reduce`` between
@@ -156,22 +176,24 @@ def score_rank_sharded(parts, reduce, uid, pos_off, pos_items, excl_off, excl_it
     ``scale`` (GMF): one [dim] tensor (or None) per part, the score_rank ``scale`` of the global call; the summed user
     rows are scaled after phase 0's reduce.
     -> [(auc, ndcg, recall)] per part, identical on every rank."""
-    bufs = []
-    for eng, kind, user, item, bias, g in parts:
-        n3 = eng.score_rank_shard_sizes(uid.numel(), user.shape[1], max_pos)
-        dev = item.device
-        bufs.append((torch.empty(n3[0], dtype=torch.int32, device=dev), torch.empty(n3[1], dtype=torch.int32, device=dev),
-                     torch.empty(n3[2], dtype=torch.int64, device=dev)))
-    outs = [None] * len(parts)
-    for phase in range(4):   # every part's phase k is issued before any part's phase k + 1
-        for k, ((eng, kind, user, item, bias, g), b) in enumerate(zip(parts, bufs)):
-            outs[k] = eng.score_rank_shard(kind, phase, g, user, item, bias, uid, pos_off, pos_items, excl_off,
-                                           excl_items, max_pos, *b, at=at)
-        if phase < 3:
-            reduce([b[phase] for b in bufs])
-        if phase == 0:
-            _scale_rows(parts, scale, bufs)
-    return outs
+    def phase_call(part, phase, b):
+        eng, kind, user, item, bias, g = part
+        return eng.score_rank_shard(kind, phase, g, user, item, bias, uid, pos_off, pos_items, excl_off, excl_items,
+                                    max_pos, *b, at=at)
+    return _rank_phases(parts, reduce, uid.numel(), max_pos, scale, phase_call)
+
+
+def score_rank_listed_sharded(parts, reduce, uid, pos_off, pos_items, neg_off, neg_items, excl_off, excl_items,
+                              max_pos, at=(), scale=None):
+    """Listed-candidate evaluation (as native.Engine.score_rank_listed on the global tables: each user ranked against
+    its listed items neg_off / neg_items only) of row-sharded tables: the four phases of orx_score_rank_listed_shard.
+    ``parts``, ``reduce``, uid, the global CSR lists and ``scale`` are as in score_rank_sharded.
+    -> [(auc, ndcg, recall)] per part, identical on every rank."""
+    def phase_call(part, phase, b):
+        eng, kind, user, item, bias, g = part
+        return eng.score_rank_listed_shard(kind, phase, g, user, item, bias, uid, pos_off, pos_items, neg_off,
+                                           neg_items, excl_off, excl_items, max_pos, *b, at=at)
+    return _rank_phases(parts, reduce, uid.numel(), max_pos, scale, phase_call)
 
 
 def score_topk_sharded(parts, reduce, uid, excl_off, excl_items, k, scale=None):
