@@ -188,7 +188,9 @@ def _bad_pair_ids(rng, U, I, B):
 class PairProb:
     """One pairwise problem: device tables + optimizer slots and their float64 oracle twins (from the float32-rounded
     device values).  run() launches one step and checks its dispatch record; verify() runs the oracle on the valid
-    triplets and checks out4, and the tables and every slot."""
+    triplets and checks out4, and the tables and every slot.  It runs the default constants (margin 0.5, c_l2 1, Keras
+    betas / eps) under the value bar; cases with other constants, slot initialisations and tie tables, judged by their
+    per-element updates, are built in tests/step_bar.py (plain numpy, shared with the CPU proof of that bar)."""
 
     def __init__(self, kind, optname, D, U, I, seed, scale=None):
         self.kind, self.optname, self.D, self.U, self.I = kind, optname, D, U, I
@@ -633,7 +635,7 @@ def test_pointwise_golden_fwd_grad(eng, golden_dir, kind):
 
 
 class PointProb:
-    """One pointwise problem (GMF: with its dense weight w), as PairProb."""
+    """One pointwise problem (GMF: with its dense weight w), as PairProb (non-default constants: tests/step_bar.py)."""
 
     def __init__(self, kind, optname, D, U, I, seed, sig=False):
         self.kind, self.optname, self.D, self.U, self.I = kind, optname, D, U, I

@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 import torch
 
+import step_bar as S
 from oracle import openrec_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -19,12 +20,14 @@ def _oracle_state(user, item, bias, opt_kind):
     return {k: (np.zeros_like(v), np.zeros_like(v)) for k, v in zip(("user", "item", "bias"), (user, item, bias))}
 
 
-def _run(world, kind, opt_kind, U, I, D, B, steps=3, bad=False, seed=5, announce=False):
+def _run(world, kind, opt_kind, U, I, D, B, steps=3, bad=False, seed=5, announce=False, c_l2=1.0, margin=0.5, eps=1e-7,
+         beta1=0.9, beta2=0.999):
     from openrec_b200.sharded import LoopbackGroup
     rng = np.random.default_rng(seed)
     sc = 0.05 if kind == 0 else 0.4
     user, item, bias = (rng.uniform(-sc, sc, s).astype(np.float32).astype(np.float64) for s in ((U, D), (I, D), (I, 1)))
-    g = LoopbackGroup(world, U, I, D, B, kind=kind, opt_kind=opt_kind, lr=0.05, init=False)
+    consts = dict(eps=eps, beta1=beta1, beta2=beta2)
+    g = LoopbackGroup(world, U, I, D, B, kind=kind, opt_kind=opt_kind, lr=0.05, margin=margin, init=False, **consts)
     try:
         g.load_global(user, item, bias)
         st = _oracle_state(user, item, bias, opt_kind)
@@ -44,13 +47,13 @@ def _run(world, kind, opt_kind, U, I, D, B, steps=3, bad=False, seed=5, announce
             # announce: the next step's route / request are issued inside this step (every second time, so that announced
             # and plain steps alternate)
             nxt = all_batches[step + 1] if announce and step + 1 < steps and step % 3 != 2 else None
-            outs = [o.cpu().numpy() for o in g.step(batches, next_batches=nxt)]
+            outs = [o.cpu().numpy() for o in g.step(batches, c_l2=c_l2, next_batches=nxt)]
             g.check()
             good = [a[ok] for a in ids]
             # BPR's 1/B is over the SUBMITTED batch (skipped triplets still count, as in the single-GPU step)
             frac = ok.sum() / (B * world) if kind == 0 else 1.0
             loss, l2 = O.pairwise_train_step("bpr" if kind == 0 else "ucml", user, item, bias, *good, oracle_opt, st,
-                                             step + 1, 0.05, margin=0.5, c_loss=frac)
+                                             step + 1, 0.05, margin=margin, c_loss=frac, c_l2=c_l2, **consts)
             loss = loss * frac
             for o in outs:
                 np.testing.assert_allclose(o, [loss, l2], rtol=3e-5, atol=1e-6)
@@ -67,6 +70,55 @@ def _run(world, kind, opt_kind, U, I, D, B, steps=3, bad=False, seed=5, announce
 @pytest.mark.parametrize("kind,opt_kind", [(0, 1), (0, 0), (1, 1), (0, 2)])
 def test_loopback_matches_oracle(world, kind, opt_kind):
     _run(world, kind, opt_kind, U=1501, I=2003, D=128, B=1024)
+
+
+def test_loopback_constants():
+    """Non-default c_l2, margin, eps and betas reach the sharded step (three steps, value bar)."""
+    _run(2, 1, 2, U=301, I=407, D=64, B=256, c_l2=0.25, margin=1.25, eps=1e-2, beta1=0.5, beta2=0.75)
+
+
+def _step_bar(world, arm, kind, opt, D=128, B=256):
+    """One step of `world` loopback ranks on the global batch of a step_bar arm (a) / (d) case, every table and slot
+    judged by step_bar.Bar: the global inv_B, the cross-rank duplicate reduction and the apply of orx_shard_step."""
+    from openrec_b200.sharded import LoopbackGroup
+    c = S.loopback_case(world, arm, kind, opt, D, B)
+    P = c.P
+    g = LoopbackGroup(world, len(c.tabs["user"]), len(c.tabs["item"]), D, B, kind=S.PAIR_KINDS.index(kind),
+                      opt_kind=opt, lr=c.lr, eps=P["eps"], beta1=P["beta1"], beta2=P["beta2"], margin=P["margin"],
+                      init=False)
+    try:
+        g.load_global(*(c.tabs[n] for n in c.names))
+        for m in g.ranks:
+            m.iterations = c.step - 1                # the step below runs at Adam step c.step
+            for name, slots in zip(c.names, (m.user_slots, m.item_slots, m.bias_slots)):
+                for k, s in enumerate(c.slots[name]):
+                    if s is not None:
+                        local = s[m.rank::world]
+                        slots[k][:len(local)] = torch.as_tensor(local, dtype=torch.float32).reshape(-1, s.shape[1])
+        batches = [tuple(torch.from_numpy(a[r * B:(r + 1) * B].copy()).cuda() for a in c.ids) for r in range(world)]
+        g.step(batches, c_loss=P["c_loss"], c_l2=P["c_l2"])
+        g.check()
+        torch.cuda.synchronize()
+        got = {}
+        for j, name in enumerate(c.names):
+            arrs = [c.tabs[name].copy()] + [None if s is None else s.copy() for s in c.slots[name]]
+            for m in g.ranks:
+                n_loc = len(arrs[0][m.rank::world])
+                shard = (m.local_shards()[j], *((m.user_slots, m.item_slots, m.bias_slots)[j]))
+                for a, t in zip(arrs, shard):
+                    if a is not None:
+                        a[m.rank::world] = t[:n_loc].cpu().numpy().reshape(n_loc, -1)
+            got[name] = tuple(arrs)
+        S.Bar(c).check(got, f"loopback world {world}")
+    finally:
+        g.close()
+
+
+@pytest.mark.parametrize("world,arm,kind,opt", S.loopback_specs())
+def test_loopback_step_updates(world, arm, kind, opt):
+    """Two ranks, arm (a) (loss only, Keras slots) and arm (d) (beta1 0.5, beta2 0.75, eps 1e-2, margin 1.25 at step 3)
+    under the per-element update bar of tests/step_bar.py; the batch has users and items shared across the ranks."""
+    _step_bar(world, arm, kind, opt)
 
 
 @pytest.mark.parametrize("D", [8, 64, 192, 256, 512])
