@@ -63,8 +63,23 @@ enum orx_score_kind { ORX_SCORE_DOT = 0, ORX_SCORE_NEG_SQDIST = 1 };
  *   ADAM_LAZY  row-sparse Adam (NOT the reference's semantics; explicit opt-in)
  *   ADAM_DENSE Keras-2.0 Adam on IndexedSlices: m,v decay and var update sweep the WHOLE table
  *              every step (what `optimizers.Adam()` in tf2_examples/bpr_citeulike.py:31 does)
- * For Adam s0 = m, s1 = v, lr_t = lr*sqrt(1-beta2^step)/(1-beta1^step), step is 1-based. */
-enum orx_opt_kind { ORX_OPT_SGD = 0, ORX_OPT_ADAGRAD = 1, ORX_OPT_ADAM_LAZY = 2, ORX_OPT_ADAM_DENSE = 3 };
+ *   ROWWISE_ADAGRAD  one accumulator per table row (an addition, not in the reference; explicit opt-in):
+ *              acc[r] += (1/dim) * sum_j G[j]^2; var[r][j] -= lr*G[j]/(sqrt(acc[r])+eps)   (s0 = acc, float[rows])
+ *              Rows the batch does not touch keep row and accumulator bit for bit.  The sum over the row runs in an
+ *              order each kernel fixes, so a row referenced once in a batch updates to the same bits on every run.  A
+ *              dim-1 table (the item bias among them) updates exactly as ADAGRAD does.  Dense variables
+ *              (orx_dense_apply's var, the pointwise step's GMF weight w) get element-wise ADAGRAD, s0 element-wise.
+ *              orx_shard_step does not take it.
+ * For Adam s0 = m, s1 = v, lr_t = lr*sqrt(1-beta2^step)/(1-beta1^step), step is 1-based.  Adagrad and Adam use the
+ * sqrt.approx / rcp.approx approximations. */
+enum orx_opt_kind {
+  ORX_OPT_SGD = 0,
+  ORX_OPT_ADAGRAD = 1,
+  ORX_OPT_ADAM_LAZY = 2,
+  ORX_OPT_ADAM_DENSE = 3,
+  /* 4 is not assigned: every entry point refuses it as an unknown kind (ORX_ERR_INVALID), as it always has */
+  ORX_OPT_ROWWISE_ADAGRAD = 5
+};
 
 typedef struct {
   int32_t kind; /* orx_opt_kind */
@@ -75,7 +90,8 @@ typedef struct {
 /* One LatentFactor (openrec/tf2/modules/latent_factor.py:4-15) and its optimizer slots. */
 typedef struct {
   float* var;   /* [rows, dim] */
-  float* s0;    /* Adagrad accumulator | Adam m ; NULL for SGD */
+  float* s0;    /* Adagrad accumulator [rows, dim] | Adam m [rows, dim] | row-wise Adagrad accumulator float[rows]
+                   (4-byte alignment is enough: it is read as scalars) ; NULL for SGD */
   float* s1;    /* Adam v ; NULL otherwise */
   int64_t rows;
   int32_t dim;

@@ -185,13 +185,23 @@ static inline auto orx_dispatch(int v, F&& f) {
 }
 template <typename F>
 static inline auto orx_dispatch_opt(int opt_kind, F&& f) {
-  return orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE>(opt_kind, f);
+  return orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE, ORX_OPT_ROWWISE_ADAGRAD>(
+      opt_kind, f);
 }
 
-// an orx_opt_kind
-static inline bool orx_opt_kind_ok(int kind) { return kind >= ORX_OPT_SGD && kind <= ORX_OPT_ADAM_DENSE; }
-// The host side of OrxOptSlots: every table carries the slot rows optimizer `kind` keeps -- s0 for every kind but SGD,
-// s1 for both Adams (ADAM_DENSE's sweep keeps m and v there).  Null tables are skipped.
+// an orx_opt_kind (4 is unassigned and refused: orx_dispatch_opt would otherwise run it as its last listed kind)
+static inline bool orx_opt_kind_ok(int kind) {
+  return (kind >= ORX_OPT_SGD && kind <= ORX_OPT_ADAM_DENSE) || kind == ORX_OPT_ROWWISE_ADAGRAD;
+}
+// The optimizer *o as a table of row width dim runs it: a dim-1 table under ROWWISE_ADAGRAD runs ADAGRAD (its one
+// accumulator per row is the element-wise one, and the update then rounds exactly as ADAGRAD's).
+static inline orx_opt_t orx_opt_dim(const orx_opt_t* o, int dim) {
+  orx_opt_t r = *o;
+  if (r.kind == ORX_OPT_ROWWISE_ADAGRAD && dim == 1) r.kind = ORX_OPT_ADAGRAD;
+  return r;
+}
+// The host side of OrxOptSlots: every table carries the slot rows optimizer `kind` keeps -- s0 for every kind but SGD
+// (ROWWISE_ADAGRAD: float[rows]), s1 for both Adams (ADAM_DENSE's sweep keeps m and v there).  Null tables are skipped.
 bool orx_opt_slots_ok(int kind, std::initializer_list<const orx_table_t*> tabs);
 
 // True when every pointer is 16-byte aligned (a null pointer, an absent slot row, counts as aligned).  The one rule of
@@ -387,19 +397,40 @@ __device__ __forceinline__ float orx_rcp_fast(float x) {
   return r;
 }
 
-// Which optimizer-slot rows an update reads and writes: S0 = Adagrad accumulator / Adam m, S1 = Adam v.  STAGE_ONLY:
-// ADAM_DENSE updates no row in a step kernel; every row is staged and the sweep (k_adam_sweep) applies Adam to the table.
+// Which optimizer-slot rows an update reads and writes: S0 = Adagrad accumulator / Adam m, S1 = Adam v, both one
+// element per table element.  STAGE_ONLY: ADAM_DENSE updates no row in a step kernel; every row is staged and the sweep
+// (k_adam_sweep) applies Adam to the table.  ROW: ROWWISE_ADAGRAD keeps S0 as one scalar per row (s0[id]) and no S1;
+// a row's update needs the sum of its squared gradient first (orx_row_scale).  ELEM: the optimizer of the dim-1 and
+// dense variables a kernel updates beside its rows (the item bias, GMF's w): element-wise ADAGRAD for ROW.
 template <int OPT>
 struct OrxOptSlots {
   static constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
   static constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
   static constexpr bool STAGE_ONLY = (OPT == ORX_OPT_ADAM_DENSE);
+  static constexpr bool ROW = (OPT == ORX_OPT_ROWWISE_ADAGRAD);
+  static constexpr int ELEM = ROW ? ORX_OPT_ADAGRAD : OPT;
 };
+
+// Row-wise Adagrad of one row of width D whose squared gradient sums to ss: acc += ss / D, and the row's factor
+// 1 / (sqrt(acc) + eps), with the approximations of ADAGRAD.  Each element then moves by lr * g * factor
+// (orx_row_apply4 / orx_row_apply1), the order in which ADAGRAD rounds lr * g * rcp(...).
+__device__ __forceinline__ float orx_row_scale(float& acc, float ss, int D, const OrxOptDev& o) {
+  acc = acc + ss / (float)D;
+  return orx_rcp_fast(orx_sqrt_fast(acc) + o.eps);
+}
+__device__ __forceinline__ float orx_sq4(float4 g) { return g.x * g.x + g.y * g.y + g.z * g.z + g.w * g.w; }
+__device__ __forceinline__ float4 orx_row_apply4(float4 w, float4 g, float f, const OrxOptDev& o) {
+  return make_float4(w.x - o.lr * g.x * f, w.y - o.lr * g.y * f, w.z - o.lr * g.z * f, w.w - o.lr * g.w * f);
+}
+__device__ __forceinline__ float orx_row_apply1(float w, float g, float f, const OrxOptDev& o) {
+  return w - o.lr * g * f;
+}
 
 // One optimizer update of one scalar.  OPT is an orx_opt_kind (ADAM_DENSE never reaches here:
 // its rows are staged and swept).
 template <int OPT>
 __device__ __forceinline__ float orx_apply(float w, float g, float& s0, float& s1, const OrxOptDev& o) {
+  static_assert(OPT != ORX_OPT_ROWWISE_ADAGRAD, "a row-wise row is updated through orx_row_scale");
   if (OPT == ORX_OPT_SGD) {
     return w - o.lr * g;
   } else if (OPT == ORX_OPT_ADAGRAD) {
@@ -441,6 +472,20 @@ __device__ __forceinline__ void orx_own_or_stage4(bool own, float* W, float* P0,
     st(W + i, orx_apply4<OPT>(w, g, s0, s1, o));
     if (SL::S0) st(P0 + i, s0);
     if (SL::S1) st(P1 + i, s1);
+  } else {
+    orx_red4(G + (int64_t)d * D + off, g);
+  }
+}
+
+// The ROWWISE_ADAGRAD form of orx_own_or_stage4: an owned row moves by its factor f (orx_row_scale, taken by the caller
+// over the whole row) and has no slot row here -- the caller stores its accumulator once.
+template <bool STREAM>
+__device__ __forceinline__ void orx_own_or_stage4_row(bool own, float* W, int id, float* G, int d, int D, int off,
+                                                      float4 w, float4 g, float f, const OrxOptDev& o) {
+  if (own) {
+    const float4 r = orx_row_apply4(w, g, f, o);
+    if (STREAM) orx_st4_stream(W + (int64_t)id * D + off, r);
+    else __stcg(reinterpret_cast<float4*>(W + (int64_t)id * D + off), r);
   } else {
     orx_red4(G + (int64_t)d * D + off, g);
   }
@@ -622,6 +667,73 @@ __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni)
     }
   }
   // (the hash tables are not cleared: the next step uses a new epoch)
+}
+
+// orx_tail_rows under ROWWISE_ADAGRAD: the same eight lanes per staged row take the sum of the row's squared gradient
+// first -- lane sl over float4 (scalar) indices sl, sl + 8, ... in order, then the fixed 8-lane tree -- and only then
+// apply: a second pass over G, which the step's red.adds left in L2.  The row's accumulator s0[id] is one scalar; the
+// item bias gets element-wise ADAGRAD.
+template <bool VEC>
+__device__ __forceinline__ void orx_tail_rows_rowwise(const TailArgs& a, int nu, int ni) {
+  const int lane = threadIdx.x & 31;
+  const int gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  const int D = a.D;
+  const bool vec = VEC && (D & 3) == 0;
+  const int nq = D >> 2;
+  const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  const int sub = lane >> 3, sl = lane & 7;
+  for (int r0 = gwarp * 4; r0 < nu + ni; r0 += nwarps * 4) {   // warp-uniform: the 8-lane sums below see every lane
+    const int r = r0 + sub;
+    const bool on = r < nu + ni;
+    const bool is_u = on && r < nu;
+    const int d = on ? (is_u ? r : r - nu) : 0;
+    const int id = on ? (is_u ? a.hu.did[d] : a.hi.did[d]) : 0;
+    float* G = (is_u ? a.gu : a.gi) + (int64_t)d * D;
+    float* W = (is_u ? a.U : a.I) + (int64_t)id * D;
+    float* P0 = (is_u ? a.Us0 : a.Is0) + id;
+    float ss = 0.f, acc = 0.f;
+    if (on) {
+      acc = __ldcg(P0);
+      if (vec) {
+        for (int e = sl; e < nq; e += 8) ss += orx_sq4(__ldcg(reinterpret_cast<const float4*>(G) + e));
+      } else {
+        for (int e = sl; e < D; e += 8) ss += G[e] * G[e];
+      }
+    }
+    ss = orx_group_sum<8>(ss);
+    const float f = orx_row_scale(acc, ss, D, a.opt);
+    if (on) {
+      if (sl == 0) __stcg(P0, acc);
+      if (vec) {
+        for (int e0 = 0; e0 < nq; e0 += 32) {   // as orx_tail_rows: a chunk's loads before its first use
+          float4 g[4], w[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int e = e0 + sl + 8 * k;
+            g[k] = e < nq ? __ldcg(reinterpret_cast<const float4*>(G) + e) : z4;
+            w[k] = e < nq ? orx_ld4_stream(W + 4 * e) : z4;
+          }
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int e = e0 + sl + 8 * k;
+            if (e >= nq) continue;
+            orx_st4_stream(W + 4 * e, orx_row_apply4(w[k], g[k], f, a.opt));
+            __stcg(reinterpret_cast<float4*>(G) + e, z4);
+          }
+        }
+      } else {
+        for (int e = sl; e < D; e += 8) {
+          W[e] = orx_row_apply1(W[e], G[e], f, a.opt);
+          G[e] = 0.f;
+        }
+      }
+      if (!is_u && sl == 0) {   // the item bias of the staged row
+        orx_update1<ORX_OPT_ADAGRAD>(a.Bv + id, a.Bs0 + id, nullptr, a.Bv[id], a.gb[d], a.opt);
+        a.gb[d] = 0.f;
+      }
+    }
+  }
 }
 #endif  // __CUDACC__
 

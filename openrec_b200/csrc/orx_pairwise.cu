@@ -117,6 +117,7 @@ struct TripRegs {
   float4 u[K], p[K], n[K];
   float4 us0[K], ps0[K], ns0[K];  // dead arrays are eliminated when the optimizer has no such slot
   float4 us1[K], ps1[K], ns1[K];
+  float uacc, pacc, nacc;         // ROWWISE_ADAGRAD: the rows' accumulators (one scalar per row)
   int fl, uu, pp, nn, du, dp, dn;
 };
 
@@ -137,6 +138,7 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
   constexpr int K = D / (4 * G);                // float4 per lane per row
   constexpr int TPW = 32 / G;                   // triplets in flight per warp
   typedef OrxOptSlots<OPT> SL;
+  typedef OrxOptSlots<SL::ELEM> BL;             // the item bias's optimizer (element-wise)
   static_assert(CH % TPW == 0, "chunk must be a multiple of the triplets per warp");
   typedef TripRegs<K, SL::S0, SL::S1> Regs;
 
@@ -196,11 +198,11 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
     bn = orx_ld_keep(a.Bv + n_id);
     if (!SL::STAGE_ONLY) {
       if (!a.res) flags |= (cu == 1u ? 2 : 0) | (cp == 1u ? 4 : 0) | (cn == 1u ? 8 : 0);
-      if (SL::S0) {
+      if (BL::S0) {
         if (flags & 4) bps0 = orx_ld_keep(a.Bs0 + p_id);
         if (flags & 8) bns0 = orx_ld_keep(a.Bs0 + n_id);
       }
-      if (SL::S1) {
+      if (BL::S1) {
         if (flags & 4) bps1 = orx_ld_keep(a.Bs1 + p_id);
         if (flags & 8) bns1 = orx_ld_keep(a.Bs1 + n_id);
       }
@@ -228,6 +230,11 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
         r.ps1[k] = (r.fl & 4) ? orx_ld4_stream(a.Is1 + (int64_t)r.pp * D + off) : z4;
         r.ns1[k] = (r.fl & 8) ? orx_ld4_stream(a.Is1 + (int64_t)r.nn * D + off) : z4;
       }
+    }
+    if (SL::ROW) {
+      r.uacc = (r.fl & 2) ? __ldcg(a.Us0 + r.uu) : 0.f;
+      r.pacc = (r.fl & 4) ? __ldcg(a.Is0 + r.pp) : 0.f;
+      r.nacc = (r.fl & 8) ? __ldcg(a.Is0 + r.nn) : 0.f;
     }
   };
   load_slots(0, ra);
@@ -264,7 +271,40 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
       const float val = __shfl_sync(ORX_FULL, gbias, q * G);
       if (lane == j + q) g_own = val;
     }
-    if (v) {
+    if constexpr (SL::ROW) {
+      // each row's sum of squared gradients over its G lanes (k in order, then the fixed xor tree), taken outside
+      // `if (v)`: v is per triplet group, the shuffles need the whole warp.  An invalid triplet's gradients are zeros.
+      float su = 0.f, sp = 0.f, sn = 0.f;
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        float4 gu, gp, gn;
+        pair_row_grads<KIND>(g, a.c_l2, r.u[k], r.p[k], r.n[k], &gu, &gp, &gn);
+        su += orx_sq4(gu);
+        sp += orx_sq4(gp);
+        sn += orx_sq4(gn);
+      }
+      su = orx_group_sum<G>(su);
+      sp = orx_group_sum<G>(sp);
+      sn = orx_group_sum<G>(sn);
+      const float fu = orx_row_scale(r.uacc, su, D, a.opt), fp = orx_row_scale(r.pacc, sp, D, a.opt),
+                  fn = orx_row_scale(r.nacc, sn, D, a.opt);
+      if (v) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+          const int off = (k * G + gl) * 4;
+          float4 gu, gp, gn;
+          pair_row_grads<KIND>(g, a.c_l2, r.u[k], r.p[k], r.n[k], &gu, &gp, &gn);
+          orx_own_or_stage4_row<true>(r.fl & 2, a.U, r.uu, a.gu, r.du, D, off, r.u[k], gu, fu, a.opt);
+          orx_own_or_stage4_row<true>(r.fl & 4, a.I, r.pp, a.gi, r.dp, D, off, r.p[k], gp, fp, a.opt);
+          orx_own_or_stage4_row<true>(r.fl & 8, a.I, r.nn, a.gi, r.dn, D, off, r.n[k], gn, fn, a.opt);
+        }
+        if (gl == 0) {
+          if (r.fl & 2) __stcg(a.Us0 + r.uu, r.uacc);
+          if (r.fl & 4) __stcg(a.Is0 + r.pp, r.pacc);
+          if (r.fl & 8) __stcg(a.Is0 + r.nn, r.nacc);
+        }
+      }
+    } else if (v) {
 #pragma unroll
       for (int k = 0; k < K; ++k) {
         const int off = (k * G + gl) * 4;
@@ -311,16 +351,16 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
   // ---- item_bias: lane-parallel, one lane per triplet of the chunk
   if (flags & 1) {
     if (flags & 4) {
-      __stcg(a.Bv + p_id, orx_apply<OPT>(bp, g_own, bps0, bps1, a.opt));
-      if (SL::S0) __stcg(a.Bs0 + p_id, bps0);
-      if (SL::S1) __stcg(a.Bs1 + p_id, bps1);
+      __stcg(a.Bv + p_id, orx_apply<SL::ELEM>(bp, g_own, bps0, bps1, a.opt));
+      if (BL::S0) __stcg(a.Bs0 + p_id, bps0);
+      if (BL::S1) __stcg(a.Bs1 + p_id, bps1);
     } else {
       atomicAdd(a.gb + dp, g_own);
     }
     if (flags & 8) {
-      __stcg(a.Bv + n_id, orx_apply<OPT>(bn, -g_own, bns0, bns1, a.opt));
-      if (SL::S0) __stcg(a.Bs0 + n_id, bns0);
-      if (SL::S1) __stcg(a.Bs1 + n_id, bns1);
+      __stcg(a.Bv + n_id, orx_apply<SL::ELEM>(bn, -g_own, bns0, bns1, a.opt));
+      if (BL::S0) __stcg(a.Bs0 + n_id, bns0);
+      if (BL::S1) __stcg(a.Bs1 + n_id, bns1);
     } else {
       atomicAdd(a.gb + dn, -g_own);
     }
@@ -380,23 +420,62 @@ __global__ void __launch_bounds__(256) k_pair_generic(const PairArgs a) {
       const uint32_t cp = orx_hash_find<!STAGE_ONLY>(a.hi, pp, &dp);
       const uint32_t cn = orx_hash_find<!STAGE_ONLY>(a.hi, nn, &dn);
       const bool fu = !STAGE_ONLY && cu == 1u, fp = !STAGE_ONLY && cp == 1u, fn = !STAGE_ONLY && cn == 1u;
-      for (int d = lane; d < D; d += 32) {
-        const float u = ur[d], p = pr[d], n = nr[d];
-        float gu, gp, gn;
-        pair_grads1<KIND>(g, a.c_l2, u, p, n, &gu, &gp, &gn);
-        const int64_t ou = (int64_t)uu * D + d, op = (int64_t)pp * D + d, on = (int64_t)nn * D + d;
-        if (fu) orx_update1<OPT>(ur + d, a.Us0 + ou, a.Us1 + ou, u, gu, a.opt);
-        else atomicAdd(a.gu + (int64_t)du * D + d, gu);
-        if (fp) orx_update1<OPT>(pr + d, a.Is0 + op, a.Is1 + op, p, gp, a.opt);
-        else atomicAdd(a.gi + (int64_t)dp * D + d, gp);
-        if (fn) orx_update1<OPT>(nr + d, a.Is0 + on, a.Is1 + on, n, gn, a.opt);
-        else atomicAdd(a.gi + (int64_t)dn * D + d, gn);
-      }
-      if (lane == 0) {
-        if (fp) orx_update1<OPT>(a.Bv + pp, a.Bs0 + pp, a.Bs1 + pp, bp, gbias, a.opt);
-        else atomicAdd(a.gb + dp, gbias);
-        if (fn) orx_update1<OPT>(a.Bv + nn, a.Bs0 + nn, a.Bs1 + nn, bn, -gbias, a.opt);
-        else atomicAdd(a.gb + dn, -gbias);
+      if constexpr (OrxOptSlots<OPT>::ROW) {
+        // each owned row's sum of squared gradients first (lane-strided, then the xor tree: ok is warp-uniform), then
+        // the apply in a second pass over the rows
+        float su = 0.f, sp = 0.f, sn = 0.f;
+        for (int d = lane; d < D; d += 32) {
+          float gu, gp, gn;
+          pair_grads1<KIND>(g, a.c_l2, ur[d], pr[d], nr[d], &gu, &gp, &gn);
+          su += gu * gu;
+          sp += gp * gp;
+          sn += gn * gn;
+        }
+        su = orx_group_sum<32>(su);
+        sp = orx_group_sum<32>(sp);
+        sn = orx_group_sum<32>(sn);
+        float au = fu ? a.Us0[uu] : 0.f, ap = fp ? a.Is0[pp] : 0.f, an = fn ? a.Is0[nn] : 0.f;
+        const float xu = orx_row_scale(au, su, D, a.opt), xp = orx_row_scale(ap, sp, D, a.opt),
+                    xn = orx_row_scale(an, sn, D, a.opt);
+        for (int d = lane; d < D; d += 32) {
+          const float u = ur[d], p = pr[d], n = nr[d];
+          float gu, gp, gn;
+          pair_grads1<KIND>(g, a.c_l2, u, p, n, &gu, &gp, &gn);
+          if (fu) ur[d] = orx_row_apply1(u, gu, xu, a.opt);
+          else atomicAdd(a.gu + (int64_t)du * D + d, gu);
+          if (fp) pr[d] = orx_row_apply1(p, gp, xp, a.opt);
+          else atomicAdd(a.gi + (int64_t)dp * D + d, gp);
+          if (fn) nr[d] = orx_row_apply1(n, gn, xn, a.opt);
+          else atomicAdd(a.gi + (int64_t)dn * D + d, gn);
+        }
+        if (lane == 0) {
+          if (fu) a.Us0[uu] = au;
+          if (fp) a.Is0[pp] = ap;
+          if (fn) a.Is0[nn] = an;
+          if (fp) orx_update1<ORX_OPT_ADAGRAD>(a.Bv + pp, a.Bs0 + pp, nullptr, bp, gbias, a.opt);
+          else atomicAdd(a.gb + dp, gbias);
+          if (fn) orx_update1<ORX_OPT_ADAGRAD>(a.Bv + nn, a.Bs0 + nn, nullptr, bn, -gbias, a.opt);
+          else atomicAdd(a.gb + dn, -gbias);
+        }
+      } else {
+        for (int d = lane; d < D; d += 32) {
+          const float u = ur[d], p = pr[d], n = nr[d];
+          float gu, gp, gn;
+          pair_grads1<KIND>(g, a.c_l2, u, p, n, &gu, &gp, &gn);
+          const int64_t ou = (int64_t)uu * D + d, op = (int64_t)pp * D + d, on = (int64_t)nn * D + d;
+          if (fu) orx_update1<OPT>(ur + d, a.Us0 + ou, a.Us1 + ou, u, gu, a.opt);
+          else atomicAdd(a.gu + (int64_t)du * D + d, gu);
+          if (fp) orx_update1<OPT>(pr + d, a.Is0 + op, a.Is1 + op, p, gp, a.opt);
+          else atomicAdd(a.gi + (int64_t)dp * D + d, gp);
+          if (fn) orx_update1<OPT>(nr + d, a.Is0 + on, a.Is1 + on, n, gn, a.opt);
+          else atomicAdd(a.gi + (int64_t)dn * D + d, gn);
+        }
+        if (lane == 0) {
+          if (fp) orx_update1<OPT>(a.Bv + pp, a.Bs0 + pp, a.Bs1 + pp, bp, gbias, a.opt);
+          else atomicAdd(a.gb + dp, gbias);
+          if (fn) orx_update1<OPT>(a.Bv + nn, a.Bs0 + nn, a.Bs1 + nn, bn, -gbias, a.opt);
+          else atomicAdd(a.gb + dn, -gbias);
+        }
       }
       continue;
     }
@@ -466,7 +545,8 @@ __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
   __shared__ bool last;
   orx_pdl_wait();
   const int nu = *a.hu.counter, ni = a.I ? *a.hi.counter : 0;
-  orx_tail_rows<OPT, VEC>(a, nu, ni);
+  if constexpr (OrxOptSlots<OPT>::ROW) orx_tail_rows_rowwise<VEC>(a, nu, ni);
+  else orx_tail_rows<OPT, VEC>(a, nu, ni);
 
   if (blockIdx.x == 0 && a.out4) {
     // deterministic loss reduction; GMF: l2_loss also holds 0.5*sum(w^2) of the PRE-step weight (gmf.py:31-32)
@@ -478,12 +558,12 @@ __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
       a.out4[2] = (float)a.counters[3];
       a.out4[3] = (float)(nu + ni);
     }
-    // GMF dense weight: grad = gw + c_l2*w  (gmf.py:31-32), Keras dense apply
+    // GMF dense weight: grad = gw + c_l2*w  (gmf.py:31-32), Keras dense apply (element-wise ADAGRAD under ROWWISE)
     if (a.W) {
       for (int e = threadIdx.x; e < a.D; e += blockDim.x) {
         const float g = a.gw[e] + a.c_l2 * a.W[e];
         if (OrxOptSlots<OPT>::STAGE_ONLY) orx_adam_dense1(a.W, a.Ws0, a.Ws1, e, g, a.opt);
-        else orx_update1<OPT>(a.W + e, a.Ws0 + e, a.Ws1 + e, a.W[e], g, a.opt);
+        else orx_update1<OrxOptSlots<OPT>::ELEM>(a.W + e, a.Ws0 + e, a.Ws1 + e, a.W[e], g, a.opt);
         a.gw[e] = 0.f;
       }
     }
@@ -501,7 +581,9 @@ __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
 
 int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st) {
   const int grid = c->num_sms * 4;  // ~1-2 staged rows per warp: the tail is a latency chain, not bandwidth
-  const bool vec = orx_aligned16(ta.U, ta.Us0, ta.Us1, ta.I, ta.Is0, ta.Is1);
+  // a row-wise accumulator is read as scalars: only the table rows decide
+  const bool vec = opt_kind == ORX_OPT_ROWWISE_ADAGRAD ? orx_aligned16(ta.U, ta.I)
+                                                       : orx_aligned16(ta.U, ta.Us0, ta.Us1, ta.I, ta.Is0, ta.Is1);
   orx_dispatch_opt(opt_kind, [&](auto O) {
     orx_dispatch<0, 1>(vec ? 1 : 0, [&](auto V) {
       orx_launch_pdl(k_sparse_tail<decltype(O)::value, decltype(V)::value == 1>, dim3(grid), dim3(256), 0, st, ta);
@@ -569,8 +651,12 @@ static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, OrxSte
     orx_launch_pdl(kern, dim3(blocks), dim3(256), 0, st, pa);
   };
   constexpr int PV = LAZY ? ORX_VARIANT_STEP : ORX_VARIANT_STEP_PIPE;
-  // k_pair_step moves table and slot rows as float4: a table or slot base off a 16-byte boundary takes k_pair_generic
-  const bool vec = orx_aligned16(pa.U, pa.Us0, pa.Us1, pa.I, pa.Is0, pa.Is1);
+  // k_pair_step moves table and slot rows as float4: a table or slot base off a 16-byte boundary takes k_pair_generic.
+  // ROWWISE_ADAGRAD reads its accumulators as scalars, so only the tables decide; it holds three accumulator scalars
+  // (and the rows' gradients over the row sum) where ADAGRAD holds 3K float4 slot registers, and takes ADAGRAD's
+  // variants: PIPE at D = 32, 64, 256, four CTAs/SM without PIPE at D = 128 (no spills under -Xptxas -v).
+  const bool vec = OrxOptSlots<OPT>::ROW ? orx_aligned16(pa.U, pa.I)
+                                         : orx_aligned16(pa.U, pa.Us0, pa.Us1, pa.I, pa.Is0, pa.Is1);
   switch (vec ? pa.D : 0) {
     case 32: go(k_pair_step<KIND, OPT, 32, 8, 2, !LAZY>, PV, 2, blocks); break;
     case 64: go(k_pair_step<KIND, OPT, 64, 8, 2, !LAZY>, PV, 2, blocks); break;
@@ -739,6 +825,11 @@ static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, con
                               cudaStream_t st) {
   ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
   ORX_REQUIRE(nid != nullptr, "empty batch or null ids");
+  orx_opt_t od;
+  if (opt && user) {   // dim-1 rows under ROWWISE_ADAGRAD run (and are recorded) as ADAGRAD
+    od = orx_opt_dim(opt, user->dim);
+    opt = &od;
+  }
   const float inv_B = 1.0f / (float)B;
   const auto kernel = [&](const SparseArgs& s, const int4* res, float* partials, OrxStepLaunch* out) {
     PairArgs pa = pair_args(s, user->rows, item->rows, uid, pid, nid, B, margin, c_loss, c_l2, inv_B);

@@ -48,6 +48,7 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
   constexpr int K = D / (4 * G);
   constexpr int TPW = 32 / G;
   typedef OrxOptSlots<OPT> SL;
+  typedef OrxOptSlots<SL::ELEM> BL;   // the item bias's optimizer (element-wise)
   constexpr bool GMF = (KIND == ORX_POINT_GMF);
   __shared__ float sgw[GMF ? D : 1];
 
@@ -73,8 +74,8 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
       flags = 1;
       if (!SL::STAGE_ONLY) {
         flags |= (cu == 1u ? 2 : 0) | (ci == 1u ? 4 : 0);
-        if (SL::S0 && (flags & 4)) bs0 = __ldcg(a.Bs0 + i_id);
-        if (SL::S1 && (flags & 4)) bs1 = __ldcg(a.Bs1 + i_id);
+        if (BL::S0 && (flags & 4)) bs0 = __ldcg(a.Bs0 + i_id);
+        if (BL::S1 && (flags & 4)) bs1 = __ldcg(a.Bs1 + i_id);
       }
     }
   }
@@ -126,7 +127,46 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
       const float val = __shfl_sync(ORX_FULL, g, q * G);
       if (lane == j + q) g_own = val;
     }
-    if (v) {
+    if constexpr (SL::ROW) {
+      // each row's sum of squared gradients over its G lanes before the apply, outside `if (v)` (per triplet group)
+      const float c2 = a.c_l2;
+      auto grads = [&](int k, float4& gu, float4& gi) {
+        gu = make_float4(g * w[k].x * it[k].x + c2 * u[k].x, g * w[k].y * it[k].y + c2 * u[k].y,
+                         g * w[k].z * it[k].z + c2 * u[k].z, g * w[k].w * it[k].w + c2 * u[k].w);
+        gi = make_float4(g * w[k].x * u[k].x + c2 * it[k].x, g * w[k].y * u[k].y + c2 * it[k].y,
+                         g * w[k].z * u[k].z + c2 * it[k].z, g * w[k].w * u[k].w + c2 * it[k].w);
+      };
+      float su = 0.f, si = 0.f;
+#pragma unroll
+      for (int k = 0; k < K; ++k) {
+        float4 gu, gi;
+        grads(k, gu, gi);
+        su += orx_sq4(gu);
+        si += orx_sq4(gi);
+      }
+      su = orx_group_sum<G>(su);
+      si = orx_group_sum<G>(si);
+      float ua = (fl & 2) ? __ldcg(a.Us0 + uu) : 0.f, ia = (fl & 4) ? __ldcg(a.Is0 + ii) : 0.f;
+      const float fu = orx_row_scale(ua, su, D, a.opt), fi = orx_row_scale(ia, si, D, a.opt);
+      if (v) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+          const int off = (k * G + gl) * 4;
+          float4 gu, gi;
+          grads(k, gu, gi);
+          if (GMF) {
+            gwacc[k].x += g * u[k].x * it[k].x; gwacc[k].y += g * u[k].y * it[k].y;
+            gwacc[k].z += g * u[k].z * it[k].z; gwacc[k].w += g * u[k].w * it[k].w;
+          }
+          orx_own_or_stage4_row<false>(fl & 2, a.U, uu, a.gu, duj, D, off, u[k], gu, fu, a.opt);
+          orx_own_or_stage4_row<false>(fl & 4, a.I, ii, a.gi, dij, D, off, it[k], gi, fi, a.opt);
+        }
+        if (gl == 0) {
+          if (fl & 2) __stcg(a.Us0 + uu, ua);
+          if (fl & 4) __stcg(a.Is0 + ii, ia);
+        }
+      }
+    } else if (v) {
       const float c2 = a.c_l2;
 #pragma unroll
       for (int k = 0; k < K; ++k) {
@@ -147,9 +187,9 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
   }
   if (flags & 1) {
     if (flags & 4) {
-      __stcg(a.Bv + i_id, orx_apply<OPT>(bi, g_own, bs0, bs1, a.opt));
-      if (SL::S0) __stcg(a.Bs0 + i_id, bs0);
-      if (SL::S1) __stcg(a.Bs1 + i_id, bs1);
+      __stcg(a.Bv + i_id, orx_apply<SL::ELEM>(bi, g_own, bs0, bs1, a.opt));
+      if (BL::S0) __stcg(a.Bs0 + i_id, bs0);
+      if (BL::S1) __stcg(a.Bs1 + i_id, bs1);
     } else {
       atomicAdd(a.gb + di, g_own);
     }
@@ -208,6 +248,36 @@ __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
       fi = !STAGE_ONLY && ci == 1u;
     }
     const float c2 = a.c_l2;
+    if constexpr (OrxOptSlots<OPT>::ROW) {   // MODE 0 only: each owned row's squared-gradient sum, then the apply
+      if (!ok) continue;   // warp-uniform
+      float su = 0.f, si = 0.f;
+      for (int d = lane; d < D; d += 32) {
+        const float u = ur[d], it = ir[d], w = GMF ? a.W[d] : 1.f;
+        const float gu = g * w * it + c2 * u, gi = g * w * u + c2 * it;
+        su += gu * gu;
+        si += gi * gi;
+      }
+      su = orx_group_sum<32>(su);
+      si = orx_group_sum<32>(si);
+      float ua = fu ? a.Us0[uu] : 0.f, ia = fi ? a.Is0[ii] : 0.f;
+      const float xu = orx_row_scale(ua, su, D, a.opt), xi = orx_row_scale(ia, si, D, a.opt);
+      for (int d = lane; d < D; d += 32) {
+        const float u = ur[d], it = ir[d], w = GMF ? a.W[d] : 1.f;
+        const float gu = g * w * it + c2 * u, gi = g * w * u + c2 * it;
+        if (GMF && a.gw) atomicAdd(a.gw + d, g * u * it);
+        if (fu) ur[d] = orx_row_apply1(u, gu, xu, a.opt);
+        else atomicAdd(a.gu + (int64_t)du * D + d, gu);
+        if (fi) ir[d] = orx_row_apply1(it, gi, xi, a.opt);
+        else atomicAdd(a.gi + (int64_t)di * D + d, gi);
+      }
+      if (lane == 0) {
+        if (fu) a.Us0[uu] = ua;
+        if (fi) a.Is0[ii] = ia;
+        if (fi) orx_update1<ORX_OPT_ADAGRAD>(a.Bv + ii, a.Bs0 + ii, nullptr, bi, g, a.opt);
+        else atomicAdd(a.gb + di, g);
+      }
+      continue;
+    } else {
     if (MODE == 0 ? ok : (a.d_user || a.d_item || a.gw)) {
       for (int d = lane; d < D; d += 32) {
         float gu = 0.f, gi = 0.f;
@@ -241,6 +311,7 @@ __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
         if (a.g_out) a.g_out[t] = g;
       }
     }
+    }
   }
   orx_warp_partial(loss_acc, l2_acc, a.partials);
 }
@@ -267,7 +338,9 @@ static int launch_point_kind_opt(const PointArgs& pa, cudaStream_t st, OrxStepLa
   const int blocks = orx_step_blocks(pa.B);
   *out = {8 * blocks, ORX_VARIANT_STEP, 0};
   // k_point_step moves table rows, slot rows and GMF's w as float4: a base off a 16-byte boundary takes k_point_generic
-  const bool vec = orx_aligned16(pa.U, pa.Us0, pa.Us1, pa.I, pa.Is0, pa.Is1, pa.W);
+  // (a row-wise accumulator is read as scalars and does not count)
+  const bool vec = OrxOptSlots<OPT>::ROW ? orx_aligned16(pa.U, pa.I, pa.W)
+                                         : orx_aligned16(pa.U, pa.Us0, pa.Us1, pa.I, pa.Is0, pa.Is1, pa.W);
   switch (vec ? pa.D : 0) {
     case 32: k_point_step<KIND, OPT, 32, 8><<<blocks, 256, 0, st>>>(pa); break;
     case 64: k_point_step<KIND, OPT, 64, 8><<<blocks, 256, 0, st>>>(pa); break;
@@ -305,6 +378,11 @@ extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_
   ORX_REQUIRE(kind == ORX_POINT_GMF || kind == ORX_POINT_WRMF, "unknown pointwise kind");
   ORX_REQUIRE(kind == ORX_POINT_WRMF || w, "GMF needs w with dim == D");
   const orx_table_t* dense_w = (kind == ORX_POINT_GMF) ? w : nullptr;
+  orx_opt_t od;
+  if (opt && user) {   // dim-1 rows under ROWWISE_ADAGRAD run (and are recorded) as ADAGRAD
+    od = orx_opt_dim(opt, user->dim);
+    opt = &od;
+  }
   ORX_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)s;
   const auto kernel = [&](const SparseArgs& sa, const int4* /*res: pairwise only*/, float* partials, OrxStepLaunch* out) {

@@ -91,8 +91,48 @@ extern "C" int orx_owner_bucket_combined(orx_handle_t h, const int32_t* ids, int
 // ---------------------------------------------------------------------------------------
 // generic sparse apply
 // ---------------------------------------------------------------------------------------
+// One warp's ROWWISE_ADAGRAD update of table row id from value row v (each element divided by nb): a row seen once in
+// the batch (own, warp-uniform) takes the sum of its squared gradient first -- lane-strided in order, then the xor tree
+// -- before its first store (a warp holds a row as lane * 4 ... e += 128, so D > 128 takes two passes over v); any other
+// row is added into its staging row d.  vec: var and the value rows move as float4 (s0[id] is one scalar).
+__device__ __forceinline__ void orx_apply_row_rowwise(bool vec, bool own, float* var, float* s0, int id, float* gstage,
+                                                      int d, int D, const float* v, float nb, const OrxOptDev& o) {
+  const int lane = threadIdx.x & 31;
+  auto val4 = [&](int e) {
+    const float4 g = __ldcg(reinterpret_cast<const float4*>(v + e));
+    return nb == 1.f ? g : make_float4(g.x / nb, g.y / nb, g.z / nb, g.w / nb);
+  };
+  auto val1 = [&](int e) { return nb == 1.f ? v[e] : v[e] / nb; };
+  if (!own) {
+    if (vec) {
+      for (int e = lane * 4; e < D; e += 128) orx_red4(gstage + (int64_t)d * D + e, val4(e));
+    } else {
+      for (int e = lane; e < D; e += 32) atomicAdd(gstage + (int64_t)d * D + e, val1(e));
+    }
+    return;
+  }
+  float ss = 0.f;
+  if (vec) {
+    for (int e = lane * 4; e < D; e += 128) ss += orx_sq4(val4(e));
+  } else {
+    for (int e = lane; e < D; e += 32) ss += val1(e) * val1(e);
+  }
+  ss = orx_group_sum<32>(ss);
+  float acc = s0[id];
+  const float f = orx_row_scale(acc, ss, D, o);
+  float* w = var + (int64_t)id * D;
+  if (vec) {
+    for (int e = lane * 4; e < D; e += 128)
+      __stcg(reinterpret_cast<float4*>(w + e), orx_row_apply4(__ldcg(reinterpret_cast<const float4*>(w + e)), val4(e), f, o));
+  } else {
+    for (int e = lane; e < D; e += 32) w[e] = orx_row_apply1(w[e], val1(e), f, o);
+  }
+  if (lane == 0) s0[id] = acc;
+}
+
 // VEC: var, s0 and s1 are 16-byte aligned (sparse_apply_impl decides); the row shape and the value rows are tested here,
-// so that the VEC instance compiles to what the kernel was before the table gate.
+// so that the VEC instance compiles to what the kernel was before the table gate.  Under ROWWISE_ADAGRAD only var is
+// (s0 is float[rows], read as scalars).
 template <int OPT, bool VEC>
 __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, float* s1, int64_t rows, int D,
                                                       const int32_t* __restrict__ ids, int64_t id_stride,
@@ -121,6 +161,11 @@ __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, flo
   if (id < 0) continue;
   const float* v = vals + (int64_t)b * val_ld;
   const bool own = !SL::STAGE_ONLY && c == 1u;
+  if constexpr (SL::ROW) {
+    orx_apply_row_rowwise(VEC && ((D & 3) == 0) && ((val_ld & 3) == 0) && (((uintptr_t)vals & 15) == 0), own, var, s0,
+                          id, gstage, d, D, v, 1.f, o);
+    continue;
+  } else
   // 128-bit path (value rows 16-byte aligned: a strided view may start mid-row): all loads of the row first, then the
   // math, then the stores
   if (VEC && ((D & 3) == 0) && ((val_ld & 3) == 0) && (((uintptr_t)vals & 15) == 0)) {
@@ -201,7 +246,10 @@ static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32
   ORX_REQUIRE(n == 0 || (ids && values), "null ids/values");
   const int D = tab->dim;
   if ((rc = orx_ensure_workspace(h, n > 0 ? n : 1, D))) return rc;
-  const bool vec = orx_aligned16(tab->var, tab->s0, tab->s1);   // a table may start anywhere (orx.h)
+  const orx_opt_t od = orx_opt_dim(opt, D);
+  opt = &od;
+  // a table may start anywhere (orx.h); a row-wise accumulator is read as scalars and does not count
+  const bool vec = od.kind == ORX_OPT_ROWWISE_ADAGRAD ? orx_aligned16(tab->var) : orx_aligned16(tab->var, tab->s0, tab->s1);
   return sparse_apply_run(h, tab, ids, id_stride, n, opt, st, [&](const OrxOptDev& o) {
     const int blocks = (n + 63) / 64;   // 8 warps x 8 pairs per block and iteration
     orx_dispatch_opt(opt->kind, [&](auto O) {
@@ -275,6 +323,10 @@ __global__ void __launch_bounds__(256) k_bag_apply(float* var, float* s0, float*
   if (id < 0) continue;
   const float* v = vals + (int64_t)(b / L) * val_ld;
   const bool own = !SL::STAGE_ONLY && c == 1u;
+  if constexpr (SL::ROW) {
+    orx_apply_row_rowwise(vec, own, var, s0, id, gstage, d, D, v, cnt ? nb : 1.f, o);
+    continue;
+  } else
   if (vec) {
     const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int e = lane * 4; e < D; e += 128) {
@@ -328,7 +380,10 @@ extern "C" int orx_bag_sparse_apply(orx_handle_t h, const orx_table_t* tab, cons
     k_bag_ids<<<blocks, 256, 0, st>>>(sparse, ld, col_lo, L, B, tab->rows, ids_c, cnt);
     ORX_LAUNCH_CHECK();
   }
-  const bool vec = orx_aligned16(tab->var, tab->s0, tab->s1);   // a table may start anywhere (orx.h)
+  const orx_opt_t od = orx_opt_dim(opt, D);
+  opt = &od;
+  // a table may start anywhere (orx.h); a row-wise accumulator is read as scalars and does not count
+  const bool vec = od.kind == ORX_OPT_ROWWISE_ADAGRAD ? orx_aligned16(tab->var) : orx_aligned16(tab->var, tab->s0, tab->s1);
   return sparse_apply_run(h, tab, ids_c, 1, n, opt, st, [&](const OrxOptDev& o) {
     const int blocks = (n + 63) / 64;
     orx_dispatch_opt(opt->kind, [&](auto O) {

@@ -10,14 +10,15 @@ import torch
 from . import _lib
 from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP,
                    ORX_OP_POINTWISE_GRAD_ROWS, ORX_OP_CENSOR_SHARD, ORX_VARIANT_CENSOR_SCALAR, ORX_VARIANT_CENSOR_VEC,
-                   ORX_OP_SCORE_RANK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_TOPK_SHARD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD, ORX_PAIR_BPR,
+                   ORX_OP_SCORE_RANK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_TOPK_SHARD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD,
+                   ORX_OPT_ROWWISE_ADAGRAD, ORX_PAIR_BPR,
                    ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
                    ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
                    ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE,
                    ORX_VARIANT_TOPK, OrxOpt, OrxTable)
 
 __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", "ORX_POINT_GMF", "ORX_POINT_WRMF",
-           "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_SCORE_DOT",
+           "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_OPT_ROWWISE_ADAGRAD", "ORX_SCORE_DOT",
            "ORX_SCORE_NEG_SQDIST", "ORX_OP_GEMM", "ORX_OP_INTERACT_FWD", "ORX_OP_INTERACT_BWD", "ORX_OP_PAIRWISE_STEP",
            "ORX_OP_POINTWISE_STEP", "ORX_VARIANT_GEMM_TMA", "ORX_VARIANT_GEMM_SIMT", "ORX_VARIANT_INTERACT_WARP",
            "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC",
@@ -69,10 +70,14 @@ def ids32(t):
     return t.contiguous().reshape(-1)
 
 
-def table(var, s0=None, s1=None):
-    """orx_table_t for a [rows, dim] variable and its optimizer slots."""
+def table(var, s0=None, s1=None, kind=None):
+    """orx_table_t for a [rows, dim] variable and its optimizer slots.  With kind=ORX_OPT_ROWWISE_ADAGRAD, s0 is the
+    table's one accumulator per row: ``[rows]`` or ``[rows, 1]``, anything else is refused."""
     _f32(var, "var"), _f32(s0, "s0"), _f32(s1, "s1")
     rows, dim = (var.shape[0], var.shape[1]) if var.dim() == 2 else (1, var.numel())
+    if kind == ORX_OPT_ROWWISE_ADAGRAD and s0 is not None and tuple(s0.shape) not in ((rows,), (rows, 1)):
+        raise ValueError(f"s0: a row-wise Adagrad accumulator has one element per row, shape ({rows},) or ({rows}, 1), "
+                         f"got {tuple(s0.shape)}")
     return OrxTable(var.data_ptr(), s0.data_ptr() if s0 is not None else None,
                     s1.data_ptr() if s1 is not None else None, rows, dim)
 

@@ -58,12 +58,21 @@ def load(path, model, optimizer=None, build=None):
             raise ValueError(f"checkpoint variable {k} is {names[k]!r}, the model's is {v.name!r}")
         if tuple(a.shape) != tuple(v.shape):
             raise ValueError(f"checkpoint variable {k} has shape {a.shape}, model expects {tuple(v.shape)}")
+    slots = []
+    if optimizer is not None and "iterations" in data.files:
+        # copy_ broadcasts: a row-wise [rows] accumulator would silently fill an element-wise [rows, dim] one
+        for k, v in enumerate(variables):
+            s = list(optimizer.slots(v))
+            for j in range(2):
+                key = f"slot{j}/{k}"
+                if key in data.files and s[j] is not None:
+                    if tuple(data[key].shape) != tuple(s[j].shape):
+                        raise ValueError(f"checkpoint slot {key} of {v.name!r} has shape {data[key].shape}, "
+                                         f"{type(optimizer).__name__} expects {tuple(s[j].shape)}")
+                    slots.append((s[j], data[key]))
     for k, v in enumerate(variables):
         v.assign(data[f"var/{k}"])
     if optimizer is not None and "iterations" in data.files:
         optimizer.iterations = int(data["iterations"])
-        for k, v in enumerate(variables):
-            s = list(optimizer.slots(v))
-            for j in range(2):
-                if f"slot{j}/{k}" in data.files and s[j] is not None:
-                    s[j].copy_(torch.from_numpy(data[f"slot{j}/{k}"]))
+        for s, a in slots:
+            s.copy_(torch.from_numpy(a))

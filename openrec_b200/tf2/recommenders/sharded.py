@@ -75,7 +75,7 @@ class _ShardedModel(Model):
         t = torch.empty(rows, cols, dtype=torch.float32, device=self._eng.device)
         self._eng.fill_uniform(t, -0.05, 0.05, seed)                 # LatentFactor's 'uniform' initializer
         v = Variable.__new__(Variable)
-        v.t, v.trainable, v.name = t, True, name
+        v.t, v.trainable, v.name, v.row_table = t, True, name, True   # a table shard
         return v
 
     def _orx_forward(self, node):
@@ -174,7 +174,8 @@ class ShardedBPR(_ShardedFactors):
         coef, _ = self._step_args(node, grads_and_vars, optimizer)
         kind = optimizer._kind
         if kind not in (N.ORX_OPT_SGD, N.ORX_OPT_ADAGRAD, N.ORX_OPT_ADAM_LAZY):
-            raise NotImplementedError("sharded tables: use SGD, Adagrad or LazyAdam (Keras Adam() sweeps whole tables)")
+            raise NotImplementedError("sharded BPR / UCML tables: use SGD, Adagrad or LazyAdam (Keras Adam() sweeps "
+                                      "whole tables; the home-routed step has no RowwiseAdagrad)")
         B = node.ids[0].numel()
         key = (id(optimizer), kind)
         if self._impl is None or self._impl_key != key or B > self._impl.B:

@@ -122,6 +122,7 @@ def convert(value, dtype=None, *, pin=True):
 
 class Variable:
     """tf.Variable: a named, trainable device tensor."""
+    row_table = False   # an embedding table (rows looked up by id): a row-wise optimizer keeps one slot entry per row
 
     def __init__(self, initial_value, trainable=True, name=None, dtype=None):
         t = convert(initial_value, dtype).t

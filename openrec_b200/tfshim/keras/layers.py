@@ -87,6 +87,7 @@ class Embedding(Layer):
             raise NotImplementedError(f"embeddings_initializer={embeddings_initializer!r}")
         self.embeddings = Variable.__new__(Variable)
         self.embeddings.t, self.embeddings.trainable, self.embeddings.name = t, True, f"{self.name}/embeddings"
+        self.embeddings.row_table = True
 
     def _own_variables(self):
         return [self.embeddings]

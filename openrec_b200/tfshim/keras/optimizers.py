@@ -4,7 +4,8 @@ liborx (fused into the recommender step when the whole gradient set of a step no
 [TF-mem] defaults: SGD lr=0.01; Adagrad lr=0.001, initial_accumulator_value=0.1, eps=1e-7;
 Adam lr=0.001, beta_1=0.9, beta_2=0.999, eps=1e-7.  Keras-2.0 Adam on IndexedSlices is NOT lazy:
 ``Adam()`` therefore maps to liborx's ADAM_DENSE mode (whole-table sweep, exact reference semantics);
-``LazyAdam`` (an addition, not in the reference) is the row-sparse variant.
+``LazyAdam`` (an addition, not in the reference) is the row-sparse variant.  ``RowwiseAdagrad`` (an addition too) keeps
+one Adagrad accumulator per embedding-table row, updated with the mean of the row's squared gradient.
 """
 from __future__ import annotations
 
@@ -119,3 +120,27 @@ class Adam(Optimizer):
 class LazyAdam(Adam):
     """Row-sparse Adam (moments of untouched rows are left alone).  NOT the reference's semantics."""
     _kind = N.ORX_OPT_ADAM_LAZY
+
+
+class RowwiseAdagrad(Adagrad):
+    """Row-wise Adagrad: one accumulator per embedding-table row, ``acc[r] += mean_j G[r, j]^2`` and
+    ``var[r] -= lr * G[r] / (sqrt(acc[r]) + eps)`` for the rows a step touches (G summed over the step's lookups of r).
+    Same per-row adaptivity as Adagrad for about SGD's memory traffic; its slot is 1/dim of Adagrad's.  NOT in the
+    reference.  Embedding tables (variables created with ``row_table = True``: Embedding / LatentFactor and the sharded
+    models' table shards) get a ``[rows]`` accumulator; every other variable (Dense kernels and biases, GMF's w) gets
+    element-wise Adagrad with an element-wise accumulator."""
+    _kind = N.ORX_OPT_ROWWISE_ADAGRAD
+
+    def __init__(self, learning_rate=0.001, initial_accumulator_value=0.1, epsilon=1e-7, name="RowwiseAdagrad",
+                 **kwargs):
+        super().__init__(learning_rate, initial_accumulator_value, epsilon, name, **kwargs)
+
+    def table(self, var: Variable):
+        s0, s1 = self.slots(var)
+        return N.table(var.t, s0, s1, kind=self._kind)   # checks that s0 holds one accumulator per row
+
+    def _init_slot(self, var, k):
+        if getattr(var, "row_table", False):
+            return torch.full((var.t.shape[0],), self.initial_accumulator_value, dtype=var.t.dtype,
+                              device=var.t.device)
+        return super()._init_slot(var, k)
