@@ -70,6 +70,12 @@ enum orx_score_kind { ORX_SCORE_DOT = 0, ORX_SCORE_NEG_SQDIST = 1 };
  *              dim-1 table (the item bias among them) updates exactly as ADAGRAD does.  Dense variables
  *              (orx_dense_apply's var, the pointwise step's GMF weight w) get element-wise ADAGRAD, s0 element-wise.
  *              orx_shard_step does not take it.
+ *   MOMENTUM   Keras SGD(momentum=beta1) on IndexedSlices (SparseApplyKerasMomentum), row-lazy like every kind here:
+ *              a[r] = beta1*a[r] - lr*G; var[r] += a[r]                   (s0 = a, [rows, dim], init 0)
+ *   NESTEROV   the same with nesterov=True: a[r] = beta1*a[r] - lr*G; var[r] += beta1*a[r] - lr*G
+ *              Both take lr as given, round each product, sum and difference to float32 (no fused multiply-add), and
+ *              run in every entry point that takes ADAGRAD, orx_shard_step included.  Dense variables get the same
+ *              formula element-wise.  Keras SGD with momentum 0 is plain SGD: pass ORX_OPT_SGD, with no slot.
  * For Adam s0 = m, s1 = v, lr_t = lr*sqrt(1-beta2^step)/(1-beta1^step), step is 1-based.  Adagrad and Adam use the
  * sqrt.approx / rcp.approx approximations. */
 enum orx_opt_kind {
@@ -77,8 +83,11 @@ enum orx_opt_kind {
   ORX_OPT_ADAGRAD = 1,
   ORX_OPT_ADAM_LAZY = 2,
   ORX_OPT_ADAM_DENSE = 3,
-  /* 4 is not assigned: every entry point refuses it as an unknown kind (ORX_ERR_INVALID), as it always has */
-  ORX_OPT_ROWWISE_ADAGRAD = 5
+  /* 4 and 7 are not assigned: every entry point refuses them as unknown kinds (ORX_ERR_INVALID), as it always has.
+   * Callers use both as the unknown kind that must be refused, so the momentum pair skips 7 rather than take it. */
+  ORX_OPT_ROWWISE_ADAGRAD = 5,
+  ORX_OPT_MOMENTUM = 6,
+  ORX_OPT_NESTEROV = 8
 };
 
 typedef struct {
@@ -91,7 +100,7 @@ typedef struct {
 typedef struct {
   float* var;   /* [rows, dim] */
   float* s0;    /* Adagrad accumulator [rows, dim] | Adam m [rows, dim] | row-wise Adagrad accumulator float[rows]
-                   (4-byte alignment is enough: it is read as scalars) ; NULL for SGD */
+                   (4-byte alignment is enough: it is read as scalars) | momentum a [rows, dim] ; NULL for SGD */
   float* s1;    /* Adam v ; NULL otherwise */
   int64_t rows;
   int32_t dim;

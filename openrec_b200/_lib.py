@@ -16,6 +16,7 @@ ORX_PAIR_BPR, ORX_PAIR_UCML = 0, 1
 ORX_POINT_GMF, ORX_POINT_WRMF = 0, 1
 ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST = 0, 1
 ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE, ORX_OPT_ROWWISE_ADAGRAD = 0, 1, 2, 3, 5   # 4: unassigned
+ORX_OPT_MOMENTUM, ORX_OPT_NESTEROV = 6, 8   # 7: unassigned
 ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP = 0, 1, 2, 3, 4
 ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK_SHARD = 5, 6, 7, 8
 ORX_OP_POINTWISE_GRAD_ROWS, ORX_OP_CENSOR_SHARD = 9, 10

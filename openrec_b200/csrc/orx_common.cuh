@@ -183,15 +183,18 @@ static inline auto orx_dispatch(int v, F&& f) {
     return orx_dispatch<Vs...>(v, f);
   }
 }
+// NESTEROV runs the MOMENTUM instances: orx_apply<MOMENTUM> picks the Nesterov form from OrxOptDev::kind, so every
+// kernel has one momentum instance, not two.
 template <typename F>
 static inline auto orx_dispatch_opt(int opt_kind, F&& f) {
-  return orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE, ORX_OPT_ROWWISE_ADAGRAD>(
-      opt_kind, f);
+  return orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE, ORX_OPT_ROWWISE_ADAGRAD,
+                      ORX_OPT_MOMENTUM>(opt_kind == ORX_OPT_NESTEROV ? ORX_OPT_MOMENTUM : opt_kind, f);
 }
 
-// an orx_opt_kind (4 is unassigned and refused: orx_dispatch_opt would otherwise run it as its last listed kind)
+// an orx_opt_kind (4 and 7 are unassigned and refused: orx_dispatch_opt would otherwise run them as its last listed kind)
 static inline bool orx_opt_kind_ok(int kind) {
-  return (kind >= ORX_OPT_SGD && kind <= ORX_OPT_ADAM_DENSE) || kind == ORX_OPT_ROWWISE_ADAGRAD;
+  return (kind >= ORX_OPT_SGD && kind <= ORX_OPT_ADAM_DENSE) || kind == ORX_OPT_ROWWISE_ADAGRAD ||
+         kind == ORX_OPT_MOMENTUM || kind == ORX_OPT_NESTEROV;
 }
 // The optimizer *o as a table of row width dim runs it: a dim-1 table under ROWWISE_ADAGRAD runs ADAGRAD (its one
 // accumulator per row is the element-wise one, and the update then rounds exactly as ADAGRAD's).
@@ -225,8 +228,8 @@ static inline int orx_grid_for(int64_t n, int threads, int num_sms) {
 // ---------------------------------------------------------------------------------------
 struct OrxOptDev {
   int32_t kind;
-  float lr;    // SGD/Adagrad: lr ; Adam: bias-corrected lr_t
-  float eps, beta1, beta2;
+  float lr;    // SGD/Adagrad/momentum: lr ; Adam: bias-corrected lr_t
+  float eps, beta1, beta2;   // MOMENTUM / NESTEROV: beta1 = the momentum coefficient
 };
 
 #ifdef __CUDACC__
@@ -397,14 +400,14 @@ __device__ __forceinline__ float orx_rcp_fast(float x) {
   return r;
 }
 
-// Which optimizer-slot rows an update reads and writes: S0 = Adagrad accumulator / Adam m, S1 = Adam v, both one
-// element per table element.  STAGE_ONLY: ADAM_DENSE updates no row in a step kernel; every row is staged and the sweep
+// Which optimizer-slot rows an update reads and writes: S0 = Adagrad accumulator / Adam m / momentum a, S1 = Adam v,
+// both one element per table element.  STAGE_ONLY: ADAM_DENSE updates no row in a step kernel; every row is staged and the sweep
 // (k_adam_sweep) applies Adam to the table.  ROW: ROWWISE_ADAGRAD keeps S0 as one scalar per row (s0[id]) and no S1;
 // a row's update needs the sum of its squared gradient first (orx_row_scale).  ELEM: the optimizer of the dim-1 and
 // dense variables a kernel updates beside its rows (the item bias, GMF's w): element-wise ADAGRAD for ROW.
 template <int OPT>
 struct OrxOptSlots {
-  static constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY);
+  static constexpr bool S0 = (OPT == ORX_OPT_ADAGRAD || OPT == ORX_OPT_ADAM_LAZY || OPT == ORX_OPT_MOMENTUM);
   static constexpr bool S1 = (OPT == ORX_OPT_ADAM_LAZY);
   static constexpr bool STAGE_ONLY = (OPT == ORX_OPT_ADAM_DENSE);
   static constexpr bool ROW = (OPT == ORX_OPT_ROWWISE_ADAGRAD);
@@ -428,6 +431,9 @@ __device__ __forceinline__ float orx_row_apply1(float w, float g, float f, const
 
 // One optimizer update of one scalar.  OPT is an orx_opt_kind (ADAM_DENSE never reaches here:
 // its rows are staged and swept).
+// MOMENTUM serves NESTEROV too, told apart by o.kind (a kernel parameter: uniform over the grid).  Its products, sum
+// and differences are rounded one by one, in the order of SparseApplyKerasMomentum, so that no path contracts them
+// into a fused multiply-add of its own choosing: every kernel rounds a row's update alike.
 template <int OPT>
 __device__ __forceinline__ float orx_apply(float w, float g, float& s0, float& s1, const OrxOptDev& o) {
   static_assert(OPT != ORX_OPT_ROWWISE_ADAGRAD, "a row-wise row is updated through orx_row_scale");
@@ -436,6 +442,10 @@ __device__ __forceinline__ float orx_apply(float w, float g, float& s0, float& s
   } else if (OPT == ORX_OPT_ADAGRAD) {
     s0 = s0 + g * g;
     return w - o.lr * g * orx_rcp_fast(orx_sqrt_fast(s0) + o.eps);
+  } else if (OPT == ORX_OPT_MOMENTUM) {
+    const float lg = __fmul_rn(o.lr, g);
+    s0 = __fsub_rn(__fmul_rn(o.beta1, s0), lg);
+    return __fadd_rn(w, o.kind == ORX_OPT_NESTEROV ? __fsub_rn(__fmul_rn(o.beta1, s0), lg) : s0);
   } else {
     s0 = o.beta1 * s0 + (1.f - o.beta1) * g;
     s1 = o.beta2 * s1 + (1.f - o.beta2) * g * g;

@@ -254,7 +254,8 @@ extern "C" int orx_stream_synchronize(orx_handle_t h, orx_stream_t s) {
 }
 
 bool orx_opt_slots_ok(int kind, std::initializer_list<const orx_table_t*> tabs) {
-  // ROWWISE_ADAGRAD needs s0 (float[rows]: its length is the caller's, as for every slot row) and no s1
+  // ROWWISE_ADAGRAD needs s0 (float[rows]: its length is the caller's, as for every slot row) and no s1; MOMENTUM and
+  // NESTEROV need s0 (a) and no s1
   const bool s0 = kind != ORX_OPT_SGD, s1 = kind == ORX_OPT_ADAM_LAZY || kind == ORX_OPT_ADAM_DENSE;
   for (const orx_table_t* t : tabs)
     if (t && ((s0 && !t->s0) || (s1 && !t->s1))) return false;
@@ -268,7 +269,7 @@ OrxOptDev orx_opt_to_dev(const orx_opt_t* o) {
   d.eps = o->eps;
   d.beta1 = o->beta1;
   d.beta2 = o->beta2;
-  // SGD, ADAGRAD and ROWWISE_ADAGRAD take lr as given
+  // SGD, ADAGRAD, ROWWISE_ADAGRAD, MOMENTUM and NESTEROV take lr as given
   if (o->kind == ORX_OPT_ADAM_LAZY || o->kind == ORX_OPT_ADAM_DENSE) {
     // lr_t = lr*sqrt(1-b2^t)/(1-b1^t), evaluated in double like the oracle's adam_lr_t
     double t = (double)(o->step < 1 ? 1 : o->step);

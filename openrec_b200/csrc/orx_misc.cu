@@ -283,10 +283,11 @@ extern "C" int orx_dense_apply(orx_handle_t h, float* var, float* s0, float* s1,
   const orx_table_t t = {var, s0, s1, n, 1};
   ORX_REQUIRE(orx_opt_slots_ok(opt->kind, {&t}), "optimizer slot rows missing");
   // ADAM_DENSE runs as ADAM_LAZY: identical on a dense variable; ROWWISE_ADAGRAD as ADAGRAD: a dense variable keeps an
-  // element-wise accumulator (orx.h)
+  // element-wise accumulator (orx.h); NESTEROV as MOMENTUM, which reads the form from o.kind
   const int kind = opt->kind == ORX_OPT_ADAM_DENSE ? ORX_OPT_ADAM_LAZY
-                   : opt->kind == ORX_OPT_ROWWISE_ADAGRAD ? ORX_OPT_ADAGRAD : opt->kind;
-  orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY>(kind, [&](auto O) {
+                   : opt->kind == ORX_OPT_ROWWISE_ADAGRAD ? ORX_OPT_ADAGRAD
+                   : opt->kind == ORX_OPT_NESTEROV ? ORX_OPT_MOMENTUM : opt->kind;
+  orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_MOMENTUM>(kind, [&](auto O) {
     k_dense_apply<decltype(O)::value><<<(int)blocks, 256, 0, st>>>(var, s0, s1, grad, n, o);
   });
   ORX_LAUNCH_CHECK();

@@ -650,6 +650,10 @@ static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, OrxSte
     *out = {n_partials, variant, minb};
     orx_launch_pdl(kern, dim3(blocks), dim3(256), 0, st, pa);
   };
+  // MOMENTUM (NESTEROV too) keeps ADAGRAD's slot rows, but under -Xptxas -v ADAGRAD's D = 128 bound (four CTAs/SM,
+  // 64 registers) spills it, and so does PIPE at D = 256 (as it spills ADAGRAD).
+  // It therefore takes PIPE at D = 32 and 64, three CTAs/SM at D = 128 and one register buffer at D = 256: no spills.
+  constexpr bool MOM = (OPT == ORX_OPT_MOMENTUM);
   constexpr int PV = LAZY ? ORX_VARIANT_STEP : ORX_VARIANT_STEP_PIPE;
   // k_pair_step moves table and slot rows as float4: a table or slot base off a 16-byte boundary takes k_pair_generic.
   // ROWWISE_ADAGRAD reads its accumulators as scalars, so only the tables decide; it holds three accumulator scalars
@@ -661,10 +665,13 @@ static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, OrxSte
     case 32: go(k_pair_step<KIND, OPT, 32, 8, 2, !LAZY>, PV, 2, blocks); break;
     case 64: go(k_pair_step<KIND, OPT, 64, 8, 2, !LAZY>, PV, 2, blocks); break;
     case 128:
-      if constexpr (LAZY) go(k_pair_step<KIND, OPT, 128, 8, 3, false>, ORX_VARIANT_STEP, 3, blocks);
+      if constexpr (LAZY || MOM) go(k_pair_step<KIND, OPT, 128, 8, 3, false>, ORX_VARIANT_STEP, 3, blocks);
       else go(k_pair_step<KIND, OPT, 128, 8, 4, false>, ORX_VARIANT_STEP, 4, blocks);
       break;
-    case 256: go(k_pair_step<KIND, OPT, 256, 8, 2, !LAZY>, PV, 2, blocks); break;
+    case 256:
+      if constexpr (MOM) go(k_pair_step<KIND, OPT, 256, 8, 2, false>, ORX_VARIANT_STEP, 2, blocks);
+      else go(k_pair_step<KIND, OPT, 256, 8, 2, !LAZY>, PV, 2, blocks);
+      break;
     default: go(k_pair_generic<KIND, OPT, 0>, ORX_VARIANT_STEP_GENERIC, 0, 8 * blocks); break;
   }
   ORX_LAUNCH_CHECK();

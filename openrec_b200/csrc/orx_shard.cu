@@ -879,11 +879,13 @@ extern "C" int orx_shard_sizes(const orx_shard_t* xs, int64_t* n8_host) {
   return ORX_OK;
 }
 
-// runtime -> template arguments of the sharded kernels: the optimizers the sharded step supports (it rejects ADAM_DENSE)
-// and the row-width classes NQ (float4 per lane: D <= 128, 256, 512)
+// runtime -> template arguments of the sharded kernels: the optimizers the sharded step supports (it rejects ADAM_DENSE
+// and ROWWISE_ADAGRAD; NESTEROV runs the MOMENTUM instances, as in orx_dispatch_opt) and the row-width classes NQ
+// (float4 per lane: D <= 128, 256, 512)
 template <typename F>
 static inline auto sh_dispatch_opt(int opt_kind, F&& f) {
-  return orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY>(opt_kind, f);
+  return orx_dispatch<ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_MOMENTUM>(
+      opt_kind == ORX_OPT_NESTEROV ? ORX_OPT_MOMENTUM : opt_kind, f);
 }
 template <typename F>
 static inline auto sh_dispatch_nq(int nq, F&& f) {
@@ -918,8 +920,9 @@ extern "C" int orx_shard_step(orx_handle_t h, int32_t kind, const orx_shard_t* x
   if (announce) ORX_REQUIRE(next_B > 0 && next_B <= x->batch_cap, "bad announced batch");
   ORX_REQUIRE(total_users > 0 && total_items > 0 && epoch > 0 && epoch < 0x7ffffffe, "bad totals / epoch");
   ORX_REQUIRE(phase_lo >= 0 && phase_hi <= 5 && phase_lo <= phase_hi, "bad phase range");
-  ORX_REQUIRE(opt->kind == ORX_OPT_SGD || opt->kind == ORX_OPT_ADAGRAD || opt->kind == ORX_OPT_ADAM_LAZY,
-              "the sharded step supports SGD, Adagrad and row-sparse Adam");
+  ORX_REQUIRE(opt->kind == ORX_OPT_SGD || opt->kind == ORX_OPT_ADAGRAD || opt->kind == ORX_OPT_ADAM_LAZY ||
+                  opt->kind == ORX_OPT_MOMENTUM || opt->kind == ORX_OPT_NESTEROV,
+              "the sharded step supports SGD, Adagrad and row-sparse Adam, and SGD with (Nesterov) momentum");
   ORX_REQUIRE(orx_opt_slots_ok(opt->kind, {user, item, item_bias}), "optimizer slot rows missing");
   {   // every launch moves local table and slot rows as float4 and there is no scalar form: refuse a misaligned base
     const struct { const float* p; const char* name; } bases[6] = {

@@ -11,14 +11,15 @@ from . import _lib
 from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP,
                    ORX_OP_POINTWISE_GRAD_ROWS, ORX_OP_CENSOR_SHARD, ORX_VARIANT_CENSOR_SCALAR, ORX_VARIANT_CENSOR_VEC,
                    ORX_OP_SCORE_RANK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_TOPK_SHARD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_DENSE, ORX_OPT_ADAM_LAZY, ORX_OPT_SGD,
-                   ORX_OPT_ROWWISE_ADAGRAD, ORX_PAIR_BPR,
+                   ORX_OPT_ROWWISE_ADAGRAD, ORX_OPT_MOMENTUM, ORX_OPT_NESTEROV, ORX_PAIR_BPR,
                    ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
                    ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
                    ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE,
                    ORX_VARIANT_TOPK, OrxOpt, OrxTable)
 
 __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", "ORX_POINT_GMF", "ORX_POINT_WRMF",
-           "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_OPT_ROWWISE_ADAGRAD", "ORX_SCORE_DOT",
+           "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_OPT_ROWWISE_ADAGRAD",
+           "ORX_OPT_MOMENTUM", "ORX_OPT_NESTEROV", "ORX_SCORE_DOT",
            "ORX_SCORE_NEG_SQDIST", "ORX_OP_GEMM", "ORX_OP_INTERACT_FWD", "ORX_OP_INTERACT_BWD", "ORX_OP_PAIRWISE_STEP",
            "ORX_OP_POINTWISE_STEP", "ORX_VARIANT_GEMM_TMA", "ORX_VARIANT_GEMM_SIMT", "ORX_VARIANT_INTERACT_WARP",
            "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC",
@@ -83,6 +84,7 @@ def table(var, s0=None, s1=None, kind=None):
 
 
 def opt(kind, lr, eps=1e-7, beta1=0.9, beta2=0.999, step=1):
+    """orx_opt_t.  Under ORX_OPT_MOMENTUM / ORX_OPT_NESTEROV, beta1 is the momentum coefficient."""
     return OrxOpt(kind, lr, eps, beta1, beta2, step)
 
 

@@ -84,7 +84,7 @@ class ShardedPairwise:
             self.table[:, :dim + 1] = tmp
             self.table[:self.ru, dim] = 0.0                      # users have no bias column
             del tmp
-        n_slots = {0: 0, 1: 1, 2: 2, 3: 2}[opt_kind]
+        n_slots = {0: 0, 1: 1, 2: 2, 3: 2, 6: 1, 8: 1}[opt_kind]     # 6 / 8: momentum, beta1 = its coefficient
         fill = 0.1 if opt_kind == 1 else 0.0
         self.slots = [torch.full_like(self.table, fill) for _ in range(n_slots)] + [None] * (2 - n_slots)
         self.launches_per_step = 3 + 1 + 2 + 3   # bucket(3) gather(1) grad+reduce(2) sparse_apply(3)
@@ -680,8 +680,9 @@ class HomeRoutedPairwise:
                  peers=None, tables=None, slots=None):
         if dim % 4 or dim > 512:
             raise ValueError("the sharded step needs dim % 4 == 0 and dim <= 512")
-        if opt_kind not in (0, 1, 2):
-            raise ValueError("the sharded step supports SGD, Adagrad and row-sparse Adam")
+        if opt_kind not in (0, 1, 2, 6, 8):
+            raise ValueError("the sharded step supports SGD, Adagrad and row-sparse Adam, and SGD with (Nesterov) "
+                             "momentum")
         self.eng, self.rank, self.world = eng, rank, world
         self.U, self.I, self.D, self.B = total_users, total_items, dim, batch
         self.kind, self.opt_kind, self.lr, self.eps, self.b1, self.b2, self.margin = kind, opt_kind, lr, eps, beta1, beta2, margin
@@ -700,7 +701,7 @@ class HomeRoutedPairwise:
             if init:
                 for k, t in enumerate((self.user, self.item, self.bias)):
                     eng.fill_uniform(t, -0.05, 0.05, seed * 1000003 + rank * 17 + k)
-        n_slots = {0: 0, 1: 1, 2: 2}[opt_kind]
+        n_slots = {0: 0, 1: 1, 2: 2, 6: 1, 8: 1}[opt_kind]           # 6 / 8: momentum, beta1 = its coefficient
         fill = 0.1 if opt_kind == 1 else 0.0
         mk = lambda t: [torch.full_like(t, fill) for _ in range(n_slots)] + [None] * (2 - n_slots)
         if slots is not None:           # optimizer slots owned by the caller (the keras optimizer's slot tensors)

@@ -173,9 +173,10 @@ class ShardedBPR(_ShardedFactors):
     def _orx_apply(self, node, grads_and_vars, optimizer):
         coef, _ = self._step_args(node, grads_and_vars, optimizer)
         kind = optimizer._kind
-        if kind not in (N.ORX_OPT_SGD, N.ORX_OPT_ADAGRAD, N.ORX_OPT_ADAM_LAZY):
-            raise NotImplementedError("sharded BPR / UCML tables: use SGD, Adagrad or LazyAdam (Keras Adam() sweeps "
-                                      "whole tables; the home-routed step has no RowwiseAdagrad)")
+        if kind not in (N.ORX_OPT_SGD, N.ORX_OPT_ADAGRAD, N.ORX_OPT_ADAM_LAZY, N.ORX_OPT_MOMENTUM, N.ORX_OPT_NESTEROV):
+            raise NotImplementedError("sharded BPR / UCML tables: use SGD (with or without momentum), Adagrad or "
+                                      "LazyAdam (Keras Adam() sweeps whole tables; the home-routed step has no "
+                                      "RowwiseAdagrad)")
         B = node.ids[0].numel()
         key = (id(optimizer), kind)
         if self._impl is None or self._impl_key != key or B > self._impl.B:

@@ -1,7 +1,7 @@
 """tf.keras.optimizers.{SGD, Adagrad, Adam} with Keras OptimizerV2 sparse semantics, executed by
 liborx (fused into the recommender step when the whole gradient set of a step node is applied).
 
-[TF-mem] defaults: SGD lr=0.01; Adagrad lr=0.001, initial_accumulator_value=0.1, eps=1e-7;
+[TF-mem] defaults: SGD lr=0.01, momentum=0.0, nesterov=False; Adagrad lr=0.001, initial_accumulator_value=0.1, eps=1e-7;
 Adam lr=0.001, beta_1=0.9, beta_2=0.999, eps=1e-7.  Keras-2.0 Adam on IndexedSlices is NOT lazy:
 ``Adam()`` therefore maps to liborx's ADAM_DENSE mode (whole-table sweep, exact reference semantics);
 ``LazyAdam`` (an addition, not in the reference) is the row-sparse variant.  ``RowwiseAdagrad`` (an addition too) keeps
@@ -83,13 +83,27 @@ class Optimizer:
 
 
 class SGD(Optimizer):
+    """Keras SGD.  With ``momentum > 0`` each touched row r keeps a velocity a (slot 0, zero-initialised):
+    ``a[r] = momentum * a[r] - lr * G[r]``, then ``var[r] += a[r]``, or with ``nesterov=True``
+    ``var[r] += momentum * a[r] - lr * G[r]``.  Rows a step does not touch keep their value and velocity, as Keras
+    momentum on IndexedSlices does.  ``momentum == 0`` is plain SGD with no slot, whatever ``nesterov`` says."""
     _kind = N.ORX_OPT_SGD
     _n_slots = 0
 
     def __init__(self, learning_rate=0.01, momentum=0.0, nesterov=False, name="SGD", **kwargs):
-        if momentum or nesterov:
-            raise NotImplementedError("SGD momentum is not on the openrec.tf2 path")
         super().__init__(learning_rate, name, **kwargs)
+        momentum = float(momentum)
+        if not 0.0 <= momentum <= 1.0:
+            raise ValueError("`momentum` must be between [0, 1].")
+        self.momentum, self.nesterov = momentum, bool(nesterov)
+        # every path that builds an orx_opt_t passes beta_1: it carries the momentum, never the base class's 0.9
+        self.beta_1 = momentum
+        if momentum > 0.0:
+            self._kind = N.ORX_OPT_NESTEROV if self.nesterov else N.ORX_OPT_MOMENTUM
+            self._n_slots = 1
+
+    def get_config(self):
+        return {**super().get_config(), "momentum": self.momentum, "nesterov": self.nesterov}
 
 
 class Adagrad(Optimizer):
