@@ -118,7 +118,7 @@ ORX_API int orx_stream_synchronize(orx_handle_t h, orx_stream_t stream);
  * dedup hash and, once it has run, of orx_shard_step's own index sets (31 bits; each table takes its next epoch at its next build, and the one whose epoch
  * wraps is emptied on the stream of that build). */
 ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
-/* Test hook: the kernel variants launched by this handle's DLRM entry points (orx_mlp_layer_*, orx_interact_*) and
+/* Test hook: the kernel variants launched by this handle's DLRM entry points (orx_mlp_layer_*, orx_interact_*, orx_cross_*) and
  * sparse steps (orx_pairwise_step, orx_pairwise_step_host, orx_pointwise_step) since the last call, oldest first, at
  * most cap of them (a ring of the last ORX_DISPATCH_LOG_CAP), then clears them.
  * Record k is rec_host[8k .. 8k+7] = {op, variant, TA, TB, M, N, K, S}: a GEMM C[M,N] = op(A)[M,K] op(B)[K,N] with the
@@ -146,8 +146,11 @@ enum orx_dispatch_op {
   ORX_OP_POINTWISE_GRAD_ROWS = 9, /* orx_pointwise_grad_rows: variant STEP (k_pgr_step, specialised on D) or
                                     STEP_GENERIC (k_pgr_generic), TA = orx_point_kind, TB = 0, M = B, N = dim, K = ld,
                                     S = 1 */
-  ORX_OP_CENSOR_SHARD = 10 /* orx_censor_shard, one per call: variant CENSOR_VEC / CENSOR_SCALAR, TA = rank, TB = 0,
-                              M = total ids (n_per_block * n_blocks), N = local_rows, K = dim, S = world */
+  ORX_OP_CENSOR_SHARD = 10, /* orx_censor_shard, one per call: variant CENSOR_VEC / CENSOR_SCALAR, TA = rank, TB = 0,
+                               M = total ids (n_per_block * n_blocks), N = local_rows, K = dim, S = world */
+  ORX_OP_CROSS = 11 /* orx_cross_fwd / orx_cross_bwd, one per call with B > 0: variant CROSS_VEC / CROSS_SCALAR,
+                       TA = 0 forward / 1 backward, TB = orx_cross_mode (0 forward), M = B, N = W,
+                       K = split (ORX_CROSS_FINAL, else 0), S = 1 */
 };
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
@@ -163,8 +166,10 @@ enum orx_dispatch_variant {
   ORX_VARIANT_TOPK = 9,          /* k_score_topk + k_topk_merge: candidate lists in the handle's global scratch */
   ORX_VARIANT_CENSOR_VEC = 10,   /* k_censor_shard, one float4 per lane (dim % 4 == 0 && dim <= 128, tab 16-byte
                                     aligned) */
-  ORX_VARIANT_CENSOR_SCALAR = 11 /* k_censor_shard, lane-strided scalar rows (any other dim, or tab off a 16-byte
-                                    boundary) */
+  ORX_VARIANT_CENSOR_SCALAR = 11, /* k_censor_shard, lane-strided scalar rows (any other dim, or tab off a 16-byte
+                                     boundary) */
+  ORX_VARIANT_CROSS_VEC = 12,     /* k_cross_fwd / k_cross_bwd, one float4 per thread */
+  ORX_VARIANT_CROSS_SCALAR = 13   /* k_cross_fwd / k_cross_bwd, one float per thread (any W, any 4-byte-aligned base) */
 };
 #define ORX_DISPATCH_LOG_CAP 64
 ORX_API int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec_host, int32_t cap, int32_t* n_host);
@@ -503,6 +508,29 @@ ORX_API int orx_interact_bwd(orx_handle_t h, const float* emb, int64_t emb_ld, c
                              int64_t ddense_ld, orx_stream_t s);
 ORX_API int orx_pred_loss(orx_handle_t h, const float* pred, const float* label, int32_t B, int32_t kind,
                           float clip_threshold, float* pred_out, float* dpred, float* out4, orx_stream_t s);
+/* DCN-v2 cross network (arch_interaction_op = "cross"; Wang et al. 2021, tfrs.layers.dcn.Cross): x0 [B, W] is the cross
+ * input, layer l computes y_l = U_l (V_l^T x_l) + b_l (or K_l x_l + b_l at full rank) with orx_mlp_layer_fwd and
+ * x_{l+1} = x0 * y_l + x_l with orx_cross_fwd.  The backward walks the layers top first with G = dL/dx_{l+1}:
+ *   orx_cross_bwd(ORX_CROSS_TOP)   (layer L-1)  dy = G * x0, A = G * y                      (P not read, G not written)
+ *   orx_cross_bwd(ORX_CROSS_MID)   (layer l)    G <- G + P_{l+1}, dy = G * x0, A <- A + G * y
+ *   orx_cross_bwd(ORX_CROSS_FINAL)              dL/dx0 = G + P_0 + A: columns [0, split) to dx_lo, [split, W) to dx_hi
+ * where dy = dL/dy_l feeds orx_mlp_layer_bwd of U_l and V_l, whose dx is P_l = dL/dx_l through the projection.  G and
+ * A are updated in place.  All operands are row-major with explicit leading dimensions (>= their widths); each element
+ * is rounded once per operation (products and a * b + c as one fused multiply-add), no atomics: the same inputs give
+ * the same bits.  float4 accesses when W, every leading dimension the mode uses, split (FINAL) and every base it
+ * touches allow them, a scalar path for any W >= 1.  One dispatch record per call (ORX_OP_CROSS).
+ *   orx_cross_fwd: out = x0 * y + xl (out may not alias the inputs).
+ *   orx_cross_bwd: TOP reads G, x0, y and writes dy, A; MID reads G, P, x0, y, A and writes G, dy, A; FINAL reads G, P, A
+ *   and writes dx_lo / dx_hi (dx_hi at column 0 of its rows); arguments a mode does not use may be null.
+ * ORX_ERR_INVALID before any device work: a null handle or a null operand the mode uses, B < 0, W < 1, a leading
+ * dimension below its width, an unknown mode, split outside [0, W].  B = 0 is a no-op. */
+enum orx_cross_mode { ORX_CROSS_TOP = 0, ORX_CROSS_MID = 1, ORX_CROSS_FINAL = 2 };
+ORX_API int orx_cross_fwd(orx_handle_t h, const float* x0, int64_t ld_x0, const float* xl, int64_t ld_xl, const float* y,
+                          int64_t ld_y, int32_t B, int32_t W, float* out, int64_t ld_out, orx_stream_t s);
+ORX_API int orx_cross_bwd(orx_handle_t h, int32_t mode, int32_t B, int32_t W, float* G, int64_t ld_G, const float* P,
+                          int64_t ld_P, const float* x0, int64_t ld_x0, const float* y, int64_t ld_y, float* A,
+                          int64_t ld_A, float* dy, int64_t ld_dy, int32_t split, float* dx_lo, int64_t ld_lo,
+                          float* dx_hi, int64_t ld_hi, orx_stream_t s);
 
 /* ---- inference: full-catalogue scoring (bpr.py:39-43, wrmf.py:36-40, ucml.py:50-53, gmf.py:36-41)
  * scores[Bu, I] = user_rows . item^T + bias   (DOT; GMF passes user_rows pre-multiplied by w via `scale`)

@@ -19,11 +19,13 @@ ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE, ORX_OPT_ROW
 ORX_OPT_MOMENTUM, ORX_OPT_NESTEROV = 6, 8   # 7: unassigned
 ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP = 0, 1, 2, 3, 4
 ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK_SHARD = 5, 6, 7, 8
-ORX_OP_POINTWISE_GRAD_ROWS, ORX_OP_CENSOR_SHARD = 9, 10
+ORX_OP_POINTWISE_GRAD_ROWS, ORX_OP_CENSOR_SHARD, ORX_OP_CROSS = 9, 10, 11
 ORX_VARIANT_GEMM_TMA, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_INTERACT = 0, 1, 2, 3
 ORX_VARIANT_STEP, ORX_VARIANT_STEP_PIPE, ORX_VARIANT_STEP_GENERIC = 4, 5, 6
 ORX_VARIANT_RANK_SMEM, ORX_VARIANT_RANK_GLOBAL, ORX_VARIANT_TOPK = 7, 8, 9
 ORX_VARIANT_CENSOR_VEC, ORX_VARIANT_CENSOR_SCALAR = 10, 11
+ORX_VARIANT_CROSS_VEC, ORX_VARIANT_CROSS_SCALAR = 12, 13
+ORX_CROSS_TOP, ORX_CROSS_MID, ORX_CROSS_FINAL = 0, 1, 2
 ORX_CENSOR_SHARD_MAX_IDS = 1 << 28
 ORX_MAX_AT = 8
 ORX_BAG_MAX_TABLES = 63
@@ -98,6 +100,9 @@ SIGNATURES = {
     "orx_interact_bwd": [_vp, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64,
                          _vp],
     "orx_pred_loss": [_vp, _vp, _vp, _i32, _i32, _f, _vp, _vp, _vp, _vp],
+    "orx_cross_fwd": [_vp, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp, _i64, _vp],
+    "orx_cross_bwd": [_vp, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _vp,
+                      _i64, _vp, _i64, _vp],
     "orx_peer_alloc": [_vp, _i64, C.POINTER(_vp), C.c_char_p],
     "orx_peer_open": [_vp, C.c_char_p, C.POINTER(_vp)],
     "orx_peer_close": [_vp, _vp],

@@ -15,7 +15,8 @@ from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP
                    ORX_PAIR_UCML, ORX_POINT_GMF, ORX_POINT_WRMF, ORX_SCORE_DOT, ORX_SCORE_NEG_SQDIST, ORX_VARIANT_GEMM_SIMT,
                    ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
                    ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE,
-                   ORX_VARIANT_TOPK, OrxOpt, OrxTable)
+                   ORX_VARIANT_TOPK, ORX_OP_CROSS, ORX_VARIANT_CROSS_VEC, ORX_VARIANT_CROSS_SCALAR, ORX_CROSS_TOP,
+                   ORX_CROSS_MID, ORX_CROSS_FINAL, OrxOpt, OrxTable)
 
 __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", "ORX_POINT_GMF", "ORX_POINT_WRMF",
            "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_OPT_ROWWISE_ADAGRAD",
@@ -25,8 +26,9 @@ __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", 
            "ORX_VARIANT_INTERACT", "ORX_VARIANT_STEP", "ORX_VARIANT_STEP_PIPE", "ORX_VARIANT_STEP_GENERIC",
            "ORX_OP_SCORE_RANK", "ORX_VARIANT_RANK_SMEM", "ORX_VARIANT_RANK_GLOBAL", "ORX_OP_SCORE_TOPK",
            "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "ORX_OP_SCORE_TOPK_SHARD", "ORX_OP_POINTWISE_GRAD_ROWS",
-           "ORX_OP_CENSOR_SHARD", "ORX_VARIANT_CENSOR_VEC", "ORX_VARIANT_CENSOR_SCALAR", "Dispatch", "RowShard", "rowshard",
-           "shard_rows"]
+           "ORX_OP_CENSOR_SHARD", "ORX_VARIANT_CENSOR_VEC", "ORX_VARIANT_CENSOR_SCALAR", "ORX_OP_CROSS",
+           "ORX_VARIANT_CROSS_VEC", "ORX_VARIANT_CROSS_SCALAR", "ORX_CROSS_TOP", "ORX_CROSS_MID", "ORX_CROSS_FINAL",
+           "Dispatch", "RowShard", "rowshard", "shard_rows"]
 
 _engines = {}
 
@@ -308,6 +310,23 @@ class Engine:
                                              _ptr(dout2d), self._ld(dout2d), B, Fm1 + 1, D, int(self_interaction),
                                              mode, _ptr(demb3d), Fm1 * D, _ptr(ddense2d), self._ld(ddense2d),
                                              self.stream()), "orx_interact_bwd")
+
+    def cross_fwd(self, x0, xl, y, out):
+        """out = x0 * y + xl (orx_cross_fwd): [B, W] views with unit inner stride, any row stride."""
+        B, W = x0.shape
+        _lib.check(self.lib.orx_cross_fwd(self.h, _ptr(x0), self._ld(x0), _ptr(xl), self._ld(xl), _ptr(y), self._ld(y),
+                                          B, W, _ptr(out), self._ld(out), self.stream()), "orx_cross_fwd")
+
+    def cross_bwd(self, mode, G, A, P=None, x0=None, y=None, dy=None, dx_lo=None, dx_hi=None):
+        """One backward pass of a cross layer (orx_cross_bwd; the operands each mode reads and writes are in
+        include/orx.h).  [B, W] views with unit inner stride; FINAL splits dL/dx0 at dx_lo's width (dx_lo may be None
+        for split 0)."""
+        B, W = G.shape
+        ld = lambda t: self._ld(t) if t is not None else 0
+        split = (dx_lo.shape[1] if dx_lo is not None else 0) if mode == ORX_CROSS_FINAL else 0
+        _lib.check(self.lib.orx_cross_bwd(self.h, int(mode), B, W, _ptr(G), ld(G), _ptr(P), ld(P), _ptr(x0), ld(x0),
+                                          _ptr(y), ld(y), _ptr(A), ld(A), _ptr(dy), ld(dy), split, _ptr(dx_lo),
+                                          ld(dx_lo), _ptr(dx_hi), ld(dx_hi), self.stream()), "orx_cross_bwd")
 
     def pred_loss(self, pred, label, kind, clip, pred_out, dpred, out4):
         _lib.check(self.lib.orx_pred_loss(self.h, _ptr(pred), _ptr(label), pred.numel(), kind, clip, _ptr(pred_out),

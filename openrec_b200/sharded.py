@@ -331,10 +331,11 @@ class DLRMShard:
     are this rank's Dense replicas as (kernel, bias or None, act) triples, ``dense_slots`` the (s0, s1) of every kernel
     and bias in that order (biases that are None skipped).  ``col_off`` ([T + 1], table k's bag = sparse columns
     col_off[k] .. col_off[k+1]) makes every feature multi-hot, pooled by a sum (``pooling`` 0) or a mean (1); None: one
-    id per table."""
+    id per table.  ``cross``: the replicas of a DCN-v2 cross network in DLRMGraph's form (per layer [(kernel, bias or
+    None)]), which replaces the dot interaction; their (s0, s1) follow the top MLP's in ``dense_slots``."""
 
     def __init__(self, eng, rank, world, vocab, dim, bot, top, table, slots, dense_slots, *, self_interaction=False,
-                 mode="reference", loss_kind=0, clip=0.0, col_off=None, pooling=0):
+                 mode="reference", loss_kind=0, clip=0.0, col_off=None, pooling=0, cross=None):
         from .tf2.mlp_ops import DLRMGraph
         self.eng, self.rank, self.world, self.D = eng, rank, world, int(dim)
         self.row_off = row_offsets(vocab)
@@ -347,14 +348,16 @@ class DLRMShard:
         if tuple(table.shape) != (max(self.rows, 1), self.D):
             raise ValueError(f"shard shape {tuple(table.shape)} != {(max(self.rows, 1), self.D)}")
         self.table, self.slots = table, tuple(slots)
-        self.bot, self.top, self.dense_slots = bot, top, list(dense_slots)
+        self.bot, self.top, self.cross, self.dense_slots = bot, top, cross, list(dense_slots)
         if len(self.dense_slots) != len(self.dense_vars()):
             raise ValueError("dense_slots needs one (s0, s1) pair per Dense kernel and bias")
-        self.graph = DLRMGraph([None] * self.T, bot, top, self.D, self_interaction, mode, loss_kind, clip)
+        self.graph = DLRMGraph([None] * self.T, bot, top, self.D, self_interaction, mode, loss_kind, clip, cross=cross)
         self.last = {}          # sizes of the last step: unique rows fetched, rows served to the other ranks
 
     def dense_vars(self):
-        return [t for w, b, _ in self.bot + self.top for t in (w, b) if t is not None]
+        """The Dense kernels and biases, then the cross network's, in the order of dense_slots."""
+        mlp = [t for w, b, _ in self.bot + self.top for t in (w, b) if t is not None]
+        return mlp + [t for p in self.cross or [] for w, b in p for t in (w, b) if t is not None]
 
     # ---- global <-> shard (tests, checkpoints)
     def load_global(self, table):
@@ -496,16 +499,17 @@ def dlrm_step_sharded(parts, xchg, batches, opt_args, c_loss=1.0, timer=None):
         grads.append(p.graph.backward(c))
     timer("fwd_bwd")
     if parts[0].col_off is None:
-        g_rows = _return_grads(parts, xchg, fetched, [dZ.view(-1, p.D) for p, (dZ, _, _) in zip(parts, grads)], timer)
+        g_rows = _return_grads(parts, xchg, fetched, [g[0].view(-1, p.D) for p, g in zip(parts, grads)], timer)
     else:
-        g_rows = _return_grads(parts, xchg, fetched, [dZ for dZ, _, _ in grads], timer, fold=_bag_fold)
+        g_rows = _return_grads(parts, xchg, fetched, [g[0] for g in grads], timer, fold=_bag_fold)
     for p, f, g in zip(parts, fetched, g_rows):
         o = p.eng.make_opt(*opt_args)
         p.eng.sparse_apply(p.eng.make_table(p.table, *p.slots), f.req, g, o)    # ADAM_DENSE: the owner sweeps its shard
     timer("owner_apply")
     flats = []
-    for (_, bot_g, top_g), c in zip(grads, caches):
-        flats.append(torch.cat([t.reshape(-1) for dw, db in bot_g + top_g for t in (dw, db) if t is not None]
+    for (_, bot_g, top_g, cross_g), c in zip(grads, caches):
+        pairs = bot_g + top_g + [pair for layer in cross_g for pair in layer]
+        flats.append(torch.cat([t.reshape(-1) for dw, db in pairs for t in (dw, db) if t is not None]
                                + [c["out4"][:1]]))
     xchg.all_reduce(flats)
     outs = []

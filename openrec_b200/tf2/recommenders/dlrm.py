@@ -1,6 +1,7 @@
 """DLRM -- mirrors openrec/tf2/recommenders/dlrm.py:6-100 on liborx (gathers, interaction, Dense layers,
 loss, sparse + dense optimizer applies); same lazy step protocol as the other recommenders.  ``bag_sizes`` adds
-multi-hot sparse features (a pooled bag of ids per table), which the reference does not have."""
+multi-hot sparse features (a pooled bag of ids per table) and ``arch_interaction_op="cross"`` the DCN-v2 cross network
+(MLPerf DLRM-DCNv2), which the reference does not have."""
 import sys
 
 import torch
@@ -10,7 +11,7 @@ from ..._lib import ORX_BAG_MAX_TABLES
 from ...tfshim.core import LazyScalar, StepNode, Tensor, convert
 from ...tfshim.keras import Model
 from ..mlp_ops import ACT, DLRMGraph
-from ..modules import MLP, LatentFactor, SecondOrderFeatureInteraction
+from ..modules import MLP, CrossNetwork, LatentFactor, SecondOrderFeatureInteraction
 
 
 def bag_layout(bag_sizes, pooling, n_tables):
@@ -35,17 +36,44 @@ def bag_layout(bag_sizes, pooling, n_tables):
     return sizes, col_off, 0 if pooling == "sum" else 1
 
 
+def cross_projections(cross):
+    """DLRMGraph's ``cross`` argument: the tensors of a built CrossNetwork's projections."""
+    return [[(w.t, None if b is None else b.t) for w, b in p] for p in cross.projections()]
+
+
+def _dense_groups(model, bot_g, top_g, cross_g):
+    """(variables, gradients) of every Dense kernel / bias and cross projection, in the order the step applies them."""
+    out = []
+    for mlp, grads in ((model._mlp_bot, bot_g), (model._mlp_top, top_g)):
+        for layer, (dw, db) in zip(mlp.layers, grads):
+            out.append((layer.kernel, dw))
+            if layer.bias is not None:
+                out.append((layer.bias, db))
+    cross = model._cross
+    for p, grads in zip(cross.projections() if cross is not None else [], cross_g):
+        for (w, b), (dw, db) in zip(p, grads):
+            out.append((w, dw))
+            if b is not None:
+                out.append((b, db))
+    return out
+
+
 class DLRM(Model):
     def __init__(self, m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op="dot", arch_interaction_itself=False,
                  sigmoid_bot=False, sigmoid_top=True, loss_func="mse", loss_threshold=0.0,
-                 interaction_mode="reference", bag_sizes=None, pooling="sum"):
+                 interaction_mode="reference", bag_sizes=None, pooling="sum", cross_layers=3,
+                 cross_projection_dim=None):
         """Reference signature (dlrm.py:8-19) + ``interaction_mode``: 'reference' reproduces the reference's
         dot interaction bit for bit (identically zero, SURVEY Q1), 'dlrm' is the strictly-lower triangle.
 
         ``bag_sizes = [L_0 .. L_{T-1}]`` makes every sparse feature multi-hot: ``sparse_features`` is then [B, sum(L)],
         table k's bag for sample b being columns sum(L[:k]) .. sum(L[:k+1]) - 1 of row b, pooled by ``pooling`` ('sum'
         or 'mean' over the bag's valid ids).  An id < 0 is padding; an id >= the vocabulary adds nothing and gets no
-        gradient; a bag without a valid id pools to the zero row.  None (the default): one id per table, [B, T]."""
+        gradient; a bag without a valid id pools to the zero row.  None (the default): one id per table, [B, T].
+
+        ``arch_interaction_op="cross"`` replaces the dot interaction by a DCN-v2 CrossNetwork(cross_layers,
+        cross_projection_dim) over x0 = (dense_vec | Z_0 | .. | Z_{T-1}), W = (T + 1) * m_spa wide; the top MLP reads
+        its [B, W] output.  ``arch_interaction_itself`` and ``interaction_mode`` apply to the dot interaction only."""
         super().__init__()
         self._bag_sizes, self._col_off, self._pooling = bag_layout(bag_sizes, pooling, len(ln_emb))
         self._m_spa = int(m_spa)
@@ -54,10 +82,12 @@ class DLRM(Model):
         self._latent_factors = [LatentFactor(num_instances=int(num), dim=m_spa) for num in ln_emb]
         self._mlp_bot = MLP(units_list=ln_bot, out_activation="sigmoid" if sigmoid_bot else "relu")
         self._mlp_top = MLP(units_list=ln_top, out_activation="sigmoid" if sigmoid_top else "relu")
-        self._dot_interaction = None
+        self._dot_interaction = self._cross = None
         if arch_interaction_op == "dot":
             self._dot_interaction = SecondOrderFeatureInteraction(self_interaction=arch_interaction_itself,
                                                                   mode=interaction_mode)
+        elif arch_interaction_op == "cross":
+            self._cross = CrossNetwork(cross_layers, cross_projection_dim)
         elif self._arch_interaction_op != "cat":   # the reference never assigns this attribute: AttributeError (Q2)
             sys.exit("ERROR: arch_interaction_op=" + self._arch_interaction_op + " is not supported")
         if loss_func not in ("mse", "bce"):
@@ -71,14 +101,20 @@ class DLRM(Model):
         width = T + 1
         P = width * (width + 1) // 2 if self._self_interaction else width * (width - 1) // 2
         self._mlp_bot.build(n_dense)
-        self._mlp_top.build(self._m_spa + P)
+        cross = self._cross
+        if cross is not None:
+            cross.build(width * self._m_spa)
+            self._mlp_top.build(width * self._m_spa)
+        else:
+            self._mlp_top.build(self._m_spa + P)
 
         def layers(mlp):
             return [(l.kernel.t, None if l.bias is None else l.bias.t, ACT[l.activation]) for l in mlp.layers]
         clip = float(self._loss_threshold) if 0.0 < self._loss_threshold < 1.0 else 0.0
         return DLRMGraph([lf.embeddings.t for lf in self._latent_factors], layers(self._mlp_bot),
                          layers(self._mlp_top), self._m_spa, self._self_interaction, self._interaction_mode,
-                         0 if self._loss_func == "mse" else 1, clip, self._col_off, self._pooling)
+                         0 if self._loss_func == "mse" else 1, clip, self._col_off, self._pooling,
+                         cross=None if cross is None else cross_projections(cross))
 
     def _checked_inputs(self, dense_features, sparse_features, label=None):
         dense, sparse, lab = self._inputs(dense_features, sparse_features, label)
@@ -133,7 +169,7 @@ class DLRM(Model):
         if got != want or any(c != coefs[0] for c in coefs):
             raise NotImplementedError("apply_gradients: DLRM's fused step needs the gradients of ALL trainable "
                                       "variables w.r.t. one objective")
-        c, (dZ, bot_g, top_g) = self._fwd_bwd(node, float(coefs[0].get(0, 0.0)))
+        c, (dZ, bot_g, top_g, cross_g) = self._fwd_bwd(node, float(coefs[0].get(0, 0.0)))
         eng, o = N.engine(), optimizer.opt_struct()
         for k, lf in enumerate(self._latent_factors):                 # IndexedSlices(ids = sparse[:,k], dZ[:,k,:])
             if self._col_off is None:
@@ -141,11 +177,8 @@ class DLRM(Model):
             else:                                                     # ... of every valid id of table k's bags
                 eng.bag_sparse_apply(optimizer.table(lf.embeddings), sparse, self._col_off[k], self._bag_sizes[k],
                                      dZ[:, k, :], self._pooling, o)
-        for mlp, grads in ((self._mlp_bot, bot_g), (self._mlp_top, top_g)):
-            for layer, (dw, db) in zip(mlp.layers, grads):
-                eng.dense_apply(layer.kernel.t, *optimizer.slots(layer.kernel), dw, o)
-                if layer.bias is not None:
-                    eng.dense_apply(layer.bias.t, *optimizer.slots(layer.bias), db, o)
+        for var, g in _dense_groups(self, bot_g, top_g, cross_g):
+            eng.dense_apply(var.t, *optimizer.slots(var), g, o)
         node.out = c["out4"]
         node.stepped = True
         node.inputs = None
@@ -154,26 +187,30 @@ class DLRM(Model):
         """liborx kernel launches of one training step (bench.py's gpu_launches): per table gather + index / apply / tail,
         per Dense layer forward (1) + backward (activation, column sum, dgrad, wgrad; split-K adds a reduce) + 2 dense
         applies, 2 interaction kernels, 1 loss kernel.  Multi-hot: one gather launch for all tables, and per table id
-        compaction / index / apply / tail."""
+        compaction / index / apply / tail.  Cross network, in place of the interaction: per projection forward (1) +
+        backward (column sum with a bias, dgrad, wgrad) + 1 apply per variable, per layer 2 cross kernels, and 1 final
+        cross kernel."""
         T = len(self._latent_factors)
         n_dense = len(self._mlp_bot.layers) + len(self._mlp_top.layers)
-        return (4 * T if self._col_off is None else 1 + 4 * T) + n_dense * (1 + 4 + 2) + 2 + 1
+        n = (4 * T if self._col_off is None else 1 + 4 * T) + n_dense * (1 + 4 + 2) + 1
+        cross = self._cross
+        if cross is None:
+            return n + 2
+        per_layer = 2 + (1 + 3 + 2 if cross.projection_dim is None else (1 + 2 + 1) + (1 + 3 + 2))
+        return n + cross.num_layers * per_layer + 1
 
     def _orx_materialize_grad(self, node, var, coef):
         if node.stepped:
             raise RuntimeError("gradients requested after the step was applied")
-        _, (dZ, bot_g, top_g) = self._fwd_bwd(node, float(coef.get(0, 0.0)))
+        _, (dZ, bot_g, top_g, cross_g) = self._fwd_bwd(node, float(coef.get(0, 0.0)))
         for k, lf in enumerate(self._latent_factors):
             if var is lf.embeddings:
                 if self._col_off is None:
                     return Tensor(node.inputs[1][:, k].contiguous()), Tensor(dZ[:, k, :].contiguous())
                 return self._bag_slices(node.inputs[1], k, dZ[:, k, :])
-        for mlp, grads in ((self._mlp_bot, bot_g), (self._mlp_top, top_g)):
-            for layer, (dw, db) in zip(mlp.layers, grads):
-                if var is layer.kernel:
-                    return None, Tensor(dw)
-                if var is layer.bias:
-                    return None, Tensor(db)
+        for v, g in _dense_groups(self, bot_g, top_g, cross_g):
+            if var is v:
+                return None, Tensor(g)
         raise KeyError("variable does not belong to this model")
 
     def _bag_slices(self, sparse, k, dz):

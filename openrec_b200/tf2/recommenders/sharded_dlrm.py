@@ -10,6 +10,9 @@ of the GLOBAL batch, identical on every rank.  SGD, Adagrad, LazyAdam and Keras 
 shard, which is the whole-table sweep).  ``openrec_b200.tf2.checkpoint`` saves one rank's shard and replicas (one file
 per rank).
 
+``arch_interaction_op="cross"`` (with ``cross_layers`` / ``cross_projection_dim``) replaces the dot interaction by the
+DCN-v2 cross network, exactly as in DLRM; its variables are replicas like the Dense layers'.
+
 ``bag_sizes`` / ``pooling`` make every sparse feature multi-hot, exactly as in DLRM: ``sparse_features`` is [B, sum(L)],
 table k's bag being its column block, pooled by a sum or a mean over the bag's valid ids.  The bags' rows are
 deduplicated over this rank's batch before they travel, and each owner applies every row once per step.  The shard
@@ -24,18 +27,19 @@ from ... import native as N
 from ...sharded import DistExchange, DLRMShard, dlrm_inference_sharded, dlrm_step_sharded, row_offsets
 from ...tfshim.core import LazyScalar, StepNode, Tensor
 from ..mlp_ops import ACT, interaction_width
-from ..modules import MLP
-from .dlrm import DLRM, bag_layout
+from ..modules import MLP, CrossNetwork
+from .dlrm import DLRM, bag_layout, cross_projections
 from .sharded import _ShardedModel
 
 
 class ShardedDLRM(_ShardedModel):
     def __init__(self, m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op="dot", arch_interaction_itself=False,
                  sigmoid_bot=False, sigmoid_top=True, loss_func="mse", loss_threshold=0.0,
-                 interaction_mode="reference", seed=0, bag_sizes=None, pooling="sum"):
+                 interaction_mode="reference", seed=0, bag_sizes=None, pooling="sum", cross_layers=3,
+                 cross_projection_dim=None):
         super().__init__()
         self._bag_sizes, self._col_off, self._pooling = bag_layout(bag_sizes, pooling, len(ln_emb))
-        if arch_interaction_op != "dot" and self._arch_interaction_op != "cat":   # as DLRM: AttributeError (SURVEY Q2)
+        if arch_interaction_op not in ("dot", "cross") and self._arch_interaction_op != "cat":   # as DLRM (SURVEY Q2)
             sys.exit("ERROR: arch_interaction_op=" + self._arch_interaction_op + " is not supported")
         if loss_func not in ("mse", "bce"):
             sys.exit("ERROR: loss_func=" + loss_func + " is not supported")
@@ -49,6 +53,7 @@ class ShardedDLRM(_ShardedModel):
                                              "embedding_shard")
         self._mlp_bot = MLP(units_list=ln_bot, out_activation="sigmoid" if sigmoid_bot else "relu")
         self._mlp_top = MLP(units_list=ln_top, out_activation="sigmoid" if sigmoid_top else "relu")
+        self._cross = CrossNetwork(cross_layers, cross_projection_dim) if arch_interaction_op == "cross" else None
         self._xchg = DistExchange()
 
     def _own_variables(self):
@@ -62,26 +67,33 @@ class ShardedDLRM(_ShardedModel):
         if self._mlp_bot.layers[0].kernel is not None:
             return
         self._mlp_bot.build(n_dense)
-        self._mlp_top.build(self._m_spa + interaction_width(len(self._vocab) + 1, self._self_interaction))
-        for mlp in (self._mlp_bot, self._mlp_top):
-            for layer in mlp.layers:
-                for var in (layer.kernel, layer.bias):
-                    if var is not None:
-                        dist.broadcast(var.t, 0)
+        if self._cross is not None:
+            self._cross.build((len(self._vocab) + 1) * self._m_spa)
+            self._mlp_top.build((len(self._vocab) + 1) * self._m_spa)
+        else:
+            self._mlp_top.build(self._m_spa + interaction_width(len(self._vocab) + 1, self._self_interaction))
+        for var in self._dense_vars():
+            dist.broadcast(var.t, 0)
+
+    def _dense_vars(self):
+        """The Dense kernels and biases, then the cross network's: DLRMShard.dense_vars() as Variables."""
+        out = [var for mlp in (self._mlp_bot, self._mlp_top) for l in mlp.layers for var in (l.kernel, l.bias)
+               if var is not None]
+        if self._cross is not None:
+            out += [var for p in self._cross.projections() for pair in p for var in pair if var is not None]
+        return out
 
     def _part(self, optimizer=None):
         def layers(mlp):
             return [(l.kernel.t, None if l.bias is None else l.bias.t, ACT[l.activation]) for l in mlp.layers]
-        dense = [var for mlp in (self._mlp_bot, self._mlp_top) for l in mlp.layers for var in (l.kernel, l.bias)
-                 if var is not None]
         slots = optimizer.slots(self.embedding_shard) if optimizer is not None else (None, None)
-        dense_slots = [optimizer.slots(var) if optimizer is not None else (None, None) for var in dense]
+        dense_slots = [optimizer.slots(var) if optimizer is not None else (None, None) for var in self._dense_vars()]
         clip = float(self._loss_threshold) if 0.0 < self._loss_threshold < 1.0 else 0.0
         return DLRMShard(self._eng, self._rank, self._world, self._vocab, self._m_spa, layers(self._mlp_bot),
                          layers(self._mlp_top), self.embedding_shard.t, slots, dense_slots,
                          self_interaction=self._self_interaction, mode=self._interaction_mode,
                          loss_kind=0 if self._loss_func == "mse" else 1, clip=clip, col_off=self._col_off,
-                         pooling=self._pooling)
+                         pooling=self._pooling, cross=None if self._cross is None else cross_projections(self._cross))
 
     def _inputs(self, dense_features, sparse_features, label=None):
         dense, sparse, lab = DLRM._inputs(dense_features, sparse_features, label)
