@@ -106,6 +106,31 @@ typedef struct {
   int32_t dim;
 } orx_table_t;
 
+/* A LatentFactor stored in bfloat16 (the *_bf16 entry points), its optimizer slots in fp32: s0 / s1 have exactly the
+ * shapes and meaning of orx_table_t's (the row-wise Adagrad accumulator is float[rows]).  var holds the [rows, dim]
+ * bf16 bit patterns.  Every kernel reads a row as fp32 (the exact upcast), computes in fp32 and rounds only the final
+ * store of an updated element, stochastically:
+ *   Element (row, col) of table t (0 = user, 1 = item), written by the apply of optimizer step opt->step with seed
+ *   sr_seed, takes 16 random bits  r = H(sr_seed, step, t, row, col) >> 16, with
+ *     mix64(z)   = splitmix64's finalizer: z = (z ^ z >> 30) * 0xbf58476d1ce4e5b9; z = (z ^ z >> 27) *
+ *                  0x94d049bb133111eb; z ^ z >> 31   (uint64 arithmetic)
+ *     mix32(x)   = x ^= x >> 16; x *= 0x7feb352d; x ^= x >> 15; x *= 0x846ca68b; x ^ x >> 16   (uint32 arithmetic)
+ *     key(t)     = (uint32)(mix64(sr_seed ^ mix64(2 * step + t)) >> 32)
+ *     H          = mix32(mix32(key(t) ^ (uint32)row) + (uint32)col * 0x9e3779b9)
+ *   and the stored bits are (bits(x) + r) >> 16 for the fp32 result x: a value exactly representable in bf16 is kept,
+ *   any other rounds away from zero with probability equal to its distance from the bf16 value below it (in units of
+ *   that ulp).  Inf is stored as is; NaN keeps sign and top mantissa bits with the quiet bit set (0x0040).  The bits
+ *   depend on those five values and x only, so every kernel that may write the row (owned in the fused step, staged in
+ *   the tail, swept under ADAM_DENSE) rounds it alike, with or without a prefetched index.
+ * Tables whose var is not 8-byte aligned, or whose dim is not a multiple of 4, take the scalar kernels (STEP_GENERIC). */
+typedef struct {
+  uint16_t* var; /* [rows, dim] bf16 bits */
+  float* s0;     /* as orx_table_t */
+  float* s1;
+  int64_t rows;
+  int32_t dim;
+} orx_table_bf16_t;
+
 /* ---- context ------------------------------------------------------------------------- */
 ORX_API int orx_abi_version(void);
 ORX_API const char* orx_last_error_string(void); /* host, thread-local */
@@ -148,9 +173,11 @@ enum orx_dispatch_op {
                                     S = 1 */
   ORX_OP_CENSOR_SHARD = 10, /* orx_censor_shard, one per call: variant CENSOR_VEC / CENSOR_SCALAR, TA = rank, TB = 0,
                                M = total ids (n_per_block * n_blocks), N = local_rows, K = dim, S = world */
-  ORX_OP_CROSS = 11 /* orx_cross_fwd / orx_cross_bwd, one per call with B > 0: variant CROSS_VEC / CROSS_SCALAR,
+  ORX_OP_CROSS = 11, /* orx_cross_fwd / orx_cross_bwd, one per call with B > 0: variant CROSS_VEC / CROSS_SCALAR,
                        TA = 0 forward / 1 backward, TB = orx_cross_mode (0 forward), M = B, N = W,
                        K = split (ORX_CROSS_FINAL, else 0), S = 1 */
+  ORX_OP_PAIRWISE_STEP_BF16 = 12 /* orx_pairwise_step_bf16, orx_pairwise_step_host_bf16: the fields of
+                                    ORX_OP_PAIRWISE_STEP */
 };
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
@@ -180,6 +207,11 @@ ORX_API int orx_debug_dispatch_log(orx_handle_t h, int32_t* rec_host, int32_t ca
  * of a set last until the second prefetch after it.  ORX_ERR_INVALID when the handle has none (ORX_PAIR_RESOLVE=0 at
  * orx_create, or no prefetch yet). */
 ORX_API int orx_debug_pair_records(orx_handle_t h, int32_t set, int32_t* rec, int32_t B, orx_stream_t stream);
+/* Test hook: the stochastic rounding of bf16 tables (orx_table_bf16_t) applied on `stream` to the device floats x[0..n),
+ * element i taken as (row0 + i / dim, i % dim) of table `table` (0 = user, 1 = item) at (sr_seed, step); the bf16 bits
+ * go to the device out[0..n). */
+ORX_API int orx_debug_round_bf16(orx_handle_t h, const float* x, uint16_t* out, int64_t n, int64_t row0, int32_t dim,
+                                 int32_t table, uint64_t sr_seed, int64_t step, orx_stream_t stream);
 
 /* Measurement hook (bench.py's roofline): while enabled, every 8th *_step call records CUDA events on its launch stream
  * around its launches -- orx_pairwise_step, orx_pairwise_step_host and orx_pointwise_step: [0] batch index (or the wait
@@ -260,6 +292,36 @@ ORX_API int orx_pairwise_grad(orx_handle_t h, int32_t kind, const orx_table_t* u
                       const orx_table_t* item_bias, const int32_t* uid, const int32_t* pid, const int32_t* nid,
                       int32_t B, float margin, float c_loss, float c_l2, float* d_user, float* d_pos, float* d_neg,
                       float* d_bp, float* d_bn, float* g_out, orx_stream_t s);
+
+/* ---- bf16 user / item tables (orx_table_bf16_t) ------------------------------------------------------------------
+ * orx_pairwise_step_bf16 / orx_pairwise_step_host_bf16: orx_pairwise_step / orx_pairwise_step_host on bf16 user and
+ * item tables, every optimizer kind included, each updated element rounded stochastically with sr_seed and opt->step.
+ * The item bias stays an fp32 orx_table_t.  A batch index built by orx_pairwise_prefetch is consumed as by the fp32
+ * step (pass it orx_table_t's with the rows and dims of these tables).  One dispatch record per call, op
+ * ORX_OP_PAIRWISE_STEP_BF16.  Untouched rows keep their bits, except under ADAM_DENSE (its sweep writes every row). */
+ORX_API int orx_pairwise_step_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                   const orx_table_bf16_t* item, const orx_table_t* item_bias, const int32_t* uid,
+                                   const int32_t* pid, const int32_t* nid, int32_t B, float margin, float c_loss,
+                                   float c_l2, const orx_opt_t* opt_host, uint64_t sr_seed, float* out4, orx_stream_t s);
+ORX_API int orx_pairwise_step_host_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                        const orx_table_bf16_t* item, const orx_table_t* item_bias,
+                                        const int32_t* uid_host, const int32_t* pid_host, const int32_t* nid_host,
+                                        int32_t B, float margin, float c_loss, float c_l2, const orx_opt_t* opt_host,
+                                        uint64_t sr_seed, float* out4_host, orx_stream_t s);
+/* orx_pairwise_fwd / orx_pairwise_grad on bf16 user and item tables (rows read as their exact fp32 upcast). */
+ORX_API int orx_pairwise_fwd_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                  const orx_table_bf16_t* item, const orx_table_t* item_bias, const int32_t* uid,
+                                  const int32_t* pid, const int32_t* nid, int32_t B, float margin, float* out4,
+                                  orx_stream_t s);
+ORX_API int orx_pairwise_grad_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                   const orx_table_bf16_t* item, const orx_table_t* item_bias, const int32_t* uid,
+                                   const int32_t* pid, const int32_t* nid, int32_t B, float margin, float c_loss,
+                                   float c_l2, float* d_user, float* d_pos, float* d_neg, float* d_bp, float* d_bn,
+                                   float* g_out, orx_stream_t s);
+/* orx_censor on a bf16 table: row / max(||row||_2, min_norm) in fp32 from the upcast row, stored rounded to nearest
+ * even (a projection, not an optimizer update). */
+ORX_API int orx_censor_bf16(orx_handle_t h, uint16_t* tab, int64_t rows, int32_t dim, const int32_t* ids, int32_t n,
+                            float min_norm, orx_stream_t s);
 
 /* ---- pointwise recommenders: GMF (recommenders/gmf.py:22-34) and WRMF (recommenders/wrmf.py:21-34 +
  *      modules/pointwise_mse_loss.py:18-31) ---------------------------------------------------

@@ -19,7 +19,7 @@ ORX_OPT_SGD, ORX_OPT_ADAGRAD, ORX_OPT_ADAM_LAZY, ORX_OPT_ADAM_DENSE, ORX_OPT_ROW
 ORX_OPT_MOMENTUM, ORX_OPT_NESTEROV = 6, 8   # 7: unassigned
 ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP = 0, 1, 2, 3, 4
 ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK_SHARD = 5, 6, 7, 8
-ORX_OP_POINTWISE_GRAD_ROWS, ORX_OP_CENSOR_SHARD, ORX_OP_CROSS = 9, 10, 11
+ORX_OP_POINTWISE_GRAD_ROWS, ORX_OP_CENSOR_SHARD, ORX_OP_CROSS, ORX_OP_PAIRWISE_STEP_BF16 = 9, 10, 11, 12
 ORX_VARIANT_GEMM_TMA, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_INTERACT = 0, 1, 2, 3
 ORX_VARIANT_STEP, ORX_VARIANT_STEP_PIPE, ORX_VARIANT_STEP_GENERIC = 4, 5, 6
 ORX_VARIANT_RANK_SMEM, ORX_VARIANT_RANK_GLOBAL, ORX_VARIANT_TOPK = 7, 8, 9
@@ -39,6 +39,11 @@ class OrxOpt(C.Structure):
 
 
 class OrxTable(C.Structure):
+    _fields_ = [("var", C.c_void_p), ("s0", C.c_void_p), ("s1", C.c_void_p), ("rows", C.c_int64),
+                ("dim", C.c_int32)]
+
+
+class OrxTableBf16(C.Structure):
     _fields_ = [("var", C.c_void_p), ("s0", C.c_void_p), ("s1", C.c_void_p), ("rows", C.c_int64),
                 ("dim", C.c_int32)]
 
@@ -63,6 +68,7 @@ class OrxSampler(C.Structure):
 
 _vp, _i32, _i64, _f, _u64 = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_uint64
 _T = C.POINTER(OrxTable)
+_TB = C.POINTER(OrxTableBf16)
 _O = C.POINTER(OrxOpt)
 _S = C.POINTER(OrxShard)
 
@@ -77,6 +83,7 @@ SIGNATURES = {
     "orx_debug_set_epoch": [_vp, C.c_uint32],
     "orx_debug_dispatch_log": [_vp, C.POINTER(_i32), _i32, C.POINTER(_i32)],
     "orx_debug_pair_records": [_vp, _i32, _vp, _i32, _vp],
+    "orx_debug_round_bf16": [_vp, _vp, _vp, _i64, _i64, _i32, _i32, _u64, _i64, _vp],
     "orx_profile_enable": [_vp, _i32],
     "orx_profile_read": [_vp, C.POINTER(C.c_float), _i32, C.POINTER(_i32)],
     "orx_fill_uniform": [_vp, _vp, _i64, _f, _f, _u64, _vp],
@@ -88,6 +95,12 @@ SIGNATURES = {
     "orx_pairwise_prefetch": [_vp, _T, _T, _vp, _vp, _vp, _i32, _i32, _i32, _vp],
     "orx_pairwise_fwd": [_vp, _i32, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _vp, _vp],
     "orx_pairwise_grad": [_vp, _i32, _T, _T, _T, _vp, _vp, _vp, _i32, _f, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
+    "orx_pairwise_step_bf16": [_vp, _i32, _TB, _TB, _T, _vp, _vp, _vp, _i32, _f, _f, _f, _O, _u64, _vp, _vp],
+    "orx_pairwise_step_host_bf16": [_vp, _i32, _TB, _TB, _T, _vp, _vp, _vp, _i32, _f, _f, _f, _O, _u64, _vp, _vp],
+    "orx_pairwise_fwd_bf16": [_vp, _i32, _TB, _TB, _T, _vp, _vp, _vp, _i32, _f, _vp, _vp],
+    "orx_pairwise_grad_bf16": [_vp, _i32, _TB, _TB, _T, _vp, _vp, _vp, _i32, _f, _f, _f, _vp, _vp, _vp, _vp, _vp, _vp,
+                               _vp],
+    "orx_censor_bf16": [_vp, _vp, _i64, _i32, _vp, _i32, _f, _vp],
     "orx_sparse_apply": [_vp, _T, _vp, _vp, _i32, _O, _vp],
     "orx_sparse_apply_strided": [_vp, _T, _vp, _i64, _vp, _i64, _i32, _O, _vp],
     "orx_gather_strided": [_vp, _vp, _i64, _i32, _vp, _i64, _i64, _vp, _i64, _vp, _vp],

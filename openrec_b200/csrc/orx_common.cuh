@@ -216,6 +216,31 @@ static inline bool orx_aligned16(const P*... p) {
   return (((uintptr_t)0 | ... | (uintptr_t)p) & 15) == 0;
 }
 
+// True when every pointer is 8-byte aligned: the rule of a bf16 table's 4-element (8-byte) row path.
+template <typename... P>
+static inline bool orx_aligned8(const P*... p) {
+  return (((uintptr_t)0 | ... | (uintptr_t)p) & 7) == 0;
+}
+
+// bf16 tables (orx_table_bf16_t): stochastic rounding of an update of table t (0 = user, 1 = item) at optimizer step
+// `step`, as include/orx.h states it.  The per-(seed, step, t) part is taken once on the host.
+__host__ __device__ inline uint32_t orx_mix32(uint32_t x) {
+  x ^= x >> 16;
+  x *= 0x7feb352du;
+  x ^= x >> 15;
+  x *= 0x846ca68bu;
+  x ^= x >> 16;
+  return x;
+}
+static inline uint64_t orx_mix64(uint64_t z) {
+  z = (z ^ (z >> 30)) * 0xbf58476d1ce4e5b9ull;
+  z = (z ^ (z >> 27)) * 0x94d049bb133111ebull;
+  return z ^ (z >> 31);
+}
+static inline uint32_t orx_sr_table_key(uint64_t seed, int64_t step, int t) {
+  return (uint32_t)(orx_mix64(seed ^ orx_mix64((uint64_t)step * 2u + (uint64_t)t)) >> 32);
+}
+
 // Grid of a grid-stride loop over n items: one thread per item, at most 32 blocks per SM, at least one block.
 static inline int orx_grid_for(int64_t n, int threads, int num_sms) {
   const int64_t b = (n + threads - 1) / threads;
@@ -368,6 +393,51 @@ __device__ __forceinline__ void orx_st4(float* p, float4 v) { *reinterpret_cast<
 // item bias + its slots, and the compact staging rows (those stay at normal priority).
 __device__ __forceinline__ float4 orx_ld4_stream(const float* p) { return __ldcs(reinterpret_cast<const float4*>(p)); }
 __device__ __forceinline__ void orx_st4_stream(float* p, float4 v) { __stcs(reinterpret_cast<float4*>(p), v); }
+// Row element access by storage type: a float table (every fp32 path, which these leave as it was) or a bf16 table held
+// as its uint16_t bits.  A bf16 row moves 4 elements per lane as one 8-byte access (the table 8-byte aligned), widened
+// to a float4 on load; all arithmetic is fp32, and only the store rounds: stochastically, with the row key
+// rk = orx_sr_row(table key, row) and the element's column (orx_bf16_sr).  The float forms ignore rk and col.
+__device__ __forceinline__ float orx_bf16_up(uint32_t b) { return __uint_as_float(b << 16); }
+__device__ __forceinline__ uint32_t orx_sr_row(uint32_t kt, int64_t row) { return orx_mix32(kt ^ (uint32_t)row); }
+__device__ __forceinline__ uint32_t orx_bf16_sr(float v, uint32_t rk, int col) {
+  const uint32_t u = __float_as_uint(v);
+  if ((u & 0x7f800000u) == 0x7f800000u) return (u >> 16) | ((u & 0x007fffffu) ? 0x40u : 0u);   // Inf; NaN stays NaN
+  return (u + (orx_mix32(rk + (uint32_t)col * 0x9e3779b9u) >> 16)) >> 16;
+}
+// round to nearest even (assign, censor): not an optimizer update
+__device__ __forceinline__ uint32_t orx_bf16_rne(float v) {
+  const uint32_t u = __float_as_uint(v);
+  if ((u & 0x7f800000u) == 0x7f800000u) return (u >> 16) | ((u & 0x007fffffu) ? 0x40u : 0u);
+  return (u + 0x7fffu + ((u >> 16) & 1u)) >> 16;
+}
+__device__ __forceinline__ float orx_ld1(const float* p) { return *p; }
+__device__ __forceinline__ float orx_ld1(const uint16_t* p) { return orx_bf16_up(*p); }
+__device__ __forceinline__ void orx_st1(float* p, float v, uint32_t, int) { *p = v; }
+__device__ __forceinline__ void orx_st1(uint16_t* p, float v, uint32_t rk, int col) {
+  *p = (uint16_t)orx_bf16_sr(v, rk, col);
+}
+__device__ __forceinline__ float4 orx_bf16x4_up(uint2 b) {
+  return make_float4(orx_bf16_up(b.x & 0xffffu), orx_bf16_up(b.x >> 16), orx_bf16_up(b.y & 0xffffu),
+                     orx_bf16_up(b.y >> 16));
+}
+__device__ __forceinline__ uint2 orx_bf16x4_sr(float4 v, uint32_t rk, int col) {
+  return make_uint2(orx_bf16_sr(v.x, rk, col) | (orx_bf16_sr(v.y, rk, col + 1) << 16),
+                    orx_bf16_sr(v.z, rk, col + 2) | (orx_bf16_sr(v.w, rk, col + 3) << 16));
+}
+__device__ __forceinline__ float4 orx_ld4_stream(const uint16_t* p) {
+  return orx_bf16x4_up(__ldcs(reinterpret_cast<const uint2*>(p)));
+}
+__device__ __forceinline__ void orx_st4_stream(float* p, float4 v, uint32_t, int) { orx_st4_stream(p, v); }
+__device__ __forceinline__ void orx_st4_stream(uint16_t* p, float4 v, uint32_t rk, int col) {
+  __stcs(reinterpret_cast<uint2*>(p), orx_bf16x4_sr(v, rk, col));
+}
+__device__ __forceinline__ void orx_st4_cg(float* p, float4 v, uint32_t, int) {
+  __stcg(reinterpret_cast<float4*>(p), v);
+}
+__device__ __forceinline__ void orx_st4_cg(uint16_t* p, float4 v, uint32_t rk, int col) {
+  __stcg(reinterpret_cast<uint2*>(p), orx_bf16x4_sr(v, rk, col));
+}
+
 // one 128-bit fire-and-forget reduction (REDG.E.ADD.F32x4 on sm_90+)
 __device__ __forceinline__ void orx_red4(float* p, float4 v) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
@@ -468,20 +538,21 @@ __device__ __forceinline__ float4 orx_apply4(float4 w, float4 g, float4& s0, flo
 // slots are written back with a 128-bit store (STREAM: evict-first, orx_st4_stream; else __stcg); any other row's
 // gradient is red.add'ed into its staging row d of G.  The addresses are formed inside each branch from the ids: taking
 // precomputed row pointers changes the register allocation of the step kernels.
-template <int OPT, bool STREAM>
-__device__ __forceinline__ void orx_own_or_stage4(bool own, float* W, float* P0, float* P1, int id, float* G, int d,
+// T: the table's storage (float or bf16 bits); kt its rounding key (orx_sr_row), unused for float.
+template <int OPT, bool STREAM, typename T>
+__device__ __forceinline__ void orx_own_or_stage4(bool own, T* W, float* P0, float* P1, int id, float* G, int d,
                                                   int D, int off, float4 w, float4 g, float4& s0, float4& s1,
-                                                  const OrxOptDev& o) {
+                                                  const OrxOptDev& o, uint32_t kt = 0) {
   typedef OrxOptSlots<OPT> SL;
-  auto st = [](float* p, float4 v) {
-    if (STREAM) orx_st4_stream(p, v);
-    else __stcg(reinterpret_cast<float4*>(p), v);
+  auto st = [](auto* p, float4 v, uint32_t rk, int col) {
+    if (STREAM) orx_st4_stream(p, v, rk, col);
+    else orx_st4_cg(p, v, rk, col);
   };
   if (!SL::STAGE_ONLY && own) {
     const int64_t i = (int64_t)id * D + off;
-    st(W + i, orx_apply4<OPT>(w, g, s0, s1, o));
-    if (SL::S0) st(P0 + i, s0);
-    if (SL::S1) st(P1 + i, s1);
+    st(W + i, orx_apply4<OPT>(w, g, s0, s1, o), orx_sr_row(kt, id), off);
+    if (SL::S0) st(P0 + i, s0, 0u, 0);
+    if (SL::S1) st(P1 + i, s1, 0u, 0);
   } else {
     orx_red4(G + (int64_t)d * D + off, g);
   }
@@ -489,13 +560,14 @@ __device__ __forceinline__ void orx_own_or_stage4(bool own, float* W, float* P0,
 
 // The ROWWISE_ADAGRAD form of orx_own_or_stage4: an owned row moves by its factor f (orx_row_scale, taken by the caller
 // over the whole row) and has no slot row here -- the caller stores its accumulator once.
-template <bool STREAM>
-__device__ __forceinline__ void orx_own_or_stage4_row(bool own, float* W, int id, float* G, int d, int D, int off,
-                                                      float4 w, float4 g, float f, const OrxOptDev& o) {
+template <bool STREAM, typename T>
+__device__ __forceinline__ void orx_own_or_stage4_row(bool own, T* W, int id, float* G, int d, int D, int off,
+                                                      float4 w, float4 g, float f, const OrxOptDev& o,
+                                                      uint32_t kt = 0) {
   if (own) {
     const float4 r = orx_row_apply4(w, g, f, o);
-    if (STREAM) orx_st4_stream(W + (int64_t)id * D + off, r);
-    else __stcg(reinterpret_cast<float4*>(W + (int64_t)id * D + off), r);
+    if (STREAM) orx_st4_stream(W + (int64_t)id * D + off, r, orx_sr_row(kt, id), off);
+    else orx_st4_cg(W + (int64_t)id * D + off, r, orx_sr_row(kt, id), off);
   } else {
     orx_red4(G + (int64_t)d * D + off, g);
   }
@@ -512,6 +584,16 @@ __device__ __forceinline__ void orx_update1(float* W, float* P0, float* P1, floa
   if (SL::S0) *P0 = s0;
   if (SL::S1) *P1 = s1;
 }
+// The same on an element of a table of storage T, rounded with row key rk at column col (orx_st1).
+template <int OPT, typename T>
+__device__ __forceinline__ void orx_update1(T* W, float* P0, float* P1, float w, float g, const OrxOptDev& o,
+                                            uint32_t rk, int col) {
+  typedef OrxOptSlots<OPT> SL;
+  float s0 = SL::S0 ? *P0 : 0.f, s1 = SL::S1 ? *P1 : 0.f;
+  orx_st1(W, orx_apply<OPT>(w, g, s0, s1, o), rk, col);
+  if (SL::S0) *P0 = s0;
+  if (SL::S1) *P1 = s1;
+}
 
 // Keras dense Adam (ADAM_DENSE) of element i, m = M, v = V: IEEE sqrtf and division, as the reference computes it.
 __device__ __forceinline__ void orx_adam_dense1(float* W, float* M, float* V, int64_t i, float g, const OrxOptDev& o) {
@@ -520,6 +602,19 @@ __device__ __forceinline__ void orx_adam_dense1(float* W, float* M, float* V, in
   M[i] = mm;
   V[i] = vv;
   W[i] = W[i] - o.lr * mm / (sqrtf(vv) + o.eps);
+}
+// The same on a bf16 table (element i at column col of the row with key rk).
+__device__ __forceinline__ void orx_adam_dense1(uint16_t* W, float* M, float* V, int64_t i, float g, const OrxOptDev& o,
+                                                uint32_t rk, int col) {
+  const float mm = o.beta1 * M[i] + (1.f - o.beta1) * g;
+  const float vv = o.beta2 * V[i] + (1.f - o.beta2) * g * g;
+  M[i] = mm;
+  V[i] = vv;
+  orx_st1(W + i, orx_ld1(W + i) - o.lr * mm / (sqrtf(vv) + o.eps), rk, col);
+}
+__device__ __forceinline__ void orx_adam_dense1(float* W, float* M, float* V, int64_t i, float g, const OrxOptDev& o,
+                                                uint32_t, int) {
+  orx_adam_dense1(W, M, V, i, g, o);
 }
 
 // One (loss, l2) float partial per block of 8 warps at partials[2 * blockIdx.x], warps summed in a fixed order.
@@ -595,6 +690,7 @@ struct SparseArgs {
   OrxHash hu, hi;
   OrxOptDev opt;
   int D;
+  uint32_t srk[2];   // bf16 tables: the rounding keys of the user / item table (orx_sr_table_key); unused for float
 };
 
 // Arguments of the shared tail kernel (staged rows -> optimizer, loss reduction).
@@ -620,7 +716,7 @@ struct TailArgs : SparseArgs {
 // step's red.adds left them in L2.
 // VEC: the table and slot rows of a are 16-byte aligned (orx_aligned16, decided by the launcher); with D % 4 == 0 the rows
 // then move as float4, else lane-strided scalars.
-template <int OPT, bool VEC>
+template <int OPT, bool VEC, typename T = float>
 __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni) {
   typedef OrxOptSlots<OPT> SL;
   constexpr bool ZERO_ONLY = SL::STAGE_ONLY;
@@ -637,7 +733,8 @@ __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni)
     const int d = on ? (is_u ? r : r - nu) : 0;
     const int id = on ? (is_u ? a.hu.did[d] : a.hi.did[d]) : 0;
     float* G = (is_u ? a.gu : a.gi) + (int64_t)d * D;
-    float* W = (is_u ? a.U : a.I) + (int64_t)id * D;
+    T* W = reinterpret_cast<T*>(is_u ? a.U : a.I) + (int64_t)id * D;
+    const uint32_t rk = orx_sr_row(a.srk[is_u ? 0 : 1], id);
     float* P0 = (is_u ? a.Us0 : a.Is0) + (int64_t)id * D;
     float* P1 = (is_u ? a.Us1 : a.Is1) + (int64_t)id * D;
     if (VEC && (D & 3) == 0) {  // 128-bit path: float4 index sl + 8k
@@ -658,7 +755,7 @@ __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni)
           const int e = e0 + sl + 8 * k;
           if (!on || e >= nq) continue;
           if (!ZERO_ONLY) {
-            orx_st4_stream(W + 4 * e, orx_apply4<OPT>(w[k], g[k], s0v[k], s1v[k], a.opt));
+            orx_st4_stream(W + 4 * e, orx_apply4<OPT>(w[k], g[k], s0v[k], s1v[k], a.opt), rk, 4 * e);
             if (SL::S0) orx_st4_stream(P0 + 4 * e, s0v[k]);
             if (SL::S1) orx_st4_stream(P1 + 4 * e, s1v[k]);
           }
@@ -667,7 +764,7 @@ __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni)
       }
     } else if (on) {
       for (int e = sl; e < D; e += 8) {
-        if (!ZERO_ONLY) orx_update1<OPT>(W + e, P0 + e, P1 + e, W[e], G[e], a.opt);
+        if (!ZERO_ONLY) orx_update1<OPT>(W + e, P0 + e, P1 + e, orx_ld1(W + e), G[e], a.opt, rk, e);
         G[e] = 0.f;
       }
     }
@@ -683,7 +780,7 @@ __device__ __forceinline__ void orx_tail_rows(const TailArgs& a, int nu, int ni)
 // first -- lane sl over float4 (scalar) indices sl, sl + 8, ... in order, then the fixed 8-lane tree -- and only then
 // apply: a second pass over G, which the step's red.adds left in L2.  The row's accumulator s0[id] is one scalar; the
 // item bias gets element-wise ADAGRAD.
-template <bool VEC>
+template <bool VEC, typename T = float>
 __device__ __forceinline__ void orx_tail_rows_rowwise(const TailArgs& a, int nu, int ni) {
   const int lane = threadIdx.x & 31;
   const int gwarp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -700,7 +797,8 @@ __device__ __forceinline__ void orx_tail_rows_rowwise(const TailArgs& a, int nu,
     const int d = on ? (is_u ? r : r - nu) : 0;
     const int id = on ? (is_u ? a.hu.did[d] : a.hi.did[d]) : 0;
     float* G = (is_u ? a.gu : a.gi) + (int64_t)d * D;
-    float* W = (is_u ? a.U : a.I) + (int64_t)id * D;
+    T* W = reinterpret_cast<T*>(is_u ? a.U : a.I) + (int64_t)id * D;
+    const uint32_t rk = orx_sr_row(a.srk[is_u ? 0 : 1], id);
     float* P0 = (is_u ? a.Us0 : a.Is0) + id;
     float ss = 0.f, acc = 0.f;
     if (on) {
@@ -728,13 +826,13 @@ __device__ __forceinline__ void orx_tail_rows_rowwise(const TailArgs& a, int nu,
           for (int k = 0; k < 4; ++k) {
             const int e = e0 + sl + 8 * k;
             if (e >= nq) continue;
-            orx_st4_stream(W + 4 * e, orx_row_apply4(w[k], g[k], f, a.opt));
+            orx_st4_stream(W + 4 * e, orx_row_apply4(w[k], g[k], f, a.opt), rk, 4 * e);
             __stcg(reinterpret_cast<float4*>(G) + e, z4);
           }
         }
       } else {
         for (int e = sl; e < D; e += 8) {
-          W[e] = orx_row_apply1(W[e], G[e], f, a.opt);
+          orx_st1(W + e, orx_row_apply1(orx_ld1(W + e), G[e], f, a.opt), rk, e);
           G[e] = 0.f;
         }
       }
@@ -777,7 +875,9 @@ typedef std::function<int(const SparseArgs& s, const int4* res, float* partials,
 int orx_sparse_step(orx_ctx* c, int op, int kind, const orx_table_t* user, const orx_table_t* item,
                     const orx_table_t* bias, const orx_table_t* w, const int32_t* uid, const int32_t* iid,
                     const int32_t* nid, int B, const orx_opt_t* opt, float loss_scale, float c_l2, float* out4,
-                    const OrxStepKernel& kernel, cudaStream_t st);
+                    const OrxStepKernel& kernel, cudaStream_t st, const uint32_t* srk = nullptr);
+// srk (orx_sparse_step, orx_launch_adam_sweeps): the user / item tables are bf16 (orx_table_bf16_t, var passed as the
+// float* of the orx_table_t) with these rounding keys (orx_sr_table_key); null = float tables.
 // The un-fused forward / gradient kernel of a family over B samples: launch(partials, blocks) on st with the handle's
 // partials, then, when out4 is given, the (loss, l2) partials reduced into it, the loss scaled by loss_scale.
 int orx_sparse_unfused(orx_ctx* c, int B, float loss_scale, float* out4,
@@ -785,9 +885,10 @@ int orx_sparse_unfused(orx_ctx* c, int B, float loss_scale, float* out4,
 // ADAM_DENSE: Keras dense Adam over every row of user / item / bias (item and bias may be null), a row's summed gradient
 // taken from its side's table of index set ix and staging rows.  Runs before the tail, which zeroes the staging rows.
 int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
-                           const OrxIndexSet& ix, const OrxOptDev& o, cudaStream_t st);
+                           const OrxIndexSet& ix, const OrxOptDev& o, cudaStream_t st, const uint32_t* srk = nullptr);
 // k_sparse_tail over ta, its 128-bit row path chosen by the alignment of ta's table and slot rows (orx_aligned16).
-int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st);
+// bf16: the user / item tables of ta are bf16 (ta.srk), whose 8-byte row path needs 8-byte aligned rows.
+int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st, bool bf16 = false);
 int orx_launch_reduce_partials(const float* partials, int n, float loss_scale, float* out4, cudaStream_t st);
 // index of n samples (a[t], b0[t]) or (a[t], b0[t], b1[t]); only samples whose ids are all in range are inserted
 int orx_launch_index_build(orx_ctx* c, const int32_t* a, int64_t rows_a, const int32_t* b0, const int32_t* b1,

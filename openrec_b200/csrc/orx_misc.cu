@@ -91,8 +91,9 @@ extern "C" int orx_gather(orx_handle_t h, const float* tab, int64_t rows, int32_
 // before the first norm is reduced; otherwise one row at a time, lane-strided.  Every lane of the warp calls it.  (The
 // row shape is tested here rather than passed in: so k_censor<true> compiles to the same SASS as k_censor did before
 // the function was factored out of it.)
-template <bool VEC>
-__device__ __forceinline__ void orx_censor_rows8(float* tab, int D, int32_t my_id, float min_norm) {
+// T = uint16_t: a bf16 table, scalar path only (VEC false), each result stored rounded to nearest even.
+template <bool VEC, typename T = float>
+__device__ __forceinline__ void orx_censor_rows8(T* tab, int D, int32_t my_id, float min_norm) {
   const int lane = threadIdx.x & 31;
   if (VEC && (D & 3) == 0 && D <= 128) {
     const int nq = D >> 2;
@@ -118,12 +119,15 @@ __device__ __forceinline__ void orx_censor_rows8(float* tab, int D, int32_t my_i
     for (int k = 0; k < 8; ++k) {
       const int32_t id = __shfl_sync(ORX_FULL, my_id, k);
       if (id < 0) continue;
-      float* row = tab + (int64_t)id * D;
+      T* row = tab + (int64_t)id * D;
       float sq = 0.f;
-      for (int e = lane; e < D; e += 32) sq += row[e] * row[e];
+      for (int e = lane; e < D; e += 32) sq += orx_ld1(row + e) * orx_ld1(row + e);
       sq = orx_group_sum<32>(sq);
       const float den = fmaxf(sqrtf(sq), min_norm);
-      for (int e = lane; e < D; e += 32) row[e] = row[e] / den;
+      for (int e = lane; e < D; e += 32) {
+        if constexpr (std::is_same<T, float>::value) row[e] = row[e] / den;
+        else row[e] = (uint16_t)orx_bf16_rne(orx_ld1(row + e) / den);
+      }
     }
   }
 }
@@ -131,8 +135,8 @@ __device__ __forceinline__ void orx_censor_rows8(float* tab, int D, int32_t my_i
 // A warp takes 8 ids per iteration: lanes 0..7 load the ids and claim the rows in the hash in parallel, then (128-bit path)
 // all 8 rows are loaded before the first norm is reduced -- one row per warp left the kernel latency-bound (id -> hash ->
 // row -> reduce -> divide -> store: 23 us for 65 536 ids at D = 128, three of them per UCML step).
-template <bool VEC>
-__global__ void __launch_bounds__(256) k_censor(float* tab, int64_t rows, int D, const int32_t* __restrict__ ids,
+template <bool VEC, typename T = float>
+__global__ void __launch_bounds__(256) k_censor(T* tab, int64_t rows, int D, const int32_t* __restrict__ ids,
                                                 int n, float min_norm, OrxHash hsh) {
   const int lane = threadIdx.x & 31;
   const int nw = (gridDim.x * blockDim.x) >> 5;
@@ -142,7 +146,7 @@ __global__ void __launch_bounds__(256) k_censor(float* tab, int64_t rows, int D,
       const int32_t id = ids[b0 + lane];
       if (id >= 0 && (int64_t)id < rows && orx_hash_insert(hsh, id, 2) == 0u) my_id = id;   // first claim owns the row
     }
-    orx_censor_rows8<VEC>(tab, D, my_id, min_norm);
+    orx_censor_rows8<VEC, T>(tab, D, my_id, min_norm);
   }
 }
 
@@ -186,8 +190,10 @@ __global__ void __launch_bounds__(256) k_censor_shard(float* tab, int D, int64_t
 }
 
 
-extern "C" int orx_censor(orx_handle_t h, float* tab, int64_t rows, int32_t dim, const int32_t* ids, int32_t n,
-                          float min_norm, orx_stream_t s) {
+// T = uint16_t: orx_censor_bf16
+template <typename T>
+static int censor_impl(orx_handle_t h, T* tab, int64_t rows, int32_t dim, const int32_t* ids, int32_t n,
+                       float min_norm, orx_stream_t s) {
   ORX_REQUIRE(h != nullptr && tab && ids, "null pointer");
   ORX_REQUIRE(rows > 0 && dim > 0 && n >= 0, "bad sizes");
   if (n == 0) return ORX_OK;
@@ -199,10 +205,21 @@ extern "C" int orx_censor(orx_handle_t h, float* tab, int64_t rows, int32_t dim,
   if ((rc = orx_take_epoch(ix.u, st))) return rc;   // the dedup hash needs no clearing: a new epoch empties it
   int blocks = (n + 63) / 64;                 // 8 warps x 8 ids per block and iteration
   if (blocks > h->num_sms * 8) blocks = h->num_sms * 8;
-  if (orx_aligned16(tab)) k_censor<true><<<blocks, 256, 0, st>>>(tab, rows, dim, ids, n, min_norm, ix.u);
+  if constexpr (std::is_same<T, uint16_t>::value) k_censor<false, T><<<blocks, 256, 0, st>>>(tab, rows, dim, ids, n, min_norm, ix.u);
+  else if (orx_aligned16(tab)) k_censor<true><<<blocks, 256, 0, st>>>(tab, rows, dim, ids, n, min_norm, ix.u);
   else k_censor<false><<<blocks, 256, 0, st>>>(tab, rows, dim, ids, n, min_norm, ix.u);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
+}
+
+extern "C" int orx_censor(orx_handle_t h, float* tab, int64_t rows, int32_t dim, const int32_t* ids, int32_t n,
+                          float min_norm, orx_stream_t s) {
+  return censor_impl(h, tab, rows, dim, ids, n, min_norm, s);
+}
+
+extern "C" int orx_censor_bf16(orx_handle_t h, uint16_t* tab, int64_t rows, int32_t dim, const int32_t* ids, int32_t n,
+                               float min_norm, orx_stream_t s) {
+  return censor_impl(h, tab, rows, dim, ids, n, min_norm, s);
 }
 
 // The dedup hash of orx_censor_shard is the handle's censor_ws: slots only (mode-2 inserts stage nothing), as many as

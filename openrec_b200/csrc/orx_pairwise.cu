@@ -132,7 +132,9 @@ struct TripRegs {
 // L2 priority: table and slot rows are loaded and stored evict-first (orx_ld4_stream / orx_st4_stream); the probes and
 // the item bias + slot loads are evict-last (orx_ld_keep), the staging red.adds and the bias stores normal, so that the
 // index, the bias and the staging rows are still in L2 when they are reused.
-template <int KIND, int OPT, int D, int CH, int MINB, bool PIPE>
+// T: the storage of the user and item tables, float or bf16 bits (uint16_t; rows 8-byte aligned, rounded on store with
+// the keys a.srk).  Slot rows, item bias and staging rows are float either way.
+template <int KIND, int OPT, int D, int CH, int MINB, bool PIPE, typename T = float>
 __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
   constexpr int G = (D / 4 < 32) ? D / 4 : 32;  // lanes per triplet
   constexpr int K = D / (4 * G);                // float4 per lane per row
@@ -176,9 +178,9 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
 #pragma unroll
     for (int k = 0; k < K; ++k) {
       const int off = (k * G + gl) * 4;
-      r.u[k] = r.fl ? orx_ld4_stream(a.U + (int64_t)r.uu * D + off) : z4;
-      r.p[k] = r.fl ? orx_ld4_stream(a.I + (int64_t)r.pp * D + off) : z4;
-      r.n[k] = r.fl ? orx_ld4_stream(a.I + (int64_t)r.nn * D + off) : z4;
+      r.u[k] = r.fl ? orx_ld4_stream(reinterpret_cast<const T*>(a.U) + (int64_t)r.uu * D + off) : z4;
+      r.p[k] = r.fl ? orx_ld4_stream(reinterpret_cast<const T*>(a.I) + (int64_t)r.pp * D + off) : z4;
+      r.n[k] = r.fl ? orx_ld4_stream(reinterpret_cast<const T*>(a.I) + (int64_t)r.nn * D + off) : z4;
     }
   };
   Regs ra, rb;
@@ -294,9 +296,12 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
           const int off = (k * G + gl) * 4;
           float4 gu, gp, gn;
           pair_row_grads<KIND>(g, a.c_l2, r.u[k], r.p[k], r.n[k], &gu, &gp, &gn);
-          orx_own_or_stage4_row<true>(r.fl & 2, a.U, r.uu, a.gu, r.du, D, off, r.u[k], gu, fu, a.opt);
-          orx_own_or_stage4_row<true>(r.fl & 4, a.I, r.pp, a.gi, r.dp, D, off, r.p[k], gp, fp, a.opt);
-          orx_own_or_stage4_row<true>(r.fl & 8, a.I, r.nn, a.gi, r.dn, D, off, r.n[k], gn, fn, a.opt);
+          orx_own_or_stage4_row<true>(r.fl & 2, reinterpret_cast<T*>(a.U), r.uu, a.gu, r.du, D, off, r.u[k], gu, fu,
+                                      a.opt, a.srk[0]);
+          orx_own_or_stage4_row<true>(r.fl & 4, reinterpret_cast<T*>(a.I), r.pp, a.gi, r.dp, D, off, r.p[k], gp, fp,
+                                      a.opt, a.srk[1]);
+          orx_own_or_stage4_row<true>(r.fl & 8, reinterpret_cast<T*>(a.I), r.nn, a.gi, r.dn, D, off, r.n[k], gn, fn,
+                                      a.opt, a.srk[1]);
         }
         if (gl == 0) {
           if (r.fl & 2) __stcg(a.Us0 + r.uu, r.uacc);
@@ -310,12 +315,12 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
         const int off = (k * G + gl) * 4;
         float4 gu, gp, gn;
         pair_row_grads<KIND>(g, a.c_l2, r.u[k], r.p[k], r.n[k], &gu, &gp, &gn);
-        orx_own_or_stage4<OPT, true>(r.fl & 2, a.U, a.Us0, a.Us1, r.uu, a.gu, r.du, D, off, r.u[k], gu, r.us0[k],
-                                     r.us1[k], a.opt);
-        orx_own_or_stage4<OPT, true>(r.fl & 4, a.I, a.Is0, a.Is1, r.pp, a.gi, r.dp, D, off, r.p[k], gp, r.ps0[k],
-                                     r.ps1[k], a.opt);
-        orx_own_or_stage4<OPT, true>(r.fl & 8, a.I, a.Is0, a.Is1, r.nn, a.gi, r.dn, D, off, r.n[k], gn, r.ns0[k],
-                                     r.ns1[k], a.opt);
+        orx_own_or_stage4<OPT, true>(r.fl & 2, reinterpret_cast<T*>(a.U), a.Us0, a.Us1, r.uu, a.gu, r.du, D, off,
+                                     r.u[k], gu, r.us0[k], r.us1[k], a.opt, a.srk[0]);
+        orx_own_or_stage4<OPT, true>(r.fl & 4, reinterpret_cast<T*>(a.I), a.Is0, a.Is1, r.pp, a.gi, r.dp, D, off,
+                                     r.p[k], gp, r.ps0[k], r.ps1[k], a.opt, a.srk[1]);
+        orx_own_or_stage4<OPT, true>(r.fl & 8, reinterpret_cast<T*>(a.I), a.Is0, a.Is1, r.nn, a.gi, r.dn, D, off,
+                                     r.n[k], gn, r.ns0[k], r.ns1[k], a.opt, a.srk[1]);
       }
     }
   };
@@ -373,7 +378,8 @@ __global__ void __launch_bounds__(256, MINB) k_pair_step(const PairArgs a) {
 // Any D (e.g. the example's D=50): one triplet per warp-iteration, lanes stride the row.  MODE 0 = fused step (launched
 // with PDL), 1 = forward / explicit (un-fused) gradients into a.d_* / a.g_out (OPT = SGD, unread), table or row form.
 // A skipped triplet (bad id) contributes nothing and, in MODE 1, gets zero gradients and g_out = 0.
-template <int KIND, int OPT, int MODE>
+// T as in k_pair_step (MODE 1 of a bf16 table: the table form only).
+template <int KIND, int OPT, int MODE, typename T = float>
 __global__ void __launch_bounds__(256) k_pair_generic(const PairArgs a) {
   constexpr bool STAGE_ONLY = OrxOptSlots<OPT>::STAGE_ONLY;
   const int lane = threadIdx.x & 31;
@@ -388,13 +394,14 @@ __global__ void __launch_bounds__(256) k_pair_generic(const PairArgs a) {
     if (t >= a.B) break;
     const int uu = a.uid[t], pp = a.pid[t], nn = a.nid[t];
     const bool ok = uu >= 0 && uu < a.rowsU && pp >= 0 && pp < a.rowsI && nn >= 0 && nn < a.rowsI;
-    float* ur = a.U + (int64_t)uu * ld;
-    float* pr = a.I + (int64_t)pp * ld;
-    float* nr = a.I + (int64_t)nn * ld;
+    T* ur = reinterpret_cast<T*>(a.U) + (int64_t)uu * ld;
+    T* pr = reinterpret_cast<T*>(a.I) + (int64_t)pp * ld;
+    T* nr = reinterpret_cast<T*>(a.I) + (int64_t)nn * ld;
+    const uint32_t rku = orx_sr_row(a.srk[0], uu), rkp = orx_sr_row(a.srk[1], pp), rkn = orx_sr_row(a.srk[1], nn);
     float s1 = 0.f, s2 = 0.f, sq = 0.f, bp = 0.f, bn = 0.f, lt = 0.f, g = 0.f;
     if (ok) {
       for (int d = lane; d < D; d += 32) {
-        const float u = ur[d], p = pr[d], n = nr[d];
+        const float u = orx_ld1(ur + d), p = orx_ld1(pr + d), n = orx_ld1(nr + d);
         if (KIND == ORX_PAIR_BPR) {
           s1 += u * p;
           s2 += u * n;
@@ -404,8 +411,8 @@ __global__ void __launch_bounds__(256) k_pair_generic(const PairArgs a) {
         }
         sq += u * u + p * p + n * n;
       }
-      bp = row_form ? pr[D] : a.Bv[pp];
-      bn = row_form ? nr[D] : a.Bv[nn];
+      bp = row_form ? orx_ld1(pr + D) : a.Bv[pp];
+      bn = row_form ? orx_ld1(nr + D) : a.Bv[nn];
     }
     l2_acc += sq;
     s1 = orx_group_sum<32>(s1);
@@ -426,7 +433,7 @@ __global__ void __launch_bounds__(256) k_pair_generic(const PairArgs a) {
         float su = 0.f, sp = 0.f, sn = 0.f;
         for (int d = lane; d < D; d += 32) {
           float gu, gp, gn;
-          pair_grads1<KIND>(g, a.c_l2, ur[d], pr[d], nr[d], &gu, &gp, &gn);
+          pair_grads1<KIND>(g, a.c_l2, orx_ld1(ur + d), orx_ld1(pr + d), orx_ld1(nr + d), &gu, &gp, &gn);
           su += gu * gu;
           sp += gp * gp;
           sn += gn * gn;
@@ -438,14 +445,14 @@ __global__ void __launch_bounds__(256) k_pair_generic(const PairArgs a) {
         const float xu = orx_row_scale(au, su, D, a.opt), xp = orx_row_scale(ap, sp, D, a.opt),
                     xn = orx_row_scale(an, sn, D, a.opt);
         for (int d = lane; d < D; d += 32) {
-          const float u = ur[d], p = pr[d], n = nr[d];
+          const float u = orx_ld1(ur + d), p = orx_ld1(pr + d), n = orx_ld1(nr + d);
           float gu, gp, gn;
           pair_grads1<KIND>(g, a.c_l2, u, p, n, &gu, &gp, &gn);
-          if (fu) ur[d] = orx_row_apply1(u, gu, xu, a.opt);
+          if (fu) orx_st1(ur + d, orx_row_apply1(u, gu, xu, a.opt), rku, d);
           else atomicAdd(a.gu + (int64_t)du * D + d, gu);
-          if (fp) pr[d] = orx_row_apply1(p, gp, xp, a.opt);
+          if (fp) orx_st1(pr + d, orx_row_apply1(p, gp, xp, a.opt), rkp, d);
           else atomicAdd(a.gi + (int64_t)dp * D + d, gp);
-          if (fn) nr[d] = orx_row_apply1(n, gn, xn, a.opt);
+          if (fn) orx_st1(nr + d, orx_row_apply1(n, gn, xn, a.opt), rkn, d);
           else atomicAdd(a.gi + (int64_t)dn * D + d, gn);
         }
         if (lane == 0) {
@@ -459,15 +466,15 @@ __global__ void __launch_bounds__(256) k_pair_generic(const PairArgs a) {
         }
       } else {
         for (int d = lane; d < D; d += 32) {
-          const float u = ur[d], p = pr[d], n = nr[d];
+          const float u = orx_ld1(ur + d), p = orx_ld1(pr + d), n = orx_ld1(nr + d);
           float gu, gp, gn;
           pair_grads1<KIND>(g, a.c_l2, u, p, n, &gu, &gp, &gn);
           const int64_t ou = (int64_t)uu * D + d, op = (int64_t)pp * D + d, on = (int64_t)nn * D + d;
-          if (fu) orx_update1<OPT>(ur + d, a.Us0 + ou, a.Us1 + ou, u, gu, a.opt);
+          if (fu) orx_update1<OPT>(ur + d, a.Us0 + ou, a.Us1 + ou, u, gu, a.opt, rku, d);
           else atomicAdd(a.gu + (int64_t)du * D + d, gu);
-          if (fp) orx_update1<OPT>(pr + d, a.Is0 + op, a.Is1 + op, p, gp, a.opt);
+          if (fp) orx_update1<OPT>(pr + d, a.Is0 + op, a.Is1 + op, p, gp, a.opt, rkp, d);
           else atomicAdd(a.gi + (int64_t)dp * D + d, gp);
-          if (fn) orx_update1<OPT>(nr + d, a.Is0 + on, a.Is1 + on, n, gn, a.opt);
+          if (fn) orx_update1<OPT>(nr + d, a.Is0 + on, a.Is1 + on, n, gn, a.opt, rkn, d);
           else atomicAdd(a.gi + (int64_t)dn * D + d, gn);
         }
         if (lane == 0) {
@@ -482,7 +489,7 @@ __global__ void __launch_bounds__(256) k_pair_generic(const PairArgs a) {
     if (a.d_user || a.d_pos || a.d_neg) {
       for (int d = lane; d < D; d += 32) {
         float gu = 0.f, gp = 0.f, gn = 0.f;
-        if (ok) pair_grads1<KIND>(g, a.c_l2, ur[d], pr[d], nr[d], &gu, &gp, &gn);
+        if (ok) pair_grads1<KIND>(g, a.c_l2, orx_ld1(ur + d), orx_ld1(pr + d), orx_ld1(nr + d), &gu, &gp, &gn);
         if (row_form) {
           if (ok) {
             a.d_user[(int64_t)uu * ld + d] = gu;
@@ -520,8 +527,10 @@ __global__ void __launch_bounds__(256) k_pair_generic(const PairArgs a) {
 // ADAM_DENSE sweep: Keras-2.0 Adam on IndexedSlices touches EVERY row (SURVEY Q5, "K12").
 // One warp per table row; the row's summed gradient comes from the staging buffer via the hash.
 // ---------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_adam_sweep(float* var, float* m, float* v, int64_t rows, int D, OrxHash h,
-                                                    const float* gstage, OrxOptDev o) {
+// T: the table's storage; kt its rounding key (bf16).
+template <typename T>
+__global__ void __launch_bounds__(256) k_adam_sweep(T* var, float* m, float* v, int64_t rows, int D, OrxHash h,
+                                                    const float* gstage, OrxOptDev o, uint32_t kt) {
   const int lane = threadIdx.x & 31;
   const int64_t nw = ((int64_t)gridDim.x * blockDim.x) >> 5;
   for (int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < rows; r += nw) {
@@ -530,8 +539,9 @@ __global__ void __launch_bounds__(256) k_adam_sweep(float* var, float* m, float*
     if (lane == 0) c = orx_hash_find(h, (int32_t)r, &d);
     c = __shfl_sync(ORX_FULL, c, 0);
     d = __shfl_sync(ORX_FULL, d, 0);
+    const uint32_t rk = orx_sr_row(kt, r);
     for (int e = lane; e < D; e += 32)
-      orx_adam_dense1(var, m, v, r * D + e, c ? gstage[(int64_t)d * D + e] : 0.f, o);
+      orx_adam_dense1(var, m, v, r * D + e, c ? gstage[(int64_t)d * D + e] : 0.f, o, rk, e);
   }
 }
 
@@ -540,13 +550,14 @@ __global__ void __launch_bounds__(256) k_adam_sweep(float* var, float* m, float*
 // ---------------------------------------------------------------------------------------
 
 // ta.I == nullptr: no item side (orx_sparse_apply: one table, in the user-side index set); ta.out4 == nullptr: no loss.
-template <int OPT, bool VEC>
+// T: the storage of the user / item tables (float, or bf16 bits with VEC meaning 8-byte aligned rows).
+template <int OPT, bool VEC, typename T = float>
 __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
   __shared__ bool last;
   orx_pdl_wait();
   const int nu = *a.hu.counter, ni = a.I ? *a.hi.counter : 0;
-  if constexpr (OrxOptSlots<OPT>::ROW) orx_tail_rows_rowwise<VEC>(a, nu, ni);
-  else orx_tail_rows<OPT, VEC>(a, nu, ni);
+  if constexpr (OrxOptSlots<OPT>::ROW) orx_tail_rows_rowwise<VEC, T>(a, nu, ni);
+  else orx_tail_rows<OPT, VEC, T>(a, nu, ni);
 
   if (blockIdx.x == 0 && a.out4) {
     // deterministic loss reduction; GMF: l2_loss also holds 0.5*sum(w^2) of the PRE-step weight (gmf.py:31-32)
@@ -579,14 +590,18 @@ __global__ void __launch_bounds__(256) k_sparse_tail(const TailArgs a) {
   if (last && threadIdx.x < 4) a.counters[threadIdx.x] = 0;
 }
 
-int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st) {
+int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t st, bool bf16) {
   const int grid = c->num_sms * 4;  // ~1-2 staged rows per warp: the tail is a latency chain, not bandwidth
-  // a row-wise accumulator is read as scalars: only the table rows decide
-  const bool vec = opt_kind == ORX_OPT_ROWWISE_ADAGRAD ? orx_aligned16(ta.U, ta.I)
-                                                       : orx_aligned16(ta.U, ta.Us0, ta.Us1, ta.I, ta.Is0, ta.Is1);
+  // a row-wise accumulator is read as scalars: only the table rows decide; bf16 rows move 8 bytes at a time
+  const bool rows_ok = bf16 ? orx_aligned8(ta.U, ta.I) : orx_aligned16(ta.U, ta.I);
+  const bool vec = opt_kind == ORX_OPT_ROWWISE_ADAGRAD ? rows_ok : rows_ok && orx_aligned16(ta.Us0, ta.Us1, ta.Is0, ta.Is1);
   orx_dispatch_opt(opt_kind, [&](auto O) {
     orx_dispatch<0, 1>(vec ? 1 : 0, [&](auto V) {
-      orx_launch_pdl(k_sparse_tail<decltype(O)::value, decltype(V)::value == 1>, dim3(grid), dim3(256), 0, st, ta);
+      if (bf16)
+        orx_launch_pdl(k_sparse_tail<decltype(O)::value, decltype(V)::value == 1, uint16_t>, dim3(grid), dim3(256), 0,
+                       st, ta);
+      else
+        orx_launch_pdl(k_sparse_tail<decltype(O)::value, decltype(V)::value == 1>, dim3(grid), dim3(256), 0, st, ta);
     });
   });
   ORX_LAUNCH_CHECK();
@@ -594,16 +609,20 @@ int orx_launch_tail(orx_ctx* c, const TailArgs& ta, int opt_kind, cudaStream_t s
 }
 
 int orx_launch_adam_sweeps(orx_ctx* c, const orx_table_t* user, const orx_table_t* item, const orx_table_t* bias,
-                           const OrxIndexSet& ix, const OrxOptDev& o, cudaStream_t st) {
-  struct { const orx_table_t* t; int D; const OrxHash* h; const float* g; } sw[3] = {
-      {user, user->dim, &ix.u, c->gu}, {item, user->dim, &ix.i, c->gi}, {bias, 1, &ix.i, c->gb}};
+                           const OrxIndexSet& ix, const OrxOptDev& o, cudaStream_t st, const uint32_t* srk) {
+  struct { const orx_table_t* t; int D; const OrxHash* h; const float* g; int k; } sw[3] = {
+      {user, user->dim, &ix.u, c->gu, 0}, {item, user->dim, &ix.i, c->gi, 1}, {bias, 1, &ix.i, c->gb, -1}};
   for (const auto& s : sw) {
     if (!s.t) continue;
     int64_t blocks = (s.t->rows + 7) / 8;
     const int64_t cap = (int64_t)c->num_sms * 16;
     if (blocks > cap) blocks = cap;
     if (blocks < 1) blocks = 1;
-    k_adam_sweep<<<(int)blocks, 256, 0, st>>>(s.t->var, s.t->s0, s.t->s1, s.t->rows, s.D, *s.h, s.g, o);
+    if (srk && s.k >= 0)   // a bf16 user / item table (the bias is float)
+      k_adam_sweep<<<(int)blocks, 256, 0, st>>>(reinterpret_cast<uint16_t*>(s.t->var), s.t->s0, s.t->s1, s.t->rows,
+                                                s.D, *s.h, s.g, o, srk[s.k]);
+    else
+      k_adam_sweep<<<(int)blocks, 256, 0, st>>>(s.t->var, s.t->s0, s.t->s1, s.t->rows, s.D, *s.h, s.g, o, 0u);
     ORX_LAUNCH_CHECK();
   }
   return ORX_OK;
@@ -641,7 +660,9 @@ int orx_check_step_tables(const orx_table_t* user, const orx_table_t* item, cons
 // "last arriver applies" form without the tail launch were all slower and are gone).  Re-checked on H100 SXM (700 W)
 // with the L2 priorities of k_pair_step in place, BPR Adagrad at the bench shape: CH = 16 measured the same as CH = 8,
 // 3 CTAs/SM was 1 % slower, and the register double-buffer (PIPE) 1-2 % slower at 2 or 3 CTAs/SM.
-template <int KIND, int OPT>
+// T = uint16_t: bf16 user / item tables, which take the same variants (and, like fp32, k_pair_generic when a table's
+// base is off the boundary its row path needs: 8 bytes for bf16 rows, 16 for float slot rows).
+template <int KIND, int OPT, typename T = float>
 static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, OrxStepLaunch* out) {
   constexpr bool LAZY = (OPT == ORX_OPT_ADAM_LAZY);  // 9 rows per triplet: no register double-buffer
   const int blocks = orx_step_blocks(pa.B);
@@ -659,20 +680,26 @@ static int launch_pair_step_kind_opt(const PairArgs& pa, cudaStream_t st, OrxSte
   // ROWWISE_ADAGRAD reads its accumulators as scalars, so only the tables decide; it holds three accumulator scalars
   // (and the rows' gradients over the row sum) where ADAGRAD holds 3K float4 slot registers, and takes ADAGRAD's
   // variants: PIPE at D = 32, 64, 256, four CTAs/SM without PIPE at D = 128 (no spills under -Xptxas -v).
-  const bool vec = OrxOptSlots<OPT>::ROW ? orx_aligned16(pa.U, pa.I)
-                                         : orx_aligned16(pa.U, pa.Us0, pa.Us1, pa.I, pa.Is0, pa.Is1);
+  // bf16 rows add the rounding's hashes to the live values: under -Xptxas -v ADAGRAD spills at four CTAs/SM at D = 128
+  // and with PIPE at D = 256, and LAZY at three CTAs/SM at D = 128.  bf16 ADAGRAD therefore takes MOMENTUM's variants
+  // and bf16 LAZY two CTAs/SM at D = 128.
+  constexpr bool BF = std::is_same<T, uint16_t>::value;
+  constexpr bool ADA = (OPT == ORX_OPT_ADAGRAD);
+  const bool rows_ok = BF ? orx_aligned8(pa.U, pa.I) : orx_aligned16(pa.U, pa.I);
+  const bool vec = OrxOptSlots<OPT>::ROW ? rows_ok : rows_ok && orx_aligned16(pa.Us0, pa.Us1, pa.Is0, pa.Is1);
   switch (vec ? pa.D : 0) {
-    case 32: go(k_pair_step<KIND, OPT, 32, 8, 2, !LAZY>, PV, 2, blocks); break;
-    case 64: go(k_pair_step<KIND, OPT, 64, 8, 2, !LAZY>, PV, 2, blocks); break;
+    case 32: go(k_pair_step<KIND, OPT, 32, 8, 2, !LAZY, T>, PV, 2, blocks); break;
+    case 64: go(k_pair_step<KIND, OPT, 64, 8, 2, !LAZY, T>, PV, 2, blocks); break;
     case 128:
-      if constexpr (LAZY || MOM) go(k_pair_step<KIND, OPT, 128, 8, 3, false>, ORX_VARIANT_STEP, 3, blocks);
-      else go(k_pair_step<KIND, OPT, 128, 8, 4, false>, ORX_VARIANT_STEP, 4, blocks);
+      if constexpr (BF && LAZY) go(k_pair_step<KIND, OPT, 128, 8, 2, false, T>, ORX_VARIANT_STEP, 2, blocks);
+      else if constexpr (LAZY || MOM || (BF && ADA)) go(k_pair_step<KIND, OPT, 128, 8, 3, false, T>, ORX_VARIANT_STEP, 3, blocks);
+      else go(k_pair_step<KIND, OPT, 128, 8, 4, false, T>, ORX_VARIANT_STEP, 4, blocks);
       break;
     case 256:
-      if constexpr (MOM) go(k_pair_step<KIND, OPT, 256, 8, 2, false>, ORX_VARIANT_STEP, 2, blocks);
-      else go(k_pair_step<KIND, OPT, 256, 8, 2, !LAZY>, PV, 2, blocks);
+      if constexpr (MOM || (BF && ADA)) go(k_pair_step<KIND, OPT, 256, 8, 2, false, T>, ORX_VARIANT_STEP, 2, blocks);
+      else go(k_pair_step<KIND, OPT, 256, 8, 2, !LAZY, T>, PV, 2, blocks);
       break;
-    default: go(k_pair_generic<KIND, OPT, 0>, ORX_VARIANT_STEP_GENERIC, 0, 8 * blocks); break;
+    default: go(k_pair_generic<KIND, OPT, 0, T>, ORX_VARIANT_STEP_GENERIC, 0, 8 * blocks); break;
   }
   ORX_LAUNCH_CHECK();
   return ORX_OK;
@@ -768,7 +795,7 @@ extern "C" int orx_debug_pair_records(orx_handle_t h, int32_t set, int32_t* rec,
 int orx_sparse_step(orx_ctx* c, int op, int kind, const orx_table_t* user, const orx_table_t* item,
                     const orx_table_t* bias, const orx_table_t* w, const int32_t* uid, const int32_t* iid,
                     const int32_t* nid, int B, const orx_opt_t* opt, float loss_scale, float c_l2, float* out4,
-                    const OrxStepKernel& kernel, cudaStream_t st) {
+                    const OrxStepKernel& kernel, cudaStream_t st, const uint32_t* srk) {
   ORX_REQUIRE(opt != nullptr && out4 != nullptr, "null opt/out");
   ORX_REQUIRE(orx_opt_kind_ok(opt->kind), "unknown optimizer kind");
   ORX_REQUIRE(B > 0 && uid && iid, "empty batch or null ids");
@@ -794,19 +821,20 @@ int orx_sparse_step(orx_ctx* c, int op, int kind, const orx_table_t* user, const
   }
   OrxIndexSet& ix = c->set[set];
   orx_prof_mark(c, 1, st);
-  const SparseArgs s = orx_sparse_args(c, user, item, bias, ix, orx_opt_to_dev(opt));
+  SparseArgs s = orx_sparse_args(c, user, item, bias, ix, orx_opt_to_dev(opt));
+  if (srk) { s.srk[0] = srk[0]; s.srk[1] = srk[1]; }
   OrxStepLaunch L = {};
   if ((rc = kernel(s, ix.res, c->partials, &L))) return rc;   // set 0 has no records
   orx_log_dispatch(c, op, L.variant, kind, opt->kind, B, D, L.minb, set);
   orx_prof_mark(c, 2, st);
-  if (dense && (rc = orx_launch_adam_sweeps(c, user, item, bias, ix, s.opt, st))) return rc;
+  if (dense && (rc = orx_launch_adam_sweeps(c, user, item, bias, ix, s.opt, st, srk))) return rc;
   TailArgs ta = {s};
   ta.partials = c->partials; ta.n_partials = L.n_partials; ta.loss_scale = loss_scale;
   ta.counters = ix.ctl; ta.out4 = out4;
   if (w) {
     ta.W = w->var; ta.Ws0 = w->s0; ta.Ws1 = w->s1; ta.gw = c->gw; ta.c_l2 = c_l2;
   }
-  rc = orx_launch_tail(c, ta, opt->kind, st);
+  rc = orx_launch_tail(c, ta, opt->kind, st, srk != nullptr);
   if (set) {   // the prefetch set is free again once this tail has run
     ORX_CUDA(cudaEventRecord(ix.free, st));
     ix.free_valid = 1;
@@ -826,10 +854,11 @@ static PairArgs pair_args(const SparseArgs& s, int64_t rows_u, int64_t rows_i, c
   return pa;
 }
 
+// srk: bf16 user / item tables with these rounding keys (their var passed as float*), null: float tables
 static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, const orx_table_t* item,
                               const orx_table_t* bias, const int32_t* uid, const int32_t* pid, const int32_t* nid,
                               int B, float margin, float c_loss, float c_l2, const orx_opt_t* opt, float* out4,
-                              cudaStream_t st) {
+                              cudaStream_t st, const uint32_t* srk = nullptr) {
   ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
   ORX_REQUIRE(nid != nullptr, "empty batch or null ids");
   orx_opt_t od;
@@ -844,12 +873,21 @@ static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, con
     pa.res = res;   // k_pair_generic probes the index whatever res is
     return orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {
       return orx_dispatch_opt(opt->kind, [&](auto O) {
+        if (srk) return launch_pair_step_kind_opt<decltype(K)::value, decltype(O)::value, uint16_t>(pa, st, out);
         return launch_pair_step_kind_opt<decltype(K)::value, decltype(O)::value>(pa, st, out);
       });
     });
   };
-  return orx_sparse_step(c, ORX_OP_PAIRWISE_STEP, kind, user, item, bias, nullptr, uid, pid, nid, B, opt,
-                         kind == ORX_PAIR_BPR ? inv_B : 1.0f, c_l2, out4, kernel, st);
+  return orx_sparse_step(c, srk ? ORX_OP_PAIRWISE_STEP_BF16 : ORX_OP_PAIRWISE_STEP, kind, user, item, bias, nullptr,
+                         uid, pid, nid, B, opt, kind == ORX_PAIR_BPR ? inv_B : 1.0f, c_l2, out4, kernel, st, srk);
+}
+
+// A bf16 table as the orx_table_t the shared host code takes: var carries the bf16 rows' address, and every kernel that
+// reads it is instantiated for uint16_t storage.  A null table stays null (the shared checks refuse it).
+static const orx_table_t* bf16_table(const orx_table_bf16_t* b, orx_table_t* t) {
+  if (!b) return nullptr;
+  *t = {reinterpret_cast<float*>(b->var), b->s0, b->s1, b->rows, b->dim};
+  return t;
 }
 
 extern "C" int orx_pairwise_step(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
@@ -862,13 +900,26 @@ extern "C" int orx_pairwise_step(orx_handle_t h, int32_t kind, const orx_table_t
                             (cudaStream_t)s);
 }
 
+extern "C" int orx_pairwise_step_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                      const orx_table_bf16_t* item, const orx_table_t* item_bias, const int32_t* uid,
+                                      const int32_t* pid, const int32_t* nid, int32_t B, float margin, float c_loss,
+                                      float c_l2, const orx_opt_t* opt, uint64_t sr_seed, float* out4, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr, "null handle");
+  ORX_REQUIRE(opt != nullptr, "null opt/out");
+  ORX_CUDA(cudaSetDevice(h->device));
+  orx_table_t tu, ti;
+  const uint32_t srk[2] = {orx_sr_table_key(sr_seed, opt->step, 0), orx_sr_table_key(sr_seed, opt->step, 1)};
+  return pairwise_step_impl(h, kind, bf16_table(user, &tu), bf16_table(item, &ti), item_bias, uid, pid, nid, B, margin,
+                            c_loss, c_l2, opt, out4, (cudaStream_t)s, srk);
+}
+
 // Host-buffer form: the upload of this batch's ids and its index build run on the side stream, i.e. under the previous
 // step's kernels whenever the caller enqueues ahead of the GPU; the step kernels and the read-back of out4 stay on `s`.
 // The id staging buffers alternate; buffer f is reused only after the step that read it has finished (stage_free[f]).
-extern "C" int orx_pairwise_step_host(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
-                                      const orx_table_t* item_bias, const int32_t* uid_host, const int32_t* pid_host,
-                                      const int32_t* nid_host, int32_t B, float margin, float c_loss, float c_l2,
-                                      const orx_opt_t* opt, float* out4_host, orx_stream_t s) {
+static int pairwise_step_host_impl(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
+                                   const orx_table_t* item_bias, const int32_t* uid_host, const int32_t* pid_host,
+                                   const int32_t* nid_host, int32_t B, float margin, float c_loss, float c_l2,
+                                   const orx_opt_t* opt, float* out4_host, orx_stream_t s, const uint32_t* srk) {
   ORX_REQUIRE(h != nullptr, "null handle");
   ORX_REQUIRE(B > 0 && uid_host && pid_host && nid_host && out4_host && user && item && opt, "empty batch or null host buffers");
   ORX_CUDA(cudaSetDevice(h->device));
@@ -891,12 +942,32 @@ extern "C" int orx_pairwise_step_host(orx_handle_t h, int32_t kind, const orx_ta
                            opt->kind == ORX_OPT_ADAM_DENSE ? 1 : 0)))
     return rc;
   rc = pairwise_step_impl(h, kind, user, item, item_bias, ids, ids + B, ids + 2 * (int64_t)B, B, margin, c_loss, c_l2,
-                          opt, h->out_stage[f], st);
+                          opt, h->out_stage[f], st, srk);
   if (rc) return rc;
   ORX_CUDA(cudaEventRecord(h->stage_free[f], st));
   h->stage_free_valid[f] = 1;
   ORX_CUDA(cudaMemcpyAsync(out4_host, h->out_stage[f], sizeof(float) * 4, cudaMemcpyDeviceToHost, st));
   return ORX_OK;
+}
+
+extern "C" int orx_pairwise_step_host(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
+                                      const orx_table_t* item_bias, const int32_t* uid_host, const int32_t* pid_host,
+                                      const int32_t* nid_host, int32_t B, float margin, float c_loss, float c_l2,
+                                      const orx_opt_t* opt, float* out4_host, orx_stream_t s) {
+  return pairwise_step_host_impl(h, kind, user, item, item_bias, uid_host, pid_host, nid_host, B, margin, c_loss, c_l2,
+                                 opt, out4_host, s, nullptr);
+}
+
+extern "C" int orx_pairwise_step_host_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                           const orx_table_bf16_t* item, const orx_table_t* item_bias,
+                                           const int32_t* uid_host, const int32_t* pid_host, const int32_t* nid_host,
+                                           int32_t B, float margin, float c_loss, float c_l2, const orx_opt_t* opt,
+                                           uint64_t sr_seed, float* out4_host, orx_stream_t s) {
+  ORX_REQUIRE(opt != nullptr, "empty batch or null host buffers");
+  orx_table_t tu, ti;
+  const uint32_t srk[2] = {orx_sr_table_key(sr_seed, opt->step, 0), orx_sr_table_key(sr_seed, opt->step, 1)};
+  return pairwise_step_host_impl(h, kind, bf16_table(user, &tu), bf16_table(item, &ti), item_bias, uid_host, pid_host,
+                                 nid_host, B, margin, c_loss, c_l2, opt, out4_host, s, srk);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -932,11 +1003,13 @@ int orx_sparse_unfused(orx_ctx* c, int B, float loss_scale, float* out4,
 
 // k_pair_generic MODE 1 over the batch of pa (kind already validated) and, when out4 is given, its (loss, l2) reduced
 // into out4: the loss scaled by inv_B for BPR (mean), summed for UCML.
-static int pair_unfused(orx_ctx* c, int kind, PairArgs pa, float* out4, cudaStream_t st) {
+// bf16: the user / item tables of pa are bf16.
+static int pair_unfused(orx_ctx* c, int kind, PairArgs pa, float* out4, cudaStream_t st, bool bf16 = false) {
   const auto launch = [&](float* partials, int blocks) {
     pa.partials = partials;
     orx_dispatch<ORX_PAIR_BPR, ORX_PAIR_UCML>(kind, [&](auto K) {
-      k_pair_generic<decltype(K)::value, ORX_OPT_SGD, 1><<<blocks, 256, 0, st>>>(pa);
+      if (bf16) k_pair_generic<decltype(K)::value, ORX_OPT_SGD, 1, uint16_t><<<blocks, 256, 0, st>>>(pa);
+      else k_pair_generic<decltype(K)::value, ORX_OPT_SGD, 1><<<blocks, 256, 0, st>>>(pa);
     });
   };
   return orx_sparse_unfused(c, pa.B, kind == ORX_PAIR_BPR ? pa.inv_B : 1.f, out4, launch, st);
@@ -945,7 +1018,7 @@ static int pair_unfused(orx_ctx* c, int kind, PairArgs pa, float* out4, cudaStre
 static int pair_fwd_grad(orx_ctx* c, int kind, const orx_table_t* user, const orx_table_t* item,
                          const orx_table_t* bias, const int32_t* uid, const int32_t* pid, const int32_t* nid, int B,
                          float margin, float c_loss, float c_l2, float* d_user, float* d_pos, float* d_neg,
-                         float* d_bp, float* d_bn, float* g_out, float* out4, cudaStream_t st) {
+                         float* d_bp, float* d_bn, float* g_out, float* out4, cudaStream_t st, bool bf16 = false) {
   ORX_REQUIRE(kind == ORX_PAIR_BPR || kind == ORX_PAIR_UCML, "unknown pairwise kind");
   ORX_REQUIRE(B > 0 && uid && pid && nid, "empty batch or null ids");
   int rc = orx_check_step_tables(user, item, bias, nullptr, ORX_OPT_SGD);
@@ -953,7 +1026,7 @@ static int pair_fwd_grad(orx_ctx* c, int kind, const orx_table_t* user, const or
   const SparseArgs s = orx_sparse_args(c, user, item, bias, c->set[0], OrxOptDev{});
   PairArgs a = pair_args(s, user->rows, item->rows, uid, pid, nid, B, margin, c_loss, c_l2, 1.0f / (float)B);
   a.d_user = d_user; a.d_pos = d_pos; a.d_neg = d_neg; a.d_bp = d_bp; a.d_bn = d_bn; a.g_out = g_out;
-  return pair_unfused(c, kind, a, out4, st);
+  return pair_unfused(c, kind, a, out4, st, bf16);
 }
 
 extern "C" int orx_pairwise_fwd(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
@@ -973,6 +1046,47 @@ extern "C" int orx_pairwise_grad(orx_handle_t h, int32_t kind, const orx_table_t
   ORX_CUDA(cudaSetDevice(h->device));
   return pair_fwd_grad(h, kind, user, item, item_bias, uid, pid, nid, B, margin, c_loss, c_l2, d_user, d_pos, d_neg,
                        d_bp, d_bn, g_out, nullptr, (cudaStream_t)s);
+}
+
+extern "C" int orx_pairwise_fwd_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                     const orx_table_bf16_t* item, const orx_table_t* item_bias, const int32_t* uid,
+                                     const int32_t* pid, const int32_t* nid, int32_t B, float margin, float* out4,
+                                     orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr && out4 != nullptr, "null handle/out");
+  ORX_CUDA(cudaSetDevice(h->device));
+  orx_table_t tu, ti;
+  return pair_fwd_grad(h, kind, bf16_table(user, &tu), bf16_table(item, &ti), item_bias, uid, pid, nid, B, margin, 1.f,
+                       1.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out4, (cudaStream_t)s, true);
+}
+
+extern "C" int orx_pairwise_grad_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                      const orx_table_bf16_t* item, const orx_table_t* item_bias, const int32_t* uid,
+                                      const int32_t* pid, const int32_t* nid, int32_t B, float margin, float c_loss,
+                                      float c_l2, float* d_user, float* d_pos, float* d_neg, float* d_bp, float* d_bn,
+                                      float* g_out, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr, "null handle");
+  ORX_CUDA(cudaSetDevice(h->device));
+  orx_table_t tu, ti;
+  return pair_fwd_grad(h, kind, bf16_table(user, &tu), bf16_table(item, &ti), item_bias, uid, pid, nid, B, margin,
+                       c_loss, c_l2, d_user, d_pos, d_neg, d_bp, d_bn, g_out, nullptr, (cudaStream_t)s, true);
+}
+
+// test hook: the stochastic rounding of include/orx.h applied to n floats, element i at (row0 + i / dim, i % dim)
+__global__ void k_debug_round_bf16(const float* x, uint16_t* out, int64_t n, int64_t row0, int dim, uint32_t kt) {
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] = (uint16_t)orx_bf16_sr(x[i], orx_sr_row(kt, row0 + i / dim), (int)(i % dim));
+}
+
+extern "C" int orx_debug_round_bf16(orx_handle_t h, const float* x, uint16_t* out, int64_t n, int64_t row0,
+                                    int32_t dim, int32_t table, uint64_t sr_seed, int64_t step, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr && x && out, "null pointer");
+  ORX_REQUIRE(n >= 0 && dim > 0 && row0 >= 0 && (table == 0 || table == 1), "bad arguments");
+  if (n == 0) return ORX_OK;
+  ORX_CUDA(cudaSetDevice(h->device));
+  k_debug_round_bf16<<<orx_grid_for(n, 256, h->num_sms), 256, 0, (cudaStream_t)s>>>(
+      x, out, n, row0, dim, orx_sr_table_key(sr_seed, step, table));
+  ORX_LAUNCH_CHECK();
+  return ORX_OK;
 }
 
 extern "C" int orx_pairwise_grad_rows(orx_handle_t h, int32_t kind, const float* rows, int64_t ld, int32_t dim,

@@ -16,7 +16,7 @@ from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP
                    ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
                    ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE,
                    ORX_VARIANT_TOPK, ORX_OP_CROSS, ORX_VARIANT_CROSS_VEC, ORX_VARIANT_CROSS_SCALAR, ORX_CROSS_TOP,
-                   ORX_CROSS_MID, ORX_CROSS_FINAL, OrxOpt, OrxTable)
+                   ORX_CROSS_MID, ORX_CROSS_FINAL, ORX_OP_PAIRWISE_STEP_BF16, OrxOpt, OrxTable, OrxTableBf16)
 
 __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", "ORX_POINT_GMF", "ORX_POINT_WRMF",
            "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_OPT_ROWWISE_ADAGRAD",
@@ -28,6 +28,7 @@ __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", 
            "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "ORX_OP_SCORE_TOPK_SHARD", "ORX_OP_POINTWISE_GRAD_ROWS",
            "ORX_OP_CENSOR_SHARD", "ORX_VARIANT_CENSOR_VEC", "ORX_VARIANT_CENSOR_SCALAR", "ORX_OP_CROSS",
            "ORX_VARIANT_CROSS_VEC", "ORX_VARIANT_CROSS_SCALAR", "ORX_CROSS_TOP", "ORX_CROSS_MID", "ORX_CROSS_FINAL",
+           "ORX_OP_PAIRWISE_STEP_BF16", "table_bf16", "as_table",
            "Dispatch", "RowShard", "rowshard", "shard_rows"]
 
 _engines = {}
@@ -83,6 +84,28 @@ def table(var, s0=None, s1=None, kind=None):
                          f"got {tuple(s0.shape)}")
     return OrxTable(var.data_ptr(), s0.data_ptr() if s0 is not None else None,
                     s1.data_ptr() if s1 is not None else None, rows, dim)
+
+
+def _bf16(t, name):
+    if not (t.is_cuda and t.dtype == torch.bfloat16 and t.is_contiguous()):
+        raise ValueError(f"{name}: expected a contiguous bfloat16 CUDA tensor")
+    return t
+
+
+def table_bf16(var, s0=None, s1=None, kind=None):
+    """orx_table_bf16_t for a bfloat16 [rows, dim] variable and its float32 optimizer slots (checked as in table)."""
+    _bf16(var, "var"), _f32(s0, "s0"), _f32(s1, "s1")
+    rows, dim = var.shape[0], var.shape[1]
+    if kind == ORX_OPT_ROWWISE_ADAGRAD and s0 is not None and tuple(s0.shape) not in ((rows,), (rows, 1)):
+        raise ValueError(f"s0: a row-wise Adagrad accumulator has one element per row, shape ({rows},) or ({rows}, 1), "
+                         f"got {tuple(s0.shape)}")
+    return OrxTableBf16(var.data_ptr(), s0.data_ptr() if s0 is not None else None,
+                        s1.data_ptr() if s1 is not None else None, rows, dim)
+
+
+def as_table(t):
+    """The orx_table_t with the fields of an orx_table_bf16_t t (orx_pairwise_prefetch reads its rows and dim)."""
+    return t if isinstance(t, OrxTable) else OrxTable(t.var, t.s0, t.s1, t.rows, t.dim)
 
 
 def opt(kind, lr, eps=1e-7, beta1=0.9, beta2=0.999, step=1):
@@ -189,10 +212,52 @@ class Engine:
                                                    c_loss, c_l2, C.byref(o), _ptr(out4_h), self.stream()),
                    "orx_pairwise_step_host")
 
+    def pairwise_step_bf16(self, kind, user, item, bias, uid, pid, nid, o, sr_seed, out4, margin=0.5, c_loss=1.0,
+                           c_l2=1.0):
+        """pairwise_step on bf16 user / item tables (table_bf16), rounding seeded with sr_seed."""
+        _lib.check(self.lib.orx_pairwise_step_bf16(self.h, kind, C.byref(user), C.byref(item), C.byref(bias), _ptr(uid),
+                                                   _ptr(pid), _ptr(nid), uid.numel(), margin, c_loss, c_l2, C.byref(o),
+                                                   int(sr_seed), _ptr(out4), self.stream()), "orx_pairwise_step_bf16")
+
+    def pairwise_step_host_bf16(self, kind, user, item, bias, uid_h, pid_h, nid_h, o, sr_seed, out4_h, margin=0.5,
+                                c_loss=1.0, c_l2=1.0):
+        _lib.check(self.lib.orx_pairwise_step_host_bf16(self.h, kind, C.byref(user), C.byref(item), C.byref(bias),
+                                                        _ptr(uid_h), _ptr(pid_h), _ptr(nid_h), uid_h.numel(), margin,
+                                                        c_loss, c_l2, C.byref(o), int(sr_seed), _ptr(out4_h),
+                                                        self.stream()), "orx_pairwise_step_host_bf16")
+
+    def pairwise_fwd_bf16(self, kind, user, item, bias, uid, pid, nid, out4, margin=0.5):
+        _lib.check(self.lib.orx_pairwise_fwd_bf16(self.h, kind, C.byref(user), C.byref(item), C.byref(bias), _ptr(uid),
+                                                  _ptr(pid), _ptr(nid), uid.numel(), margin, _ptr(out4),
+                                                  self.stream()), "orx_pairwise_fwd_bf16")
+
+    def pairwise_grad_bf16(self, kind, user, item, bias, uid, pid, nid, margin=0.5, c_loss=1.0, c_l2=1.0, *,
+                           d_user=None, d_pos=None, d_neg=None, d_bp=None, d_bn=None, g_out=None):
+        _lib.check(self.lib.orx_pairwise_grad_bf16(self.h, kind, C.byref(user), C.byref(item), C.byref(bias), _ptr(uid),
+                                                   _ptr(pid), _ptr(nid), uid.numel(), margin, c_loss, c_l2,
+                                                   _ptr(d_user), _ptr(d_pos), _ptr(d_neg), _ptr(d_bp), _ptr(d_bn),
+                                                   _ptr(g_out), self.stream()), "orx_pairwise_grad_bf16")
+
+    def censor_bf16(self, tab, ids, min_norm=0.1):
+        ids = ids32(ids)
+        _lib.check(self.lib.orx_censor_bf16(self.h, _ptr(_bf16(tab, "tab")), tab.shape[0], tab.shape[1], _ptr(ids),
+                                            ids.numel(), min_norm, self.stream()), "orx_censor_bf16")
+
+    def debug_round_bf16(self, x, row0, dim, table, sr_seed, step):
+        """-> bfloat16 tensor: the stochastic rounding of bf16 tables applied to the float32 CUDA tensor x, element i
+        taken as (row0 + i // dim, i % dim) of table `table` (0 user, 1 item) at (sr_seed, step)."""
+        x = _f32(x, "x")
+        out = torch.empty(x.shape, dtype=torch.bfloat16, device=x.device)
+        _lib.check(self.lib.orx_debug_round_bf16(self.h, _ptr(x), _ptr(out), x.numel(), int(row0), int(dim),
+                                                 int(table), int(sr_seed), int(step), self.stream()),
+                   "orx_debug_round_bf16")
+        return out
+
     def pairwise_prefetch(self, user, item, uid, pid, nid, opt_kind, ids_ready=False):
         """Pipelining hint: build the batch index of these id tensors on the side stream now (the next pairwise_step
         with these very tensors consumes it).  ids_ready=True: the tensors are already complete (pre-staged batches),
         so the build does not wait for anything queued on the current stream."""
+        user, item = as_table(user), as_table(item)
         _lib.check(self.lib.orx_pairwise_prefetch(self.h, C.byref(user), C.byref(item), _ptr(uid), _ptr(pid), _ptr(nid),
                                                   uid.numel(), opt_kind, 1 if ids_ready else 0, self.stream()),
                    "orx_pairwise_prefetch")

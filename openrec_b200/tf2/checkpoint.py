@@ -7,7 +7,11 @@ Format: one ``.npz`` with ``var/<k>`` in ``model.variables`` order and their ``n
 A Keras model creates its Dense layers during the first call, so an un-called DLRM / GMF does not have all of its
 variables yet: saving or loading such a model would silently drop the MLP weights.  Both directions therefore insist
 that the variable lists match (count, names, shapes); ``load(..., build=fn)`` lets the caller run one forward call
-(``fn()``) first when the model is fresh."""
+(``fn()``) first when the model is fresh.
+
+A bfloat16 table (``embedding_dtype="bfloat16"``) is saved as its raw 16-bit words (uint16) with ``dtype/<k>`` =
+"bfloat16", so a round trip is bit-exact; loading it into a float32 variable, or a float32 one into a bfloat16 variable,
+is refused."""
 from __future__ import annotations
 
 import numpy as np
@@ -24,13 +28,23 @@ def _unbuilt(model):
     return out
 
 
+def _dtype(v):
+    return "bfloat16" if v.t.dtype == torch.bfloat16 else "float32"
+
+
+def _words(v):
+    """the raw bf16 bits of a bfloat16 variable, as uint16"""
+    return v.t.detach().view(torch.int16).cpu().numpy().view(np.uint16)
+
+
 def save(path, model, optimizer=None):
     pending = _unbuilt(model)
     if pending:
         raise ValueError(f"checkpoint.save: {pending} have no variables yet (call the model once first); a checkpoint "
                          "written now would silently lack them")
     variables = model.variables
-    out = {f"var/{k}": v.numpy() for k, v in enumerate(variables)}
+    out = {f"var/{k}": _words(v) if _dtype(v) == "bfloat16" else v.numpy() for k, v in enumerate(variables)}
+    out.update({f"dtype/{k}": np.array("bfloat16") for k, v in enumerate(variables) if _dtype(v) == "bfloat16"})
     out["names"] = np.array([v.name for v in variables])
     if optimizer is not None:
         out["iterations"] = np.int64(optimizer.iterations)
@@ -58,6 +72,9 @@ def load(path, model, optimizer=None, build=None):
             raise ValueError(f"checkpoint variable {k} is {names[k]!r}, the model's is {v.name!r}")
         if tuple(a.shape) != tuple(v.shape):
             raise ValueError(f"checkpoint variable {k} has shape {a.shape}, model expects {tuple(v.shape)}")
+        saved = str(data[f"dtype/{k}"]) if f"dtype/{k}" in data.files else "float32"
+        if saved != _dtype(v):
+            raise ValueError(f"checkpoint variable {k} ({v.name!r}) is {saved}, the model's is {_dtype(v)}")
     slots = []
     if optimizer is not None and "iterations" in data.files:
         # copy_ broadcasts: a row-wise [rows] accumulator would silently fill an element-wise [rows, dim] one
@@ -71,7 +88,10 @@ def load(path, model, optimizer=None, build=None):
                                          f"{type(optimizer).__name__} expects {tuple(s[j].shape)}")
                     slots.append((s[j], data[key]))
     for k, v in enumerate(variables):
-        v.assign(data[f"var/{k}"])
+        if _dtype(v) == "bfloat16":
+            v.t.view(torch.int16).copy_(torch.from_numpy(data[f"var/{k}"].view(np.int16)))
+        else:
+            v.assign(data[f"var/{k}"])
     if optimizer is not None and "iterations" in data.files:
         optimizer.iterations = int(data["iterations"])
         for s, a in slots:

@@ -81,7 +81,7 @@ class FusedRecommender(Model):
             return ent[0]
         vs = (self.user_latent_factor.embeddings, self.item_latent_factor.embeddings, self.item_bias.embeddings)
         if optimizer is None:
-            ent = (tuple(N.table(v.t) for v in vs), None, None)
+            ent = (tuple((N.table_bf16 if v.t.dtype == torch.bfloat16 else N.table)(v.t) for v in vs), None, None)
         else:
             import weakref
             ent = (tuple(optimizer.table(v) for v in vs), weakref.ref(optimizer), [optimizer.slots(v) for v in vs])

@@ -7,18 +7,32 @@ from ..modules import LatentFactor, PairwiseLogLoss
 from ._base import FusedRecommender, ids_any, ids_of
 
 
+def _check_dtype(embedding_dtype):
+    if embedding_dtype not in ("float32", "bfloat16"):
+        raise ValueError(f"embedding_dtype must be 'float32' or 'bfloat16', got {embedding_dtype!r}")
+    return embedding_dtype
+
+
 class BPR(FusedRecommender):
+    """``embedding_dtype="bfloat16"`` stores the user and item tables in bfloat16 (the item bias and every optimizer
+    slot stay float32); each step rounds its updates stochastically, seeded by ``rounding_seed`` and the optimizer's
+    iteration count, so a run is reproducible bit for bit."""
     _kind = N.ORX_PAIR_BPR
     _score = N.ORX_SCORE_DOT
 
-    def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items):
+    def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items, embedding_dtype="float32",
+                 rounding_seed=0):
         super().__init__()
+        self.embedding_dtype, self.rounding_seed = _check_dtype(embedding_dtype), int(rounding_seed)
         self.user_latent_factor = LatentFactor(num_instances=total_users, dim=dim_user_embed,
-                                               name="user_latent_factor")
+                                               name="user_latent_factor", dtype=embedding_dtype)
         self.item_latent_factor = LatentFactor(num_instances=total_items, dim=dim_item_embed,
-                                               name="item_latent_factor")
+                                               name="item_latent_factor", dtype=embedding_dtype)
         self.item_bias = LatentFactor(num_instances=total_items, dim=1, name="item_bias")
         self.pairwise_log_loss = PairwiseLogLoss()
+
+    def _bf16(self):
+        return self.embedding_dtype == "bfloat16"
 
     def _get_margin(self):
         return 0.0
@@ -35,9 +49,15 @@ class BPR(FusedRecommender):
 
     # ---- kernels behind the step protocol
     def _orx_forward(self, node):
-        N.engine().pairwise_fwd(self._kind, *self._tables(), *self._device_ids(node), node.out, self._get_margin())
+        fwd = N.engine().pairwise_fwd_bf16 if self._bf16() else N.engine().pairwise_fwd
+        fwd(self._kind, *self._tables(), *self._device_ids(node), node.out, self._get_margin())
 
     def _orx_run_step(self, node, optimizer, c_loss, c_l2):
+        if self._bf16():
+            N.engine().pairwise_step_bf16(self._kind, *self._tables(optimizer), *self._device_ids(node),
+                                          optimizer.opt_struct(), self.rounding_seed, node.out, self._get_margin(),
+                                          c_loss, c_l2)
+            return
         N.engine().pairwise_step(self._kind, *self._tables(optimizer), *self._device_ids(node),
                                  optimizer.opt_struct(), node.out, self._get_margin(), c_loss, c_l2)
 
@@ -45,8 +65,13 @@ class BPR(FusedRecommender):
         """ids in pinned host memory -> orx_pairwise_step_host: H2D, the three kernels and the D2H of
         (loss, l2_loss) are one C call's worth of stream work; the result lands in a pinned buffer."""
         buf, ev = self._out_ring().take(node, keep=node.host_ids)
-        N.engine().pairwise_step_host(self._kind, *self._tables(optimizer), *node.host_ids, optimizer.opt_struct(),
-                                      buf, self._get_margin(), c_loss, c_l2)
+        if self._bf16():
+            N.engine().pairwise_step_host_bf16(self._kind, *self._tables(optimizer), *node.host_ids,
+                                               optimizer.opt_struct(), self.rounding_seed, buf, self._get_margin(),
+                                               c_loss, c_l2)
+        else:
+            N.engine().pairwise_step_host(self._kind, *self._tables(optimizer), *node.host_ids,
+                                          optimizer.opt_struct(), buf, self._get_margin(), c_loss, c_l2)
         ev.record()
         node.out_host, node.event = buf, ev
 
@@ -64,7 +89,8 @@ class BPR(FusedRecommender):
         else:
             kw["d_bp"], kw["d_bn"] = torch.empty(B, device=dev), torch.empty(B, device=dev)
             idx = torch.cat([pid, nid])
-        N.engine().pairwise_grad(self._kind, *self._tables(), uid, pid, nid, self._get_margin(), c_loss, c_l2, **kw)
+        grad = N.engine().pairwise_grad_bf16 if self._bf16() else N.engine().pairwise_grad
+        grad(self._kind, *self._tables(), uid, pid, nid, self._get_margin(), c_loss, c_l2, **kw)
         if "d_user" in kw:
             val = out
         elif "d_pos" in kw:
@@ -74,9 +100,12 @@ class BPR(FusedRecommender):
         return Tensor(idx), Tensor(val)
 
     def _score_operands(self):
-        """(kind, user table, item table, item bias, scale) of the full-catalogue score (inference, RankingEvaluator)."""
-        return (self._score, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
-                self.item_bias.embeddings.t, None)
+        """(kind, user table, item table, item bias, scale) of the full-catalogue score (inference, RankingEvaluator,
+        Retriever).  bf16 tables are scored as their exact float32 upcast, made here for the call."""
+        user, item = self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t
+        if self._bf16():
+            user, item = user.float(), item.float()
+        return (self._score, user, item, self.item_bias.embeddings.t, None)
 
     def inference(self, user_id):
         """scores [Bu, total_items] = U[user] @ Item^T + bias (bpr.py:39-43)."""

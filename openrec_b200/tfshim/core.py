@@ -131,7 +131,10 @@ class Variable:
         self.name = name or "Variable"
 
     def numpy(self):
-        return self.t.detach().cpu().numpy()
+        t = self.t.detach()
+        if t.dtype == torch.bfloat16:   # a bf16 table reads as its exact float32 upcast
+            t = t.float()
+        return t.cpu().numpy()
 
     @property
     def shape(self):
@@ -145,6 +148,9 @@ class Variable:
         return Tensor(self.t)
 
     def assign(self, v):
+        if self.t.dtype == torch.bfloat16:   # float32 first, then round to nearest even
+            self.t.copy_(torch.as_tensor(unwrap(v), dtype=torch.float32, device=self.t.device).to(torch.bfloat16))
+            return self
         self.t.copy_(torch.as_tensor(unwrap(v), dtype=self.t.dtype, device=self.t.device))
         return self
 

@@ -15,6 +15,12 @@ from ... import native as N
 from ..core import SparseGrad, Tensor, Variable, unwrap
 
 
+def _table(var, s0, s1, **kind):
+    """orx_table_t (float32 variable) or orx_table_bf16_t (bfloat16 table) of var with its slots; kind=: see N.table."""
+    make = N.table_bf16 if var.t.dtype == torch.bfloat16 else N.table
+    return make(var.t, s0, s1, **kind)
+
+
 class Optimizer:
     _kind = None
     _n_slots = 0
@@ -47,12 +53,13 @@ class Optimizer:
         ent = self._slots.get(id(var))
         return ent[1] if ent is not None and ent[0]() is var else ()
 
+    # slots are float32 whatever the variable's dtype (a bf16 table keeps fp32 optimizer state)
     def _init_slot(self, var, k):
-        return torch.zeros_like(var.t)
+        return torch.zeros_like(var.t, dtype=torch.float32)
 
     def table(self, var: Variable):
         s0, s1 = self.slots(var)
-        return N.table(var.t, s0, s1)
+        return _table(var, s0, s1)
 
     def opt_struct(self):
         return N.opt(self._kind, self.learning_rate, self.epsilon, self.beta_1, self.beta_2, self.iterations)
@@ -116,7 +123,7 @@ class Adagrad(Optimizer):
         self.epsilon = float(epsilon)
 
     def _init_slot(self, var, k):
-        return torch.full_like(var.t, self.initial_accumulator_value)
+        return torch.full_like(var.t, self.initial_accumulator_value, dtype=torch.float32)
 
 
 class Adam(Optimizer):
@@ -151,10 +158,10 @@ class RowwiseAdagrad(Adagrad):
 
     def table(self, var: Variable):
         s0, s1 = self.slots(var)
-        return N.table(var.t, s0, s1, kind=self._kind)   # checks that s0 holds one accumulator per row
+        return _table(var, s0, s1, kind=self._kind)   # checks that s0 holds one accumulator per row
 
     def _init_slot(self, var, k):
         if getattr(var, "row_table", False):
-            return torch.full((var.t.shape[0],), self.initial_accumulator_value, dtype=var.t.dtype,
+            return torch.full((var.t.shape[0],), self.initial_accumulator_value, dtype=torch.float32,
                               device=var.t.device)
         return super()._init_slot(var, k)
