@@ -176,8 +176,9 @@ enum orx_dispatch_op {
   ORX_OP_CROSS = 11, /* orx_cross_fwd / orx_cross_bwd, one per call with B > 0: variant CROSS_VEC / CROSS_SCALAR,
                        TA = 0 forward / 1 backward, TB = orx_cross_mode (0 forward), M = B, N = W,
                        K = split (ORX_CROSS_FINAL, else 0), S = 1 */
-  ORX_OP_PAIRWISE_STEP_BF16 = 12 /* orx_pairwise_step_bf16, orx_pairwise_step_host_bf16: the fields of
-                                    ORX_OP_PAIRWISE_STEP */
+  ORX_OP_PAIRWISE_STEP_BF16 = 12, /* orx_pairwise_step_bf16, orx_pairwise_step_host_bf16: the fields of
+                                     ORX_OP_PAIRWISE_STEP */
+  ORX_OP_POINTWISE_STEP_BF16 = 13 /* orx_pointwise_step_bf16: the fields of ORX_OP_POINTWISE_STEP */
 };
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
@@ -318,6 +319,26 @@ ORX_API int orx_pairwise_grad_bf16(orx_handle_t h, int32_t kind, const orx_table
                                    const int32_t* pid, const int32_t* nid, int32_t B, float margin, float c_loss,
                                    float c_l2, float* d_user, float* d_pos, float* d_neg, float* d_bp, float* d_bn,
                                    float* g_out, orx_stream_t s);
+/* orx_pointwise_step_bf16: orx_pointwise_step (below) on bf16 user and item tables, every optimizer kind included, each
+ * updated element rounded stochastically with sr_seed and opt->step (table 0 = user, 1 = item).  The item bias and
+ * GMF's w stay fp32 orx_table_t's.  One dispatch record per call, op ORX_OP_POINTWISE_STEP_BF16.  Untouched rows keep
+ * their bits, except under ADAM_DENSE (its sweep writes every row). */
+ORX_API int orx_pointwise_step_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                    const orx_table_bf16_t* item, const orx_table_t* item_bias, const orx_table_t* w,
+                                    const int32_t* uid, const int32_t* iid, const float* label, int32_t B, float a,
+                                    float b, int32_t use_sigmoid, float c_loss, float c_l2, const orx_opt_t* opt_host,
+                                    uint64_t sr_seed, float* out4, orx_stream_t s);
+/* orx_pointwise_fwd / orx_pointwise_grad on bf16 user and item tables (rows read as their exact fp32 upcast); GMF's
+ * d_w included. */
+ORX_API int orx_pointwise_fwd_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                   const orx_table_bf16_t* item, const orx_table_t* item_bias, const orx_table_t* w,
+                                   const int32_t* uid, const int32_t* iid, const float* label, int32_t B, float a,
+                                   float b, int32_t use_sigmoid, float* out4, orx_stream_t s);
+ORX_API int orx_pointwise_grad_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                    const orx_table_bf16_t* item, const orx_table_t* item_bias, const orx_table_t* w,
+                                    const int32_t* uid, const int32_t* iid, const float* label, int32_t B, float a,
+                                    float b, int32_t use_sigmoid, float c_loss, float c_l2, float* d_user,
+                                    float* d_item, float* d_bias, float* d_w, float* g_out, orx_stream_t s);
 /* orx_censor on a bf16 table: row / max(||row||_2, min_norm) in fp32 from the upcast row, stored rounded to nearest
  * even (a projection, not an optimizer update). */
 ORX_API int orx_censor_bf16(orx_handle_t h, uint16_t* tab, int64_t rows, int32_t dim, const int32_t* ids, int32_t n,

@@ -427,6 +427,11 @@ __device__ __forceinline__ uint2 orx_bf16x4_sr(float4 v, uint32_t rk, int col) {
 __device__ __forceinline__ float4 orx_ld4_stream(const uint16_t* p) {
   return orx_bf16x4_up(__ldcs(reinterpret_cast<const uint2*>(p)));
 }
+// Cache-global (ld.global.cg) row loads of the pointwise step: the float form is the plain __ldcg of a float4.
+__device__ __forceinline__ float4 orx_ld4_cg(const float* p) { return __ldcg(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ float4 orx_ld4_cg(const uint16_t* p) {
+  return orx_bf16x4_up(__ldcg(reinterpret_cast<const uint2*>(p)));
+}
 __device__ __forceinline__ void orx_st4_stream(float* p, float4 v, uint32_t, int) { orx_st4_stream(p, v); }
 __device__ __forceinline__ void orx_st4_stream(uint16_t* p, float4 v, uint32_t rk, int col) {
   __stcs(reinterpret_cast<uint2*>(p), orx_bf16x4_sr(v, rk, col));
@@ -878,6 +883,13 @@ int orx_sparse_step(orx_ctx* c, int op, int kind, const orx_table_t* user, const
                     const OrxStepKernel& kernel, cudaStream_t st, const uint32_t* srk = nullptr);
 // srk (orx_sparse_step, orx_launch_adam_sweeps): the user / item tables are bf16 (orx_table_bf16_t, var passed as the
 // float* of the orx_table_t) with these rounding keys (orx_sr_table_key); null = float tables.
+// A bf16 table as the orx_table_t the shared host code takes: var carries the bf16 rows' address, and every kernel that
+// reads it is instantiated for uint16_t storage.  A null table stays null (the shared checks refuse it).
+static inline const orx_table_t* orx_bf16_table(const orx_table_bf16_t* b, orx_table_t* t) {
+  if (!b) return nullptr;
+  *t = {reinterpret_cast<float*>(b->var), b->s0, b->s1, b->rows, b->dim};
+  return t;
+}
 // The un-fused forward / gradient kernel of a family over B samples: launch(partials, blocks) on st with the handle's
 // partials, then, when out4 is given, the (loss, l2) partials reduced into it, the loss scaled by loss_scale.
 int orx_sparse_unfused(orx_ctx* c, int B, float loss_scale, float* out4,

@@ -882,14 +882,6 @@ static int pairwise_step_impl(orx_ctx* c, int kind, const orx_table_t* user, con
                          uid, pid, nid, B, opt, kind == ORX_PAIR_BPR ? inv_B : 1.0f, c_l2, out4, kernel, st, srk);
 }
 
-// A bf16 table as the orx_table_t the shared host code takes: var carries the bf16 rows' address, and every kernel that
-// reads it is instantiated for uint16_t storage.  A null table stays null (the shared checks refuse it).
-static const orx_table_t* bf16_table(const orx_table_bf16_t* b, orx_table_t* t) {
-  if (!b) return nullptr;
-  *t = {reinterpret_cast<float*>(b->var), b->s0, b->s1, b->rows, b->dim};
-  return t;
-}
-
 extern "C" int orx_pairwise_step(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
                                  const orx_table_t* item_bias, const int32_t* uid, const int32_t* pid,
                                  const int32_t* nid, int32_t B, float margin, float c_loss, float c_l2,
@@ -909,7 +901,7 @@ extern "C" int orx_pairwise_step_bf16(orx_handle_t h, int32_t kind, const orx_ta
   ORX_CUDA(cudaSetDevice(h->device));
   orx_table_t tu, ti;
   const uint32_t srk[2] = {orx_sr_table_key(sr_seed, opt->step, 0), orx_sr_table_key(sr_seed, opt->step, 1)};
-  return pairwise_step_impl(h, kind, bf16_table(user, &tu), bf16_table(item, &ti), item_bias, uid, pid, nid, B, margin,
+  return pairwise_step_impl(h, kind, orx_bf16_table(user, &tu), orx_bf16_table(item, &ti), item_bias, uid, pid, nid, B, margin,
                             c_loss, c_l2, opt, out4, (cudaStream_t)s, srk);
 }
 
@@ -966,7 +958,7 @@ extern "C" int orx_pairwise_step_host_bf16(orx_handle_t h, int32_t kind, const o
   ORX_REQUIRE(opt != nullptr, "empty batch or null host buffers");
   orx_table_t tu, ti;
   const uint32_t srk[2] = {orx_sr_table_key(sr_seed, opt->step, 0), orx_sr_table_key(sr_seed, opt->step, 1)};
-  return pairwise_step_host_impl(h, kind, bf16_table(user, &tu), bf16_table(item, &ti), item_bias, uid_host, pid_host,
+  return pairwise_step_host_impl(h, kind, orx_bf16_table(user, &tu), orx_bf16_table(item, &ti), item_bias, uid_host, pid_host,
                                  nid_host, B, margin, c_loss, c_l2, opt, out4_host, s, srk);
 }
 
@@ -1055,7 +1047,7 @@ extern "C" int orx_pairwise_fwd_bf16(orx_handle_t h, int32_t kind, const orx_tab
   ORX_REQUIRE(h != nullptr && out4 != nullptr, "null handle/out");
   ORX_CUDA(cudaSetDevice(h->device));
   orx_table_t tu, ti;
-  return pair_fwd_grad(h, kind, bf16_table(user, &tu), bf16_table(item, &ti), item_bias, uid, pid, nid, B, margin, 1.f,
+  return pair_fwd_grad(h, kind, orx_bf16_table(user, &tu), orx_bf16_table(item, &ti), item_bias, uid, pid, nid, B, margin, 1.f,
                        1.f, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out4, (cudaStream_t)s, true);
 }
 
@@ -1067,7 +1059,7 @@ extern "C" int orx_pairwise_grad_bf16(orx_handle_t h, int32_t kind, const orx_ta
   ORX_REQUIRE(h != nullptr, "null handle");
   ORX_CUDA(cudaSetDevice(h->device));
   orx_table_t tu, ti;
-  return pair_fwd_grad(h, kind, bf16_table(user, &tu), bf16_table(item, &ti), item_bias, uid, pid, nid, B, margin,
+  return pair_fwd_grad(h, kind, orx_bf16_table(user, &tu), orx_bf16_table(item, &ti), item_bias, uid, pid, nid, B, margin,
                        c_loss, c_l2, d_user, d_pos, d_neg, d_bp, d_bn, g_out, nullptr, (cudaStream_t)s, true);
 }
 

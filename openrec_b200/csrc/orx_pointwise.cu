@@ -42,7 +42,9 @@ __device__ __forceinline__ void point_score(float s, float bias, float label, co
   }
 }
 
-template <int KIND, int OPT, int D, int CH>
+// T: the storage of the user and item tables, float or bf16 bits (uint16_t; rows 8-byte aligned, read as their exact
+// fp32 upcast and rounded on store with the keys a.srk).  Slot rows, the item bias and GMF's w are float either way.
+template <int KIND, int OPT, int D, int CH, typename T = float>
 __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
   constexpr int G = (D / 4 < 32) ? D / 4 : 32;
   constexpr int K = D / (4 * G);
@@ -101,8 +103,8 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
 #pragma unroll
     for (int k = 0; k < K; ++k) {
       const int off = (k * G + gl) * 4;
-      u[k] = v ? __ldcg(reinterpret_cast<const float4*>(a.U + (int64_t)uu * D + off)) : z4;
-      it[k] = v ? __ldcg(reinterpret_cast<const float4*>(a.I + (int64_t)ii * D + off)) : z4;
+      u[k] = v ? orx_ld4_cg(reinterpret_cast<const T*>(a.U) + (int64_t)uu * D + off) : z4;
+      it[k] = v ? orx_ld4_cg(reinterpret_cast<const T*>(a.I) + (int64_t)ii * D + off) : z4;
       if (SL::S0) {
         us0[k] = (fl & 2) ? __ldcg(reinterpret_cast<const float4*>(a.Us0 + (int64_t)uu * D + off)) : z4;
         is0[k] = (fl & 4) ? __ldcg(reinterpret_cast<const float4*>(a.Is0 + (int64_t)ii * D + off)) : z4;
@@ -158,8 +160,10 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
             gwacc[k].x += g * u[k].x * it[k].x; gwacc[k].y += g * u[k].y * it[k].y;
             gwacc[k].z += g * u[k].z * it[k].z; gwacc[k].w += g * u[k].w * it[k].w;
           }
-          orx_own_or_stage4_row<false>(fl & 2, a.U, uu, a.gu, duj, D, off, u[k], gu, fu, a.opt);
-          orx_own_or_stage4_row<false>(fl & 4, a.I, ii, a.gi, dij, D, off, it[k], gi, fi, a.opt);
+          orx_own_or_stage4_row<false>(fl & 2, reinterpret_cast<T*>(a.U), uu, a.gu, duj, D, off, u[k], gu, fu, a.opt,
+                                       a.srk[0]);
+          orx_own_or_stage4_row<false>(fl & 4, reinterpret_cast<T*>(a.I), ii, a.gi, dij, D, off, it[k], gi, fi, a.opt,
+                                       a.srk[1]);
         }
         if (gl == 0) {
           if (fl & 2) __stcg(a.Us0 + uu, ua);
@@ -180,8 +184,10 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
           gwacc[k].x += g * u[k].x * it[k].x; gwacc[k].y += g * u[k].y * it[k].y;
           gwacc[k].z += g * u[k].z * it[k].z; gwacc[k].w += g * u[k].w * it[k].w;
         }
-        orx_own_or_stage4<OPT, false>(fl & 2, a.U, a.Us0, a.Us1, uu, a.gu, duj, D, off, u[k], gu, us0[k], us1[k], a.opt);
-        orx_own_or_stage4<OPT, false>(fl & 4, a.I, a.Is0, a.Is1, ii, a.gi, dij, D, off, it[k], gi, is0[k], is1[k], a.opt);
+        orx_own_or_stage4<OPT, false>(fl & 2, reinterpret_cast<T*>(a.U), a.Us0, a.Us1, uu, a.gu, duj, D, off, u[k], gu,
+                                      us0[k], us1[k], a.opt, a.srk[0]);
+        orx_own_or_stage4<OPT, false>(fl & 4, reinterpret_cast<T*>(a.I), a.Is0, a.Is1, ii, a.gi, dij, D, off, it[k], gi,
+                                      is0[k], is1[k], a.opt, a.srk[1]);
       }
     }
   }
@@ -209,8 +215,8 @@ __global__ void __launch_bounds__(256) k_point_step(const PointArgs a) {
   orx_warp_partial(loss_acc, l2_acc, a.partials);
 }
 
-// Any dim; MODE 0 = fused step, 1 = forward / explicit (un-fused) gradients.
-template <int KIND, int OPT, int MODE>
+// Any dim; MODE 0 = fused step, 1 = forward / explicit (un-fused) gradients.  T as in k_point_step.
+template <int KIND, int OPT, int MODE, typename T = float>
 __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
   constexpr bool STAGE_ONLY = OrxOptSlots<OPT>::STAGE_ONLY;
   constexpr bool GMF = (KIND == ORX_POINT_GMF);
@@ -223,12 +229,12 @@ __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
     if (t >= a.B) break;
     const int uu = a.uid[t], ii = a.iid[t];
     const bool ok = uu >= 0 && uu < a.rowsU && ii >= 0 && ii < a.rowsI;
-    float* ur = a.U + (int64_t)uu * D;
-    float* ir = a.I + (int64_t)ii * D;
+    T* ur = reinterpret_cast<T*>(a.U) + (int64_t)uu * D;
+    T* ir = reinterpret_cast<T*>(a.I) + (int64_t)ii * D;
     float s = 0.f, sq = 0.f;
     if (ok) {
       for (int d = lane; d < D; d += 32) {
-        const float u = ur[d], it = ir[d], w = GMF ? a.W[d] : 1.f;
+        const float u = orx_ld1(ur + d), it = orx_ld1(ir + d), w = GMF ? a.W[d] : 1.f;
         s += w * u * it;
         sq += u * u + it * it;
       }
@@ -250,9 +256,10 @@ __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
     const float c2 = a.c_l2;
     if constexpr (OrxOptSlots<OPT>::ROW) {   // MODE 0 only: each owned row's squared-gradient sum, then the apply
       if (!ok) continue;   // warp-uniform
+      const uint32_t rku = orx_sr_row(a.srk[0], uu), rki = orx_sr_row(a.srk[1], ii);
       float su = 0.f, si = 0.f;
       for (int d = lane; d < D; d += 32) {
-        const float u = ur[d], it = ir[d], w = GMF ? a.W[d] : 1.f;
+        const float u = orx_ld1(ur + d), it = orx_ld1(ir + d), w = GMF ? a.W[d] : 1.f;
         const float gu = g * w * it + c2 * u, gi = g * w * u + c2 * it;
         su += gu * gu;
         si += gi * gi;
@@ -262,12 +269,12 @@ __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
       float ua = fu ? a.Us0[uu] : 0.f, ia = fi ? a.Is0[ii] : 0.f;
       const float xu = orx_row_scale(ua, su, D, a.opt), xi = orx_row_scale(ia, si, D, a.opt);
       for (int d = lane; d < D; d += 32) {
-        const float u = ur[d], it = ir[d], w = GMF ? a.W[d] : 1.f;
+        const float u = orx_ld1(ur + d), it = orx_ld1(ir + d), w = GMF ? a.W[d] : 1.f;
         const float gu = g * w * it + c2 * u, gi = g * w * u + c2 * it;
         if (GMF && a.gw) atomicAdd(a.gw + d, g * u * it);
-        if (fu) ur[d] = orx_row_apply1(u, gu, xu, a.opt);
+        if (fu) orx_st1(ur + d, orx_row_apply1(u, gu, xu, a.opt), rku, d);
         else atomicAdd(a.gu + (int64_t)du * D + d, gu);
-        if (fi) ir[d] = orx_row_apply1(it, gi, xi, a.opt);
+        if (fi) orx_st1(ir + d, orx_row_apply1(it, gi, xi, a.opt), rki, d);
         else atomicAdd(a.gi + (int64_t)di * D + d, gi);
       }
       if (lane == 0) {
@@ -279,18 +286,19 @@ __global__ void __launch_bounds__(256) k_point_generic(const PointArgs a) {
       continue;
     } else {
     if (MODE == 0 ? ok : (a.d_user || a.d_item || a.gw)) {
+      const uint32_t rku = orx_sr_row(a.srk[0], uu), rki = orx_sr_row(a.srk[1], ii);
       for (int d = lane; d < D; d += 32) {
         float gu = 0.f, gi = 0.f;
         if (ok) {
-          const float u = ur[d], it = ir[d], w = GMF ? a.W[d] : 1.f;
+          const float u = orx_ld1(ur + d), it = orx_ld1(ir + d), w = GMF ? a.W[d] : 1.f;
           gu = g * w * it + c2 * u;
           gi = g * w * u + c2 * it;
           if (GMF && a.gw) atomicAdd(a.gw + d, g * u * it);
           if (MODE == 0) {
             const int64_t ou = (int64_t)uu * D + d, oi = (int64_t)ii * D + d;
-            if (fu) orx_update1<OPT>(ur + d, a.Us0 + ou, a.Us1 + ou, u, gu, a.opt);
+            if (fu) orx_update1<OPT>(ur + d, a.Us0 + ou, a.Us1 + ou, u, gu, a.opt, rku, d);
             else atomicAdd(a.gu + (int64_t)du * D + d, gu);
-            if (fi) orx_update1<OPT>(ir + d, a.Is0 + oi, a.Is1 + oi, it, gi, a.opt);
+            if (fi) orx_update1<OPT>(ir + d, a.Is0 + oi, a.Is1 + oi, it, gi, a.opt, rki, d);
             else atomicAdd(a.gi + (int64_t)di * D + d, gi);
           }
         }
@@ -333,22 +341,26 @@ __global__ void k_gmf_w_terms(const float* W, int D, float* out4, float* d_w, fl
   if (threadIdx.x == 0 && out4) out4[1] += 0.5f * sh[0];
 }
 
-template <int KIND, int OPT>
+// T = uint16_t: bf16 user / item tables, which take the same variants.
+template <int KIND, int OPT, typename T = float>
 static int launch_point_kind_opt(const PointArgs& pa, cudaStream_t st, OrxStepLaunch* out) {
   const int blocks = orx_step_blocks(pa.B);
   *out = {8 * blocks, ORX_VARIANT_STEP, 0};
-  // k_point_step moves table rows, slot rows and GMF's w as float4: a base off a 16-byte boundary takes k_point_generic
-  // (a row-wise accumulator is read as scalars and does not count)
-  const bool vec = OrxOptSlots<OPT>::ROW ? orx_aligned16(pa.U, pa.I, pa.W)
-                                         : orx_aligned16(pa.U, pa.Us0, pa.Us1, pa.I, pa.Is0, pa.Is1, pa.W);
+  // k_point_step moves table rows as 4-element vectors (float4, or 8 bytes of bf16), slot rows and GMF's w as float4: a
+  // base off the boundary its row path needs takes k_point_generic (a row-wise accumulator is read as scalars and does
+  // not count)
+  constexpr bool BF = std::is_same<T, uint16_t>::value;
+  const bool rows_ok = BF ? orx_aligned8(pa.U, pa.I) : orx_aligned16(pa.U, pa.I);
+  const bool vec = OrxOptSlots<OPT>::ROW ? rows_ok && orx_aligned16(pa.W)
+                                         : rows_ok && orx_aligned16(pa.Us0, pa.Us1, pa.Is0, pa.Is1, pa.W);
   switch (vec ? pa.D : 0) {
-    case 32: k_point_step<KIND, OPT, 32, 8><<<blocks, 256, 0, st>>>(pa); break;
-    case 64: k_point_step<KIND, OPT, 64, 8><<<blocks, 256, 0, st>>>(pa); break;
-    case 128: k_point_step<KIND, OPT, 128, 8><<<blocks, 256, 0, st>>>(pa); break;
-    case 256: k_point_step<KIND, OPT, 256, 8><<<blocks, 256, 0, st>>>(pa); break;
+    case 32: k_point_step<KIND, OPT, 32, 8, T><<<blocks, 256, 0, st>>>(pa); break;
+    case 64: k_point_step<KIND, OPT, 64, 8, T><<<blocks, 256, 0, st>>>(pa); break;
+    case 128: k_point_step<KIND, OPT, 128, 8, T><<<blocks, 256, 0, st>>>(pa); break;
+    case 256: k_point_step<KIND, OPT, 256, 8, T><<<blocks, 256, 0, st>>>(pa); break;
     default:
       out->variant = ORX_VARIANT_STEP_GENERIC;
-      k_point_generic<KIND, OPT, 0><<<blocks, 256, 0, st>>>(pa);
+      k_point_generic<KIND, OPT, 0, T><<<blocks, 256, 0, st>>>(pa);
       break;
   }
   ORX_LAUNCH_CHECK();
@@ -368,12 +380,12 @@ static PointArgs point_args(const SparseArgs& s, const orx_table_t* dense_w, con
   return pa;
 }
 
-extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
-                                  const orx_table_t* item_bias, const orx_table_t* w, const int32_t* uid,
-                                  const int32_t* iid, const float* label, int32_t B, float a, float b,
-                                  int32_t use_sigmoid, float c_loss, float c_l2, const orx_opt_t* opt, float* out4,
-                                  orx_stream_t s) {
-  ORX_REQUIRE(h != nullptr, "null handle");
+// srk: bf16 user / item tables with these rounding keys (their var passed as float*), null: float tables
+static int pointwise_step_impl(orx_ctx* h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
+                               const orx_table_t* item_bias, const orx_table_t* w, const int32_t* uid,
+                               const int32_t* iid, const float* label, int32_t B, float a, float b,
+                               int32_t use_sigmoid, float c_loss, float c_l2, const orx_opt_t* opt, float* out4,
+                               cudaStream_t st, const uint32_t* srk = nullptr) {
   ORX_REQUIRE(label != nullptr, "empty batch or null inputs");
   ORX_REQUIRE(kind == ORX_POINT_GMF || kind == ORX_POINT_WRMF, "unknown pointwise kind");
   ORX_REQUIRE(kind == ORX_POINT_WRMF || w, "GMF needs w with dim == D");
@@ -383,27 +395,53 @@ extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_
     od = orx_opt_dim(opt, user->dim);
     opt = &od;
   }
-  ORX_CUDA(cudaSetDevice(h->device));
-  cudaStream_t st = (cudaStream_t)s;
   const auto kernel = [&](const SparseArgs& sa, const int4* /*res: pairwise only*/, float* partials, OrxStepLaunch* out) {
     PointArgs pa = point_args(sa, dense_w, user, item, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2);
     pa.partials = partials;
     pa.gw = dense_w ? h->gw : nullptr;
     return orx_dispatch<ORX_POINT_GMF, ORX_POINT_WRMF>(kind, [&](auto K) {
       return orx_dispatch_opt(opt->kind, [&](auto O) {
+        if (srk) return launch_point_kind_opt<decltype(K)::value, decltype(O)::value, uint16_t>(pa, st, out);
         return launch_point_kind_opt<decltype(K)::value, decltype(O)::value>(pa, st, out);
       });
     });
   };
-  return orx_sparse_step(h, ORX_OP_POINTWISE_STEP, kind, user, item, item_bias, dense_w, uid, iid, nullptr, B, opt,
-                         dense_w ? 1.0f / (float)B : 1.0f, c_l2, out4, kernel, st);
+  return orx_sparse_step(h, srk ? ORX_OP_POINTWISE_STEP_BF16 : ORX_OP_POINTWISE_STEP, kind, user, item, item_bias,
+                         dense_w, uid, iid, nullptr, B, opt, dense_w ? 1.0f / (float)B : 1.0f, c_l2, out4, kernel, st,
+                         srk);
+}
+
+extern "C" int orx_pointwise_step(orx_handle_t h, int32_t kind, const orx_table_t* user, const orx_table_t* item,
+                                  const orx_table_t* item_bias, const orx_table_t* w, const int32_t* uid,
+                                  const int32_t* iid, const float* label, int32_t B, float a, float b,
+                                  int32_t use_sigmoid, float c_loss, float c_l2, const orx_opt_t* opt, float* out4,
+                                  orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr, "null handle");
+  ORX_CUDA(cudaSetDevice(h->device));
+  return pointwise_step_impl(h, kind, user, item, item_bias, w, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2,
+                             opt, out4, (cudaStream_t)s);
+}
+
+extern "C" int orx_pointwise_step_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                       const orx_table_bf16_t* item, const orx_table_t* item_bias,
+                                       const orx_table_t* w, const int32_t* uid, const int32_t* iid,
+                                       const float* label, int32_t B, float a, float b, int32_t use_sigmoid,
+                                       float c_loss, float c_l2, const orx_opt_t* opt, uint64_t sr_seed, float* out4,
+                                       orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr, "null handle");
+  ORX_REQUIRE(opt != nullptr, "null opt/out");
+  ORX_CUDA(cudaSetDevice(h->device));
+  orx_table_t tu, ti;
+  const uint32_t srk[2] = {orx_sr_table_key(sr_seed, opt->step, 0), orx_sr_table_key(sr_seed, opt->step, 1)};
+  return pointwise_step_impl(h, kind, orx_bf16_table(user, &tu), orx_bf16_table(item, &ti), item_bias, w, uid, iid,
+                             label, B, a, b, use_sigmoid, c_loss, c_l2, opt, out4, (cudaStream_t)s, srk);
 }
 
 static int point_fwd_grad(orx_ctx* h, int kind, const orx_table_t* user, const orx_table_t* item,
                           const orx_table_t* bias, const orx_table_t* w, const int32_t* uid, const int32_t* iid,
                           const float* label, int B, float a, float b, int use_sigmoid, float c_loss, float c_l2,
                           float* d_user, float* d_item, float* d_bias, float* d_w, float* g_out, float* out4,
-                          cudaStream_t st) {
+                          cudaStream_t st, bool bf16 = false) {
   ORX_REQUIRE(B > 0 && uid && iid && label, "empty batch or null inputs");
   ORX_REQUIRE(kind == ORX_POINT_GMF || kind == ORX_POINT_WRMF, "unknown pointwise kind");
   ORX_REQUIRE(kind == ORX_POINT_WRMF || w, "GMF needs w with dim == D");
@@ -420,7 +458,8 @@ static int point_fwd_grad(orx_ctx* h, int kind, const orx_table_t* user, const o
   const auto launch = [&](float* partials, int blocks) {
     pa.partials = partials;
     orx_dispatch<ORX_POINT_GMF, ORX_POINT_WRMF>(kind, [&](auto K) {
-      k_point_generic<decltype(K)::value, ORX_OPT_SGD, 1><<<blocks, 256, 0, st>>>(pa);
+      if (bf16) k_point_generic<decltype(K)::value, ORX_OPT_SGD, 1, uint16_t><<<blocks, 256, 0, st>>>(pa);
+      else k_point_generic<decltype(K)::value, ORX_OPT_SGD, 1><<<blocks, 256, 0, st>>>(pa);
     });
   };
   if ((rc = orx_sparse_unfused(h, B, dense_w ? pa.inv_B : 1.f, out4, launch, st))) return rc;
@@ -450,4 +489,30 @@ extern "C" int orx_pointwise_grad(orx_handle_t h, int32_t kind, const orx_table_
   ORX_CUDA(cudaSetDevice(h->device));
   return point_fwd_grad(h, kind, user, item, item_bias, w, uid, iid, label, B, a, b, use_sigmoid, c_loss, c_l2, d_user,
                         d_item, d_bias, d_w, g_out, nullptr, (cudaStream_t)s);
+}
+
+extern "C" int orx_pointwise_fwd_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                      const orx_table_bf16_t* item, const orx_table_t* item_bias, const orx_table_t* w,
+                                      const int32_t* uid, const int32_t* iid, const float* label, int32_t B, float a,
+                                      float b, int32_t use_sigmoid, float* out4, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr && out4 != nullptr, "null handle/out");
+  ORX_CUDA(cudaSetDevice(h->device));
+  orx_table_t tu, ti;
+  return point_fwd_grad(h, kind, orx_bf16_table(user, &tu), orx_bf16_table(item, &ti), item_bias, w, uid, iid, label, B,
+                        a, b, use_sigmoid, 1.f, 1.f, nullptr, nullptr, nullptr, nullptr, nullptr, out4, (cudaStream_t)s,
+                        true);
+}
+
+extern "C" int orx_pointwise_grad_bf16(orx_handle_t h, int32_t kind, const orx_table_bf16_t* user,
+                                       const orx_table_bf16_t* item, const orx_table_t* item_bias,
+                                       const orx_table_t* w, const int32_t* uid, const int32_t* iid,
+                                       const float* label, int32_t B, float a, float b, int32_t use_sigmoid,
+                                       float c_loss, float c_l2, float* d_user, float* d_item, float* d_bias,
+                                       float* d_w, float* g_out, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr, "null handle");
+  ORX_CUDA(cudaSetDevice(h->device));
+  orx_table_t tu, ti;
+  return point_fwd_grad(h, kind, orx_bf16_table(user, &tu), orx_bf16_table(item, &ti), item_bias, w, uid, iid, label, B,
+                        a, b, use_sigmoid, c_loss, c_l2, d_user, d_item, d_bias, d_w, g_out, nullptr, (cudaStream_t)s,
+                        true);
 }

@@ -16,7 +16,8 @@ from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP
                    ORX_VARIANT_GEMM_TMA, ORX_VARIANT_INTERACT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_RANK_GLOBAL,
                    ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE,
                    ORX_VARIANT_TOPK, ORX_OP_CROSS, ORX_VARIANT_CROSS_VEC, ORX_VARIANT_CROSS_SCALAR, ORX_CROSS_TOP,
-                   ORX_CROSS_MID, ORX_CROSS_FINAL, ORX_OP_PAIRWISE_STEP_BF16, OrxOpt, OrxTable, OrxTableBf16)
+                   ORX_CROSS_MID, ORX_CROSS_FINAL, ORX_OP_PAIRWISE_STEP_BF16, ORX_OP_POINTWISE_STEP_BF16, OrxOpt,
+                   OrxTable, OrxTableBf16)
 
 __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", "ORX_POINT_GMF", "ORX_POINT_WRMF",
            "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_OPT_ROWWISE_ADAGRAD",
@@ -28,7 +29,7 @@ __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", 
            "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "ORX_OP_SCORE_TOPK_SHARD", "ORX_OP_POINTWISE_GRAD_ROWS",
            "ORX_OP_CENSOR_SHARD", "ORX_VARIANT_CENSOR_VEC", "ORX_VARIANT_CENSOR_SCALAR", "ORX_OP_CROSS",
            "ORX_VARIANT_CROSS_VEC", "ORX_VARIANT_CROSS_SCALAR", "ORX_CROSS_TOP", "ORX_CROSS_MID", "ORX_CROSS_FINAL",
-           "ORX_OP_PAIRWISE_STEP_BF16", "table_bf16", "as_table",
+           "ORX_OP_PAIRWISE_STEP_BF16", "ORX_OP_POINTWISE_STEP_BF16", "table_bf16", "as_table",
            "Dispatch", "RowShard", "rowshard", "shard_rows"]
 
 _engines = {}
@@ -568,6 +569,29 @@ class Engine:
                                                _ptr(label), uid.numel(), a, b, int(use_sigmoid), c_loss, c_l2,
                                                _ptr(d_user), _ptr(d_item), _ptr(d_bias), _ptr(d_w), _ptr(g_out),
                                                self.stream()), "orx_pointwise_grad")
+
+    def pointwise_step_bf16(self, kind, user, item, bias, w, uid, iid, label, o, sr_seed, out4, a=1.0, b=1.0,
+                            use_sigmoid=False, c_loss=1.0, c_l2=1.0):
+        """pointwise_step on bf16 user / item tables (table_bf16), rounding seeded with sr_seed; bias and w fp32."""
+        _lib.check(self.lib.orx_pointwise_step_bf16(self.h, kind, C.byref(user), C.byref(item), C.byref(bias),
+                                                    C.byref(w) if w is not None else None, _ptr(uid), _ptr(iid),
+                                                    _ptr(label), uid.numel(), a, b, int(use_sigmoid), c_loss, c_l2,
+                                                    C.byref(o), int(sr_seed), _ptr(out4), self.stream()),
+                   "orx_pointwise_step_bf16")
+
+    def pointwise_fwd_bf16(self, kind, user, item, bias, w, uid, iid, label, out4, a=1.0, b=1.0, use_sigmoid=False):
+        _lib.check(self.lib.orx_pointwise_fwd_bf16(self.h, kind, C.byref(user), C.byref(item), C.byref(bias),
+                                                   C.byref(w) if w is not None else None, _ptr(uid), _ptr(iid),
+                                                   _ptr(label), uid.numel(), a, b, int(use_sigmoid), _ptr(out4),
+                                                   self.stream()), "orx_pointwise_fwd_bf16")
+
+    def pointwise_grad_bf16(self, kind, user, item, bias, w, uid, iid, label, a=1.0, b=1.0, use_sigmoid=False,
+                            c_loss=1.0, c_l2=1.0, *, d_user=None, d_item=None, d_bias=None, d_w=None, g_out=None):
+        _lib.check(self.lib.orx_pointwise_grad_bf16(self.h, kind, C.byref(user), C.byref(item), C.byref(bias),
+                                                    C.byref(w) if w is not None else None, _ptr(uid), _ptr(iid),
+                                                    _ptr(label), uid.numel(), a, b, int(use_sigmoid), c_loss, c_l2,
+                                                    _ptr(d_user), _ptr(d_item), _ptr(d_bias), _ptr(d_w), _ptr(g_out),
+                                                    self.stream()), "orx_pointwise_grad_bf16")
 
     # ---- dense / inference / metrics -----------------------------------------------------
     def dense_apply(self, var, s0, s1, grad, o):

@@ -14,6 +14,13 @@ from ...tfshim.core import LazyScalar, StepNode, Tensor, convert
 from ...tfshim.keras import Model
 
 
+def _check_dtype(embedding_dtype):
+    """The embedding_dtype keyword of the fused-step recommenders: "float32" or "bfloat16"."""
+    if embedding_dtype not in ("float32", "bfloat16"):
+        raise ValueError(f"embedding_dtype must be 'float32' or 'bfloat16', got {embedding_dtype!r}")
+    return embedding_dtype
+
+
 def ids_of(x):
     """int32 device ids from whatever the caller feeds (Keras Embedding casts to int32)."""
     return N.ids32(convert(x).t)

@@ -4,13 +4,7 @@ import torch
 from ... import native as N
 from ...tfshim.core import Tensor
 from ..modules import LatentFactor, PairwiseLogLoss
-from ._base import FusedRecommender, ids_any, ids_of
-
-
-def _check_dtype(embedding_dtype):
-    if embedding_dtype not in ("float32", "bfloat16"):
-        raise ValueError(f"embedding_dtype must be 'float32' or 'bfloat16', got {embedding_dtype!r}")
-    return embedding_dtype
+from ._base import FusedRecommender, _check_dtype, ids_any, ids_of
 
 
 class BPR(FusedRecommender):

@@ -2,21 +2,21 @@
 import torch
 
 from ... import native as N
-from ..modules import MLP, LatentFactor
+from ..modules import MLP
 from ._base import FusedRecommender, w_table
 from .wrmf import WRMF
 
 
 class GMF(WRMF):
+    """``embedding_dtype="bfloat16"`` stores the user and item tables in bfloat16 (the item bias, ``w`` and every
+    optimizer slot stay float32); each step rounds its updates stochastically, seeded by ``rounding_seed`` and the
+    optimizer's iteration count, so a run is reproducible bit for bit."""
     _kind = N.ORX_POINT_GMF
 
-    def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items):
+    def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items, embedding_dtype="float32",
+                 rounding_seed=0):
         FusedRecommender.__init__(self)
-        self.user_latent_factor = LatentFactor(num_instances=total_users, dim=dim_user_embed,
-                                               name="user_latent_factor")
-        self.item_latent_factor = LatentFactor(num_instances=total_items, dim=dim_item_embed,
-                                               name="item_latent_factor")
-        self.item_bias = LatentFactor(num_instances=total_items, dim=1, name="item_bias")
+        self._latent_factors(dim_user_embed, dim_item_embed, total_users, total_items, embedding_dtype, rounding_seed)
         self.mlp = MLP(units_list=[1], use_bias=False)
         self.mlp.build(dim_user_embed)   # Dense(1) kernel [D,1], glorot uniform (gmf.py:19)
 
@@ -32,5 +32,5 @@ class GMF(WRMF):
 
     def _score_operands(self):
         """(u * w) . item^T + bias (gmf.py:36-41): WRMF's score with GMF's w as the user-side scale."""
-        return (N.ORX_SCORE_DOT, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
-                self.item_bias.embeddings.t, self.mlp.layers[0].kernel.t.reshape(-1))
+        return (N.ORX_SCORE_DOT, *self._score_tables(), self.item_bias.embeddings.t,
+                self.mlp.layers[0].kernel.t.reshape(-1))

@@ -1,8 +1,8 @@
 """UCML -- mirrors openrec/tf2/recommenders/ucml.py:5-53 on the fused liborx step (K2)."""
 from ... import native as N
 from ..modules import LatentFactor
-from .bpr import BPR, _check_dtype
-from ._base import FusedRecommender
+from .bpr import BPR
+from ._base import FusedRecommender, _check_dtype
 
 
 class UCML(BPR):
