@@ -151,9 +151,10 @@ ORX_API int orx_debug_set_epoch(orx_handle_t h, uint32_t epoch);
  * TA = TB = 0, S = 1.  A sparse step (one record per call) has TA = kind (orx_pair_kind / orx_point_kind), TB = optimizer
  * (orx_opt_kind), M = B, N = D, K = the CTAs/SM bound of the fused kernel's __launch_bounds__ (0: none) and S = the batch
  * index set it used: 0 = built on the caller's stream, 1 or 2 = a consumed prefetch (orx_pairwise_prefetch, or the side
- * stream of orx_pairwise_step_host).  orx_score_rank and orx_score_topk write one record per call, orx_score_rank_shard
- * one per phase-2 call and orx_score_topk_shard one per phase-1 call (fields at ORX_OP_SCORE_RANK / ORX_OP_SCORE_TOPK /
- * ORX_OP_SCORE_RANK_SHARD / ORX_OP_SCORE_TOPK_SHARD).
+ * stream of orx_pairwise_step_host).  orx_score_rank, orx_score_topk and their bf16 forms write one record per call,
+ * orx_score_rank_shard one per phase-2 call and orx_score_topk_shard one per phase-1 call (fields at ORX_OP_SCORE_RANK /
+ * ORX_OP_SCORE_TOPK / ORX_OP_SCORE_RANK_BF16 / ORX_OP_SCORE_TOPK_BF16 / ORX_OP_SCORE_RANK_SHARD /
+ * ORX_OP_SCORE_TOPK_SHARD); orx_score_all, orx_score_rank_listed and their bf16 forms write none.
  * Host-side bookkeeping only: no device work, no synchronisation. */
 enum orx_dispatch_op {
   ORX_OP_GEMM = 0,
@@ -178,7 +179,11 @@ enum orx_dispatch_op {
                        K = split (ORX_CROSS_FINAL, else 0), S = 1 */
   ORX_OP_PAIRWISE_STEP_BF16 = 12, /* orx_pairwise_step_bf16, orx_pairwise_step_host_bf16: the fields of
                                      ORX_OP_PAIRWISE_STEP */
-  ORX_OP_POINTWISE_STEP_BF16 = 13 /* orx_pointwise_step_bf16: the fields of ORX_OP_POINTWISE_STEP */
+  ORX_OP_POINTWISE_STEP_BF16 = 13, /* orx_pointwise_step_bf16: the fields of ORX_OP_POINTWISE_STEP */
+  ORX_OP_SCORE_RANK_BF16 = 14, /* orx_score_rank_bf16: the fields of ORX_OP_SCORE_RANK (same variant and item splits
+                                  as orx_score_rank on the same shapes) */
+  ORX_OP_SCORE_TOPK_BF16 = 15  /* orx_score_topk_bf16: the fields of ORX_OP_SCORE_TOPK (same item splits as
+                                  orx_score_topk on the same shapes) */
 };
 enum orx_dispatch_variant {
   ORX_VARIANT_GEMM_TMA = 0,      /* k_gemm_tma: TMA-fed wgmma 3xTF32 (orx_mlp_tc.cu) */
@@ -623,6 +628,20 @@ ORX_API int orx_score_all(orx_handle_t h, int32_t kind, const float* user_tab, i
                   const float* scale, const float* item_tab, const float* item_bias, int64_t I, int32_t dim,
                   float* scores, orx_stream_t s);
 
+/* ---- scoring on bf16 tables: orx_score_all_bf16, orx_score_rank_bf16, orx_score_rank_listed_bf16 and
+ * orx_score_topk_bf16 take the user and item tables as bf16 bits (uint16_t) and are otherwise their fp32 forms.
+ * Each element is widened to fp32 exactly as it is read; scale, item_bias, the arithmetic and its order are fp32 and
+ * unchanged.  So every output (scores, auc / ndcg / recall, top_items, top_scores, NaN and +-inf included) equals the
+ * fp32 form called on the fp32 upcast of the two tables, bit for bit.  The refusals, size limits, bad-uid rule, CSR
+ * rules, scratch, determinism and dispatch fields are those of the fp32 form (orx_score_rank_bf16 logs
+ * ORX_OP_SCORE_RANK_BF16, orx_score_topk_bf16 ORX_OP_SCORE_TOPK_BF16, the other two nothing).  Alignment: a table at
+ * any 2-byte-aligned address is accepted and gives the same bits; with dim % 4 == 0 and both tables 8-byte aligned the
+ * catalogue passes of orx_score_rank_bf16 / orx_score_topk_bf16 load 4 columns at a time, which is faster.  No
+ * sharded form takes bf16 tables. */
+ORX_API int orx_score_all_bf16(orx_handle_t h, int32_t kind, const uint16_t* user_tab, int64_t U, const int32_t* uid,
+                               int32_t Bu, const float* scale, const uint16_t* item_tab, const float* item_bias,
+                               int64_t I, int32_t dim, float* scores, orx_stream_t s);
+
 /* ---- device-side samplers (SURVEY 8f N3; semantics of openrec/tf2/data/dataset.py:7-58 + data/utils.py:82-87,102-116).
  * orx_sampler_t: the interaction records, the random permutations of the current and of the next epoch (records are
  * consumed in permutation order and never dropped: a batch that crosses the end of an epoch continues in perm_next),
@@ -671,6 +690,13 @@ ORX_API int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_tab, 
                            int32_t dim, const int64_t* pos_off, const int32_t* pos_items, const int64_t* excl_off,
                            const int32_t* excl_items, int32_t max_pos, const int32_t* at_host, int32_t n_at,
                            float* auc, float* ndcg, float* recall, orx_stream_t s);
+/* orx_score_rank on bf16 tables (see orx_score_all_bf16): bit-equal to orx_score_rank on their fp32 upcast. */
+ORX_API int orx_score_rank_bf16(orx_handle_t h, int32_t kind, const uint16_t* user_tab, int64_t U, const int32_t* uid,
+                                int32_t Bu, const float* scale, const uint16_t* item_tab, const float* item_bias,
+                                int64_t I, int32_t dim, const int64_t* pos_off, const int32_t* pos_items,
+                                const int64_t* excl_off, const int32_t* excl_items, int32_t max_pos,
+                                const int32_t* at_host, int32_t n_at, float* auc, float* ndcg, float* recall,
+                                orx_stream_t s);
 
 /* ---- sharded catalogue evaluation: orx_score_rank over row-sharded user / item tables (the layout of orx_shard_step:
  * row r of every table lives on rank r % world at local row r / world), each rank counting over its own item rows
@@ -739,6 +765,15 @@ ORX_API int orx_score_rank_listed(orx_handle_t h, int32_t kind, const float* use
                                   const int64_t* neg_off, const int32_t* neg_items, const int64_t* excl_off,
                                   const int32_t* excl_items, int32_t max_pos, const int32_t* at_host, int32_t n_at,
                                   float* auc, float* ndcg, float* recall, orx_stream_t s);
+/* orx_score_rank_listed on bf16 tables (see orx_score_all_bf16): bit-equal to orx_score_rank_listed on their fp32
+ * upcast; no dispatch record. */
+ORX_API int orx_score_rank_listed_bf16(orx_handle_t h, int32_t kind, const uint16_t* user_tab, int64_t U,
+                                       const int32_t* uid, int32_t Bu, const float* scale, const uint16_t* item_tab,
+                                       const float* item_bias, int64_t I, int32_t dim, const int64_t* pos_off,
+                                       const int32_t* pos_items, const int64_t* neg_off, const int32_t* neg_items,
+                                       const int64_t* excl_off, const int32_t* excl_items, int32_t max_pos,
+                                       const int32_t* at_host, int32_t n_at, float* auc, float* ndcg, float* recall,
+                                       orx_stream_t s);
 /* orx_score_rank_listed over row-sharded tables: the four phases, buffers (sizes from orx_score_rank_shard_sizes),
  * exchange and geometry rules of orx_score_rank_shard.  Phases 0 and 1 are its phases 0 and 1; phase 2 writes
  * xcnt[b, 0] = the AUC count of the eval items this rank owns and xcnt[b, 1..n] the rank hits of the listed items and
@@ -783,6 +818,13 @@ ORX_API int orx_score_topk(orx_handle_t h, int32_t kind, const float* user_tab, 
                            int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
                            int32_t dim, const int64_t* excl_off, const int32_t* excl_items, int32_t k,
                            int32_t* top_items /*[Bu, k]*/, float* top_scores /*[Bu, k], may be NULL*/, orx_stream_t s);
+/* orx_score_topk on bf16 tables (see orx_score_all_bf16): bit-equal to orx_score_topk on their fp32 upcast, with the
+ * same item splits and scratch. */
+ORX_API int orx_score_topk_bf16(orx_handle_t h, int32_t kind, const uint16_t* user_tab, int64_t U, const int32_t* uid,
+                                int32_t Bu, const float* scale, const uint16_t* item_tab, const float* item_bias,
+                                int64_t I, int32_t dim, const int64_t* excl_off, const int32_t* excl_items, int32_t k,
+                                int32_t* top_items /*[Bu, k]*/, float* top_scores /*[Bu, k], may be NULL*/,
+                                orx_stream_t s);
 
 /* ---- sharded top-K retrieval: orx_score_topk over row-sharded user / item tables (orx_rowshard_t, the layout of
  * orx_score_rank_shard), each rank keeping the k best of its own item rows (openrec_b200/sharded.py score_topk_sharded,

@@ -20,7 +20,7 @@ ORX_OPT_MOMENTUM, ORX_OPT_NESTEROV = 6, 8   # 7: unassigned
 ORX_OP_GEMM, ORX_OP_INTERACT_FWD, ORX_OP_INTERACT_BWD, ORX_OP_PAIRWISE_STEP, ORX_OP_POINTWISE_STEP = 0, 1, 2, 3, 4
 ORX_OP_SCORE_RANK, ORX_OP_SCORE_TOPK, ORX_OP_SCORE_RANK_SHARD, ORX_OP_SCORE_TOPK_SHARD = 5, 6, 7, 8
 ORX_OP_POINTWISE_GRAD_ROWS, ORX_OP_CENSOR_SHARD, ORX_OP_CROSS, ORX_OP_PAIRWISE_STEP_BF16 = 9, 10, 11, 12
-ORX_OP_POINTWISE_STEP_BF16 = 13
+ORX_OP_POINTWISE_STEP_BF16, ORX_OP_SCORE_RANK_BF16, ORX_OP_SCORE_TOPK_BF16 = 13, 14, 15
 ORX_VARIANT_GEMM_TMA, ORX_VARIANT_GEMM_SIMT, ORX_VARIANT_INTERACT_WARP, ORX_VARIANT_INTERACT = 0, 1, 2, 3
 ORX_VARIANT_STEP, ORX_VARIANT_STEP_PIPE, ORX_VARIANT_STEP_GENERIC = 4, 5, 6
 ORX_VARIANT_RANK_SMEM, ORX_VARIANT_RANK_GLOBAL, ORX_VARIANT_TOPK = 7, 8, 9
@@ -146,18 +146,24 @@ SIGNATURES = {
                                 _vp, _vp, _vp, _vp, _vp, _vp],
     "orx_dense_apply": [_vp, _vp, _vp, _vp, _vp, _i64, _O, _vp],
     "orx_score_all": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp],
+    "orx_score_all_bf16": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp],
     "orx_sample_pairwise": [_vp, C.POINTER(OrxSampler), _u64, _i64, _i32, _vp, _vp, _vp, _vp],
     "orx_sample_stratified": [_vp, C.POINTER(OrxSampler), _u64, _i64, _i32, _f, _vp, _vp, _vp, _vp, _vp],
     "orx_sample_per_positive": [_vp, C.POINTER(OrxSampler), _u64, _i64, _i32, _i32, _vp, _vp, _vp, _vp],
     "orx_rank_metrics": [_vp, _vp, _vp, _vp, _i32, _i64, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp],
     "orx_score_rank": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _i32,
                        C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp],
+    "orx_score_rank_bf16": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _i32,
+                            C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp],
     "orx_score_topk": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp],
+    "orx_score_topk_bf16": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _i32, _vp, _vp, _vp],
     "orx_score_rank_shard_sizes": [_i32, _i32, _i32, C.POINTER(_i64)],
     "orx_score_rank_shard": [_vp, _i32, _i32, C.POINTER(OrxRowShard), _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp,
                              _i32, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "orx_score_rank_listed": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                               _i32, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp],
+    "orx_score_rank_listed_bf16": [_vp, _i32, _vp, _i64, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp,
+                                   _vp, _i32, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp],
     "orx_score_rank_listed_shard": [_vp, _i32, _i32, C.POINTER(OrxRowShard), _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp,
                                     _vp, _vp, _vp, _vp, _i32, C.POINTER(_i32), _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp],
     "orx_score_topk_shard": [_vp, _i32, _i32, C.POINTER(OrxRowShard), _vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _i32,

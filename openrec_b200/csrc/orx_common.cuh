@@ -424,6 +424,10 @@ __device__ __forceinline__ uint2 orx_bf16x4_sr(float4 v, uint32_t rk, int col) {
   return make_uint2(orx_bf16_sr(v.x, rk, col) | (orx_bf16_sr(v.y, rk, col + 1) << 16),
                     orx_bf16_sr(v.z, rk, col + 2) | (orx_bf16_sr(v.w, rk, col + 3) << 16));
 }
+// 4 bf16 elements as one 8-byte load (p 8-byte aligned), widened exactly
+__device__ __forceinline__ float4 orx_ld4(const uint16_t* p) {
+  return orx_bf16x4_up(*reinterpret_cast<const uint2*>(p));
+}
 __device__ __forceinline__ float4 orx_ld4_stream(const uint16_t* p) {
   return orx_bf16x4_up(__ldcs(reinterpret_cast<const uint2*>(p)));
 }

@@ -31,13 +31,16 @@ namespace {
 constexpr int EV_TU = 128, EV_TI = 128, EV_KC = 8, EV_NT = 256, EV_LD = EV_TU + 4;
 
 // What the tile kernels (k_score_rank, k_score_topk) read.  Kept at this layout: their register allocation is tight.
-struct EvalArgs {
-  const float* user_tab;
+// T: the storage of the user and item tables, float or bf16 held as its uint16_t bits (widened exactly by orx_ld1 as
+// each element is read; scale, bias and every score stay fp32).  The sharded phases take float tables only.
+template <typename T>
+struct EvalArgsT {
+  const T* user_tab;
   int64_t U;
   const int32_t* uid;
   int Bu;
   const float* scale;
-  const float* item_tab;
+  const T* item_tab;
   const float* bias;
   int64_t I;   // item rows the tile loop walks (rows of item_tab / bias)
   int D;
@@ -46,16 +49,19 @@ struct EvalArgs {
   int max_pos;
   int P;  // max_pos + 1: row stride of the threshold and histogram rows
 };
+using EvalArgs = EvalArgsT<float>;
 
 // What the per-row kernels (one CTA per batch row) read on top: the catalogue, the item ownership and the exchange.
-struct EvalRowArgs : EvalArgs {
+template <typename T>
+struct EvalRowArgsT : EvalArgsT<T> {
   int64_t I_all;        // the catalogue: list entries in [0, I_all) count, n_eval = I_all - n - extra
   int world, rank;      // row r is local row r / world on rank r % world (1, 0: the whole table)
-  const float* xrows;   // non-null: batch row b's user row is xrows[b * D ..] (uid still decides bad rows)
+  const T* xrows;       // non-null: batch row b's user row is xrows[b * D ..] (uid still decides bad rows)
   const float* xpred;   // non-null: prep reads the positives' scores from xpred[b * P + q] instead of computing them
   const int64_t* neg_off;      // orx_score_rank_listed: the listed items' CSR (unused by the catalogue pass)
   const int32_t* neg_items;
 };
+using EvalRowArgs = EvalRowArgsT<float>;
 
 // Scratch of one call (handle workspace).  keys_in / keys: [2][Bu][P] -- pred thresholds of row b at b * P, sp
 // thresholds at (Bu + b) * P; keys holds them sorted ascending.  info[2b] = positives of row b (-1: longer than
@@ -77,22 +83,27 @@ struct EvalOut {
 };
 
 // XROWS: user_tab holds one row per batch position (the summed exchange of the sharded pass), not per user id
-template <bool XROWS>
-__device__ __forceinline__ const float* ev_user_row(const EvalArgs& a, int b) {
+template <bool XROWS, typename T>
+__device__ __forceinline__ const T* ev_user_row(const EvalArgsT<T>& a, int b) {
   const int32_t id = a.uid[b];
   return (id >= 0 && (int64_t)id < a.U) ? a.user_tab + (int64_t)(XROWS ? b : id) * a.D : nullptr;
 }
-__device__ __forceinline__ const float* ev_urow(const EvalRowArgs& a, int b) {
+template <typename T>
+__device__ __forceinline__ const T* ev_urow(const EvalRowArgsT<T>& a, int b) {
   if (!a.xrows) return ev_user_row<false>(a, b);
   const int32_t id = a.uid[b];
   return (id >= 0 && (int64_t)id < a.U) ? a.xrows + (int64_t)b * a.D : nullptr;
 }
 
 // ownership of a (user or item) id in [0, 2^31): row r lives on rank r % world at local row r / world
-__device__ __forceinline__ bool ev_owns(const EvalRowArgs& a, int32_t r) {
+template <typename T>
+__device__ __forceinline__ bool ev_owns(const EvalRowArgsT<T>& a, int32_t r) {
   return (uint32_t)r % (uint32_t)a.world == (uint32_t)a.rank;
 }
-__device__ __forceinline__ int64_t ev_local(const EvalRowArgs& a, int32_t r) { return (uint32_t)r / (uint32_t)a.world; }
+template <typename T>
+__device__ __forceinline__ int64_t ev_local(const EvalRowArgsT<T>& a, int32_t r) {
+  return (uint32_t)r / (uint32_t)a.world;
+}
 
 // first position in items[lo, hi) holding a value >= v (the row is sorted)
 __device__ __forceinline__ int64_t ev_lower(const int32_t* items, int64_t lo, int64_t hi, int64_t v) {
@@ -122,10 +133,11 @@ __device__ __forceinline__ bool ev_contains(const int32_t* items, int64_t lo, in
 
 // The user value at k of the chain of k_score_all (urow nullptr: a zero row).  Explicit roundings: u * scale - i must
 // not contract into one fused multiply-add.
-__device__ __forceinline__ float ev_uval(const EvalArgs& a, const float* urow, int k) {
+template <typename T>
+__device__ __forceinline__ float ev_uval(const EvalArgsT<T>& a, const T* urow, int k) {
   float uv = 0.f;
   if (urow) {
-    uv = urow[k];
+    uv = orx_ld1(urow + k);
     if (a.scale) uv = __fmul_rn(uv, a.scale[k]);
   }
   return uv;
@@ -140,12 +152,12 @@ __device__ __forceinline__ float ev_step(float acc, float uv, float iv) {
 }
 
 // One score by the chain of k_score_all, of an item i this rank owns (ev_owns).
-template <int KIND>
-__device__ __forceinline__ float ev_score1(const EvalRowArgs& a, const float* urow, int32_t i_global) {
+template <int KIND, typename T>
+__device__ __forceinline__ float ev_score1(const EvalRowArgsT<T>& a, const T* urow, int32_t i_global) {
   const int64_t i = ev_local(a, i_global);
-  const float* irow = a.item_tab + i * a.D;
+  const T* irow = a.item_tab + i * a.D;
   float acc = 0.f;
-  for (int k = 0; k < a.D; ++k) acc = ev_step<KIND>(acc, ev_uval(a, urow, k), irow[k]);
+  for (int k = 0; k < a.D; ++k) acc = ev_step<KIND>(acc, ev_uval(a, urow, k), orx_ld1(irow + k));
   return acc + (a.bias ? a.bias[i] : 0.f);
 }
 
@@ -188,7 +200,8 @@ struct EvRow {
   bool bad;
 };
 
-__device__ __forceinline__ EvRow ev_row(const EvalRowArgs& a, int b) {
+template <typename T>
+__device__ __forceinline__ EvRow ev_row(const EvalRowArgsT<T>& a, int b) {
   EvRow r;
   int64_t praw, eraw;
   const int32_t u = a.uid[b];
@@ -198,11 +211,11 @@ __device__ __forceinline__ EvRow ev_row(const EvalRowArgs& a, int b) {
   return r;
 }
 
-template <int KIND>
-__global__ void __launch_bounds__(EV_NT) k_eval_prep(const EvalRowArgs a, const EvalWs w) {
+template <int KIND, typename T>
+__global__ void __launch_bounds__(EV_NT) k_eval_prep(const EvalRowArgsT<T> a, const EvalWs w) {
   __shared__ int s_nan, s_kp;
   const int b = blockIdx.x;
-  const float* urow = ev_urow(a, b);
+  const T* urow = ev_urow(a, b);
   const EvRow r = ev_row(a, b);
   const int64_t plo = r.plo, elo = r.elo, ehi = r.ehi;
   const bool bad = r.bad;
@@ -270,8 +283,9 @@ __global__ void __launch_bounds__(EV_NT) k_eval_pos_scores(const EvalRowArgs a, 
 // shared tile.  A CTA takes one user tile and walks a contiguous range of item tiles; the thresholds and histograms
 // of its rows sit in shared memory (USE_SMEM) or stay in the global scratch, reached through the same generic pointers.
 // ---------------------------------------------------------------------------------------
+template <typename T>
 struct RowMeta {
-  const float* urow;
+  const T* urow;
   const float* pth;
   const float* sth;
   unsigned* hist;
@@ -313,38 +327,70 @@ __device__ __forceinline__ void ev_mma_chunk(float (&acc)[8][8], const float (*s
 // through the double-buffered shared tiles sA / sB.  After each tile every thread calls epi(i0, acc): acc[x][y] is the
 // score of row ev_frag(ty, x) and item i0 + ev_frag(tx, y) before the bias, by the chain of k_score_all.  Every thread
 // passes a __syncthreads after epi returns and before the next tile's scores are read.
-template <int KIND, class UrowOf, class Epi>
-__device__ __forceinline__ void ev_tiles(const EvalArgs& a, float (*sA)[EV_KC][EV_LD], float (*sB)[EV_KC][EV_LD],
+// VEC (bf16 tables only, dim % 4 == 0, both tables 8-byte aligned: ev_vec): each thread moves 4 columns of one row of
+// each table as one 8-byte load, where the scalar loader makes 4 two-byte loads.  The loaders differ only in which
+// thread carries which element, so the shared tiles, and every score, are the same bits.
+template <int KIND, bool VEC, typename T, class UrowOf, class Epi>
+__device__ __forceinline__ void ev_tiles(const EvalArgsT<T>& a, float (*sA)[EV_KC][EV_LD], float (*sB)[EV_KC][EV_LD],
                                          UrowOf urow_of, Epi epi) {
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const int64_t n_tiles = (a.I + EV_TI - 1) / EV_TI;
   const int64_t t_begin = n_tiles * blockIdx.x / gridDim.x, t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
   const int n_chunks = (a.D + EV_KC - 1) / EV_KC;
   float ru[4], ri[4];
-  // chunk k0 of this tile into registers: element e = tid + 256 j is row e / 8, k e % 8
+  // chunk k0 of this tile into registers: element e = tid + 256 j is row e / 8, k e % 8; with VEC, thread tid holds
+  // row tid / 2, k (tid % 2) * 4 + j
   auto load = [&](int64_t i0, int k0) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int e = tid + EV_NT * j, r = e >> 3, k = k0 + (e & 7);
-      float uv = 0.f, iv = 0.f;
-      if (k < a.D) {
-        const float* urow = urow_of(r);
+    if constexpr (VEC) {
+      const int r = tid >> 1, k = k0 + (tid & 1) * 4;
+      float4 uv = make_float4(0.f, 0.f, 0.f, 0.f), iv = uv;
+      if (k < a.D) {   // dim % 4 == 0: the 4 columns are all inside the row or all past it
+        const T* urow = urow_of(r);
         if (urow) {
-          uv = urow[k];
-          if (a.scale) uv = __fmul_rn(uv, a.scale[k]);
+          uv = orx_ld4(urow + k);
+          if (a.scale) {
+            uv.x = __fmul_rn(uv.x, a.scale[k]);
+            uv.y = __fmul_rn(uv.y, a.scale[k + 1]);
+            uv.z = __fmul_rn(uv.z, a.scale[k + 2]);
+            uv.w = __fmul_rn(uv.w, a.scale[k + 3]);
+          }
         }
-        if (i0 + r < a.I) iv = a.item_tab[(i0 + r) * a.D + k];
+        if (i0 + r < a.I) iv = orx_ld4(a.item_tab + (i0 + r) * a.D + k);
       }
-      ru[j] = uv;
-      ri[j] = iv;
+      ru[0] = uv.x; ru[1] = uv.y; ru[2] = uv.z; ru[3] = uv.w;
+      ri[0] = iv.x; ri[1] = iv.y; ri[2] = iv.z; ri[3] = iv.w;
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int e = tid + EV_NT * j, r = e >> 3, k = k0 + (e & 7);
+        float uv = 0.f, iv = 0.f;
+        if (k < a.D) {
+          const T* urow = urow_of(r);
+          if (urow) {
+            uv = orx_ld1(urow + k);
+            if (a.scale) uv = __fmul_rn(uv, a.scale[k]);
+          }
+          if (i0 + r < a.I) iv = orx_ld1(a.item_tab + (i0 + r) * a.D + k);
+        }
+        ru[j] = uv;
+        ri[j] = iv;
+      }
     }
   };
   auto store = [&](int buf) {
+    if constexpr (VEC) {   // rows tid / 2 of a warp's 16 row pairs: banks (4k + r) % 32 of the two halves are disjoint
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int e = tid + EV_NT * j;
-      sA[buf][e & 7][e >> 3] = ru[j];
-      sB[buf][e & 7][e >> 3] = ri[j];
+      for (int j = 0; j < 4; ++j) {
+        sA[buf][(tid & 1) * 4 + j][tid >> 1] = ru[j];
+        sB[buf][(tid & 1) * 4 + j][tid >> 1] = ri[j];
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int e = tid + EV_NT * j;
+        sA[buf][e & 7][e >> 3] = ru[j];
+        sB[buf][e & 7][e >> 3] = ri[j];
+      }
     }
   };
 
@@ -370,12 +416,12 @@ __device__ __forceinline__ void ev_tiles(const EvalArgs& a, float (*sA)[EV_KC][E
   }
 }
 
-template <int KIND, bool XROWS>
-__global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const EvalWs w, int use_smem) {
+template <int KIND, bool XROWS, typename T, bool VEC = false>
+__global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgsT<T> a, const EvalWs w, int use_smem) {
   extern __shared__ float4 ev_dyn4[];
   __shared__ __align__(16) float sA[2][EV_KC][EV_LD];
   __shared__ __align__(16) float sB[2][EV_KC][EV_LD];
-  __shared__ RowMeta meta[EV_TU];
+  __shared__ RowMeta<T> meta[EV_TU];
   __shared__ unsigned long long s_auc[EV_TU];
   float* dyn = reinterpret_cast<float*>(ev_dyn4);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -386,7 +432,7 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
   const int64_t P = a.P;
 
   if (tid < EV_TU) {
-    RowMeta m = {};
+    RowMeta<T> m = {};
     if (tid < rows) {
       const int b = u0 + tid;
       m.urow = ev_user_row<XROWS>(a, b);
@@ -409,7 +455,7 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
   if (use_smem) {
     for (int r = warp; r < rows; r += EV_NT / 32) {
       const int b = u0 + r;
-      const RowMeta& m = meta[r];
+      const RowMeta<T>& m = meta[r];
       float* pth = const_cast<float*>(m.pth);
       float* sth = const_cast<float*>(m.sth);
       for (int q = lane; q < m.n; q += 32) {
@@ -421,7 +467,7 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
     __syncthreads();
   }
   if (tid < rows) {
-    RowMeta& m = meta[tid];
+    RowMeta<T>& m = meta[tid];
     m.pmin = m.n_auc ? m.pth[0] : __int_as_float(0x7f800000);
     m.pmax = m.n_auc ? m.pth[m.n_auc - 1] : __int_as_float(0xff800000);
     m.smin = m.n ? m.sth[0] : __int_as_float(0x7f800000);
@@ -430,7 +476,7 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
   __syncthreads();
 
   // epilogue: the AUC terms and rank hits of each tile's scores
-  ev_tiles<KIND>(a, sA, sB, [&](int r) { return meta[r].urow; }, [&](int64_t i0, const float (&acc)[8][8]) {
+  ev_tiles<KIND, VEC>(a, sA, sB, [&](int r) { return meta[r].urow; }, [&](int64_t i0, const float (&acc)[8][8]) {
     float bv[8];
 #pragma unroll
     for (int y = 0; y < 8; ++y) {
@@ -441,7 +487,7 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
     for (int x = 0; x < 8; ++x) {
       const int r = ev_frag(ty, x);
       if (r >= rows) continue;
-      const RowMeta& m = meta[r];
+      const RowMeta<T>& m = meta[r];
       if (m.n == 0) continue;
       unsigned long long cnt = 0ull;
 #pragma unroll
@@ -457,7 +503,7 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
   });
   __syncthreads();
   for (int r = warp; r < rows; r += EV_NT / 32) {
-    const RowMeta& m = meta[r];
+    const RowMeta<T>& m = meta[r];
     if (use_smem)
       for (int j = 1 + lane; j <= m.n; j += 32) {
         const unsigned h = m.hist[j];
@@ -477,12 +523,12 @@ __global__ void __launch_bounds__(EV_NT, 2) k_score_rank(const EvalArgs a, const
 // owns (the main pass counted them as eval items) and takes their rank hits off hist (excluded items only: an excluded
 // item's sp is 0 or NaN and never ranks above anything); adds to *s_extra the excluded items that are not positives,
 // owned or not.  TAKE = false: *s_extra only (no scores, no thresholds).
-template <int KIND, bool TAKE>
-__device__ __forceinline__ void ev_take_back(const EvalRowArgs& a, int b, const EvRow& r, int n, int n_auc,
+template <int KIND, bool TAKE, typename T>
+__device__ __forceinline__ void ev_take_back(const EvalRowArgsT<T>& a, int b, const EvRow& r, int n, int n_auc,
                                              const float* pth, const float* sth, unsigned* hist,
                                              unsigned long long* s_sub, long long* s_extra) {
   const int tid = threadIdx.x;
-  const float* urow = TAKE ? ev_urow(a, b) : nullptr;
+  const T* urow = TAKE ? ev_urow(a, b) : nullptr;
   float pmin = 0.f, pmax = 0.f, smin = 0.f, smax = 0.f;
   if (TAKE) {
     pmin = n_auc ? pth[0] : __int_as_float(0x7f800000);
@@ -528,8 +574,8 @@ __device__ __forceinline__ void ev_nan_row(const EvalOut& o, int b) {   // a pos
 
 // The outputs of row b from its final counts: auc_cnt, and hist_at(j) for j = 1..n (the rank hits).  Block-wide; every
 // thread must call it.
-template <class Hist>
-__device__ __forceinline__ void ev_finish_row(const EvalRowArgs& a, const EvalOut& o, int b, int n, long long extra,
+template <typename T, class Hist>
+__device__ __forceinline__ void ev_finish_row(const EvalRowArgsT<T>& a, const EvalOut& o, int b, int n, long long extra,
                                               unsigned long long auc_cnt, Hist hist_at) {
   __shared__ unsigned s_part[EV_NT];
   __shared__ unsigned s_after[EV_NT];
@@ -591,8 +637,8 @@ __device__ __forceinline__ void ev_finish_row(const EvalRowArgs& a, const EvalOu
   }
 }
 
-template <int KIND>
-__global__ void __launch_bounds__(EV_NT) k_eval_finish(const EvalRowArgs a, const EvalWs w, const EvalOut o) {
+template <int KIND, typename T>
+__global__ void __launch_bounds__(EV_NT) k_eval_finish(const EvalRowArgsT<T> a, const EvalWs w, const EvalOut o) {
   __shared__ unsigned long long s_sub;
   __shared__ long long s_extra;
   const int b = blockIdx.x, tid = threadIdx.x;
@@ -669,13 +715,15 @@ constexpr int EL_LD = 33;    // slab row stride, odd: thread t reading row t mee
 constexpr int EL_UNR = 4;    // rows each warp has in flight while staging a slab
 
 // Whether listed entry q of row r (an entry in [0, I_all)) is an eval item: neither a positive nor excluded.
-__device__ __forceinline__ bool el_eval_item(const EvalRowArgs& a, const EvRow& r, int64_t q) {
+template <typename T>
+__device__ __forceinline__ bool el_eval_item(const EvalRowArgsT<T>& a, const EvRow& r, int64_t q) {
   const int32_t i = a.neg_items[q];
   return !ev_contains(a.pos_items, r.plo, r.phi, i) && !ev_contains(a.excl_items, r.elo, r.ehi, i);
 }
 
 // The listed entries of batch row b in [0, I_all): [*lo, *hi).
-__device__ __forceinline__ void el_range(const EvalRowArgs& a, int b, int64_t* lo, int64_t* hi) {
+template <typename T>
+__device__ __forceinline__ void el_range(const EvalRowArgsT<T>& a, int b, int64_t* lo, int64_t* hi) {
   int64_t raw;
   ev_range(a.neg_off, a.neg_items, a.uid[b], a.U, a.I_all, lo, hi, &raw);
 }
@@ -686,9 +734,9 @@ __device__ __forceinline__ void el_range(const EvalRowArgs& a, int b, int64_t* l
 // 128-byte load per item row, and each thread runs the chain of ev_score1 (ascending k) over the slabs.
 // xcnt == nullptr: the outputs by ev_finish_row.  Else (sharded phase 2): xcnt[b][0] = the AUC count, xcnt[b][1..n]
 // the rank hits, the rest of the row 0 (every element written).
-template <int KIND>
-__global__ void __launch_bounds__(EV_NT, 3) k_eval_listed(const EvalRowArgs a, const EvalWs w, const EvalOut o,
-                                                       int64_t* xcnt) {
+template <int KIND, typename T>
+__global__ void __launch_bounds__(EV_NT, 3) k_eval_listed(const EvalRowArgsT<T> a, const EvalWs w, const EvalOut o,
+                                                          int64_t* xcnt) {
   __shared__ float s_rows[EV_NT * EL_LD];
   __shared__ float s_u[EL_KS];
   __shared__ int32_t s_row[EV_NT];     // local item row of chunk entry t, -1: not scored on this rank
@@ -715,7 +763,7 @@ __global__ void __launch_bounds__(EV_NT, 3) k_eval_listed(const EvalRowArgs a, c
   const EvRow r = ev_row(a, b);
   int64_t lo, hi;
   el_range(a, b, &lo, &hi);
-  const float* urow = ev_urow(a, b);
+  const T* urow = ev_urow(a, b);
   if (tid == 0) {
     s_auc = 0ull;
     s_eval = 0;
@@ -748,7 +796,7 @@ __global__ void __launch_bounds__(EV_NT, 3) k_eval_listed(const EvalRowArgs a, c
         for (int x = 0; x < EL_UNR; ++x) {
           const int t = t0 + (EV_NT / 32) * x;
           const int32_t rt = t < nc ? s_row[t] : -1;
-          v[x] = rt >= 0 && lane < ks ? a.item_tab[(int64_t)rt * a.D + k0 + lane] : 0.f;
+          v[x] = rt >= 0 && lane < ks ? orx_ld1(a.item_tab + (int64_t)rt * a.D + k0 + lane) : 0.f;
         }
 #pragma unroll
         for (int x = 0; x < EL_UNR; ++x) {
@@ -903,19 +951,20 @@ __device__ unsigned long long tk_kth(Each each, int k, unsigned* hist, unsigned 
 // Main pass: the tile loop of k_score_rank with a top-K epilogue.  Row r of the CTA's user tile keeps a threshold key
 // (0 until its list is first cut) and appends every eligible key above it to its list in the scratch.  Cutting a list
 // (one warp) keeps its exact top k, and the threshold becomes the k-th key.
+template <typename T>
 struct TkRow {
-  const float* urow;
+  const T* urow;
   int64_t elo, ehi;   // the row's exclusion entries in [0, I)
 };
 
 // SHARD: the tile loop walks this rank's a.I local rows of a row-sharded table (local row i is item i * world + rank of
 // [0, I_all)) and takes user rows by batch position (a.user_tab = the summed exchange); keys and the exclusion lookup
 // use the global item id, so keys stay unique across ranks and equal scores order by global id as on one device.
-template <int KIND, bool SHARD>
-__device__ __forceinline__ void tk_main(const EvalArgs& a, const TopkWs& w, int k, int world, int rank, int64_t I_all) {
+template <int KIND, bool SHARD, typename T, bool VEC = false>
+__device__ __forceinline__ void tk_main(const EvalArgsT<T>& a, const TopkWs& w, int k, int world, int rank, int64_t I_all) {
   __shared__ __align__(16) float sA[2][EV_KC][EV_LD];
   __shared__ __align__(16) float sB[2][EV_KC][EV_LD];
-  __shared__ TkRow meta[EV_TU];
+  __shared__ TkRow<T> meta[EV_TU];
   __shared__ unsigned long long s_thr[EV_TU];
   __shared__ int s_cnt[EV_TU];
   __shared__ unsigned s_hist[EV_NT / 32][256];
@@ -954,7 +1003,7 @@ __device__ __forceinline__ void tk_main(const EvalArgs& a, const TopkWs& w, int 
   };
 
   if (tid < EV_TU) {
-    TkRow m = {};
+    TkRow<T> m = {};
     if (tid < rows) {
       int64_t raw;
       m.urow = ev_user_row<SHARD>(a, u0 + tid);
@@ -966,7 +1015,7 @@ __device__ __forceinline__ void tk_main(const EvalArgs& a, const TopkWs& w, int 
   }
   __syncthreads();
 
-  ev_tiles<KIND>(a, sA, sB, [&](int r) { return meta[r].urow; }, [&](int64_t i0, const float (&acc)[8][8]) {
+  ev_tiles<KIND, VEC>(a, sA, sB, [&](int r) { return meta[r].urow; }, [&](int64_t i0, const float (&acc)[8][8]) {
     float bv[8];
 #pragma unroll
     for (int y = 0; y < 8; ++y) {
@@ -996,9 +1045,9 @@ __device__ __forceinline__ void tk_main(const EvalArgs& a, const TopkWs& w, int 
   if (tid < rows) w.cnt[(int64_t)(u0 + tid) * gridDim.x + blockIdx.x] = s_cnt[tid];
 }
 
-template <int KIND>
-__global__ void __launch_bounds__(EV_NT, 2) k_score_topk(const EvalArgs a, const TopkWs w, int k) {
-  tk_main<KIND, false>(a, w, k, 1, 0, a.I);
+template <int KIND, typename T, bool VEC = false>
+__global__ void __launch_bounds__(EV_NT, 2) k_score_topk(const EvalArgsT<T> a, const TopkWs w, int k) {
+  tk_main<KIND, false, T, VEC>(a, w, k, 1, 0, a.I);
 }
 
 // Sharded phase 1's main pass (a.user_tab: the summed user rows of phase 0, by batch position).
@@ -1123,6 +1172,14 @@ size_t ev_layout(char* base, int Bu, int P, size_t sort_bytes, EvalWs* w) {
   return m.off;
 }
 
+// Whether a call's tile loop runs the VEC loader of ev_tiles: bf16 tables, dim % 4 == 0 and both tables 8-byte
+// aligned (so is every row start).  Any other table takes the scalar loader, with the same bits.
+template <typename T>
+bool ev_vec(const EvalArgsT<T>& a) {
+  const uintptr_t bases = reinterpret_cast<uintptr_t>(a.user_tab) | reinterpret_cast<uintptr_t>(a.item_tab);
+  return std::is_same<T, uint16_t>::value && a.D % 4 == 0 && bases % 8 == 0;
+}
+
 // Item splits of a grid of user tiles x item splits for kern at dyn bytes of dynamic shared memory: enough CTAs for one
 // wave over the SMs, at most one item tile per CTA.
 template <class Kern>
@@ -1150,8 +1207,8 @@ int ev_workspace(orx_ctx* h, int Bu, int P, cudaStream_t st, EvalWs* w) {
 }
 
 // prep and the segmented sort: every batch row's sorted thresholds, zeroed histogram and AUC count in w.
-template <int KIND>
-int ev_prep_sort(const EvalRowArgs& a, const EvalWs& w, cudaStream_t st) {
+template <int KIND, typename T>
+int ev_prep_sort(const EvalRowArgsT<T>& a, const EvalWs& w, cudaStream_t st) {
   k_eval_prep<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w);
   ORX_LAUNCH_CHECK();
   size_t bytes = w.sort_bytes;
@@ -1163,9 +1220,11 @@ int ev_prep_sort(const EvalRowArgs& a, const EvalWs& w, cudaStream_t st) {
 // prep, sort and the main pass over the a.I item rows (no main pass when a.I == 0): the thresholds, AUC counts and
 // rank histograms of every batch row in w, before the take-back.  *variant / *splits: the main pass's dispatch fields
 // (splits 0: not launched).
-template <int KIND, bool XROWS>
-int ev_count(orx_ctx* h, const EvalRowArgs& a, const EvalWs& w, cudaStream_t st, int* variant, int64_t* splits) {
-  auto kern = k_score_rank<KIND, XROWS>;
+template <int KIND, bool XROWS, typename T>
+int ev_count(orx_ctx* h, const EvalRowArgsT<T>& a, const EvalWs& w, cudaStream_t st, int* variant, int64_t* splits) {
+  auto kern = k_score_rank<KIND, XROWS, T, false>;
+  if constexpr (std::is_same<T, uint16_t>::value)
+    if (ev_vec(a)) kern = k_score_rank<KIND, XROWS, T, true>;
   int optin = 0;
   ORX_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, h->device));
   cudaFuncAttributes fa;
@@ -1188,7 +1247,7 @@ int ev_count(orx_ctx* h, const EvalRowArgs& a, const EvalWs& w, cudaStream_t st,
   const int rc = ev_prep_sort<KIND>(a, w, st);
   if (rc != ORX_OK) return rc;
   if (*splits > 0) {
-    EvalArgs t = a;
+    EvalArgsT<T> t = a;
     if (XROWS) t.user_tab = a.xrows;
     kern<<<dim3((unsigned)*splits, (unsigned)user_tiles), EV_NT, dyn, st>>>(t, w, use_smem);
     ORX_LAUNCH_CHECK();
@@ -1196,16 +1255,20 @@ int ev_count(orx_ctx* h, const EvalRowArgs& a, const EvalWs& w, cudaStream_t st,
   return ORX_OK;
 }
 
-template <int KIND>
-int ev_launch(orx_ctx* h, const EvalRowArgs& a, const EvalWs& w, const EvalOut& o, cudaStream_t st) {
+// The dispatch op of an orx_score_rank / orx_score_topk call on tables of storage T.
+template <typename T>
+constexpr int ev_op(int op_fp32, int op_bf16) { return std::is_same<T, uint16_t>::value ? op_bf16 : op_fp32; }
+
+template <int KIND, typename T>
+int ev_launch(orx_ctx* h, const EvalRowArgsT<T>& a, const EvalWs& w, const EvalOut& o, cudaStream_t st) {
   int variant = 0;
   int64_t splits = 0;
   const int rc = ev_count<KIND, false>(h, a, w, st, &variant, &splits);
   if (rc != ORX_OK) return rc;
   k_eval_finish<KIND><<<a.Bu, EV_NT, 0, st>>>(a, w, o);
   ORX_LAUNCH_CHECK();
-  orx_log_dispatch(h, ORX_OP_SCORE_RANK, variant, KIND, 0, a.Bu, (int)(a.I > INT32_MAX ? INT32_MAX : a.I), a.D,
-                   (int)splits);
+  orx_log_dispatch(h, ev_op<T>(ORX_OP_SCORE_RANK, ORX_OP_SCORE_RANK_BF16), variant, KIND, 0, a.Bu,
+                   (int)(a.I > INT32_MAX ? INT32_MAX : a.I), a.D, (int)splits);
   return ORX_OK;
 }
 
@@ -1217,8 +1280,8 @@ void ev_user_rows(const EvalRowArgs& a, int32_t* xrows, cudaStream_t st) {
 
 // orx_score_rank_listed's counts of every batch row from the handle's evaluation scratch: its outputs (xcnt nullptr),
 // or phase 2 of orx_score_rank_listed_shard (the counts into xcnt).
-template <int KIND>
-int el_launch(orx_ctx* h, const EvalRowArgs& a, const EvalOut& o, int64_t* xcnt, cudaStream_t st) {
+template <int KIND, typename T>
+int el_launch(orx_ctx* h, const EvalRowArgsT<T>& a, const EvalOut& o, int64_t* xcnt, cudaStream_t st) {
   EvalWs w;
   int rc = ev_workspace(h, a.Bu, a.P, st, &w);
   if (rc != ORX_OK) return rc;
@@ -1271,8 +1334,8 @@ size_t tk_layout(char* base, int Bu, int64_t splits, int k, TopkWs* w) {
 }
 
 // The item splits of kern over a.I rows and the top-K scratch for them, from the handle's evaluation scratch.
-template <class Kern>
-int tk_workspace(orx_ctx* h, Kern kern, const EvalArgs& a, int k, int64_t* splits, TopkWs* w) {
+template <class Kern, typename T>
+int tk_workspace(orx_ctx* h, Kern kern, const EvalArgsT<T>& a, int k, int64_t* splits, TopkWs* w) {
   int rc = ev_item_splits(h, kern, 0, a.Bu, a.I, splits);
   if (rc != ORX_OK) return rc;
   rc = orx_grow(&h->eval_ws, &h->eval_cap, tk_layout(nullptr, a.Bu, *splits, k, w));
@@ -1281,18 +1344,22 @@ int tk_workspace(orx_ctx* h, Kern kern, const EvalArgs& a, int k, int64_t* split
   return ORX_OK;
 }
 
-template <int KIND>
-int tk_launch(orx_ctx* h, const EvalArgs& a, int k, int32_t* top_items, float* top_scores, cudaStream_t st) {
+template <int KIND, typename T>
+int tk_launch(orx_ctx* h, const EvalArgsT<T>& a, int k, int32_t* top_items, float* top_scores, cudaStream_t st) {
   int64_t splits = 1;
   TopkWs w;
-  const int rc = tk_workspace(h, k_score_topk<KIND>, a, k, &splits, &w);
+  auto kern = k_score_topk<KIND, T, false>;
+  if constexpr (std::is_same<T, uint16_t>::value)
+    if (ev_vec(a)) kern = k_score_topk<KIND, T, true>;
+  const int rc = tk_workspace(h, kern, a, k, &splits, &w);
   if (rc != ORX_OK) return rc;
   const int64_t user_tiles = (a.Bu + EV_TU - 1) / EV_TU;
-  k_score_topk<KIND><<<dim3((unsigned)splits, (unsigned)user_tiles), EV_NT, 0, st>>>(a, w, k);
+  kern<<<dim3((unsigned)splits, (unsigned)user_tiles), EV_NT, 0, st>>>(a, w, k);
   ORX_LAUNCH_CHECK();
   k_topk_merge<<<a.Bu, EV_NT, 0, st>>>(w, (int)splits, k, top_items, top_scores);
   ORX_LAUNCH_CHECK();
-  orx_log_dispatch(h, ORX_OP_SCORE_TOPK, ORX_VARIANT_TOPK, KIND, k, a.Bu, (int)a.I, a.D, (int)splits);
+  orx_log_dispatch(h, ev_op<T>(ORX_OP_SCORE_TOPK, ORX_OP_SCORE_TOPK_BF16), ORX_VARIANT_TOPK, KIND, k, a.Bu, (int)a.I,
+                   a.D, (int)splits);
   return ORX_OK;
 }
 
@@ -1326,8 +1393,8 @@ EvalOut ev_out(const int32_t* at_host, int n_at, float* auc, float* ndcg, float*
 }
 
 // Why orx_score_rank / orx_score_rank_listed refuse their arguments, or nullptr (the size limit only for Bu > 0).
-const char* ev_rank_refusal(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
-                            int32_t Bu, const float* item_tab, int64_t I, int32_t dim, const int64_t* pos_off,
+const char* ev_rank_refusal(orx_handle_t h, int32_t kind, const void* user_tab, int64_t U, const int32_t* uid,
+                            int32_t Bu, const void* item_tab, int64_t I, int32_t dim, const int64_t* pos_off,
                             int32_t max_pos, const int32_t* at_host, int32_t n_at) {
   if (!(h != nullptr && user_tab && uid && item_tab && pos_off)) return "null pointer";
   if (!(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST)) return "unknown score kind";
@@ -1340,11 +1407,12 @@ const char* ev_rank_refusal(orx_handle_t h, int32_t kind, const float* user_tab,
 }
 
 // The row arguments of a checked orx_score_rank / orx_score_rank_listed call (neg_off nullptr for the former).
-EvalRowArgs ev_rank_args(const float* user_tab, int64_t U, const int32_t* uid, int32_t Bu, const float* scale,
-                         const float* item_tab, const float* item_bias, int64_t I, int32_t dim, const int64_t* pos_off,
-                         const int32_t* pos_items, const int64_t* neg_off, const int32_t* neg_items,
-                         const int64_t* excl_off, const int32_t* excl_items, int32_t max_pos) {
-  EvalRowArgs a = {};
+template <typename T>
+EvalRowArgsT<T> ev_rank_args(const T* user_tab, int64_t U, const int32_t* uid, int32_t Bu, const float* scale,
+                             const T* item_tab, const float* item_bias, int64_t I, int32_t dim, const int64_t* pos_off,
+                             const int32_t* pos_items, const int64_t* neg_off, const int32_t* neg_items,
+                             const int64_t* excl_off, const int32_t* excl_items, int32_t max_pos) {
+  EvalRowArgsT<T> a = {};
   a.user_tab = user_tab; a.U = U; a.uid = uid; a.Bu = Bu; a.scale = scale; a.item_tab = item_tab;
   a.bias = item_bias; a.I = I; a.I_all = I; a.world = 1; a.rank = 0; a.D = dim; a.pos_off = pos_off;
   a.excl_off = excl_off; a.pos_items = pos_items; a.excl_items = excl_items; a.max_pos = max_pos; a.P = max_pos + 1;
@@ -1397,13 +1465,14 @@ EvalRowArgs ev_shard_args(int32_t phase, const orx_rowshard_t& g, const float* u
   return a;
 }
 
-}  // namespace
-
-extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
-                              int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
-                              int32_t dim, const int64_t* pos_off, const int32_t* pos_items, const int64_t* excl_off,
-                              const int32_t* excl_items, int32_t max_pos, const int32_t* at_host, int32_t n_at,
-                              float* auc, float* ndcg, float* recall, orx_stream_t s) {
+// orx_score_rank, orx_score_rank_listed and orx_score_topk on tables of storage T (float, or bf16 bits): one body for
+// both forms, so the bf16 entries refuse, size and dispatch exactly as the fp32 ones.
+template <typename T>
+int score_rank_impl(orx_handle_t h, int32_t kind, const T* user_tab, int64_t U, const int32_t* uid, int32_t Bu,
+                    const float* scale, const T* item_tab, const float* item_bias, int64_t I, int32_t dim,
+                    const int64_t* pos_off, const int32_t* pos_items, const int64_t* excl_off, const int32_t* excl_items,
+                    int32_t max_pos, const int32_t* at_host, int32_t n_at, float* auc, float* ndcg, float* recall,
+                    orx_stream_t s) {
   const char* why = ev_rank_refusal(h, kind, user_tab, U, uid, Bu, item_tab, I, dim, pos_off, max_pos, at_host, n_at);
   ORX_REQUIRE(why == nullptr, why);
   if (Bu == 0) return ORX_OK;
@@ -1414,11 +1483,71 @@ extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_ta
   const int rc = ev_workspace(h, Bu, max_pos + 1, st, &w);
   if (rc != ORX_OK) return rc;
 
-  const EvalRowArgs a = ev_rank_args(user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, pos_off, pos_items,
-                                     nullptr, nullptr, excl_off, excl_items, max_pos);
+  const EvalRowArgsT<T> a = ev_rank_args(user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, pos_off, pos_items,
+                                         nullptr, nullptr, excl_off, excl_items, max_pos);
   const EvalOut o = ev_out(at_host, n_at, auc, ndcg, recall);
   return kind == ORX_SCORE_DOT ? ev_launch<ORX_SCORE_DOT>(h, a, w, o, st)
                                : ev_launch<ORX_SCORE_NEG_SQDIST>(h, a, w, o, st);
+}
+
+template <typename T>
+int score_rank_listed_impl(orx_handle_t h, int32_t kind, const T* user_tab, int64_t U, const int32_t* uid, int32_t Bu,
+                           const float* scale, const T* item_tab, const float* item_bias, int64_t I, int32_t dim,
+                           const int64_t* pos_off, const int32_t* pos_items, const int64_t* neg_off,
+                           const int32_t* neg_items, const int64_t* excl_off, const int32_t* excl_items,
+                           int32_t max_pos, const int32_t* at_host, int32_t n_at, float* auc, float* ndcg,
+                           float* recall, orx_stream_t s) {
+  const char* why = ev_rank_refusal(h, kind, user_tab, U, uid, Bu, item_tab, I, dim, pos_off, max_pos, at_host, n_at);
+  ORX_REQUIRE(why == nullptr, why);
+  ORX_REQUIRE(neg_off != nullptr, "null pointer");
+  if (Bu == 0) return ORX_OK;
+  ORX_CUDA(cudaSetDevice(h->device));
+  const EvalRowArgsT<T> a = ev_rank_args(user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, pos_off, pos_items,
+                                         neg_off, neg_items, excl_off, excl_items, max_pos);
+  const EvalOut o = ev_out(at_host, n_at, auc, ndcg, recall);
+  cudaStream_t st = (cudaStream_t)s;
+  return kind == ORX_SCORE_DOT ? el_launch<ORX_SCORE_DOT>(h, a, o, nullptr, st)
+                               : el_launch<ORX_SCORE_NEG_SQDIST>(h, a, o, nullptr, st);
+}
+
+template <typename T>
+int score_topk_impl(orx_handle_t h, int32_t kind, const T* user_tab, int64_t U, const int32_t* uid, int32_t Bu,
+                    const float* scale, const T* item_tab, const float* item_bias, int64_t I, int32_t dim,
+                    const int64_t* excl_off, const int32_t* excl_items, int32_t k, int32_t* top_items,
+                    float* top_scores, orx_stream_t s) {
+  ORX_REQUIRE(h != nullptr, "null handle");
+  ORX_REQUIRE(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST, "unknown score kind");
+  ORX_REQUIRE(U > 0 && I > 0 && I <= INT32_MAX && dim > 0 && Bu >= 0, "bad sizes");
+  ORX_REQUIRE(k >= 1 && k <= ORX_MAX_TOPK, "k must lie in [1, ORX_MAX_TOPK]");
+  if (Bu == 0) return ORX_OK;   // before the pointer checks: an empty batch may come with NULL buffers
+  ORX_REQUIRE(user_tab && uid && item_tab && top_items, "null pointer");
+  ORX_CUDA(cudaSetDevice(h->device));
+  EvalArgsT<T> a = {};
+  a.user_tab = user_tab; a.U = U; a.uid = uid; a.Bu = Bu; a.scale = scale; a.item_tab = item_tab;
+  a.bias = item_bias; a.I = I; a.D = dim; a.excl_off = excl_off; a.excl_items = excl_items;
+  return kind == ORX_SCORE_DOT ? tk_launch<ORX_SCORE_DOT>(h, a, k, top_items, top_scores, (cudaStream_t)s)
+                               : tk_launch<ORX_SCORE_NEG_SQDIST>(h, a, k, top_items, top_scores, (cudaStream_t)s);
+}
+
+}  // namespace
+
+extern "C" int orx_score_rank(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
+                              int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
+                              int32_t dim, const int64_t* pos_off, const int32_t* pos_items, const int64_t* excl_off,
+                              const int32_t* excl_items, int32_t max_pos, const int32_t* at_host, int32_t n_at,
+                              float* auc, float* ndcg, float* recall, orx_stream_t s) {
+  return score_rank_impl(h, kind, user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, pos_off, pos_items,
+                         excl_off, excl_items, max_pos, at_host, n_at, auc, ndcg, recall, s);
+}
+
+extern "C" int orx_score_rank_bf16(orx_handle_t h, int32_t kind, const uint16_t* user_tab, int64_t U,
+                                   const int32_t* uid, int32_t Bu, const float* scale, const uint16_t* item_tab,
+                                   const float* item_bias, int64_t I, int32_t dim, const int64_t* pos_off,
+                                   const int32_t* pos_items, const int64_t* excl_off, const int32_t* excl_items,
+                                   int32_t max_pos, const int32_t* at_host, int32_t n_at, float* auc, float* ndcg,
+                                   float* recall, orx_stream_t s) {
+  return score_rank_impl(h, kind, user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, pos_off, pos_items,
+                         excl_off, excl_items, max_pos, at_host, n_at, auc, ndcg, recall, s);
 }
 
 extern "C" int orx_score_rank_listed(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U,
@@ -1428,35 +1557,36 @@ extern "C" int orx_score_rank_listed(orx_handle_t h, int32_t kind, const float* 
                                      const int64_t* excl_off, const int32_t* excl_items, int32_t max_pos,
                                      const int32_t* at_host, int32_t n_at, float* auc, float* ndcg, float* recall,
                                      orx_stream_t s) {
-  const char* why = ev_rank_refusal(h, kind, user_tab, U, uid, Bu, item_tab, I, dim, pos_off, max_pos, at_host, n_at);
-  ORX_REQUIRE(why == nullptr, why);
-  ORX_REQUIRE(neg_off != nullptr, "null pointer");
-  if (Bu == 0) return ORX_OK;
-  ORX_CUDA(cudaSetDevice(h->device));
-  const EvalRowArgs a = ev_rank_args(user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, pos_off, pos_items,
-                                     neg_off, neg_items, excl_off, excl_items, max_pos);
-  const EvalOut o = ev_out(at_host, n_at, auc, ndcg, recall);
-  cudaStream_t st = (cudaStream_t)s;
-  return kind == ORX_SCORE_DOT ? el_launch<ORX_SCORE_DOT>(h, a, o, nullptr, st)
-                               : el_launch<ORX_SCORE_NEG_SQDIST>(h, a, o, nullptr, st);
+  return score_rank_listed_impl(h, kind, user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, pos_off, pos_items,
+                                neg_off, neg_items, excl_off, excl_items, max_pos, at_host, n_at, auc, ndcg, recall, s);
+}
+
+extern "C" int orx_score_rank_listed_bf16(orx_handle_t h, int32_t kind, const uint16_t* user_tab, int64_t U,
+                                          const int32_t* uid, int32_t Bu, const float* scale, const uint16_t* item_tab,
+                                          const float* item_bias, int64_t I, int32_t dim, const int64_t* pos_off,
+                                          const int32_t* pos_items, const int64_t* neg_off, const int32_t* neg_items,
+                                          const int64_t* excl_off, const int32_t* excl_items, int32_t max_pos,
+                                          const int32_t* at_host, int32_t n_at, float* auc, float* ndcg,
+                                          float* recall, orx_stream_t s) {
+  return score_rank_listed_impl(h, kind, user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, pos_off, pos_items,
+                                neg_off, neg_items, excl_off, excl_items, max_pos, at_host, n_at, auc, ndcg, recall, s);
 }
 
 extern "C" int orx_score_topk(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
                               int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
                               int32_t dim, const int64_t* excl_off, const int32_t* excl_items, int32_t k,
                               int32_t* top_items, float* top_scores, orx_stream_t s) {
-  ORX_REQUIRE(h != nullptr, "null handle");
-  ORX_REQUIRE(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST, "unknown score kind");
-  ORX_REQUIRE(U > 0 && I > 0 && I <= INT32_MAX && dim > 0 && Bu >= 0, "bad sizes");
-  ORX_REQUIRE(k >= 1 && k <= ORX_MAX_TOPK, "k must lie in [1, ORX_MAX_TOPK]");
-  if (Bu == 0) return ORX_OK;   // before the pointer checks: an empty batch may come with NULL buffers
-  ORX_REQUIRE(user_tab && uid && item_tab && top_items, "null pointer");
-  ORX_CUDA(cudaSetDevice(h->device));
-  EvalArgs a = {};
-  a.user_tab = user_tab; a.U = U; a.uid = uid; a.Bu = Bu; a.scale = scale; a.item_tab = item_tab;
-  a.bias = item_bias; a.I = I; a.D = dim; a.excl_off = excl_off; a.excl_items = excl_items;
-  return kind == ORX_SCORE_DOT ? tk_launch<ORX_SCORE_DOT>(h, a, k, top_items, top_scores, (cudaStream_t)s)
-                               : tk_launch<ORX_SCORE_NEG_SQDIST>(h, a, k, top_items, top_scores, (cudaStream_t)s);
+  return score_topk_impl(h, kind, user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, excl_off, excl_items, k,
+                         top_items, top_scores, s);
+}
+
+extern "C" int orx_score_topk_bf16(orx_handle_t h, int32_t kind, const uint16_t* user_tab, int64_t U,
+                                   const int32_t* uid, int32_t Bu, const float* scale, const uint16_t* item_tab,
+                                   const float* item_bias, int64_t I, int32_t dim, const int64_t* excl_off,
+                                   const int32_t* excl_items, int32_t k, int32_t* top_items, float* top_scores,
+                                   orx_stream_t s) {
+  return score_topk_impl(h, kind, user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, excl_off, excl_items, k,
+                         top_items, top_scores, s);
 }
 
 extern "C" int orx_score_rank_shard_sizes(int32_t Bu, int32_t dim, int32_t max_pos, int64_t* n3_host) {

@@ -313,12 +313,13 @@ extern "C" int orx_dense_apply(orx_handle_t h, float* var, float* s0, float* s1,
 
 // ---------------------------------------------------------------------------------------
 // inference: scores[Bu, I]  (bpr.py:39-43, wrmf.py:36-40, ucml.py:50-53, gmf.py:36-41), "K11".
-// 64 users x 64 items per block, D consumed in chunks of 16 through shared memory; 4x4 per thread.
+// 64 users x 64 items per block, D consumed in chunks of 16 through shared memory; 4x4 per thread.  Tab: the tables'
+// storage, float or bf16 bits widened exactly by orx_ld1 (orx_score_all_bf16); scale, bias and scores are fp32.
 // ---------------------------------------------------------------------------------------
-template <int KIND>
-__global__ void __launch_bounds__(256) k_score_all(const float* __restrict__ user_tab, int64_t U,
+template <int KIND, typename Tab>
+__global__ void __launch_bounds__(256) k_score_all(const Tab* __restrict__ user_tab, int64_t U,
                                                    const int32_t* __restrict__ uid, int Bu,
-                                                   const float* __restrict__ scale, const float* __restrict__ item_tab,
+                                                   const float* __restrict__ scale, const Tab* __restrict__ item_tab,
                                                    const float* __restrict__ bias, int64_t I, int D,
                                                    float* __restrict__ scores) {
   constexpr int T = 64, KC = 16;
@@ -339,11 +340,11 @@ __global__ void __launch_bounds__(256) k_score_all(const float* __restrict__ use
         if (u0 + r < Bu) {
           const int32_t id = uid[u0 + r];
           if (id >= 0 && (int64_t)id < U) {
-            uv = user_tab[(int64_t)id * D + k0 + k];
+            uv = orx_ld1(user_tab + (int64_t)id * D + k0 + k);
             if (scale) uv *= scale[k0 + k];
           }
         }
-        if (i0 + r < I) iv = item_tab[(i0 + r) * D + k0 + k];
+        if (i0 + r < I) iv = orx_ld1(item_tab + (i0 + r) * D + k0 + k);
       }
       su[k][r] = uv;
       si[k][r] = iv;
@@ -380,21 +381,36 @@ __global__ void __launch_bounds__(256) k_score_all(const float* __restrict__ use
   }
 }
 
-extern "C" int orx_score_all(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
-                             int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
-                             int32_t dim, float* scores, orx_stream_t s) {
+template <typename T>
+static int score_all_impl(orx_handle_t h, int32_t kind, const T* user_tab, int64_t U, const int32_t* uid, int32_t Bu,
+                          const float* scale, const T* item_tab, const float* item_bias, int64_t I, int32_t dim,
+                          float* scores, orx_stream_t s) {
   ORX_REQUIRE(h != nullptr && user_tab && uid && item_tab && scores, "null pointer");
   ORX_REQUIRE(kind == ORX_SCORE_DOT || kind == ORX_SCORE_NEG_SQDIST, "unknown score kind");
   ORX_REQUIRE(U > 0 && I > 0 && dim > 0 && Bu >= 0, "bad sizes");
   if (Bu == 0) return ORX_OK;
   ORX_CUDA(cudaSetDevice(h->device));
   dim3 grid((unsigned)((I + 63) / 64), (unsigned)((Bu + 63) / 64));
+  cudaStream_t st = (cudaStream_t)s;
   if (kind == ORX_SCORE_DOT)
-    k_score_all<ORX_SCORE_DOT><<<grid, 256, 0, (cudaStream_t)s>>>(user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, scores);
+    k_score_all<ORX_SCORE_DOT><<<grid, 256, 0, st>>>(user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, scores);
   else
-    k_score_all<ORX_SCORE_NEG_SQDIST><<<grid, 256, 0, (cudaStream_t)s>>>(user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, scores);
+    k_score_all<ORX_SCORE_NEG_SQDIST><<<grid, 256, 0, st>>>(user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim,
+                                                            scores);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
+}
+
+extern "C" int orx_score_all(orx_handle_t h, int32_t kind, const float* user_tab, int64_t U, const int32_t* uid,
+                             int32_t Bu, const float* scale, const float* item_tab, const float* item_bias, int64_t I,
+                             int32_t dim, float* scores, orx_stream_t s) {
+  return score_all_impl(h, kind, user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, scores, s);
+}
+
+extern "C" int orx_score_all_bf16(orx_handle_t h, int32_t kind, const uint16_t* user_tab, int64_t U, const int32_t* uid,
+                                  int32_t Bu, const float* scale, const uint16_t* item_tab, const float* item_bias,
+                                  int64_t I, int32_t dim, float* scores, orx_stream_t s) {
+  return score_all_impl(h, kind, user_tab, U, uid, Bu, scale, item_tab, item_bias, I, dim, scores, s);
 }
 
 // ---------------------------------------------------------------------------------------

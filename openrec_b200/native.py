@@ -17,7 +17,7 @@ from ._lib import (ORX_OP_GEMM, ORX_OP_INTERACT_BWD, ORX_OP_INTERACT_FWD, ORX_OP
                    ORX_VARIANT_RANK_SMEM, ORX_VARIANT_STEP, ORX_VARIANT_STEP_GENERIC, ORX_VARIANT_STEP_PIPE,
                    ORX_VARIANT_TOPK, ORX_OP_CROSS, ORX_VARIANT_CROSS_VEC, ORX_VARIANT_CROSS_SCALAR, ORX_CROSS_TOP,
                    ORX_CROSS_MID, ORX_CROSS_FINAL, ORX_OP_PAIRWISE_STEP_BF16, ORX_OP_POINTWISE_STEP_BF16, OrxOpt,
-                   OrxTable, OrxTableBf16)
+                   ORX_OP_SCORE_RANK_BF16, ORX_OP_SCORE_TOPK_BF16, OrxTable, OrxTableBf16)
 
 __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", "ORX_POINT_GMF", "ORX_POINT_WRMF",
            "ORX_OPT_SGD", "ORX_OPT_ADAGRAD", "ORX_OPT_ADAM_LAZY", "ORX_OPT_ADAM_DENSE", "ORX_OPT_ROWWISE_ADAGRAD",
@@ -29,7 +29,8 @@ __all__ = ["Engine", "engine", "table", "opt", "ORX_PAIR_BPR", "ORX_PAIR_UCML", 
            "ORX_VARIANT_TOPK", "ORX_OP_SCORE_RANK_SHARD", "ORX_OP_SCORE_TOPK_SHARD", "ORX_OP_POINTWISE_GRAD_ROWS",
            "ORX_OP_CENSOR_SHARD", "ORX_VARIANT_CENSOR_VEC", "ORX_VARIANT_CENSOR_SCALAR", "ORX_OP_CROSS",
            "ORX_VARIANT_CROSS_VEC", "ORX_VARIANT_CROSS_SCALAR", "ORX_CROSS_TOP", "ORX_CROSS_MID", "ORX_CROSS_FINAL",
-           "ORX_OP_PAIRWISE_STEP_BF16", "ORX_OP_POINTWISE_STEP_BF16", "table_bf16", "as_table",
+           "ORX_OP_PAIRWISE_STEP_BF16", "ORX_OP_POINTWISE_STEP_BF16", "ORX_OP_SCORE_RANK_BF16",
+           "ORX_OP_SCORE_TOPK_BF16", "table_bf16", "as_table",
            "Dispatch", "RowShard", "rowshard", "shard_rows"]
 
 _engines = {}
@@ -91,6 +92,17 @@ def _bf16(t, name):
     if not (t.is_cuda and t.dtype == torch.bfloat16 and t.is_contiguous()):
         raise ValueError(f"{name}: expected a contiguous bfloat16 CUDA tensor")
     return t
+
+
+def _score_tables(op, user_tab, item_tab):
+    """-> (entry point, user_tab, item_tab) of scoring call `op` for the tables' dtype: op itself on float32 tables, its
+    _bf16 form on bfloat16 ones (bit-equal to op on their float32 upcast).  Mixed dtypes are refused."""
+    if user_tab.dtype == torch.float32 and item_tab.dtype == torch.float32:
+        return op, _f32(user_tab, "user_tab"), _f32(item_tab, "item_tab")
+    if user_tab.dtype == torch.bfloat16 and item_tab.dtype == torch.bfloat16:
+        return op + "_bf16", _bf16(user_tab, "user_tab"), _bf16(item_tab, "item_tab")
+    raise ValueError(f"{op}: user_tab and item_tab must both be float32 or both bfloat16, got {user_tab.dtype} and "
+                     f"{item_tab.dtype}")
 
 
 def table_bf16(var, s0=None, s1=None, kind=None):
@@ -600,12 +612,13 @@ class Engine:
                    "orx_dense_apply")
 
     def score_all(self, kind, user_tab, uid, item_tab, item_bias, scale=None):
+        """-> float32 [Bu, I] scores.  user_tab / item_tab both float32 or both bfloat16 (orx_score_all_bf16)."""
+        fn, user_tab, item_tab = _score_tables("orx_score_all", user_tab, item_tab)
         uid = ids32(uid)
         out = torch.empty((uid.numel(), item_tab.shape[0]), dtype=torch.float32, device=item_tab.device)
-        _lib.check(self.lib.orx_score_all(self.h, kind, _ptr(_f32(user_tab, "user_tab")), user_tab.shape[0], _ptr(uid),
-                                          uid.numel(), _ptr(scale), _ptr(_f32(item_tab, "item_tab")),
-                                          _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(out),
-                                          self.stream()), "orx_score_all")
+        _lib.check(getattr(self.lib, fn)(self.h, kind, _ptr(user_tab), user_tab.shape[0], _ptr(uid), uid.numel(),
+                                         _ptr(scale), _ptr(item_tab), _ptr(item_bias), item_tab.shape[0],
+                                         item_tab.shape[1], _ptr(out), self.stream()), fn)
         return out
 
     def rank_metrics(self, pred, pos, excl, at=(), want=("auc", "ndcg", "recall")):
@@ -626,7 +639,9 @@ class Engine:
         """score_all + rank_metrics in one pass for the users uid, from CSR lists indexed by user id: positives
         pos_items[pos_off[u]:pos_off[u + 1]] and exclusions likewise (excl_off / excl_items may be None); int64 offsets,
         int32 items, rows sorted and unique.  max_pos bounds every positive row length (a longer row gets NaN outputs).
+        user_tab / item_tab both float32 or both bfloat16 (orx_score_rank_bf16).
         -> (auc [Bu], ndcg [Bu, len(at)], recall [Bu, len(at)])."""
+        fn, user_tab, item_tab = _score_tables("orx_score_rank", user_tab, item_tab)
         uid = ids32(uid)
         Bu, dev = uid.numel(), item_tab.device
         pos_off, pos_items = _csr(pos_off, pos_items, user_tab.shape[0])
@@ -637,11 +652,10 @@ class Engine:
         auc = torch.empty(Bu, dtype=torch.float32, device=dev)
         ndcg = torch.empty((Bu, len(at)), dtype=torch.float32, device=dev)
         rec = torch.empty((Bu, len(at)), dtype=torch.float32, device=dev)
-        _lib.check(self.lib.orx_score_rank(
-            self.h, kind, _ptr(_f32(user_tab, "user_tab")), user_tab.shape[0], _ptr(uid), Bu, _ptr(scale),
-            _ptr(_f32(item_tab, "item_tab")), _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(pos_off),
-            _ptr(pos_items), _ptr(excl_off), _ptr(excl_items), int(max_pos), at_arr, len(at), _ptr(auc), _ptr(ndcg),
-            _ptr(rec), self.stream()), "orx_score_rank")
+        _lib.check(getattr(self.lib, fn)(
+            self.h, kind, _ptr(user_tab), user_tab.shape[0], _ptr(uid), Bu, _ptr(scale), _ptr(item_tab),
+            _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(pos_off), _ptr(pos_items), _ptr(excl_off),
+            _ptr(excl_items), int(max_pos), at_arr, len(at), _ptr(auc), _ptr(ndcg), _ptr(rec), self.stream()), fn)
         return auc, ndcg, rec
 
     @staticmethod
@@ -686,7 +700,9 @@ class Engine:
         """score_rank with each user ranked against its listed items only (orx_score_rank_listed in include/orx.h):
         positives, listed items (neg_off / neg_items) and exclusions as CSR lists indexed by user id, as in score_rank
         (excl_off / excl_items may be None).  Equals score_all + rank_metrics on the masks pos = P,
-        excl = ~(P | L) | E.  -> (auc [Bu], ndcg [Bu, len(at)], recall [Bu, len(at)])."""
+        excl = ~(P | L) | E.  user_tab / item_tab both float32 or both bfloat16 (orx_score_rank_listed_bf16).
+        -> (auc [Bu], ndcg [Bu, len(at)], recall [Bu, len(at)])."""
+        fn, user_tab, item_tab = _score_tables("orx_score_rank_listed", user_tab, item_tab)
         uid = ids32(uid)
         Bu, dev = uid.numel(), item_tab.device
         pos_off, pos_items = _csr(pos_off, pos_items, user_tab.shape[0])
@@ -698,11 +714,11 @@ class Engine:
         auc = torch.empty(Bu, dtype=torch.float32, device=dev)
         ndcg = torch.empty((Bu, len(at)), dtype=torch.float32, device=dev)
         rec = torch.empty((Bu, len(at)), dtype=torch.float32, device=dev)
-        _lib.check(self.lib.orx_score_rank_listed(
-            self.h, kind, _ptr(_f32(user_tab, "user_tab")), user_tab.shape[0], _ptr(uid), Bu, _ptr(scale),
-            _ptr(_f32(item_tab, "item_tab")), _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(pos_off),
-            _ptr(pos_items), _ptr(neg_off), _ptr(neg_items), _ptr(excl_off), _ptr(excl_items), int(max_pos), at_arr,
-            len(at), _ptr(auc), _ptr(ndcg), _ptr(rec), self.stream()), "orx_score_rank_listed")
+        _lib.check(getattr(self.lib, fn)(
+            self.h, kind, _ptr(user_tab), user_tab.shape[0], _ptr(uid), Bu, _ptr(scale), _ptr(item_tab),
+            _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(pos_off), _ptr(pos_items), _ptr(neg_off),
+            _ptr(neg_items), _ptr(excl_off), _ptr(excl_items), int(max_pos), at_arr, len(at), _ptr(auc), _ptr(ndcg),
+            _ptr(rec), self.stream()), fn)
         return auc, ndcg, rec
 
     def score_rank_listed_shard(self, kind, phase, g, user_shard, item_shard, bias_shard, uid, pos_off, pos_items,
@@ -738,7 +754,9 @@ class Engine:
         """The k best eligible items of each user uid in one pass over the item table, without the [Bu, I] score
         matrix: order score descending then item ascending, the user's CSR exclusion row (excl_off / excl_items as in
         score_rank, may be None) and NaN scores left out, slots past the eligible items padded with item -1 and score
-        -inf.  -> (items int32 [Bu, k], scores float32 [Bu, k]), scores bit-equal to score_all's (-0.0 may read +0.0)."""
+        -inf.  -> (items int32 [Bu, k], scores float32 [Bu, k]), scores bit-equal to score_all's (-0.0 may read +0.0).
+        user_tab / item_tab both float32 or both bfloat16 (orx_score_topk_bf16)."""
+        fn, user_tab, item_tab = _score_tables("orx_score_topk", user_tab, item_tab)
         uid = ids32(uid)
         Bu, dev = uid.numel(), item_tab.device
         excl_off, excl_items = _csr(excl_off, excl_items, user_tab.shape[0])
@@ -747,10 +765,10 @@ class Engine:
             raise ValueError(f"k must lie in [1, {_lib.ORX_MAX_TOPK}]")
         items = torch.empty((Bu, k), dtype=torch.int32, device=dev)
         scores = torch.empty((Bu, k), dtype=torch.float32, device=dev)
-        _lib.check(self.lib.orx_score_topk(
-            self.h, kind, _ptr(_f32(user_tab, "user_tab")), user_tab.shape[0], _ptr(uid), Bu, _ptr(scale),
-            _ptr(_f32(item_tab, "item_tab")), _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(excl_off),
-            _ptr(excl_items), k, _ptr(items), _ptr(scores), self.stream()), "orx_score_topk")
+        _lib.check(getattr(self.lib, fn)(
+            self.h, kind, _ptr(user_tab), user_tab.shape[0], _ptr(uid), Bu, _ptr(scale), _ptr(item_tab),
+            _ptr(item_bias), item_tab.shape[0], item_tab.shape[1], _ptr(excl_off), _ptr(excl_items), k, _ptr(items),
+            _ptr(scores), self.stream()), fn)
         return items, scores
 
     def score_topk_shard(self, kind, phase, g, user_shard, item_shard, bias_shard, uid, excl_off, excl_items, k, xrows,

@@ -10,7 +10,8 @@ from ._base import FusedRecommender, _check_dtype, ids_any, ids_of
 class BPR(FusedRecommender):
     """``embedding_dtype="bfloat16"`` stores the user and item tables in bfloat16 (the item bias and every optimizer
     slot stay float32); each step rounds its updates stochastically, seeded by ``rounding_seed`` and the optimizer's
-    iteration count, so a run is reproducible bit for bit."""
+    iteration count, so a run is reproducible bit for bit.  ``inference``, the evaluators and ``Retriever`` score the
+    bfloat16 tables in place, with results bit-equal to scoring their float32 upcast."""
     _kind = N.ORX_PAIR_BPR
     _score = N.ORX_SCORE_DOT
 
@@ -95,11 +96,9 @@ class BPR(FusedRecommender):
 
     def _score_operands(self):
         """(kind, user table, item table, item bias, scale) of the full-catalogue score (inference, RankingEvaluator,
-        Retriever).  bf16 tables are scored as their exact float32 upcast, made here for the call."""
-        user, item = self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t
-        if self._bf16():
-            user, item = user.float(), item.float()
-        return (self._score, user, item, self.item_bias.embeddings.t, None)
+        CandidateEvaluator, Retriever): the stored tables, so bf16 ones are read in place by the _bf16 entry points."""
+        return (self._score, self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t,
+                self.item_bias.embeddings.t, None)
 
     def inference(self, user_id):
         """scores [Bu, total_items] = U[user] @ Item^T + bias (bpr.py:39-43)."""

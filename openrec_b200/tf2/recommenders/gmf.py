@@ -10,7 +10,9 @@ from .wrmf import WRMF
 class GMF(WRMF):
     """``embedding_dtype="bfloat16"`` stores the user and item tables in bfloat16 (the item bias, ``w`` and every
     optimizer slot stay float32); each step rounds its updates stochastically, seeded by ``rounding_seed`` and the
-    optimizer's iteration count, so a run is reproducible bit for bit."""
+    optimizer's iteration count, so a run is reproducible bit for bit.  ``inference``, the evaluators and ``Retriever``
+    score the bfloat16 tables in place (``w`` and the bias in float32), with results bit-equal to scoring their float32
+    upcast."""
     _kind = N.ORX_POINT_GMF
 
     def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items, embedding_dtype="float32",

@@ -10,7 +10,8 @@ from ._base import FusedRecommender, _check_dtype, ids_of
 class WRMF(FusedRecommender):
     """``embedding_dtype="bfloat16"`` stores the user and item tables in bfloat16 (the item bias and every optimizer
     slot stay float32); each step rounds its updates stochastically, seeded by ``rounding_seed`` and the optimizer's
-    iteration count, so a run is reproducible bit for bit."""
+    iteration count, so a run is reproducible bit for bit.  ``inference``, the evaluators and ``Retriever`` score the
+    bfloat16 tables in place, with results bit-equal to scoring their float32 upcast."""
     _kind = N.ORX_POINT_WRMF
 
     def __init__(self, dim_user_embed, dim_item_embed, total_users, total_items, a=1.0, b=1.0,
@@ -82,15 +83,12 @@ class WRMF(FusedRecommender):
         return Tensor(idx), Tensor(val.reshape(B, -1))
 
     def _score_tables(self):
-        """(user, item) tables to score: bf16 tables as their exact float32 upcast, made here for the call."""
-        user, item = self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t
-        if self._bf16():
-            user, item = user.float(), item.float()
-        return user, item
+        """(user, item) tables to score: the stored tables, so bf16 ones are read in place by the _bf16 entry points."""
+        return self.user_latent_factor.embeddings.t, self.item_latent_factor.embeddings.t
 
     def _score_operands(self):
         """(kind, user table, item table, item bias, scale) of the full-catalogue score (inference, RankingEvaluator,
-        CandidateEvaluator, Retriever).  bf16 tables are scored as their exact float32 upcast, made here for the call."""
+        CandidateEvaluator, Retriever), on the stored tables (_score_tables)."""
         return (N.ORX_SCORE_DOT, *self._score_tables(), self.item_bias.embeddings.t, None)
 
     def inference(self, user_id):
