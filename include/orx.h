@@ -394,6 +394,21 @@ ORX_API int orx_sparse_apply_strided(orx_handle_t h, const orx_table_t* tab, con
 ORX_API int orx_bag_sparse_apply(orx_handle_t h, const orx_table_t* tab, const int32_t* sparse, int64_t ld,
                                  int32_t col_lo, int32_t L, int32_t B, const float* dZ, int64_t dz_ld, int32_t mode,
                                  const orx_opt_t* opt_host, orx_stream_t s);
+/* orx_sparse_apply_strided_bf16 / orx_bag_sparse_apply_bf16: orx_sparse_apply_strided / orx_bag_sparse_apply on a bf16
+ * table (orx_table_bf16_t), with the same arguments, checks, scratch and optimizer kinds.  A touched row is read as its
+ * exact fp32 upcast and each updated element rounded stochastically as orx_table_bf16_t states, as table t = 0 with
+ * sr_seed and opt->step (the staged-row tail and the ADAM_DENSE sweep use the same key).  A caller with several tables
+ * gives each its own seed: DLRM gives table k mix64(rounding_seed + k) (mod 2^64), distinct for every k since mix64 is a
+ * bijection.  Untouched rows keep their bits, except under ADAM_DENSE (its sweep writes every row).  Alignment: rows
+ * move 4 elements (8 bytes) per lane when var is 8-byte aligned, dim % 4 == 0 and the slot rows the optimizer keeps are
+ * 16-byte aligned (a row-wise accumulator does not count); any other 2-byte-aligned table takes the scalar path, which
+ * rounds alike. */
+ORX_API int orx_sparse_apply_strided_bf16(orx_handle_t h, const orx_table_bf16_t* tab, const int32_t* ids,
+                                          int64_t id_stride, const float* values, int64_t value_ld, int32_t n,
+                                          const orx_opt_t* opt_host, uint64_t sr_seed, orx_stream_t s);
+ORX_API int orx_bag_sparse_apply_bf16(orx_handle_t h, const orx_table_bf16_t* tab, const int32_t* sparse, int64_t ld,
+                                      int32_t col_lo, int32_t L, int32_t B, const float* dZ, int64_t dz_ld,
+                                      int32_t mode, const orx_opt_t* opt_host, uint64_t sr_seed, orx_stream_t s);
 /* Combined form used by openrec_b200/sharded.py: each rank stores ONE local table [user rows | item rows] of
  * width ld = D+4 (item bias in column D), so a lookup is (owner, combined local row) whatever its table.
  * orx_owner_bucket_combined: ids = uid | pid | nid (n_user user ids first).  Row r lives on rank r % world at
@@ -582,6 +597,17 @@ ORX_API int orx_gather_strided(orx_handle_t h, const float* tab, int64_t rows, i
 ORX_API int orx_bag_gather(orx_handle_t h, const float* const* tabs_host, const int64_t* rows_host, int32_t T,
                            int32_t dim, const int32_t* sparse, int64_t ld, const int32_t* col_off_host, int32_t B,
                            int32_t mode, float* out, int64_t out_ld, int32_t* n_bad, orx_stream_t s);
+/* orx_gather_strided_bf16 / orx_bag_gather_bf16: orx_gather_strided / orx_bag_gather on bf16 tables (uint16_t bits;
+ *   every table of orx_bag_gather_bf16 is bf16), with the same arguments and checks.  Rows are widened exactly and
+ *   pooled in fp32 in the same column order, so out and *n_bad are those of the fp32 call on the fp32 upcast of the
+ *   tables, bit for bit.  Alignment: a lane moves 4 columns as one 8-byte load when dim % 4 == 0, out_ld % 4 == 0, out
+ *   is 16-byte aligned and every table 8-byte aligned; any other 2-byte-aligned table takes the scalar path (same bits). */
+ORX_API int orx_gather_strided_bf16(orx_handle_t h, const uint16_t* tab, int64_t rows, int32_t dim, const int32_t* ids,
+                                    int64_t id_stride, int64_t n, float* out, int64_t out_ld, int32_t* n_bad,
+                                    orx_stream_t s);
+ORX_API int orx_bag_gather_bf16(orx_handle_t h, const uint16_t* const* tabs_host, const int64_t* rows_host, int32_t T,
+                                int32_t dim, const int32_t* sparse, int64_t ld, const int32_t* col_off_host, int32_t B,
+                                int32_t mode, float* out, int64_t out_ld, int32_t* n_bad, orx_stream_t s);
 ORX_API int orx_mlp_layer_fwd(orx_handle_t h, const float* x, int64_t ldx, int32_t B, int32_t in, const float* w,
                               const float* bias, int32_t out, int32_t act, float* y, int64_t ldy, orx_stream_t s);
 ORX_API int orx_mlp_layer_bwd(orx_handle_t h, const float* x, int64_t ldx, const float* y, int64_t ldy, const float* w,

@@ -107,7 +107,12 @@ SIGNATURES = {
     "orx_gather_strided": [_vp, _vp, _i64, _i32, _vp, _i64, _i64, _vp, _i64, _vp, _vp],
     "orx_bag_gather": [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _i64, C.POINTER(_i32), _i32, _i32, _vp,
                        _i64, _vp, _vp],
+    "orx_gather_strided_bf16": [_vp, _vp, _i64, _i32, _vp, _i64, _i64, _vp, _i64, _vp, _vp],
+    "orx_bag_gather_bf16": [_vp, C.POINTER(_vp), C.POINTER(_i64), _i32, _i32, _vp, _i64, C.POINTER(_i32), _i32, _i32,
+                            _vp, _i64, _vp, _vp],
     "orx_bag_sparse_apply": [_vp, _T, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _i32, _O, _vp],
+    "orx_sparse_apply_strided_bf16": [_vp, _TB, _vp, _i64, _vp, _i64, _i32, _O, _u64, _vp],
+    "orx_bag_sparse_apply_bf16": [_vp, _TB, _vp, _i64, _i32, _i32, _i32, _vp, _i64, _i32, _O, _u64, _vp],
     "orx_mlp_layer_fwd": [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _i32, _i32, _vp, _i64, _vp],
     "orx_mlp_layer_bwd": [_vp, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _vp, _i64, _vp, _vp, _vp],
     "orx_interact_fwd": [_vp, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _vp],

@@ -9,10 +9,23 @@
 // ---------------------------------------------------------------------------------------
 // K5: out[b*out_ld + :D] = tab[ids[b*id_stride], :D]   (dlrm.py:83-85, one call per sparse feature)
 // ---------------------------------------------------------------------------------------
-// VEC: tab and out are 16-byte aligned (orx_gather_strided decides); with D and out_ld multiples of 4 the rows then move
-// as float4 (the row shape is tested here, as in k_gather)
-template <bool VEC>
-__global__ void __launch_bounds__(256) k_gather_strided(const float* __restrict__ tab, int64_t rows, int D,
+// Row loads of the DLRM gathers by table storage: a float row as float4 / scalar (__ldg), a bf16 row (uint16_t bits) as
+// 4 elements in one 8-byte load / one 2-byte load, widened exactly.
+// gather_ld4(row, q): columns 4q .. 4q + 3 of a row (16-byte / 8-byte aligned)
+__device__ __forceinline__ float4 gather_ld4(const float* row, int q) {
+  return __ldg(reinterpret_cast<const float4*>(row) + q);
+}
+__device__ __forceinline__ float4 gather_ld4(const uint16_t* row, int q) {
+  return orx_bf16x4_up(__ldg(reinterpret_cast<const uint2*>(row) + q));
+}
+__device__ __forceinline__ float gather_ld1(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float gather_ld1(const uint16_t* p) { return orx_bf16_up(__ldg(p)); }
+
+// VEC: out is 16-byte aligned and tab 16-byte (float) / 8-byte (bf16) aligned (gather_strided_impl decides); with D and
+// out_ld multiples of 4 the rows then move 4 columns per lane (the row shape is tested here, as in k_gather).
+// T: the table's storage, float or bf16 bits (uint16_t); out is float either way.
+template <bool VEC, typename T = float>
+__global__ void __launch_bounds__(256) k_gather_strided(const T* __restrict__ tab, int64_t rows, int D,
                                                         const int32_t* __restrict__ ids, int64_t id_stride, int64_t n,
                                                         float* __restrict__ out, int64_t out_ld, int32_t* n_bad) {
   const int lane = threadIdx.x & 31;
@@ -23,18 +36,19 @@ __global__ void __launch_bounds__(256) k_gather_strided(const float* __restrict_
     const bool ok = id >= 0 && id < rows;
     if (!ok && lane == 0 && n_bad) atomicAdd(n_bad, 1);
     if (vec) {
-      const float4* src = reinterpret_cast<const float4*>(tab + id * D);
+      const T* src = tab + id * D;
       float4* dst = reinterpret_cast<float4*>(out + b * out_ld);
-      for (int e = lane; e < D / 4; e += 32) dst[e] = ok ? __ldg(src + e) : make_float4(0.f, 0.f, 0.f, 0.f);
+      for (int e = lane; e < D / 4; e += 32) dst[e] = ok ? gather_ld4(src, e) : make_float4(0.f, 0.f, 0.f, 0.f);
     } else {
-      for (int e = lane; e < D; e += 32) out[b * out_ld + e] = ok ? __ldg(tab + id * D + e) : 0.f;
+      for (int e = lane; e < D; e += 32) out[b * out_ld + e] = ok ? gather_ld1(tab + id * D + e) : 0.f;
     }
   }
 }
 
-extern "C" int orx_gather_strided(orx_handle_t h, const float* tab, int64_t rows, int32_t dim, const int32_t* ids,
-                                  int64_t id_stride, int64_t n, float* out, int64_t out_ld, int32_t* n_bad,
-                                  orx_stream_t s) {
+template <typename T>
+static int gather_strided_impl(orx_handle_t h, const T* tab, int64_t rows, int32_t dim, const int32_t* ids,
+                               int64_t id_stride, int64_t n, float* out, int64_t out_ld, int32_t* n_bad,
+                               orx_stream_t s) {
   ORX_REQUIRE(h != nullptr && tab && ids && out, "null pointer");
   ORX_REQUIRE(rows > 0 && dim > 0 && n >= 0 && id_stride >= 1 && out_ld >= dim, "bad sizes");
   if (n == 0) return ORX_OK;
@@ -42,12 +56,25 @@ extern "C" int orx_gather_strided(orx_handle_t h, const float* tab, int64_t rows
   int64_t blocks = (n + 7) / 8;
   if (blocks > (int64_t)h->num_sms * 32) blocks = (int64_t)h->num_sms * 32;
   cudaStream_t st = (cudaStream_t)s;
-  if (orx_aligned16(tab, out))
-    k_gather_strided<true><<<(int)blocks, 256, 0, st>>>(tab, rows, dim, ids, id_stride, n, out, out_ld, n_bad);
+  const bool vec = std::is_same<T, float>::value ? orx_aligned16(tab, out) : orx_aligned8(tab) && orx_aligned16(out);
+  if (vec)
+    k_gather_strided<true, T><<<(int)blocks, 256, 0, st>>>(tab, rows, dim, ids, id_stride, n, out, out_ld, n_bad);
   else
-    k_gather_strided<false><<<(int)blocks, 256, 0, st>>>(tab, rows, dim, ids, id_stride, n, out, out_ld, n_bad);
+    k_gather_strided<false, T><<<(int)blocks, 256, 0, st>>>(tab, rows, dim, ids, id_stride, n, out, out_ld, n_bad);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
+}
+
+extern "C" int orx_gather_strided(orx_handle_t h, const float* tab, int64_t rows, int32_t dim, const int32_t* ids,
+                                  int64_t id_stride, int64_t n, float* out, int64_t out_ld, int32_t* n_bad,
+                                  orx_stream_t s) {
+  return gather_strided_impl(h, tab, rows, dim, ids, id_stride, n, out, out_ld, n_bad, s);
+}
+
+extern "C" int orx_gather_strided_bf16(orx_handle_t h, const uint16_t* tab, int64_t rows, int32_t dim,
+                                       const int32_t* ids, int64_t id_stride, int64_t n, float* out, int64_t out_ld,
+                                       int32_t* n_bad, orx_stream_t s) {
+  return gather_strided_impl(h, tab, rows, dim, ids, id_stride, n, out, out_ld, n_bad, s);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -614,17 +641,27 @@ extern "C" int orx_pred_loss(orx_handle_t h, const float* pred, const float* lab
 // ---------------------------------------------------------------------------------------
 static_assert(ORX_BAG_MAX_TABLES + 1 <= ORX_MAX_F, "the pooled features and the dense vector must fit the interaction");
 
+template <typename T>
 struct BagTables {   // kernel parameter block: ~1.3 KB, read with register-indexed constant loads
-  const float* tab[ORX_BAG_MAX_TABLES];
+  const T* tab[ORX_BAG_MAX_TABLES];
   int64_t rows[ORX_BAG_MAX_TABLES];
   int32_t col_off[ORX_BAG_MAX_TABLES + 1];
 };
 
+// One lane's load of a bag row chunk as stored (VEC: 4 columns, else 1): a float4 of a float table, the raw 8 bytes
+// (uint2) of a bf16 one, so that the four loads in flight hold half the registers; bag_up widens it exactly.
 template <bool VEC>
 __device__ __forceinline__ float4 bag_ld(const float* p) {
   if (VEC) return __ldg(reinterpret_cast<const float4*>(p));
   return make_float4(__ldg(p), 0.f, 0.f, 0.f);
 }
+template <bool VEC>
+__device__ __forceinline__ uint2 bag_ld(const uint16_t* p) {
+  if (VEC) return __ldg(reinterpret_cast<const uint2*>(p));
+  return make_uint2(__ldg(p), 0u);
+}
+__device__ __forceinline__ float4 bag_up(float4 v) { return v; }
+__device__ __forceinline__ float4 bag_up(uint2 v) { return orx_bf16x4_up(v); }
 
 __device__ __forceinline__ float4 bag_add(float4 a, float4 b) {
   return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w);
@@ -633,9 +670,10 @@ __device__ __forceinline__ float4 bag_add(float4 a, float4 b) {
 // One warp per bag, w = b*T + k (consecutive warps fill consecutive Z rows).  VEC: a lane holds one float4 of a
 // 128-float column chunk, else one float of a 32-float chunk; wider rows take several chunks, each re-reading the ids.
 // The ids are read 32 at a time (coalesced); a ballot gives the valid ones, which are taken four at a time: four row
-// loads are issued before they are added, in column order.
-template <bool VEC>
-__global__ void __launch_bounds__(256) k_bag_gather(const __grid_constant__ BagTables bt, int T, int D,
+// loads are issued before they are added, in column order.  S: the tables' storage, float or bf16 bits (uint16_t, rows
+// widened exactly, so Z is the fp32 call's on the upcast tables bit for bit).
+template <bool VEC, typename S = float>
+__global__ void __launch_bounds__(256) k_bag_gather(const __grid_constant__ BagTables<S> bt, int T, int D,
                                                     const int32_t* __restrict__ sparse, int64_t ld, int64_t B,
                                                     int mean, float* __restrict__ out, int64_t out_ld,
                                                     int32_t* n_bad) {
@@ -646,7 +684,7 @@ __global__ void __launch_bounds__(256) k_bag_gather(const __grid_constant__ BagT
   for (int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < B * T; w += nw) {
     const int64_t b = w / T;
     const int k = (int)(w - b * T);
-    const float* tab = bt.tab[k];
+    const S* tab = bt.tab[k];
     const int64_t rows = bt.rows[k];
     const int L = bt.col_off[k + 1] - bt.col_off[k];
     const int32_t* ids = sparse + b * ld + bt.col_off[k];
@@ -667,16 +705,16 @@ __global__ void __launch_bounds__(256) k_bag_gather(const __grid_constant__ BagT
             src[q] = m ? __ffs(m) - 1 : -1;
             m &= m - 1;
           }
-          float4 v[4];
+          decltype(bag_ld<VEC>(tab)) v[4];
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             const int64_t r = __shfl_sync(ORX_FULL, id, src[q] & 31);
-            v[q] = (src[q] >= 0 && on) ? bag_ld<VEC>(tab + r * D + e) : z4;
+            v[q] = (src[q] >= 0 && on) ? bag_ld<VEC>(tab + r * D + e) : decltype(bag_ld<VEC>(tab)){};
           }
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             if (src[q] < 0) break;
-            acc = n ? bag_add(acc, v[q]) : v[q];
+            acc = n ? bag_add(acc, bag_up(v[q])) : bag_up(v[q]);
             ++n;
           }
         }
@@ -693,16 +731,18 @@ __global__ void __launch_bounds__(256) k_bag_gather(const __grid_constant__ BagT
   }
 }
 
-extern "C" int orx_bag_gather(orx_handle_t h, const float* const* tabs_host, const int64_t* rows_host, int32_t T,
-                              int32_t dim, const int32_t* sparse, int64_t ld, const int32_t* col_off_host, int32_t B,
-                              int32_t mode, float* out, int64_t out_ld, int32_t* n_bad, orx_stream_t s) {
+// VEC rule: out 16-byte aligned, every table 16-byte (float) / 8-byte (bf16) aligned, dim and out_ld multiples of 4.
+template <typename S>
+static int bag_gather_impl(orx_handle_t h, const S* const* tabs_host, const int64_t* rows_host, int32_t T,
+                           int32_t dim, const int32_t* sparse, int64_t ld, const int32_t* col_off_host, int32_t B,
+                           int32_t mode, float* out, int64_t out_ld, int32_t* n_bad, orx_stream_t s) {
   ORX_REQUIRE(h != nullptr && tabs_host && rows_host && col_off_host, "null pointer");
   ORX_REQUIRE(B == 0 || (sparse && out), "null sparse / out");
   ORX_REQUIRE(T >= 1 && T <= ORX_BAG_MAX_TABLES, "T outside [1, ORX_BAG_MAX_TABLES]");
   ORX_REQUIRE(dim >= 1 && B >= 0 && ld >= 1 && (mode == 0 || mode == 1), "bad sizes / mode");
   ORX_REQUIRE(out_ld >= (int64_t)T * dim, "out_ld < T * dim");
   ORX_REQUIRE(col_off_host[0] >= 0 && col_off_host[T] <= ld, "col_off outside [0, ld]");
-  BagTables bt;
+  BagTables<S> bt;
   bool aligned = orx_aligned16(out);
   for (int k = 0; k < T; ++k) {
     ORX_REQUIRE(tabs_host[k] != nullptr && rows_host[k] > 0, "null table / empty vocabulary");
@@ -710,7 +750,7 @@ extern "C" int orx_bag_gather(orx_handle_t h, const float* const* tabs_host, con
     bt.tab[k] = tabs_host[k];
     bt.rows[k] = rows_host[k];
     bt.col_off[k] = col_off_host[k];
-    aligned = aligned && orx_aligned16(tabs_host[k]);
+    aligned = aligned && (std::is_same<S, float>::value ? orx_aligned16(tabs_host[k]) : orx_aligned8(tabs_host[k]));
   }
   bt.col_off[T] = col_off_host[T];
   if (B == 0) return ORX_OK;
@@ -720,9 +760,22 @@ extern "C" int orx_bag_gather(orx_handle_t h, const float* const* tabs_host, con
   if (blocks > (int64_t)h->num_sms * 32) blocks = (int64_t)h->num_sms * 32;
   cudaStream_t st = (cudaStream_t)s;
   if ((dim & 3) == 0 && (out_ld & 3) == 0 && aligned)
-    k_bag_gather<true><<<(int)blocks, 256, 0, st>>>(bt, T, dim, sparse, ld, B, mode, out, out_ld, n_bad);
+    k_bag_gather<true, S><<<(int)blocks, 256, 0, st>>>(bt, T, dim, sparse, ld, B, mode, out, out_ld, n_bad);
   else
-    k_bag_gather<false><<<(int)blocks, 256, 0, st>>>(bt, T, dim, sparse, ld, B, mode, out, out_ld, n_bad);
+    k_bag_gather<false, S><<<(int)blocks, 256, 0, st>>>(bt, T, dim, sparse, ld, B, mode, out, out_ld, n_bad);
   ORX_LAUNCH_CHECK();
   return ORX_OK;
+}
+
+extern "C" int orx_bag_gather(orx_handle_t h, const float* const* tabs_host, const int64_t* rows_host, int32_t T,
+                              int32_t dim, const int32_t* sparse, int64_t ld, const int32_t* col_off_host, int32_t B,
+                              int32_t mode, float* out, int64_t out_ld, int32_t* n_bad, orx_stream_t s) {
+  return bag_gather_impl(h, tabs_host, rows_host, T, dim, sparse, ld, col_off_host, B, mode, out, out_ld, n_bad, s);
+}
+
+extern "C" int orx_bag_gather_bf16(orx_handle_t h, const uint16_t* const* tabs_host, const int64_t* rows_host,
+                                   int32_t T, int32_t dim, const int32_t* sparse, int64_t ld,
+                                   const int32_t* col_off_host, int32_t B, int32_t mode, float* out, int64_t out_ld,
+                                   int32_t* n_bad, orx_stream_t s) {
+  return bag_gather_impl(h, tabs_host, rows_host, T, dim, sparse, ld, col_off_host, B, mode, out, out_ld, n_bad, s);
 }

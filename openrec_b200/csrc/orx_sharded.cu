@@ -94,9 +94,12 @@ extern "C" int orx_owner_bucket_combined(orx_handle_t h, const int32_t* ids, int
 // One warp's ROWWISE_ADAGRAD update of table row id from value row v (each element divided by nb): a row seen once in
 // the batch (own, warp-uniform) takes the sum of its squared gradient first -- lane-strided in order, then the xor tree
 // -- before its first store (a warp holds a row as lane * 4 ... e += 128, so D > 128 takes two passes over v); any other
-// row is added into its staging row d.  vec: var and the value rows move as float4 (s0[id] is one scalar).
-__device__ __forceinline__ void orx_apply_row_rowwise(bool vec, bool own, float* var, float* s0, int id, float* gstage,
-                                                      int d, int D, const float* v, float nb, const OrxOptDev& o) {
+// row is added into its staging row d.  vec: var moves 4 elements per lane (float4, or 8 bytes of bf16) and the value
+// rows as float4 (s0[id] is one scalar).  T: the table's storage; an owned bf16 row is rounded with orx_sr_row(kt, id).
+template <typename T>
+__device__ __forceinline__ void orx_apply_row_rowwise(bool vec, bool own, T* var, float* s0, int id, float* gstage,
+                                                      int d, int D, const float* v, float nb, const OrxOptDev& o,
+                                                      uint32_t kt) {
   const int lane = threadIdx.x & 31;
   auto val4 = [&](int e) {
     const float4 g = __ldcg(reinterpret_cast<const float4*>(v + e));
@@ -120,24 +123,27 @@ __device__ __forceinline__ void orx_apply_row_rowwise(bool vec, bool own, float*
   ss = orx_group_sum<32>(ss);
   float acc = s0[id];
   const float f = orx_row_scale(acc, ss, D, o);
-  float* w = var + (int64_t)id * D;
+  T* w = var + (int64_t)id * D;
   if (vec) {
     for (int e = lane * 4; e < D; e += 128)
-      __stcg(reinterpret_cast<float4*>(w + e), orx_row_apply4(__ldcg(reinterpret_cast<const float4*>(w + e)), val4(e), f, o));
+      orx_own_or_stage4_row<false>(true, var, id, gstage, d, D, e, orx_ld4_cg(w + e), val4(e), f, o, kt);
   } else {
-    for (int e = lane; e < D; e += 32) w[e] = orx_row_apply1(w[e], val1(e), f, o);
+    const uint32_t rk = orx_sr_row(kt, id);
+    for (int e = lane; e < D; e += 32) orx_st1(w + e, orx_row_apply1(orx_ld1(w + e), val1(e), f, o), rk, e);
   }
   if (lane == 0) s0[id] = acc;
 }
 
-// VEC: var, s0 and s1 are 16-byte aligned (sparse_apply_impl decides); the row shape and the value rows are tested here,
+// VEC: var, s0 and s1 are 16-byte aligned (sparse_apply_vec decides); the row shape and the value rows are tested here,
 // so that the VEC instance compiles to what the kernel was before the table gate.  Under ROWWISE_ADAGRAD only var is
 // (s0 is float[rows], read as scalars).
-template <int OPT, bool VEC>
-__global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, float* s1, int64_t rows, int D,
+// T: the table's storage, float or bf16 bits (uint16_t: VEC means var 8-byte aligned; an owned row is read as its exact
+// fp32 upcast and stored rounded with the row key orx_sr_row(kt, id)); slots and staging rows are float either way.
+template <int OPT, bool VEC, typename T = float>
+__global__ void __launch_bounds__(256) k_sparse_apply(T* var, float* s0, float* s1, int64_t rows, int D,
                                                       const int32_t* __restrict__ ids, int64_t id_stride,
                                                       const float* __restrict__ vals, int64_t val_ld, int n,
-                                                      OrxHash hsh, float* gstage, OrxOptDev o) {
+                                                      OrxHash hsh, float* gstage, OrxOptDev o, uint32_t kt) {
   typedef OrxOptSlots<OPT> SL;
   const int lane = threadIdx.x & 31;
   const int nw = (gridDim.x * blockDim.x) >> 5;
@@ -151,7 +157,8 @@ __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, flo
     if (my_id < 0 || (int64_t)my_id >= rows) my_id = -1;
     else my_c = orx_hash_find(hsh, my_id, &my_d);
   }
-#pragma unroll 2
+// bf16 under ROWWISE_ADAGRAD: not unrolled (unrolled, 16 bytes spill around the division's slow-path call)
+#pragma unroll (SL::ROW && !std::is_same<T, float>::value ? 1 : 2)
   for (int k = 0; k < 8; ++k) {
   const int b = b0 + k;
   if (b >= n) break;
@@ -163,7 +170,7 @@ __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, flo
   const bool own = !SL::STAGE_ONLY && c == 1u;
   if constexpr (SL::ROW) {
     orx_apply_row_rowwise(VEC && ((D & 3) == 0) && ((val_ld & 3) == 0) && (((uintptr_t)vals & 15) == 0), own, var, s0,
-                          id, gstage, d, D, v, 1.f, o);
+                          id, gstage, d, D, v, 1.f, o, kt);
     continue;
   } else
   // 128-bit path (value rows 16-byte aligned: a strided view may start mid-row): all loads of the row first, then the
@@ -173,15 +180,16 @@ __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, flo
     for (int e = lane * 4; e < D; e += 128) {
       const int64_t off = (int64_t)id * D + e;
       const float4 g = __ldcg(reinterpret_cast<const float4*>(v + e));
-      const float4 wv = own ? __ldcg(reinterpret_cast<const float4*>(var + off)) : z4;
+      const float4 wv = own ? orx_ld4_cg(var + off) : z4;
       float4 a = (SL::S0 && own) ? __ldcg(reinterpret_cast<const float4*>(s0 + off)) : z4;
       float4 bb = (SL::S1 && own) ? __ldcg(reinterpret_cast<const float4*>(s1 + off)) : z4;
-      orx_own_or_stage4<OPT, false>(own, var, s0, s1, id, gstage, d, D, e, wv, g, a, bb, o);
+      orx_own_or_stage4<OPT, false>(own, var, s0, s1, id, gstage, d, D, e, wv, g, a, bb, o, kt);
     }
   } else {
+    const uint32_t rk = orx_sr_row(kt, id);
     for (int e = lane; e < D; e += 32) {
       const int64_t off = (int64_t)id * D + e;
-      if (own) orx_update1<OPT>(var + off, s0 + off, s1 + off, var[off], v[e], o);
+      if (own) orx_update1<OPT, T>(var + off, s0 + off, s1 + off, orx_ld1(var + off), v[e], o, rk, e);
       else atomicAdd(gstage + (int64_t)d * D + e, v[e]);
     }
   }
@@ -190,7 +198,8 @@ __global__ void __launch_bounds__(256) k_sparse_apply(float* var, float* s0, flo
 }
 
 static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
-                             const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt, orx_stream_t s);
+                             const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt, orx_stream_t s,
+                             const uint32_t* srk = nullptr);
 
 extern "C" int orx_sparse_apply(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, const float* values,
                                 int32_t n, const orx_opt_t* opt, orx_stream_t s) {
@@ -205,6 +214,16 @@ extern "C" int orx_sparse_apply_strided(orx_handle_t h, const orx_table_t* tab, 
   return sparse_apply_impl(h, tab, ids, id_stride, values, value_ld, n, opt, s);
 }
 
+extern "C" int orx_sparse_apply_strided_bf16(orx_handle_t h, const orx_table_bf16_t* tab, const int32_t* ids,
+                                             int64_t id_stride, const float* values, int64_t value_ld, int32_t n,
+                                             const orx_opt_t* opt, uint64_t sr_seed, orx_stream_t s) {
+  ORX_REQUIRE(tab != nullptr && id_stride >= 1 && value_ld >= tab->dim, "bad strides");
+  ORX_REQUIRE(opt != nullptr, "null pointer");
+  orx_table_t t;
+  const uint32_t srk = orx_sr_table_key(sr_seed, opt->step, 0);
+  return sparse_apply_impl(h, orx_bf16_table(tab, &t), ids, id_stride, values, value_ld, n, opt, s, &srk);
+}
+
 // The checks every un-fused sparse apply makes before any device work.
 static int sparse_apply_check(orx_handle_t h, const orx_table_t* tab, int64_t n, const orx_opt_t* opt) {
   ORX_REQUIRE(h != nullptr && tab && tab->var && opt, "null pointer");
@@ -214,12 +233,20 @@ static int sparse_apply_check(orx_handle_t h, const orx_table_t* tab, int64_t n,
   return ORX_OK;
 }
 
+// The 4-element row path of an apply's table: a table may start anywhere (orx.h); its rows need a 16-byte (float) or
+// 8-byte (bf16) boundary, its slot rows 16 bytes; a row-wise accumulator is read as scalars and does not count.
+static bool sparse_apply_vec(const orx_table_t* tab, int opt_kind, bool bf16) {
+  const bool rows_ok = bf16 ? orx_aligned8(tab->var) : orx_aligned16(tab->var);
+  return opt_kind == ORX_OPT_ROWWISE_ADAGRAD ? rows_ok : rows_ok && orx_aligned16(tab->s0, tab->s1);
+}
+
 // The rest of an un-fused sparse apply of n lookups whose ids are ids[i * id_stride]: the batch index (mode 1 under
 // ADAM_DENSE), apply(o) -- the launch that updates the rows seen once and stages the others --, the ADAM_DENSE sweeps
-// and the staged-row tail.  The caller has checked the arguments and made the workspace hold n lookups.
+// and the staged-row tail.  The caller has checked the arguments and made the workspace hold n lookups.  srk: a bf16
+// table (var passed as the float* of the orx_table_t) whose updates round with the table key *srk; null: a float table.
 template <typename Apply>
 static int sparse_apply_run(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride, int32_t n,
-                            const orx_opt_t* opt, cudaStream_t st, Apply&& apply) {
+                            const orx_opt_t* opt, cudaStream_t st, const uint32_t* srk, Apply&& apply) {
   const bool dense = opt->kind == ORX_OPT_ADAM_DENSE;
   const OrxOptDev o = orx_opt_to_dev(opt);
   int rc;
@@ -229,15 +256,17 @@ static int sparse_apply_run(orx_handle_t h, const orx_table_t* tab, const int32_
     apply(o);
     ORX_LAUNCH_CHECK();
   }
-  if (dense && (rc = orx_launch_adam_sweeps(h, tab, nullptr, nullptr, h->set[0], o, st))) return rc;
+  if (dense && (rc = orx_launch_adam_sweeps(h, tab, nullptr, nullptr, h->set[0], o, st, srk))) return rc;
   // staged rows: the shared tail with no item side and no loss
   TailArgs ta = {orx_sparse_args(h, tab, nullptr, nullptr, h->set[0], o)};
   ta.counters = h->set[0].ctl;
-  return orx_launch_tail(h, ta, opt->kind, st);
+  if (srk) ta.srk[0] = *srk;
+  return orx_launch_tail(h, ta, opt->kind, st, srk != nullptr);
 }
 
 static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32_t* ids, int64_t id_stride,
-                             const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt, orx_stream_t s) {
+                             const float* values, int64_t value_ld, int32_t n, const orx_opt_t* opt, orx_stream_t s,
+                             const uint32_t* srk) {
   int rc = sparse_apply_check(h, tab, n, opt);
   if (rc) return rc;
   ORX_CUDA(cudaSetDevice(h->device));
@@ -248,14 +277,20 @@ static int sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32
   if ((rc = orx_ensure_workspace(h, n > 0 ? n : 1, D))) return rc;
   const orx_opt_t od = orx_opt_dim(opt, D);
   opt = &od;
-  // a table may start anywhere (orx.h); a row-wise accumulator is read as scalars and does not count
-  const bool vec = od.kind == ORX_OPT_ROWWISE_ADAGRAD ? orx_aligned16(tab->var) : orx_aligned16(tab->var, tab->s0, tab->s1);
-  return sparse_apply_run(h, tab, ids, id_stride, n, opt, st, [&](const OrxOptDev& o) {
+  const bool vec = sparse_apply_vec(tab, od.kind, srk != nullptr);
+  return sparse_apply_run(h, tab, ids, id_stride, n, opt, st, srk, [&](const OrxOptDev& o) {
     const int blocks = (n + 63) / 64;   // 8 warps x 8 pairs per block and iteration
     orx_dispatch_opt(opt->kind, [&](auto O) {
       orx_dispatch<0, 1>(vec ? 1 : 0, [&](auto V) {
-        k_sparse_apply<decltype(O)::value, decltype(V)::value == 1><<<blocks, 256, 0, st>>>(
-            tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride, values, value_ld, n, h->set[0].u, h->gu, o);
+        constexpr int OPT = decltype(O)::value;
+        constexpr bool VEC = decltype(V)::value == 1;
+        if (srk)
+          k_sparse_apply<OPT, VEC, uint16_t><<<blocks, 256, 0, st>>>(
+              reinterpret_cast<uint16_t*>(tab->var), tab->s0, tab->s1, tab->rows, D, ids, id_stride, values, value_ld,
+              n, h->set[0].u, h->gu, o, *srk);
+        else
+          k_sparse_apply<OPT, VEC><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, tab->rows, D, ids, id_stride,
+                                                          values, value_ld, n, h->set[0].u, h->gu, o, 0u);
       });
     });
   });
@@ -288,14 +323,14 @@ __global__ void __launch_bounds__(256) k_bag_ids(const int32_t* __restrict__ spa
 
 // k_sparse_apply's update over compacted bag lookups: value row i / L, divided by cnt[i / L] for a mean (cnt != null).
 // A separate kernel so that k_sparse_apply's parameter block, and with it its register allocation, stays as it is.
-// VEC: var, s0 and s1 are 16-byte aligned (orx_bag_sparse_apply decides); the row shape and the value rows are tested
-// here, as in k_sparse_apply.
-template <int OPT, bool VEC>
-__global__ void __launch_bounds__(256) k_bag_apply(float* var, float* s0, float* s1, int D,
+// VEC: var, s0 and s1 are 16-byte aligned (sparse_apply_vec decides); the row shape and the value rows are tested
+// here, as in k_sparse_apply.  T and kt as in k_sparse_apply.
+template <int OPT, bool VEC, typename T = float>
+__global__ void __launch_bounds__(256) k_bag_apply(T* var, float* s0, float* s1, int D,
                                                    const int32_t* __restrict__ ids, int L,
                                                    const float* __restrict__ vals, int64_t val_ld,
                                                    const float* __restrict__ cnt, int n, OrxHash hsh, float* gstage,
-                                                   OrxOptDev o) {
+                                                   OrxOptDev o, uint32_t kt) {
   typedef OrxOptSlots<OPT> SL;
   const int lane = threadIdx.x & 31;
   const int nw = (gridDim.x * blockDim.x) >> 5;
@@ -324,7 +359,7 @@ __global__ void __launch_bounds__(256) k_bag_apply(float* var, float* s0, float*
   const float* v = vals + (int64_t)(b / L) * val_ld;
   const bool own = !SL::STAGE_ONLY && c == 1u;
   if constexpr (SL::ROW) {
-    orx_apply_row_rowwise(vec, own, var, s0, id, gstage, d, D, v, cnt ? nb : 1.f, o);
+    orx_apply_row_rowwise(vec, own, var, s0, id, gstage, d, D, v, cnt ? nb : 1.f, o, kt);
     continue;
   } else
   if (vec) {
@@ -333,16 +368,17 @@ __global__ void __launch_bounds__(256) k_bag_apply(float* var, float* s0, float*
       const int64_t off = (int64_t)id * D + e;
       float4 g = __ldcg(reinterpret_cast<const float4*>(v + e));
       if (cnt) g = make_float4(g.x / nb, g.y / nb, g.z / nb, g.w / nb);
-      const float4 wv = own ? __ldcg(reinterpret_cast<const float4*>(var + off)) : z4;
+      const float4 wv = own ? orx_ld4_cg(var + off) : z4;
       float4 a = (SL::S0 && own) ? __ldcg(reinterpret_cast<const float4*>(s0 + off)) : z4;
       float4 bb = (SL::S1 && own) ? __ldcg(reinterpret_cast<const float4*>(s1 + off)) : z4;
-      orx_own_or_stage4<OPT, false>(own, var, s0, s1, id, gstage, d, D, e, wv, g, a, bb, o);
+      orx_own_or_stage4<OPT, false>(own, var, s0, s1, id, gstage, d, D, e, wv, g, a, bb, o, kt);
     }
   } else {
+    const uint32_t rk = orx_sr_row(kt, id);
     for (int e = lane; e < D; e += 32) {
       const int64_t off = (int64_t)id * D + e;
       const float g = cnt ? v[e] / nb : v[e];
-      if (own) orx_update1<OPT>(var + off, s0 + off, s1 + off, var[off], g, o);
+      if (own) orx_update1<OPT, T>(var + off, s0 + off, s1 + off, orx_ld1(var + off), g, o, rk, e);
       else atomicAdd(gstage + (int64_t)d * D + e, g);
     }
   }
@@ -350,9 +386,10 @@ __global__ void __launch_bounds__(256) k_bag_apply(float* var, float* s0, float*
   }
 }
 
-extern "C" int orx_bag_sparse_apply(orx_handle_t h, const orx_table_t* tab, const int32_t* sparse, int64_t ld,
-                                    int32_t col_lo, int32_t L, int32_t B, const float* dZ, int64_t dz_ld, int32_t mode,
-                                    const orx_opt_t* opt, orx_stream_t s) {
+// srk as in sparse_apply_run
+static int bag_sparse_apply_impl(orx_handle_t h, const orx_table_t* tab, const int32_t* sparse, int64_t ld,
+                                 int32_t col_lo, int32_t L, int32_t B, const float* dZ, int64_t dz_ld, int32_t mode,
+                                 const orx_opt_t* opt, orx_stream_t s, const uint32_t* srk) {
   const int64_t n64 = (int64_t)B * L;
   int rc = sparse_apply_check(h, tab, B, opt);
   if (rc) return rc;
@@ -382,15 +419,37 @@ extern "C" int orx_bag_sparse_apply(orx_handle_t h, const orx_table_t* tab, cons
   }
   const orx_opt_t od = orx_opt_dim(opt, D);
   opt = &od;
-  // a table may start anywhere (orx.h); a row-wise accumulator is read as scalars and does not count
-  const bool vec = od.kind == ORX_OPT_ROWWISE_ADAGRAD ? orx_aligned16(tab->var) : orx_aligned16(tab->var, tab->s0, tab->s1);
-  return sparse_apply_run(h, tab, ids_c, 1, n, opt, st, [&](const OrxOptDev& o) {
+  const bool vec = sparse_apply_vec(tab, od.kind, srk != nullptr);
+  return sparse_apply_run(h, tab, ids_c, 1, n, opt, st, srk, [&](const OrxOptDev& o) {
     const int blocks = (n + 63) / 64;
     orx_dispatch_opt(opt->kind, [&](auto O) {
       orx_dispatch<0, 1>(vec ? 1 : 0, [&](auto V) {
-        k_bag_apply<decltype(O)::value, decltype(V)::value == 1><<<blocks, 256, 0, st>>>(
-            tab->var, tab->s0, tab->s1, D, ids_c, L, dZ, dz_ld, cnt, n, h->set[0].u, h->gu, o);
+        constexpr int OPT = decltype(O)::value;
+        constexpr bool VEC = decltype(V)::value == 1;
+        if (srk)
+          k_bag_apply<OPT, VEC, uint16_t><<<blocks, 256, 0, st>>>(reinterpret_cast<uint16_t*>(tab->var), tab->s0,
+                                                                  tab->s1, D, ids_c, L, dZ, dz_ld, cnt, n,
+                                                                  h->set[0].u, h->gu, o, *srk);
+        else
+          k_bag_apply<OPT, VEC><<<blocks, 256, 0, st>>>(tab->var, tab->s0, tab->s1, D, ids_c, L, dZ, dz_ld, cnt, n,
+                                                       h->set[0].u, h->gu, o, 0u);
       });
     });
   });
+}
+
+extern "C" int orx_bag_sparse_apply(orx_handle_t h, const orx_table_t* tab, const int32_t* sparse, int64_t ld,
+                                    int32_t col_lo, int32_t L, int32_t B, const float* dZ, int64_t dz_ld, int32_t mode,
+                                    const orx_opt_t* opt, orx_stream_t s) {
+  return bag_sparse_apply_impl(h, tab, sparse, ld, col_lo, L, B, dZ, dz_ld, mode, opt, s, nullptr);
+}
+
+extern "C" int orx_bag_sparse_apply_bf16(orx_handle_t h, const orx_table_bf16_t* tab, const int32_t* sparse,
+                                         int64_t ld, int32_t col_lo, int32_t L, int32_t B, const float* dZ,
+                                         int64_t dz_ld, int32_t mode, const orx_opt_t* opt, uint64_t sr_seed,
+                                         orx_stream_t s) {
+  ORX_REQUIRE(opt != nullptr, "null pointer");
+  orx_table_t t;
+  const uint32_t srk = orx_sr_table_key(sr_seed, opt->step, 0);
+  return bag_sparse_apply_impl(h, orx_bf16_table(tab, &t), sparse, ld, col_lo, L, B, dZ, dz_ld, mode, opt, s, &srk);
 }

@@ -105,6 +105,13 @@ def _score_tables(op, user_tab, item_tab):
                      f"{item_tab.dtype}")
 
 
+def _sr_seed(sr_seed, op):
+    """The uint64 rounding seed of a bf16 table's apply; a bf16 table has no default seed."""
+    if sr_seed is None:
+        raise ValueError(f"{op}: a bfloat16 table's updates need sr_seed")
+    return int(sr_seed) & 0xFFFFFFFFFFFFFFFF
+
+
 def table_bf16(var, s0=None, s1=None, kind=None):
     """orx_table_bf16_t for a bfloat16 [rows, dim] variable and its float32 optimizer slots (checked as in table)."""
     _bf16(var, "var"), _f32(s0, "s0"), _f32(s1, "s1")
@@ -312,14 +319,20 @@ class Engine:
         _lib.check(self.lib.orx_sparse_apply(self.h, C.byref(tab), _ptr(ids), _ptr(values), n, C.byref(o),
                                              self.stream()), "orx_sparse_apply")
 
-    def sparse_apply_strided(self, tab, ids2d, col, values3d, o):
-        """ids = ids2d[:, col] (int32 [n, F]); value rows = values3d[:, col, :] ([n, F, D]) -- no copies."""
+    def sparse_apply_strided(self, tab, ids2d, col, values3d, o, sr_seed=None):
+        """ids = ids2d[:, col] (int32 [n, F]); value rows = values3d[:, col, :] ([n, F, D]) -- no copies.  A bf16 table
+        (table_bf16) takes orx_sparse_apply_strided_bf16, its updates rounded with sr_seed (required)."""
         n, F = ids2d.shape
         D = values3d.shape[2]
-        _lib.check(self.lib.orx_sparse_apply_strided(
-            self.h, C.byref(tab), C.c_void_p(ids2d.data_ptr() + 4 * col), F,
-            C.c_void_p(values3d.data_ptr() + 4 * col * D), values3d.shape[1] * D, n, C.byref(o), self.stream()),
-            "orx_sparse_apply_strided")
+        args = (C.c_void_p(ids2d.data_ptr() + 4 * col), F, C.c_void_p(values3d.data_ptr() + 4 * col * D),
+                values3d.shape[1] * D, n, C.byref(o))
+        if isinstance(tab, OrxTableBf16):
+            op = "orx_sparse_apply_strided_bf16"
+            _lib.check(self.lib.orx_sparse_apply_strided_bf16(self.h, C.byref(tab), *args, _sr_seed(sr_seed, op),
+                                                              self.stream()), op)
+        else:
+            _lib.check(self.lib.orx_sparse_apply_strided(self.h, C.byref(tab), *args, self.stream()),
+                       "orx_sparse_apply_strided")
 
     # ---- DLRM pieces (2-D operands may be column-slices: the leading dimension is taken from stride(0)) ----
     @staticmethod
@@ -328,17 +341,30 @@ class Engine:
             raise ValueError("expected a 2-D float32 view with unit inner stride")
         return t.stride(0)
 
-    def gather_strided(self, tab, ids2d, col, out2d):
+    def gather_strided(self, tab, ids2d, col, out2d, n_bad=None):
+        """out2d[b] = tab[ids2d[b, col]] (float32 rows; a bfloat16 tab takes orx_gather_strided_bf16, widened exactly)."""
         n, F = ids2d.shape
-        _lib.check(self.lib.orx_gather_strided(self.h, _ptr(tab), tab.shape[0], tab.shape[1],
-                                               C.c_void_p(ids2d.data_ptr() + 4 * col), F, n, _ptr(out2d),
-                                               self._ld(out2d), None, self.stream()), "orx_gather_strided")
+        op = "orx_gather_strided_bf16" if tab.dtype == torch.bfloat16 else "orx_gather_strided"
+        if tab.dtype == torch.bfloat16:
+            _bf16(tab, "tab")
+        _lib.check(getattr(self.lib, op)(self.h, _ptr(tab), tab.shape[0], tab.shape[1],
+                                         C.c_void_p(ids2d.data_ptr() + 4 * col), F, n, _ptr(out2d), self._ld(out2d),
+                                         _ptr(n_bad), self.stream()), op)
 
     def bag_gather(self, tabs, sparse, col_off, mode, out2d, n_bad=None):
         """Multi-hot lookup of every table in one launch (orx_bag_gather in include/orx.h): sparse int32 [B, C] on the
         device, col_off [T + 1] host ints (table k's bag = columns col_off[k] .. col_off[k+1]), mode 0 sum / 1 mean;
-        out2d [B, >= T*D] (any row stride) gets Z[b, k, :] at columns k*D .. (k+1)*D."""
+        out2d [B, >= T*D] (any row stride) gets Z[b, k, :] at columns k*D .. (k+1)*D.  bfloat16 tables take
+        orx_bag_gather_bf16 (every table bfloat16; a mix of float32 and bfloat16 tables is refused)."""
         T = len(tabs)
+        dtypes = {t.dtype for t in tabs}
+        bf16 = torch.bfloat16 in dtypes
+        if bf16 and dtypes != {torch.bfloat16}:
+            raise ValueError(f"bag_gather: the tables must all be float32 or all bfloat16, got {sorted(map(str, dtypes))}")
+        if bf16:
+            for k, t in enumerate(tabs):
+                _bf16(t, f"tabs[{k}]")
+        op = "orx_bag_gather_bf16" if bf16 else "orx_bag_gather"
         if sparse.dtype != torch.int32 or sparse.dim() != 2 or sparse.stride(1) != 1:
             raise ValueError("sparse: expected an int32 [B, C] tensor with unit inner stride")
         if len(col_off) != T + 1:
@@ -347,23 +373,28 @@ class Engine:
         ptrs = (C.c_void_p * T)(*[t.data_ptr() for t in tabs])
         rows = (C.c_int64 * T)(*[t.shape[0] for t in tabs])
         off = (C.c_int32 * (T + 1))(*[int(x) for x in col_off])
-        _lib.check(self.lib.orx_bag_gather(self.h, ptrs, rows, T, tabs[0].shape[1] if T else 0,
-                                           _ptr(sparse) if B else None, max(sparse.stride(0), 1), off, B, int(mode),
-                                           _ptr(out2d) if B else None, self._ld(out2d), _ptr(n_bad), self.stream()),
-                   "orx_bag_gather")
+        _lib.check(getattr(self.lib, op)(self.h, ptrs, rows, T, tabs[0].shape[1] if T else 0,
+                                         _ptr(sparse) if B else None, max(sparse.stride(0), 1), off, B, int(mode),
+                                         _ptr(out2d) if B else None, self._ld(out2d), _ptr(n_bad), self.stream()), op)
 
-    def bag_sparse_apply(self, tab, sparse, col_lo, L, dz2d, mode, o):
+    def bag_sparse_apply(self, tab, sparse, col_lo, L, dz2d, mode, o, sr_seed=None):
         """optimizer.apply_gradients of one table's bag lookups (orx_bag_sparse_apply): bag b = sparse[b, col_lo :
-        col_lo + L], its pooled gradient row dz2d[b] ([B, D], any row stride), mode 0 sum / 1 mean."""
+        col_lo + L], its pooled gradient row dz2d[b] ([B, D], any row stride), mode 0 sum / 1 mean.  A bf16 table
+        (table_bf16) takes orx_bag_sparse_apply_bf16, its updates rounded with sr_seed (required)."""
         B = sparse.shape[0]
         if sparse.dtype != torch.int32 or sparse.dim() != 2 or sparse.stride(1) != 1:
             raise ValueError("sparse: expected an int32 [B, C] tensor with unit inner stride")
         if dz2d.shape[0] != B:
             raise ValueError("one gradient row per bag")
-        _lib.check(self.lib.orx_bag_sparse_apply(self.h, C.byref(tab), _ptr(sparse) if B else None,
-                                                 max(sparse.stride(0), 1), int(col_lo), int(L), B,
-                                                 _ptr(dz2d) if B else None, self._ld(dz2d), int(mode), C.byref(o),
-                                                 self.stream()), "orx_bag_sparse_apply")
+        args = (_ptr(sparse) if B else None, max(sparse.stride(0), 1), int(col_lo), int(L), B,
+                _ptr(dz2d) if B else None, self._ld(dz2d), int(mode), C.byref(o))
+        if isinstance(tab, OrxTableBf16):
+            op = "orx_bag_sparse_apply_bf16"
+            _lib.check(self.lib.orx_bag_sparse_apply_bf16(self.h, C.byref(tab), *args, _sr_seed(sr_seed, op),
+                                                          self.stream()), op)
+        else:
+            _lib.check(self.lib.orx_bag_sparse_apply(self.h, C.byref(tab), *args, self.stream()),
+                       "orx_bag_sparse_apply")
 
     def mlp_fwd(self, x, w, bias, act, y):
         _lib.check(self.lib.orx_mlp_layer_fwd(self.h, _ptr(x), self._ld(x), x.shape[0], w.shape[0], _ptr(w), _ptr(bias),

@@ -12,6 +12,24 @@ from ...tfshim.core import LazyScalar, StepNode, Tensor, convert
 from ...tfshim.keras import Model
 from ..mlp_ops import ACT, DLRMGraph
 from ..modules import MLP, CrossNetwork, LatentFactor, SecondOrderFeatureInteraction
+from ._base import _check_dtype
+
+_M64 = (1 << 64) - 1
+
+
+def _mix64(z):
+    """splitmix64's finalizer (include/orx.h), a bijection of the uint64s."""
+    z = ((z ^ (z >> 30)) * 0xbf58476d1ce4e5b9) & _M64
+    z = ((z ^ (z >> 27)) * 0x94d049bb133111eb) & _M64
+    return z ^ (z >> 31)
+
+
+def table_rounding_seed(rounding_seed, k):
+    """The stochastic-rounding seed of DLRM's bf16 table k: mix64(rounding_seed + k) (mod 2^64).  Each table's apply
+    rounds as table 0 of the orx.h rule under its own seed; mix64 is a bijection, so every table of a model gets a
+    distinct seed, whatever the number of tables (keying tables by t in mix64(2 * step + t) would give table 2 at step s
+    the bits of table 0 at step s + 1)."""
+    return _mix64((int(rounding_seed) + int(k)) & _M64)
 
 
 def bag_layout(bag_sizes, pooling, n_tables):
@@ -62,7 +80,7 @@ class DLRM(Model):
     def __init__(self, m_spa, ln_emb, ln_bot, ln_top, arch_interaction_op="dot", arch_interaction_itself=False,
                  sigmoid_bot=False, sigmoid_top=True, loss_func="mse", loss_threshold=0.0,
                  interaction_mode="reference", bag_sizes=None, pooling="sum", cross_layers=3,
-                 cross_projection_dim=None):
+                 cross_projection_dim=None, embedding_dtype="float32", rounding_seed=0):
         """Reference signature (dlrm.py:8-19) + ``interaction_mode``: 'reference' reproduces the reference's
         dot interaction bit for bit (identically zero, SURVEY Q1), 'dlrm' is the strictly-lower triangle.
 
@@ -73,13 +91,19 @@ class DLRM(Model):
 
         ``arch_interaction_op="cross"`` replaces the dot interaction by a DCN-v2 CrossNetwork(cross_layers,
         cross_projection_dim) over x0 = (dense_vec | Z_0 | .. | Z_{T-1}), W = (T + 1) * m_spa wide; the top MLP reads
-        its [B, W] output.  ``arch_interaction_itself`` and ``interaction_mode`` apply to the dot interaction only."""
+        its [B, W] output.  ``arch_interaction_itself`` and ``interaction_mode`` apply to the dot interaction only.
+
+        ``embedding_dtype="bfloat16"`` stores the embedding tables in bfloat16 (optimizer slots, Dense layers, cross
+        projections, Z and every activation stay float32).  A lookup widens rows exactly; each apply rounds table k's
+        updated elements stochastically under seed ``table_rounding_seed(rounding_seed, k)`` and the optimizer's step,
+        so a run repeats bit for bit."""
+        self.embedding_dtype, self.rounding_seed = _check_dtype(embedding_dtype), int(rounding_seed)
         super().__init__()
         self._bag_sizes, self._col_off, self._pooling = bag_layout(bag_sizes, pooling, len(ln_emb))
         self._m_spa = int(m_spa)
         self._loss_threshold = loss_threshold
         self._loss_func = loss_func
-        self._latent_factors = [LatentFactor(num_instances=int(num), dim=m_spa) for num in ln_emb]
+        self._latent_factors = [LatentFactor(num_instances=int(num), dim=m_spa, dtype=embedding_dtype) for num in ln_emb]
         self._mlp_bot = MLP(units_list=ln_bot, out_activation="sigmoid" if sigmoid_bot else "relu")
         self._mlp_top = MLP(units_list=ln_top, out_activation="sigmoid" if sigmoid_top else "relu")
         self._dot_interaction = self._cross = None
@@ -172,11 +196,12 @@ class DLRM(Model):
         c, (dZ, bot_g, top_g, cross_g) = self._fwd_bwd(node, float(coefs[0].get(0, 0.0)))
         eng, o = N.engine(), optimizer.opt_struct()
         for k, lf in enumerate(self._latent_factors):                 # IndexedSlices(ids = sparse[:,k], dZ[:,k,:])
+            bf16 = {"sr_seed": table_rounding_seed(self.rounding_seed, k)} if self.embedding_dtype == "bfloat16" else {}
             if self._col_off is None:
-                eng.sparse_apply_strided(optimizer.table(lf.embeddings), sparse, k, dZ, o)
+                eng.sparse_apply_strided(optimizer.table(lf.embeddings), sparse, k, dZ, o, **bf16)
             else:                                                     # ... of every valid id of table k's bags
                 eng.bag_sparse_apply(optimizer.table(lf.embeddings), sparse, self._col_off[k], self._bag_sizes[k],
-                                     dZ[:, k, :], self._pooling, o)
+                                     dZ[:, k, :], self._pooling, o, **bf16)
         for var, g in _dense_groups(self, bot_g, top_g, cross_g):
             eng.dense_apply(var.t, *optimizer.slots(var), g, o)
         node.out = c["out4"]
